@@ -2,12 +2,14 @@
 """Benchmark of the PV-RAFT hot path (BASELINE.json metric: RAFT iters/sec at N=8192, iters=32;
 corr-kernel HBM GB/s vs peak).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--dump-outputs DIR]
 
 A "step" is one full `RSF.forward(p, num_iters=32)` (encoders + correlation build + 32 RAFT
 iterations) on a batch of synthetic N=8192 cloud pairs with seeded random-init weights.
 value = sample-iterations/s = global_batch * iters / T_forward (CUDA events, max over ranks).
 Rank 0 prints ONE JSON line.  See DESIGN.md "Measurement" for every field.
+--dump-outputs DIR writes what the last timed step returned as DIR/<name>.npy (float32); the inputs and weights are
+seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -19,13 +21,16 @@ import threading
 import time
 import types
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 N_POINTS, TRUNC_K, ITERS, LEVELS, BASE_SCALE = 8192, 512, 32, 3, 0.25
-BATCH_PER_GPU = 8        # 8 x 32 MiB of (corr, index) state = 268 MB > the 126 MB L2: the lookup streams from HBM
+BATCH_PER_GPU = 8        # 8 x 32 MiB of (corr, index) state = 268 MB > the 50 MB L2 of an H100: the lookup streams from HBM
+L2_MB = 50
+DUMP_LIMIT_BYTES = 64 << 20
 
 
 def alg_bytes_lookup(n, k, levels=LEVELS, bf16=False):
@@ -44,11 +49,11 @@ def measured_peaks():
             return json.load(open(path)), 'measured'
         except Exception:   # noqa: BLE001
             pass
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0}, 'fallback'
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'fallback'
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
          'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
 
@@ -160,8 +165,8 @@ def cpu_sample(threads, loop_iters=ITERS, n=N_POINTS):
 
 def gpu_reference_sample(dev, batch, iters):
     """The reference FORMULATION on the same GPU: the oracle's op sequence (= the reference's own ATen ops, model/*.py) run by
-    torch eager on `dev`, fp32, TF32 off -- "the reference GPU build" of BASELINE.json's >= 10x target (the unmodified
-    reference cannot travel to the GPU box).  One warm-up at 2 iterations, one timed forward; returns seconds."""
+    torch eager on `dev`, fp32, TF32 off -- "the reference GPU build" of BASELINE.json's >= 10x target (the reference
+    tree itself is not needed).  One warm-up at 2 iterations, one timed forward; returns seconds."""
     from oracle import pvraft_oracle as O
     tf32 = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -216,8 +221,8 @@ def gpu_reference_train_sample(dev, batch, iters):
 
 
 def run_reference(a):
-    """`--impl reference`: the reference's CPU formulation (oracle port; the reference itself is pure PyTorch and is not present on
-    the GPU box) timed on the host cores, same metric / unit / config.  A step is ONE full forward at B=1: the pre-loop work
+    """`--impl reference`: the reference's CPU formulation (oracle port of the reference, which is pure PyTorch and is not needed
+    at run time) timed on the host cores, same metric / unit / config.  A step is ONE full forward at B=1: the pre-loop work
     and all 32 iterations are executed and timed (no extrapolation); steps stop early once ~200 s have been spent."""
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
@@ -255,7 +260,7 @@ def run_reference(a):
 
 def workload_config(batch_per_gpu, world, iters, graph=False, refine=False, dtype='f32'):
     state_mb = batch_per_gpu * N_POINTS * TRUNC_K * (4 if dtype == 'bf16' else 8) / 1e6
-    l2 = (f'per-iteration candidate state ({state_mb:.0f} MB/GPU) exceeds the 126 MB L2; no explicit flush' if state_mb > 126
+    l2 = (f'per-iteration candidate state ({state_mb:.0f} MB/GPU) exceeds the {L2_MB} MB L2; no explicit flush' if state_mb > L2_MB
           else f'per-iteration candidate state is {state_mb:.0f} MB/GPU: L2-resident after the first iteration (labelled as such)')
     mode = ('bf16 correlation state + uint16 ids, fp32 coordinates / index math / layers (BASELINE.json configs[2])' if dtype == 'bf16'
             else 'fp32 (BASELINE.json metric config; batch from configs[2])')
@@ -266,19 +271,19 @@ def workload_config(batch_per_gpu, world, iters, graph=False, refine=False, dtyp
             'parallelism': f'batch-shard x{world} (no data-path collective)', 'l2_policy': l2}
 
 
-def lookup_traffic():
-    """dram__bytes_read+write per launch of the lookup kernel from the committed ncu capture -- only while that capture
-    belongs to the kernel source that is being timed (profiles/lookup_dram_bytes.json records the source's sha256)."""
-    import hashlib
-    path = os.path.join(ROOT, 'profiles', 'lookup_dram_bytes.json')
-    src = os.path.join(ROOT, 'pvraft_b200', 'csrc', 'corr_lookup.cu')
-    try:
-        rec = json.load(open(path))
-        if rec.get('source_sha256') == hashlib.sha256(open(src, 'rb').read()).hexdigest():
-            return rec.get('dram_bytes_per_launch')
-    except Exception:   # noqa: BLE001
-        pass
-    return None
+def dump_outputs(directory, arrays):
+    """Write {name: tensor} as directory/<name>.npy in float32.  Above DUMP_LIMIT_BYTES in all, every array keeps the same
+    fixed, seeded sample of points (axis -2, the point axis of every output here)."""
+    os.makedirs(directory, exist_ok=True)
+    total = sum(t.numel() * 4 for t in arrays.values())
+    for name, t in arrays.items():
+        t = t.detach().float().cpu()
+        if total > DUMP_LIMIT_BYTES and t.dim() >= 2:
+            n = t.shape[-2]
+            keep = max(1, int(n * DUMP_LIMIT_BYTES / total))
+            idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            t = t.index_select(t.dim() - 2, idx)
+        np.save(os.path.join(directory, f'{name}.npy'), t.numpy().astype(np.float32))
 
 
 # --------------------------------------------------------------------------------------------------
@@ -304,10 +309,12 @@ def run_native(a):
     pc1_h, pc2_h = pc1_h.pin_memory(), pc2_h.pin_memory()
     pc1, pc2 = pc1_h.to(dev), pc2_h.to(dev)
     out_h = torch.empty(B, N_POINTS, 3).pin_memory()
+    latest = [None]
 
     def step_resident():
         with torch.no_grad():
-            return last(model([pc1, pc2], iters))
+            latest[0] = model([pc1, pc2], iters)
+            return last(latest[0])
 
     def step_e2e():
         with torch.no_grad():
@@ -338,6 +345,9 @@ def run_native(a):
     ms, launches, clocks = timed(step_resident, a.steps, sample_clocks=True)
     if clocks and set(clocks['reasons']) & {'hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown'}:
         ms, launches, clocks = timed(step_resident, a.steps, sample_clocks=True)     # re-measure once
+    if a.dump_outputs and rank == 0:   # what the caller of the timed forward received in the last timed step
+        out = latest[0]
+        dump_outputs(a.dump_outputs, {'refined_flow': out} if a.refine else {'flows': torch.stack(list(out))})
     step_e2e()
     ms_e2e, _, _ = timed(step_e2e, a.steps)
     gb = B * world
@@ -374,7 +384,7 @@ def run_native(a):
     achieved = alg / (lookup_ms * 1e-3) / 1e9
     roofline = {'kernel': 'k_corr_lookup (pvraft_corr_lookup_bf16_fwd)' if a.dtype == 'bf16' else 'k_corr_lookup (pvraft_corr_lookup_fwd)', 'bound': 'hbm', 'achieved': achieved,
                 'peak': peaks['hbm_gbs'], 'peak_kind': peak_kind + ' (MEASURED_PEAKS.json hbm_gbs)' if peak_kind == 'measured' else 'fallback',
-                'unit': 'GB/s', 'frac': achieved / peaks['hbm_gbs'], 'traffic': lookup_traffic() if a.dtype == 'f32' else None,
+                'unit': 'GB/s', 'frac': achieved / peaks['hbm_gbs'],
                 'alg_bytes_per_launch': alg, 'avg_launch_ms': lookup_ms, 'launches_timed': len(durs),
                 'share_of_step': lookup_ms * iters / (ms / a.steps)}
 
@@ -449,6 +459,7 @@ def run_train(a):
     pc1_h, pc2_h = pc1_h.pin_memory(), pc2_h.pin_memory()
     pc1, pc2 = pc1_h.to(dev), pc2_h.to(dev)
     loss_h = torch.empty(1).pin_memory()
+    last_loss = [None]
 
     def loss_fn(flows, gt, gamma=0.8):                                        # tools/loss.py:4-13 (all-ones mask)
         n = len(flows)
@@ -460,6 +471,7 @@ def run_train(a):
         loss = loss_fn(flows, x2 - x1)
         loss.backward()                                                       # DDP: the 750 KiB gradient all-reduce happens here
         opt.step()
+        last_loss[0] = loss
         return loss
 
     def step_resident():
@@ -519,6 +531,11 @@ def run_train(a):
         sampler.start()
     ms, launches = timed(step_resident, a.steps)
     clocks = sampler.stop() if sampler else None
+    if a.dump_outputs and rank == 0:   # the step's results: the loss (eager steps) and the parameters after the update
+        arrays = {'params': torch.cat([p.detach().reshape(-1) for p in model.parameters()])}
+        if last_loss[0] is not None:
+            arrays['loss'] = last_loss[0].detach().reshape(1)
+        dump_outputs(a.dump_outputs, arrays)
     ms_e2e, _ = timed(step_e2e, a.steps)
     # the collective alone: one all-reduce of a gradient-sized fp32 buffer
     nparam = sum(p.numel() for p in model.parameters())
@@ -606,6 +623,8 @@ def main():
     ap.add_argument('--refine', action='store_true', help='RSF_refine instead of RSF (configs[2])')
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
     ap.add_argument('--no-gpu-ref', action='store_true', help='skip the gpu_reference leg')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step as DIR/<name>.npy (float32, at most 64 MB in all)')
     a = ap.parse_args()
     if a.batch is None:
         a.batch = 2 if a.mode == 'train' else BATCH_PER_GPU

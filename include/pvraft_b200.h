@@ -1,5 +1,5 @@
 /*
- * pvraft_b200 -- C ABI of the B200-native (sm_100a) PV-RAFT hot path.
+ * pvraft_b200 -- C ABI of the H100-native (sm_90a) PV-RAFT hot path.
  *
  * The reference (weiyithu/PV-RAFT) has no FFI layer: its boundary is the Python nn.Module API
  * (SURVEY.md section 8b).  This header is the drop-in boundary underneath that API: every entry
@@ -56,7 +56,7 @@ PVRAFT_API const char* pvraft_last_error_string(void);
 PVRAFT_API int pvraft_device_info(int* sm_count, int* smem_optin_bytes);
 
 /* ------------------------------------------------------------------------------------------------
- * All-pairs feature correlation on the tcgen05 tensor cores with an fp32-accurate 3xTF32 split.
+ * All-pairs feature correlation on the Hopper tensor cores (wgmma) with an fp32-accurate 3xTF32 split.
  * Replaces CorrBlock.calculate_corr, model/corr.py:95-100: corr[b,i,j] = <fmap1[b,i,:], fmap2[b,j,:]> / sqrt(C).
  *   fmap1, fmap2 [B,N,C] POINT-major f32 -> corr [B,N,N] f32.   N % 128 == 0, C % 32 == 0.
  *   workspace: pvraft_corr_matmul_workspace_bytes(B,N,C) bytes (16-byte aligned) for the hi/lo operand splits.
@@ -165,7 +165,7 @@ typedef struct pvraft_linear_args {
 PVRAFT_API int pvraft_linear_fwd(const pvraft_linear_args* a, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * The same fused layer on the tcgen05 tensor cores (TMA + TMEM), fp32-accurate through a 3xTF32 operand split.
+ * The same fused layer on the Hopper tensor cores (TMA + wgmma), fp32-accurate through a 3xTF32 operand split.
  * Up to three activation sources are concatenated along K (e.g. [h | inp | motion] of the ConvGRU,
  * model/update.py:32,36); the GroupNorm(+max/min selection)+activation prologue and the bias / ReLU / residual /
  * GroupNorm-statistics epilogue match pvraft_linear_fwd; two extra epilogues implement the ConvGRU gates
@@ -282,7 +282,7 @@ typedef struct pvraft_corrfeat_args {
 PVRAFT_API int pvraft_corr_feature_fwd(const pvraft_corrfeat_args* a, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * The ALU part of the feature head, for the tcgen05 path (the 1x1 convolutions around it run as pvraft_tc_linear_fwd):
+ * The ALU part of the feature head, for the tensor-core path (the 1x1 convolutions around it run as pvraft_tc_linear_fwd):
  *   kfeat[b,n,c] = max over the 32 selected candidates of PReLU(GroupNorm(knn_conv.0(f)))      (model/corr.py:86-92)
  *   cflow[b,n,c] = relu(conv_flow(flow))                                                        (model/update.py:17)
  * knn_sel [B,N,32,4] and moments [B,PVRAFT_MOMENTS] come from pvraft_corr_lookup_fwd; the GroupNorm statistics follow

@@ -2,13 +2,13 @@
 
 A functional (no nn.Module) fp32 restatement, on torch-CPU tensors, of the reference's
 point-voxel correlation lookup + GRU update loop.  Every function cites the reference
-file:line it follows (paths relative to /root/reference).  Only `tests/`,
+file:line it follows (paths relative to the reference tree).  Only `tests/`,
 `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline / `--impl reference` leg may import
 this module; the product package `pvraft_b200` never does.
 
 Pinning: the reference ships no tests or golden vectors (SURVEY.md section 4), so this
-restatement is pinned against outputs of the reference itself, imported unmodified in the
-build container by `tests/golden/make_golden.py` (fixtures committed under `tests/golden/`)
+restatement is pinned against outputs of the reference itself, imported unmodified and run on
+CPU by `tests/golden/make_golden.py` (fixtures committed under `tests/golden/`)
 and checked by `tests/test_oracle_golden.py`.
 
 Weights are a flat dict keyed exactly like the reference `state_dict()`

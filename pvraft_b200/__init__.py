@@ -1,4 +1,4 @@
-"""pvraft_b200 -- B200-native (sm_100a) implementation of PV-RAFT's per-iteration hot path behind the
+"""pvraft_b200 -- H100-native (sm_90a) implementation of PV-RAFT's per-iteration hot path behind the
 reference's own nn.Module API.  See DESIGN.md; the C ABI is include/pvraft_b200.h."""
 from .corr import CorrBlock
 from .extractor import FlotEncoder

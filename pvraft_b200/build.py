@@ -1,5 +1,5 @@
-"""Build libpvraft_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so must travel with the
-repo snapshot to the GPU box).  `python -m pvraft_b200.build [--force]`."""
+"""Build libpvraft_b200.so in-tree with nvcc for sm_90a (H100), ahead of time: the library sits next to the
+package, so a tree that was built once imports and runs without nvcc.  `python -m pvraft_b200.build [--force]`."""
 import os
 import shlex
 import subprocess
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libpvraft_b200.so')
 SOURCES = ['capi.cu', 'flow_metrics.cu', 'corr_gemm.cu', 'corr_lookup.cu', 'corr_topk.cu', 'knn.cu', 'knn_branch.cu', 'pointmlp.cu', 'setconv_edge.cu', 'tc_linear.cu', 'train.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '--expt-relaxed-constexpr']
 
 
@@ -30,7 +30,7 @@ def stale():
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a and link the C-ABI shared library.  Returns its path."""
+    """Compile every CUDA source for sm_90a and link the C-ABI shared library.  Returns its path."""
     if not force and not stale():
         return LIB
     nvcc = _nvcc()
@@ -49,7 +49,7 @@ def build(force=False, verbose=False):
             print(out)
         if p.returncode != 0:
             raise RuntimeError(f'nvcc failed on {src}:\n{out}')
-    cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a']
+    cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a']
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n' + r.stdout)

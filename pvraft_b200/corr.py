@@ -1,6 +1,6 @@
 """CorrBlock -- mirror of the reference module (model/corr.py:8-100): same constructor, parameters,
 state_dict keys and call surface (`init_module`, `__call__(coords)`, `get_voxel_feature`,
-`get_knn_feature`, `calculate_corr`), with the arithmetic on the B200 kernels.
+`get_knn_feature`, `calculate_corr`), with the arithmetic on the H100 kernels.
 
 State layout differs from the reference on purpose: instead of the materialised
 `truncate_xyz2 [B,N,K,3]` (12 B/candidate) the block keeps the candidate INDEX (int32) next to the
@@ -65,12 +65,12 @@ class CorrBlock(nn.Module):
     # ------------------------------------------------------------------------------------------
     @staticmethod
     def calculate_corr_pm(fmap1_pm, fmap2_pm):
-        """Point-major [B,N,C] feature maps -> corr [B,N,N] = <f1_i, f2_j> / sqrt(C) on the tcgen05 GEMM (3xTF32, fp32-accurate).
+        """Point-major [B,N,C] feature maps -> corr [B,N,N] = <f1_i, f2_j> / sqrt(C) on the wgmma GEMM (3xTF32, fp32-accurate).
         The kernel works on 128-point tiles: a ragged N is zero-padded to the next multiple of 128 and the result cropped
         (no library GEMM on any path)."""
         b, n, c = fmap1_pm.shape
         if c % 32 != 0:
-            raise NotImplementedError(f'calculate_corr: {c} feature channels (the tcgen05 GEMM needs a multiple of 32; the model has 128)')
+            raise NotImplementedError(f'calculate_corr: {c} feature channels (the wgmma GEMM needs a multiple of 32; the model has 128)')
         pad = (-n) % 128
         if pad == 0:
             return ops.corr_matmul(fmap1_pm, fmap2_pm)
@@ -95,7 +95,7 @@ class CorrBlock(nn.Module):
         b, n_p, _ = xyz2.shape
         if n_p < self.truncate_k:
             raise ValueError(f'truncate_k={self.truncate_k} exceeds the number of points {n_p}')
-        corr = self.calculate_corr_pm(fmap1_pm.contiguous(), fmap2_pm.contiguous())   # tcgen05, 3xTF32 (fp32-accurate)
+        corr = self.calculate_corr_pm(fmap1_pm.contiguous(), fmap2_pm.contiguous())   # wgmma, 3xTF32 (fp32-accurate)
         val, idx = ops.corr_topk(corr, self.truncate_k)
         self._install(*ops.corr_reorder(val, idx))
         self._xyz2 = xyz2.detach().contiguous().float()
@@ -164,7 +164,7 @@ class CorrBlock(nn.Module):
         oc = self.out_conv
         kpad = (nvox + 31) // 32 * 32
         if ops.tc_supported(n) and kpad - nvox <= 32:
-            # out_conv[0] on tcgen05: the lookup pads the voxel rows to a multiple of 32 channels (zeros)
+            # out_conv[0] on wgmma: the lookup pads the voxel rows to a multiple of 32 channels (zeros)
             lk = self.lookup(coords, vox_ld=kpad)
             y1 = ops.tc_linear([lk['vox']], ops.tc_weights(oc[0].weight, cols=nvox, k_pad=kpad), _w(oc[0].bias),
                                out_stats=stats[0])
@@ -181,7 +181,7 @@ class CorrBlock(nn.Module):
         return corr, keep
 
     def feature_motion_tc(self, coords, flow, motion_encoder, need_corr=True):
-        """Lookup + feature head + MotionEncoder with every 1x1 convolution on the tcgen05 tensor cores
+        """Lookup + feature head + MotionEncoder with every 1x1 convolution on the Hopper tensor cores (wgmma)
         (model/corr.py:42-45 and model/update.py:15-21): coords, flow [B,N,3] -> (corr [B,N,64], motion [B,N,64]);
         with need_corr=False the correlation feature itself is not materialised (one launch fewer) and None is returned.
         Needs ops.tc_supported(N)."""

@@ -32,10 +32,10 @@ int check_launch(const char* what) {
 int sm_count() {
     static thread_local int cached_dev = -1, cached = 0;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (dev != cached_dev) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         cached = n;
         cached_dev = dev;
     }

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the pvraft_b200 kernels (sm_100a only).
+// Shared device/host helpers for the pvraft_b200 kernels (sm_90a).
 #pragma once
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -11,7 +11,7 @@ namespace pvraft {
 
 constexpr int kWarp = 32;
 constexpr unsigned kFull = 0xffffffffu;
-constexpr int kSmemBudget = 227 * 1024;  // opt-in dynamic shared memory per CTA on sm_100
+constexpr int kSmemBudget = 227 * 1024;  // opt-in dynamic shared memory per CTA on sm_90 (H100)
 
 // ---- host side error plumbing (definitions in capi.cu) -------------------------------------------
 void set_error(const char* fmt, ...);

@@ -1,4 +1,4 @@
-// All-pairs feature correlation on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), fp32-accurate.
+// All-pairs feature correlation on the Hopper tensor cores (wgmma + TMA), fp32-accurate.
 //
 // Replaces CorrBlock.calculate_corr (reference model/corr.py:95-100):  corr[b,i,j] = <fmap1[b,:,i], fmap2[b,:,j]> / sqrt(C).
 // This is the one large dense contraction of the model (2*N*N*C = 17.2 GFLOP per sample at N=8192).
@@ -10,15 +10,16 @@
 // k_corr_gemm below.  The division by sqrt(C) is a true division, as on the reference's CPU path.
 #include <cuda.h>
 
-#include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pvraft {
 
-constexpr int kGemmThreads = 320;   // TMA producer | MMA issuer | 8 epilogue warps
+constexpr int kGemmThreads = 384;   // warpgroup 0: TMA producer (one thread) | warpgroups 1, 2: MMA + epilogue
 constexpr int kTileM = 128, kTileN = 128, kBlockK = 32;     // 32 tf32 = one 128-byte swizzle row
 constexpr int kOperandBytes = kTileM * kBlockK * 4;         // 16 KB
 constexpr int kStageBytes = 4 * kOperandBytes;              // A_hi, A_lo, B_hi, B_lo
 constexpr int kStages = 3;
+constexpr int kConsumerWarps = 8;
 
 __device__ __forceinline__ unsigned su32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 
@@ -39,38 +40,13 @@ __device__ __forceinline__ void mbar_wait_(void* bar, unsigned parity) {
         "r"(parity)
         : "memory");
 }
+__device__ __forceinline__ void mbar_arrive_(void* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(su32(bar)) : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, void* bar, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(su32(dst)),
                  "l"(map), "r"(su32(bar)), "r"(c0), "r"(c1)
                  : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start address >> 4 in bits
-// [0,14), leading byte offset (unused for swizzled K-major, 1) in [16,30), stride byte offset = 8 rows * 128 B = 1024 B
-// (>> 4 = 64) in [32,46), version 1 in [46,48), layout type 2 (SWIZZLE_128B) in [61,64).
-__device__ __forceinline__ unsigned long long umma_desc(const void* smem_tile) {
-    unsigned long long d = 0;
-    d |= (unsigned long long)((su32(smem_tile) >> 4) & 0x3FFFu);
-    d |= (unsigned long long)1 << 16;
-    d |= (unsigned long long)64 << 32;
-    d |= (unsigned long long)1 << 46;
-    d |= (unsigned long long)2 << 61;
-    return d;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1) at [4,6), a/b format TF32 (2) at [7,10)/[10,13),
-// K-major A and B (0), n_dim = N>>3 at [17,23), m_dim = M>>4 at [24,29)
-__host__ __device__ constexpr unsigned umma_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(N >> 3) << 17) | ((unsigned)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(unsigned tmem_d, unsigned long long da, unsigned long long db, unsigned idesc, unsigned accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(void* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(su32(bar)) : "memory");
 }
 
 struct GemmParams {
@@ -82,22 +58,6 @@ struct GemmParams {
     long long n_tiles;   // B * tiles_n * tiles_n
 };
 
-__device__ __forceinline__ bool elect_one() {
-    unsigned pred;
-    asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void mbar_arrive_(void* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(su32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(unsigned taddr, unsigned (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 // x / s, correctly rounded, from r = RN(1/s) (Markstein): q0 = x r; q = q0 + (x - q0 s) r.  Three instructions instead of
 // the ~10 of the generic division, bit-identical to it (checked against true division on 1.3e8 values, see DESIGN.md).
 __device__ __forceinline__ float div_by_const(float x, float s, float r) {
@@ -105,19 +65,13 @@ __device__ __forceinline__ float div_by_const(float x, float s, float r) {
     return fmaf(fmaf(-q0, s, x), r, q0);
 }
 
-constexpr int kEpiWarps = 8;
-constexpr int kStageCols = 16;                                   // columns staged per epilogue step
-constexpr int kStagePitch = kStageCols + 4;                      // floats; keeps float4 alignment, spreads banks
-constexpr int kEpiStageBytes = kEpiWarps * 32 * kStagePitch * 4; // 20 KB
-
 // Persistent kernel, one CTA per SM, tiles t = blockIdx.x + i * gridDim.x with the column tile fastest (neighbouring CTAs
 // share the A row-panel in L2):
-//   warp 0      TMA producer: four 128 x 32 boxes (A hi/lo, B hi/lo) per k-block into a 3-stage ring
-//   warp 1      MMA issuer (whole warp walks the loop, one elected lane issues): 3 x 4 tcgen05.mma per k-block into one of
-//               two 128-column TMEM accumulators
-//   warps 2-9   epilogue, two warps per TMEM lane quadrant: tcgen05.ld 16 columns -> exact division by sqrt(C) -> transpose
-//               through shared memory -> 64-byte row segments to global.  It drains accumulator t while the MMAs of tile
-//               t+1 run.
+//   warp 0          TMA producer: four 128 x 32 boxes (A hi/lo, B hi/lo) per k-block into a 3-stage ring; it runs up to
+//                   three k-blocks ahead, across tile boundaries, so the next tile's operands land during the epilogue
+//   warpgroups 1-2  rows [64 (g - 1), +64) of the tile: 3 x 4 wgmma.m64n128k8 per k-block (the stage is released once
+//                   the next k-block's group is in flight), then the epilogue straight from the accumulator registers:
+//                   exact division by sqrt(C), each store instruction writes 8 rows x 32 contiguous bytes
 __global__ void __launch_bounds__(kGemmThreads, 1)
 k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
             const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const GemmParams p) {
@@ -125,9 +79,7 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
     // 1024-byte alignment (SWIZZLE_128B) by pointer arithmetic on the shared array: an integer round trip would lose the
     // address space and turn every shared-memory access into a generic LD/ST
     unsigned char* tiles = smem_raw + ((1024u - ((unsigned)__cvta_generic_to_shared(smem_raw) & 1023u)) & 1023u);
-    float* s_stage = reinterpret_cast<float*>(tiles + (size_t)kStages * kStageBytes);
-    __shared__ __align__(8) unsigned long long s_full[kStages], s_empty[kStages], s_acc_full[2], s_acc_empty[2];
-    __shared__ unsigned s_tmem_base;
+    __shared__ __align__(8) unsigned long long s_full[kStages], s_empty[kStages];
     const int warp = warp_id(), lane = lane_id();
     const int num_kb = p.C / kBlockK;
     const long long my_tiles = blockIdx.x < p.n_tiles ? (p.n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
@@ -137,25 +89,15 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b_lo) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init_(&s_full[s], 1); mbar_init_(&s_empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init_(&s_acc_full[a], 1); mbar_init_(&s_acc_empty[a], kEpiWarps); }
+        for (int s = 0; s < kStages; ++s) { mbar_init_(&s_full[s], 1); mbar_init_(&s_empty[s], kConsumerWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {   // two 128-column fp32 accumulators
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(su32(&s_tmem_base)), "r"(256u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const unsigned tmem = s_tmem_base;
     const int tiles_per_batch = p.tiles_n * p.tiles_n;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ===== TMA producer =====
-        if (lane == 0) {
+        if (warp == 0 && lane == 0) {
             int s = 0;
             unsigned phase = 0;
             for (long long i = 0; i < my_tiles; ++i) {
@@ -175,82 +117,51 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        constexpr unsigned idesc = umma_idesc_tf32(kTileM, kTileN);
-        int s = 0;
-        unsigned phase = 0;
-        for (long long i = 0; i < my_tiles; ++i) {
-            const int acc = (int)(i & 1);
-            mbar_wait_(&s_acc_empty[acc], (((unsigned)(i >> 1)) & 1u) ^ 1u);   // the epilogue has drained this accumulator
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const unsigned tacc = tmem + (unsigned)(acc * kTileN);
-            for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_wait_(&s_full[s], phase);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                unsigned char* st = tiles + (size_t)s * kStageBytes;
-                const unsigned long long a_hi = umma_desc(st + 0 * kOperandBytes), a_lo = umma_desc(st + 1 * kOperandBytes);
-                const unsigned long long b_hi = umma_desc(st + 2 * kOperandBytes), b_lo = umma_desc(st + 3 * kOperandBytes);
-                if (elect_one()) {
-#pragma unroll
-                    for (int k = 0; k < kBlockK / 8; ++k) {
-                        // one MMA covers K = 8 tf32 = 32 bytes: advance the start address field by 32 B >> 4 = 2
-                        const unsigned long long off = (unsigned long long)(k * 2);
-                        umma_tf32(tacc, a_hi + off, b_hi + off, idesc, (kb | k) != 0 ? 1u : 0u);
-                        umma_tf32(tacc, a_lo + off, b_hi + off, idesc, 1u);
-                        umma_tf32(tacc, a_hi + off, b_lo + off, idesc, 1u);
-                    }
-                    umma_commit(&s_empty[s]);                            // the stage may be refilled once these MMAs retire
-                    if (kb == num_kb - 1) umma_commit(&s_acc_full[acc]);  // accumulator complete
-                }
-                __syncwarp();
-                if (++s == kStages) { s = 0; phase ^= 1u; }
-            }
-        }
-    } else {
-        // ===== epilogue: TMEM -> registers -> shared (transpose) -> global =====
-        const int quad = warp & 3;                 // a warp may only touch TMEM lanes 32*(warp%4) .. +31
-        const int half = (warp - 2) >> 2;          // columns [64*half, 64*half + 64) of the tile
-        float* stg = s_stage + (size_t)(warp - 2) * 32 * kStagePitch;
-        const int rsub = lane >> 2, cq = lane & 3; // store phase: 8 rows x 4 float4 per instruction
-        for (long long i = 0; i < my_tiles; ++i) {
-            const long long t = blockIdx.x + i * gridDim.x;
-            const int b = (int)(t / tiles_per_batch), r = (int)(t - (long long)b * tiles_per_batch);
-            const int tile_m = r / p.tiles_n, tile_n = r - tile_m * p.tiles_n;
-            const int acc = (int)(i & 1);
-            mbar_wait_(&s_acc_full[acc], ((unsigned)(i >> 1)) & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const unsigned tl = tmem + (unsigned)(acc * kTileN) + ((unsigned)(quad * 32) << 16);
-            float* obase = p.corr + ((size_t)b * p.N + (size_t)tile_m * kTileM + quad * 32 + rsub) * p.N + (size_t)tile_n * kTileN + cq * 4;
-#pragma unroll 1
-            for (int c0 = half * 64; c0 < half * 64 + 64; c0 += kStageCols) {
-                unsigned v[16];
-                tmem_ld16(tl + (unsigned)c0, v);
-                __syncwarp();   // the previous step's readers are done with the staging tile
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    // corr / sqrt(C) as a true (correctly rounded) division (model/corr.py:99)
-                    *reinterpret_cast<float4*>(stg + lane * kStagePitch + q * 4) =
-                        make_float4(div_by_const(__uint_as_float(v[q * 4 + 0]), p.scale, p.rscale), div_by_const(__uint_as_float(v[q * 4 + 1]), p.scale, p.rscale),
-                                    div_by_const(__uint_as_float(v[q * 4 + 2]), p.scale, p.rscale), div_by_const(__uint_as_float(v[q * 4 + 3]), p.scale, p.rscale));
-                }
-                __syncwarp();
-                float4 o[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) o[j] = *reinterpret_cast<const float4*>(stg + (j * 8 + rsub) * kStagePitch + cq * 4);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) *reinterpret_cast<float4*>(obase + (size_t)(j * 8) * p.N + c0) = o[j];
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive_(&s_acc_empty[acc]);
-        }
+        return;
     }
-    __syncwarp();   // the producer runs on one lane: re-converge before the CTA-wide (aligned) barrier
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(256u) : "memory");
+    // ===== MMA + epilogue, one warpgroup per 64-row half of the tile =====
+    const int half = (warp >> 2) - 1;             // 0 | 1
+    const int wq = warp & 3;                       // warp within the warpgroup: rows 16 wq .. +15 of the half
+    const int a_off = half * 64 * 128;             // byte offset of the half's rows inside an A box (1024-aligned)
+    float acc[64];
+    int s = 0, prev_s = -1;
+    unsigned phase = 0;
+    for (long long i = 0; i < my_tiles; ++i) {
+        const long long t = blockIdx.x + i * gridDim.x;
+        const int b = (int)(t / tiles_per_batch), r = (int)(t - (long long)b * tiles_per_batch);
+        const int tile_m = r / p.tiles_n, tile_n = r - tile_m * p.tiles_n;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait_(&s_full[s], phase);
+            unsigned char* st = tiles + (size_t)s * kStageBytes;
+            const unsigned long long a_hi = wgmma_desc(st + 0 * kOperandBytes + a_off), a_lo = wgmma_desc(st + 1 * kOperandBytes + a_off);
+            const unsigned long long b_hi = wgmma_desc(st + 2 * kOperandBytes), b_lo = wgmma_desc(st + 3 * kOperandBytes);
+            wgmma_fence_regs(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kBlockK / 8; ++k) {
+                wgmma_tf32<kTileN>(acc, wgmma_desc_k(a_hi, k), wgmma_desc_k(b_hi, k), (kb | k) != 0);
+                wgmma_tf32<kTileN>(acc, wgmma_desc_k(a_lo, k), wgmma_desc_k(b_hi, k), 1);
+                wgmma_tf32<kTileN>(acc, wgmma_desc_k(a_hi, k), wgmma_desc_k(b_lo, k), 1);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                       // the previous k-block's MMAs have retired: its stage may be refilled
+            if (prev_s >= 0 && lane == 0) mbar_arrive_(&s_empty[prev_s]);
+            prev_s = s;
+            if (++s == kStages) { s = 0; phase ^= 1u; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (lane == 0) mbar_arrive_(&s_empty[prev_s]);
+        prev_s = -1;
+        // corr / sqrt(C) as a true (correctly rounded) division (model/corr.py:99)
+        const int row = tile_m * kTileM + half * 64 + wq * 16 + (lane >> 2);
+        float* o = p.corr + ((size_t)b * p.N + row) * p.N + (size_t)tile_n * kTileN + 2 * (lane & 3);
+        const size_t down8 = (size_t)8 * p.N;
+#pragma unroll
+        for (int j = 0; j < kTileN / 8; ++j) {
+            *reinterpret_cast<float2*>(o + 8 * j) = make_float2(div_by_const(acc[4 * j + 0], p.scale, p.rscale), div_by_const(acc[4 * j + 1], p.scale, p.rscale));
+            *reinterpret_cast<float2*>(o + down8 + 8 * j) = make_float2(div_by_const(acc[4 * j + 2], p.scale, p.rscale), div_by_const(acc[4 * j + 3], p.scale, p.rscale));
+        }
     }
 }
 
@@ -340,7 +251,7 @@ extern "C" int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, in
     p.rscale = (float)(1.0 / (double)p.scale);
     p.tiles_n = N / kTileN;
     p.n_tiles = (long long)B * p.tiles_n * p.tiles_n;
-    const size_t smem = (size_t)kStages * kStageBytes + kEpiStageBytes + 1024;
+    const size_t smem = (size_t)kStages * kStageBytes + 1024;
     if ((rc = opt_in_smem(k_corr_gemm, smem))) return rc;
     const int grid = (int)(p.n_tiles < sm_count() ? p.n_tiles : sm_count());
     k_corr_gemm<<<grid, kGemmThreads, smem, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, p);

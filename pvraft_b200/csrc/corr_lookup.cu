@@ -256,8 +256,6 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
                 unsigned dist[KPL];       // fp32 bits of the (non-negative) squared distance
                 unsigned valid_bits = 0;  // bit e: candidate e of this lane lies inside the coarsest 3x3x3 cube
                 const float thr = p.thr_c;
-                unsigned long long cxy;
-                asm("mov.b64 %0, {%1, %2};" : "=l"(cxy) : "f"(cx), "f"(cy));
 #pragma unroll
                 for (int j = 0; j < NJ; ++j) {
                     int ci[VEC];
@@ -274,17 +272,10 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
 #pragma unroll
                     for (int s = 0; s < VEC; ++s) {
                         const float4 q = SMEM_TAB ? s_tab[ci[s]] : __ldg(tab_g + ci[s]);
-                        // (dx,dy) and their squares as packed fp32x2 operations (one issue slot each; every component is an
-                        // IEEE round-to-nearest subtract / multiply, exactly the scalar sequence of model/corr.py:78-79)
-                        float dx, dy, sx, sy;
-                        {
-                            unsigned long long qxy, dxy, sxy;
-                            asm("mov.b64 %0, {%1, %2};" : "=l"(qxy) : "f"(q.x), "f"(q.y));
-                            asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(dxy) : "l"(qxy), "l"(cxy));
-                            asm("mul.rn.f32x2 %0, %1, %1;" : "=l"(sxy) : "l"(dxy));
-                            asm("mov.b64 {%0, %1}, %2;" : "=f"(dx), "=f"(dy) : "l"(dxy));
-                            asm("mov.b64 {%0, %1}, %2;" : "=f"(sx), "=f"(sy) : "l"(sxy));
-                        }
+                        // every component an IEEE round-to-nearest subtract / multiply, exactly the scalar sequence of
+                        // model/corr.py:78-79
+                        const float dx = __fsub_rn(q.x, cx), dy = __fsub_rn(q.y, cy);
+                        const float sx = __fmul_rn(dx, dx), sy = __fmul_rn(dy, dy);
                         const float dz = __fsub_rn(q.z, cz);
                         const float d2 = __fadd_rn(__fadd_rn(sx, sy), __fmul_rn(dz, dz));
                         dist[j * VEC + s] = __float_as_uint(d2);

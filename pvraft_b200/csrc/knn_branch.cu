@@ -1,12 +1,11 @@
-// kNN branch of the correlation feature head + the flow embedding of the MotionEncoder, for the tcgen05 path.
+// kNN branch of the correlation feature head + the flow embedding of the MotionEncoder, for the tensor-core path.
 //
 //   kfeat[b,n,c] = max_e PReLU(GN(knn_conv.0(f_e)))      reference model/corr.py:86-92 (knn_conv, then max over dim 3)
 //   cflow[b,n,c] = relu(conv_flow(flow))                 reference model/update.py:17
 //
 // f_e = (corr, dx, dy, dz) of the 32 selected candidates (knn_sel from the lookup kernel).  The GroupNorm statistics of the
 // [B,64,N,32] tensor follow analytically from the per-sample moments of f that the lookup accumulated, so the affine is
-// folded into the 4->64 convolution and the whole branch is one pass: 4 FMA + max + min per (candidate, channel), the FMAs
-// issued as packed fp32x2 instructions (FFMA2) over candidate pairs.
+// folded into the 4->64 convolution and the whole branch is one pass: 4 FMA + max + min per (candidate, channel).
 // PReLU with slope <= 1 is convex, so max_e PReLU(t_e) = max(PReLU(max_e t_e), PReLU(min_e t_e)) exactly; a learned slope
 // above 1 takes the per-candidate path.
 //
@@ -19,16 +18,9 @@ namespace pvraft {
 constexpr int kKbThreads = 256;
 constexpr int kKbTile = 64;
 
-// packed fp32x2 FMA (sm_100 FFMA2): two IEEE fma.rn per instruction, results identical to the scalar form
+// two IEEE fma.rn over a candidate pair
 __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-    unsigned long long ra, rb, rc, rd;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-    float2 d;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-    return d;
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 template <bool CONVEX>

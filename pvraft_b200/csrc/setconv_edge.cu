@@ -16,8 +16,8 @@ namespace pvraft {
 
 constexpr int kEdgeThreads = 256;
 
-// packed fp32x2 arithmetic (sm_100 FFMA2 / FADD2 / FMUL2): two IEEE-rounded operations per instruction, bit-identical to
-// the scalar forms
+// elementwise arithmetic on channel pairs held as one 64-bit value: each component is one IEEE round-to-nearest operation
+// (the _rn intrinsics are never contracted into an FMA)
 __device__ __forceinline__ unsigned long long pk(float lo, float hi) {
     unsigned long long r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -29,24 +29,20 @@ __device__ __forceinline__ float2 upk(unsigned long long v) {
     return d;
 }
 __device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
+    const float2 x = upk(a), y = upk(b), z = upk(c);
+    return pk(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
 }
 __device__ __forceinline__ unsigned long long mul2(unsigned long long a, unsigned long long b) {
-    unsigned long long d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    const float2 x = upk(a), y = upk(b);
+    return pk(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y));
 }
 __device__ __forceinline__ unsigned long long add2(unsigned long long a, unsigned long long b) {
-    unsigned long long d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    const float2 x = upk(a), y = upk(b);
+    return pk(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y));
 }
 __device__ __forceinline__ unsigned long long sub2(unsigned long long a, unsigned long long b) {
-    unsigned long long d;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    const float2 x = upk(a), y = upk(b);
+    return pk(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y));
 }
 
 template <int PAIRS>

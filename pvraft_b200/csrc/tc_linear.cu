@@ -1,33 +1,34 @@
-// Per-point linear layers on the tcgen05 tensor cores, fp32-accurate (3xTF32), with the GroupNorm / activation
+// Per-point linear layers on the Hopper tensor cores (wgmma), fp32-accurate (3xTF32), with the GroupNorm / activation
 // prologue and the bias / activation / residual / GroupNorm-statistics / GRU-gate epilogues fused around the MMA.
 //
 //   out[M x N] = epilogue( prologue(A)[M x K] . W[N x K]^T )          M = B*Npts points, N = cout, K = cin
 //
-// Persistent kernel, one CTA (18 warps) per SM, tiles of 128 consecutive points (= 128 TMEM lanes), 32-channel k-blocks:
-//   warp 0       TMA producer: raw fp32 activation boxes [128 x 32] (SWIZZLE_128B; up to three source tensors concatenated
+// Persistent kernel, one CTA (17 warps) per SM, tiles of 128 consecutive points, 32-channel k-blocks:
+//   warp 16      TMA producer: raw fp32 activation boxes [128 x 32] (SWIZZLE_128B; up to three source tensors concatenated
 //                along K, e.g. [h | inp | motion] for the GRU) into a ring of 2..6 stages; the pre-split weight boxes
 //                W_hi, W_lo once per CTA when they fit next to the ring, else with every k-block
-//   warps 2-9    transform, two groups on alternate k-blocks: every 16-byte chunk of the raw box gets the folded GroupNorm
-//                affine + activation of its channels (optionally choosing the max or the min input by the sign of the
-//                scale), is split into hi = tf32(x), lo = tf32(x - hi) and written in place / next to it AT THE SAME swizzled
-//                offset (the split is elementwise); fence.proxy.async; one mbarrier arrival per warp
-//   warp 1       MMA issuer (the warp walks the loop, one elected lane issues): A_hi.W_hi + A_lo.W_hi + A_hi.W_lo =
-//                3 x 4 tcgen05.mma.kind::tf32 (K = 8 each) per k-block into one of two TMEM accumulators
-//   warps 10-17  epilogue, two per TMEM lane quadrant, one accumulator behind the MMA: tcgen05.ld -> bias / activation /
-//                residual -> transpose through shared memory -> coalesced stores; GroupNorm (sum, sum^2) of the output
-//                combined across the warps into one double atomic per (group, moment) and tile; ConvGRU-gate, cat-tail and
-//                flow-head (64 -> 3 + RAFT coordinate update) variants
+//   warps 8-15   two warpgroups, one per 64-row half of the tile.  Each transforms its rows of the raw box in place: every
+//                16-byte chunk gets the folded GroupNorm affine + activation of its channels (optionally choosing the max or
+//                the min input by the sign of the scale), is split into hi = tf32(x), lo = tf32(x - hi) and written AT THE
+//                SAME swizzled offset (the split is elementwise); fence.proxy.async; then it issues A_hi.W_hi + A_lo.W_hi +
+//                A_hi.W_lo = 3 x 4 wgmma.m64nNk8.tf32 and transforms the next k-block while they run.  At the end of a tile
+//                the accumulator registers go to a shared-memory tile [128 rows][N] and the warpgroup moves on
+//   warps 0-7    epilogue, two per 32-row lane quadrant, one tile behind the MMA: thread = row reads its accumulator row ->
+//                bias / activation / residual -> transpose through shared memory -> coalesced stores; GroupNorm (sum,
+//                sum^2) of the output combined across the warps into one double atomic per (group, moment) and tile;
+//                ConvGRU-gate, cat-tail and flow-head (64 -> 3 + RAFT coordinate update) variants
 // Launched with programmatic stream serialization: the prologue overlaps the previous kernel's tail (griddepcontrol.wait
 // precedes the first global read).  Replaces the k_linear / k_gru / k_corrfeat / k_flowout CUDA-core kernels whenever
 // Npts % 128 == 0 and every source has a multiple of 32 channels.
 #include <cuda.h>
 #include <stdlib.h>
 
-#include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pvraft {
 
-constexpr int kTcThreads = 576;   // TMA producer | MMA | 8 transform warps (two groups) | 8 epilogue warps
+constexpr int kTcThreads = 544;   // 8 epilogue warps | 2 transform + MMA warpgroups | TMA producer
+constexpr int kTcEpiThreads = 256, kTcProducerWarp = 16;
 constexpr int kTcM = 128, kTcKB = 32;
 constexpr int kTcABytes = kTcM * kTcKB * 4;   // 16 KB: one activation box
 constexpr int kTcMaxStages = 6;
@@ -110,49 +111,19 @@ __device__ __forceinline__ void ttma_load_2d(void* dst, const CUtensorMap* map, 
                  "l"(map), "r"(tsu32(bar)), "r"(c0), "r"(c1)
                  : "memory");
 }
-__device__ __forceinline__ unsigned long long tumma_desc(const void* smem_tile) {   // K-major, SWIZZLE_128B (see corr_gemm.cu)
-    unsigned long long d = 0;
-    d |= (unsigned long long)((tsu32(smem_tile) >> 4) & 0x3FFFu);
-    d |= (unsigned long long)1 << 16;
-    d |= (unsigned long long)64 << 32;
-    d |= (unsigned long long)1 << 46;
-    d |= (unsigned long long)2 << 61;
-    return d;
-}
-__device__ __forceinline__ void tumma_tf32(unsigned tmem_d, unsigned long long da, unsigned long long db, unsigned idesc, unsigned accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tumma_commit(void* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(tsu32(bar)) : "memory");
-}
 // round-to-nearest (ties away from zero) to the 10-bit TF32 mantissa with two full-rate integer ops; identical to
 // cvt.rna.tf32.f32 for finite values (the conversion instruction runs at a fraction of the ALU rate)
 __device__ __forceinline__ float tf32_rna(float x) {
     return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
-__device__ __forceinline__ void tmem_ld32(unsigned taddr, unsigned (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,"
-        "%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld16(unsigned taddr, unsigned (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// row `arow` of the shared accumulator tile, W consecutive columns, as raw bits (thread = row)
+template <int W>
+__device__ __forceinline__ void acc_ld(const float* arow, unsigned (&v)[W]) {
+#pragma unroll
+    for (int q = 0; q < W / 4; ++q) {
+        const uint4 u = *reinterpret_cast<const uint4*>(arow + 4 * q);
+        v[4 * q + 0] = u.x; v[4 * q + 1] = u.y; v[4 * q + 2] = u.z; v[4 * q + 3] = u.w;
+    }
 }
 // thread-per-row values of a [32 rows x 16 columns] block -> shared-memory transpose -> stores of 8 rows x 64 B per instruction
 // (thread-per-row stores would scatter 32 half-filled sectors per instruction).  stg: this warp's [32][20] staging tile.
@@ -200,32 +171,27 @@ __device__ __forceinline__ unsigned ld_acquire_gpu(const int* p) {
 __device__ __forceinline__ void red_release_gpu(int* p) {
     asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p) : "memory");
 }
-__device__ __forceinline__ bool telect_one() {
-    unsigned pred;
-    asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(pred));
-    return pred != 0;
-}
 __device__ __forceinline__ float tsigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 
-// epilogue of one accumulator buffer: thread = point (TMEM lane)
-__device__ __forceinline__ void tc_epilogue(const TcParams& p, unsigned tacc, int quad, int half, int lane, int row0, int sample,
-                                            const float* __restrict__ s_bias, float* __restrict__ s_stage, float* __restrict__ s_part) {
+// epilogue of the accumulator tile s_acc [128 rows][pitch]: thread = point (row quad * 32 + lane)
+__device__ __forceinline__ void tc_epilogue(const TcParams& p, float* __restrict__ s_acc, int pitch, int quad, int half, int lane, int row0,
+                                            int sample, const float* __restrict__ s_bias, float* __restrict__ s_stage, float* __restrict__ s_part) {
     const int row = row0 + quad * 32 + lane;
     const int gsz = p.cout / PVRAFT_GN_GROUPS;
-    const unsigned tl = tacc + ((unsigned)(quad * 32) << 16);
+    const float* arow = s_acc + (size_t)(quad * 32 + lane) * pitch;
     if (p.epi == TC_EPI_PLAIN) {
         // Every tile is full (M is a multiple of 128).  This code runs on one warp per scheduler, so it is written for
         // latency: no per-element branches, addresses hoisted, loads batched ahead of their consumers.
         const bool vec = (p.out_ld & 3) == 0;
         const ActCoef oact = act_coef(p.out_act, 0.f);
-        float* stg = s_stage + (size_t)(half * 4 + quad) * 32 * 36;   // this warp's [32 rows][36] staging tile
         const int rsub = lane >> 3, cq = lane & 7;
         float* obase = p.out + (size_t)(row0 + quad * 32 + rsub) * p.out_ld + cq * 4;
         const size_t ostep = (size_t)4 * p.out_ld;
         const bool want_stats = p.out_stats != nullptr;
         for (int c0 = half * 32; c0 < p.N; c0 += 64) {
             unsigned v[32];
-            tmem_ld32(tl + (unsigned)c0, v);
+            acc_ld(arow + c0, v);
+            float* stg = s_acc + (size_t)(quad * 32) * pitch + c0;   // this warp's [32 rows][32 columns]: staged in place
             float y[32];
 #pragma unroll
             for (int q = 0; q < 8; ++q) {
@@ -250,11 +216,11 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, unsigned tacc, in
                 __syncwarp();
 #pragma unroll
                 for (int q = 0; q < 8; ++q)
-                    *reinterpret_cast<float4*>(stg + lane * 36 + q * 4) = make_float4(y[q * 4], y[q * 4 + 1], y[q * 4 + 2], y[q * 4 + 3]);
+                    *reinterpret_cast<float4*>(stg + lane * pitch + q * 4) = make_float4(y[q * 4], y[q * 4 + 1], y[q * 4 + 2], y[q * 4 + 3]);
                 __syncwarp();
                 float4 t[8];
 #pragma unroll
-                for (int i = 0; i < 8; ++i) t[i] = *reinterpret_cast<const float4*>(stg + (i * 4 + rsub) * 36 + cq * 4);
+                for (int i = 0; i < 8; ++i) t[i] = *reinterpret_cast<const float4*>(stg + (i * 4 + rsub) * pitch + cq * 4);
                 if (c0 + cq * 4 < p.out_ld) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) *reinterpret_cast<float4*>(obase + i * ostep + c0) = t[i];
@@ -264,7 +230,7 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, unsigned tacc, in
                     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
                     for (int r = 0; r < 32; ++r) {
-                        const float a = stg[r * 36 + lane];
+                        const float a = stg[r * pitch + lane];
                         s1 += a;
                         s2 = fmaf(a, a, s2);
                     }
@@ -311,8 +277,8 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, unsigned tacc, in
         float* stg = s_stage + (size_t)(half * 4 + quad) * 32 * kTcPitch16;
         for (int c = half * 32; c < half * 32 + 32; c += 16) {
             unsigned vz[16], vr[16];
-            tmem_ld16(tl + (unsigned)c, vz);
-            tmem_ld16(tl + (unsigned)(64 + c), vr);
+            acc_ld(arow + c, vz);
+            acc_ld(arow + 64 + c, vr);
             float z[16], rh[16], hh[16];
             stage_load16(stg, lane, p.h + (size_t)(row0 + quad * 32) * 64 + c, 64, hh);
 #pragma unroll
@@ -340,7 +306,7 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, unsigned tacc, in
         const float* s_w3 = s_part + 512;   // [3][64], staged at kernel start; s_part[0..511] = [128 rows][4] exchange
         unsigned v[32];
         const int c0 = half * 32;
-        tmem_ld32(tl + (unsigned)c0, v);
+        acc_ld(arow + c0, v);
         float d0 = 0.f, d1 = 0.f, d2 = 0.f;
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
@@ -381,7 +347,7 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, unsigned tacc, in
         float* stg = s_stage + (size_t)(half * 4 + quad) * 32 * kTcPitch16;
         for (int c = half * 32; c < half * 32 + 32; c += 16) {
             unsigned vq[16];
-            tmem_ld16(tl + (unsigned)c, vq);
+            acc_ld(arow + c, vq);
             float o[16], hh[16], zz[16];
             stage_load16(stg, lane, p.h + (size_t)(row0 + quad * 32) * 64 + c, 64, hh);
             stage_load16<true>(stg, lane, p.z + (size_t)(row0 + quad * 32) * 64 + c, 64, zz);   // z comes from the launch before
@@ -404,8 +370,7 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, unsigned tacc, in
     }
 }
 
-// A CTA walks tiles blockIdx.x, +gridDim.x, ...; the operand ring and the two accumulators run across tile boundaries.
-constexpr int kTcXform = 256;   // transform threads
+// A CTA walks tiles blockIdx.x, +gridDim.x, ...; the operand ring runs across tile boundaries.
 
 // Position of one pipeline role in the (tile, k-block) walk and in the operand ring; advanced without divisions (a
 // runtime integer division is a ~100-cycle dependent chain, paid per step by warps that have nothing to hide it behind)
@@ -418,6 +383,23 @@ struct TcCursor {
     }
 };
 
+// one k-block (32 channels) of a warpgroup's 64 x N accumulator: 3xTF32, four K = 8 slices
+template <int N>
+__device__ __forceinline__ void tc_mma_kblock(float (&acc)[64], unsigned long long a_hi, unsigned long long a_lo, unsigned long long b_hi,
+                                              unsigned long long b_lo, int kb) {
+#pragma unroll
+    for (int k = 0; k < kTcKB / 8; ++k) {
+        wgmma_tf32<N>(acc, wgmma_desc_k(a_hi, k), wgmma_desc_k(b_hi, k), (kb | k) != 0);
+        wgmma_tf32<N>(acc, wgmma_desc_k(a_lo, k), wgmma_desc_k(b_hi, k), 1);
+        wgmma_tf32<N>(acc, wgmma_desc_k(a_hi, k), wgmma_desc_k(b_lo, k), 1);
+    }
+}
+// row pitch (floats) of the shared accumulator tile: whole 32-column epilogue chunks plus 4, so that thread-per-row 16-byte
+// accesses of 8 consecutive rows fall into distinct bank groups
+__host__ __device__ __forceinline__ int tc_acc_pitch(int n) { return ((n + 31) & ~31) + 4; }
+
+// NT = p.N (the padded cout): the wgmma shape is part of the instruction
+template <int NT>
 __global__ void __launch_bounds__(kTcThreads, 1)
 k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
             const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
@@ -433,45 +415,39 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
     const int stage_bytes = w_off + (p.w_resident ? 0 : 2 * w_bytes);
     const int S = p.stages;
     const int num_kb = p.K / kTcKB;
+    const int acc_pitch = tc_acc_pitch(NT);
     unsigned char* w_res = tiles + (size_t)S * stage_bytes;
-    float* s_scale = reinterpret_cast<float*>(w_res + (p.w_resident ? (size_t)num_kb * 2 * w_bytes : 0));   // [K]
-    float* s_bias = s_scale + 4 * p.K;                                            // ([2 groups][scale K | shift K] above)                                                // [2 * N]
-    float* s_estage = s_bias + 2 * p.N;                                           // [4 warps][32][36] epilogue staging
-    float* s_part = s_estage + (p.epi == TC_EPI_PLAIN ? 8 * 32 * 36 : (p.epi == TC_EPI_FLOW ? 0 : 8 * 32 * kTcPitch16));   // staging tiles by epilogue                                       // [4 warps][128 columns][2]
-    __shared__ __align__(8) unsigned long long s_full[kTcMaxStages], s_ready[kTcMaxStages], s_empty[kTcMaxStages];
-    __shared__ __align__(8) unsigned long long s_acc_full[2], s_acc_empty[2], s_w_full;
-    __shared__ unsigned s_tmem_base;
+    float* s_scale = reinterpret_cast<float*>(w_res + (p.w_resident ? (size_t)num_kb * 2 * w_bytes : 0));   // [2 groups][scale K | shift K]
+    float* s_bias = s_scale + 4 * p.K;                                            // [2 * N]
+    float* s_acc = s_bias + 2 * p.N;                                              // [128 rows][acc_pitch] accumulator tile
+    float* s_estage = s_acc + (size_t)kTcM * acc_pitch;                           // GRU epilogues: [8 warps][32][20] staging
+    float* s_part = s_estage + (p.epi == TC_EPI_GRU_ZR || p.epi == TC_EPI_GRU_Q ? 8 * 32 * kTcPitch16 : 0);   // [4 warps][128 columns][2]
+    __shared__ __align__(8) unsigned long long s_full[kTcMaxStages], s_empty[kTcMaxStages];
+    __shared__ __align__(8) unsigned long long s_acc_full, s_acc_empty, s_w_full;
     const int warp = warp_id(), lane = lane_id();
     const int n_tiles = (p.M + kTcM - 1) / kTcM;
     const int my_tiles = blockIdx.x < n_tiles ? (n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
     const int total_steps = my_tiles * num_kb;
-    const unsigned acc_cols = p.N <= 32 ? 32u : p.N <= 64 ? 64u : 128u;   // columns per accumulator buffer
-    const unsigned tmem_cols = acc_cols * 2;
 #ifdef PVRAFT_TC_TIMELINE
     const bool clk = p.dbg && blockIdx.x == 0;
 #endif
     TC_MARK(threadIdx.x == 0, 0);
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kTcProducerWarp && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a0) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < S; ++s) { tmbar_init(&s_full[s], 1); tmbar_init(&s_ready[s], kTcXform / 64); tmbar_init(&s_empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { tmbar_init(&s_acc_full[a], 1); tmbar_init(&s_acc_empty[a], 8); }
+        for (int s = 0; s < S; ++s) { tmbar_init(&s_full[s], 1); tmbar_init(&s_empty[s], 8); }   // 8 MMA warps release a stage
+        tmbar_init(&s_acc_full, 8);     // 8 MMA warps deposit the accumulator tile
+        tmbar_init(&s_acc_empty, 8);    // 8 epilogue warps have consumed it
         tmbar_init(&s_w_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tsu32(&s_tmem_base)), "r"(tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    // Programmatic dependent launch: everything above (shared-memory carve-up, barrier init, TMEM allocation, descriptor
-    // prefetch) may overlap the tail of the previous kernel on this stream.  The layer's PARAMETERS (hi/lo weights, biases)
-    // are fetched in that window too when the caller vouches that they are settled (p.settled: last written several
-    // launches ago -- the steady state of a forward, whose weights are split once): the SMs that finished the previous
-    // kernel early then hold their weights when the dependency resolves.  Every read of an ACTIVATION is below the wait.
+    // Programmatic dependent launch: everything above (shared-memory carve-up, barrier init, descriptor prefetch) may
+    // overlap the tail of the previous kernel on this stream.  The layer's PARAMETERS (hi/lo weights, biases) are fetched
+    // in that window too when the caller vouches that they are settled (p.settled: last written several launches ago --
+    // the steady state of a forward, whose weights are split once): the SMs that finished the previous kernel early then
+    // hold their weights when the dependency resolves.  Every read of an ACTIVATION is below the wait.
     auto load_weights = [&]() {   // the whole weight matrix (hi and lo) once per CTA
         tmbar_expect_tx(&s_w_full, (unsigned)(num_kb * 2 * w_bytes));
         for (int kb = 0; kb < num_kb; ++kb) {
@@ -479,34 +455,31 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
             ttma_load_2d(w_res + (size_t)kb * 2 * w_bytes + w_bytes, &map_w_lo, &s_w_full, kb * kTcKB, 0);
         }
     };
-    auto load_bias = [&]() {
-        for (int c = threadIdx.x - 320; c < p.N; c += 256) {
+    auto load_bias = [&]() {   // by the epilogue threads 0..255
+        for (int c = threadIdx.x; c < p.N; c += kTcEpiThreads) {
             s_bias[c] = (p.bias != nullptr && c < p.cout) ? __ldg(p.bias + c) : 0.f;
             s_bias[p.N + c] = (p.bias2 != nullptr && c < p.cout) ? __ldg(p.bias2 + c) : 0.f;
         }
         if (p.epi == TC_EPI_FLOW) {   // out_conv.2: weights behind the exchange buffer, bias in the bias2 slots
-            for (int i = threadIdx.x - 320; i < 192; i += 256) s_part[512 + i] = __ldg(p.w3 + i);
-            if (threadIdx.x - 320 < 3) s_bias[p.N + threadIdx.x - 320] = __ldg(p.b3 + threadIdx.x - 320);
+            for (int i = threadIdx.x; i < 192; i += kTcEpiThreads) s_part[512 + i] = __ldg(p.w3 + i);
+            if (threadIdx.x < 3) s_bias[p.N + threadIdx.x] = __ldg(p.b3 + threadIdx.x);
         }
     };
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    __syncthreads();   // barrier init visible to every role
     if (p.settled) {
-        __syncthreads();   // barrier init visible to the TMA issuer
-        if (warp == 0 && lane == 0 && p.w_resident) load_weights();
-        if (warp >= 10) load_bias();
+        if (warp == kTcProducerWarp && lane == 0 && p.w_resident) load_weights();
+        if (warp < 8) load_bias();
     }
     // Chained on the previous launch (p.wait_on): no grid-wide wait -- the TMA producer waits per sample on that launch's
     // `done` counters instead, so this CTA starts on the tiles whose inputs are complete while the stragglers of the
     // previous launch still run on other SMs.  Everything else this kernel reads is older than the previous launch,
     // which itself only signals after its own dependencies resolved.
     if (p.wait_on == nullptr) asm volatile("griddepcontrol.wait;" ::: "memory");
-    if (!p.settled && warp >= 10) load_bias();
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    if (!p.settled && warp < 8) load_bias();
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const unsigned tmem = s_tmem_base;
 
-    if (warp == 0) {
+    if (warp == kTcProducerWarp) {
         // ===== TMA producer: raw activation boxes (and the weights) =====
         if (lane == 0) {
             if (p.w_resident && !p.settled) load_weights();
@@ -539,62 +512,26 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        // The whole warp walks the loop (convergent control flow keeps the descriptor arithmetic on the uniform datapath)
-        // and one elected lane issues; under `if (lane == 0)` the compiler wraps every UTCHMMA in an election loop.
-        {
-            const unsigned idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(p.N >> 3) << 17) | ((unsigned)(kTcM >> 4) << 24);
-            if (p.w_resident) tmbar_wait(&s_w_full, 0u);
-            int step = 0;
-            TcCursor cm;
-            for (int ti = 0; ti < my_tiles; ++ti) {
-                const int acc = ti & 1;
-                const unsigned acc_phase = (unsigned)(ti >> 1) & 1u;
-                tmbar_wait(&s_acc_empty[acc], acc_phase ^ 1u);   // the epilogue has drained this accumulator buffer
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const unsigned tacc = tmem + (unsigned)acc * acc_cols;
-                for (int kb = 0; kb < num_kb; ++kb, ++step, cm.next(num_kb, S)) {
-                    const int s = cm.s;
-                    const unsigned phase = cm.phase;
-                    tmbar_wait(&s_ready[s], phase);               // transformed activations are in place
-                    tmbar_wait(&s_full[s], phase);                // (already complete: the transform waited on it)
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    unsigned char* st = tiles + (size_t)s * stage_bytes;
-                    const unsigned long long a_hi = tumma_desc(st), a_lo = tumma_desc(st + kTcABytes);
-                    const unsigned char* wb = p.w_resident ? w_res + (size_t)kb * 2 * w_bytes : st + w_off;
-                    const unsigned long long b_hi = tumma_desc(wb), b_lo = tumma_desc(wb + w_bytes);
-                    if (telect_one()) {
-#pragma unroll
-                        for (int k = 0; k < kTcKB / 8; ++k) {
-                            const unsigned long long off = (unsigned long long)(k * 2);
-                            tumma_tf32(tacc, a_hi + off, b_hi + off, idesc, (kb | k) != 0 ? 1u : 0u);
-                            tumma_tf32(tacc, a_lo + off, b_hi + off, idesc, 1u);
-                            tumma_tf32(tacc, a_hi + off, b_lo + off, idesc, 1u);
-                        }
-                        tumma_commit(&s_empty[s]);
-                        if (kb == num_kb - 1) tumma_commit(&s_acc_full[acc]);
-                        TC_MARK(step < 8, 16 + step);
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else if (warp < 10) {
-        // ===== transform: raw fp32 box -> GroupNorm affine + activation -> tf32 hi/lo operand tiles, in place =====
-        // Two groups of four warps take alternate k-blocks, so the load -> math -> store -> fence chain of one step
-        // overlaps the next step's; each group keeps its own copy of the per-sample GroupNorm table.
-        const int grp = (warp - 2) >> 2;
-        const int t = (threadIdx.x - 64) & 127;   // chunk c = t + 128*i, i < 8, of the 1024 16-byte chunks of a k-block
+    } else if (warp >= 8) {
+        // ===== transform + MMA: warpgroup grp owns rows [64 grp, 64 grp + 64) of every tile =====
+        // raw fp32 box -> GroupNorm affine + activation -> tf32 hi/lo operand tiles, in place; then the wgmma of this k-block
+        // run asynchronously while the next k-block is transformed.  Each group keeps its own copy of the per-sample
+        // GroupNorm table.
+        const int grp = (warp >> 2) - 2;
+        const int t = threadIdx.x & 127;   // chunk c = t + 128*i, i < 4, of the group's 512 16-byte chunks of a k-block
+        const int a_off = grp * 64 * 128;  // byte offset of the group's rows in an activation box (1024-aligned)
         float* g_scale = s_scale + grp * 2 * p.K;
         float* g_shift = g_scale + p.K;
         const ActCoef iact = act_coef(p.in_act, p.in_slope);
         TcCursor cp;
         const int tiles_per_sample = p.pts_per_sample / kTcM;
         int table_first = -1, table_end = -1;   // tile range [first, end) of the sample whose table this group holds
-        if (grp == 1) cp.next(num_kb, S);
-        for (int step = grp; step < total_steps; step += 2) {
-            const int kb = cp.kb, s = cp.s;
+        if (p.w_resident) tmbar_wait(&s_w_full, 0u);
+        float acc[64];
+        int prev_s = -1;
+        for (int ti = 0; ti < my_tiles; ++ti) {
+          for (int kb = 0; kb < num_kb; ++kb) {
+            const int s = cp.s;
             auto gn_table = [&]() {
                 const int tile = blockIdx.x + cp.ti * gridDim.x;
                 if (tile < table_first || tile >= table_end) {   // folded GroupNorm affine of every input channel of this sample
@@ -620,8 +557,8 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
             if (p.in_stats != nullptr && p.wait_on != nullptr) gn_table();
             unsigned char* st = tiles + (size_t)s * stage_bytes;
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int c = t + i * 128, r = c >> 3, lc = c & 7;
+            for (int i = 0; i < 4; ++i) {
+                const int c = t + i * 128, r = grp * 64 + (c >> 3), lc = c & 7;
                 // K-major SWIZZLE_128B: 16-byte chunk lc of row r lives at chunk (lc ^ (r & 7)) of the row's 128 bytes
                 const int off = r * 128 + ((lc ^ (r & 7)) << 4);
                 float4 x = *reinterpret_cast<const float4*>(st + off);
@@ -645,17 +582,39 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
                 *reinterpret_cast<float4*>(st + off) = hi;   // in place: raw -> hi; the lo half of the stage held the min array
                 *reinterpret_cast<float4*>(st + kTcABytes + off) = lo;
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the MMA (async proxy)
-            __syncwarp();
-            if (lane == 0) tmbar_arrive(&s_ready[s]);   // one arrival per warp of the group
-            TC_MARK(t == 0 && step < 8, 8 + step);
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma (async proxy)
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");   // the group's 64 rows are in place
+            TC_MARK(t == 0 && ti * num_kb + kb < 8, 8 + ti * num_kb + kb);
+            const unsigned char* wb = p.w_resident ? w_res + (size_t)kb * 2 * w_bytes : st + w_off;
+            wgmma_fence_regs(acc);
+            wgmma_fence();
+            tc_mma_kblock<NT>(acc, wgmma_desc(st + a_off), wgmma_desc(st + kTcABytes + a_off), wgmma_desc(wb), wgmma_desc(wb + w_bytes), kb);
+            wgmma_commit();
+            wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
+            if (prev_s >= 0 && lane == 0) tmbar_arrive(&s_empty[prev_s]);
+            prev_s = s;
             cp.next(num_kb, S);
-            cp.next(num_kb, S);
+          }
+          wgmma_wait<0>();
+          wgmma_fence_regs(acc);
+          if (lane == 0) tmbar_arrive(&s_empty[prev_s]);
+          prev_s = -1;
+          TC_MARK(t == 0 && ti < 8, 16 + ti);
+          tmbar_wait(&s_acc_empty, ((unsigned)ti & 1u) ^ 1u);   // the epilogue has consumed the previous tile
+          // accumulator fragment -> rows 64 grp + 16 (warp % 4) + lane / 4 (+8), columns 8 j + 2 (lane % 4) (+1)
+          float* a0 = s_acc + (size_t)(grp * 64 + (warp & 3) * 16 + (lane >> 2)) * acc_pitch + 2 * (lane & 3);
+#pragma unroll
+          for (int j = 0; j < NT / 8; ++j) {
+              *reinterpret_cast<float2*>(a0 + 8 * j) = make_float2(acc[4 * j + 0], acc[4 * j + 1]);
+              *reinterpret_cast<float2*>(a0 + (size_t)8 * acc_pitch + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          }
+          __syncwarp();
+          if (lane == 0) tmbar_arrive(&s_acc_full);
         }
     } else {
-        // ===== epilogue: TMEM -> registers -> global, one accumulator buffer behind the MMA =====
-        const int quad = warp & 3;          // a warp may only touch TMEM lanes 32*(warp%4) .. +31
-        const int half = (warp - 10) >> 2;  // two warps per lane quadrant: 32-column chunks c0 = 32*half, +64, ...
+        // ===== epilogue: accumulator tile -> registers -> global, one tile behind the MMA =====
+        const int quad = warp & 3;   // rows 32 quad .. +31 of the tile
+        const int half = warp >> 2;  // two warps per quadrant: 32-column chunks c0 = 32*half, +64, ...
         // Completion signal of a tile (p.done: one release-add per epilogue warp and tile).  The release has to wait for the
         // warp's outstanding stores, ~1 us if issued right behind them -- exposed, because this warp is alone on its
         // scheduler.  So the signal of tile i is sent when the accumulator of tile i+1 arrives (its stores have long
@@ -663,30 +622,20 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
         // this SM before this CTA exits, and samples that complete in an earlier round are not needed sooner.
         int unsignalled = -1;
         for (int ti = 0; ti < my_tiles; ++ti) {
-            const int acc = ti & 1;
-            const unsigned acc_phase = (unsigned)(ti >> 1) & 1u;
             const int row0 = (blockIdx.x + ti * gridDim.x) * kTcM;
-            tmbar_wait(&s_acc_full[acc], acc_phase);
+            tmbar_wait(&s_acc_full, (unsigned)ti & 1u);
             if (unsignalled >= 0 && lane == 0) red_release_gpu(p.done + unsignalled);
-            TC_MARK(threadIdx.x == 320 && ti < 4, 24 + ti);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            TC_MARK(threadIdx.x == 0 && ti < 4, 24 + ti);
             const int sample = row0 / p.pts_per_sample;
-            tc_epilogue(p, tmem + (unsigned)acc * acc_cols, quad, half, lane, row0, sample, s_bias, s_estage, s_part);
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+            tc_epilogue(p, s_acc, acc_pitch, quad, half, lane, row0, sample, s_bias, s_estage, s_part);
             __syncwarp();   // (also orders every lane's stores of this tile before lane 0's later release)
-            if (lane == 0) tmbar_arrive(&s_acc_empty[acc]);   // one arrival per epilogue warp
+            if (lane == 0) tmbar_arrive(&s_acc_empty);   // one arrival per epilogue warp
             if (p.done != nullptr) unsignalled = sample;
-            TC_MARK(threadIdx.x == 320 && ti < 4, 28 + ti);
+            TC_MARK(threadIdx.x == 0 && ti < 4, 28 + ti);
         }
         if (unsignalled >= 0 && lane == 0) red_release_gpu(p.done + unsignalled);
     }
-    __syncwarp();   // the producer / MMA roles run on one lane: re-converge those warps before the CTA-wide barrier
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols) : "memory");
-    }
-    TC_MARK(threadIdx.x == 64, 1);
+    TC_MARK(threadIdx.x == 256, 1);
 }
 
 // hi = tf32(w), lo = tf32(w - hi) of a [rows, ld] weight window [rows, cols] written as [rows_pad, cols_pad] (zero padded)
@@ -797,7 +746,8 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     if ((rc = tc_make_map(&mmin, a->in_min ? a->in_min : a->in[0], M, a->in_channels[0], a->in_channels[0], kTcM))) return rc;
     const size_t a_stage = (size_t)2 * kTcABytes;
     const size_t w_all = (size_t)(K / kTcKB) * 2 * a->n_pad * kTcKB * 4;          // hi + lo of the whole weight matrix
-    const size_t fixed = (size_t)(4 * K + 2 * a->n_pad + (a->epilogue == TC_EPI_PLAIN ? 8 * 32 * 36 : (a->epilogue == TC_EPI_FLOW ? 0 : 8 * 32 * 20)) + 4 * 128 * 2) * sizeof(float) + 1024 + 64;
+    const bool gru = a->epilogue == TC_EPI_GRU_ZR || a->epilogue == TC_EPI_GRU_Q;
+    const size_t fixed = (size_t)(4 * K + 2 * a->n_pad + kTcM * tc_acc_pitch(a->n_pad) + (gru ? 8 * 32 * kTcPitch16 : 0) + 4 * 128 * 2) * sizeof(float) + 1024 + 64;
     const size_t budget = (size_t)kSmemBudget - 2048 /* static barriers */ - fixed;
     // Weights stay resident in shared memory when that still leaves a ring of >= 3 activation stages (re-streaming the
     // same few KB per tile from every SM hot-spots a handful of L2 slices); otherwise they travel with the k-blocks.
@@ -814,7 +764,18 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     p.stages = stages;
     if (const char* e = getenv("PVRAFT_TC_DBG")) p.dbg = atoi(e);
     const size_t smem = stages * stage + (p.w_resident ? w_all : 0) + fixed;
-    if ((rc = opt_in_smem(k_tc_linear, smem))) return rc;
+    decltype(&k_tc_linear<16>) kernel = nullptr;
+    switch (a->n_pad) {
+        case 16: kernel = k_tc_linear<16>; break;
+        case 32: kernel = k_tc_linear<32>; break;
+        case 48: kernel = k_tc_linear<48>; break;
+        case 64: kernel = k_tc_linear<64>; break;
+        case 80: kernel = k_tc_linear<80>; break;
+        case 96: kernel = k_tc_linear<96>; break;
+        case 112: kernel = k_tc_linear<112>; break;
+        default: kernel = k_tc_linear<128>; break;
+    }
+    if ((rc = opt_in_smem(kernel, smem))) return rc;
     const long long n_tiles = (M + kTcM - 1) / kTcM;
     const int grid = (int)(n_tiles < sm_count() ? n_tiles : sm_count());
     // launched with programmatic stream serialization: the kernel's prologue may start while the previous kernel drains
@@ -831,7 +792,7 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    const cudaError_t le = cudaLaunchKernelEx(&cfg, k_tc_linear, mw_hi, mw_lo, ma[0], ma[1], ma[2], mmin, p);
+    const cudaError_t le = cudaLaunchKernelEx(&cfg, kernel, mw_hi, mw_lo, ma[0], ma[1], ma[2], mmin, p);
     if (le != cudaSuccess) return fail((int)le, "tc_linear: launch failed: %s", cudaGetErrorString(le));
     return check_launch("tc_linear");
 }

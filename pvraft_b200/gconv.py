@@ -1,5 +1,5 @@
 """SetConv -- mirror of the reference module (model/flot/gconv.py:4-85), same parameters and
-state_dict keys (fc1/gn1/fc2/gn2/fc3/gn3), forward on the B200 kernels."""
+state_dict keys (fc1/gn1/fc2/gn2/fc3/gn3), forward on the H100 kernels."""
 import torch
 
 from . import ops
@@ -36,7 +36,7 @@ class SetConv(torch.nn.Module):
 
     def forward_deferred(self, signal, graph):
         """signal: [B,N,cin] tensor or a Deferred from the previous SetConv -> Deferred.
-        Layers whose shapes fit the tensor-core kernel (N % 128 == 0, K % 32 == 0) run on tcgen05 (3xTF32),
+        Layers whose shapes fit the tensor-core kernel (N % 128 == 0, K % 32 == 0) run on wgmma (3xTF32),
         the others on the CUDA-core kernel; both are fp32-accurate."""
         cin, mid, cout = self.nb_feat_in, self.mid, self.nb_feat_out
         deferred = isinstance(signal, Deferred)

@@ -41,7 +41,7 @@ class Graph:
     def construct_graph(pcloud, nb_neighbors):
         b, n, _ = pcloud.shape
         if nb_neighbors != ops.KNN:
-            raise NotImplementedError('the B200 SetConv kernels are built for 32 neighbours (the only value the '
+            raise NotImplementedError('the SetConv kernels are built for 32 neighbours (the only value the '
                                       'reference uses, model/extractor.py:9)')
         if n < nb_neighbors:
             raise ValueError(f'need at least {nb_neighbors} points per cloud, got {n}')

@@ -114,7 +114,7 @@ def corr_state_pack_bf16(val, idx):
 
 
 def corr_matmul(fmap1_pm, fmap2_pm):
-    """Point-major feature maps [B,N,C] -> all-pairs correlation [B,N,N] / sqrt(C) on tcgen05 (3xTF32)."""
+    """Point-major feature maps [B,N,C] -> all-pairs correlation [B,N,N] / sqrt(C) on wgmma (3xTF32)."""
     b, n, c = fmap1_pm.shape
     corr = torch.empty(b, n, n, dtype=torch.float32, device=fmap1_pm.device)
     ws = torch.empty(int(lib().pvraft_corr_matmul_workspace_bytes(b, n, c)), dtype=torch.uint8, device=fmap1_pm.device)
@@ -284,7 +284,7 @@ def morton_order(points):
 
 
 def tc_supported(n_points, *channels):
-    """The tcgen05 layer needs 128-point tiles that do not straddle samples and 32-channel k-blocks."""
+    """The tensor-core layer needs 128-point tiles that do not straddle samples and 32-channel k-blocks."""
     return n_points % 128 == 0 and all(c % 32 == 0 for c in channels)
 
 
@@ -292,7 +292,7 @@ def tc_linear(sources, w, bias=None, *, in_min=None, in_stats=None, in_gamma=Non
               in_act=ACT_NONE, in_slope=0.0, out_act=ACT_NONE, residual=None, out=None, out_stats=None, epilogue=TC_PLAIN,
               bias2=None, out2=None, h=None, z=None, cout=None, tail=None, w3=None, b3=None, coords1=None, coords2=None,
               coords2_out=None, flow_out=None, flow_user=None, row_map=None, chain=False):
-    """Fused layer on the tcgen05 tensor cores.  sources: list of [B,N,C_i] tensors concatenated along K (the
+    """Fused layer on the Hopper tensor cores (wgmma).  sources: list of [B,N,C_i] tensors concatenated along K (the
     GroupNorm prologue applies to sources[0]); w = (hi, lo, n_pad, rows) from tc_weights(); tail [B,N,3] fills the
     output columns cout..cout+2.
     chain=True: the caller states that everything this layer reads was produced by the tensor-core launch issued

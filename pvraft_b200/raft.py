@@ -143,7 +143,7 @@ class _RaftBase(nn.Module):
             offs = (torch.arange(xyz1.shape[0], device=xyz1.device) * xyz1.shape[1]).view(-1, 1)
             self._row_map = (perm + offs).to(torch.int32).reshape(-1).contiguous()   # row of permuted point r in the input order
         # both clouds go through the shared feature encoder as one batch of 2B samples (RAFTSceneFlow.py:25-26: every op is
-        # per sample): half the launches, and 2B*N/128 tiles fill the 148 SMs more evenly
+        # per sample): half the launches, and 2B*N/128 tiles fill the 132 SMs more evenly
         b = xyz1.shape[0]
         both = torch.cat([xyz1, xyz2], 0)
         fmap, graph2 = self.feature_extractor(both, point_major=True)

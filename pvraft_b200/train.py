@@ -10,7 +10,7 @@ The forward runs layer by layer -- the fused inference kernels keep no activatio
     GnActMaxFn      ... + max over 32 rows    pvraft_gn_act_maxk_fwd / pvraft_gn_act_bwd (arg form: no dense max gradient)
     EdgeFn          SetConv edge stage        pvraft_edge_fwd / pvraft_edge_bwd          (model/flot/gconv.py:65-73)
     MaxKFn          max over 32 neighbours    pvraft_maxk_fwd / pvraft_maxk_bwd          (gconv.py:80, model/corr.py:92)
-    CorrInitFn      truncated correlation     tcgen05 GEMM + top-k + reorder / pvraft_corr_init_bwd (sparse)   (corr.py:31-42,95-100)
+    CorrInitFn      truncated correlation     wgmma GEMM + top-k + reorder / pvraft_corr_init_bwd (sparse)   (corr.py:31-42,95-100)
     CorrLookupFn    voxel means + kNN gather  pvraft_corr_lookup_fwd / pvraft_corr_lookup_bwd                  (corr.py:47-66,75-91)
 
 PyTorch is the tape (which Function follows which) and the allocator; the glue between Functions that the reference also
@@ -32,7 +32,7 @@ def _zeros64(*shape, device):
     return torch.zeros(*shape, dtype=torch.float64, device=device)
 
 
-# Per-point layers of the training path on the tcgen05 kernel: 'auto' = while the step is being captured into a CUDA graph
+# Per-point layers of the training path on the wgmma kernel: 'auto' = while the step is being captured into a CUDA graph
 # (26.9 vs 30.0 ms per step); with eager launches the host cost of the tensor-core launch path (tensor-map encodes, the weight
 # splits after every optimizer step) outweighs the faster kernels (40.5 vs 33.0 ms), so there the CUDA-core kernels stay.
 _TC_TRAIN = os.environ.get('PVRAFT_TC_TRAIN', 'auto')
@@ -52,7 +52,7 @@ class LinearFn(torch.autograd.Function):
         x = x.contiguous()
         stats = _zeros64(x.shape[0], 8, 2, device=x.device) if want_stats else None
         cout, cin = w2.shape
-        # per-point layers whose shapes fit go to the tcgen05 kernel (3xTF32: fp32-accurate), forward and dx; the weight is
+        # per-point layers whose shapes fit go to the wgmma kernel (3xTF32: fp32-accurate), forward and dx; the weight is
         # split once per parameter version, i.e. once per optimizer step however many iterations use the layer
         ctx.tc = _tc_train() and x.dim() == 3 and ops.tc_supported(x.shape[1], cin) and cout <= 128 and (not want_stats or cout % 32 == 0)
         ctx.w_ref = w

@@ -1,5 +1,5 @@
 """UpdateBlock = MotionEncoder + ConvGRU + FlowHead -- mirrors of model/update.py:8-87 with the same
-parameters / state_dict keys; forward passes run on the B200 kernels.
+parameters / state_dict keys; forward passes run on the H100 kernels.
 
 Layouts: the module-level `forward` methods take and return the reference's channel-major [B,C,N]
 tensors (drop-in seam); the `*_pm` methods work on point-major [B,N,C] buffers and are what the
@@ -69,7 +69,7 @@ class ConvGRU(nn.Module):
         if out is None:
             out = torch.empty_like(net)
         if ops.tc_supported(n):
-            # tcgen05: [z|r] = sigmoid(W_zr [h,x]); q = tanh(W_q [r*h, x]); h' = (1-z) h + z q   (update.py:32-39)
+            # wgmma: [z|r] = sigmoid(W_zr [h,x]); q = tanh(W_q [r*h, x]); h' = (1-z) h + z q   (update.py:32-39)
             z, rh = torch.empty_like(net), torch.empty_like(net)
             ops.tc_linear([net, inp, motion], ops.tc_weights((self.convz.weight, self.convr.weight)), _w(self.convz.bias),
                           bias2=_w(self.convr.bias), epilogue=ops.TC_GRU_ZR, out=z, out2=rh, h=net, cout=64, chain=True)
@@ -122,7 +122,7 @@ class FlowHead(nn.Module):
         delta = torch.empty(b, n, 3, dtype=torch.float32, device=net.device)
         oc = self.out_conv
         if ops.tc_supported(n):
-            # tcgen05, one launch: out_conv.0 on [setconv(x), conv1(x)] (update.py:68-71) is linear in x through conv1, so
+            # wgmma, one launch: out_conv.0 on [setconv(x), conv1(x)] (update.py:68-71) is linear in x through conv1, so
             # conv1 is folded into the second half of its weight: W [a3 | W_b W_c1] with bias W_b b_c1 + b_o0 (products in
             # float64, rounded once).  Prologue: a3 = lrelu(GN3(z3)); epilogue: ReLU, out_conv.2 and the RAFT update
             # (update.py:72, RAFTSceneFlow.py:45-46).

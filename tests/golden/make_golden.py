@@ -1,9 +1,9 @@
-"""Generate golden vectors by running the UNMODIFIED reference (mounted read-only at
-/root/reference) on CPU in the build container.  The reference cannot travel to the GPU box,
+"""Generate golden vectors by running the UNMODIFIED reference (read-only; its tree is given by
+PVRAFT_REFERENCE) on CPU.  The tests must not depend on the reference tree being present,
 so the vectors are committed next to this script (tests/golden/*.npz) and this script is the
 record of how they were made.
 
-    python tests/golden/make_golden.py            # rewrites tests/golden/*.npz
+    PVRAFT_REFERENCE=<reference tree> python tests/golden/make_golden.py   # rewrites tests/golden/*.npz
 
 The only thing added to the reference is a shim for its one absent third-party import,
 `torch_scatter.scatter_add` (model/corr.py:50), with torch-scatter's documented semantics
@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = os.environ.get('PVRAFT_REFERENCE', '/root/reference')
+REF = os.environ.get('PVRAFT_REFERENCE')
 
 
 def install_scatter_shim():
@@ -109,6 +109,8 @@ def trace_forward(model, pc1, pc2, iters):
 
 
 def main():
+    if not REF or not os.path.isdir(REF):
+        sys.exit('set PVRAFT_REFERENCE to the reference tree (weiyithu/PV-RAFT)')
     install_scatter_shim()
     sys.path.insert(0, REF)
     from model.RAFTSceneFlow import RSF
@@ -171,6 +173,19 @@ def main():
     idx = knn_point(16, xyz, q)
     np.savez_compressed(os.path.join(HERE, 'knn_point.npz'), xyz=xyz.numpy(), query=q.numpy(),
                         idx=np.sort(idx.numpy(), axis=-1).astype(np.int32))
+    # ---- fixture 5: Batch collation (datasets/generic.py:6-28) of three seeded items ----------
+    #      (loaded by file path: the HuggingFace `datasets` package shadows the reference's namespace package)
+    import importlib.util
+    spec = importlib.util.spec_from_file_location('ref_generic', os.path.join(REF, 'datasets', 'generic.py'))
+    generic = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(generic)
+    g = torch.Generator().manual_seed(0)
+    items = [{'sequence': [torch.rand(1, 50, 3, generator=g), torch.rand(1, 50, 3, generator=g)],
+              'ground_truth': [(torch.rand(1, 50, 1, generator=g) > 0.2).float(), torch.randn(1, 50, 3, generator=g)]}
+             for _ in range(3)]
+    data = generic.Batch(items).data
+    np.savez_compressed(os.path.join(HERE, 'batch_collate.npz'),
+                        **{f'{k}/{i}': data[k][i].numpy() for k in ('sequence', 'ground_truth') for i in range(2)})
     for f in sorted(os.listdir(HERE)):
         if f.endswith('.npz'):
             print(f, os.path.getsize(os.path.join(HERE, f)) // 1024, 'KiB')

@@ -95,7 +95,7 @@ def config2(dev):
 
 
 def test_config2_teacher_forced_loop_path(dev, config2):
-    """The loop's own kernels (feature_motion_tc, UpdateBlock.forward_pm: lookup with per-sample dynamic claims, tcgen05
+    """The loop's own kernels (feature_motion_tc, UpdateBlock.forward_pm: lookup with per-sample dynamic claims, wgmma
     layers, SetConv edge kernel) on oracle-produced state, iteration by iteration."""
     c = config2
     m, b = c['m'], c['b']
@@ -133,7 +133,7 @@ def test_config2_teacher_forced_loop_path(dev, config2):
 
 
 def test_config2_build_matches_oracle_state(dev, config2):
-    """Pre-loop path at N=8192: encoders (2B-batched), tcgen05 correlation GEMM, top-512 -- candidate SETS equal to the
+    """Pre-loop path at N=8192: encoders (2B-batched), wgmma correlation GEMM, top-512 -- candidate SETS equal to the
     oracle's except at near-ties of the 512th value (3xTF32 vs fp32 summation order), values and context features 1e-5;
     the kNN adjacency differs from the oracle's argsort only where the 32nd distance ties exactly."""
     c = config2
@@ -218,7 +218,7 @@ def test_free_running_32_iterations(dev):
 @pytest.mark.parametrize('n,k', [(300, 128), (1000, 256)])
 def test_ragged_point_count_model_level(dev, n, k):
     """N % 128 != 0 (`--max_points` is a free flag, train.py:8-71): the CUDA-core kernels (k_corrfeat + motion stage,
-    k_gru, k_flowout, k_linear) carry the loop and the padded tcgen05 GEMM builds the correlation; teacher-forced
+    k_gru, k_flowout, k_linear) carry the loop and the padded wgmma GEMM builds the correlation; teacher-forced
     module seams and free-running flows against the oracle."""
     b, iters = 2, 3
     args = types.SimpleNamespace(corr_levels=LEVELS, base_scales=SCALE, truncate_k=k)
@@ -244,7 +244,7 @@ def test_ragged_point_count_model_level(dev, n, k):
             assert rel_err(net2.cpu(), t['net']) < 1e-5
             assert rel_err(delta.cpu(), t['delta']) < 5e-5
             net = t['net'].to(dev)
-        # the correlation build of a ragged N (tcgen05 GEMM on zero-padded feature maps, no library GEMM)
+        # the correlation build of a ragged N (wgmma GEMM on zero-padded feature maps, no library GEMM)
         m._encode([pc1.to(dev), pc2.to(dev)])
         assert rel_err(m.corr_block.truncated_corr.cpu(), li.state.truncated_corr) < 1e-5
 
@@ -273,7 +273,7 @@ def test_chained_tensor_core_launches_equal_grid_wide_waits(dev):
     counters of the launch before them instead of waiting for its whole grid (ops.tc_linear(chain=True)): scheduling only.  The flows must equal those of
     the same launches with grid-wide waits up to the order of the double-precision GroupNorm partial sums (the bound of the
     batch-of-8 test) -- a stale or early read would show at 1e-2.  Eager launches and CUDA-graph replay, several repeats,
-    a batch large enough (4 x 64 tiles over 148 SMs) for CTAs to run ahead of the previous launch's last tiles."""
+    a batch large enough (4 x 64 tiles over 132 SMs) for CTAs to run ahead of the previous launch's last tiles."""
     from pvraft_b200 import ops
     m, _ = make_model(dev)
     b, iters = 4, 12

@@ -323,7 +323,7 @@ def test_modules_teacher_forced_vs_reference(dev, fixture, refine):
     g = golden_graph(arr, dev)
     iters = int(arr['meta'][4])
     inp = torch.relu(arr['fct1'][:, 64:]).to(dev)
-    # tanh through float64: on the GPU box the fp32 CPU tanh was seen (about 1 process in 40) to return one 2048-element
+    # tanh through float64: on a GPU test machine the fp32 CPU tanh was seen (about 1 process in 40) to return one 2048-element
     # block that is 5e-5 off, which then shows up as a 'kernel' mismatch in net; the upload is verified as well
     net_cpu = torch.tanh(arr['fct1'][:, :64].double()).float()
     net = net_cpu.to(dev)
@@ -420,8 +420,8 @@ def test_rsf_default_init_medium(dev):
 
 
 @pytest.mark.parametrize('b,n,c', [(1, 128, 32), (2, 256, 128), (1, 1024, 128), (1, 384, 64)])
-def test_corr_matmul_tcgen05(dev, b, n, c):
-    """calculate_corr on tcgen05 with the 3xTF32 split: fp32-level agreement with an fp64 product."""
+def test_corr_matmul_wgmma(dev, b, n, c):
+    """calculate_corr on the tensor cores (wgmma) with the 3xTF32 split: fp32-level agreement with an fp64 product."""
     from pvraft_b200 import ops
     g = torch.Generator().manual_seed(n + c)
     f1 = torch.randn(b, n, c, generator=g) * 2.0
@@ -438,7 +438,7 @@ def test_corr_matmul_tcgen05(dev, b, n, c):
 @pytest.mark.parametrize('b,n,cin,cout,mode', [(2, 256, 64, 64, 'plain'), (1, 1024, 96, 128, 'gn'), (2, 128, 64, 64, 'minmax'),
                                                (1, 256, 32, 48, 'plain'), (1, 384, 128, 3, 'gn')])
 def test_tc_linear_matches_fp64(dev, b, n, cin, cout, mode):
-    """tcgen05 3xTF32 layer (prologue + epilogue) against an fp64 evaluation and against the CUDA-core kernel."""
+    """wgmma 3xTF32 layer (prologue + epilogue) against an fp64 evaluation and against the CUDA-core kernel."""
     from pvraft_b200 import ops
     g = torch.Generator().manual_seed(cin * 7 + cout)
     x = torch.randn(b, n, cin, generator=g) * 1.5 + 0.2

@@ -75,7 +75,7 @@ def test_linear_fn(dev, b, r, cin, cout, bias):
 @pytest.mark.parametrize('b,r,cin,cout,bias,stats', [(2, 1024, 192, 64, True, True), (1, 2048, 64, 96, False, True),
                                                      (2, 512, 128, 61, True, False), (1, 256, 32, 128, True, True)])
 def test_linear_fn_on_tensor_cores(dev, b, r, cin, cout, bias, stats):
-    """The per-point layers of a CAPTURED training step run on the tcgen05 kernel (3xTF32), forward and dx (PVRAFT_TC_TRAIN=auto;
+    """The per-point layers of a CAPTURED training step run on the wgmma kernel (3xTF32), forward and dx (PVRAFT_TC_TRAIN=auto;
     forced here): same Function, same bounds as the CUDA-core path."""
     from pvraft_b200 import ops, train as T
     g = torch.Generator().manual_seed(cin * 7 + cout)
@@ -367,7 +367,7 @@ def test_training_steps_like_the_engine(dev):
 
 
 def test_whole_model_gradients_with_tensor_core_layers(dev):
-    """The same training step with the per-point layers on the tcgen05 kernel (what a captured step runs) and on the CUDA-core
+    """The same training step with the per-point layers on the wgmma kernel (what a captured step runs) and on the CUDA-core
     kernels: all 95 gradients agree (both are fp32-accurate; N = 1024 so that the tensor-core shapes apply)."""
     from pvraft_b200 import RSF, train as T
     args = types.SimpleNamespace(corr_levels=3, base_scales=0.25, truncate_k=128)

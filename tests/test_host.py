@@ -260,20 +260,13 @@ def _items(b, n, seed=0):
 
 
 def test_batch_collate_matches_the_reference_class():
-    """pvraft_b200.data.Batch against datasets/generic.py:6-66 (the reference class itself when its tree is present, loaded by
-    file path because the HuggingFace `datasets` package shadows the namespace package; its documented behaviour otherwise)."""
+    """pvraft_b200.data.Batch against datasets/generic.py:6-66: the reference class's output for the same seeded items
+    (tests/golden/batch_collate.npz, tests/golden/make_golden.py fixture 5)."""
     from pvraft_b200.data import Batch, subsample
     items = _items(3, 50)
     mine = Batch(items)
-    ref_path = '/root/reference/datasets/generic.py'
-    if os.path.exists(ref_path):
-        import importlib.util
-        spec = importlib.util.spec_from_file_location('ref_generic', ref_path)
-        mod = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(mod)
-        ref = mod.Batch(items).data
-    else:
-        ref = {k: [torch.cat([it[k][i] for it in items], 0) for i in range(2)] for k in ('sequence', 'ground_truth')}
+    arr, _ = load_golden('batch_collate.npz')
+    ref = {k: [arr[f'{k}/{i}'] for i in range(2)] for k in ('sequence', 'ground_truth')}
     for key in ('sequence', 'ground_truth'):
         for a, b in zip(mine[key], ref[key]):
             assert a.shape == b.shape and torch.equal(a, b)

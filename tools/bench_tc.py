@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 fused layer: python tools/bench_tc.py"""
+"""Micro-benchmark of the wgmma fused layer: python tools/bench_tc.py"""
 import os, sys, json
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
