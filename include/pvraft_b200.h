@@ -215,18 +215,9 @@ typedef struct pvraft_tc_linear_args {
     const float* coords2;   /* FLOW: [B,N,3] or NULL */
     float* coords2_out;     /* FLOW: [B,N,3] or NULL (may alias coords2) */
     float* flow_out;        /* FLOW: [B,N,3] or NULL */
-    float* flow_user;       /* FLOW: second copy of the flow, row r written at row row_map[r] ([B*N,3]) -- the caller's
-                               point order when the cloud was spatially reordered for locality -- or NULL */
-    const int32_t* row_map; /* FLOW: [B*N] destination rows of flow_user */
     int params_settled;     /* nonzero: w_hi, w_lo, bias, bias2, w3, b3 were last written at least three launches ago on this
                                stream (or before a synchronisation).  The kernel is launched with programmatic stream
                                serialization and then fetches them while the previous kernel drains.  0 is always safe. */
-    int32_t* done;          /* [B] zero-initialised counters or NULL: every finished 128-point tile adds 8 to its sample's entry
-                               (release), after its rows and GroupNorm sums are written */
-    const int32_t* wait_on; /* NULL, or the `done` array of the launch IMMEDIATELY BEFORE this one on the stream, which produced
-                               this layer's inputs: the kernel then starts on a sample as soon as that launch has finished it
-                               (acquire on its counter) instead of waiting for the whole grid.  Needs params_settled; outputs must
-                               not alias anything the previous launch reads.  Ignored (full wait) otherwise. */
 } pvraft_tc_linear_args;
 
 PVRAFT_API int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream);

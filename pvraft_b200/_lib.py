@@ -35,7 +35,7 @@ class TcLinearArgs(C.Structure):
                 ('w_lo', VP), ('n_pad', C.c_int), ('cout', C.c_int), ('bias', VP), ('bias2', VP), ('out_act', C.c_int),
                 ('residual', VP), ('out', VP), ('out2', VP), ('h', VP), ('z', VP), ('out_stats', VP), ('epilogue', C.c_int),
                 ('B', C.c_int), ('N', C.c_int), ('tail', VP), ('w3', VP), ('b3', VP), ('coords1', VP), ('coords2', VP),
-                ('coords2_out', VP), ('flow_out', VP), ('flow_user', VP), ('row_map', VP), ('params_settled', C.c_int), ('done', VP), ('wait_on', VP)]
+                ('coords2_out', VP), ('flow_out', VP), ('params_settled', C.c_int)]
 
 
 class KnnBranchArgs(C.Structure):

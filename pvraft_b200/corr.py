@@ -219,7 +219,7 @@ class CorrBlock(nn.Module):
                                         self.knn_out.bias), 'corr_cc', fold_corr_motion)
             corr = None
             cc = ops.tc_linear([y1, kfeat], ops.tc_weights(w_eff), b_eff, out_act=ACT_RELU, **gn)
-        motion = ops.tc_linear([cc, cflow], ops.tc_weights(me.conv.weight), _w(me.conv.bias), out_act=ACT_RELU, tail=flow, chain=True)
+        motion = ops.tc_linear([cc, cflow], ops.tc_weights(me.conv.weight), _w(me.conv.bias), out_act=ACT_RELU, tail=flow)
         return corr, motion
 
     def __call__(self, coords):

@@ -110,12 +110,11 @@ __host__ __device__ __forceinline__ void split_range(long long total, int parts,
 
 // Launch with programmatic stream serialization (PDL): the grid may be scheduled while the previous kernel of the stream
 // drains.  The kernel MUST execute pdl_wait() before its first global access (and may call pdl_trigger() at entry so that
-// its own successor can be staged early).  PVRAFT_PDL=0 turns the attribute off.
+// its own successor can be staged early).
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t stream, Args... args) {
-    static const bool on = []() { const char* e = getenv("PVRAFT_PDL"); return !(e && atoi(e) == 0); }();
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)grid);
     cfg.blockDim = dim3((unsigned)block);
@@ -123,7 +122,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), int grid, int block, siz
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = on ? 1 : 0;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);

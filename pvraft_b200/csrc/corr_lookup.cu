@@ -634,7 +634,6 @@ static int launch_lookup(LookupParams& p, cudaStream_t st) {
     if (warps < 1) return fail(PVRAFT_ERR_SMEM, "corr_lookup: K=%d does not fit shared memory", K);
     p.warps = warps;
     p.chunk = 2;   // in-situ sweep at B=8, N=8192 (v8 kernel): 1 -> 108.4 us, 2 -> 102.6, 3 -> 103.3, 4 -> 103.8, 6 -> 105.0, 8 -> 105.3
-    if (const char* e = getenv("PVRAFT_LOOKUP_CHUNK")) { const int v = atoi(e); if (v >= 1 && v <= 64) p.chunk = v; }
     const size_t rcp = (size_t)(K + 1) * sizeof(double) + 8;
     const size_t smem = (smem_tab ? tab : 0) + warps * per_warp + rcp;
     const long long total = (long long)p.B * p.N;

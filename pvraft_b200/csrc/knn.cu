@@ -13,8 +13,6 @@
 // Distances reproduce the reference's expanded form bit-for-bit on the CPU oracle: |q|^2 and |x|^2 as
 // (x*x+y*y)+z*z, q.x as fma(z,z',fma(y,y',x*x')); ranking is on (distance, original id), so the result does not
 // depend on the visiting order.  Clouds too large for the shared-memory sort fall back to the brute-force kernel.
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace pvraft {
@@ -347,9 +345,7 @@ extern "C" int pvraft_knn_fwd(const float* xyz, const float* query, int B, int N
         const size_t smem = (size_t)NP * sizeof(unsigned long long);
         int rc;
         if ((rc = opt_in_smem(k_grid_sort, smem))) return rc;
-        float occ = kCellOcc;
-        if (const char* e = getenv("PVRAFT_KNN_OCC")) { const float v = (float)atof(e); if (v > 0.f) occ = v; }
-        k_grid_sort<<<B, 1024, smem, st>>>(xyz, N, NP, occ, 0, params, sorted, ids, keys);
+        k_grid_sort<<<B, 1024, smem, st>>>(xyz, N, NP, kCellOcc, 0, params, sorted, ids, keys);
         if ((rc = check_launch("knn grid sort"))) return rc;
         k_grid_cells<<<dim3((kMaxCells + 1 + 255) / 256, B), 256, 0, st>>>(keys, N, cell_start);
         if ((rc = check_launch("knn grid cells"))) return rc;

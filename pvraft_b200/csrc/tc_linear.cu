@@ -72,17 +72,12 @@ struct TcParams {
     int stages;               // depth of the shared-memory ring (1..4)
     int w_resident;           // 1: all weight boxes are loaded once per CTA and stay in shared memory
     int settled;              // 1: weights / biases may be read before griddepcontrol.wait
-    int* done;                // [B] or null: every epilogue warp adds 1 per finished tile of the sample (release)
-    const int* wait_on;       // [B] or null: the `done` counters of the previous launch, which produced this layer's inputs.
-                              // Non-null: the grid-wide dependency wait is replaced by per-sample waits in the TMA producer
-    unsigned wait_target;     // 8 * tiles per sample
     int dbg;                  // 1: CTA 0 records a globaltimer timeline into g_tc_clock
     int gn_kb;                // k-blocks (from the start: source 0) that go through the GroupNorm prologue
     int out_ld;               // row stride of `out` in floats (cout, or cout + 3 with a tail)
     const float* tail;        // [M,3] copied into output columns cout..cout+2, or nullptr
     const float *w3, *b3, *coords1, *coords2;   // FLOW epilogue
-    float *coords2_out, *flow_out, *flow_user;
-    const int32_t* row_map;
+    float *coords2_out, *flow_out;
 };
 
 __device__ __forceinline__ unsigned tsu32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -142,8 +137,8 @@ __device__ __forceinline__ void stage_store16(float* __restrict__ stg, int lane,
 }
 // the inverse: a [32 rows x 16 columns] block of a row-major global tensor, loaded as 8 rows x 64 B per instruction and handed
 // to the thread that owns each row (thread-per-row loads would touch 32 sectors per instruction)
-// COHERENT: the operand may have been written by the previous launch while this one was already running (chained launches):
-// ld.global.cg (L2) instead of the non-coherent path.
+// COHERENT: the operand is written by the previous launch, which may still run when this one starts (programmatic dependent
+// launch), so it is not read-only over this kernel's lifetime: ld.global.cg (L2) instead of the non-coherent path.
 template <bool COHERENT = false>
 __device__ __forceinline__ void stage_load16(float* __restrict__ stg, int lane, const float* gbase, int ld, float (&x)[16]) {
     const int rsub = lane >> 2, cq = lane & 3;
@@ -162,14 +157,6 @@ __device__ __forceinline__ void stage_load16(float* __restrict__ stg, int lane, 
         const float4 v = *reinterpret_cast<const float4*>(stg + lane * kTcPitch16 + q * 4);
         x[q * 4 + 0] = v.x; x[q * 4 + 1] = v.y; x[q * 4 + 2] = v.z; x[q * 4 + 3] = v.w;
     }
-}
-__device__ __forceinline__ unsigned ld_acquire_gpu(const int* p) {
-    unsigned v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void red_release_gpu(int* p) {
-    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p) : "memory");
 }
 __device__ __forceinline__ float tsigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 
@@ -336,7 +323,6 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, float* __restrict
                     if (p.flow_out != nullptr) {
                         const float fl = c2 - __ldg(p.coords1 + g);   // RAFTSceneFlow.py:46
                         p.flow_out[g] = fl;
-                        if (p.flow_user != nullptr) p.flow_user[(size_t)__ldg(p.row_map + row) * 3 + k] = fl;
                     }
                 }
             }
@@ -471,11 +457,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
         if (warp == kTcProducerWarp && lane == 0 && p.w_resident) load_weights();
         if (warp < 8) load_bias();
     }
-    // Chained on the previous launch (p.wait_on): no grid-wide wait -- the TMA producer waits per sample on that launch's
-    // `done` counters instead, so this CTA starts on the tiles whose inputs are complete while the stragglers of the
-    // previous launch still run on other SMs.  Everything else this kernel reads is older than the previous launch,
-    // which itself only signals after its own dependencies resolved.
-    if (p.wait_on == nullptr) asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.wait;" ::: "memory");
     if (!p.settled && warp < 8) load_bias();
     __syncthreads();
 
@@ -485,18 +467,9 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
             if (p.w_resident && !p.settled) load_weights();
             const unsigned tx = (unsigned)(kTcABytes * (p.minmax ? 2 : 1) + (p.w_resident ? 0 : 2 * w_bytes));
             TcCursor cw;
-            int ready_sample = -1;
             for (int step = 0; step < total_steps; ++step, cw.next(num_kb, S)) {
                 const int s = cw.s, kb = cw.kb;
                 const int row0 = (blockIdx.x + cw.ti * gridDim.x) * kTcM;
-                if (p.wait_on != nullptr && kb == 0) {
-                    const int sample = row0 / p.pts_per_sample;
-                    if (sample != ready_sample) {   // all tiles of this sample (rows and GroupNorm sums) are out
-                        while (ld_acquire_gpu(p.wait_on + sample) < p.wait_target) __nanosleep(40);
-                        asm volatile("fence.proxy.async;" ::: "memory");   // generic-proxy acquire -> the TMA reads below
-                        ready_sample = sample;
-                    }
-                }
                 tmbar_wait(&s_empty[s], cw.phase ^ 1u);   // the MMAs that read this stage last time have retired
                 unsigned char* st = tiles + (size_t)s * stage_bytes;
                 tmbar_expect_tx(&s_full[s], tx);
@@ -550,11 +523,9 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
                     asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
                 }
             };
-            // the sums are complete once the previous launch is: before the box wait normally (the table overlaps the TMA
-            // latency), after it when chained (the producer issued this box only after the sample's `done` count was reached)
-            if (p.in_stats != nullptr && p.wait_on == nullptr) gn_table();
+            // the sums are complete once the previous launch is: the table is built before the box wait, under the TMA latency
+            if (p.in_stats != nullptr) gn_table();
             tmbar_wait(&s_full[s], cp.phase);   // the raw box(es) of this k-block have landed
-            if (p.in_stats != nullptr && p.wait_on != nullptr) gn_table();
             unsigned char* st = tiles + (size_t)s * stage_bytes;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
@@ -615,25 +586,16 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
         // ===== epilogue: accumulator tile -> registers -> global, one tile behind the MMA =====
         const int quad = warp & 3;   // rows 32 quad .. +31 of the tile
         const int half = warp >> 2;  // two warps per quadrant: 32-column chunks c0 = 32*half, +64, ...
-        // Completion signal of a tile (p.done: one release-add per epilogue warp and tile).  The release has to wait for the
-        // warp's outstanding stores, ~1 us if issued right behind them -- exposed, because this warp is alone on its
-        // scheduler.  So the signal of tile i is sent when the accumulator of tile i+1 arrives (its stores have long
-        // landed: the fence is free), and only the last tile signals at once.  A consumer loses nothing: it cannot run on
-        // this SM before this CTA exits, and samples that complete in an earlier round are not needed sooner.
-        int unsignalled = -1;
         for (int ti = 0; ti < my_tiles; ++ti) {
             const int row0 = (blockIdx.x + ti * gridDim.x) * kTcM;
             tmbar_wait(&s_acc_full, (unsigned)ti & 1u);
-            if (unsignalled >= 0 && lane == 0) red_release_gpu(p.done + unsignalled);
             TC_MARK(threadIdx.x == 0 && ti < 4, 24 + ti);
             const int sample = row0 / p.pts_per_sample;
             tc_epilogue(p, s_acc, acc_pitch, quad, half, lane, row0, sample, s_bias, s_estage, s_part);
-            __syncwarp();   // (also orders every lane's stores of this tile before lane 0's later release)
+            __syncwarp();
             if (lane == 0) tmbar_arrive(&s_acc_empty);   // one arrival per epilogue warp
-            if (p.done != nullptr) unsignalled = sample;
             TC_MARK(threadIdx.x == 0 && ti < 4, 28 + ti);
         }
-        if (unsignalled >= 0 && lane == 0) red_release_gpu(p.done + unsignalled);
     }
     TC_MARK(threadIdx.x == 256, 1);
 }
@@ -713,7 +675,7 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     if (a->out_stats && (a->epilogue != TC_EPI_PLAIN || a->cout % PVRAFT_GN_GROUPS || (a->cout / PVRAFT_GN_GROUPS) % 4)) return fail(PVRAFT_ERR_UNSUPPORTED, "tc_linear: out_stats needs a GroupNorm group size that is a multiple of 4 (cout=%d)", a->cout);
     if (a->epilogue < TC_EPI_PLAIN || a->epilogue > TC_EPI_FLOW) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: unknown epilogue %d", a->epilogue);
     if ((a->epilogue == TC_EPI_GRU_ZR || a->epilogue == TC_EPI_GRU_Q) && (a->cout != 64 || !a->h || (!a->bias && !a->residual))) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: GRU epilogues need cout=64, h and a bias or a pre-activation term");
-    if (a->epilogue == TC_EPI_FLOW && (a->cout != 64 || a->n_pad != 64 || !a->bias || !a->w3 || !a->b3 || (a->coords2_out && !a->coords2) || (a->flow_out && (!a->coords2_out || !a->coords1)) || (a->flow_user && (!a->flow_out || !a->row_map)))) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: flow epilogue needs cout = n_pad = 64, bias, w3, b3 and consistent coordinate pointers");
+    if (a->epilogue == TC_EPI_FLOW && (a->cout != 64 || a->n_pad != 64 || !a->bias || !a->w3 || !a->b3 || (a->coords2_out && !a->coords2) || (a->flow_out && (!a->coords2_out || !a->coords1)))) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: flow epilogue needs cout = n_pad = 64, bias, w3, b3 and consistent coordinate pointers");
     if (a->epilogue == TC_EPI_GRU_ZR && (a->n_pad != 128 || (!a->bias2 && !a->residual) || !a->out2)) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: GRU zr epilogue needs n_pad=128, bias2, out2");
     if (a->epilogue == TC_EPI_GRU_Q && (a->n_pad != 64 || !a->z)) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: GRU q epilogue needs n_pad=64 and z");
     const long long M = (long long)a->B * a->N;
@@ -732,11 +694,9 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     p.src_min = a->in_min;
     p.gn_kb = a->in_stats ? a->in_channels[0] / kTcKB : 0;
     p.tail = a->tail;
-    p.w3 = a->w3; p.b3 = a->b3; p.coords1 = a->coords1; p.coords2 = a->coords2; p.coords2_out = a->coords2_out; p.flow_out = a->flow_out; p.flow_user = a->flow_user; p.row_map = a->row_map;
+    p.w3 = a->w3; p.b3 = a->b3; p.coords1 = a->coords1; p.coords2 = a->coords2; p.coords2_out = a->coords2_out; p.flow_out = a->flow_out;
     p.out_ld = a->tail ? a->cout + 3 : a->cout;
     p.settled = a->params_settled ? 1 : 0;
-    p.done = a->done;
-    p.wait_target = 8u * (unsigned)(a->N / kTcM);
     if ((rc = tc_make_map(&mw_hi, a->w_hi, a->n_pad, K, K, a->n_pad)) || (rc = tc_make_map(&mw_lo, a->w_lo, a->n_pad, K, K, a->n_pad))) return rc;
     CUtensorMap ma[3], mmin;
     for (int s = 0; s < 3; ++s) {   // unused slots repeat source 0 (a tensor map must be valid even if never dereferenced)
@@ -755,11 +715,9 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     const int stages_res = w_all < budget ? (int)((budget - w_all) / a_stage) : 0;
     const int stages_str = (int)(budget / (a_stage + w_kb));
     p.w_resident = (stages_res >= 3 || stages_res >= stages_str) ? 1 : 0;
-    if (const char* e = getenv("PVRAFT_TC_WRES")) p.w_resident = (atoi(e) != 0 && stages_res >= 2) ? 1 : 0;   // (debug override)
     int stages = p.w_resident ? stages_res : stages_str;
     stages = stages < 1 ? 1 : (stages > kTcMaxStages ? kTcMaxStages : stages);
     const size_t stage = a_stage + (p.w_resident ? 0 : w_kb);
-    if (const char* e = getenv("PVRAFT_TC_STAGES")) { const int v = atoi(e); if (v >= 1 && v <= stages) stages = v; }
     if (stages < 2) return fail(PVRAFT_ERR_SMEM, "tc_linear: K=%d, n_pad=%d leave room for only %d operand stage(s) (2 needed)", K, a->n_pad, stages);
     p.stages = stages;
     if (const char* e = getenv("PVRAFT_TC_DBG")) p.dbg = atoi(e);
@@ -779,20 +737,7 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     const long long n_tiles = (M + kTcM - 1) / kTcM;
     const int grid = (int)(n_tiles < sm_count() ? n_tiles : sm_count());
     // launched with programmatic stream serialization: the kernel's prologue may start while the previous kernel drains
-    static const bool pdl = []() { const char* e = getenv("PVRAFT_TC_PDL"); return !(e && atoi(e) == 0); }();
-    // chaining replaces the grid-wide wait, so it needs the early start PDL gives and parameters that are already in place
-    p.wait_on = (a->wait_on && pdl && p.settled) ? a->wait_on : nullptr;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(kTcThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    const cudaError_t le = cudaLaunchKernelEx(&cfg, kernel, mw_hi, mw_lo, ma[0], ma[1], ma[2], mmin, p);
+    const cudaError_t le = launch_pdl(kernel, grid, kTcThreads, smem, (cudaStream_t)stream, mw_hi, mw_lo, ma[0], ma[1], ma[2], mmin, p);
     if (le != cudaSuccess) return fail((int)le, "tc_linear: launch failed: %s", cudaGetErrorString(le));
     return check_launch("tc_linear");
 }

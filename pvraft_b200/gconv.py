@@ -49,7 +49,7 @@ class SetConv(torch.nn.Module):
                    in_act=ACT_LRELU, in_slope=0.1) if deferred else {}
         # fc1 pre-transform P = fc1.weight[:, :cin] . x   (gconv.py:65-73: fc1 is linear and bias-free)
         if ops.tc_supported(n, cin) and mid <= 128:
-            p = ops.tc_linear([x], ops.tc_weights(self.fc1.weight, col0=0, cols=cin), chain=True, **pro)
+            p = ops.tc_linear([x], ops.tc_weights(self.fc1.weight, col0=0, cols=cin), **pro)
         else:
             p = ops.linear(x, _w(self.fc1.weight), cin=cin, w_ld=cin + 3, cout=mid, in_mode=IN_GN if deferred else ops.IN_PLAIN, **pro)
         ymax, ymin = ops.setconv_edge(p, graph.nbr, graph._rel, _w(self.fc1.weight), cin, stats[0], order=getattr(graph, 'order', None))
@@ -63,7 +63,7 @@ class SetConv(torch.nn.Module):
         pro2 = dict(in_stats=stats[1], in_gamma=_w(self.gn2.weight), in_beta=_w(self.gn2.bias), in_count=float(n) * gsz,
                     in_act=ACT_LRELU, in_slope=0.1)
         if ops.tc_supported(n, cout) and cout <= 128:
-            z3 = ops.tc_linear([z2], ops.tc_weights(self.fc3.weight), out_stats=stats[2], chain=True, **pro2)
+            z3 = ops.tc_linear([z2], ops.tc_weights(self.fc3.weight), out_stats=stats[2], **pro2)
         else:
             z3 = ops.linear(z2, _w(self.fc3.weight), in_mode=IN_GN, out_stats=stats[2], **pro2)
         return Deferred(z3, stats[2], _w(self.gn3.weight), _w(self.gn3.bias), float(n) * gsz)

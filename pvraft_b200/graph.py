@@ -5,16 +5,12 @@
 `k_neighbors`, `size`) but is built by the brute-force kNN kernel (pvraft_knn_fwd) instead of a
 full N x N argsort; the kernels consume the compact int32 LOCAL adjacency `nbr` [B,N,k].
 """
-import os
-
 import torch
 
 from . import ops
 
 
 class Graph:
-    locality_order = os.environ.get('PVRAFT_EDGE_ORDER', '1') != '0'
-
     def __init__(self, nbr, edge_feats, k_neighbors, size, order=None):
         self.nbr = nbr                    # int32 [B,N,k] local ids
         self._rel = edge_feats            # f32 [B,N,k,3]
@@ -49,5 +45,5 @@ class Graph:
         nbr, rel = ops.knn(pc, pc, nb_neighbors, mode=0, want_rel=True)
         # spatially coherent processing order for the edge kernel (changes no result: the 8 warps of a CTA then gather
         # overlapping neighbourhoods, which L1 serves)
-        order = ops.point_order(pc, as_int32=True) if Graph.locality_order and n >= 64 else None
+        order = ops.point_order(pc) if n >= 64 else None
         return Graph(nbr, rel, nb_neighbors, [b * n, b * n], order)

@@ -5,7 +5,6 @@ hot path happens inside libpvraft_b200.so.  All wrappers require contiguous CUDA
 on anything else -- there is deliberately no CPU / eager fallback.
 """
 import ctypes as C
-import os
 import threading
 import weakref
 
@@ -65,21 +64,7 @@ class stats_arena:
 
     def __exit__(self, *exc):
         _TLS.arena = self.prev
-        _TLS.last_tc = None   # (drops the operand references a launch chain holds)
         return False
-
-
-def new_flags(b, device):
-    """[B] zeroed int32 `done` counters for one tensor-core launch, carved out of the arena (None outside an arena scope:
-    no chaining there)."""
-    arena = getattr(_TLS, 'arena', None)
-    if arena is None:
-        return None
-    buf, pos = arena
-    if pos + 1 > buf.shape[0] or buf.shape[1] != b or buf.device != torch.device(device):
-        return None
-    arena[1] = pos + 1
-    return buf[pos].view(torch.int32).reshape(-1)[:b]
 
 
 def new_stats(b, device, n=1):
@@ -185,8 +170,6 @@ def linear(x, weight, bias=None, *, cin=None, w_ld=0, w_cin=0, in_mode=IN_PLAIN,
 
 
 _TC_WEIGHTS = {}
-_EARLY_PARAMS = os.environ.get('PVRAFT_TC_EARLY_PARAMS', '1') != '0'
-_CHAIN = os.environ.get('PVRAFT_TC_CHAIN', '0') == '1'   # opt-in: see tc_linear(chain=...)
 TC_PLAIN, TC_GRU_ZR, TC_GRU_Q, TC_FLOW = 0, 1, 2, 3
 
 
@@ -253,18 +236,17 @@ def derived(tensors, tag, fn):
     return value
 
 
-def point_order(points, as_int32=False):
-    """[B,N,3] -> [B,N] int64 (int32 with as_int32): Morton order over the cells of the kNN grid, from the library's
-    in-shared-memory sort (one launch; the torch formulation below costs ~40 launches)."""
+def point_order(points):
+    """[B,N,3] -> [B,N] int32: Morton order over the cells of the kNN grid, from the library's in-shared-memory sort
+    (one launch; the torch formulation below costs ~40 launches)."""
     b, n, _ = points.shape
     ws_bytes = int(lib().pvraft_knn_workspace_bytes(b, n))
     if ws_bytes <= 0 or n < 64:
-        perm = morton_order(points)
-        return perm.to(torch.int32).contiguous() if as_int32 else perm
+        return morton_order(points).to(torch.int32).contiguous()
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=points.device)
     perm = torch.empty(b, n, dtype=torch.int32, device=points.device)
     _count(lib().pvraft_point_order_fwd(_p(points), b, n, _p(perm, torch.int32), _p(ws, torch.uint8), _stream()), 'point_order')
-    return perm if as_int32 else perm.long()
+    return perm
 
 
 def morton_order(points):
@@ -291,13 +273,10 @@ def tc_supported(n_points, *channels):
 def tc_linear(sources, w, bias=None, *, in_min=None, in_stats=None, in_gamma=None, in_beta=None, in_count=0.0,
               in_act=ACT_NONE, in_slope=0.0, out_act=ACT_NONE, residual=None, out=None, out_stats=None, epilogue=TC_PLAIN,
               bias2=None, out2=None, h=None, z=None, cout=None, tail=None, w3=None, b3=None, coords1=None, coords2=None,
-              coords2_out=None, flow_out=None, flow_user=None, row_map=None, chain=False):
+              coords2_out=None, flow_out=None):
     """Fused layer on the Hopper tensor cores (wgmma).  sources: list of [B,N,C_i] tensors concatenated along K (the
     GroupNorm prologue applies to sources[0]); w = (hi, lo, n_pad, rows) from tc_weights(); tail [B,N,3] fills the
-    output columns cout..cout+2.
-    chain=True: the caller states that everything this layer reads was produced by the tensor-core launch issued
-    immediately before it (or earlier).  Inside a `stats_arena` scope the kernel then waits per SAMPLE on that launch's
-    completion counters instead of on the whole grid, so CTAs start while the previous layer's last tiles still run."""
+    output columns cout..cout+2."""
     hi, lo, n_pad, rows = w
     b, n, _ = sources[0].shape
     cout = rows if cout is None else cout
@@ -316,30 +295,13 @@ def tc_linear(sources, w, bias=None, *, in_min=None, in_stats=None, in_gamma=Non
     a.tail = _p(tail)
     a.w3, a.b3, a.coords1, a.coords2 = _p(w3), _p(b3), _p(coords1), _p(coords2)
     a.coords2_out, a.flow_out = _p(coords2_out), _p(flow_out)
-    a.flow_user, a.row_map = _p(flow_user), _p(row_map, torch.int32)
     # The kernel may fetch its parameters while the previous kernel drains (PDL) once they are settled: not during the
     # three tensor-core launches that follow a weight split or a re-derived folded parameter on this thread.
     pending = getattr(_TLS, 'unsettled', 0)
-    a.params_settled = 1 if pending == 0 and _EARLY_PARAMS else 0
+    a.params_settled = 1 if pending == 0 else 0
     if pending:
         _TLS.unsettled = pending - 1
-    done = new_flags(b, out.device) if _CHAIN else None
-    a.done = _p(done, torch.int32)
-    prev = getattr(_TLS, 'last_tc', None)
-    # chain only on the launch that directly precedes this one (no other library launch in between), same tiling
-    # (worth it only when CTAs walk several tiles: with one tile per CTA the per-sample spin costs more than the grid-wide
-    #  wait it replaces -- measured -1.7 % at B=2, N=8192 = 128 tiles, +0.8 % at 512 tiles with eager launches and nothing
-    #  under graph replay, which is why it is opt-in, PVRAFT_TC_CHAIN=1)
-    chained = (chain and done is not None and prev is not None and prev[0] == launch_count and prev[1] is not None
-               and prev[2] == (b, n) and bool(a.params_settled) and b * n // 128 > _sm_count())
-    if chained:
-        a.wait_on = _p(prev[1], torch.int32)
     _count(lib().pvraft_tc_linear_fwd(C.byref(a), _stream()), 'tc_linear')
-    # A chained successor runs while its predecessors are still reading their operands, so the allocator must not hand that
-    # storage out for a successor's outputs: the operands of a whole chain stay referenced until a launch with a full
-    # grid-wide wait follows (chains are short: motion -> zr -> q -> P, fc3 -> flow head).
-    keep = (sources, in_min, residual, out, out2, h, z, tail, coords2) if done is not None else None
-    _TLS.last_tc = (launch_count, done, (b, n), ((keep,) + (prev[3] if chained else ())) if keep is not None else ())
     return out
 
 
@@ -483,16 +445,6 @@ def corr_init_bwd(g, idx, fmap1, fmap2):
     _count(lib().pvraft_corr_init_bwd(_p(g), _p(idx, torch.int32), _p(fmap1), _p(fmap2), b, n, c, g.shape[-1], _p(d1), _p(d2), _stream()),
            'corr_init_bwd')
     return d1, d2
-
-
-_SM_COUNT = {}
-
-
-def _sm_count():
-    dev = torch.cuda.current_device()
-    if dev not in _SM_COUNT:
-        _SM_COUNT[dev] = torch.cuda.get_device_properties(dev).multi_processor_count
-    return _SM_COUNT[dev]
 
 
 def device_info():

@@ -46,10 +46,6 @@ class _RaftBase(nn.Module):
     # graph is only valid for the parameter values it was captured with: every entry records (version, data_ptr) of all
     # parameters and is re-captured when any of them changed (optimizer step, load_state_dict, .to()).
     use_cuda_graph = {'1': True, '0': False}.get(os.environ.get('PVRAFT_CUDA_GRAPH', ''), None)
-    # Morton-order the first cloud internally (see _encode).  Off by default: in isolation the edge kernel gains 18 %
-    # (101 -> 83 us), but per forward it is a wash at B = 8 (20.87 vs 20.88 ms with the order from the library's grid sort,
-    # 21.34 with a torch-side sort).
-    sort_points = os.environ.get('PVRAFT_SORT_POINTS', '0') == '1'
 
     def reset_graphs(self):
         self.__dict__.pop('_graphs', None)
@@ -66,7 +62,7 @@ class _RaftBase(nn.Module):
         return self
 
     def _graph_key(self, xyz1, num_iters):
-        return (tuple(xyz1.shape), xyz1.device, int(num_iters), bool(self.sort_points))
+        return (tuple(xyz1.shape), xyz1.device, int(num_iters))
 
     def _stamp(self):
         return tuple((q._version, q.data_ptr()) for q in self.parameters())
@@ -127,21 +123,12 @@ class _RaftBase(nn.Module):
                 return self._graphed(p, num_iters)
             return self._forward_impl(p, num_iters)
 
-    def _encode(self, p, allow_sort=True):
+    def _encode(self, p):
         xyz1, xyz2 = p[0], p[1]
         if xyz1.dim() != 3 or xyz1.shape[-1] != 3 or xyz1.shape != xyz2.shape:
             raise ValueError('expected p = [xyz1 [B,N,3], xyz2 [B,N,3]]')
         xyz1 = xyz1.detach().contiguous().float()
         xyz2 = xyz2.detach().contiguous().float()
-        # Spatial reordering of the first cloud (every op is per point or per neighbourhood, so the point order carries no
-        # meaning): along a Morton curve the 32 neighbour rows that the SetConv edge kernel gathers for consecutive points
-        # overlap in L1/L2 (edge kernel 101 -> 83 us).  The flows are written back in the caller's order (`row_map`).
-        self._row_map = None
-        if self.sort_points and allow_sort and ops.tc_supported(xyz1.shape[1]):
-            perm = ops.point_order(xyz1)
-            xyz1 = torch.gather(xyz1, 1, perm.unsqueeze(-1).expand(-1, -1, 3)).contiguous()
-            offs = (torch.arange(xyz1.shape[0], device=xyz1.device) * xyz1.shape[1]).view(-1, 1)
-            self._row_map = (perm + offs).to(torch.int32).reshape(-1).contiguous()   # row of permuted point r in the input order
         # both clouds go through the shared feature encoder as one batch of 2B samples (RAFTSceneFlow.py:25-26: every op is
         # per sample): half the launches, and 2B*N/128 tiles fill the 132 SMs more evenly
         b = xyz1.shape[0]
@@ -166,8 +153,8 @@ class _RaftBase(nn.Module):
         use_tc = ops.tc_supported(n)
         # (hoisting the constant context part of the GRU pre-activations out of the loop -- K = 128 per iteration instead of 192 --
         #  was measured slower in round 1, 22.15 vs 21.72 ms per forward: the two extra per-point reads outweigh the shorter GEMM)
-        # per iteration: moments + 4 GroupNorm accumulators + the completion counters of the 9 tensor-core launches; one memset
-        with ops.stats_arena(b, xyz1.device, 14 * num_iters):
+        # per iteration: the lookup moments, the lookup-feature GroupNorm sums and the three SetConv sums; one memset
+        with ops.stats_arena(b, xyz1.device, 5 * num_iters):
             return self._iterate_body(xyz1, graph_context, net, inp, num_iters, keep_all, coords2, flow, preds, me, use_tc)
 
     def _iterate_body(self, xyz1, graph_context, net, inp, num_iters, keep_all, coords2, flow, preds, me, use_tc):
@@ -185,22 +172,12 @@ class _RaftBase(nn.Module):
 
                 _, keep = self.corr_block.feature_point_major(coords2, motion_args=attach)   # :42 + update.py:83
             new_flow = torch.empty_like(xyz1)
-            user_flow = torch.empty_like(xyz1) if (keep_all and self._row_map is not None) else None   # caller's point order
             net, _ = self.update_block.forward_pm(net, inp, motion, graph_context, coords1=xyz1, coords2=coords2,
-                                                  coords2_out=coords2, flow_out=new_flow, flow_user=user_flow,
-                                                  row_map=self._row_map if user_flow is not None else None)   # :44-46
+                                                  coords2_out=coords2, flow_out=new_flow)   # :44-46
             flow = new_flow
             if keep_all:
-                preds.append(flow if user_flow is None else user_flow)
+                preds.append(flow)
         return flow, preds
-
-    def _to_input_order(self, x):
-        """[B,N,C] in the internal (Morton) point order -> the caller's order."""
-        if self._row_map is None:
-            return x
-        out = torch.empty_like(x)
-        out.view(-1, x.shape[-1])[self._row_map.long()] = x.reshape(-1, x.shape[-1])
-        return out
 
 
 class RSF(_RaftBase):
@@ -238,12 +215,12 @@ class RSF_refine(_RaftBase):
     def _forward_impl(self, p, num_iters=12):
         xyz1, _, graph, graph_context, net, inp = self._encode(p)
         flow, _ = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=False)
-        return self._to_input_order(self.refine_block(flow, graph))      # RAFTSceneFlowRefine.py:46
+        return self.refine_block(flow, graph)      # RAFTSceneFlowRefine.py:46
 
     def _forward_train(self, p, num_iters=12):
         """model/RAFTSceneFlowRefine.py:22-48: everything up to the last flow under no_grad (the fused inference kernels),
         the refiner -- the only part tools/engine_refine.py trains -- layer by layer with gradients."""
         with torch.no_grad():
-            xyz1, _, graph, graph_context, net, inp = self._encode(p, allow_sort=False)
+            xyz1, _, graph, graph_context, net, inp = self._encode(p)
             flow, _ = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=False)
         return train.flot_refine(self.refine_block, flow, graph)

@@ -72,9 +72,9 @@ class ConvGRU(nn.Module):
             # wgmma: [z|r] = sigmoid(W_zr [h,x]); q = tanh(W_q [r*h, x]); h' = (1-z) h + z q   (update.py:32-39)
             z, rh = torch.empty_like(net), torch.empty_like(net)
             ops.tc_linear([net, inp, motion], ops.tc_weights((self.convz.weight, self.convr.weight)), _w(self.convz.bias),
-                          bias2=_w(self.convr.bias), epilogue=ops.TC_GRU_ZR, out=z, out2=rh, h=net, cout=64, chain=True)
+                          bias2=_w(self.convr.bias), epilogue=ops.TC_GRU_ZR, out=z, out2=rh, h=net, cout=64)
             ops.tc_linear([rh, inp, motion], ops.tc_weights(self.convq.weight), _w(self.convq.bias), epilogue=ops.TC_GRU_Q,
-                          out=out, h=net, z=z, cout=64, chain=True)
+                          out=out, h=net, z=z, cout=64)
             return out
         a = _lib.GruArgs(ops._p(net), ops._p(inp), ops._p(motion), ops._p(_w(self.convz.weight)), ops._p(_w(self.convz.bias)),
                          ops._p(_w(self.convr.weight)), ops._p(_w(self.convr.bias)), ops._p(_w(self.convq.weight)),
@@ -115,7 +115,7 @@ class FlowHead(nn.Module):
             nn.Conv1d(64, 3, 1),
         )
 
-    def forward_pm(self, net, graph, coords1=None, coords2=None, coords2_out=None, flow_out=None, flow_user=None, row_map=None):
+    def forward_pm(self, net, graph, coords1=None, coords2=None, coords2_out=None, flow_out=None):
         """net [B,N,64] -> delta_flow [B,N,3]; optionally also the RAFT coordinate update."""
         b, n, _ = net.shape
         d = self.setconv.forward_deferred(net, graph)
@@ -130,7 +130,7 @@ class FlowHead(nn.Module):
             ops.tc_linear([d.z, net], ops.tc_weights(w_eff), b_eff, in_stats=d.stats, in_gamma=d.gamma, in_beta=d.beta,
                           in_count=d.count, in_act=ops.ACT_LRELU, in_slope=0.1, epilogue=ops.TC_FLOW, out=delta, cout=64,
                           w3=_w(oc[2].weight), b3=_w(oc[2].bias), coords1=coords1, coords2=coords2, coords2_out=coords2_out,
-                          flow_out=flow_out, flow_user=flow_user, row_map=row_map, chain=True)
+                          flow_out=flow_out)
             return delta
         a = _lib.FlowOutArgs(ops._p(d.z), ops._p(d.stats, torch.float64), ops._p(d.gamma), ops._p(d.beta), ops._p(net),
                              ops._p(_w(self.conv1.weight)), ops._p(_w(self.conv1.bias)), ops._p(_w(oc[0].weight)),

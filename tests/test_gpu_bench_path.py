@@ -266,34 +266,3 @@ def test_cuda_graph_recaptured_after_weight_update(dev):
         eager = m([pc1, pc2], 2)[-1]
     assert rel_err(graphed.cpu(), eager.cpu()) < 1e-6
     assert rel_err(before.cpu(), eager.cpu()) > 1e-3
-
-
-def test_chained_tensor_core_launches_equal_grid_wide_waits(dev):
-    """Opt-in (PVRAFT_TC_CHAIN=1): inside the loop six of the nine tensor-core launches start per SAMPLE on the completion
-    counters of the launch before them instead of waiting for its whole grid (ops.tc_linear(chain=True)): scheduling only.  The flows must equal those of
-    the same launches with grid-wide waits up to the order of the double-precision GroupNorm partial sums (the bound of the
-    batch-of-8 test) -- a stale or early read would show at 1e-2.  Eager launches and CUDA-graph replay, several repeats,
-    a batch large enough (4 x 64 tiles over 132 SMs) for CTAs to run ahead of the previous launch's last tiles."""
-    from pvraft_b200 import ops
-    m, _ = make_model(dev)
-    b, iters = 4, 12
-    pc1, pc2 = [t.to(dev) for t in O.synthetic_clouds(b, N, seed=123)]
-    was = ops._CHAIN
-    runs = {}
-    with torch.no_grad():
-        for graph in (False, True):
-            m.use_cuda_graph = graph
-            try:
-                ops._CHAIN = False
-                m.reset_graphs()
-                plain = m([pc1, pc2], iters)[-1].clone()
-                ops._CHAIN = True
-                m.reset_graphs()
-                runs[graph] = (plain, [m([pc1, pc2], iters)[-1].clone() for _ in range(4)])
-            finally:
-                ops._CHAIN = was
-    scale = float(runs[False][0].abs().mean())
-    for graph, (plain, chained) in runs.items():
-        errs = [float((c - plain).abs().mean()) / scale for c in chained]
-        print(f'chained vs grid-wide waits ({"graph replay" if graph else "eager"}): mean-abs / mean|flow| =', [f'{e:.1e}' for e in errs])
-        assert max(errs) < 2e-4
