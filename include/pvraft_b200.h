@@ -66,6 +66,22 @@ PVRAFT_API int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, in
                            void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * The same GEMM over one window of the correlation matrix, for clouds whose N x N matrix is not built whole.
+ *   pvraft_tf32_split_fwd: x [n] f32 -> hi = tf32(x), lo = tf32(x - hi) (the operand split of pvraft_corr_matmul_fwd),
+ *     n % 4 == 0, 16-byte aligned buffers.  Run once per feature map and build, not once per window.
+ *   pvraft_corr_matmul_window_fwd: split operands a_hi/a_lo (fmap1) and b_hi/b_lo (fmap2), each [B,N,C] point-major with
+ *     N % 128 == 0, C % 32 == 0
+ *     -> corr [B, R, ldc] with R = rows rounded up to 128: corr[b,i,j] = <fmap1[b,r0+i,:], fmap2[b,c0+j,:]> / sqrt(C) for
+ *     i < R, j < cols rounded up to 128.  Whole 128 x 128 tiles are written: an operand row past the caller's points (a
+ *     padding row, of any content) only reaches the slab rows / columns past `rows` / `cols`, which the caller ignores.
+ *     r0, c0 multiples of 128; ldc % 4 == 0; the window's whole tiles lie inside [0, N).  Every value is bit-identical to
+ *     the same entry of pvraft_corr_matmul_fwd on the same operands.
+ * --------------------------------------------------------------------------------------------- */
+PVRAFT_API int pvraft_tf32_split_fwd(const float* x, int64_t n, float* hi, float* lo, void* stream);
+PVRAFT_API int pvraft_corr_matmul_window_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
+                                             int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Correlation truncation: the K largest entries of every row of a dense correlation matrix.
  * Replaces torch.topk(corr, k, dim=2, sorted=True) in CorrBlock.init_module, model/corr.py:37-40.
  *   corr [B,N,M] -> val [B,N,K] f32, idx [B,N,K] int32 column ids, written in ASCENDING COLUMN order
@@ -74,6 +90,19 @@ PVRAFT_API int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, in
  * Requires 1 <= K <= min(M, 1024) and M <= 49152 (the row is staged in shared memory).
  * --------------------------------------------------------------------------------------------- */
 PVRAFT_API int pvraft_corr_topk_fwd(const float* corr, int B, int N, int M, int K, float* val, int32_t* idx, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * The same selection over a strided window, with an optional id map: the two steps of the windowed build.
+ *   corr [rows, ld] (cols <= ld valid columns per row) -> val / idx [rows, ld_out] (the first K entries of each row),
+ *   the K largest of each row in ascending column order, value ties at the K-th place: lowest columns win.
+ *   idx = cand_ids ? cand_ids[row * ld + j] : col_base + j for the kept column j (cand_ids [rows, ld] int32 or NULL).
+ *   Per column window: col_base = first column, ld_out = W*K, val/idx offset by w*K -> the concatenated candidate lists.
+ *   Merge: corr = the [rows, W*K] candidate values, cand_ids = their ids -> the row's exact top-K, because each list is in
+ *   ascending column order.
+ * Requires 1 <= K <= min(cols, 1024), cols <= 49152.
+ * --------------------------------------------------------------------------------------------- */
+PVRAFT_API int pvraft_corr_topk_window_fwd(const float* corr, int rows, int cols, int64_t ld, int K, int col_base, const int32_t* cand_ids,
+                                           float* val, int32_t* idx, int64_t ld_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Bank-aware arrangement of the truncated state, once per forward (no reference counterpart: the order of

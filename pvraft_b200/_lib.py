@@ -69,7 +69,11 @@ _SIGNATURES = {
     'pvraft_device_info': (C.c_int, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     'pvraft_corr_matmul_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
     'pvraft_corr_matmul_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_tf32_split_fwd': (C.c_int, [VP, C.c_int64, VP, VP, VP]),
+    'pvraft_corr_matmul_window_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                VP, C.c_int64, VP]),
     'pvraft_corr_topk_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_corr_topk_window_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, VP, VP, VP, C.c_int64, VP]),
     'pvraft_corr_reorder': (C.c_int, [VP, VP, C.c_int64, C.c_int, VP, VP, VP]),
     'pvraft_xyz_pad_fwd': (C.c_int, [VP, C.c_int64, VP, VP]),
     'pvraft_corr_lookup_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

@@ -71,12 +71,7 @@ class CorrBlock(nn.Module):
         b, n, c = fmap1_pm.shape
         if c % 32 != 0:
             raise NotImplementedError(f'calculate_corr: {c} feature channels (the wgmma GEMM needs a multiple of 32; the model has 128)')
-        pad = (-n) % 128
-        if pad == 0:
-            return ops.corr_matmul(fmap1_pm, fmap2_pm)
-        f1 = torch.nn.functional.pad(fmap1_pm, (0, 0, 0, pad)).contiguous()
-        f2 = torch.nn.functional.pad(fmap2_pm, (0, 0, 0, pad)).contiguous()
-        return ops.corr_matmul(f1, f2)[:, :n, :n].contiguous()
+        return ops.corr_dense(fmap1_pm, fmap2_pm)
 
     @staticmethod
     def calculate_corr(fmap1, fmap2):
@@ -95,8 +90,8 @@ class CorrBlock(nn.Module):
         b, n_p, _ = xyz2.shape
         if n_p < self.truncate_k:
             raise ValueError(f'truncate_k={self.truncate_k} exceeds the number of points {n_p}')
-        corr = self.calculate_corr_pm(fmap1_pm.contiguous(), fmap2_pm.contiguous())   # wgmma, 3xTF32 (fp32-accurate)
-        val, idx = ops.corr_topk(corr, self.truncate_k)
+        # wgmma GEMM (3xTF32, fp32-accurate) + top-K; in column windows above 49152 points (ops.CorrPlan)
+        val, idx = ops.corr_build(fmap1_pm.contiguous(), fmap2_pm.contiguous(), self.truncate_k)
         self._install(*ops.corr_reorder(val, idx))
         self._xyz2 = xyz2.detach().contiguous().float()
         self._xyz2p = ops.xyz_pad(self._xyz2)

@@ -50,12 +50,14 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, v
 }
 
 struct GemmParams {
-    float* corr;   // [B,N,N]
-    int N, C;
+    float* corr;   // [B, tiles_m * 128, ldc]: rows [r0, r0 + 128 tiles_m) x columns [c0, c0 + 128 tiles_n) of every sample
+    int N, C;      // operand rows per sample, channels
     float scale;   // sqrt(C): the divisor of model/corr.py:99
     float rscale;  // RN(1 / scale)
-    int tiles_n;   // N / 128
-    long long n_tiles;   // B * tiles_n * tiles_n
+    int r0, c0;    // first row of fmap1 / of fmap2 (multiples of 128)
+    int tiles_m, tiles_n;   // 128-row / 128-column tiles of the window
+    long long ldc;          // output row stride in floats
+    long long n_tiles;      // B * tiles_m * tiles_n
 };
 
 // x / s, correctly rounded, from r = RN(1/s) (Markstein): q0 = x r; q = q0 + (x - q0 s) r.  Three instructions instead of
@@ -93,7 +95,7 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    const int tiles_per_batch = p.tiles_n * p.tiles_n;
+    const int tiles_per_batch = p.tiles_m * p.tiles_n;
 
     if (warp < 4) {
         // ===== TMA producer =====
@@ -104,7 +106,7 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
                 const long long t = blockIdx.x + i * gridDim.x;
                 const int b = (int)(t / tiles_per_batch), r = (int)(t - (long long)b * tiles_per_batch);
                 const int tile_m = r / p.tiles_n, tile_n = r - tile_m * p.tiles_n;
-                const int row_a = b * p.N + tile_m * kTileM, row_b = b * p.N + tile_n * kTileN;
+                const int row_a = b * p.N + p.r0 + tile_m * kTileM, row_b = b * p.N + p.c0 + tile_n * kTileN;
                 for (int kb = 0; kb < num_kb; ++kb) {
                     mbar_wait_(&s_empty[s], phase ^ 1u);
                     unsigned char* st = tiles + (size_t)s * kStageBytes;
@@ -155,8 +157,8 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
         prev_s = -1;
         // corr / sqrt(C) as a true (correctly rounded) division (model/corr.py:99)
         const int row = tile_m * kTileM + half * 64 + wq * 16 + (lane >> 2);
-        float* o = p.corr + ((size_t)b * p.N + row) * p.N + (size_t)tile_n * kTileN + 2 * (lane & 3);
-        const size_t down8 = (size_t)8 * p.N;
+        float* o = p.corr + ((size_t)b * p.tiles_m * kTileM + row) * (size_t)p.ldc + (size_t)tile_n * kTileN + 2 * (lane & 3);
+        const size_t down8 = (size_t)8 * p.ldc;
 #pragma unroll
         for (int j = 0; j < kTileN / 8; ++j) {
             *reinterpret_cast<float2*>(o + 8 * j) = make_float2(div_by_const(acc[4 * j + 0], p.scale, p.rscale), div_by_const(acc[4 * j + 1], p.scale, p.rscale));
@@ -215,6 +217,34 @@ static int make_map(CUtensorMap* m, const float* base, long long rows, int C) {
     return 0;
 }
 
+// Rows [r0, r0 + 128 tiles_m) x columns [c0, c0 + 128 tiles_n) of every sample, from split operands [B*N, C] (hi/lo of
+// both maps), into corr [B, 128 tiles_m, ldc]
+static int launch_gemm(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N, int C, int r0,
+                       int tiles_m, int c0, int tiles_n, float* corr, long long ldc, cudaStream_t st) {
+    int rc;
+    CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
+    if ((rc = make_map(&ma_hi, a_hi, (long long)B * N, C)) || (rc = make_map(&ma_lo, a_lo, (long long)B * N, C)) ||
+        (rc = make_map(&mb_hi, b_hi, (long long)B * N, C)) || (rc = make_map(&mb_lo, b_lo, (long long)B * N, C)))
+        return rc;
+    GemmParams p{};
+    p.corr = corr; p.N = N; p.C = C;
+    p.scale = sqrtf((float)C);
+    p.rscale = (float)(1.0 / (double)p.scale);
+    p.r0 = r0; p.c0 = c0;
+    p.tiles_m = tiles_m; p.tiles_n = tiles_n;
+    p.ldc = ldc;
+    p.n_tiles = (long long)B * tiles_m * tiles_n;
+    const size_t smem = (size_t)kStages * kStageBytes + 1024;
+    if ((rc = opt_in_smem(k_corr_gemm, smem))) return rc;
+    const int grid = (int)(p.n_tiles < sm_count() ? p.n_tiles : sm_count());
+    k_corr_gemm<<<grid, kGemmThreads, smem, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, p);
+    return check_launch("corr_gemm");
+}
+
+static void launch_split(const float* x, long long n, float* hi, float* lo, cudaStream_t st) {
+    k_tf32_split<<<(unsigned)((n / 4 + 255) / 256), 256, 0, st>>>(x, n, hi, lo);
+}
+
 }  // namespace pvraft
 
 using namespace pvraft;
@@ -236,24 +266,35 @@ extern "C" int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, in
     float* a_lo = a_hi + n;
     float* b_hi = a_lo + n;
     float* b_lo = b_hi + n;
-    const unsigned blocks = (unsigned)((n / 4 + 255) / 256);
-    k_tf32_split<<<blocks, 256, 0, st>>>(fmap1, n, a_hi, a_lo);
-    k_tf32_split<<<blocks, 256, 0, st>>>(fmap2, n, b_hi, b_lo);
-    int rc = check_launch("tf32_split");
+    launch_split(fmap1, n, a_hi, a_lo, st);
+    launch_split(fmap2, n, b_hi, b_lo, st);
+    const int rc = check_launch("tf32_split");
     if (rc) return rc;
-    CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
-    if ((rc = make_map(&ma_hi, a_hi, (long long)B * N, C)) || (rc = make_map(&ma_lo, a_lo, (long long)B * N, C)) ||
-        (rc = make_map(&mb_hi, b_hi, (long long)B * N, C)) || (rc = make_map(&mb_lo, b_lo, (long long)B * N, C)))
-        return rc;
-    GemmParams p{};
-    p.corr = corr; p.N = N; p.C = C;
-    p.scale = sqrtf((float)C);
-    p.rscale = (float)(1.0 / (double)p.scale);
-    p.tiles_n = N / kTileN;
-    p.n_tiles = (long long)B * p.tiles_n * p.tiles_n;
-    const size_t smem = (size_t)kStages * kStageBytes + 1024;
-    if ((rc = opt_in_smem(k_corr_gemm, smem))) return rc;
-    const int grid = (int)(p.n_tiles < sm_count() ? p.n_tiles : sm_count());
-    k_corr_gemm<<<grid, kGemmThreads, smem, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, p);
-    return check_launch("corr_gemm");
+    return launch_gemm(a_hi, a_lo, b_hi, b_lo, B, N, C, 0, N / kTileM, 0, N / kTileN, corr, N, st);
+}
+
+extern "C" int pvraft_tf32_split_fwd(const float* x, int64_t n, float* hi, float* lo, void* stream) {
+    if (!x || !hi || !lo || n <= 0) return fail(PVRAFT_ERR_BAD_ARG, "tf32_split: bad argument");
+    if (n % 4 || ((uintptr_t)x | (uintptr_t)hi | (uintptr_t)lo) % 16)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "tf32_split: n=%lld must be a multiple of 4 and the buffers 16-byte aligned", (long long)n);
+    launch_split(x, n, hi, lo, (cudaStream_t)stream);
+    return check_launch("tf32_split");
+}
+
+extern "C" int pvraft_corr_matmul_window_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
+                                             int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream) {
+    if (!a_hi || !a_lo || !b_hi || !b_lo || !corr) return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul_window: null pointer");
+    if (B <= 0 || N <= 0 || C <= 0 || rows <= 0 || cols <= 0 || r0 < 0 || c0 < 0)
+        return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul_window: bad shape");
+    if (N % kTileM || C % kBlockK || r0 % kTileM || c0 % kTileN)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: N=%d, r0=%d and c0=%d must be multiples of 128 and C=%d of 32", N, r0,
+                    c0, C);
+    const int tiles_m = (rows + kTileM - 1) / kTileM, tiles_n = (cols + kTileN - 1) / kTileN;
+    if (rows > N - r0 || cols > N - c0 || r0 + tiles_m * kTileM > N || c0 + tiles_n * kTileN > N)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: rows [%d, %d) x columns [%d, %d), whole tiles, exceed N=%d", r0,
+                    r0 + tiles_m * kTileM, c0, c0 + tiles_n * kTileN, N);
+    if (ldc < (int64_t)tiles_n * kTileN || ldc % 4)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: ldc=%lld (need a multiple of 4, >= %d)", (long long)ldc, tiles_n * kTileN);
+    if ((long long)B * N > 0x7fffffffLL) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: B*N=%lld operand rows", (long long)B * N);
+    return launch_gemm(a_hi, a_lo, b_hi, b_lo, B, N, C, r0, tiles_m, c0, tiles_n, corr, ldc, (cudaStream_t)stream);
 }

@@ -8,6 +8,8 @@
 // written in ASCENDING COLUMN order (ties at the threshold: lowest columns win).  The reference sorts the K
 // values descending; nothing downstream depends on that order (pvraft_corr_reorder rearranges every row
 // anyway), so the sort is not done here -- CorrBlock.truncated_corr sorts on demand for API parity.
+// The same kernels run the two steps of the windowed build of large clouds (pvraft_corr_topk_window_fwd): the top-K of
+// each column window of a slab, and the merge of a row's per-window candidate lists through their stored column ids.
 #include "common.cuh"
 
 namespace pvraft {
@@ -23,15 +25,18 @@ __device__ __forceinline__ float key2f(unsigned k) {
 }
 __device__ __forceinline__ int padded(int i) { return i + (i >> 5); }
 
-__global__ void __launch_bounds__(kTopkThreads) k_corr_topk(const float* __restrict__ corr, int M, int K,
-                                                            float* __restrict__ val, int32_t* __restrict__ idx) {
+// Both kernels read M columns of row r at corr + r * ld and write its K survivors to val / idx + r * ld_out; the id of column j
+// is ids[r * ld + j] when an id map is given (a candidate list), col_base + j otherwise.
+__global__ void __launch_bounds__(kTopkThreads) k_corr_topk(const float* __restrict__ corr, int M, long long ld, int K,
+                                                            float* __restrict__ val, int32_t* __restrict__ idx, long long ld_out,
+                                                            int col_base, const int32_t* __restrict__ ids) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     unsigned* s_key = reinterpret_cast<unsigned*>(smem_raw);   // [padded(M)]
     __shared__ int s_hist[256];
     __shared__ unsigned s_prefix, s_need;
     __shared__ unsigned s_warp[kTopkThreads / 32];
     const size_t row = blockIdx.x;
-    const float* src = corr + row * (size_t)M;
+    const float* src = corr + row * (size_t)ld;
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
     for (int i = tid; i < M; i += kTopkThreads) s_key[padded(i)] = f2key(__ldg(src + i));
     if (tid == 0) { s_prefix = 0u; s_need = (unsigned)K; }
@@ -105,8 +110,8 @@ __global__ void __launch_bounds__(kTopkThreads) k_corr_topk(const float* __restr
         bool keep = k > T;
         if (k == T) { keep = eq_seen < need_eq; ++eq_seen; }
         if (keep) {
-            val[row * K + pos] = key2f(k);
-            idx[row * K + pos] = i;
+            val[row * ld_out + pos] = key2f(k);
+            idx[row * ld_out + pos] = ids ? __ldg(ids + row * ld + i) : col_base + i;
             ++pos;
         }
     }
@@ -118,8 +123,9 @@ __global__ void __launch_bounds__(kTopkThreads) k_corr_topk(const float* __restr
 // loads); the K-th largest key is found with three radix passes (11 + 11 + 10 bits) of which only the first counts every
 // key; the ordered compaction scans packed per-chunk counts (11-bit fields) across the block.
 // ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kTopkThreads) k_corr_topk_vec(const float* __restrict__ corr, int M, int K, float* __restrict__ val,
-                                                                int32_t* __restrict__ idx) {
+__global__ void __launch_bounds__(kTopkThreads) k_corr_topk_vec(const float* __restrict__ corr, int M, long long ld, int K,
+                                                                float* __restrict__ val, int32_t* __restrict__ idx, long long ld_out,
+                                                                int col_base, const int32_t* __restrict__ ids) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     uint4* s_key = reinterpret_cast<uint4*>(smem_raw);   // [8 * 256]
     constexpr int kCand = 1024;                          // capacity of the candidate list of the second and third pass
@@ -131,7 +137,7 @@ __global__ void __launch_bounds__(kTopkThreads) k_corr_topk_vec(const float* __r
     __shared__ int s_need;
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
     const size_t row = blockIdx.x;
-    const float4* src = reinterpret_cast<const float4*>(corr + row * (size_t)M);
+    const float4* src = reinterpret_cast<const float4*>(corr + row * (size_t)ld);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         const int c4 = j * kTopkThreads + tid;
@@ -333,12 +339,26 @@ __global__ void __launch_bounds__(kTopkThreads) k_corr_topk_vec(const float* __r
         }
     }
     __syncthreads();
-    float* vrow = val + row * (size_t)K;
-    int32_t* irow = idx + row * (size_t)K;
+    float* vrow = val + row * (size_t)ld_out;
+    int32_t* irow = idx + row * (size_t)ld_out;
+    const int32_t* idrow = ids ? ids + row * (size_t)ld : nullptr;
     for (int i = tid; i < K; i += kTopkThreads) {
         vrow[i] = key2f(s_oval[i]);
-        irow[i] = s_oidx[i];
+        irow[i] = idrow ? __ldg(idrow + s_oidx[i]) : col_base + s_oidx[i];
     }
+}
+
+static int launch_topk(const float* corr, long long rows, int M, long long ld, int K, int col_base, const int32_t* ids, float* val,
+                       int32_t* idx, long long ld_out, cudaStream_t st) {
+    if (M <= 8192 && M % 4 == 0 && ld % 4 == 0 && (uintptr_t)corr % 16 == 0) {
+        k_corr_topk_vec<<<(unsigned)rows, kTopkThreads, 8 * kTopkThreads * sizeof(uint4), st>>>(corr, M, ld, K, val, idx, ld_out, col_base, ids);
+        return check_launch("corr_topk");
+    }
+    const size_t smem = (size_t)(M + (M >> 5) + 4) * 4;
+    int rc;
+    if ((rc = opt_in_smem(k_corr_topk, smem))) return rc;
+    k_corr_topk<<<(unsigned)rows, kTopkThreads, smem, st>>>(corr, M, ld, K, val, idx, ld_out, col_base, ids);
+    return check_launch("corr_topk");
 }
 
 }  // namespace pvraft
@@ -352,13 +372,17 @@ extern "C" int pvraft_corr_topk_fwd(const float* corr, int B, int N, int M, int 
     if (M > 49152) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_topk: M=%d columns (max 49152)", M);
     const long long rows = (long long)B * N;
     if (rows > 0x7fffffffLL) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_topk: too many rows");
-    if (M <= 8192 && M % 4 == 0) {
-        k_corr_topk_vec<<<(unsigned)rows, kTopkThreads, 8 * kTopkThreads * sizeof(uint4), (cudaStream_t)stream>>>(corr, M, K, val, idx);
-        return check_launch("corr_topk");
-    }
-    const size_t smem = (size_t)(M + (M >> 5) + 4) * 4;
-    int rc;
-    if ((rc = opt_in_smem(k_corr_topk, smem))) return rc;
-    k_corr_topk<<<(unsigned)rows, kTopkThreads, smem, (cudaStream_t)stream>>>(corr, M, K, val, idx);
-    return check_launch("corr_topk");
+    return launch_topk(corr, rows, M, M, K, 0, nullptr, val, idx, K, (cudaStream_t)stream);
+}
+
+extern "C" int pvraft_corr_topk_window_fwd(const float* corr, int rows, int cols, int64_t ld, int K, int col_base, const int32_t* cand_ids,
+                                           float* val, int32_t* idx, int64_t ld_out, void* stream) {
+    if (!corr || !val || !idx) return fail(PVRAFT_ERR_BAD_ARG, "corr_topk_window: null pointer");
+    if (rows <= 0 || cols <= 0 || ld < cols || col_base < 0) return fail(PVRAFT_ERR_BAD_ARG, "corr_topk_window: bad shape");
+    if (K < 1 || K > cols || K > 1024 || ld_out < K)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_topk_window: K=%d with cols=%d, ld_out=%lld (need 1 <= K <= min(cols,1024), ld_out >= K)", K,
+                    cols, (long long)ld_out);
+    if (cols > 49152) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_topk_window: cols=%d (max 49152)", cols);
+    if (!cand_ids && (long long)col_base + cols > 0x7fffffffLL) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_topk_window: column ids overflow");
+    return launch_topk(corr, rows, cols, ld, K, col_base, cand_ids, val, idx, ld_out, (cudaStream_t)stream);
 }

@@ -7,6 +7,7 @@ on anything else -- there is deliberately no CPU / eager fallback.
 import ctypes as C
 import threading
 import weakref
+from typing import NamedTuple
 
 import torch
 
@@ -114,6 +115,110 @@ def corr_topk(corr, k):
     val = torch.empty(b, n, k, dtype=torch.float32, device=corr.device)
     idx = torch.empty(b, n, k, dtype=torch.int32, device=corr.device)
     _count(lib().pvraft_corr_topk_fwd(_p(corr), b, n, m, k, _p(val), _p(idx, torch.int32), _stream()), 'corr_topk')
+    return val, idx
+
+
+def corr_dense(fmap1_pm, fmap2_pm):
+    """corr_matmul for any N: a ragged N is zero-padded to the next multiple of 128 (the kernel's tile) and the result cropped."""
+    n = fmap1_pm.shape[1]
+    pad = (-n) % 128
+    if pad == 0:
+        return corr_matmul(fmap1_pm, fmap2_pm)
+    f1 = torch.nn.functional.pad(fmap1_pm, (0, 0, 0, pad)).contiguous()
+    f2 = torch.nn.functional.pad(fmap2_pm, (0, 0, 0, pad)).contiguous()
+    return corr_matmul(f1, f2)[:, :n, :n].contiguous()
+
+
+CORR_ROW_MAX = 49152      # widest row the top-K kernels stage in shared memory (csrc/corr_topk.cu)
+# Bytes of the windowed build's scratch: the correlation slab of one row block and window plus the row block's candidate
+# lists.  A forward captured into a CUDA graph keeps this memory in its pool for as long as the graph lives, so the cap is a
+# fixed, modest size rather than a share of the free memory; row blocks of >= 1800 rows keep every GEMM launch at more
+# than ten 128 x 128 tiles per SM.
+CORR_SLAB_CAP = 1 << 30
+
+
+class CorrPlan(NamedTuple):
+    """How corr_build computes the truncated correlation of a [B,N,C] x [B,M,C] pair.
+    dense: one [B,N,M] matrix (corr_dense) and one corr_topk, as long as a whole row fits the top-K kernels (M <= 49152).
+    Otherwise, for every sample and row block of fmap1, the slab of each column window of fmap2 is computed and reduced to its
+    K best candidates, and the W*K candidates of a row are reduced to the row's K best: the same result as the dense build."""
+    dense: bool
+    windows: tuple      # ((c0, width), ...) column windows of fmap2, in ascending order, tiling [0, M); starts are 128-aligned
+    row_blocks: tuple   # ((r0, rows), ...) row blocks of fmap1, in ascending order, tiling [0, N); starts are 128-aligned
+    ld: int             # slab row stride in floats (the widest window; a multiple of 128)
+    slab_bytes: int     # scratch: the [B,N,M] matrix (dense) or one row block's slab + candidate lists (windowed)
+
+
+def _pad128(x):
+    return (x + 127) // 128 * 128
+
+
+def corr_plan(b, n, m, c, k, window=CORR_ROW_MAX, cap=CORR_SLAB_CAP):
+    """Plan of corr_build for B samples of N x M correlations over C channels, truncated to K per row.  `window` (the widest
+    column window, a multiple of 128) and `cap` (bytes of slab + candidate lists) exist for tests; the model uses the defaults."""
+    if min(b, n, m, c, k) <= 0:
+        raise ValueError(f'corr_plan: bad shape B={b} N={n} M={m} C={c} K={k}')
+    if window % 128 or not 0 < window <= CORR_ROW_MAX:
+        raise ValueError(f'corr_plan: window={window} must be a multiple of 128 and at most {CORR_ROW_MAX}')
+    if m <= window:
+        return CorrPlan(True, ((0, m),), ((0, n),), _pad128(m), 4 * b * _pad128(n) * _pad128(m))
+    if k > m:
+        raise ValueError(f'truncate_k={k} exceeds the number of points {m}')
+    w = -(-m // window)
+    if w * k > CORR_ROW_MAX:
+        raise ValueError(f'a cloud of {m} points needs {w} column windows, and their {w * k} candidates per row exceed the '
+                         f'{CORR_ROW_MAX} the merge step can stage (truncate_k={k}: at most {CORR_ROW_MAX // k * window} points)')
+    width = _pad128(-(-m // w))   # <= window, and (w - 1) * width < m
+    windows = tuple((i * width, min(width, m - i * width)) for i in range(w))
+    if windows[-1][1] < k:
+        raise ValueError(f'corr_plan: the last column window has {windows[-1][1]} columns, fewer than truncate_k={k}')
+    per_row = 4 * width + 8 * w * k   # slab row + candidate values and ids
+    rows = max(128, cap // per_row // 128 * 128)
+    nb = -(-_pad128(n) // rows)
+    rows = _pad128(-(-n // nb))
+    row_blocks = tuple((r0, min(rows, n - r0)) for r0 in range(0, n, rows))
+    return CorrPlan(False, windows, row_blocks, width, rows * per_row)
+
+
+def corr_build(fmap1_pm, fmap2_pm, k, plan=None):
+    """Point-major feature maps [B,N,C] -> (val [B,N,K] f32, idx [B,N,K] int32): the K largest correlations of every row,
+    in ascending column order (corr_topk of corr_dense), without the [B,N,N] matrix when N > 49152 (see CorrPlan).
+    Both paths give the same bits."""
+    b, n, c = fmap1_pm.shape
+    m = fmap2_pm.shape[1]
+    if fmap2_pm.shape != (b, m, c) or m != n:
+        raise ValueError(f'corr_build: feature maps {tuple(fmap1_pm.shape)} and {tuple(fmap2_pm.shape)} (clouds of equal size)')
+    if c % 32 != 0:
+        raise NotImplementedError(f'calculate_corr: {c} feature channels (the wgmma GEMM needs a multiple of 32; the model has 128)')
+    plan = corr_plan(b, n, m, c, k) if plan is None else plan
+    if plan.dense:
+        return corr_topk(corr_dense(fmap1_pm, fmap2_pm), k)
+    dev = fmap1_pm.device
+    npad = _pad128(n)
+    # tf32 hi/lo of both maps, split once.  The padding rows are left unset: a row of A or B only reaches the slab entries of
+    # that row / column, and the top-K steps never read the entries past N.
+    ws = torch.empty(4, b, npad, c, dtype=torch.float32, device=dev)
+    for i, f in enumerate((fmap1_pm, fmap2_pm)):
+        for s in range(b):
+            _count(lib().pvraft_tf32_split_fwd(_p(f[s]), n * c, _p(ws[2 * i, s]), _p(ws[2 * i + 1, s]), _stream()), 'tf32_split')
+    nw = len(plan.windows)
+    wk = nw * k
+    rows = max(r for _, r in plan.row_blocks)
+    slab = torch.empty(_pad128(rows), plan.ld, dtype=torch.float32, device=dev)
+    cand_val = torch.empty(rows, wk, dtype=torch.float32, device=dev)
+    cand_idx = torch.empty(rows, wk, dtype=torch.int32, device=dev)
+    val = torch.empty(b, n, k, dtype=torch.float32, device=dev)
+    idx = torch.empty(b, n, k, dtype=torch.int32, device=dev)
+    for s in range(b):
+        split = [_p(ws[q, s]) for q in range(4)]
+        for r0, nr in plan.row_blocks:
+            for j, (c0, nc) in enumerate(plan.windows):
+                _count(lib().pvraft_corr_matmul_window_fwd(*split, 1, npad, c, r0, nr, c0, nc, _p(slab), plan.ld, _stream()),
+                       'corr_matmul_window')
+                _count(lib().pvraft_corr_topk_window_fwd(_p(slab), nr, nc, plan.ld, k, c0, None, _p(cand_val) + 4 * j * k,
+                                                         _p(cand_idx, torch.int32) + 4 * j * k, wk, _stream()), 'corr_topk_window')
+            _count(lib().pvraft_corr_topk_window_fwd(_p(cand_val), nr, wk, wk, k, 0, _p(cand_idx, torch.int32), _p(val[s, r0:r0 + nr]),
+                                                     _p(idx[s, r0:r0 + nr], torch.int32), k, _stream()), 'corr_topk_merge')
     return val, idx
 
 

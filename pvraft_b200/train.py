@@ -206,9 +206,7 @@ class CorrInitFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, fmap1, fmap2, k, corr_block):
         fmap1, fmap2 = fmap1.contiguous(), fmap2.contiguous()
-        corr = corr_block.calculate_corr_pm(fmap1, fmap2)
-        val, idx = ops.corr_topk(corr, k)
-        del corr
+        val, idx = ops.corr_build(fmap1, fmap2, k)
         val, idx = ops.corr_reorder(val, idx)
         ctx.save_for_backward(fmap1, fmap2, idx)
         ctx.mark_non_differentiable(idx)
