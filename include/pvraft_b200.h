@@ -19,7 +19,8 @@
  *     per-point feature array (one point's channels are contiguous), coordinates are [B,N,3].
  *   - GroupNorm statistics travel as raw double-precision sums ("stats": [B,8,2] = per sample,
  *     per group (sum, sum of squares)); producers ACCUMULATE with atomics, so the caller zeroes
- *     them (cudaMemsetAsync) before the producing call.
+ *     them (cudaMemsetAsync) before the producing call (the *_det producers: a fixed order, see
+ *     "Deterministic entry points").
  *   - Weights are passed in the reference's own state_dict layouts ([Cout,Cin(,1(,1))] row-major).
  */
 #ifndef PVRAFT_B200_H
@@ -410,7 +411,8 @@ PVRAFT_API int pvraft_point_order_fwd(const float* xyz, int B, int N, int32_t* p
 /* ================================================================================================
  * Gradient contract (SURVEY.md section 8b): what tools/engine.py:131-147 differentiates through.
  * The training path runs layer by layer; each backward entry point below pairs with a forward one.
- * Parameter-gradient outputs are ACCUMULATED with atomics into buffers the caller has zeroed.
+ * Parameter-gradient outputs are ACCUMULATED with atomics into buffers the caller has zeroed (in an order that varies from
+ * run to run; the *_det forms under "Deterministic entry points" accumulate in a fixed order).
  * ============================================================================================= */
 
 /* 1x1 convolution (pvraft_linear_fwd without prologue / activation), weight and bias gradient:
@@ -479,6 +481,58 @@ PVRAFT_API int pvraft_sizeof(int which);
 
 /* [B,C,N] <-> [B,N,C] transposes used at the reference-layout seams of the Python modules. */
 PVRAFT_API int pvraft_transpose_fwd(const float* in, int B, int R, int C, float* out, void* stream); /* [B,R,C] -> [B,C,R] */
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Deterministic entry points (what pvraft_b200 runs while torch.are_deterministic_algorithms_enabled() is true).
+ * Each takes the arguments of the entry point it mirrors plus `workspace`: pvraft_*_det*_workspace_bytes(...) bytes of
+ * caller-provided, 8-byte aligned scratch that the caller ZERO-FILLS before every call.  The kernels add exact fixed-point
+ * values (Q64.64 in 128 bits) into the workspace and then one launch adds the workspace, rounded, into the destination
+ * the default form accumulates into.  Integer additions are exact, and every value added is a floating-point sum whose
+ * order is a function of the shapes (a point, a 128-point tile, a warp's rows of a grid sized from the shapes), so the
+ * results are bitwise identical from run to run, under graph replay, and for any SM count.  Each value added is truncated
+ * toward zero to a multiple of 2^-64, so the exact sum of n values is known to within an ABSOLUTE n * 2^-64 (terms below
+ * 2^-64 vanish); it is rounded once to double and then added to the destination.  A non-finite value,
+ * or one of magnitude >= 2^62, makes its destination entry NaN.  Same results as the default forms up to summation order.
+ * Forward statistics are per (sample, tile / point), so with N % 128 == 0 a sample's statistics do not depend on the batch.
+ * ------------------------------------------------------------------------------------------------------------------ */
+PVRAFT_API int64_t pvraft_linear_det_workspace_bytes(int B);
+PVRAFT_API int pvraft_linear_det_fwd(const pvraft_linear_args* args, void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_tc_linear_det_workspace_bytes(int B);
+PVRAFT_API int pvraft_tc_linear_det_fwd(const pvraft_tc_linear_args* args, void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_setconv_edge_det_workspace_bytes(int B);
+PVRAFT_API int pvraft_setconv_edge_det_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
+                                           int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order,
+                                           void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_corr_lookup_det_workspace_bytes(int B);
+PVRAFT_API int pvraft_corr_lookup_det_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
+                                          int B, int N, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
+                                          int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace, void* stream);
+PVRAFT_API int pvraft_corr_lookup_bf16_det_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
+                                               const float* coords, int B, int N, int K, int levels, float base_scale, float* vox,
+                                               int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
+                                               void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_edge_det_fwd_workspace_bytes(int B);
+PVRAFT_API int pvraft_edge_det_fwd(const float* P, const int32_t* nbr, float* E, int B, int N, int C, double* stats, void* workspace,
+                                   void* stream);
+PVRAFT_API int64_t pvraft_flow_metrics_det_workspace_bytes(void);
+PVRAFT_API int pvraft_flow_metrics_det_fwd(const float* est, const float* gt, const float* mask, int64_t points, double* acc,
+                                           void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_linear_wgrad_det_workspace_bytes(int cin, int cout);
+PVRAFT_API int pvraft_linear_wgrad_det(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
+                                       void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_linear_bwd_small_det_workspace_bytes(int cin, int cout);
+PVRAFT_API int pvraft_linear_bwd_small_det(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld,
+                                           float* dW, int dw_ld, float* db, float* dx, void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_gn_act_bwd_det_workspace_bytes(int B, int C);
+PVRAFT_API int pvraft_gn_act_bwd_det(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta,
+                                     double count, int act, float slope, int B, int64_t rows, int C, double* gsum, double* dgamma,
+                                     double* dbeta, double* dslope, float* dx, const float* slope_dev, const uint8_t* arg,
+                                     void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_edge_bwd_det_workspace_bytes(int B, int N, int C);
+PVRAFT_API int pvraft_edge_bwd_det(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int N, int C);
+PVRAFT_API int pvraft_corr_init_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C,
+                                        int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream);
 
 #ifdef __cplusplus
 }

@@ -109,6 +109,33 @@ _SIGNATURES = {
     'pvraft_flow_l1_bwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, C.c_float, VP, VP]),
     'pvraft_sizeof': (C.c_int, [C.c_int]),
     'pvraft_transpose_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, VP]),
+    # deterministic forms (include/pvraft_b200.h, "Deterministic entry points"): the same arguments plus a zeroed workspace
+    'pvraft_linear_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_linear_det_fwd': (C.c_int, [C.POINTER(LinearArgs), VP, VP]),
+    'pvraft_tc_linear_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_tc_linear_det_fwd': (C.c_int, [C.POINTER(TcLinearArgs), VP, VP]),
+    'pvraft_setconv_edge_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_setconv_edge_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_corr_lookup_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                             VP, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_bf16_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                                  VP, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_edge_det_fwd_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_edge_det_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_flow_metrics_det_workspace_bytes': (C.c_int64, []),
+    'pvraft_flow_metrics_det_fwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, VP]),
+    'pvraft_linear_wgrad_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
+    'pvraft_linear_wgrad_det': (C.c_int, [VP, VP, C.c_int64, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP]),
+    'pvraft_linear_bwd_small_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
+    'pvraft_linear_bwd_small_det': (C.c_int, [VP, VP, VP, C.c_int64, C.c_int, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP, VP]),
+    'pvraft_gn_act_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
+    'pvraft_gn_act_bwd_det': (C.c_int, [VP, VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int64, C.c_int, VP, VP, VP,
+                                        VP, VP, VP, VP, VP, VP]),
+    'pvraft_edge_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    'pvraft_edge_bwd_det': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_corr_init_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    'pvraft_corr_init_bwd_det': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
 }
 EXPORTS = tuple(_SIGNATURES)
 

@@ -25,7 +25,7 @@
 // subtract / multiply / add (no FMA contraction), true IEEE division, round-half-even.
 #include <math.h>
 
-#include "common.cuh"
+#include "fixed_point.cuh"
 
 namespace pvraft {
 
@@ -127,7 +127,27 @@ __device__ __forceinline__ unsigned warp_scan_packed(unsigned w, int lane) {
     return w;
 }
 
-template <int KPL, bool POW2, bool SMEM_TAB, bool HALF>
+// 16 per-lane partial sums -> one total per lane pair with a reduce-scatter butterfly (15 + 1 double shuffles instead of
+// 14 x 5): after the step with partner lane ^ d a lane keeps the half of its values selected by that bit of its id, so lane l
+// ends up with the total of value ((l >> 1) & 15)
+__device__ __forceinline__ double moments_reduce_scatter(double (&v)[16], int lane) {
+#pragma unroll
+    for (int d = 16, h = 8; d >= 2; d >>= 1, h >>= 1) {
+        const bool up = (lane & d) != 0;
+#pragma unroll
+        for (int i = 0; i < h; ++i) {
+            const double send = up ? v[i] : v[i + h];
+            const double keep = up ? v[i + h] : v[i];
+            v[i] = keep + __shfl_xor_sync(kFull, send, d);
+        }
+    }
+    return v[0] + __shfl_xor_sync(kFull, v[0], 1);
+}
+
+// DET: every point's moments (the fixed butterfly over its 32 kNN edges) enter a per-lane fixed-point sum, added at the end
+// to the [B,16] fixed-point workspace p.moments then points at (slot 15 of a sample holds its work counter): the sums do not
+// depend on which warp claimed which point (fixed_point.cuh)
+template <int KPL, bool POW2, bool SMEM_TAB, bool HALF, bool DET>
 __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupParams p) {
     using val_t = typename StateT<HALF>::val;
     using idx_t = typename StateT<HALF>::idx;
@@ -197,6 +217,8 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
         if (seg_end > pt_end) seg_end = pt_end;
         const float4* tab_g = p.tab + (size_t)b * p.N;
         int* counter = dyn ? reinterpret_cast<int*>(p.moments + (size_t)b * PVRAFT_MOMENTS + 15) : nullptr;
+        if constexpr (DET)   // slot 15 of the sample's fixed-point moments
+            counter = dyn ? reinterpret_cast<int*>(reinterpret_cast<unsigned long long*>(p.moments) + ((size_t)b * PVRAFT_MOMENTS + 15) * kFxWords) : nullptr;
         auto claim_chunk = [&]() -> long long {   // first point of the next unclaimed chunk of this sample
             int c = 0;
             if (lane == 0) c = atomicAdd(counter, kChunk);
@@ -233,6 +255,7 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
         double mom[14];
 #pragma unroll
         for (int i = 0; i < 14; ++i) mom[i] = 0.0;
+        Fx fmom{0ull, 0ull, 0u};
 
         if (active_warp) {
             int left = left0, done = 0;
@@ -496,6 +519,15 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
                     mom[8] += f1 * f1; mom[9] += f1 * f2; mom[10] += f1 * f3;
                     mom[11] += f2 * f2; mom[12] += f2 * f3; mom[13] += f3 * f3;
                 }
+                if (DET && p.moments) {
+                    double v[16];
+#pragma unroll
+                    for (int i = 0; i < 14; ++i) { v[i] = mom[i]; mom[i] = 0.0; }
+                    v[14] = 1.0;
+                    v[15] = 0.0;
+                    const double t = moments_reduce_scatter(v, lane);
+                    if ((lane & 1) == 0) fx_add(fmom, fx_from(t));
+                }
                 __syncwarp();
                 // the point after next (its row is requested once `nxt` has been streamed)
                 pt = nxt;
@@ -507,10 +539,12 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
                     nxt = seg + __shfl_sync(kFull, claim, 0);
                 }
             }
-            if (p.moments) {
-                // 16 per-lane partial sums -> one total per lane pair with a reduce-scatter butterfly (15 + 1 double shuffles
-                // instead of 14 x 5): after the step with partner lane ^ d a lane keeps the half of its values selected by that
-                // bit of its id, so lane l ends up with the total of value ((l >> 1) & 15)
+            if (DET && p.moments) {
+                const int which = (lane >> 1) & 15;
+                if ((lane & 1) == 0 && which < 15)
+                    fx_atomic(reinterpret_cast<unsigned long long*>(p.moments) + ((size_t)b * PVRAFT_MOMENTS + which) * kFxWords, fmom);
+            } else if (p.moments) {
+                // (moments_reduce_scatter, written out)
                 double v[16];
 #pragma unroll
                 for (int i = 0; i < 14; ++i) v[i] = mom[i];
@@ -621,7 +655,7 @@ static float cube_threshold(float r) {
     return t;
 }
 
-template <int KPL, bool POW2, bool HALF>
+template <int KPL, bool POW2, bool HALF, bool DET>
 static int launch_lookup(LookupParams& p, cudaStream_t st) {
     const int K = KPL * 32;
     const size_t per_warp = lookup_warp_bytes(K);
@@ -642,11 +676,11 @@ static int launch_lookup(LookupParams& p, cudaStream_t st) {
     if (grid < 1) grid = 1;
     int rc;
     if (smem_tab) {
-        auto k = k_corr_lookup<KPL, POW2, true, HALF>;
+        auto k = k_corr_lookup<KPL, POW2, true, HALF, DET>;
         if ((rc = opt_in_smem(k, smem))) return rc;
         launch_pdl(k, grid, kLookupThreads, smem, st, p);
     } else {
-        auto k = k_corr_lookup<KPL, POW2, false, HALF>;
+        auto k = k_corr_lookup<KPL, POW2, false, HALF, DET>;
         if ((rc = opt_in_smem(k, smem))) return rc;
         launch_pdl(k, grid, kLookupThreads, smem, st, p);
     }
@@ -681,9 +715,11 @@ extern "C" int pvraft_xyz_pad_fwd(const float* xyz, int64_t rows, float* out, vo
     return check_launch("xyz_pad");
 }
 
+template <bool DET>
 static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half, const float* xyz2_pad, const float* coords, int B, int N,
                            int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
-                           int8_t* dbg_cube, void* stream) {
+                           int8_t* dbg_cube, void* ws, void* stream) {
+    if (DET && moments && !ws) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: the deterministic form needs its workspace");
     if (!corr_val || !corr_idx || !xyz2_pad || !coords || !vox || !knn_sel) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: null pointer");
     if (B <= 0 || N <= 0) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: B=%d N=%d", B, N);
     if (levels < 1 || levels > 4) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_lookup: levels=%d (1..4 supported)", levels);
@@ -693,7 +729,8 @@ static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half
     if (half && N > 65536) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_lookup: uint16 candidate ids need N <= 65536 (N=%d)", N);
     LookupParams p{};
     p.corr_val = corr_val; p.corr_idx = corr_idx; p.tab = reinterpret_cast<const float4*>(xyz2_pad); p.coords = coords;
-    p.vox = vox; p.knn_sel = reinterpret_cast<float4*>(knn_sel); p.knn_slot = knn_slot; p.moments = moments;
+    p.vox = vox; p.knn_sel = reinterpret_cast<float4*>(knn_sel); p.knn_slot = knn_slot;
+    p.moments = DET && moments ? static_cast<double*>(ws) : moments;
     p.dbg_cube = dbg_cube;
     p.B = B; p.N = N; p.K = K; p.levels = levels;
     p.vox_ld = vox_ld > 0 ? vox_ld : levels * 27;
@@ -708,12 +745,15 @@ static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half
     }
     p.thr_c = cube_threshold(p.r[levels - 1]);
     cudaStream_t st = (cudaStream_t)stream;
+    int rc = 0;
 #define PVRAFT_LOOKUP_CASE(KPL_)                                                            \
     case KPL_ * 32:                                                                         \
-        return pow2 ? launch_lookup<KPL_, true, false>(p, st) : launch_lookup<KPL_, false, false>(p, st);
+        rc = pow2 ? launch_lookup<KPL_, true, false, DET>(p, st) : launch_lookup<KPL_, false, false, DET>(p, st); \
+        break;
 #define PVRAFT_LOOKUP_CASE_H(KPL_)                                                          \
     case KPL_ * 32:                                                                         \
-        return pow2 ? launch_lookup<KPL_, true, true>(p, st) : launch_lookup<KPL_, false, true>(p, st);
+        rc = pow2 ? launch_lookup<KPL_, true, true, DET>(p, st) : launch_lookup<KPL_, false, true, DET>(p, st); \
+        break;
     if (half) {
         switch (K) {
             PVRAFT_LOOKUP_CASE_H(4)
@@ -723,7 +763,7 @@ static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half
             default:
                 return fail(PVRAFT_ERR_UNSUPPORTED, "corr_lookup (bf16 state): truncate_k=%d (supported: 128,256,512,1024)", K);
         }
-    }
+    } else {
     switch (K) {
         PVRAFT_LOOKUP_CASE(1)
         PVRAFT_LOOKUP_CASE(2)
@@ -734,24 +774,44 @@ static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half
         default:
             return fail(PVRAFT_ERR_UNSUPPORTED, "corr_lookup: truncate_k=%d (supported: 32,64,128,256,512,1024)", K);
     }
+    }
 #undef PVRAFT_LOOKUP_CASE
 #undef PVRAFT_LOOKUP_CASE_H
+    if (rc || !DET || !moments) return rc;
+    return fx_flush_f64(static_cast<const unsigned long long*>(ws), B, 15, PVRAFT_MOMENTS, PVRAFT_MOMENTS, moments, st);
 }
 
 extern "C" int pvraft_corr_lookup_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad,
                                       const float* coords, int B, int N, int K, int levels, float base_scale,
                                       float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
                                       int8_t* dbg_cube, void* stream) {
-    return corr_lookup_any(corr_val, corr_idx, false, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel, knn_slot, moments,
-                           dbg_cube, stream);
+    return corr_lookup_any<false>(corr_val, corr_idx, false, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel, knn_slot,
+                                  moments, dbg_cube, nullptr, stream);
 }
 
 extern "C" int pvraft_corr_lookup_bf16_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
                                            const float* coords, int B, int N, int K, int levels, float base_scale,
                                            float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
                                            int8_t* dbg_cube, void* stream) {
-    return corr_lookup_any(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel, knn_slot,
-                           moments, dbg_cube, stream);
+    return corr_lookup_any<false>(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel,
+                                  knn_slot, moments, dbg_cube, nullptr, stream);
+}
+
+extern "C" int64_t pvraft_corr_lookup_det_workspace_bytes(int B) { return (int64_t)B * PVRAFT_MOMENTS * kFxWords * 8; }
+
+extern "C" int pvraft_corr_lookup_det_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords, int B,
+                                          int N, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
+                                          int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace, void* stream) {
+    return corr_lookup_any<true>(corr_val, corr_idx, false, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel, knn_slot,
+                                 moments, dbg_cube, workspace, stream);
+}
+
+extern "C" int pvraft_corr_lookup_bf16_det_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
+                                               const float* coords, int B, int N, int K, int levels, float base_scale, float* vox, int vox_ld,
+                                               float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace,
+                                               void* stream) {
+    return corr_lookup_any<true>(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel,
+                                 knn_slot, moments, dbg_cube, workspace, stream);
 }
 
 // fp32 correlation values -> bf16 (round to nearest even), int32 candidate ids -> uint16: the 4-byte-per-candidate state

@@ -1,13 +1,16 @@
 // Training extras on the device (SURVEY.md section 8f, row f3): the masked L1 flow loss of tools/loss.py:16-40 and the
 // end-point-error statistics of tools/metric.py:6-79, one pass over the points each, accumulated in double; the loss's
 // backward needs no host synchronisation (the point count and the incoming gradient are read from device memory).
-#include "common.cuh"
+#include "fixed_point.cuh"
 
 namespace pvraft {
 
 // acc[0] = sum over valid points of |ex|+|ey|+|ez|     acc[1] = number of valid points (mask > 0)
 // acc[2] = sum of the end-point errors ||e||            acc[3..5] = points with (epe < .05 or rel < .05), (epe < .1 or rel < .1),
 //                                                                  (epe > .3 or rel > .1), rel = epe / (||gt|| + 1e-4)   (metric.py:66-77)
+// DET: the grid is capped by a constant, so each warp's sums cover the same points on every GPU; they enter the [6]
+// fixed-point workspace `acc` points at then (fixed_point.cuh)
+template <bool DET>
 __global__ void __launch_bounds__(256) k_flow_metrics(const float* __restrict__ est, const float* __restrict__ gt, const float* __restrict__ mask,
                                                       long long points, double* __restrict__ acc) {
     __shared__ double s_acc[6];
@@ -30,8 +33,13 @@ __global__ void __launch_bounds__(256) k_flow_metrics(const float* __restrict__ 
 #pragma unroll
     for (int i = 0; i < 6; ++i) {
         const float s = warp_sum(v[i]);
-        if (lane_id() == 0 && s != 0.f) atomicAdd(&s_acc[i], (double)s);
+        if constexpr (DET) {
+            if (lane_id() == 0 && s != 0.f) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + i * kFxWords, (double)s);
+        } else {
+            if (lane_id() == 0 && s != 0.f) atomicAdd(&s_acc[i], (double)s);
+        }
     }
+    if constexpr (DET) return;
     __syncthreads();
     if (threadIdx.x < 6 && s_acc[threadIdx.x] != 0.0) atomicAdd(acc + threadIdx.x, s_acc[threadIdx.x]);
 }
@@ -59,8 +67,22 @@ extern "C" int pvraft_flow_metrics_fwd(const float* est, const float* gt, const 
     long long blocks = (points + 255) / 256;
     const long long cap = (long long)sm_count() * 8;
     if (blocks > cap) blocks = cap;
-    k_flow_metrics<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(est, gt, mask, points, acc);
+    k_flow_metrics<false><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(est, gt, mask, points, acc);
     return check_launch("flow_metrics");
+}
+
+extern "C" int64_t pvraft_flow_metrics_det_workspace_bytes(void) { return 6 * kFxWords * 8; }
+
+extern "C" int pvraft_flow_metrics_det_fwd(const float* est, const float* gt, const float* mask, int64_t points, double* acc, void* workspace,
+                                           void* stream) {
+    if (!est || !gt || !acc || !workspace || points <= 0) return fail(PVRAFT_ERR_BAD_ARG, "flow_metrics_det: bad argument");
+    long long blocks = (points + 255) / 256;
+    if (blocks > kDetCtas) blocks = kDetCtas;
+    cudaStream_t st = (cudaStream_t)stream;
+    k_flow_metrics<true><<<(unsigned)blocks, 256, 0, st>>>(est, gt, mask, points, static_cast<double*>(workspace));
+    int rc = check_launch("flow_metrics_det");
+    if (rc) return rc;
+    return fx_flush_f64(static_cast<const unsigned long long*>(workspace), 1, 6, 6, 0, acc, st);
 }
 
 extern "C" int pvraft_flow_l1_bwd(const float* est, const float* gt, const float* mask, int64_t points, const double* acc, const float* g,

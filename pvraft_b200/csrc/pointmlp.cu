@@ -10,6 +10,7 @@
 // GroupNorm needs statistics over all points of a sample, so every GroupNorm is a kernel boundary:
 // the producer accumulates double-precision (sum, sum^2) per (sample, group) with atomics and the
 // consumer folds mean/rstd/gamma/beta into one FMA per element while staging its input tile.
+#include "fixed_point.cuh"
 #include "tile_gemm.cuh"
 
 namespace pvraft {
@@ -59,6 +60,31 @@ __device__ __forceinline__ void flush_stats(double* s_g /*[16] smem*/, double* g
     }
     __syncthreads();
     if (threadIdx.x < 16 && s_g[threadIdx.x] != 0.0) atomicAdd(gstats + threadIdx.x, s_g[threadIdx.x]);
+}
+
+// DET form (fixed_point.cuh): after every tile, each thread's sums over its points of the tile enter the CTA's fixed-point
+// slots s_fx [16]; when the CTA leaves a sample these are added to the sample's slots of the [B,16] workspace
+__device__ __forceinline__ void tile_stats_fx(unsigned long long* s_fx, double* dS, double* dSS, const int* ch, int n, int cout) {
+    const int gsz = cout / PVRAFT_GN_GROUPS;
+    for (int i = 0; i < n; ++i) {
+        if (ch[i] < cout && (dS[i] != 0.0 || dSS[i] != 0.0)) {
+            const int g = ch[i] / gsz;
+            fx_atomic(s_fx + (g * 2) * kFxWords, dS[i]);
+            fx_atomic(s_fx + (g * 2 + 1) * kFxWords, dSS[i]);
+        }
+        dS[i] = 0.0;
+        dSS[i] = 0.0;
+    }
+}
+
+__device__ __forceinline__ void flush_stats_fx(unsigned long long* s_fx, unsigned long long* gfx /*[16] slots of the sample*/) {
+    __syncthreads();
+    if (threadIdx.x < 16) {
+        const Fx v{s_fx[threadIdx.x * kFxWords], s_fx[threadIdx.x * kFxWords + 1], (unsigned)s_fx[threadIdx.x * kFxWords + 2]};
+        fx_atomic(gfx + threadIdx.x * kFxWords, v);
+    }
+    __syncthreads();
+    if (threadIdx.x < 16 * kFxWords) s_fx[threadIdx.x] = 0ull;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -119,6 +145,7 @@ __device__ __forceinline__ void linear_compute(const LinearParams& P, const floa
     }
 }
 
+template <bool DET>
 __global__ void __launch_bounds__(kMlpThreads, 2) k_linear(const LinearParams P) {
     const pvraft_linear_args& a = P.a;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -127,7 +154,10 @@ __global__ void __launch_bounds__(kMlpThreads, 2) k_linear(const LinearParams P)
     float* s_scale = s_bias + P.CP;
     float* s_shift = s_scale + P.KD;
     float* s_act = s_shift + P.KD;
-    double* s_g = reinterpret_cast<double*>(s_act + kTP * P.AS);   // [16]
+    double* s_g = reinterpret_cast<double*>(s_act + kTP * P.AS);   // [16]  (DET: [16] fixed-point slots; a.out_stats is the workspace)
+    unsigned long long* s_fx = reinterpret_cast<unsigned long long*>(s_g);
+    if constexpr (DET)
+        if (threadIdx.x < 16 * kFxWords) s_fx[threadIdx.x] = 0ull;
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
 
     const int w_cin = a.w_cin > 0 ? a.w_cin : a.cin;
@@ -144,7 +174,11 @@ __global__ void __launch_bounds__(kMlpThreads, 2) k_linear(const LinearParams P)
     for (TileIter it(a.B, a.N); it.valid(); ++it.t) {
         const int b = it.sample(), p0 = it.p0(), npts = it.npts();
         if (b != cur_b) {
+            if constexpr (DET) {
+                if (a.out_stats && cur_b >= 0) flush_stats_fx(s_fx, reinterpret_cast<unsigned long long*>(a.out_stats) + (size_t)cur_b * 16 * kFxWords);
+            } else {
             if (a.out_stats && cur_b >= 0) flush_stats(s_g, a.out_stats + (size_t)cur_b * 16, dS, dSS, ch, P.passes * 4, a.cout);
+            }
             if (cur_b >= 0) {
 #pragma unroll
                 for (int i = 0; i < 8; ++i) { dS[i] = 0.0; dSS[i] = 0.0; }
@@ -208,6 +242,12 @@ __global__ void __launch_bounds__(kMlpThreads, 2) k_linear(const LinearParams P)
         // ---- GEMM: all (<= 128) output channels in one sweep over the activations + epilogue ------------------
         if (P.passes == 2) linear_compute<2>(P, s_act, s_w, s_bias, row0, npts, dS, dSS);
         else linear_compute<1>(P, s_act, s_w, s_bias, row0, npts, dS, dSS);
+        if constexpr (DET)
+            if (a.out_stats) tile_stats_fx(s_fx, dS, dSS, ch, P.passes * 4, a.cout);
+    }
+    if constexpr (DET) {
+        if (a.out_stats && cur_b >= 0) flush_stats_fx(s_fx, reinterpret_cast<unsigned long long*>(a.out_stats) + (size_t)cur_b * 16 * kFxWords);
+        return;
     }
     if (a.out_stats && cur_b >= 0) flush_stats(s_g, a.out_stats + (size_t)cur_b * 16, dS, dSS, ch, P.passes * 4, a.cout);
 }
@@ -724,8 +764,9 @@ __global__ void __launch_bounds__(kMlpThreads, 2) k_flowout(const pvraft_flowout
 
 using namespace pvraft;
 
-extern "C" int pvraft_linear_fwd(const pvraft_linear_args* a, void* stream) {
-    if (!a || !a->in || !a->weight || !a->out) return fail(PVRAFT_ERR_BAD_ARG, "linear: null pointer");
+template <bool DET>
+static int linear_fwd(const pvraft_linear_args* a, void* ws, void* stream) {
+    if (!a || !a->in || !a->weight || !a->out || (DET && a->out_stats && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "linear: null pointer");
     if (a->B <= 0 || a->N <= 0 || a->cin <= 0 || a->cout <= 0) return fail(PVRAFT_ERR_BAD_ARG, "linear: bad shape");
     if (a->cout > 128 || a->cin > 256) return fail(PVRAFT_ERR_UNSUPPORTED, "linear: cin=%d cout=%d (max 256/128)", a->cin, a->cout);
     if (a->in_mode != PVRAFT_IN_PLAIN) {
@@ -735,17 +776,26 @@ extern "C" int pvraft_linear_fwd(const pvraft_linear_args* a, void* stream) {
     if (a->out_stats && a->cout % PVRAFT_GN_GROUPS) return fail(PVRAFT_ERR_BAD_ARG, "linear: out_stats needs cout %% 8 == 0");
     LinearParams P{};
     P.a = *a;
+    if (DET && a->out_stats) P.a.out_stats = static_cast<double*>(ws);
     P.KD = pad4(a->cin);
     P.CP = pad64(a->cout);
     P.WS = wstride(P.CP);
     P.AS = act_stride(P.KD);
     P.passes = P.CP / 64;
-    const size_t smem = sizeof(float) * ((size_t)P.KD * P.WS + P.CP + 2 * P.KD + (size_t)kTP * P.AS) + 16 * sizeof(double) + 16;
+    const size_t smem = sizeof(float) * ((size_t)P.KD * P.WS + P.CP + 2 * P.KD + (size_t)kTP * P.AS) + 16 * (DET ? kFxWords * 8 : sizeof(double)) + 16;
     int rc;
-    if ((rc = opt_in_smem(k_linear, smem))) return rc;
-    k_linear<<<tile_grid(k_linear, a->B, a->N, smem), kMlpThreads, smem, (cudaStream_t)stream>>>(P);
-    return check_launch("linear");
+    if ((rc = opt_in_smem(k_linear<DET>, smem))) return rc;
+    k_linear<DET><<<tile_grid(k_linear<DET>, a->B, a->N, smem), kMlpThreads, smem, (cudaStream_t)stream>>>(P);
+    rc = check_launch("linear");
+    if (rc || !DET || !a->out_stats) return rc;
+    return fx_flush_f64(static_cast<const unsigned long long*>(ws), 1, (long long)a->B * 16, (long long)a->B * 16, 0, a->out_stats, (cudaStream_t)stream);
 }
+
+extern "C" int pvraft_linear_fwd(const pvraft_linear_args* a, void* stream) { return linear_fwd<false>(a, nullptr, stream); }
+
+extern "C" int64_t pvraft_linear_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
+
+extern "C" int pvraft_linear_det_fwd(const pvraft_linear_args* a, void* workspace, void* stream) { return linear_fwd<true>(a, workspace, stream); }
 
 extern "C" int pvraft_gn_act_fwd(const float* in, const double* stats, const float* gamma, const float* beta, double count,
                                  int act, float slope, int B, int N, int C, int transpose_out, float* out, const float* slope_dev,

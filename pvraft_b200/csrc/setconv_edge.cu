@@ -10,7 +10,7 @@
 //
 // One warp per point; lane l owns the adjacent channel pairs (2l, 2l+1) + 64q: a neighbour row is one 8-byte load per lane
 // and pair, and the per-edge scalars (neighbour id, edge vector) are read back as ONE broadcast 16-byte shared-memory load.
-#include "common.cuh"
+#include "fixed_point.cuh"
 
 namespace pvraft {
 
@@ -45,8 +45,10 @@ __device__ __forceinline__ unsigned long long sub2(unsigned long long a, unsigne
     return pk(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y));
 }
 
-template <int PAIRS>
-__global__ void __launch_bounds__(kEdgeThreads, PAIRS == 1 ? 6 : 4) k_setconv_edge_pairs(const float* __restrict__ fc1p, const int32_t* __restrict__ nbr,
+// DET: every point's per-channel (sum, sum^2) over its 32 edges enters a per-lane fixed-point register sum, and those enter the
+// [B,16] fixed-point workspace `stats` points at then (fixed_point.cuh): the sums do not depend on which CTA took which points
+template <int PAIRS, bool DET>
+__global__ void __launch_bounds__(kEdgeThreads, DET ? 2 : (PAIRS == 1 ? 6 : 4)) k_setconv_edge_pairs(const float* __restrict__ fc1p, const int32_t* __restrict__ nbr,
                                                                      const float* __restrict__ edge_feats, const float* __restrict__ w_fc1,
                                                                      int cin, int B, int N, int C, float* __restrict__ ymax,
                                                                      float* __restrict__ ymin, double* __restrict__ stats,
@@ -79,6 +81,13 @@ __global__ void __launch_bounds__(kEdgeThreads, PAIRS == 1 ? 6 : 4) k_setconv_ed
         double dS[PAIRS][2], dSS[PAIRS][2];
 #pragma unroll
         for (int q = 0; q < PAIRS; ++q) { dS[q][0] = dS[q][1] = 0.0; dSS[q][0] = dSS[q][1] = 0.0; }
+        Fx fS[PAIRS][2], fSS[PAIRS][2];
+        if constexpr (DET) {
+#pragma unroll
+            for (int q = 0; q < PAIRS; ++q)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) fS[q][h] = fSS[q][h] = Fx{0ull, 0ull, 0u};
+        }
         bool on[PAIRS];   // C need not fill the last group of 64 channels (encoder layers: 16, 48, 96)
         int coff[PAIRS];
 #pragma unroll
@@ -129,9 +138,37 @@ __global__ void __launch_bounds__(kEdgeThreads, PAIRS == 1 ? 6 : 4) k_setconv_ed
                     *reinterpret_cast<float2*>(ymin + o) = mn[q];
                 }
                 const float2 a1 = upk(s1[q]), a2 = upk(s2[q]);
+                if constexpr (DET) {
+                    fx_add(fS[q][0], fx_from((double)a1.x)); fx_add(fS[q][1], fx_from((double)a1.y));
+                    fx_add(fSS[q][0], fx_from((double)a2.x)); fx_add(fSS[q][1], fx_from((double)a2.y));
+                } else {
                 dS[q][0] += (double)a1.x; dS[q][1] += (double)a1.y;
                 dSS[q][0] += (double)a2.x; dSS[q][1] += (double)a2.y;
+                }
             }
+        }
+        if constexpr (DET) {   // lanes -> the CTA's shared slots -> one global addition per (group, moment)
+            __shared__ unsigned long long s_fx[16 * kFxWords];
+            __syncthreads();
+            if (threadIdx.x < 16 * kFxWords) s_fx[threadIdx.x] = 0ull;
+            __syncthreads();
+            const int gsz = C / PVRAFT_GN_GROUPS;
+#pragma unroll
+            for (int q = 0; q < PAIRS; ++q)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    if (on[q]) {
+                        const int g = (2 * lane + 64 * q + h) / gsz;
+                        fx_atomic(s_fx + (g * 2) * kFxWords, fS[q][h]);
+                        fx_atomic(s_fx + (g * 2 + 1) * kFxWords, fSS[q][h]);
+                    }
+            __syncthreads();
+            if (threadIdx.x < 16) {
+                const Fx v{s_fx[threadIdx.x * kFxWords], s_fx[threadIdx.x * kFxWords + 1], (unsigned)s_fx[threadIdx.x * kFxWords + 2]};
+                fx_atomic(reinterpret_cast<unsigned long long*>(stats) + ((size_t)b * 16 + threadIdx.x) * kFxWords, v);
+            }
+            seg = seg_end;
+            continue;
         }
         // block reduction of the per-channel partials -> per-group sums -> one atomic per (group, moment)
         __syncthreads();
@@ -161,9 +198,10 @@ __global__ void __launch_bounds__(kEdgeThreads, PAIRS == 1 ? 6 : 4) k_setconv_ed
 
 using namespace pvraft;
 
-extern "C" int pvraft_setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
-                                       int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order, void* stream) {
-    if (!fc1p || !nbr || !edge_feats || !w_fc1 || !ymax || !ymin || !stats) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: null pointer");
+template <bool DET>
+static int setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin, int B, int N, int C,
+                            float* ymax, float* ymin, double* stats, const int32_t* order, void* ws, void* stream) {
+    if (!fc1p || !nbr || !edge_feats || !w_fc1 || !ymax || !ymin || !stats || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: null pointer");
     if (B <= 0 || N <= 0 || cin <= 0) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: bad shape");
     if (C <= 0 || C > 128 || C % PVRAFT_GN_GROUPS) return fail(PVRAFT_ERR_UNSUPPORTED, "setconv_edge: C=%d (multiple of 8, <= 128)", C);
     const long long total = (long long)B * N;
@@ -172,13 +210,23 @@ extern "C" int pvraft_setconv_edge_fwd(const float* fc1p, const int32_t* nbr, co
     if (g > need) g = need;
     const int grid = (int)(g < 1 ? 1 : g);
     cudaStream_t st = (cudaStream_t)stream;
-    if (C <= 64) {
-        launch_pdl(k_setconv_edge_pairs<1>, grid, kEdgeThreads, 0, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order);
-        return check_launch("setconv_edge");
-    }
-    if (C <= 128) {
-        launch_pdl(k_setconv_edge_pairs<2>, grid, kEdgeThreads, 0, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order);
-        return check_launch("setconv_edge");
-    }
-    return fail(PVRAFT_ERR_UNSUPPORTED, "setconv_edge: C=%d", C);
+    double* kstats = DET ? static_cast<double*>(ws) : stats;
+    if (C <= 64) launch_pdl(k_setconv_edge_pairs<1, DET>, grid, kEdgeThreads, 0, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, kstats, order);
+    else launch_pdl(k_setconv_edge_pairs<2, DET>, grid, kEdgeThreads, 0, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, kstats, order);
+    const int rc = check_launch("setconv_edge");
+    if (rc || !DET) return rc;
+    return fx_flush_f64(static_cast<const unsigned long long*>(ws), 1, (long long)B * 16, (long long)B * 16, 0, stats, st);
+}
+
+extern "C" int pvraft_setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
+                                       int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order, void* stream) {
+    return setconv_edge_fwd<false>(fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order, nullptr, stream);
+}
+
+extern "C" int64_t pvraft_setconv_edge_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
+
+extern "C" int pvraft_setconv_edge_det_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
+                                           int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order, void* workspace,
+                                           void* stream) {
+    return setconv_edge_fwd<true>(fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order, workspace, stream);
 }

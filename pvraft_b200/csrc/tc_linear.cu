@@ -23,6 +23,7 @@
 #include <cuda.h>
 #include <stdlib.h>
 
+#include "fixed_point.cuh"
 #include "wgmma.cuh"
 
 namespace pvraft {
@@ -161,6 +162,9 @@ __device__ __forceinline__ void stage_load16(float* __restrict__ stg, int lane, 
 __device__ __forceinline__ float tsigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 
 // epilogue of the accumulator tile s_acc [128 rows][pitch]: thread = point (row quad * 32 + lane)
+// DET: the tile's (sum, sum^2) per group -- fixed-order sums over its 128 rows -- enter p.out_stats, which then points at the
+// [B,16] fixed-point workspace (fixed_point.cuh), as exact additions
+template <bool DET>
 __device__ __forceinline__ void tc_epilogue(const TcParams& p, float* __restrict__ s_acc, int pitch, int quad, int half, int lane, int row0,
                                             int sample, const float* __restrict__ s_bias, float* __restrict__ s_stage, float* __restrict__ s_part) {
     const int row = row0 + quad * 32 + lane;
@@ -250,9 +254,19 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, float* __restrict
                     a2 += __shfl_xor_sync(kFull, a2, o);
                 }
                 if ((t & (gsz - 1)) == 0 && t < p.cout) {
+                    if constexpr (DET) {
+                        unsigned long long* fx = reinterpret_cast<unsigned long long*>(p.out_stats) + ((size_t)sample * 16 + (t / gsz) * 2) * kFxWords;
+                        fx_atomic(fx, a1);
+                        fx_atomic(fx + kFxWords, a2);
+                    } else {
                     atomicAdd(p.out_stats + (size_t)sample * 16 + (t / gsz) * 2 + 0, a1);
                     atomicAdd(p.out_stats + (size_t)sample * 16 + (t / gsz) * 2 + 1, a2);
+                    }
                 }
+            } else if (DET && t < p.cout) {
+                unsigned long long* fx = reinterpret_cast<unsigned long long*>(p.out_stats) + ((size_t)sample * 16 + (t / gsz) * 2) * kFxWords;
+                fx_atomic(fx, a1);
+                fx_atomic(fx + kFxWords, a2);
             } else if (t < p.cout) {
                 atomicAdd(p.out_stats + (size_t)sample * 16 + (t / gsz) * 2 + 0, a1);
                 atomicAdd(p.out_stats + (size_t)sample * 16 + (t / gsz) * 2 + 1, a2);
@@ -385,7 +399,7 @@ __device__ __forceinline__ void tc_mma_kblock(float (&acc)[64], unsigned long lo
 __host__ __device__ __forceinline__ int tc_acc_pitch(int n) { return ((n + 31) & ~31) + 4; }
 
 // NT = p.N (the padded cout): the wgmma shape is part of the instruction
-template <int NT>
+template <int NT, bool DET>
 __global__ void __launch_bounds__(kTcThreads, 1)
 k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
             const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
@@ -591,7 +605,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
             tmbar_wait(&s_acc_full, (unsigned)ti & 1u);
             TC_MARK(threadIdx.x == 0 && ti < 4, 24 + ti);
             const int sample = row0 / p.pts_per_sample;
-            tc_epilogue(p, s_acc, acc_pitch, quad, half, lane, row0, sample, s_bias, s_estage, s_part);
+            tc_epilogue<DET>(p, s_acc, acc_pitch, quad, half, lane, row0, sample, s_bias, s_estage, s_part);
             __syncwarp();
             if (lane == 0) tmbar_arrive(&s_acc_empty);   // one arrival per epilogue warp
             TC_MARK(threadIdx.x == 0 && ti < 4, 28 + ti);
@@ -659,8 +673,9 @@ extern "C" int pvraft_tc_weight_split(const float* w, int rows, int cols, int ld
     return check_launch("tc_weight_split");
 }
 
-extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream) {
-    if (!a || !a->in[0] || !a->w_hi || !a->w_lo || !a->out) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: null pointer");
+template <bool DET>
+static int tc_linear_fwd(const pvraft_tc_linear_args* a, void* ws, void* stream) {
+    if (!a || !a->in[0] || !a->w_hi || !a->w_lo || !a->out || (DET && a->out_stats && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: null pointer");
     if (a->B <= 0 || a->N <= 0 || a->n_pad < 16 || a->n_pad > 128 || a->n_pad % 16) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: bad shape (n_pad=%d)", a->n_pad);
     if (a->N % kTcM) return fail(PVRAFT_ERR_UNSUPPORTED, "tc_linear: points per sample (%d) must be a multiple of 128", a->N);
     int K = 0;
@@ -683,7 +698,7 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     p.in_stats = a->in_stats; p.in_gamma = a->in_gamma; p.in_beta = a->in_beta; p.in_count = a->in_count; p.in_act = a->in_act;
     p.in_slope = a->in_slope; p.minmax = a->in_min != nullptr;
     p.epi = a->epilogue; p.bias = a->bias; p.bias2 = a->bias2; p.out_act = a->out_act; p.residual = a->residual; p.out = a->out;
-    p.out2 = a->out2; p.h = a->h; p.z = a->z; p.out_stats = a->out_stats;
+    p.out2 = a->out2; p.h = a->h; p.z = a->z; p.out_stats = DET && a->out_stats ? static_cast<double*>(ws) : a->out_stats;
     p.M = (int)M; p.N = a->n_pad; p.K = K; p.cout = a->cout; p.pts_per_sample = a->N;
     CUtensorMap mw_hi, mw_lo;
     int rc;
@@ -722,16 +737,16 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     p.stages = stages;
     if (const char* e = getenv("PVRAFT_TC_DBG")) p.dbg = atoi(e);
     const size_t smem = stages * stage + (p.w_resident ? w_all : 0) + fixed;
-    decltype(&k_tc_linear<16>) kernel = nullptr;
+    decltype(&k_tc_linear<16, DET>) kernel = nullptr;
     switch (a->n_pad) {
-        case 16: kernel = k_tc_linear<16>; break;
-        case 32: kernel = k_tc_linear<32>; break;
-        case 48: kernel = k_tc_linear<48>; break;
-        case 64: kernel = k_tc_linear<64>; break;
-        case 80: kernel = k_tc_linear<80>; break;
-        case 96: kernel = k_tc_linear<96>; break;
-        case 112: kernel = k_tc_linear<112>; break;
-        default: kernel = k_tc_linear<128>; break;
+        case 16: kernel = k_tc_linear<16, DET>; break;
+        case 32: kernel = k_tc_linear<32, DET>; break;
+        case 48: kernel = k_tc_linear<48, DET>; break;
+        case 64: kernel = k_tc_linear<64, DET>; break;
+        case 80: kernel = k_tc_linear<80, DET>; break;
+        case 96: kernel = k_tc_linear<96, DET>; break;
+        case 112: kernel = k_tc_linear<112, DET>; break;
+        default: kernel = k_tc_linear<128, DET>; break;
     }
     if ((rc = opt_in_smem(kernel, smem))) return rc;
     const long long n_tiles = (M + kTcM - 1) / kTcM;
@@ -739,5 +754,15 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream
     // launched with programmatic stream serialization: the kernel's prologue may start while the previous kernel drains
     const cudaError_t le = launch_pdl(kernel, grid, kTcThreads, smem, (cudaStream_t)stream, mw_hi, mw_lo, ma[0], ma[1], ma[2], mmin, p);
     if (le != cudaSuccess) return fail((int)le, "tc_linear: launch failed: %s", cudaGetErrorString(le));
-    return check_launch("tc_linear");
+    rc = check_launch("tc_linear");
+    if (rc || !DET || !a->out_stats) return rc;
+    return fx_flush_f64(static_cast<const unsigned long long*>(ws), 1, (long long)a->B * 16, (long long)a->B * 16, 0, a->out_stats, (cudaStream_t)stream);
+}
+
+extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream) { return tc_linear_fwd<false>(a, nullptr, stream); }
+
+extern "C" int64_t pvraft_tc_linear_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
+
+extern "C" int pvraft_tc_linear_det_fwd(const pvraft_tc_linear_args* a, void* workspace, void* stream) {
+    return tc_linear_fwd<true>(a, workspace, stream);
 }

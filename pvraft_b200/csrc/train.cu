@@ -6,8 +6,11 @@
 // The training path runs layer by layer (pvraft_b200/train.py wraps each entry point in a torch.autograd.Function); every
 // arithmetic step of forward and backward is one of the kernels of this library.  Layout conventions as in the forward
 // kernels: per-point features point-major [B,rows,C]; "rows" is N for per-point layers and N*32 for per-edge layers.
-// Reductions into parameter gradients use fp32 / fp64 atomics (order-nondeterministic, like ATen's own CUDA backward).
-#include "common.cuh"
+// Reductions into parameter gradients use fp32 / fp64 atomics (order-nondeterministic, like ATen's own CUDA backward) in
+// the default instantiations.  The DET instantiations (the *_det entry points) add exact fixed-point values instead
+// (fixed_point.cuh) and size their grids from the shapes alone, so their results are bitwise reproducible; their
+// accumulator arguments then point at the caller's fixed-point workspace.
+#include "fixed_point.cuh"
 
 namespace pvraft {
 
@@ -20,6 +23,7 @@ namespace pvraft {
 constexpr int kWgRows = 64;
 constexpr int kWgThreads = 256;
 
+template <bool DET>
 __global__ void __launch_bounds__(kWgThreads) k_linear_wgrad(const float* __restrict__ x, const float* __restrict__ dy, long long rows,
                                                              int cin, int cout, float* __restrict__ dW, int dw_ld, float* __restrict__ db) {
     extern __shared__ __align__(16) float smem_wg[];
@@ -87,9 +91,15 @@ __global__ void __launch_bounds__(kWgThreads) k_linear_wgrad(const float* __rest
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int ii = ib * 4 + i;
-                    if (ii < cin && acc[t][o * 4 + i] != 0.f) atomicAdd(dW + (size_t)oo * dw_ld + ii, acc[t][o * 4 + i]);
+                    if (ii < cin && acc[t][o * 4 + i] != 0.f) {
+                        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dW) + ((size_t)oo * cin + ii) * kFxWords, (double)acc[t][o * 4 + i]);
+                        else atomicAdd(dW + (size_t)oo * dw_ld + ii, acc[t][o * 4 + i]);
+                    }
                 }
-                if (db && ib == 0 && accb[t][o] != 0.f) atomicAdd(db + oo, accb[t][o]);
+                if (db && ib == 0 && accb[t][o] != 0.f) {
+                    if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(db) + (size_t)oo * kFxWords, (double)accb[t][o]);
+                    else atomicAdd(db + oo, accb[t][o]);
+                }
             }
         }
     }
@@ -101,7 +111,7 @@ __global__ void __launch_bounds__(kWgThreads) k_linear_wgrad(const float* __rest
 // generic pair (k_linear with the transposed weight + k_linear_wgrad) reads dy twice and keeps 8 of 256 threads busy in
 // the weight-gradient tile loop at this shape.  LPR lanes share a row, 16 output channels each (cout = 16 * LPR).
 // ---------------------------------------------------------------------------------------------------------------------
-template <int LPR>
+template <int LPR, bool DET>
 __global__ void __launch_bounds__(256) k_linear_bwd_small(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ W,
                                                           long long rows, int cin, int w_ld, float* __restrict__ dW, int dw_ld,
                                                           float* __restrict__ db, float* __restrict__ dx) {
@@ -194,11 +204,20 @@ __global__ void __launch_bounds__(256) k_linear_bwd_small(const float* __restric
             }
         }
         if (rr == 0) {
+            if constexpr (DET) {   // every warp's sums straight into the fixed-point slots [COUT][cin] | [COUT]
+                unsigned long long* fx = reinterpret_cast<unsigned long long*>(dW);
 #pragma unroll
-            for (int k = 0; k < 4; ++k) atomicAdd(&s_acc[q * 16 + o][k], acc[o][k]);
-            atomicAdd(&s_acc[q * 16 + o][4], accb[o]);
+                for (int k = 0; k < 4; ++k)
+                    if (k < cin) fx_atomic(fx + ((size_t)(q * 16 + o) * cin + k) * kFxWords, (double)acc[o][k]);
+                if (db) fx_atomic(reinterpret_cast<unsigned long long*>(db) + (size_t)(q * 16 + o) * kFxWords, (double)accb[o]);
+            } else {
+#pragma unroll
+                for (int k = 0; k < 4; ++k) atomicAdd(&s_acc[q * 16 + o][k], acc[o][k]);
+                atomicAdd(&s_acc[q * 16 + o][4], accb[o]);
+            }
         }
     }
+    if constexpr (DET) return;
     __syncthreads();
     for (int i = threadIdx.x; i < COUT * 5; i += blockDim.x) {
         const int o = i / 5, k = i - o * 5;
@@ -246,12 +265,25 @@ __device__ __forceinline__ void gn_mean_rstd(const double* st, double count, flo
     rstd = (float)rsqrt(var + 1e-5);
 }
 
+// DET: a CTA's fixed-point slots -> the workspace [B*16 gsum | C dgamma | C dbeta | 1 dslope] (p.gsum points at it)
+__device__ __forceinline__ void gn_bwd_flush_fx(const GnBwdParams& p, const unsigned long long* s_fx, int b) {
+    unsigned long long* ws = reinterpret_cast<unsigned long long*>(p.gsum);
+    for (int i = threadIdx.x; i < 16 + 2 * p.C + 1; i += blockDim.x) {
+        const Fx v{s_fx[i * kFxWords], s_fx[i * kFxWords + 1], (unsigned)s_fx[i * kFxWords + 2]};
+        if (!v.lo && !v.hi && !v.bad) continue;
+        fx_atomic(ws + (size_t)(i < 16 ? b * 16 + i : p.B * 16 + (i - 16)) * kFxWords, v);
+    }
+}
+
+template <bool DET>
 __global__ void __launch_bounds__(256) k_gn_bwd_reduce(const GnBwdParams pp) {
     GnBwdParams p = pp;
     if (p.slope_dev) p.slope = __ldg(p.slope_dev);
     __shared__ double s_g[8][2];
     __shared__ double s_par[3];   // unused slots keep the layout simple
     __shared__ double s_ch[2][256];   // dgamma | dbeta of this CTA: ONE global atomic per channel and CTA
+    unsigned long long* s_fx = nullptr;   // DET: [16 gsum | C dgamma | C dbeta | dslope] fixed-point slots of this CTA
+    if constexpr (DET) { __shared__ unsigned long long s_fx_[(16 + 2 * 256 + 1) * kFxWords]; s_fx = s_fx_; }
     const int b = blockIdx.y;
     const int C = p.C, gsz = C / PVRAFT_GN_GROUPS;
     const int rpp = blockDim.x / C;   // rows per pass
@@ -261,6 +293,8 @@ __global__ void __launch_bounds__(256) k_gn_bwd_reduce(const GnBwdParams pp) {
     if (threadIdx.x < 3) s_par[threadIdx.x] = 0.0;
     s_ch[0][threadIdx.x] = 0.0;
     s_ch[1][threadIdx.x] = 0.0;
+    if constexpr (DET)
+        for (int i = threadIdx.x; i < (16 + 2 * C + 1) * kFxWords; i += blockDim.x) s_fx[i] = 0ull;
     __syncthreads();
     const int g = c / gsz;
     float mean, rstd;
@@ -284,13 +318,25 @@ __global__ void __launch_bounds__(256) k_gn_bwd_reduce(const GnBwdParams pp) {
             if (++pend == 32) { a0 += f0; a1 += f1; dg += fg; dbt += fb; dsl += fs; f0 = f1 = fg = fb = fs = 0.f; pend = 0; }
         }
         a0 += f0; a1 += f1; dg += fg; dbt += fb; dsl += fs;
+        if constexpr (DET) {
+            fx_atomic(s_fx + (g * 2) * kFxWords, a0);
+            fx_atomic(s_fx + (g * 2 + 1) * kFxWords, a1);
+            fx_atomic(s_fx + (16 + c) * kFxWords, dg);
+            fx_atomic(s_fx + (16 + C + c) * kFxWords, dbt);
+            if (p.dslope && dsl != 0.0) fx_atomic(s_fx + (16 + 2 * C) * kFxWords, dsl);
+        } else {
         atomicAdd(&s_g[g][0], a0);
         atomicAdd(&s_g[g][1], a1);
         atomicAdd(&s_ch[0][c], dg);
         atomicAdd(&s_ch[1][c], dbt);
         if (p.dslope && dsl != 0.0) atomicAdd(&s_par[0], dsl);
+        }
     }
     __syncthreads();
+    if constexpr (DET) {
+        gn_bwd_flush_fx(p, s_fx, b);
+        return;
+    }
     if (threadIdx.x < 16) {
         const double v = (&s_g[0][0])[threadIdx.x];
         if (v != 0.0) atomicAdd(p.gsum + (size_t)b * 16 + threadIdx.x, v);
@@ -331,12 +377,15 @@ __global__ void __launch_bounds__(256) k_gn_bwd_apply(const GnBwdParams pp) {
 // The same two passes when the activation was followed by a max over each point's 32 consecutive rows (GnActMaxFn): only the
 // arg-max row of a (point, channel) carries gradient, so pass 1 gathers ONE x per (point, channel) -- 1/32 of the tensor -- and
 // pass 2 streams x -> dx in 16-byte pieces with the point's (arg, dy) held in registers across its 32 rows.
+template <bool DET>
 __global__ void __launch_bounds__(256) k_gn_bwd_reduce_arg(const GnBwdParams pp) {
     GnBwdParams p = pp;
     if (p.slope_dev) p.slope = __ldg(p.slope_dev);
     __shared__ double s_g[8][2];
     __shared__ double s_par;
     __shared__ double s_ch[2][256];
+    unsigned long long* s_fx = nullptr;   // DET: as in k_gn_bwd_reduce
+    if constexpr (DET) { __shared__ unsigned long long s_fx_[(16 + 2 * 256 + 1) * kFxWords]; s_fx = s_fx_; }
     const int b = blockIdx.y;
     const int C = p.C, gsz = C / PVRAFT_GN_GROUPS;
     const int ppp = blockDim.x / C;   // points per pass
@@ -345,6 +394,8 @@ __global__ void __launch_bounds__(256) k_gn_bwd_reduce_arg(const GnBwdParams pp)
     if (threadIdx.x == 0) s_par = 0.0;
     s_ch[0][threadIdx.x] = 0.0;
     s_ch[1][threadIdx.x] = 0.0;
+    if constexpr (DET)
+        for (int i = threadIdx.x; i < (16 + 2 * C + 1) * kFxWords; i += blockDim.x) s_fx[i] = 0ull;
     __syncthreads();
     const int g = c / gsz;
     float mean, rstd;
@@ -369,13 +420,25 @@ __global__ void __launch_bounds__(256) k_gn_bwd_reduce_arg(const GnBwdParams pp)
             if (++pend == 32) { a0 += f0; a1 += f1; dg += fg; dbt += fb; dsl += fs; f0 = f1 = fg = fb = fs = 0.f; pend = 0; }
         }
         a0 += f0; a1 += f1; dg += fg; dbt += fb; dsl += fs;
+        if constexpr (DET) {
+            fx_atomic(s_fx + (g * 2) * kFxWords, a0);
+            fx_atomic(s_fx + (g * 2 + 1) * kFxWords, a1);
+            fx_atomic(s_fx + (16 + c) * kFxWords, dg);
+            fx_atomic(s_fx + (16 + C + c) * kFxWords, dbt);
+            if (p.dslope && dsl != 0.0) fx_atomic(s_fx + (16 + 2 * C) * kFxWords, dsl);
+        } else {
         atomicAdd(&s_g[g][0], a0);
         atomicAdd(&s_g[g][1], a1);
         atomicAdd(&s_ch[0][c], dg);
         atomicAdd(&s_ch[1][c], dbt);
         if (p.dslope && dsl != 0.0) atomicAdd(&s_par, dsl);
+        }
     }
     __syncthreads();
+    if constexpr (DET) {
+        gn_bwd_flush_fx(p, s_fx, b);
+        return;
+    }
     if (threadIdx.x < 16) {
         const double v = (&s_g[0][0])[threadIdx.x];
         if (v != 0.0) atomicAdd(p.gsum + (size_t)b * 16 + threadIdx.x, v);
@@ -467,13 +530,18 @@ __global__ void __launch_bounds__(256) k_gn_act_maxk(const float* __restrict__ x
 //   backward  dP[b,nbr,:] += dT[b,n,j,:],  dP[b,n,:] -= sum_j dT[b,n,j,:]   (dE = dT)
 // One warp per point; lanes stride over the channels.
 // ---------------------------------------------------------------------------------------------------------------------
+template <bool DET>
 __global__ void __launch_bounds__(256) k_edge_fwd(const float* __restrict__ P, const int32_t* __restrict__ nbr, float* __restrict__ E,
                                                   int B, int N, int C, double* __restrict__ stats) {
     __shared__ double s_g[16];
     const int lane = lane_id(), w = warp_id();
     const long long pt = (long long)blockIdx.x * 8 + w;
     const int b0 = (int)(((long long)blockIdx.x * 8) / N);   // a CTA's 8 points may straddle two samples
+    unsigned long long* s_fx = nullptr;   // DET: fixed-point [16] of the CTA's first sample; `stats` is the [B,16] workspace
+    if constexpr (DET) { __shared__ unsigned long long s_fx_[16 * kFxWords]; s_fx = s_fx_; }
     if (threadIdx.x < 16) s_g[threadIdx.x] = 0.0;
+    if constexpr (DET)
+        if (threadIdx.x < 16 * kFxWords) s_fx[threadIdx.x] = 0ull;
     __syncthreads();
     const int gsz = C / PVRAFT_GN_GROUPS;
     if (pt < (long long)B * N) {
@@ -491,7 +559,12 @@ __global__ void __launch_bounds__(256) k_edge_fwd(const float* __restrict__ P, c
                 s += t;
                 ss += t * t;
             }
-            if (stats) {
+            if (DET && stats) {   // one (point, channel) sum of 32 neighbours per contribution
+                unsigned long long* gfx = reinterpret_cast<unsigned long long*>(stats) + (size_t)b * 16 * kFxWords;
+                unsigned long long* dst = b == b0 ? s_fx : gfx;
+                fx_atomic(dst + ((c / gsz) * 2) * kFxWords, (double)s);
+                fx_atomic(dst + ((c / gsz) * 2 + 1) * kFxWords, (double)ss);
+            } else if (stats) {
                 if (b == b0) {
                     atomicAdd(&s_g[(c / gsz) * 2], (double)s);
                     atomicAdd(&s_g[(c / gsz) * 2 + 1], (double)ss);
@@ -503,9 +576,17 @@ __global__ void __launch_bounds__(256) k_edge_fwd(const float* __restrict__ P, c
         }
     }
     __syncthreads();
+    if constexpr (DET) {
+        if (stats && threadIdx.x < 16) {
+            const Fx v{s_fx[threadIdx.x * kFxWords], s_fx[threadIdx.x * kFxWords + 1], (unsigned)s_fx[threadIdx.x * kFxWords + 2]};
+            fx_atomic(reinterpret_cast<unsigned long long*>(stats) + ((size_t)b0 * 16 + threadIdx.x) * kFxWords, v);
+        }
+        return;
+    }
     if (stats && threadIdx.x < 16 && s_g[threadIdx.x] != 0.0) atomicAdd(stats + (size_t)b0 * 16 + threadIdx.x, s_g[threadIdx.x]);
 }
 
+template <bool DET>
 __global__ void __launch_bounds__(256) k_edge_bwd(const float* __restrict__ dT, const int32_t* __restrict__ nbr, int B, int N, int C,
                                                   float* __restrict__ dP) {
     const int lane = lane_id(), w = warp_id();
@@ -519,9 +600,11 @@ __global__ void __launch_bounds__(256) k_edge_bwd(const float* __restrict__ dT, 
             const int nb = __ldg(nbr + pt * PVRAFT_KNN + j);
             const float g = __ldg(dT + ((size_t)pt * PVRAFT_KNN + j) * C + c);
             s += g;
-            atomicAdd(dPb + (size_t)nb * C + c, g);
+            if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dP) + ((size_t)b * N * C + (size_t)nb * C + c) * kFxWords, (double)g);
+            else atomicAdd(dPb + (size_t)nb * C + c, g);
         }
-        atomicAdd(dP + (size_t)pt * C + c, -s);
+        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dP) + ((size_t)pt * C + c) * kFxWords, -(double)s);
+        else atomicAdd(dP + (size_t)pt * C + c, -s);
     }
 }
 
@@ -632,7 +715,7 @@ __global__ void __launch_bounds__(256) k_lookup_bwd(const LookupBwdParams p) {
 //   d f1[b,n,:] = (1/sqrt(C)) sum_k g[b,n,k] f2[b,idx[b,n,k],:]      d f2[b,m,:] += (1/sqrt(C)) g[b,n,k] f1[b,n,:]  (m = idx[b,n,k])
 // One warp per row; lanes own C/32 (<= 8) consecutive channels.
 // ---------------------------------------------------------------------------------------------------------------------
-template <int CPL>
+template <int CPL, bool DET>
 __global__ void __launch_bounds__(256) k_corr_init_bwd(const float* __restrict__ g, const int32_t* __restrict__ idx, const float* __restrict__ f1,
                                                        const float* __restrict__ f2, int B, int N, int K, float scale, float* __restrict__ d_f1,
                                                        float* __restrict__ d_f2) {
@@ -654,7 +737,14 @@ __global__ void __launch_bounds__(256) k_corr_init_bwd(const float* __restrict__
             const float gj = __shfl_sync(kFull, gk, j);
             const int m = __shfl_sync(kFull, ik, j);
             if (gj == 0.f) continue;
-            if constexpr (CPL == 4) {   // the model's C = 128: one 128-bit load and one vector reduction per lane
+            if constexpr (DET) {   // d_f2 is the fixed-point workspace [B,N,C]
+                unsigned long long* fx = reinterpret_cast<unsigned long long*>(d_f2) + ((size_t)b * N + m) * C * kFxWords;
+#pragma unroll
+                for (int i = 0; i < CPL; ++i) {
+                    acc[i] = fmaf(gj, __ldg(f2b + (size_t)m * C + lane * CPL + i), acc[i]);
+                    fx_atomic(fx + (size_t)(lane * CPL + i) * kFxWords, (double)(gj * a[i]));
+                }
+            } else if constexpr (CPL == 4) {   // the model's C = 128: one 128-bit load and one vector reduction per lane
                 const float4 v = __ldg(reinterpret_cast<const float4*>(f2b + (size_t)m * C) + lane);
                 acc[0] = fmaf(gj, v.x, acc[0]); acc[1] = fmaf(gj, v.y, acc[1]); acc[2] = fmaf(gj, v.z, acc[2]); acc[3] = fmaf(gj, v.w, acc[3]);
                 atomicAdd(reinterpret_cast<float4*>(d2b + (size_t)m * C) + lane, make_float4(gj * a[0], gj * a[1], gj * a[2], gj * a[3]));
@@ -675,26 +765,53 @@ __global__ void __launch_bounds__(256) k_corr_init_bwd(const float* __restrict__
 
 using namespace pvraft;
 
-extern "C" int pvraft_linear_wgrad(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
-                                   void* stream) {
-    if (!x || !dy || !dW || rows <= 0 || cin <= 0 || cout <= 0) return fail(PVRAFT_ERR_BAD_ARG, "linear_wgrad: bad argument");
+template <bool DET>
+static int linear_wgrad(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db, void* ws,
+                        void* stream) {
+    if (!x || !dy || !dW || rows <= 0 || cin <= 0 || cout <= 0 || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "linear_wgrad: bad argument");
     if (cin > 256 || cout > 128) return fail(PVRAFT_ERR_UNSUPPORTED, "linear_wgrad: cin=%d cout=%d (max 256/128)", cin, cout);
     const int cin_p = (cin + 3) & ~3;
     if (8 * (cin_p >> 2) > 2 * kWgThreads) return fail(PVRAFT_ERR_UNSUPPORTED, "linear_wgrad: cin=%d", cin);
     const size_t smem = sizeof(float) * ((size_t)kWgRows * (cin_p + 4) + (size_t)kWgRows * 36);
     int rc;
-    if ((rc = opt_in_smem(k_linear_wgrad, smem))) return rc;
+    if ((rc = opt_in_smem(k_linear_wgrad<DET>, smem))) return rc;
     long long workers = (rows + kWgRows - 1) / kWgRows;
-    const long long cap = (long long)sm_count() * 2;
+    const long long cap = DET ? kDetCtas : (long long)sm_count() * 2;
     if (workers > cap) workers = cap;
     dim3 grid((unsigned)workers, (unsigned)((cout + 31) / 32));
-    k_linear_wgrad<<<grid, kWgThreads, smem, (cudaStream_t)stream>>>(x, dy, rows, cin, cout, dW, dw_ld > 0 ? dw_ld : cin, db);
+    const int ld = dw_ld > 0 ? dw_ld : cin;
+    cudaStream_t st = (cudaStream_t)stream;
+    if constexpr (DET) {
+        unsigned long long* fx = static_cast<unsigned long long*>(ws);
+        unsigned long long* fxb = fx + (size_t)cout * cin * kFxWords;
+        k_linear_wgrad<true><<<grid, kWgThreads, smem, st>>>(x, dy, rows, cin, cout, reinterpret_cast<float*>(fx), ld,
+                                                             db ? reinterpret_cast<float*>(fxb) : nullptr);
+        if ((rc = check_launch("linear_wgrad"))) return rc;
+        if ((rc = fx_flush_f32(fx, cout, cin, cin, ld, dW, st))) return rc;
+        return db ? fx_flush_f32(fxb, 1, cout, cout, cout, db, st) : 0;
+    }
+    k_linear_wgrad<false><<<grid, kWgThreads, smem, st>>>(x, dy, rows, cin, cout, dW, ld, db);
     return check_launch("linear_wgrad");
 }
 
-extern "C" int pvraft_linear_bwd_small(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld, float* dW,
-                                       int dw_ld, float* db, float* dx, void* stream) {
-    if (!x || !dy || !W || !dW || rows <= 0) return fail(PVRAFT_ERR_BAD_ARG, "linear_bwd_small: bad argument");
+extern "C" int pvraft_linear_wgrad(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
+                                   void* stream) {
+    return linear_wgrad<false>(x, dy, rows, cin, cout, dW, dw_ld, db, nullptr, stream);
+}
+
+extern "C" int64_t pvraft_linear_wgrad_det_workspace_bytes(int cin, int cout) {
+    return (int64_t)((int64_t)cout * cin + cout) * kFxWords * 8;
+}
+
+extern "C" int pvraft_linear_wgrad_det(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
+                                       void* workspace, void* stream) {
+    return linear_wgrad<true>(x, dy, rows, cin, cout, dW, dw_ld, db, workspace, stream);
+}
+
+template <bool DET>
+static int linear_bwd_small(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld, float* dW, int dw_ld,
+                            float* db, float* dx, void* ws, void* stream) {
+    if (!x || !dy || !W || !dW || rows <= 0 || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "linear_bwd_small: bad argument");
     const int lpr = cout / 16;
     if (cin < 1 || cin > 4 || cout % 16 || !(lpr == 1 || lpr == 2 || lpr == 3 || lpr == 4 || lpr == 6 || lpr == 8))
         return fail(PVRAFT_ERR_UNSUPPORTED, "linear_bwd_small: cin=%d cout=%d (cin <= 4, cout in {16,32,48,64,96,128})", cin, cout);
@@ -702,11 +819,15 @@ extern "C" int pvraft_linear_bwd_small(const float* x, const float* dy, const fl
         return fail(PVRAFT_ERR_BAD_ARG, "linear_bwd_small: dy (and x, dx when cin == 4) must be 16-byte aligned");
     const int rpc = 8 * (32 / lpr);
     long long ctas = (rows + rpc - 1) / rpc;
-    const long long cap = (long long)sm_count();   // 152 registers x 256 threads: one resident CTA per SM
+    const long long cap = DET ? kDetCtas / 2 : (long long)sm_count();   // 152 registers x 256 threads: one resident CTA per SM
     if (ctas > cap) ctas = cap;
     const int wl = w_ld > 0 ? w_ld : cin, dl = dw_ld > 0 ? dw_ld : cin;
     cudaStream_t st = (cudaStream_t)stream;
-#define PVRAFT_LBS(L) k_linear_bwd_small<L><<<(unsigned)ctas, 256, 0, st>>>(x, dy, W, rows, cin, wl, dW, dl, db, dx)
+    unsigned long long* fx = static_cast<unsigned long long*>(ws);
+    unsigned long long* fxb = DET ? fx + (size_t)cout * cin * kFxWords : nullptr;
+    float* kdW = DET ? reinterpret_cast<float*>(fx) : dW;
+    float* kdb = DET ? (db ? reinterpret_cast<float*>(fxb) : nullptr) : db;
+#define PVRAFT_LBS(L) k_linear_bwd_small<L, DET><<<(unsigned)ctas, 256, 0, st>>>(x, dy, W, rows, cin, wl, kdW, dl, kdb, dx)
     switch (lpr) {
         case 1: PVRAFT_LBS(1); break;
         case 2: PVRAFT_LBS(2); break;
@@ -716,27 +837,58 @@ extern "C" int pvraft_linear_bwd_small(const float* x, const float* dy, const fl
         default: PVRAFT_LBS(8); break;
     }
 #undef PVRAFT_LBS
-    return check_launch("linear_bwd_small");
+    int rc = check_launch("linear_bwd_small");
+    if (rc || !DET) return rc;
+    if ((rc = fx_flush_f32(fx, cout, cin, cin, dl, dW, st))) return rc;
+    return db ? fx_flush_f32(fxb, 1, cout, cout, cout, db, st) : 0;
 }
 
-extern "C" int pvraft_gn_act_bwd(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta, double count,
-                                 int act, float slope, int B, int64_t rows, int C, double* gsum, double* dgamma, double* dbeta,
-                                 double* dslope, float* dx, const float* slope_dev, const uint8_t* arg, void* stream) {
-    if (!x || !dy || !stats || !gamma || !beta || !gsum || !dgamma || !dbeta || !dx) return fail(PVRAFT_ERR_BAD_ARG, "gn_act_bwd: null pointer");
+extern "C" int pvraft_linear_bwd_small(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld, float* dW,
+                                       int dw_ld, float* db, float* dx, void* stream) {
+    return linear_bwd_small<false>(x, dy, W, rows, cin, cout, w_ld, dW, dw_ld, db, dx, nullptr, stream);
+}
+
+extern "C" int64_t pvraft_linear_bwd_small_det_workspace_bytes(int cin, int cout) {
+    return (int64_t)((int64_t)cout * cin + cout) * kFxWords * 8;
+}
+
+extern "C" int pvraft_linear_bwd_small_det(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld,
+                                           float* dW, int dw_ld, float* db, float* dx, void* workspace, void* stream) {
+    return linear_bwd_small<true>(x, dy, W, rows, cin, cout, w_ld, dW, dw_ld, db, dx, workspace, stream);
+}
+
+template <bool DET>
+static int gn_act_bwd(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta, double count, int act,
+                      float slope, int B, int64_t rows, int C, double* gsum, double* dgamma, double* dbeta, double* dslope, float* dx,
+                      const float* slope_dev, const uint8_t* arg, void* ws, void* stream) {
+    if (!x || !dy || !stats || !gamma || !beta || !gsum || !dgamma || !dbeta || !dx || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "gn_act_bwd: null pointer");
     if (C > 256 || C % PVRAFT_GN_GROUPS || B <= 0 || rows <= 0) return fail(PVRAFT_ERR_UNSUPPORTED, "gn_act_bwd: C=%d", C);
     if (arg && rows % PVRAFT_KNN) return fail(PVRAFT_ERR_BAD_ARG, "gn_act_bwd: the max-pooled form needs rows %% 32 == 0");
     GnBwdParams p{x, dy, stats, gamma, beta, count, act, slope, (long long)rows, B, C, gsum, dgamma, dbeta, dslope, dx, slope_dev, arg};
-    const long long cap = ((long long)sm_count() * 8 + B - 1) / B;
+    GnBwdParams pr = p;   // the reducing pass: DET accumulates into the fixed-point workspace, flushed before the apply pass
+    if (DET) pr.gsum = static_cast<double*>(ws);
+    const long long cap = ((DET ? kDetCtas * 4 : (long long)sm_count() * 8) + B - 1) / B;
+    cudaStream_t st = (cudaStream_t)stream;
+    auto flush = [&]() -> int {
+        if (!DET) return 0;
+        const unsigned long long* fx = static_cast<const unsigned long long*>(ws);
+        int rc;
+        if ((rc = fx_flush_f64(fx, 1, (long long)B * 16, (long long)B * 16, 0, gsum, st))) return rc;
+        fx += (size_t)B * 16 * kFxWords;
+        if ((rc = fx_flush_f64(fx, 1, C, C, 0, dgamma, st))) return rc;
+        if ((rc = fx_flush_f64(fx + (size_t)C * kFxWords, 1, C, C, 0, dbeta, st))) return rc;
+        return dslope ? fx_flush_f64(fx + (size_t)2 * C * kFxWords, 1, 1, 1, 0, dslope, st) : 0;
+    };
     if (arg) {
         const long long pts = rows / PVRAFT_KNN;
         const int ppp_r = 256 / C, ppp_a = 256 / (C / 4);
         long long wr = (pts + ppp_r * 16 - 1) / (ppp_r * 16), wa = (pts + ppp_a - 1) / ppp_a;   // >= 16 points per reducing thread
         if (wr > cap) wr = cap;
         if (wa > cap) wa = cap;
-        k_gn_bwd_reduce_arg<<<dim3((unsigned)wr, (unsigned)B), 256, 0, (cudaStream_t)stream>>>(p);
+        k_gn_bwd_reduce_arg<DET><<<dim3((unsigned)wr, (unsigned)B), 256, 0, st>>>(pr);
         int rc = check_launch("gn_bwd_reduce_arg");
-        if (rc) return rc;
-        k_gn_bwd_apply_arg<<<dim3((unsigned)wa, (unsigned)B), 256, 0, (cudaStream_t)stream>>>(p);
+        if (rc || (rc = flush())) return rc;
+        k_gn_bwd_apply_arg<<<dim3((unsigned)wa, (unsigned)B), 256, 0, st>>>(p);
         return check_launch("gn_bwd_apply_arg");
     }
     const int rpp = 256 / C;
@@ -744,11 +896,30 @@ extern "C" int pvraft_gn_act_bwd(const float* x, const float* dy, const double* 
     if (workers > cap) workers = cap;
     if (wr > cap) wr = cap;
     dim3 grid((unsigned)workers, (unsigned)B);
-    k_gn_bwd_reduce<<<dim3((unsigned)wr, (unsigned)B), 256, 0, (cudaStream_t)stream>>>(p);
+    k_gn_bwd_reduce<DET><<<dim3((unsigned)wr, (unsigned)B), 256, 0, st>>>(pr);
     int rc = check_launch("gn_bwd_reduce");
-    if (rc) return rc;
-    k_gn_bwd_apply<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
+    if (rc || (rc = flush())) return rc;
+    k_gn_bwd_apply<<<grid, 256, 0, st>>>(p);
     return check_launch("gn_bwd_apply");
+}
+
+extern "C" int pvraft_gn_act_bwd(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta, double count,
+                                 int act, float slope, int B, int64_t rows, int C, double* gsum, double* dgamma, double* dbeta,
+                                 double* dslope, float* dx, const float* slope_dev, const uint8_t* arg, void* stream) {
+    return gn_act_bwd<false>(x, dy, stats, gamma, beta, count, act, slope, B, rows, C, gsum, dgamma, dbeta, dslope, dx, slope_dev, arg,
+                             nullptr, stream);
+}
+
+extern "C" int64_t pvraft_gn_act_bwd_det_workspace_bytes(int B, int C) {
+    return (int64_t)((int64_t)B * 16 + 2 * (int64_t)C + 1) * kFxWords * 8;
+}
+
+extern "C" int pvraft_gn_act_bwd_det(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta,
+                                     double count, int act, float slope, int B, int64_t rows, int C, double* gsum, double* dgamma,
+                                     double* dbeta, double* dslope, float* dx, const float* slope_dev, const uint8_t* arg, void* workspace,
+                                     void* stream) {
+    return gn_act_bwd<true>(x, dy, stats, gamma, beta, count, act, slope, B, rows, C, gsum, dgamma, dbeta, dslope, dx, slope_dev, arg,
+                            workspace, stream);
 }
 
 extern "C" int pvraft_gn_act_maxk_fwd(const float* x, const double* stats, const float* gamma, const float* beta, double count, int act,
@@ -766,15 +937,41 @@ extern "C" int pvraft_edge_fwd(const float* P, const int32_t* nbr, float* E, int
     if (!P || !nbr || !E || B <= 0 || N <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "edge_fwd: bad argument");
     if (stats && C % PVRAFT_GN_GROUPS) return fail(PVRAFT_ERR_BAD_ARG, "edge_fwd: statistics need C %% 8 == 0");
     const long long pts = (long long)B * N;
-    k_edge_fwd<<<(unsigned)((pts + 7) / 8), 256, 0, (cudaStream_t)stream>>>(P, nbr, E, B, N, C, stats);
+    k_edge_fwd<false><<<(unsigned)((pts + 7) / 8), 256, 0, (cudaStream_t)stream>>>(P, nbr, E, B, N, C, stats);
     return check_launch("edge_fwd");
+}
+
+extern "C" int64_t pvraft_edge_det_fwd_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
+
+extern "C" int pvraft_edge_det_fwd(const float* P, const int32_t* nbr, float* E, int B, int N, int C, double* stats, void* workspace,
+                                   void* stream) {
+    if (!P || !nbr || !E || B <= 0 || N <= 0 || C <= 0 || (stats && !workspace)) return fail(PVRAFT_ERR_BAD_ARG, "edge_det_fwd: bad argument");
+    if (stats && C % PVRAFT_GN_GROUPS) return fail(PVRAFT_ERR_BAD_ARG, "edge_det_fwd: statistics need C %% 8 == 0");
+    const long long pts = (long long)B * N;
+    cudaStream_t st = (cudaStream_t)stream;
+    k_edge_fwd<true><<<(unsigned)((pts + 7) / 8), 256, 0, st>>>(P, nbr, E, B, N, C, stats ? static_cast<double*>(workspace) : nullptr);
+    int rc = check_launch("edge_det_fwd");
+    if (rc || !stats) return rc;
+    return fx_flush_f64(static_cast<const unsigned long long*>(workspace), 1, (long long)B * 16, (long long)B * 16, 0, stats, st);
 }
 
 extern "C" int pvraft_edge_bwd(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* stream) {
     if (!dT || !nbr || !dP || B <= 0 || N <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "edge_bwd: bad argument");
     const long long pts = (long long)B * N;
-    k_edge_bwd<<<(unsigned)((pts + 7) / 8), 256, 0, (cudaStream_t)stream>>>(dT, nbr, B, N, C, dP);
+    k_edge_bwd<false><<<(unsigned)((pts + 7) / 8), 256, 0, (cudaStream_t)stream>>>(dT, nbr, B, N, C, dP);
     return check_launch("edge_bwd");
+}
+
+extern "C" int64_t pvraft_edge_bwd_det_workspace_bytes(int B, int N, int C) { return (int64_t)B * N * C * kFxWords * 8; }
+
+extern "C" int pvraft_edge_bwd_det(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* workspace, void* stream) {
+    if (!dT || !nbr || !dP || !workspace || B <= 0 || N <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "edge_bwd_det: bad argument");
+    const long long pts = (long long)B * N;
+    cudaStream_t st = (cudaStream_t)stream;
+    k_edge_bwd<true><<<(unsigned)((pts + 7) / 8), 256, 0, st>>>(dT, nbr, B, N, C, static_cast<float*>(workspace));
+    int rc = check_launch("edge_bwd_det");
+    if (rc) return rc;
+    return fx_flush_f32(static_cast<const unsigned long long*>(workspace), 1, pts * C, pts * C, 0, dP, st);
 }
 
 extern "C" int pvraft_maxk_fwd(const float* x, int64_t pts, int C, float* y, uint8_t* arg, void* stream) {
@@ -814,19 +1011,35 @@ extern "C" int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2
     return check_launch("corr_lookup_bwd");
 }
 
-extern "C" int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C, int K,
-                                    float* d_fmap1, float* d_fmap2, void* stream) {
-    if (!g || !idx || !fmap1 || !fmap2 || !d_fmap1 || !d_fmap2 || B <= 0 || N <= 0 || K <= 0) return fail(PVRAFT_ERR_BAD_ARG, "corr_init_bwd: bad argument");
+template <bool DET>
+static int corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C, int K, float* d_fmap1,
+                         float* d_fmap2, void* ws, void* stream) {
+    if (!g || !idx || !fmap1 || !fmap2 || !d_fmap1 || !d_fmap2 || B <= 0 || N <= 0 || K <= 0 || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "corr_init_bwd: bad argument");
+    float* kd2 = DET ? static_cast<float*>(ws) : d_fmap2;
     const long long rows = (long long)B * N;
     const unsigned blocks = (unsigned)((rows + 7) / 8);
     const float scale = 1.0f / sqrtf((float)C);
     cudaStream_t st = (cudaStream_t)stream;
     switch (C) {
-        case 32: k_corr_init_bwd<1><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, d_fmap2); break;
-        case 64: k_corr_init_bwd<2><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, d_fmap2); break;
-        case 128: k_corr_init_bwd<4><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, d_fmap2); break;
-        case 256: k_corr_init_bwd<8><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, d_fmap2); break;
+        case 32: k_corr_init_bwd<1, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, kd2); break;
+        case 64: k_corr_init_bwd<2, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, kd2); break;
+        case 128: k_corr_init_bwd<4, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, kd2); break;
+        case 256: k_corr_init_bwd<8, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, kd2); break;
         default: return fail(PVRAFT_ERR_UNSUPPORTED, "corr_init_bwd: C=%d (32, 64, 128, 256)", C);
     }
-    return check_launch("corr_init_bwd");
+    int rc = check_launch("corr_init_bwd");
+    if (rc || !DET) return rc;
+    return fx_flush_f32(static_cast<const unsigned long long*>(ws), 1, rows * C, rows * C, 0, d_fmap2, st);
+}
+
+extern "C" int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C, int K,
+                                    float* d_fmap1, float* d_fmap2, void* stream) {
+    return corr_init_bwd<false>(g, idx, fmap1, fmap2, B, N, C, K, d_fmap1, d_fmap2, nullptr, stream);
+}
+
+extern "C" int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int N, int C) { return (int64_t)B * N * C * kFxWords * 8; }
+
+extern "C" int pvraft_corr_init_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C,
+                                        int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream) {
+    return corr_init_bwd<true>(g, idx, fmap1, fmap2, B, N, C, K, d_fmap1, d_fmap2, workspace, stream);
 }

@@ -62,7 +62,8 @@ class _RaftBase(nn.Module):
         return self
 
     def _graph_key(self, xyz1, num_iters):
-        return (tuple(xyz1.shape), xyz1.device, int(num_iters))
+        # a graph records the kernels of one setting of torch.use_deterministic_algorithms: never replayed under the other
+        return (tuple(xyz1.shape), xyz1.device, int(num_iters), ops.deterministic())
 
     def _stamp(self):
         return tuple((q._version, q.data_ptr()) for q in self.parameters())
