@@ -251,6 +251,45 @@ typedef struct pvraft_tc_linear_args {
 } pvraft_tc_linear_args;
 
 PVRAFT_API int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * The update chain of one RAFT iteration in one launch: the same five layers and the same bits as the five
+ * pvraft_tc_linear_fwd calls they replace, with the intermediates (cc, motion, r*h) kept on chip:
+ *   cc     = relu(W_cc [PReLU(GN(y1)) | kfeat] + b_cc)            (conv_corr folded into the feature head)
+ *   motion = [relu(W_m [cc | cflow] + b_m) (61) | flow (3)]        (MotionEncoder.conv, model/update.py:19-20)
+ *   z, r   = sigmoid(W_zr [net | inp | motion] + [b_z | b_r])     (ConvGRU, model/update.py:34-35)
+ *   net_out = (1 - z) net + z tanh(W_q [r*net | inp | motion] + b_q)   (model/update.py:36-39)
+ *   p_out  = W_fc1[:, :64] net_out                                 (flow-head SetConv fc1 pre-transform, no bias)
+ * Weights pre-split with pvraft_tc_weight_split into hi/lo, [n_pad, K] row-major, in this order:
+ *   0 W_cc [64,192], 1 W_m [64,128] (61 rows + zero padding), 2 [W_z; W_r] [128,192], 3 W_q [64,192], 4 W_fc1 [64,64].
+ * Requirements: N % 128 == 0, hidden = context = 64, y1_channels = 128 (PVRAFT_ERR_UNSUPPORTED otherwise); net_out != net.
+ * No reductions: the results do not depend on the launch configuration.
+ * --------------------------------------------------------------------------------------------- */
+typedef struct pvraft_update_chain_args {
+    const float* y1;         /* [B,N,y1_channels] pre-GroupNorm lookup features */
+    const double* y1_stats;  /* [B,8,2] GroupNorm sums of y1 */
+    const float* gn_gamma;   /* [y1_channels] */
+    const float* gn_beta;
+    double gn_count;         /* elements per group and sample */
+    float gn_slope;          /* PReLU slope after the GroupNorm */
+    const float* kfeat;      /* [B,N,64] */
+    const float* cflow;      /* [B,N,64] */
+    const float* flow;       /* [B,N,3] */
+    const float* net;        /* [B,N,hidden] */
+    const float* inp;        /* [B,N,context] */
+    const float* w_hi[5];
+    const float* w_lo[5];
+    const float* b_cc;       /* [64] */
+    const float* b_m;        /* [61] */
+    const float* b_z;        /* [64] */
+    const float* b_r;        /* [64] */
+    const float* b_q;        /* [64] */
+    float* net_out;          /* [B,N,hidden] */
+    float* p_out;            /* [B,N,64] */
+    int B, N, hidden, context, y1_channels;
+} pvraft_update_chain_args;
+
+PVRAFT_API int pvraft_update_chain_fwd(const pvraft_update_chain_args* a, void* stream);
 /* hi = tf32(w), lo = tf32(w - hi) of the window w[0:rows, col0:col0+cols] of a row-major matrix with row stride ld,
  * written zero-padded as [rows_pad, cols_pad]. */
 PVRAFT_API int pvraft_tc_weight_split(const float* w, int rows, int cols, int ld, int col0, int rows_pad, int cols_pad,

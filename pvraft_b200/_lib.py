@@ -38,6 +38,14 @@ class TcLinearArgs(C.Structure):
                 ('coords2_out', VP), ('flow_out', VP), ('params_settled', C.c_int)]
 
 
+class UpdateChainArgs(C.Structure):
+    _fields_ = [('y1', VP), ('y1_stats', VP), ('gn_gamma', VP), ('gn_beta', VP), ('gn_count', C.c_double),
+                ('gn_slope', C.c_float), ('kfeat', VP), ('cflow', VP), ('flow', VP), ('net', VP), ('inp', VP),
+                ('w_hi', VP * 5), ('w_lo', VP * 5), ('b_cc', VP), ('b_m', VP), ('b_z', VP), ('b_r', VP), ('b_q', VP),
+                ('net_out', VP), ('p_out', VP), ('B', C.c_int), ('N', C.c_int), ('hidden', C.c_int), ('context', C.c_int),
+                ('y1_channels', C.c_int)]
+
+
 class KnnBranchArgs(C.Structure):
     _fields_ = [('knn_sel', VP), ('moments', VP), ('w_knn', VP), ('b_knn', VP), ('gnk_gamma', VP), ('gnk_beta', VP),
                 ('preluk', VP), ('preluk_host', C.c_float), ('kfeat', VP), ('flow', VP), ('w_cf', VP), ('b_cf', VP),
@@ -83,7 +91,8 @@ _SIGNATURES = {
     'pvraft_corr_state_pack_bf16': (C.c_int, [VP, VP, C.c_int64, VP, VP, VP]),
     'pvraft_linear_fwd': (C.c_int, [C.POINTER(LinearArgs), VP]),
     'pvraft_tc_linear_fwd': (C.c_int, [C.POINTER(TcLinearArgs), VP]),
-    'pvraft_tc_weight_split': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_update_chain_fwd': (C.c_int, [C.POINTER(UpdateChainArgs), VP]),
+    'pvraft_tc_weight_split':(C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_gn_act_fwd': (C.c_int, [VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int,
                                     C.c_int, VP, VP, VP]),
     'pvraft_corr_feature_fwd': (C.c_int, [C.POINTER(CorrFeatArgs), VP]),

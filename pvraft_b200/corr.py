@@ -180,6 +180,30 @@ class CorrBlock(nn.Module):
         (model/corr.py:42-45 and model/update.py:15-21): coords, flow [B,N,3] -> (corr [B,N,64], motion [B,N,64]);
         with need_corr=False the correlation feature itself is not materialised (one launch fewer) and None is returned.
         Needs ops.tc_supported(N)."""
+        y1, kfeat, cflow, gn = self.motion_inputs_tc(coords, flow, motion_encoder)
+        oc, me = self.out_conv, motion_encoder
+        if need_corr:
+            # corr = out_conv[3](PReLU(GN(y1))) + knn_out(kfeat): one GEMM over K = 128 + 64
+            bias = ops.derived((oc[3].bias, self.knn_out.bias), 'sum', lambda x, y: (x.detach() + y.detach()).contiguous())
+            corr = ops.tc_linear([y1, kfeat], ops.tc_weights((oc[3].weight, self.knn_out.weight), kcat=True), bias, **gn)
+            cc = ops.tc_linear([corr], ops.tc_weights(me.conv_corr.weight), _w(me.conv_corr.bias), out_act=ACT_RELU)
+        else:
+            w_eff, b_eff = self.corr_motion_weights(me)
+            corr = None
+            cc = ops.tc_linear([y1, kfeat], ops.tc_weights(w_eff), b_eff, out_act=ACT_RELU, **gn)
+        motion = ops.tc_linear([cc, cflow], ops.tc_weights(me.conv.weight), _w(me.conv.bias), out_act=ACT_RELU, tail=flow)
+        return corr, motion
+
+    def corr_motion_weights(self, motion_encoder):
+        """The loop only consumes relu(conv_corr(corr)) (update.py:16), and corr is linear in [a1, kfeat]: conv_corr folded
+        into the weights, W_cc [W_out | W_kout] with bias W_cc (b_out + b_kout) + b_cc (float64 products, rounded once)."""
+        me, oc = motion_encoder, self.out_conv
+        return ops.derived((me.conv_corr.weight, me.conv_corr.bias, oc[3].weight, oc[3].bias, self.knn_out.weight,
+                            self.knn_out.bias), 'corr_cc', fold_corr_motion)
+
+    def motion_inputs_tc(self, coords, flow, motion_encoder):
+        """The lookup, out_conv[0] and the kNN branch: (y1 [B,N,128] before its GroupNorm, kfeat [B,N,64], cflow [B,N,64],
+        the keyword arguments of y1's GroupNorm + PReLU prologue).  Needs ops.tc_supported(N)."""
         b, n, _ = coords.shape
         dev = coords.device
         nvox = self.num_levels * 27
@@ -202,20 +226,7 @@ class CorrBlock(nn.Module):
         ops.knn_branch(a)
         gn = dict(in_stats=stats[0], in_gamma=_w(oc[1].weight), in_beta=_w(oc[1].bias), in_count=float(n) * 16.0, in_act=ACT_LRELU,
                   in_slope=ops.derived((oc[2].weight,), 'slope', lambda w: float(w.detach().reshape(-1)[0])))
-        if need_corr:
-            # corr = out_conv[3](PReLU(GN(y1))) + knn_out(kfeat): one GEMM over K = 128 + 64
-            bias = ops.derived((oc[3].bias, self.knn_out.bias), 'sum', lambda x, y: (x.detach() + y.detach()).contiguous())
-            corr = ops.tc_linear([y1, kfeat], ops.tc_weights((oc[3].weight, self.knn_out.weight), kcat=True), bias, **gn)
-            cc = ops.tc_linear([corr], ops.tc_weights(me.conv_corr.weight), _w(me.conv_corr.bias), out_act=ACT_RELU)
-        else:
-            # the loop only consumes relu(conv_corr(corr)) (update.py:16), and corr is linear in [a1, kfeat]: fold conv_corr
-            # into the weights, W_cc [W_out | W_kout] with bias W_cc (b_out + b_kout) + b_cc (float64 products, rounded once)
-            w_eff, b_eff = ops.derived((me.conv_corr.weight, me.conv_corr.bias, oc[3].weight, oc[3].bias, self.knn_out.weight,
-                                        self.knn_out.bias), 'corr_cc', fold_corr_motion)
-            corr = None
-            cc = ops.tc_linear([y1, kfeat], ops.tc_weights(w_eff), b_eff, out_act=ACT_RELU, **gn)
-        motion = ops.tc_linear([cc, cflow], ops.tc_weights(me.conv.weight), _w(me.conv.bias), out_act=ACT_RELU, tail=flow)
-        return corr, motion
+        return y1, kfeat, cflow, gn
 
     def __call__(self, coords):
         """model/corr.py:44-45 -> [B,64,N]."""

@@ -34,10 +34,11 @@ class SetConv(torch.nn.Module):
         self.fc3 = torch.nn.Conv1d(nb_feat_out, nb_feat_out, 1, bias=False)
         self.gn3 = torch.nn.GroupNorm(8, nb_feat_out, affine=True)
 
-    def forward_deferred(self, signal, graph):
+    def forward_deferred(self, signal, graph, p=None):
         """signal: [B,N,cin] tensor or a Deferred from the previous SetConv -> Deferred.
         Layers whose shapes fit the tensor-core kernel (N % 128 == 0, K % 32 == 0) run on wgmma (3xTF32),
-        the others on the CUDA-core kernel; both are fp32-accurate."""
+        the others on the CUDA-core kernel; both are fp32-accurate.  p: the fc1 pre-transform of a plain signal when the
+        caller has already computed it (the fused update chain of the RAFT loop)."""
         cin, mid, cout = self.nb_feat_in, self.mid, self.nb_feat_out
         deferred = isinstance(signal, Deferred)
         x = signal.z if deferred else signal.detach().contiguous().float()
@@ -48,7 +49,10 @@ class SetConv(torch.nn.Module):
         pro = dict(in_stats=signal.stats, in_gamma=signal.gamma, in_beta=signal.beta, in_count=signal.count,
                    in_act=ACT_LRELU, in_slope=0.1) if deferred else {}
         # fc1 pre-transform P = fc1.weight[:, :cin] . x   (gconv.py:65-73: fc1 is linear and bias-free)
-        if ops.tc_supported(n, cin) and mid <= 128:
+        if p is not None:
+            if deferred or p.shape != (b, n, mid):
+                raise ValueError('a precomputed fc1 pre-transform needs a plain signal and shape [B,N,mid]')
+        elif ops.tc_supported(n, cin) and mid <= 128:
             p = ops.tc_linear([x], ops.tc_weights(self.fc1.weight, col0=0, cols=cin), **pro)
         else:
             p = ops.linear(x, _w(self.fc1.weight), cin=cin, w_ld=cin + 3, cout=mid, in_mode=IN_GN if deferred else ops.IN_PLAIN, **pro)

@@ -433,6 +433,29 @@ def tc_linear(sources, w, bias=None, *, in_min=None, in_stats=None, in_gamma=Non
     return out
 
 
+fuse_update_chain = True   # False: the RAFT loop runs the update chain as its five tc_linear launches (tests compare the two)
+
+
+def update_chain(y1, gn, kfeat, cflow, flow, net, inp, weights, biases):
+    """MotionEncoder + ConvGRU + flow-head fc1 pre-transform of one RAFT iteration in one launch (include/pvraft_b200.h,
+    pvraft_update_chain_fwd): the same bits as the five tc_linear launches it replaces.  gn: y1's prologue (in_stats,
+    in_gamma, in_beta, in_count, in_slope as for tc_linear); weights: five tc_weights() results in the order cc, motion,
+    [z|r], q, fc1; biases: (b_cc, b_m, b_z, b_r, b_q).  Returns (net' [B,N,64], P [B,N,64])."""
+    b, n, _ = net.shape
+    net_out, p_out = torch.empty_like(net), torch.empty_like(net)
+    a = _lib.UpdateChainArgs()
+    a.y1, a.y1_stats = _p(y1), _p(gn['in_stats'], torch.float64)
+    a.gn_gamma, a.gn_beta, a.gn_count, a.gn_slope = _p(gn['in_gamma']), _p(gn['in_beta']), float(gn['in_count']), float(gn['in_slope'])
+    a.kfeat, a.cflow, a.flow, a.net, a.inp = _p(kfeat), _p(cflow), _p(flow), _p(net), _p(inp)
+    for i, (hi, lo, _, _) in enumerate(weights):
+        a.w_hi[i], a.w_lo[i] = _p(hi), _p(lo)
+    a.b_cc, a.b_m, a.b_z, a.b_r, a.b_q = (_p(x) for x in biases)
+    a.net_out, a.p_out = _p(net_out), _p(p_out)
+    a.B, a.N, a.hidden, a.context, a.y1_channels = b, n, net.shape[-1], inp.shape[-1], y1.shape[-1]
+    _count(lib().pvraft_update_chain_fwd(C.byref(a), _stream()), 'update_chain')
+    return net_out, p_out
+
+
 def gn_act(x, stats, gamma, beta, count, act=ACT_LRELU, slope=0.1, transpose_out=False, slope_dev=None):
     """slope_dev: optional one-element device tensor (a PReLU weight) the kernel reads instead of the scalar `slope`."""
     b, n, c = x.shape

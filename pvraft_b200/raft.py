@@ -161,6 +161,17 @@ class _RaftBase(nn.Module):
     def _iterate_body(self, xyz1, graph_context, net, inp, num_iters, keep_all, coords2, flow, preds, me, use_tc):
         b, n, _ = xyz1.shape
         for _ in range(num_iters):
+            if use_tc and ops.fuse_update_chain:
+                y1, kfeat, cflow, gn = self.corr_block.motion_inputs_tc(coords2, flow, me)                # :42
+                new_flow = torch.empty_like(xyz1)
+                net, _ = self.update_block.forward_chain_pm(net, inp, y1, kfeat, cflow, flow, gn,
+                                                            self.corr_block.corr_motion_weights(me), graph_context,
+                                                            coords1=xyz1, coords2=coords2, coords2_out=coords2,
+                                                            flow_out=new_flow)                              # :43-46
+                flow = new_flow
+                if keep_all:
+                    preds.append(flow)
+                continue
             if use_tc:
                 _, motion = self.corr_block.feature_motion_tc(coords2, flow, me, need_corr=False)          # :42 + update.py:83
             else:

@@ -115,10 +115,11 @@ class FlowHead(nn.Module):
             nn.Conv1d(64, 3, 1),
         )
 
-    def forward_pm(self, net, graph, coords1=None, coords2=None, coords2_out=None, flow_out=None):
-        """net [B,N,64] -> delta_flow [B,N,3]; optionally also the RAFT coordinate update."""
+    def forward_pm(self, net, graph, coords1=None, coords2=None, coords2_out=None, flow_out=None, p=None):
+        """net [B,N,64] -> delta_flow [B,N,3]; optionally also the RAFT coordinate update.  p: the SetConv's fc1
+        pre-transform of net when it was computed with net (UpdateBlock.forward_chain_pm)."""
         b, n, _ = net.shape
-        d = self.setconv.forward_deferred(net, graph)
+        d = self.setconv.forward_deferred(net, graph, p=p)
         delta = torch.empty(b, n, 3, dtype=torch.float32, device=net.device)
         oc = self.out_conv
         if ops.tc_supported(n):
@@ -154,6 +155,20 @@ class UpdateBlock(nn.Module):
     def forward_pm(self, net, inp, motion, graph, **coords):
         net = self.gru.forward_pm(net, inp, motion)
         delta = self.flow_head.forward_pm(net, graph, **coords)
+        return net, delta
+
+    def forward_chain_pm(self, net, inp, y1, kfeat, cflow, flow, gn, corr_motion, graph, **coords):
+        """One RAFT update from the correlation block's pre-activations (CorrBlock.motion_inputs_tc) with the motion
+        encoder, the ConvGRU and the flow head's fc1 pre-transform in one launch (ops.update_chain); the same values as
+        CorrBlock.feature_motion_tc followed by forward_pm.  corr_motion: CorrBlock.corr_motion_weights().  Needs
+        ops.tc_supported(N)."""
+        me, gru, sc = self.motion_encoder, self.gru, self.flow_head.setconv
+        w_eff, b_eff = corr_motion
+        weights = (ops.tc_weights(w_eff), ops.tc_weights(me.conv.weight), ops.tc_weights((gru.convz.weight, gru.convr.weight)),
+                   ops.tc_weights(gru.convq.weight), ops.tc_weights(sc.fc1.weight, col0=0, cols=sc.nb_feat_in))
+        biases = (b_eff, _w(me.conv.bias), _w(gru.convz.bias), _w(gru.convr.bias), _w(gru.convq.bias))
+        net, p = ops.update_chain(y1, gn, kfeat, cflow, flow, net, inp, weights, biases)
+        delta = self.flow_head.forward_pm(net, graph, p=p, **coords)
         return net, delta
 
     def forward(self, net, inp, corr, flow, graph):
