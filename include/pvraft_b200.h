@@ -65,6 +65,12 @@ PVRAFT_API int pvraft_device_info(int* sm_count, int* smem_optin_bytes);
 PVRAFT_API int64_t pvraft_corr_matmul_workspace_bytes(int B, int N, int C);
 PVRAFT_API int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, int B, int N, int C, float* corr, void* workspace,
                            void* stream);
+/* Clouds of different sizes: fmap1 [B,N,C] x fmap2 [B,M,C] -> corr [B,N,M]; N % 128 == 0, M % 128 == 0, C % 32 == 0.
+ * The workspace is pvraft_corr_matmul_nm_workspace_bytes(B,N,M,C) bytes.  With M == N these are the two entry points above
+ * (which forward to them). */
+PVRAFT_API int64_t pvraft_corr_matmul_nm_workspace_bytes(int B, int N, int M, int C);
+PVRAFT_API int pvraft_corr_matmul_nm_fwd(const float* fmap1, const float* fmap2, int B, int N, int M, int C, float* corr,
+                                         void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * The same GEMM over one window of the correlation matrix, for clouds whose N x N matrix is not built whole.
@@ -81,6 +87,11 @@ PVRAFT_API int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, in
 PVRAFT_API int pvraft_tf32_split_fwd(const float* x, int64_t n, float* hi, float* lo, void* stream);
 PVRAFT_API int pvraft_corr_matmul_window_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
                                              int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream);
+/* The window GEMM for clouds of different sizes: a_hi/a_lo [B,N,C], b_hi/b_lo [B,M,C], N and M multiples of 128 (each
+ * sample's operand rows padded separately); the window's whole row tiles lie inside [0, N) and its column tiles inside
+ * [0, M).  pvraft_corr_matmul_window_fwd is this entry point with M == N. */
+PVRAFT_API int pvraft_corr_matmul_window_nm_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
+                                                int M, int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Correlation truncation: the K largest entries of every row of a dense correlation matrix.
@@ -151,6 +162,21 @@ PVRAFT_API int pvraft_xyz_pad_fwd(const float* xyz, int64_t rows, float* out, vo
 PVRAFT_API int pvraft_corr_lookup_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
                            int B, int N, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
                            int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* stream);
+/* Clouds of different sizes: N query points (corr_val, corr_idx, coords and every output have N rows per sample), M points
+ * in the second cloud (xyz2_pad [B,M,4]; candidate ids < M).  A cell mean divides by clamp(count, 1, N) (model/corr.py:65),
+ * which differs from the count only when N < K.  The gather table is staged in shared memory while M*16 bytes fit next to
+ * the warps' stages, and read from global memory (through L1/L2) otherwise.  The bf16 form needs M <= 65536.  The entry
+ * points above are these with M == N. */
+PVRAFT_API int pvraft_corr_lookup_nm_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
+                                         int B, int N, int M, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
+                                         int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* stream);
+/* 1 when the lookup stages the gather table of a second cloud of M points in shared memory at truncate_k = K, 0 when it
+ * gathers from global memory (a query for tools and tests). */
+PVRAFT_API int pvraft_corr_lookup_table_in_smem(int M, int K);
+PVRAFT_API int pvraft_corr_lookup_bf16_nm_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
+                                              const float* coords, int B, int N, int M, int K, int levels, float base_scale, float* vox,
+                                              int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
+                                              void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Generic fused (GroupNorm -> activation -> 1x1 conv [-> bias] [-> ReLU]) layer over points with
@@ -496,12 +522,19 @@ PVRAFT_API int pvraft_maxk_bwd(const float* dy, const uint8_t* arg, int64_t pts,
 PVRAFT_API int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
                            const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int K, int levels, float base_scale,
                            float* d_corr, void* stream);
+/* The same for clouds of different sizes: N query points, xyz2_pad [B,M,4]; the means' divisor is clamp(count, 1, N). */
+PVRAFT_API int pvraft_corr_lookup_nm_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
+                                         const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int M, int K, int levels,
+                                         float base_scale, float* d_corr, void* stream);
 
 /* Backward of the truncated correlation (model/corr.py:95-100 + the top-k gather of :37-38), sparse over the K kept entries:
  *   g [B,N,K], idx [B,N,K] (same stored order), fmap1/fmap2 [B,N,C] point-major
  *   -> d_fmap1 [B,N,C] (overwritten), d_fmap2 [B,N,C] (ACCUMULATED, zeroed by the caller).  C in {32,64,128,256}. */
 PVRAFT_API int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C, int K,
                          float* d_fmap1, float* d_fmap2, void* stream);
+/* The same for clouds of different sizes: fmap1, d_fmap1 [B,N,C]; fmap2, d_fmap2 [B,M,C]; idx < M. */
+PVRAFT_API int pvraft_corr_init_nm_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M,
+                                       int C, int K, float* d_fmap1, float* d_fmap2, void* stream);
 
 /* Training extras on the device (SURVEY.md 8f row f3).  est, gt [points,3]; mask [points] (> 0 = valid) or NULL.
  *   pvraft_flow_metrics_fwd: acc[6] double, ZEROED by the caller, accumulates over the valid points
@@ -550,6 +583,14 @@ PVRAFT_API int pvraft_corr_lookup_bf16_det_fwd(const uint16_t* corr_val_bf16, co
                                                const float* coords, int B, int N, int K, int levels, float base_scale, float* vox,
                                                int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
                                                void* workspace, void* stream);
+PVRAFT_API int pvraft_corr_lookup_nm_det_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
+                                             int B, int N, int M, int K, int levels, float base_scale, float* vox, int vox_ld,
+                                             float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace,
+                                             void* stream);
+PVRAFT_API int pvraft_corr_lookup_bf16_nm_det_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
+                                                  const float* coords, int B, int N, int M, int K, int levels, float base_scale, float* vox,
+                                                  int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
+                                                  void* workspace, void* stream);
 PVRAFT_API int64_t pvraft_edge_det_fwd_workspace_bytes(int B);
 PVRAFT_API int pvraft_edge_det_fwd(const float* P, const int32_t* nbr, float* E, int B, int N, int C, double* stats, void* workspace,
                                    void* stream);
@@ -572,6 +613,9 @@ PVRAFT_API int pvraft_edge_bwd_det(const float* dT, const int32_t* nbr, int B, i
 PVRAFT_API int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int N, int C);
 PVRAFT_API int pvraft_corr_init_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C,
                                         int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_corr_init_nm_bwd_det_workspace_bytes(int B, int M, int C);
+PVRAFT_API int pvraft_corr_init_nm_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M,
+                                           int C, int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream);
 
 #ifdef __cplusplus
 }

@@ -77,9 +77,13 @@ _SIGNATURES = {
     'pvraft_device_info': (C.c_int, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     'pvraft_corr_matmul_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
     'pvraft_corr_matmul_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_corr_matmul_nm_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    'pvraft_corr_matmul_nm_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_tf32_split_fwd': (C.c_int, [VP, C.c_int64, VP, VP, VP]),
     'pvraft_corr_matmul_window_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                                 VP, C.c_int64, VP]),
+    'pvraft_corr_matmul_window_nm_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                   C.c_int, VP, C.c_int64, VP]),
     'pvraft_corr_topk_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_corr_topk_window_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, VP, VP, VP, C.c_int64, VP]),
     'pvraft_corr_reorder': (C.c_int, [VP, VP, C.c_int64, C.c_int, VP, VP, VP]),
@@ -88,6 +92,11 @@ _SIGNATURES = {
                                          VP, C.c_int, VP, VP, VP, VP, VP]),
     'pvraft_corr_lookup_bf16_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                               VP, C.c_int, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_nm_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                            VP, C.c_int, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_bf16_nm_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                                 VP, C.c_int, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_table_in_smem': (C.c_int, [C.c_int, C.c_int]),
     'pvraft_corr_state_pack_bf16': (C.c_int, [VP, VP, C.c_int64, VP, VP, VP]),
     'pvraft_linear_fwd': (C.c_int, [C.POINTER(LinearArgs), VP]),
     'pvraft_tc_linear_fwd': (C.c_int, [C.POINTER(TcLinearArgs), VP]),
@@ -114,6 +123,9 @@ _SIGNATURES = {
     'pvraft_maxk_bwd': (C.c_int, [VP, VP, C.c_int64, C.c_int, VP, VP]),
     'pvraft_corr_lookup_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_int, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, VP, VP]),
     'pvraft_corr_init_bwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_corr_lookup_nm_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_int, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                            VP, VP]),
+    'pvraft_corr_init_nm_bwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_flow_metrics_fwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP]),
     'pvraft_flow_l1_bwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, C.c_float, VP, VP]),
     'pvraft_sizeof': (C.c_int, [C.c_int]),
@@ -130,6 +142,10 @@ _SIGNATURES = {
                                              VP, C.c_int, VP, VP, VP, VP, VP, VP]),
     'pvraft_corr_lookup_bf16_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                                   VP, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_nm_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                                VP, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_bf16_nm_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                                     VP, C.c_int, VP, VP, VP, VP, VP, VP]),
     'pvraft_edge_det_fwd_workspace_bytes': (C.c_int64, [C.c_int]),
     'pvraft_edge_det_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_flow_metrics_det_workspace_bytes': (C.c_int64, []),
@@ -145,6 +161,8 @@ _SIGNATURES = {
     'pvraft_edge_bwd_det': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_corr_init_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
     'pvraft_corr_init_bwd_det': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
+    'pvraft_corr_init_nm_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    'pvraft_corr_init_nm_bwd_det': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
 }
 EXPORTS = tuple(_SIGNATURES)
 

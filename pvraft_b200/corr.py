@@ -54,20 +54,20 @@ class CorrBlock(nn.Module):
             nn.PReLU(),
         )
         self.knn_out = nn.Conv1d(64, 64, 1)
-        self.corr_val = None     # [B,N,K] f32 correlation of the kept candidates (bank-aware order, see ops.corr_reorder)
-        self.corr_idx = None     # [B,N,K] int32 candidate ids (rows of xyz2), same order
+        self.corr_val = None     # [B,N1,K] f32 correlation of the kept candidates (bank-aware order, see ops.corr_reorder)
+        self.corr_idx = None     # [B,N1,K] int32 candidate ids (rows of xyz2 [B,N2,3]), same order
         # torch.bfloat16 = the reduced-precision state of BASELINE configs[2] (bf16 values + uint16 ids, 4 B per candidate and
         # iteration; index math stays fp32): inference only, set through RSF.set_precision('bf16')
         self.state_dtype = torch.float32
         self._xyz2 = None
-        self._xyz2p = None   # [B,N,4] (x,y,z,0): the lookup kernel's gather table
+        self._xyz2p = None   # [B,N2,4] (x,y,z,0): the lookup kernel's gather table
 
     # ------------------------------------------------------------------------------------------
     @staticmethod
     def calculate_corr_pm(fmap1_pm, fmap2_pm):
-        """Point-major [B,N,C] feature maps -> corr [B,N,N] = <f1_i, f2_j> / sqrt(C) on the wgmma GEMM (3xTF32, fp32-accurate).
-        The kernel works on 128-point tiles: a ragged N is zero-padded to the next multiple of 128 and the result cropped
-        (no library GEMM on any path)."""
+        """Point-major feature maps [B,N1,C], [B,N2,C] -> corr [B,N1,N2] = <f1_i, f2_j> / sqrt(C) on the wgmma GEMM (3xTF32,
+        fp32-accurate).  The kernel works on 128-point tiles: a ragged N1 or N2 is zero-padded to the next multiple of 128 and
+        the result cropped (no library GEMM on any path)."""
         b, n, c = fmap1_pm.shape
         if c % 32 != 0:
             raise NotImplementedError(f'calculate_corr: {c} feature channels (the wgmma GEMM needs a multiple of 32; the model has 128)')
@@ -81,30 +81,34 @@ class CorrBlock(nn.Module):
 
     def init_module(self, fmap1, fmap2, xyz2):
         """model/corr.py:31-42: build the truncated correlation state for one forward pass
-        (fmap1, fmap2 [B,C,N] channel-major as in the reference)."""
+        (fmap1 [B,C,N1], fmap2 [B,C,N2] channel-major as in the reference; xyz2 [B,N2,3])."""
         return self.init_module_pm(ops.transpose(fmap1.detach().contiguous().float()),
                                    ops.transpose(fmap2.detach().contiguous().float()), xyz2)
 
     def init_module_pm(self, fmap1_pm, fmap2_pm, xyz2):
-        """Same with point-major feature maps [B,N,C] (what the encoders produce natively)."""
+        """Same with point-major feature maps fmap1 [B,N1,C], fmap2 [B,N2,C] (what the encoders produce natively).  The state
+        has N1 rows of K candidates, each a row of xyz2 [B,N2,3]."""
         b, n_p, _ = xyz2.shape
+        if fmap2_pm.shape[:2] != (b, n_p) or fmap1_pm.shape[0] != b:
+            raise ValueError(f'init_module: fmap1 {tuple(fmap1_pm.shape)}, fmap2 {tuple(fmap2_pm.shape)} and xyz2 {tuple(xyz2.shape)} '
+                             'disagree (expected [B,N1,C], [B,N2,C], [B,N2,3])')
         if n_p < self.truncate_k:
             raise ValueError(f'truncate_k={self.truncate_k} exceeds the number of points {n_p}')
         # wgmma GEMM (3xTF32, fp32-accurate) + top-K; in column windows above 49152 points (ops.CorrPlan)
         val, idx = ops.corr_build(fmap1_pm.contiguous(), fmap2_pm.contiguous(), self.truncate_k)
-        self._install(*ops.corr_reorder(val, idx))
+        self._install(*ops.corr_reorder(val, idx), n_p)
         self._xyz2 = xyz2.detach().contiguous().float()
         self._xyz2p = ops.xyz_pad(self._xyz2)
 
     def set_state(self, truncated_corr, corr_idx, xyz2):
-        """Install an externally built state (tests / benchmarks): corr [B,N,K] f32, idx [B,N,K] int."""
-        self._install(*ops.corr_reorder(truncated_corr.contiguous().float(), corr_idx.contiguous().to(torch.int32)))
+        """Install an externally built state (tests / benchmarks): corr [B,N1,K] f32, idx [B,N1,K] int rows of xyz2 [B,N2,3]."""
+        self._install(*ops.corr_reorder(truncated_corr.contiguous().float(), corr_idx.contiguous().to(torch.int32)), xyz2.shape[1])
         self._xyz2 = xyz2.contiguous().float()
         self._xyz2p = ops.xyz_pad(self._xyz2)
 
-    def _install(self, val, idx):
+    def _install(self, val, idx, n2):
         if self.state_dtype == torch.bfloat16:
-            val, idx = ops.corr_state_pack_bf16(val, idx)
+            val, idx = ops.corr_state_pack_bf16(val, idx, n2)
         self.corr_val, self.corr_idx = val, idx
 
     def candidate_ids(self):

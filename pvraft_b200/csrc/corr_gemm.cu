@@ -51,7 +51,7 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, v
 
 struct GemmParams {
     float* corr;   // [B, tiles_m * 128, ldc]: rows [r0, r0 + 128 tiles_m) x columns [c0, c0 + 128 tiles_n) of every sample
-    int N, C;      // operand rows per sample, channels
+    int N, M, C;   // rows per sample of operand A (fmap1) and of operand B (fmap2), channels
     float scale;   // sqrt(C): the divisor of model/corr.py:99
     float rscale;  // RN(1 / scale)
     int r0, c0;    // first row of fmap1 / of fmap2 (multiples of 128)
@@ -106,7 +106,7 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
                 const long long t = blockIdx.x + i * gridDim.x;
                 const int b = (int)(t / tiles_per_batch), r = (int)(t - (long long)b * tiles_per_batch);
                 const int tile_m = r / p.tiles_n, tile_n = r - tile_m * p.tiles_n;
-                const int row_a = b * p.N + p.r0 + tile_m * kTileM, row_b = b * p.N + p.c0 + tile_n * kTileN;
+                const int row_a = b * p.N + p.r0 + tile_m * kTileM, row_b = b * p.M + p.c0 + tile_n * kTileN;
                 for (int kb = 0; kb < num_kb; ++kb) {
                     mbar_wait_(&s_empty[s], phase ^ 1u);
                     unsigned char* st = tiles + (size_t)s * kStageBytes;
@@ -217,17 +217,17 @@ static int make_map(CUtensorMap* m, const float* base, long long rows, int C) {
     return 0;
 }
 
-// Rows [r0, r0 + 128 tiles_m) x columns [c0, c0 + 128 tiles_n) of every sample, from split operands [B*N, C] (hi/lo of
-// both maps), into corr [B, 128 tiles_m, ldc]
-static int launch_gemm(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N, int C, int r0,
+// Rows [r0, r0 + 128 tiles_m) x columns [c0, c0 + 128 tiles_n) of every sample, from split operands A [B*N, C] and
+// B [B*M, C] (hi/lo of both maps), into corr [B, 128 tiles_m, ldc]
+static int launch_gemm(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N, int M, int C, int r0,
                        int tiles_m, int c0, int tiles_n, float* corr, long long ldc, cudaStream_t st) {
     int rc;
     CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
     if ((rc = make_map(&ma_hi, a_hi, (long long)B * N, C)) || (rc = make_map(&ma_lo, a_lo, (long long)B * N, C)) ||
-        (rc = make_map(&mb_hi, b_hi, (long long)B * N, C)) || (rc = make_map(&mb_lo, b_lo, (long long)B * N, C)))
+        (rc = make_map(&mb_hi, b_hi, (long long)B * M, C)) || (rc = make_map(&mb_lo, b_lo, (long long)B * M, C)))
         return rc;
     GemmParams p{};
-    p.corr = corr; p.N = N; p.C = C;
+    p.corr = corr; p.N = N; p.M = M; p.C = C;
     p.scale = sqrtf((float)C);
     p.rscale = (float)(1.0 / (double)p.scale);
     p.r0 = r0; p.c0 = c0;
@@ -249,28 +249,36 @@ static void launch_split(const float* x, long long n, float* hi, float* lo, cuda
 
 using namespace pvraft;
 
-extern "C" int64_t pvraft_corr_matmul_workspace_bytes(int B, int N, int C) {
-    if (B <= 0 || N <= 0 || C <= 0) return 0;
-    return (int64_t)4 * B * N * C * (int64_t)sizeof(float);   // hi/lo copies of both feature maps
+extern "C" int64_t pvraft_corr_matmul_nm_workspace_bytes(int B, int N, int M, int C) {
+    if (B <= 0 || N <= 0 || M <= 0 || C <= 0) return 0;
+    return (int64_t)2 * B * ((int64_t)N + M) * C * (int64_t)sizeof(float);   // hi/lo copies of both feature maps
+}
+
+extern "C" int64_t pvraft_corr_matmul_workspace_bytes(int B, int N, int C) { return pvraft_corr_matmul_nm_workspace_bytes(B, N, N, C); }
+
+extern "C" int pvraft_corr_matmul_nm_fwd(const float* fmap1, const float* fmap2, int B, int N, int M, int C, float* corr, void* workspace,
+                                         void* stream) {
+    if (!fmap1 || !fmap2 || !corr || !workspace) return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul: null pointer");
+    if (B <= 0 || N <= 0 || M <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul: bad shape");
+    if (N % kTileM || M % kTileN || C % kBlockK)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul: N=%d and M=%d must be multiples of 128 and C=%d of 32", N, M, C);
+    if (B > 65535 || N / kTileM > 65535 || M / kTileN > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul: grid too large");
+    cudaStream_t st = (cudaStream_t)stream;
+    const long long na = (long long)B * N * C, nb = (long long)B * M * C;
+    float* a_hi = reinterpret_cast<float*>(workspace);
+    float* a_lo = a_hi + na;
+    float* b_hi = a_lo + na;
+    float* b_lo = b_hi + nb;
+    launch_split(fmap1, na, a_hi, a_lo, st);
+    launch_split(fmap2, nb, b_hi, b_lo, st);
+    const int rc = check_launch("tf32_split");
+    if (rc) return rc;
+    return launch_gemm(a_hi, a_lo, b_hi, b_lo, B, N, M, C, 0, N / kTileM, 0, M / kTileN, corr, M, st);
 }
 
 extern "C" int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, int B, int N, int C, float* corr, void* workspace,
                                       void* stream) {
-    if (!fmap1 || !fmap2 || !corr || !workspace) return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul: null pointer");
-    if (B <= 0 || N <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul: bad shape");
-    if (N % kTileM || C % kBlockK) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul: N=%d must be a multiple of 128 and C=%d of 32", N, C);
-    if (B > 65535 || N / kTileM > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul: grid too large");
-    cudaStream_t st = (cudaStream_t)stream;
-    const long long n = (long long)B * N * C;
-    float* a_hi = reinterpret_cast<float*>(workspace);
-    float* a_lo = a_hi + n;
-    float* b_hi = a_lo + n;
-    float* b_lo = b_hi + n;
-    launch_split(fmap1, n, a_hi, a_lo, st);
-    launch_split(fmap2, n, b_hi, b_lo, st);
-    const int rc = check_launch("tf32_split");
-    if (rc) return rc;
-    return launch_gemm(a_hi, a_lo, b_hi, b_lo, B, N, C, 0, N / kTileM, 0, N / kTileN, corr, N, st);
+    return pvraft_corr_matmul_nm_fwd(fmap1, fmap2, B, N, N, C, corr, workspace, stream);
 }
 
 extern "C" int pvraft_tf32_split_fwd(const float* x, int64_t n, float* hi, float* lo, void* stream) {
@@ -281,20 +289,26 @@ extern "C" int pvraft_tf32_split_fwd(const float* x, int64_t n, float* hi, float
     return check_launch("tf32_split");
 }
 
-extern "C" int pvraft_corr_matmul_window_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
-                                             int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream) {
+extern "C" int pvraft_corr_matmul_window_nm_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
+                                                int M, int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream) {
     if (!a_hi || !a_lo || !b_hi || !b_lo || !corr) return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul_window: null pointer");
-    if (B <= 0 || N <= 0 || C <= 0 || rows <= 0 || cols <= 0 || r0 < 0 || c0 < 0)
+    if (B <= 0 || N <= 0 || M <= 0 || C <= 0 || rows <= 0 || cols <= 0 || r0 < 0 || c0 < 0)
         return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul_window: bad shape");
-    if (N % kTileM || C % kBlockK || r0 % kTileM || c0 % kTileN)
-        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: N=%d, r0=%d and c0=%d must be multiples of 128 and C=%d of 32", N, r0,
-                    c0, C);
+    if (N % kTileM || M % kTileN || C % kBlockK || r0 % kTileM || c0 % kTileN)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: N=%d, M=%d, r0=%d and c0=%d must be multiples of 128 and C=%d of 32", N,
+                    M, r0, c0, C);
     const int tiles_m = (rows + kTileM - 1) / kTileM, tiles_n = (cols + kTileN - 1) / kTileN;
-    if (rows > N - r0 || cols > N - c0 || r0 + tiles_m * kTileM > N || c0 + tiles_n * kTileN > N)
-        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: rows [%d, %d) x columns [%d, %d), whole tiles, exceed N=%d", r0,
-                    r0 + tiles_m * kTileM, c0, c0 + tiles_n * kTileN, N);
+    if (rows > N - r0 || cols > M - c0 || r0 + tiles_m * kTileM > N || c0 + tiles_n * kTileN > M)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: rows [%d, %d) x columns [%d, %d), whole tiles, exceed N=%d x M=%d", r0,
+                    r0 + tiles_m * kTileM, c0, c0 + tiles_n * kTileN, N, M);
     if (ldc < (int64_t)tiles_n * kTileN || ldc % 4)
         return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: ldc=%lld (need a multiple of 4, >= %d)", (long long)ldc, tiles_n * kTileN);
-    if ((long long)B * N > 0x7fffffffLL) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: B*N=%lld operand rows", (long long)B * N);
-    return launch_gemm(a_hi, a_lo, b_hi, b_lo, B, N, C, r0, tiles_m, c0, tiles_n, corr, ldc, (cudaStream_t)stream);
+    if ((long long)B * N > 0x7fffffffLL || (long long)B * M > 0x7fffffffLL)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: B*N=%lld / B*M=%lld operand rows", (long long)B * N, (long long)B * M);
+    return launch_gemm(a_hi, a_lo, b_hi, b_lo, B, N, M, C, r0, tiles_m, c0, tiles_n, corr, ldc, (cudaStream_t)stream);
+}
+
+extern "C" int pvraft_corr_matmul_window_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
+                                             int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream) {
+    return pvraft_corr_matmul_window_nm_fwd(a_hi, a_lo, b_hi, b_lo, B, N, N, C, r0, rows, c0, cols, corr, ldc, stream);
 }

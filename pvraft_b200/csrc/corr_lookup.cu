@@ -42,7 +42,7 @@ __host__ __device__ constexpr size_t lookup_warp_bytes(int K) {
 struct LookupParams {
     const void* corr_val;   // [B,N,K] f32, or bf16 bit patterns (uint16) in the reduced-precision state mode
     const void* corr_idx;   // [B,N,K] int32, or uint16 in the reduced-precision state mode
-    const float4* tab;   // [B,N] (x,y,z,0) rows of xyz2
+    const float4* tab;   // [B,M] (x,y,z,0) rows of xyz2
     const float* coords; // [B,N,3]
     float* vox;          // [B,N,levels*27]
     float4* knn_sel;     // [B,N,32]
@@ -50,6 +50,7 @@ struct LookupParams {
     double* moments;     // [B,16] or null
     int8_t* dbg_cube;    // [B,N,K,levels] or null: the cell id (-1 = outside) this kernel derived for every candidate
     int B, N, K, levels;
+    int M;               // points of the second cloud: rows of a sample's gather table
     int vox_ld;          // floats per vox row (>= levels*27; the pad is zero-filled)
     float r[4];          // cell edge per level
     float inv_r[4];      // exact reciprocal when r is a power of two
@@ -158,8 +159,8 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
     constexpr int K = KPL * 32;
     constexpr unsigned NIB = (1u << VEC) - 1u;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    const size_t tab_bytes = SMEM_TAB ? (((size_t)p.N * 16 + 127) & ~(size_t)127) : 0;
-    const float4* s_tab = reinterpret_cast<const float4*>(smem_raw);   // [N] (x,y,z,0), a verbatim copy of the sample's table
+    const size_t tab_bytes = SMEM_TAB ? (((size_t)p.M * 16 + 127) & ~(size_t)127) : 0;
+    const float4* s_tab = reinterpret_cast<const float4*>(smem_raw);   // [M] (x,y,z,0), a verbatim copy of the sample's table
     const int w = warp_id();
     int lane;   // pinned: left to itself the compiler re-derives threadIdx.x & 31 (S2R + LOP) ~9 times per point
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
@@ -176,10 +177,11 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
     const bool active_warp = w < p.warps;
     __shared__ int s_next;   // next unclaimed point of the current segment (static mode: warps take points dynamically)
     __shared__ unsigned long long s_tabbar;
-    // 1/c in double for c = 0..K: (float)(double(sum) * rcp[c]) is the correctly rounded fp32 quotient sum/c for
-    // every integer c <= 2^20 (x/c is never within 2^-34 relative of a rounding boundary), without a division
+    // 1/clamp(c, 1, N) in double for c = 0..K (corr.py:65 clamps the count by the number of query points, which is below K
+    // only when the first cloud is the smaller one): (float)(double(sum) * rcp[c]) is the correctly rounded fp32 quotient
+    // for every integer divisor <= 2^20 (x/c is never within 2^-34 relative of a rounding boundary), without a division
     double* s_rcp = reinterpret_cast<double*>(smem_raw + tab_bytes + (size_t)p.warps * lookup_warp_bytes(K));
-    for (int i = threadIdx.x; i <= K; i += blockDim.x) s_rcp[i] = i > 0 ? 1.0 / (double)i : 1.0;
+    for (int i = threadIdx.x; i <= K; i += blockDim.x) s_rcp[i] = i > 0 ? 1.0 / (double)min(i, p.N) : 1.0;
 
     if (active_warp && lane == 0) mbar_init(s_bar, 1);
     if (threadIdx.x == 0) mbar_init(&s_tabbar, 1);
@@ -215,7 +217,7 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
         const int b = (int)(seg / p.N);
         long long seg_end = (long long)(b + 1) * p.N;
         if (seg_end > pt_end) seg_end = pt_end;
-        const float4* tab_g = p.tab + (size_t)b * p.N;
+        const float4* tab_g = p.tab + (size_t)b * p.M;
         int* counter = dyn ? reinterpret_cast<int*>(p.moments + (size_t)b * PVRAFT_MOMENTS + 15) : nullptr;
         if constexpr (DET)   // slot 15 of the sample's fixed-point moments
             counter = dyn ? reinterpret_cast<int*>(reinterpret_cast<unsigned long long*>(p.moments) + ((size_t)b * PVRAFT_MOMENTS + 15) * kFxWords) : nullptr;
@@ -226,10 +228,10 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
         };
         __syncthreads();   // previous segment's readers are done (table and point counter)
         if (SMEM_TAB && threadIdx.x == 0) {
-            // the sample's table: N*16 bytes by the TMA engine (written once per forward, long before this launch, so the
+            // the sample's table: M*16 bytes by the TMA engine (written once per forward, long before this launch, so the
             // request may precede griddepcontrol.wait and overlap the previous kernel's tail)
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            const unsigned bytes = (unsigned)p.N * 16u;
+            const unsigned bytes = (unsigned)p.M * 16u;
             mbar_expect_tx(&s_tabbar, bytes);
             for (unsigned off = 0; off < bytes; off += 32768u)
                 bulk_g2s(smem_raw + off, reinterpret_cast<const unsigned char*>(tab_g) + off, min(32768u, bytes - off), &s_tabbar);
@@ -391,7 +393,7 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
                     }
                 }
                 __syncwarp();
-                {   // sum / clamp(count, 1, N) (corr.py:65-66; rcp[0] = 1) of every cell, and zeros in the row padding
+                {   // sum / clamp(count, 1, N) (corr.py:65-66; rcp[0] = 1, N = query points) of every cell, and zeros in the row padding
                     float* vo = p.vox + pt * p.vox_ld;
 #pragma unroll
                     for (int i = 0; i < 3; ++i) {   // columns 0..95 (3 levels: 81 cells + the padding of the 96-wide layout)
@@ -655,13 +657,21 @@ static float cube_threshold(float r) {
     return t;
 }
 
+// The gather table of a sample (M rows of 16 bytes) is staged in shared memory when it fits next to 8 warps' stages and the
+// reciprocal table; otherwise the kernel gathers from global memory (through L1 / L2)
+static bool lookup_table_in_smem(long long M, int K) {
+    const size_t tab = (((size_t)M * 16 + 127) & ~(size_t)127);
+    const size_t rcp_bytes = (size_t)(K + 1) * sizeof(double) + 8;
+    return tab + 8 * lookup_warp_bytes(K) + rcp_bytes <= (size_t)kSmemBudget;
+}
+
 template <int KPL, bool POW2, bool HALF, bool DET>
 static int launch_lookup(LookupParams& p, cudaStream_t st) {
     const int K = KPL * 32;
     const size_t per_warp = lookup_warp_bytes(K);
-    const size_t tab = (((size_t)p.N * 16 + 127) & ~(size_t)127);
+    const size_t tab = (((size_t)p.M * 16 + 127) & ~(size_t)127);   // the gather table of the second cloud
     const size_t rcp_bytes = (size_t)(K + 1) * sizeof(double) + 8;
-    const bool smem_tab = tab + 8 * per_warp + rcp_bytes <= (size_t)kSmemBudget;
+    const bool smem_tab = lookup_table_in_smem(p.M, K);
     const size_t avail = (size_t)kSmemBudget - (smem_tab ? tab : 0) - rcp_bytes;
     int warps = (int)(avail / per_warp);
     if (warps > kLookupThreads / 32) warps = kLookupThreads / 32;
@@ -709,6 +719,8 @@ extern "C" int pvraft_corr_reorder(const float* val_in, const int32_t* idx_in, i
     return check_launch("corr_reorder");
 }
 
+extern "C" int pvraft_corr_lookup_table_in_smem(int M, int K) { return M > 0 && K > 0 && lookup_table_in_smem(M, K) ? 1 : 0; }
+
 extern "C" int pvraft_xyz_pad_fwd(const float* xyz, int64_t rows, float* out, void* stream) {
     if (!xyz || !out || rows <= 0) return fail(PVRAFT_ERR_BAD_ARG, "xyz_pad: bad argument");
     k_xyz_pad<<<(unsigned)((rows + 255) / 256), 256, 0, (cudaStream_t)stream>>>(xyz, rows, reinterpret_cast<float4*>(out));
@@ -717,22 +729,23 @@ extern "C" int pvraft_xyz_pad_fwd(const float* xyz, int64_t rows, float* out, vo
 
 template <bool DET>
 static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half, const float* xyz2_pad, const float* coords, int B, int N,
-                           int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
+                           int M, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
                            int8_t* dbg_cube, void* ws, void* stream) {
     if (DET && moments && !ws) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: the deterministic form needs its workspace");
     if (!corr_val || !corr_idx || !xyz2_pad || !coords || !vox || !knn_sel) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: null pointer");
-    if (B <= 0 || N <= 0) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: B=%d N=%d", B, N);
+    if (B <= 0 || N <= 0 || M <= 0) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: B=%d N=%d M=%d", B, N, M);
     if (levels < 1 || levels > 4) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_lookup: levels=%d (1..4 supported)", levels);
     if (!(base_scale > 0.f)) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: base_scale must be > 0");
     if ((reinterpret_cast<uintptr_t>(xyz2_pad) & 15u) || (reinterpret_cast<uintptr_t>(corr_idx) & 15u))
         return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: xyz2_pad and corr_idx must be 16-byte aligned (bulk copies)");
-    if (half && N > 65536) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_lookup: uint16 candidate ids need N <= 65536 (N=%d)", N);
+    if (half && M > 65536)
+        return fail(PVRAFT_ERR_UNSUPPORTED, "corr_lookup: uint16 candidate ids need M <= 65536 points in the second cloud (M=%d)", M);
     LookupParams p{};
     p.corr_val = corr_val; p.corr_idx = corr_idx; p.tab = reinterpret_cast<const float4*>(xyz2_pad); p.coords = coords;
     p.vox = vox; p.knn_sel = reinterpret_cast<float4*>(knn_sel); p.knn_slot = knn_slot;
     p.moments = DET && moments ? static_cast<double*>(ws) : moments;
     p.dbg_cube = dbg_cube;
-    p.B = B; p.N = N; p.K = K; p.levels = levels;
+    p.B = B; p.N = N; p.M = M; p.K = K; p.levels = levels;
     p.vox_ld = vox_ld > 0 ? vox_ld : levels * 27;
     if (p.vox_ld < levels * 27 || p.vox_ld > levels * 27 + 32) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: vox_ld=%d", vox_ld);
     bool pow2 = true;
@@ -781,37 +794,69 @@ static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half
     return fx_flush_f64(static_cast<const unsigned long long*>(ws), B, 15, PVRAFT_MOMENTS, PVRAFT_MOMENTS, moments, st);
 }
 
+extern "C" int pvraft_corr_lookup_nm_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad,
+                                         const float* coords, int B, int N, int M, int K, int levels, float base_scale,
+                                         float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
+                                         int8_t* dbg_cube, void* stream) {
+    return corr_lookup_any<false>(corr_val, corr_idx, false, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld, knn_sel,
+                                  knn_slot, moments, dbg_cube, nullptr, stream);
+}
+
 extern "C" int pvraft_corr_lookup_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad,
                                       const float* coords, int B, int N, int K, int levels, float base_scale,
                                       float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
                                       int8_t* dbg_cube, void* stream) {
-    return corr_lookup_any<false>(corr_val, corr_idx, false, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel, knn_slot,
-                                  moments, dbg_cube, nullptr, stream);
+    return pvraft_corr_lookup_nm_fwd(corr_val, corr_idx, xyz2_pad, coords, B, N, N, K, levels, base_scale, vox, vox_ld, knn_sel,
+                                     knn_slot, moments, dbg_cube, stream);
+}
+
+extern "C" int pvraft_corr_lookup_bf16_nm_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
+                                              const float* coords, int B, int N, int M, int K, int levels, float base_scale,
+                                              float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
+                                              int8_t* dbg_cube, void* stream) {
+    return corr_lookup_any<false>(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld,
+                                  knn_sel, knn_slot, moments, dbg_cube, nullptr, stream);
 }
 
 extern "C" int pvraft_corr_lookup_bf16_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
                                            const float* coords, int B, int N, int K, int levels, float base_scale,
                                            float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
                                            int8_t* dbg_cube, void* stream) {
-    return corr_lookup_any<false>(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel,
-                                  knn_slot, moments, dbg_cube, nullptr, stream);
+    return pvraft_corr_lookup_bf16_nm_fwd(corr_val_bf16, corr_idx_u16, xyz2_pad, coords, B, N, N, K, levels, base_scale, vox, vox_ld,
+                                          knn_sel, knn_slot, moments, dbg_cube, stream);
 }
 
 extern "C" int64_t pvraft_corr_lookup_det_workspace_bytes(int B) { return (int64_t)B * PVRAFT_MOMENTS * kFxWords * 8; }
 
+extern "C" int pvraft_corr_lookup_nm_det_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
+                                             int B, int N, int M, int K, int levels, float base_scale, float* vox, int vox_ld,
+                                             float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace,
+                                             void* stream) {
+    return corr_lookup_any<true>(corr_val, corr_idx, false, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld, knn_sel,
+                                 knn_slot, moments, dbg_cube, workspace, stream);
+}
+
 extern "C" int pvraft_corr_lookup_det_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords, int B,
                                           int N, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
                                           int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace, void* stream) {
-    return corr_lookup_any<true>(corr_val, corr_idx, false, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel, knn_slot,
-                                 moments, dbg_cube, workspace, stream);
+    return pvraft_corr_lookup_nm_det_fwd(corr_val, corr_idx, xyz2_pad, coords, B, N, N, K, levels, base_scale, vox, vox_ld, knn_sel,
+                                         knn_slot, moments, dbg_cube, workspace, stream);
+}
+
+extern "C" int pvraft_corr_lookup_bf16_nm_det_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
+                                                  const float* coords, int B, int N, int M, int K, int levels, float base_scale, float* vox,
+                                                  int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
+                                                  void* workspace, void* stream) {
+    return corr_lookup_any<true>(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld,
+                                 knn_sel, knn_slot, moments, dbg_cube, workspace, stream);
 }
 
 extern "C" int pvraft_corr_lookup_bf16_det_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
                                                const float* coords, int B, int N, int K, int levels, float base_scale, float* vox, int vox_ld,
                                                float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace,
                                                void* stream) {
-    return corr_lookup_any<true>(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, K, levels, base_scale, vox, vox_ld, knn_sel,
-                                 knn_slot, moments, dbg_cube, workspace, stream);
+    return pvraft_corr_lookup_bf16_nm_det_fwd(corr_val_bf16, corr_idx_u16, xyz2_pad, coords, B, N, N, K, levels, base_scale, vox, vox_ld,
+                                              knn_sel, knn_slot, moments, dbg_cube, workspace, stream);
 }
 
 // fp32 correlation values -> bf16 (round to nearest even), int32 candidate ids -> uint16: the 4-byte-per-candidate state

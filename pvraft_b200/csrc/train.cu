@@ -641,12 +641,13 @@ __global__ void __launch_bounds__(256) k_maxk_bwd(const float* __restrict__ dy, 
 // ---------------------------------------------------------------------------------------------------------------------
 // Correlation lookup, backward w.r.t. the truncated correlation values (model/corr.py:47-66 and :84; the index math is
 // under no_grad in the reference, corr.py:52-62, and the query coordinates are detached, RAFTSceneFlow.py:41):
-//   d corr[b,n,k] = sum_levels valid_l(k) * g_vox[b,n,l*27+cell_l(k)] / max(count_l[cell], 1)  +  [k selected as j-th nn] g_sel[b,n,j,0]
+//   d corr[b,n,k] = sum_levels valid_l(k) * g_vox[b,n,l*27+cell_l(k)] / clamp(count_l[cell], 1, N)  +  [k selected as j-th nn] g_sel[b,n,j,0]
+// (N = query points; the table holds the M points of the second cloud)
 // One warp per point; cells are re-derived with the forward's arithmetic (cell edge by true division or exact reciprocal).
 // ---------------------------------------------------------------------------------------------------------------------
 struct LookupBwdParams {
     const int32_t* corr_idx;
-    const float4* tab;
+    const float4* tab;         // [B,M]
     const float* coords;
     const int32_t* knn_slot;   // [B,N,32]
     const float* g_vox;        // [B,N,vox_ld]
@@ -655,6 +656,7 @@ struct LookupBwdParams {
     int B, N, K, levels, vox_ld;
     float r[4], inv_r[4];
     int pow2;
+    int M;
 };
 
 __global__ void __launch_bounds__(256) k_lookup_bwd(const LookupBwdParams p) {
@@ -671,7 +673,7 @@ __global__ void __launch_bounds__(256) k_lookup_bwd(const LookupBwdParams p) {
     }
     __syncwarp();
     const float cx = __ldg(p.coords + pt * 3), cy = __ldg(p.coords + pt * 3 + 1), cz = __ldg(p.coords + pt * 3 + 2);
-    const float4* tab = p.tab + (size_t)b * p.N;
+    const float4* tab = p.tab + (size_t)b * p.M;
     const int32_t* ri = p.corr_idx + pt * p.K;
     float* dr = p.d_corr + pt * p.K;
     // pass 1: counts per (level, cell)
@@ -697,7 +699,7 @@ __global__ void __launch_bounds__(256) k_lookup_bwd(const LookupBwdParams p) {
             const float qz = rintf(p.pow2 ? __fmul_rn(dz, p.inv_r[l]) : __fdiv_rn(dz, p.r[l]));
             if (fmaxf(fmaxf(fabsf(qx), fabsf(qy)), fabsf(qz)) <= 1.f) {
                 const int cell = l * 27 + (int)fmaf(qx, 9.f, fmaf(qy, 3.f, qz + 13.f));
-                g += s_g[w][cell] / (float)s_cnt[w][cell];
+                g += s_g[w][cell] / (float)min(s_cnt[w][cell], p.N);
             }
         }
         dr[k] = g;
@@ -711,21 +713,21 @@ __global__ void __launch_bounds__(256) k_lookup_bwd(const LookupBwdParams p) {
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Truncated correlation, backward (model/corr.py:95-100 then the top-k gather of :37-38), sparse: only the K kept entries
-// of a row carry gradient, so the dense N x N gradient of the reference is never formed:
+// of a row carry gradient, so the dense N x M gradient of the reference is never formed (f2, d_f2: M rows per sample):
 //   d f1[b,n,:] = (1/sqrt(C)) sum_k g[b,n,k] f2[b,idx[b,n,k],:]      d f2[b,m,:] += (1/sqrt(C)) g[b,n,k] f1[b,n,:]  (m = idx[b,n,k])
 // One warp per row; lanes own C/32 (<= 8) consecutive channels.
 // ---------------------------------------------------------------------------------------------------------------------
 template <int CPL, bool DET>
 __global__ void __launch_bounds__(256) k_corr_init_bwd(const float* __restrict__ g, const int32_t* __restrict__ idx, const float* __restrict__ f1,
-                                                       const float* __restrict__ f2, int B, int N, int K, float scale, float* __restrict__ d_f1,
-                                                       float* __restrict__ d_f2) {
+                                                       const float* __restrict__ f2, int B, int N, int M, int K, float scale,
+                                                       float* __restrict__ d_f1, float* __restrict__ d_f2) {
     constexpr int C = CPL * 32;
     const int lane = lane_id(), w = warp_id();
     const long long row = (long long)blockIdx.x * 8 + w;
     if (row >= (long long)B * N) return;
     const int b = (int)(row / N);
-    const float* f2b = f2 + (size_t)b * N * C;
-    float* d2b = d_f2 + (size_t)b * N * C;
+    const float* f2b = f2 + (size_t)b * M * C;
+    float* d2b = d_f2 + (size_t)b * M * C;
     float a[CPL], acc[CPL];
 #pragma unroll
     for (int i = 0; i < CPL; ++i) { a[i] = __ldg(f1 + row * C + lane * CPL + i) * scale; acc[i] = 0.f; }
@@ -737,8 +739,8 @@ __global__ void __launch_bounds__(256) k_corr_init_bwd(const float* __restrict__
             const float gj = __shfl_sync(kFull, gk, j);
             const int m = __shfl_sync(kFull, ik, j);
             if (gj == 0.f) continue;
-            if constexpr (DET) {   // d_f2 is the fixed-point workspace [B,N,C]
-                unsigned long long* fx = reinterpret_cast<unsigned long long*>(d_f2) + ((size_t)b * N + m) * C * kFxWords;
+            if constexpr (DET) {   // d_f2 is the fixed-point workspace [B,M,C]
+                unsigned long long* fx = reinterpret_cast<unsigned long long*>(d_f2) + ((size_t)b * M + m) * C * kFxWords;
 #pragma unroll
                 for (int i = 0; i < CPL; ++i) {
                     acc[i] = fmaf(gj, __ldg(f2b + (size_t)m * C + lane * CPL + i), acc[i]);
@@ -989,15 +991,16 @@ extern "C" int pvraft_maxk_bwd(const float* dy, const uint8_t* arg, int64_t pts,
     return check_launch("maxk_bwd");
 }
 
-extern "C" int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
-                                      const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int K, int levels, float base_scale,
-                                      float* d_corr, void* stream) {
+extern "C" int pvraft_corr_lookup_nm_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
+                                         const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int M, int K, int levels,
+                                         float base_scale, float* d_corr, void* stream) {
     if (!corr_idx || !xyz2_pad || !coords || !knn_slot || !g_vox || !g_sel || !d_corr) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup_bwd: null pointer");
-    if (B <= 0 || N <= 0 || K < 32 || levels < 1 || levels > 4 || vox_ld < levels * 27) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup_bwd: bad shape");
+    if (B <= 0 || N <= 0 || M <= 0 || K < 32 || levels < 1 || levels > 4 || vox_ld < levels * 27)
+        return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup_bwd: bad shape");
     LookupBwdParams p{};
     p.corr_idx = corr_idx; p.tab = reinterpret_cast<const float4*>(xyz2_pad); p.coords = coords; p.knn_slot = knn_slot;
     p.g_vox = g_vox; p.g_sel = g_sel; p.d_corr = d_corr;
-    p.B = B; p.N = N; p.K = K; p.levels = levels; p.vox_ld = vox_ld;
+    p.B = B; p.N = N; p.M = M; p.K = K; p.levels = levels; p.vox_ld = vox_ld;
     p.pow2 = 1;
     for (int l = 0; l < 4; ++l) {
         const float r = (float)((double)base_scale * (double)(1 << l));   // as pvraft_corr_lookup_fwd
@@ -1011,35 +1014,56 @@ extern "C" int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2
     return check_launch("corr_lookup_bwd");
 }
 
+extern "C" int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
+                                      const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int K, int levels, float base_scale,
+                                      float* d_corr, void* stream) {
+    return pvraft_corr_lookup_nm_bwd(corr_idx, xyz2_pad, coords, knn_slot, g_vox, vox_ld, g_sel, B, N, N, K, levels, base_scale, d_corr,
+                                     stream);
+}
+
 template <bool DET>
-static int corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C, int K, float* d_fmap1,
-                         float* d_fmap2, void* ws, void* stream) {
-    if (!g || !idx || !fmap1 || !fmap2 || !d_fmap1 || !d_fmap2 || B <= 0 || N <= 0 || K <= 0 || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "corr_init_bwd: bad argument");
+static int corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M, int C, int K,
+                         float* d_fmap1, float* d_fmap2, void* ws, void* stream) {
+    if (!g || !idx || !fmap1 || !fmap2 || !d_fmap1 || !d_fmap2 || B <= 0 || N <= 0 || M <= 0 || K <= 0 || (DET && !ws))
+        return fail(PVRAFT_ERR_BAD_ARG, "corr_init_bwd: bad argument");
     float* kd2 = DET ? static_cast<float*>(ws) : d_fmap2;
     const long long rows = (long long)B * N;
     const unsigned blocks = (unsigned)((rows + 7) / 8);
     const float scale = 1.0f / sqrtf((float)C);
     cudaStream_t st = (cudaStream_t)stream;
     switch (C) {
-        case 32: k_corr_init_bwd<1, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, kd2); break;
-        case 64: k_corr_init_bwd<2, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, kd2); break;
-        case 128: k_corr_init_bwd<4, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, kd2); break;
-        case 256: k_corr_init_bwd<8, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, K, scale, d_fmap1, kd2); break;
+        case 32: k_corr_init_bwd<1, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, M, K, scale, d_fmap1, kd2); break;
+        case 64: k_corr_init_bwd<2, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, M, K, scale, d_fmap1, kd2); break;
+        case 128: k_corr_init_bwd<4, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, M, K, scale, d_fmap1, kd2); break;
+        case 256: k_corr_init_bwd<8, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, M, K, scale, d_fmap1, kd2); break;
         default: return fail(PVRAFT_ERR_UNSUPPORTED, "corr_init_bwd: C=%d (32, 64, 128, 256)", C);
     }
     int rc = check_launch("corr_init_bwd");
     if (rc || !DET) return rc;
-    return fx_flush_f32(static_cast<const unsigned long long*>(ws), 1, rows * C, rows * C, 0, d_fmap2, st);
+    const long long rows2 = (long long)B * M;
+    return fx_flush_f32(static_cast<const unsigned long long*>(ws), 1, rows2 * C, rows2 * C, 0, d_fmap2, st);
+}
+
+extern "C" int pvraft_corr_init_nm_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M, int C,
+                                       int K, float* d_fmap1, float* d_fmap2, void* stream) {
+    return corr_init_bwd<false>(g, idx, fmap1, fmap2, B, N, M, C, K, d_fmap1, d_fmap2, nullptr, stream);
 }
 
 extern "C" int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C, int K,
                                     float* d_fmap1, float* d_fmap2, void* stream) {
-    return corr_init_bwd<false>(g, idx, fmap1, fmap2, B, N, C, K, d_fmap1, d_fmap2, nullptr, stream);
+    return pvraft_corr_init_nm_bwd(g, idx, fmap1, fmap2, B, N, N, C, K, d_fmap1, d_fmap2, stream);
 }
 
-extern "C" int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int N, int C) { return (int64_t)B * N * C * kFxWords * 8; }
+extern "C" int64_t pvraft_corr_init_nm_bwd_det_workspace_bytes(int B, int M, int C) { return (int64_t)B * M * C * kFxWords * 8; }
+
+extern "C" int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int N, int C) { return pvraft_corr_init_nm_bwd_det_workspace_bytes(B, N, C); }
+
+extern "C" int pvraft_corr_init_nm_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M,
+                                           int C, int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream) {
+    return corr_init_bwd<true>(g, idx, fmap1, fmap2, B, N, M, C, K, d_fmap1, d_fmap2, workspace, stream);
+}
 
 extern "C" int pvraft_corr_init_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C,
                                         int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream) {
-    return corr_init_bwd<true>(g, idx, fmap1, fmap2, B, N, C, K, d_fmap1, d_fmap2, workspace, stream);
+    return pvraft_corr_init_nm_bwd_det(g, idx, fmap1, fmap2, B, N, N, C, K, d_fmap1, d_fmap2, workspace, stream);
 }

@@ -100,10 +100,13 @@ def corr_reorder(val, idx):
     return val_out, idx_out
 
 
-def corr_state_pack_bf16(val, idx):
-    """Reordered fp32 / int32 state -> (bf16 values, uint16 ids held in an int16 tensor): 4 B per candidate and iteration."""
-    if int(idx.shape[1]) > 65536:
-        raise ValueError('uint16 candidate ids need N <= 65536')
+def corr_state_pack_bf16(val, idx, m=None):
+    """Reordered fp32 / int32 state -> (bf16 values, uint16 ids held in an int16 tensor): 4 B per candidate and iteration.
+    The ids are rows of the second cloud, so its size `m` (default: the rows of the state, i.e. clouds of equal size) is what
+    the 16-bit ids must address."""
+    m = int(idx.shape[1]) if m is None else int(m)
+    if m > 65536:
+        raise ValueError(f'uint16 candidate ids need a second cloud of at most 65536 points (N2 <= 65536), got {m}')
     v16 = torch.empty(val.shape, dtype=torch.bfloat16, device=val.device)
     i16 = torch.empty(idx.shape, dtype=torch.int16, device=idx.device)
     _count(lib().pvraft_corr_state_pack_bf16(_p(val), _p(idx, torch.int32), val.numel(), _p(v16, torch.bfloat16), _p(i16, torch.int16),
@@ -112,11 +115,14 @@ def corr_state_pack_bf16(val, idx):
 
 
 def corr_matmul(fmap1_pm, fmap2_pm):
-    """Point-major feature maps [B,N,C] -> all-pairs correlation [B,N,N] / sqrt(C) on wgmma (3xTF32)."""
+    """Point-major feature maps [B,N,C] x [B,M,C] -> all-pairs correlation [B,N,M] / sqrt(C) on wgmma (3xTF32)."""
     b, n, c = fmap1_pm.shape
-    corr = torch.empty(b, n, n, dtype=torch.float32, device=fmap1_pm.device)
-    ws = torch.empty(int(lib().pvraft_corr_matmul_workspace_bytes(b, n, c)), dtype=torch.uint8, device=fmap1_pm.device)
-    _count(lib().pvraft_corr_matmul_fwd(_p(fmap1_pm), _p(fmap2_pm), b, n, c, _p(corr), _p(ws, torch.uint8), _stream()),
+    m = fmap2_pm.shape[1]
+    if fmap2_pm.shape != (b, m, c):
+        raise ValueError(f'corr_matmul: feature maps {tuple(fmap1_pm.shape)} and {tuple(fmap2_pm.shape)}')
+    corr = torch.empty(b, n, m, dtype=torch.float32, device=fmap1_pm.device)
+    ws = torch.empty(int(lib().pvraft_corr_matmul_nm_workspace_bytes(b, n, m, c)), dtype=torch.uint8, device=fmap1_pm.device)
+    _count(lib().pvraft_corr_matmul_nm_fwd(_p(fmap1_pm), _p(fmap2_pm), b, n, m, c, _p(corr), _p(ws, torch.uint8), _stream()),
            'corr_matmul')
     return corr
 
@@ -131,14 +137,15 @@ def corr_topk(corr, k):
 
 
 def corr_dense(fmap1_pm, fmap2_pm):
-    """corr_matmul for any N: a ragged N is zero-padded to the next multiple of 128 (the kernel's tile) and the result cropped."""
-    n = fmap1_pm.shape[1]
-    pad = (-n) % 128
-    if pad == 0:
+    """corr_matmul for any N and M: each ragged size is zero-padded on its own to the next multiple of 128 (the kernel's
+    tile), and the result cropped."""
+    n, m = fmap1_pm.shape[1], fmap2_pm.shape[1]
+    pad_n, pad_m = (-n) % 128, (-m) % 128
+    if pad_n == 0 and pad_m == 0:
         return corr_matmul(fmap1_pm, fmap2_pm)
-    f1 = torch.nn.functional.pad(fmap1_pm, (0, 0, 0, pad)).contiguous()
-    f2 = torch.nn.functional.pad(fmap2_pm, (0, 0, 0, pad)).contiguous()
-    return corr_matmul(f1, f2)[:, :n, :n].contiguous()
+    f1 = torch.nn.functional.pad(fmap1_pm, (0, 0, 0, pad_n)).contiguous()
+    f2 = torch.nn.functional.pad(fmap2_pm, (0, 0, 0, pad_m)).contiguous()
+    return corr_matmul(f1, f2)[:, :n, :m].contiguous()
 
 
 CORR_ROW_MAX = 49152      # widest row the top-K kernels stage in shared memory (csrc/corr_topk.cu)
@@ -193,26 +200,30 @@ def corr_plan(b, n, m, c, k, window=CORR_ROW_MAX, cap=CORR_SLAB_CAP):
 
 
 def corr_build(fmap1_pm, fmap2_pm, k, plan=None):
-    """Point-major feature maps [B,N,C] -> (val [B,N,K] f32, idx [B,N,K] int32): the K largest correlations of every row,
-    in ascending column order (corr_topk of corr_dense), without the [B,N,N] matrix when N > 49152 (see CorrPlan).
-    Both paths give the same bits."""
+    """Point-major feature maps [B,N,C] x [B,M,C] -> (val [B,N,K] f32, idx [B,N,K] int32 rows of fmap2): the K largest
+    correlations of every row, in ascending column order (corr_topk of corr_dense), without the [B,N,M] matrix when
+    M > 49152 (see CorrPlan).  Both paths give the same bits."""
     b, n, c = fmap1_pm.shape
     m = fmap2_pm.shape[1]
-    if fmap2_pm.shape != (b, m, c) or m != n:
-        raise ValueError(f'corr_build: feature maps {tuple(fmap1_pm.shape)} and {tuple(fmap2_pm.shape)} (clouds of equal size)')
+    if fmap2_pm.dim() != 3 or fmap2_pm.shape[0] != b or fmap2_pm.shape[2] != c:
+        raise ValueError(f'corr_build: feature maps {tuple(fmap1_pm.shape)} and {tuple(fmap2_pm.shape)} (same batch and channels)')
+    if k > m:
+        raise ValueError(f'truncate_k={k} exceeds the number of points {m} of the second cloud')
     if c % 32 != 0:
         raise NotImplementedError(f'calculate_corr: {c} feature channels (the wgmma GEMM needs a multiple of 32; the model has 128)')
     plan = corr_plan(b, n, m, c, k) if plan is None else plan
     if plan.dense:
         return corr_topk(corr_dense(fmap1_pm, fmap2_pm), k)
     dev = fmap1_pm.device
-    npad = _pad128(n)
-    # tf32 hi/lo of both maps, split once.  The padding rows are left unset: a row of A or B only reaches the slab entries of
-    # that row / column, and the top-K steps never read the entries past N.
-    ws = torch.empty(4, b, npad, c, dtype=torch.float32, device=dev)
-    for i, f in enumerate((fmap1_pm, fmap2_pm)):
+    npad, mpad = _pad128(n), _pad128(m)
+    # tf32 hi/lo of both maps, split once, each map's rows per sample padded to 128 on their own.  The padding rows are left
+    # unset: a row of A or B only reaches the slab entries of that row / column, and the top-K steps never read the entries
+    # past N / M.
+    ws_a = torch.empty(2, b, npad, c, dtype=torch.float32, device=dev)
+    ws_b = torch.empty(2, b, mpad, c, dtype=torch.float32, device=dev)
+    for ws, f, rows_f in ((ws_a, fmap1_pm, n), (ws_b, fmap2_pm, m)):
         for s in range(b):
-            _count(lib().pvraft_tf32_split_fwd(_p(f[s]), n * c, _p(ws[2 * i, s]), _p(ws[2 * i + 1, s]), _stream()), 'tf32_split')
+            _count(lib().pvraft_tf32_split_fwd(_p(f[s]), rows_f * c, _p(ws[0, s]), _p(ws[1, s]), _stream()), 'tf32_split')
     nw = len(plan.windows)
     wk = nw * k
     rows = max(r for _, r in plan.row_blocks)
@@ -222,16 +233,38 @@ def corr_build(fmap1_pm, fmap2_pm, k, plan=None):
     val = torch.empty(b, n, k, dtype=torch.float32, device=dev)
     idx = torch.empty(b, n, k, dtype=torch.int32, device=dev)
     for s in range(b):
-        split = [_p(ws[q, s]) for q in range(4)]
+        split = [_p(ws_a[0, s]), _p(ws_a[1, s]), _p(ws_b[0, s]), _p(ws_b[1, s])]
         for r0, nr in plan.row_blocks:
             for j, (c0, nc) in enumerate(plan.windows):
-                _count(lib().pvraft_corr_matmul_window_fwd(*split, 1, npad, c, r0, nr, c0, nc, _p(slab), plan.ld, _stream()),
+                _count(lib().pvraft_corr_matmul_window_nm_fwd(*split, 1, npad, mpad, c, r0, nr, c0, nc, _p(slab), plan.ld, _stream()),
                        'corr_matmul_window')
                 _count(lib().pvraft_corr_topk_window_fwd(_p(slab), nr, nc, plan.ld, k, c0, None, _p(cand_val) + 4 * j * k,
                                                          _p(cand_idx, torch.int32) + 4 * j * k, wk, _stream()), 'corr_topk_window')
             _count(lib().pvraft_corr_topk_window_fwd(_p(cand_val), nr, wk, wk, k, 0, _p(cand_idx, torch.int32), _p(val[s, r0:r0 + nr]),
                                                      _p(idx[s, r0:r0 + nr], torch.int32), k, _stream()), 'corr_topk_merge')
     return val, idx
+
+
+def _table_rows(xyz2_pad, b):
+    """M, the points of the second cloud, from its gather table [B,M,4]."""
+    if xyz2_pad.dim() != 3 or xyz2_pad.shape[0] != b or xyz2_pad.shape[2] != 4:
+        raise ValueError(f'expected a gather table [B={b},M,4], got {tuple(xyz2_pad.shape)}')
+    return int(xyz2_pad.shape[1])
+
+
+def check_pair(xyz1, xyz2, truncate_k):
+    """The shape rules of a pair of clouds p = [xyz1 [B,N1,3], xyz2 [B,N2,3]]: one batch size, at least 32 points in each
+    cloud (the 32-neighbour graphs) and at least truncate_k points in the second (the candidates of a row are distinct
+    rows of xyz2).  N1 and N2 may differ; within a batch every sample has the same N1 and the same N2."""
+    if xyz1.dim() != 3 or xyz1.shape[-1] != 3 or xyz2.dim() != 3 or xyz2.shape[-1] != 3:
+        raise ValueError(f'expected p = [xyz1 [B,N1,3], xyz2 [B,N2,3]], got {tuple(xyz1.shape)} and {tuple(xyz2.shape)}')
+    if xyz1.shape[0] != xyz2.shape[0]:
+        raise ValueError(f'xyz1 {tuple(xyz1.shape)} and xyz2 {tuple(xyz2.shape)} must have the same batch size')
+    n1, n2 = int(xyz1.shape[1]), int(xyz2.shape[1])
+    if min(n1, n2) < KNN:
+        raise ValueError(f'need at least {KNN} points per cloud, got N1={n1} and N2={n2}')
+    if truncate_k > n2:
+        raise ValueError(f'truncate_k={truncate_k} exceeds the number of points {n2} of the second cloud')
 
 
 def xyz_pad(xyz):
@@ -244,9 +277,11 @@ def xyz_pad(xyz):
 
 def corr_lookup(corr_val, corr_idx, xyz2_pad, coords, levels, base_scale, vox=None, knn_sel=None, moments=None,
                 want_slots=False, want_cube=False, vox_ld=None):
-    """-> dict(vox [B,N,pad4(levels*27)], knn_sel [B,N,32,4], moments [B,16] f64, [knn_slot], [cube]).
+    """State [B,N,K], gather table xyz2_pad [B,M,4] of the second cloud, query coords [B,N,3]
+    -> dict(vox [B,N,pad4(levels*27)], knn_sel [B,N,32,4], moments [B,16] f64, [knn_slot], [cube]).
     `cube` [B,N,K,levels] int8 is the fused kernel's own cell decision for every candidate (test hook)."""
     b, n, k = corr_val.shape
+    m = _table_rows(xyz2_pad, b)
     dev = corr_val.device
     if vox_ld is None:
         vox_ld = (levels * 27 + 3) // 4 * 4      # rows padded to a multiple of 4 floats (zero-filled by the kernel)
@@ -260,16 +295,16 @@ def corr_lookup(corr_val, corr_idx, xyz2_pad, coords, levels, base_scale, vox=No
     cube = torch.empty(b, n, k, levels, dtype=torch.int8, device=dev) if want_cube else None
     half = corr_val.dtype == torch.bfloat16   # reduced-precision state: bf16 values + uint16 ids (stored as int16)
     args = ((_p(corr_val, torch.bfloat16), _p(corr_idx, torch.int16)) if half else (_p(corr_val), _p(corr_idx, torch.int32))) + \
-        (_p(xyz2_pad), _p(coords), b, n, k, levels, float(base_scale), _p(vox), vox.shape[-1], _p(knn_sel), _p(slots, torch.int32),
+        (_p(xyz2_pad), _p(coords), b, n, m, k, levels, float(base_scale), _p(vox), vox.shape[-1], _p(knn_sel), _p(slots, torch.int32),
          _p(moments, torch.float64), _p(cube, torch.int8))
     if deterministic():
         ws = _det_workspace(lib().pvraft_corr_lookup_det_workspace_bytes(b), dev)
-        fn = lib().pvraft_corr_lookup_bf16_det_fwd if half else lib().pvraft_corr_lookup_det_fwd
+        fn = lib().pvraft_corr_lookup_bf16_nm_det_fwd if half else lib().pvraft_corr_lookup_nm_det_fwd
         _count(fn(*args, _p(ws, torch.uint8), _stream()), 'corr_lookup_det')
     elif half:
-        _count(lib().pvraft_corr_lookup_bf16_fwd(*args, _stream()), 'corr_lookup_bf16')
+        _count(lib().pvraft_corr_lookup_bf16_nm_fwd(*args, _stream()), 'corr_lookup_bf16')
     else:
-        _count(lib().pvraft_corr_lookup_fwd(*args, _stream()), 'corr_lookup')
+        _count(lib().pvraft_corr_lookup_nm_fwd(*args, _stream()), 'corr_lookup')
     return dict(vox=vox, knn_sel=knn_sel, moments=moments, knn_slot=slots, cube=cube)
 
 
@@ -606,25 +641,38 @@ def maxk_bwd(dy, arg, pts, c):
     return dx
 
 
+def lookup_table_in_smem(m, k):
+    """True when corr_lookup stages the gather table of a second cloud of m points in shared memory at truncate_k = k (the
+    faster path).  At K = 512 a table of 8 192 points fits and one of 12 000 does not: the kernel then gathers from global
+    memory."""
+    return bool(lib().pvraft_corr_lookup_table_in_smem(int(m), int(k)))
+
+
 def corr_lookup_bwd(corr_idx, xyz2_pad, coords, slots, g_vox, g_sel, levels, base_scale):
+    """-> d_corr [B,N,K]; the state's ids are rows of the gather table xyz2_pad [B,M,4]."""
     b, n, k = corr_idx.shape
+    m = _table_rows(xyz2_pad, b)
     d_corr = torch.empty(b, n, k, dtype=torch.float32, device=corr_idx.device)
-    _count(lib().pvraft_corr_lookup_bwd(_p(corr_idx, torch.int32), _p(xyz2_pad), _p(coords), _p(slots, torch.int32), _p(g_vox),
-                                        g_vox.shape[-1], _p(g_sel), b, n, k, levels, float(base_scale), _p(d_corr), _stream()),
+    _count(lib().pvraft_corr_lookup_nm_bwd(_p(corr_idx, torch.int32), _p(xyz2_pad), _p(coords), _p(slots, torch.int32), _p(g_vox),
+                                           g_vox.shape[-1], _p(g_sel), b, n, m, k, levels, float(base_scale), _p(d_corr), _stream()),
            'corr_lookup_bwd')
     return d_corr
 
 
 def corr_init_bwd(g, idx, fmap1, fmap2):
+    """g, idx [B,N,K], fmap1 [B,N,C], fmap2 [B,M,C] -> (d fmap1 [B,N,C], d fmap2 [B,M,C])."""
     b, n, c = fmap1.shape
+    m = fmap2.shape[1]
+    if fmap2.shape != (b, m, c):
+        raise ValueError(f'corr_init_bwd: feature maps {tuple(fmap1.shape)} and {tuple(fmap2.shape)}')
     d1 = torch.empty_like(fmap1)
     d2 = torch.zeros_like(fmap2)
-    args = (_p(g), _p(idx, torch.int32), _p(fmap1), _p(fmap2), b, n, c, g.shape[-1], _p(d1), _p(d2))
+    args = (_p(g), _p(idx, torch.int32), _p(fmap1), _p(fmap2), b, n, m, c, g.shape[-1], _p(d1), _p(d2))
     if deterministic():
-        ws = _det_workspace(lib().pvraft_corr_init_bwd_det_workspace_bytes(b, n, c), fmap1.device)
-        _count(lib().pvraft_corr_init_bwd_det(*args, _p(ws, torch.uint8), _stream()), 'corr_init_bwd_det')
+        ws = _det_workspace(lib().pvraft_corr_init_nm_bwd_det_workspace_bytes(b, m, c), fmap1.device)
+        _count(lib().pvraft_corr_init_nm_bwd_det(*args, _p(ws, torch.uint8), _stream()), 'corr_init_bwd_det')
     else:
-        _count(lib().pvraft_corr_init_bwd(*args, _stream()), 'corr_init_bwd')
+        _count(lib().pvraft_corr_init_nm_bwd(*args, _stream()), 'corr_init_bwd')
     return d1, d2
 
 

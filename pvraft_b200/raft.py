@@ -40,7 +40,7 @@ class _RaftBase(nn.Module):
     # way).  `use_cuda_graph = None` (default) replays graphs for inference batches of at most 2 samples from the first call,
     # and for larger batches from the SECOND call with the same shape and unchanged weights (a stream of differently sized
     # clouds, or evaluation calls interleaved with optimizer steps, stays eager: a capture costs three forwards);
-    # True / False (or PVRAFT_CUDA_GRAPH=1 / 0) force it on / off.  One graph per (B, N, num_iters), at most 8 kept; inputs are
+    # True / False (or PVRAFT_CUDA_GRAPH=1 / 0) force it on / off.  One graph per (B, N1, N2, num_iters), at most 8 kept; inputs are
     # copied into the graph's static buffers, outputs are returned as copies.  The kernels read DERIVED copies of the weights
     # (tf32 hi/lo splits, folded products, bias sums, PReLU slopes known to the host) that are fixed at capture time, so a
     # graph is only valid for the parameter values it was captured with: every entry records (version, data_ptr) of all
@@ -61,9 +61,12 @@ class _RaftBase(nn.Module):
         self.reset_graphs()
         return self
 
-    def _graph_key(self, xyz1, num_iters):
-        # a graph records the kernels of one setting of torch.use_deterministic_algorithms: never replayed under the other
-        return (tuple(xyz1.shape), xyz1.device, int(num_iters), ops.deterministic())
+    def _graph_key(self, xyz1, xyz2, num_iters):
+        # a graph records the kernels of one setting of torch.use_deterministic_algorithms: never replayed under the other.
+        # A pair of clouds of different sizes adds the second cloud's shape (pairs that share N1 and differ in N2 run on
+        # different buffers); a pair of equal sizes keeps the short key.
+        key = (tuple(xyz1.shape), xyz1.device, int(num_iters), ops.deterministic())
+        return key if xyz2.shape == xyz1.shape else key + (tuple(xyz2.shape),)
 
     def _stamp(self):
         return tuple((q._version, q.data_ptr()) for q in self.parameters())
@@ -71,7 +74,7 @@ class _RaftBase(nn.Module):
     def _graphed(self, p, num_iters):
         xyz1, xyz2 = p[0].detach().contiguous().float(), p[1].detach().contiguous().float()
         graphs = self.__dict__.setdefault('_graphs', {})
-        key = self._graph_key(xyz1, num_iters)
+        key = self._graph_key(xyz1, xyz2, num_iters)
         entry = graphs.get(key)
         stamp = self._stamp()
         if entry is not None and entry[3] != stamp:
@@ -115,7 +118,7 @@ class _RaftBase(nn.Module):
                     graph = True     # host-bound from the first call
                 else:                # larger batches: once the same shape has come back with the same weights
                     seen = self.__dict__.setdefault('_seen', {})
-                    key, stamp = self._graph_key(p[0], num_iters), self._stamp()
+                    key, stamp = self._graph_key(p[0], p[1], num_iters), self._stamp()
                     graph = seen.get(key) == stamp
                     if len(seen) > 64:
                         seen.clear()
@@ -126,18 +129,22 @@ class _RaftBase(nn.Module):
 
     def _encode(self, p):
         xyz1, xyz2 = p[0], p[1]
-        if xyz1.dim() != 3 or xyz1.shape[-1] != 3 or xyz1.shape != xyz2.shape:
-            raise ValueError('expected p = [xyz1 [B,N,3], xyz2 [B,N,3]]')
+        ops.check_pair(xyz1, xyz2, self.corr_block.truncate_k)
         xyz1 = xyz1.detach().contiguous().float()
         xyz2 = xyz2.detach().contiguous().float()
-        # both clouds go through the shared feature encoder as one batch of 2B samples (RAFTSceneFlow.py:25-26: every op is
-        # per sample): half the launches, and 2B*N/128 tiles fill the 132 SMs more evenly
         b = xyz1.shape[0]
-        both = torch.cat([xyz1, xyz2], 0)
-        fmap, graph2 = self.feature_extractor(both, point_major=True)
-        fmap1, fmap2 = fmap[:b], fmap[b:]
-        graph = Graph(graph2.nbr[:b], graph2._rel[:b], graph2.k_neighbors, [b * xyz1.shape[1]] * 2,
-                      None if graph2.order is None else graph2.order[:b])   # pc1's graph
+        if xyz1.shape == xyz2.shape:
+            # both clouds go through the shared feature encoder as one batch of 2B samples (RAFTSceneFlow.py:25-26: every op
+            # is per sample): half the launches, and 2B*N/128 tiles fill the 132 SMs more evenly
+            both = torch.cat([xyz1, xyz2], 0)
+            fmap, graph2 = self.feature_extractor(both, point_major=True)
+            fmap1, fmap2 = fmap[:b], fmap[b:]
+            graph = Graph(graph2.nbr[:b], graph2._rel[:b], graph2.k_neighbors, [b * xyz1.shape[1]] * 2,
+                          None if graph2.order is None else graph2.order[:b])   # pc1's graph
+        else:
+            # clouds of different sizes: one encoder pass per cloud (the kernels take one N per launch)
+            fmap1, graph = self.feature_extractor(xyz1, point_major=True)   # pc1's graph
+            fmap2, _ = self.feature_extractor(xyz2, point_major=True)
         self.corr_block.init_module_pm(fmap1, fmap2, xyz2)               # :29
         # the reference rebuilds the same pc1 graph for the context encoder (:31); reuse it
         fct1, graph_context = self.context_extractor(xyz1, graph=graph, point_major=True)

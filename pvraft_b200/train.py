@@ -200,8 +200,9 @@ class MaxKFn(torch.autograd.Function):
 
 
 class CorrInitFn(torch.autograd.Function):
-    """(fmap1, fmap2) [B,N,C] -> the K largest correlations of every row, in the lookup kernel's stored order, with their
-    column ids (not differentiable).  Backward is sparse: only the kept entries carry gradient (model/corr.py:37-40)."""
+    """(fmap1 [B,N1,C], fmap2 [B,N2,C]) -> the K largest correlations of every row of fmap1, in the lookup kernel's stored
+    order, with their column ids (rows of fmap2; not differentiable).  Backward is sparse: only the kept entries carry
+    gradient (model/corr.py:37-40)."""
 
     @staticmethod
     def forward(ctx, fmap1, fmap2, k, corr_block):
@@ -220,7 +221,8 @@ class CorrInitFn(torch.autograd.Function):
 
 
 class CorrLookupFn(torch.autograd.Function):
-    """corr_val [B,N,K] (+ ids, gather table, query coordinates) -> voxel means [B,N,levels*27], kNN 4-vectors [B,N*32,4]."""
+    """corr_val [B,N1,K] (+ ids, gather table [B,N2,4], query coordinates [B,N1,3]) -> voxel means [B,N1,levels*27],
+    kNN 4-vectors [B,N1*32,4]."""
 
     @staticmethod
     def forward(ctx, corr_val, corr_idx, xyz2p, coords, levels, base_scale):
@@ -301,20 +303,25 @@ def flot_refine(m, flow, graph):
 
 
 def rsf_forward(model, p, num_iters):
-    """RSF.forward with gradients (model/RAFTSceneFlow.py:22-50) -> list of num_iters flows [B,N,3]."""
+    """RSF.forward with gradients (model/RAFTSceneFlow.py:22-50) -> list of num_iters flows [B,N1,3]."""
+    cb = model.corr_block
+    ops.check_pair(p[0], p[1], cb.truncate_k)
     xyz1 = p[0].detach().contiguous().float()
     xyz2 = p[1].detach().contiguous().float()
-    if xyz1.dim() != 3 or xyz1.shape[-1] != 3 or xyz1.shape != xyz2.shape:
-        raise ValueError('expected p = [xyz1 [B,N,3], xyz2 [B,N,3]]')
     b, n, _ = xyz1.shape
-    cb = model.corr_block
     if cb.state_dtype != torch.float32:
         raise NotImplementedError("training differentiates through the fp32 state: call model.set_precision('fp32')")
-    both = torch.cat([xyz1, xyz2], 0)
-    g_both = Graph.construct_graph(both, 32)                                   # :25-26 (one batch of 2B clouds)
-    fmap = flot_encoder(model.feature_extractor, both, g_both)
-    graph1 = Graph(g_both.nbr[:b].contiguous(), g_both._rel[:b].contiguous(), 32, [b * n] * 2)   # (the training path does not use .order)
-    corr_val, corr_idx = CorrInitFn.apply(fmap[:b], fmap[b:], cb.truncate_k, cb)   # :29
+    if xyz1.shape == xyz2.shape:
+        both = torch.cat([xyz1, xyz2], 0)
+        g_both = Graph.construct_graph(both, 32)                               # :25-26 (one batch of 2B clouds)
+        fmap = flot_encoder(model.feature_extractor, both, g_both)
+        graph1 = Graph(g_both.nbr[:b].contiguous(), g_both._rel[:b].contiguous(), 32, [b * n] * 2)   # (the training path does not use .order)
+        fmap1, fmap2 = fmap[:b], fmap[b:]
+    else:                                                                      # clouds of different sizes: one pass per cloud
+        graph1 = Graph.construct_graph(xyz1, 32)
+        fmap1 = flot_encoder(model.feature_extractor, xyz1, graph1)
+        fmap2 = flot_encoder(model.feature_extractor, xyz2, Graph.construct_graph(xyz2, 32))
+    corr_val, corr_idx = CorrInitFn.apply(fmap1, fmap2, cb.truncate_k, cb)     # :29
     xyz2p = ops.xyz_pad(xyz2)
     fct1 = flot_encoder(model.context_extractor, xyz1, graph1)                 # :31 (same cloud, same graph)
     net = torch.tanh(fct1[..., :model.hidden_dim])                             # :33-35
