@@ -19,9 +19,22 @@
  *     per-point feature array (one point's channels are contiguous), coordinates are [B,N,3].
  *   - GroupNorm statistics travel as raw double-precision sums ("stats": [B,8,2] = per sample,
  *     per group (sum, sum of squares)); producers ACCUMULATE with atomics, so the caller zeroes
- *     them (cudaMemsetAsync) before the producing call (the *_det producers: a fixed order, see
- *     "Deterministic entry points").
+ *     them (cudaMemsetAsync) before the producing call (in a fixed order with a det_workspace, see "Deterministic mode").
  *   - Weights are passed in the reference's own state_dict layouts ([Cout,Cin(,1(,1))] row-major).
+ *   - Deterministic mode (what pvraft_b200 runs while torch.are_deterministic_algorithms_enabled() is true).  Every entry
+ *     point that reduces floating-point values takes `void* det_workspace` as its last argument before `stream`.  NULL runs
+ *     the default kernels, which accumulate with atomics in an order that varies from run to run.  Otherwise det_workspace
+ *     is pvraft_*_det_workspace_bytes(...) bytes (the size query declared beside the entry point) of caller-provided,
+ *     8-byte aligned scratch that the caller ZERO-FILLS before every call.  The kernels then add exact fixed-point values
+ *     (Q64.64 in 128 bits) into the workspace, and one launch adds the workspace, rounded, into the destination the default
+ *     kernels accumulate into.  Integer additions are exact, and every value added is a floating-point sum whose order is
+ *     a function of the shapes (a point, a 128-point tile, a warp's rows of a grid sized from the shapes), so the results
+ *     are bitwise identical from run to run, under graph replay, and for any SM count.  Each value added is truncated
+ *     toward zero to a multiple of 2^-64, so the exact sum of n values is known to within an ABSOLUTE n * 2^-64 (terms
+ *     below 2^-64 vanish); it is rounded once to double and then added to the destination.  A non-finite value, or one of
+ *     magnitude >= 2^62, makes its destination entry NaN.  Same results as the default kernels up to summation order.
+ *     Forward statistics are per (sample, tile / point), so with N % 128 == 0 a sample's statistics do not depend on the
+ *     batch.
  */
 #ifndef PVRAFT_B200_H
 #define PVRAFT_B200_H
@@ -32,7 +45,7 @@
 extern "C" {
 #endif
 
-#define PVRAFT_VERSION 100 /* 0.1.0 */
+#define PVRAFT_VERSION 200 /* 0.2.0 */
 
 #if defined(__GNUC__)
 #define PVRAFT_API __attribute__((visibility("default")))
@@ -59,39 +72,28 @@ PVRAFT_API int pvraft_device_info(int* sm_count, int* smem_optin_bytes);
 /* ------------------------------------------------------------------------------------------------
  * All-pairs feature correlation on the Hopper tensor cores (wgmma) with an fp32-accurate 3xTF32 split.
  * Replaces CorrBlock.calculate_corr, model/corr.py:95-100: corr[b,i,j] = <fmap1[b,i,:], fmap2[b,j,:]> / sqrt(C).
- *   fmap1, fmap2 [B,N,C] POINT-major f32 -> corr [B,N,N] f32.   N % 128 == 0, C % 32 == 0.
- *   workspace: pvraft_corr_matmul_workspace_bytes(B,N,C) bytes (16-byte aligned) for the hi/lo operand splits.
+ *   fmap1 [B,N,C], fmap2 [B,M,C] POINT-major f32 -> corr [B,N,M] f32.   N % 128 == 0, M % 128 == 0, C % 32 == 0.
+ *   workspace: pvraft_corr_matmul_workspace_bytes(B,N,M,C) bytes (16-byte aligned) for the hi/lo operand splits.
  * --------------------------------------------------------------------------------------------- */
-PVRAFT_API int64_t pvraft_corr_matmul_workspace_bytes(int B, int N, int C);
-PVRAFT_API int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, int B, int N, int C, float* corr, void* workspace,
-                           void* stream);
-/* Clouds of different sizes: fmap1 [B,N,C] x fmap2 [B,M,C] -> corr [B,N,M]; N % 128 == 0, M % 128 == 0, C % 32 == 0.
- * The workspace is pvraft_corr_matmul_nm_workspace_bytes(B,N,M,C) bytes.  With M == N these are the two entry points above
- * (which forward to them). */
-PVRAFT_API int64_t pvraft_corr_matmul_nm_workspace_bytes(int B, int N, int M, int C);
-PVRAFT_API int pvraft_corr_matmul_nm_fwd(const float* fmap1, const float* fmap2, int B, int N, int M, int C, float* corr,
-                                         void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_corr_matmul_workspace_bytes(int B, int N, int M, int C);
+PVRAFT_API int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, int B, int N, int M, int C, float* corr, void* workspace,
+                                      void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * The same GEMM over one window of the correlation matrix, for clouds whose N x N matrix is not built whole.
+ * The same GEMM over one window of the correlation matrix, for clouds whose N x M matrix is not built whole.
  *   pvraft_tf32_split_fwd: x [n] f32 -> hi = tf32(x), lo = tf32(x - hi) (the operand split of pvraft_corr_matmul_fwd),
  *     n % 4 == 0, 16-byte aligned buffers.  Run once per feature map and build, not once per window.
- *   pvraft_corr_matmul_window_fwd: split operands a_hi/a_lo (fmap1) and b_hi/b_lo (fmap2), each [B,N,C] point-major with
- *     N % 128 == 0, C % 32 == 0
+ *   pvraft_corr_matmul_window_fwd: split operands a_hi/a_lo (fmap1) [B,N,C] and b_hi/b_lo (fmap2) [B,M,C], point-major
+ *     with N % 128 == 0, M % 128 == 0 (each sample's operand rows padded separately), C % 32 == 0
  *     -> corr [B, R, ldc] with R = rows rounded up to 128: corr[b,i,j] = <fmap1[b,r0+i,:], fmap2[b,c0+j,:]> / sqrt(C) for
  *     i < R, j < cols rounded up to 128.  Whole 128 x 128 tiles are written: an operand row past the caller's points (a
  *     padding row, of any content) only reaches the slab rows / columns past `rows` / `cols`, which the caller ignores.
- *     r0, c0 multiples of 128; ldc % 4 == 0; the window's whole tiles lie inside [0, N).  Every value is bit-identical to
- *     the same entry of pvraft_corr_matmul_fwd on the same operands.
+ *     r0, c0 multiples of 128; ldc % 4 == 0; the window's whole row tiles lie inside [0, N) and its column tiles inside
+ *     [0, M).  Every value is bit-identical to the same entry of pvraft_corr_matmul_fwd on the same operands.
  * --------------------------------------------------------------------------------------------- */
 PVRAFT_API int pvraft_tf32_split_fwd(const float* x, int64_t n, float* hi, float* lo, void* stream);
 PVRAFT_API int pvraft_corr_matmul_window_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
-                                             int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream);
-/* The window GEMM for clouds of different sizes: a_hi/a_lo [B,N,C], b_hi/b_lo [B,M,C], N and M multiples of 128 (each
- * sample's operand rows padded separately); the window's whole row tiles lie inside [0, N) and its column tiles inside
- * [0, M).  pvraft_corr_matmul_window_fwd is this entry point with M == N. */
-PVRAFT_API int pvraft_corr_matmul_window_nm_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
-                                                int M, int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream);
+                                             int M, int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Correlation truncation: the K largest entries of every row of a dense correlation matrix.
@@ -129,7 +131,7 @@ PVRAFT_API int pvraft_corr_reorder(const float* val_in, const int32_t* idx_in, i
  * Point-voxel correlation lookup (index + reduce part), one fused pass over the K candidates of
  * every point.  Replaces CorrBlock.get_voxel_feature up to (not incl.) out_conv, model/corr.py:47-71,
  * and CorrBlock.get_knn_feature up to (not incl.) knn_conv, model/corr.py:75-91.
- *   corr_val [B,N,K] f32, corr_idx [B,N,K] int32 (rows of xyz2), xyz2_pad [B,N,4] = (x,y,z,0) rows of the second cloud
+ *   corr_val [B,N,K] f32, corr_idx [B,N,K] int32 (rows of xyz2, < M), xyz2_pad [B,M,4] = (x,y,z,0) rows of the second cloud
  *   (pvraft_xyz_pad_fwd, once per forward; 16-byte aligned, as corr_idx), coords [B,N,3]
  *   -> vox      [B,N,vox_ld]     (vox_ld >= levels*27, 0 = dense; pad columns are written as zeros so that the
  *                                consumer can read rows with 128-bit loads)  channel = level*27 + cell; mean corr of the candidates whose
@@ -146,37 +148,30 @@ PVRAFT_API int pvraft_corr_reorder(const float* val_in, const int32_t* idx_in, i
  *   -> dbg_cube [B,N,K,levels] int8  cell id or -1 of every candidate AS DERIVED BY THE FUSED KERNEL ITSELF (the coarsest-cube
  *                                pre-test, the compaction and the per-level cell codes); test hook, NULL in production
  * K in {32,64,128,256,512,1024}; 1 <= levels <= 4; knn fixed at 32.
+ * N query points (corr_val, corr_idx, coords and every output have N rows per sample), M points in the second cloud.  A cell
+ * mean divides by clamp(count, 1, N) (model/corr.py:65), which differs from the count only when N < K.  The gather table is
+ * staged in shared memory while M*16 bytes fit next to the warps' stages, and read from global memory (through L1/L2) otherwise.
+ * det_workspace: pvraft_corr_lookup_det_workspace_bytes(B) bytes or NULL ("Deterministic mode"; it orders the moments).
  * --------------------------------------------------------------------------------------------- */
-/* The same lookup on the reduced-precision state of BASELINE.json configs[2] ("bf16 mode", SURVEY.md H7): correlation values as
- * bf16 bit patterns and candidate ids as uint16 (N <= 65536) -- 4 B instead of 8 B per candidate and iteration.  Index math
- * (coordinates, cells, kNN distances) stays fp32 and bit-exact; values are widened to fp32 exactly and accumulated in fp32, so
- * the outputs equal pvraft_corr_lookup_fwd on the bf16-rounded correlations.  K in {128,256,512,1024}.
- * pvraft_corr_state_pack_bf16 converts a reordered fp32/int32 state (round to nearest even). */
-PVRAFT_API int pvraft_corr_lookup_bf16_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
-                                const float* coords, int B, int N, int K, int levels, float base_scale, float* vox, int vox_ld,
-                                float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* stream);
-PVRAFT_API int pvraft_corr_state_pack_bf16(const float* val, const int32_t* idx, int64_t n, uint16_t* val_out, uint16_t* idx_out, void* stream);
-
 /* xyz [rows,3] -> out [rows,4] = (x,y,z,0): the gather table of the lookup kernel (one 128-bit load per candidate). */
 PVRAFT_API int pvraft_xyz_pad_fwd(const float* xyz, int64_t rows, float* out, void* stream);
 PVRAFT_API int pvraft_corr_lookup_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
-                           int B, int N, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
-                           int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* stream);
-/* Clouds of different sizes: N query points (corr_val, corr_idx, coords and every output have N rows per sample), M points
- * in the second cloud (xyz2_pad [B,M,4]; candidate ids < M).  A cell mean divides by clamp(count, 1, N) (model/corr.py:65),
- * which differs from the count only when N < K.  The gather table is staged in shared memory while M*16 bytes fit next to
- * the warps' stages, and read from global memory (through L1/L2) otherwise.  The bf16 form needs M <= 65536.  The entry
- * points above are these with M == N. */
-PVRAFT_API int pvraft_corr_lookup_nm_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
-                                         int B, int N, int M, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
-                                         int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* stream);
+                                      int B, int N, int M, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
+                                      int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_corr_lookup_det_workspace_bytes(int B);
 /* 1 when the lookup stages the gather table of a second cloud of M points in shared memory at truncate_k = K, 0 when it
  * gathers from global memory (a query for tools and tests). */
 PVRAFT_API int pvraft_corr_lookup_table_in_smem(int M, int K);
-PVRAFT_API int pvraft_corr_lookup_bf16_nm_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
-                                              const float* coords, int B, int N, int M, int K, int levels, float base_scale, float* vox,
-                                              int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
-                                              void* stream);
+/* The same lookup on the reduced-precision state of BASELINE.json configs[2] ("bf16 mode", SURVEY.md H7): correlation values as
+ * bf16 bit patterns and candidate ids as uint16 (M <= 65536) -- 4 B instead of 8 B per candidate and iteration.  Index math
+ * (coordinates, cells, kNN distances) stays fp32 and bit-exact; values are widened to fp32 exactly and accumulated in fp32, so
+ * the outputs equal pvraft_corr_lookup_fwd on the bf16-rounded correlations.  K in {128,256,512,1024}; det_workspace as there.
+ * pvraft_corr_state_pack_bf16 converts a reordered fp32/int32 state (round to nearest even). */
+PVRAFT_API int pvraft_corr_lookup_bf16_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
+                                           const float* coords, int B, int N, int M, int K, int levels, float base_scale, float* vox,
+                                           int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
+                                           void* det_workspace, void* stream);
+PVRAFT_API int pvraft_corr_state_pack_bf16(const float* val, const int32_t* idx, int64_t n, uint16_t* val_out, uint16_t* idx_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Generic fused (GroupNorm -> activation -> 1x1 conv [-> bias] [-> ReLU]) layer over points with
@@ -218,7 +213,9 @@ typedef struct pvraft_linear_args {
     int B, N, cin, cout;
 } pvraft_linear_args;
 
-PVRAFT_API int pvraft_linear_fwd(const pvraft_linear_args* a, void* stream);
+/* det_workspace: pvraft_linear_det_workspace_bytes(B) bytes or NULL ("Deterministic mode"; it orders out_stats). */
+PVRAFT_API int pvraft_linear_fwd(const pvraft_linear_args* a, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_linear_det_workspace_bytes(int B);
 
 /* ------------------------------------------------------------------------------------------------
  * The same fused layer on the Hopper tensor cores (TMA + wgmma), fp32-accurate through a 3xTF32 operand split.
@@ -276,7 +273,9 @@ typedef struct pvraft_tc_linear_args {
                                serialization and then fetches them while the previous kernel drains.  0 is always safe. */
 } pvraft_tc_linear_args;
 
-PVRAFT_API int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream);
+/* det_workspace: pvraft_tc_linear_det_workspace_bytes(B) bytes or NULL ("Deterministic mode"; it orders out_stats). */
+PVRAFT_API int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_tc_linear_det_workspace_bytes(int B);
 
 /* ---------------------------------------------------------------------------------------------
  * The update chain of one RAFT iteration in one launch: the same five layers and the same bits as the five
@@ -421,9 +420,12 @@ PVRAFT_API int pvraft_gru_fwd(const pvraft_gru_args* a, void* stream);
  *   order [B,N] int32 or NULL: the LOCAL point processed r-th in every sample (pvraft_point_order_fwd: a Morton rank table).
  *   It changes no result, only which points a CTA works on at the same time, so that their overlapping neighbourhoods are
  *   gathered from L1 instead of L2.
+ *   det_workspace: pvraft_setconv_edge_det_workspace_bytes(B) bytes or NULL ("Deterministic mode").
  * --------------------------------------------------------------------------------------------- */
 PVRAFT_API int pvraft_setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
-                            int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order, void* stream);
+                                       int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order,
+                                       void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_setconv_edge_det_workspace_bytes(int B);
 
 /* ------------------------------------------------------------------------------------------------
  * FlowHead output stage + RAFT coordinate update.  Replaces model/update.py:69,71-72 (conv1, cat,
@@ -477,26 +479,30 @@ PVRAFT_API int pvraft_point_order_fwd(const float* xyz, int B, int N, int32_t* p
  * Gradient contract (SURVEY.md section 8b): what tools/engine.py:131-147 differentiates through.
  * The training path runs layer by layer; each backward entry point below pairs with a forward one.
  * Parameter-gradient outputs are ACCUMULATED with atomics into buffers the caller has zeroed (in an order that varies from
- * run to run; the *_det forms under "Deterministic entry points" accumulate in a fixed order).
+ * run to run; in a fixed order with a det_workspace, see "Deterministic mode").  The det_workspace of each entry point is
+ * pvraft_<name>_det_workspace_bytes(...) bytes, declared beside it.
  * ============================================================================================= */
 
 /* 1x1 convolution (pvraft_linear_fwd without prologue / activation), weight and bias gradient:
  *   x [rows,cin], dy [rows,cout]  ->  dW[o,i] += sum_r dy[r,o] x[r,i]  (row stride dw_ld floats, 0 = cin),  db[o] += sum_r dy[r,o] (or NULL).
  * The data gradient dx = dy . W is pvraft_linear_fwd with the transposed weight.  cin <= 256, cout <= 128. */
 PVRAFT_API int pvraft_linear_wgrad(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
-                        void* stream);
+                                   void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_linear_wgrad_det_workspace_bytes(int cin, int cout);
 
 /* GroupNorm(8) + activation backward (model/corr.py:17-18,25-26; model/flot/gconv.py:27-36 via autograd in the reference):
  *   x, dy [B,rows,C]; stats [B,8,2] raw sums of x (as produced in the forward); count = rows * C/8; act/slope as pvraft_gn_act_fwd
  *   -> dx [B,rows,C]; dgamma, dbeta [C] double (accumulated); dslope [1] double (PReLU slope gradient, or NULL);
  *      gsum [B,8,2] double scratch, ZEROED by the caller. */
 PVRAFT_API int pvraft_gn_act_bwd(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta, double count,
-                      int act, float slope, int B, int64_t rows, int C, double* gsum, double* dgamma, double* dbeta, double* dslope,
-                      float* dx, const float* slope_dev, const uint8_t* arg, void* stream);
+                                 int act, float slope, int B, int64_t rows, int C, double* gsum, double* dgamma, double* dbeta,
+                                 double* dslope, float* dx, const float* slope_dev, const uint8_t* arg, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_gn_act_bwd_det_workspace_bytes(int B, int C);
 /* Backward of a linear layer with cin <= 4 and cout in {16,32,48,64,96,128} (the SetConv edge term and the knn_conv: rows = B*N*32) in one
  * pass over dy: dW [cout,dw_ld] += dy^T x, db [cout] += column sums (or NULL), dx [rows,cin] = dy W (or NULL).  W is [cout,w_ld]. */
 PVRAFT_API int pvraft_linear_bwd_small(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld, float* dW,
-                            int dw_ld, float* db, float* dx, void* stream);
+                                       int dw_ld, float* db, float* dx, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_linear_bwd_small_det_workspace_bytes(int cin, int cout);
 /* GroupNorm + activation + max over each point's 32 consecutive rows, fused (model/flot/gconv.py:76-80, model/corr.py:87-92):
  *   x [B, pts*32, C] -> y [B,pts,C], arg [B,pts,C] uint8 (first row attaining the maximum); count = pts*32 * C/8.
  * Its backward is pvraft_gn_act_bwd with `arg` set and dy = d y [B,pts,C]: the dense, 31/32-zero gradient of the max is never formed. */
@@ -508,8 +514,11 @@ PVRAFT_API int pvraft_gn_act_maxk_fwd(const float* x, const double* stats, const
  *             stats [B,8,2] accumulated sums of the result (or NULL)
  *   backward: dP[b,nbr,:] += dT[b,n,j,:]; dP[b,n,:] -= sum_j dT[b,n,j,:]   (dP zeroed by the caller; dE = dT)
  *   P [B,N,C], nbr [B,N,32] int32 local ids, E/dT [B,N,32,C]. */
-PVRAFT_API int pvraft_edge_fwd(const float* P, const int32_t* nbr, float* E, int B, int N, int C, double* stats, void* stream);
-PVRAFT_API int pvraft_edge_bwd(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* stream);
+PVRAFT_API int pvraft_edge_fwd(const float* P, const int32_t* nbr, float* E, int B, int N, int C, double* stats, void* det_workspace,
+                               void* stream);
+PVRAFT_API int64_t pvraft_edge_fwd_det_workspace_bytes(int B);
+PVRAFT_API int pvraft_edge_bwd(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_edge_bwd_det_workspace_bytes(int B, int N, int C);
 
 /* max over the 32 neighbours (model/flot/gconv.py:80, model/corr.py:92): x [pts,32,C] -> y [pts,C], arg [pts,C] uint8 (first
  * maximum); backward writes dx [pts,32,C] = dy at arg, 0 elsewhere. */
@@ -518,23 +527,18 @@ PVRAFT_API int pvraft_maxk_bwd(const float* dy, const uint8_t* arg, int64_t pts,
 
 /* Backward of pvraft_corr_lookup_fwd w.r.t. corr_val (model/corr.py:47-66,84; indices and coordinates carry no gradient:
  * corr.py:52-62 is under no_grad and RAFTSceneFlow.py:41 detaches the coordinates):
- *   g_vox [B,N,vox_ld], g_sel [B,N,32,4] (channel 0 used), knn_slot [B,N,32] from the forward -> d_corr [B,N,K] (overwritten). */
+ *   g_vox [B,N,vox_ld], g_sel [B,N,32,4] (channel 0 used), knn_slot [B,N,32] from the forward, xyz2_pad [B,M,4]
+ *   -> d_corr [B,N,K] (overwritten).  The means' divisor is clamp(count, 1, N), as in the forward. */
 PVRAFT_API int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
-                           const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int K, int levels, float base_scale,
-                           float* d_corr, void* stream);
-/* The same for clouds of different sizes: N query points, xyz2_pad [B,M,4]; the means' divisor is clamp(count, 1, N). */
-PVRAFT_API int pvraft_corr_lookup_nm_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
-                                         const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int M, int K, int levels,
-                                         float base_scale, float* d_corr, void* stream);
+                                      const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int M, int K, int levels,
+                                      float base_scale, float* d_corr, void* stream);
 
 /* Backward of the truncated correlation (model/corr.py:95-100 + the top-k gather of :37-38), sparse over the K kept entries:
- *   g [B,N,K], idx [B,N,K] (same stored order), fmap1/fmap2 [B,N,C] point-major
- *   -> d_fmap1 [B,N,C] (overwritten), d_fmap2 [B,N,C] (ACCUMULATED, zeroed by the caller).  C in {32,64,128,256}. */
-PVRAFT_API int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C, int K,
-                         float* d_fmap1, float* d_fmap2, void* stream);
-/* The same for clouds of different sizes: fmap1, d_fmap1 [B,N,C]; fmap2, d_fmap2 [B,M,C]; idx < M. */
-PVRAFT_API int pvraft_corr_init_nm_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M,
-                                       int C, int K, float* d_fmap1, float* d_fmap2, void* stream);
+ *   g [B,N,K], idx [B,N,K] (same stored order, ids < M), fmap1 [B,N,C], fmap2 [B,M,C] point-major
+ *   -> d_fmap1 [B,N,C] (overwritten), d_fmap2 [B,M,C] (ACCUMULATED, zeroed by the caller).  C in {32,64,128,256}. */
+PVRAFT_API int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M, int C,
+                                    int K, float* d_fmap1, float* d_fmap2, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int M, int C);
 
 /* Training extras on the device (SURVEY.md 8f row f3).  est, gt [points,3]; mask [points] (> 0 = valid) or NULL.
  *   pvraft_flow_metrics_fwd: acc[6] double, ZEROED by the caller, accumulates over the valid points
@@ -543,79 +547,19 @@ PVRAFT_API int pvraft_corr_init_nm_bwd(const float* g, const int32_t* idx, const
  *       [3],[4],[5] points with (epe<.05 or rel<.05), (epe<.1 or rel<.1), (epe>.3 or rel>.1), rel = epe/(||gt||+1e-4)  (metric.py:66-77)
  *   pvraft_flow_l1_bwd: d_est = g[0] * weight * sign(est - gt) / (3 acc[1]) on valid points, 0 elsewhere; g is a DEVICE scalar
  *       (the upstream gradient), acc the forward's accumulator: no host synchronisation between forward and backward. */
-PVRAFT_API int pvraft_flow_metrics_fwd(const float* est, const float* gt, const float* mask, int64_t points, double* acc, void* stream);
+PVRAFT_API int pvraft_flow_metrics_fwd(const float* est, const float* gt, const float* mask, int64_t points, double* acc, void* det_workspace,
+                                       void* stream);
+PVRAFT_API int64_t pvraft_flow_metrics_det_workspace_bytes(void);
 PVRAFT_API int pvraft_flow_l1_bwd(const float* est, const float* gt, const float* mask, int64_t points, const double* acc, const float* g,
                        float weight, float* d_est, void* stream);
 
-/* sizeof() of the argument structs as compiled into the library (0 = linear, 1 = corrfeat, 2 = gru,
- * 3 = flowout, 4 = tc_linear; -1 otherwise): lets a foreign-language binding verify its struct layout at load time. */
+/* sizeof() of the argument structs as compiled into the library (0 = linear, 1 = corrfeat, 2 = gru, 3 = flowout,
+ * 4 = tc_linear, 5 = knn_branch, 6 = update_chain; -1 otherwise): lets a foreign-language binding verify its struct layout
+ * at load time. */
 PVRAFT_API int pvraft_sizeof(int which);
 
 /* [B,C,N] <-> [B,N,C] transposes used at the reference-layout seams of the Python modules. */
 PVRAFT_API int pvraft_transpose_fwd(const float* in, int B, int R, int C, float* out, void* stream); /* [B,R,C] -> [B,C,R] */
-
-/* ------------------------------------------------------------------------------------------------------------------
- * Deterministic entry points (what pvraft_b200 runs while torch.are_deterministic_algorithms_enabled() is true).
- * Each takes the arguments of the entry point it mirrors plus `workspace`: pvraft_*_det*_workspace_bytes(...) bytes of
- * caller-provided, 8-byte aligned scratch that the caller ZERO-FILLS before every call.  The kernels add exact fixed-point
- * values (Q64.64 in 128 bits) into the workspace and then one launch adds the workspace, rounded, into the destination
- * the default form accumulates into.  Integer additions are exact, and every value added is a floating-point sum whose
- * order is a function of the shapes (a point, a 128-point tile, a warp's rows of a grid sized from the shapes), so the
- * results are bitwise identical from run to run, under graph replay, and for any SM count.  Each value added is truncated
- * toward zero to a multiple of 2^-64, so the exact sum of n values is known to within an ABSOLUTE n * 2^-64 (terms below
- * 2^-64 vanish); it is rounded once to double and then added to the destination.  A non-finite value,
- * or one of magnitude >= 2^62, makes its destination entry NaN.  Same results as the default forms up to summation order.
- * Forward statistics are per (sample, tile / point), so with N % 128 == 0 a sample's statistics do not depend on the batch.
- * ------------------------------------------------------------------------------------------------------------------ */
-PVRAFT_API int64_t pvraft_linear_det_workspace_bytes(int B);
-PVRAFT_API int pvraft_linear_det_fwd(const pvraft_linear_args* args, void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_tc_linear_det_workspace_bytes(int B);
-PVRAFT_API int pvraft_tc_linear_det_fwd(const pvraft_tc_linear_args* args, void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_setconv_edge_det_workspace_bytes(int B);
-PVRAFT_API int pvraft_setconv_edge_det_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
-                                           int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order,
-                                           void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_corr_lookup_det_workspace_bytes(int B);
-PVRAFT_API int pvraft_corr_lookup_det_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
-                                          int B, int N, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
-                                          int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace, void* stream);
-PVRAFT_API int pvraft_corr_lookup_bf16_det_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
-                                               const float* coords, int B, int N, int K, int levels, float base_scale, float* vox,
-                                               int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
-                                               void* workspace, void* stream);
-PVRAFT_API int pvraft_corr_lookup_nm_det_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
-                                             int B, int N, int M, int K, int levels, float base_scale, float* vox, int vox_ld,
-                                             float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace,
-                                             void* stream);
-PVRAFT_API int pvraft_corr_lookup_bf16_nm_det_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
-                                                  const float* coords, int B, int N, int M, int K, int levels, float base_scale, float* vox,
-                                                  int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
-                                                  void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_edge_det_fwd_workspace_bytes(int B);
-PVRAFT_API int pvraft_edge_det_fwd(const float* P, const int32_t* nbr, float* E, int B, int N, int C, double* stats, void* workspace,
-                                   void* stream);
-PVRAFT_API int64_t pvraft_flow_metrics_det_workspace_bytes(void);
-PVRAFT_API int pvraft_flow_metrics_det_fwd(const float* est, const float* gt, const float* mask, int64_t points, double* acc,
-                                           void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_linear_wgrad_det_workspace_bytes(int cin, int cout);
-PVRAFT_API int pvraft_linear_wgrad_det(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
-                                       void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_linear_bwd_small_det_workspace_bytes(int cin, int cout);
-PVRAFT_API int pvraft_linear_bwd_small_det(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld,
-                                           float* dW, int dw_ld, float* db, float* dx, void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_gn_act_bwd_det_workspace_bytes(int B, int C);
-PVRAFT_API int pvraft_gn_act_bwd_det(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta,
-                                     double count, int act, float slope, int B, int64_t rows, int C, double* gsum, double* dgamma,
-                                     double* dbeta, double* dslope, float* dx, const float* slope_dev, const uint8_t* arg,
-                                     void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_edge_bwd_det_workspace_bytes(int B, int N, int C);
-PVRAFT_API int pvraft_edge_bwd_det(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int N, int C);
-PVRAFT_API int pvraft_corr_init_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C,
-                                        int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream);
-PVRAFT_API int64_t pvraft_corr_init_nm_bwd_det_workspace_bytes(int B, int M, int C);
-PVRAFT_API int pvraft_corr_init_nm_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M,
-                                           int C, int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream);
 
 #ifdef __cplusplus
 }

@@ -75,31 +75,26 @@ _SIGNATURES = {
     'pvraft_version': (C.c_int, []),
     'pvraft_last_error_string': (C.c_char_p, []),
     'pvraft_device_info': (C.c_int, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
-    'pvraft_corr_matmul_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
-    'pvraft_corr_matmul_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_corr_matmul_nm_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
-    'pvraft_corr_matmul_nm_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_corr_matmul_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    'pvraft_corr_matmul_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_tf32_split_fwd': (C.c_int, [VP, C.c_int64, VP, VP, VP]),
     'pvraft_corr_matmul_window_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                                VP, C.c_int64, VP]),
-    'pvraft_corr_matmul_window_nm_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                                   C.c_int, VP, C.c_int64, VP]),
+                                                C.c_int, VP, C.c_int64, VP]),
     'pvraft_corr_topk_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_corr_topk_window_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, VP, VP, VP, C.c_int64, VP]),
     'pvraft_corr_reorder': (C.c_int, [VP, VP, C.c_int64, C.c_int, VP, VP, VP]),
     'pvraft_xyz_pad_fwd': (C.c_int, [VP, C.c_int64, VP, VP]),
-    'pvraft_corr_lookup_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                         VP, C.c_int, VP, VP, VP, VP, VP]),
-    'pvraft_corr_lookup_bf16_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                              VP, C.c_int, VP, VP, VP, VP, VP]),
-    'pvraft_corr_lookup_nm_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                            VP, C.c_int, VP, VP, VP, VP, VP]),
-    'pvraft_corr_lookup_bf16_nm_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                                 VP, C.c_int, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                         VP, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_bf16_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                              VP, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_corr_lookup_det_workspace_bytes': (C.c_int64, [C.c_int]),
     'pvraft_corr_lookup_table_in_smem': (C.c_int, [C.c_int, C.c_int]),
     'pvraft_corr_state_pack_bf16': (C.c_int, [VP, VP, C.c_int64, VP, VP, VP]),
-    'pvraft_linear_fwd': (C.c_int, [C.POINTER(LinearArgs), VP]),
-    'pvraft_tc_linear_fwd': (C.c_int, [C.POINTER(TcLinearArgs), VP]),
+    'pvraft_linear_fwd': (C.c_int, [C.POINTER(LinearArgs), VP, VP]),
+    'pvraft_linear_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_tc_linear_fwd': (C.c_int, [C.POINTER(TcLinearArgs), VP, VP]),
+    'pvraft_tc_linear_det_workspace_bytes': (C.c_int64, [C.c_int]),
     'pvraft_update_chain_fwd': (C.c_int, [C.POINTER(UpdateChainArgs), VP]),
     'pvraft_tc_weight_split':(C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_gn_act_fwd': (C.c_int, [VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int,
@@ -108,61 +103,34 @@ _SIGNATURES = {
     'pvraft_knn_branch_fwd': (C.c_int, [C.POINTER(KnnBranchArgs), VP]),
     'pvraft_point_order_fwd': (C.c_int, [VP, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_gru_fwd': (C.c_int, [C.POINTER(GruArgs), VP]),
-    'pvraft_setconv_edge_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP]),
+    'pvraft_setconv_edge_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_setconv_edge_det_workspace_bytes': (C.c_int64, [C.c_int]),
     'pvraft_flow_out_fwd': (C.c_int, [C.POINTER(FlowOutArgs), VP]),
     'pvraft_knn_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
     'pvraft_knn_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
-    'pvraft_linear_wgrad': (C.c_int, [VP, VP, C.c_int64, C.c_int, C.c_int, VP, C.c_int, VP, VP]),
+    'pvraft_linear_wgrad': (C.c_int, [VP, VP, C.c_int64, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP]),
+    'pvraft_linear_wgrad_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
     'pvraft_gn_act_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int64, C.c_int, VP, VP, VP, VP,
-                                    VP, VP, VP, VP]),
-    'pvraft_linear_bwd_small': (C.c_int, [VP, VP, VP, C.c_int64, C.c_int, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP]),
+                                    VP, VP, VP, VP, VP]),
+    'pvraft_gn_act_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
+    'pvraft_linear_bwd_small': (C.c_int, [VP, VP, VP, C.c_int64, C.c_int, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP, VP]),
+    'pvraft_linear_bwd_small_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
     'pvraft_gn_act_maxk_fwd': (C.c_int, [VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int64, C.c_int, VP, VP, VP, VP]),
-    'pvraft_edge_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, VP, VP]),
-    'pvraft_edge_bwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP]),
+    'pvraft_edge_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_edge_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_edge_bwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_edge_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
     'pvraft_maxk_fwd': (C.c_int, [VP, C.c_int64, C.c_int, VP, VP, VP]),
     'pvraft_maxk_bwd': (C.c_int, [VP, VP, C.c_int64, C.c_int, VP, VP]),
-    'pvraft_corr_lookup_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_int, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, VP, VP]),
-    'pvraft_corr_init_bwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_corr_lookup_nm_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_int, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                            VP, VP]),
-    'pvraft_corr_init_nm_bwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_flow_metrics_fwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP]),
+    'pvraft_corr_lookup_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_int, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                         VP, VP]),
+    'pvraft_corr_init_bwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
+    'pvraft_corr_init_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    'pvraft_flow_metrics_fwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, VP]),
+    'pvraft_flow_metrics_det_workspace_bytes': (C.c_int64, []),
     'pvraft_flow_l1_bwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, C.c_float, VP, VP]),
     'pvraft_sizeof': (C.c_int, [C.c_int]),
     'pvraft_transpose_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, VP]),
-    # deterministic forms (include/pvraft_b200.h, "Deterministic entry points"): the same arguments plus a zeroed workspace
-    'pvraft_linear_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_linear_det_fwd': (C.c_int, [C.POINTER(LinearArgs), VP, VP]),
-    'pvraft_tc_linear_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_tc_linear_det_fwd': (C.c_int, [C.POINTER(TcLinearArgs), VP, VP]),
-    'pvraft_setconv_edge_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_setconv_edge_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP]),
-    'pvraft_corr_lookup_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_corr_lookup_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                             VP, C.c_int, VP, VP, VP, VP, VP, VP]),
-    'pvraft_corr_lookup_bf16_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                                  VP, C.c_int, VP, VP, VP, VP, VP, VP]),
-    'pvraft_corr_lookup_nm_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                                VP, C.c_int, VP, VP, VP, VP, VP, VP]),
-    'pvraft_corr_lookup_bf16_nm_det_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                                     VP, C.c_int, VP, VP, VP, VP, VP, VP]),
-    'pvraft_edge_det_fwd_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_edge_det_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_flow_metrics_det_workspace_bytes': (C.c_int64, []),
-    'pvraft_flow_metrics_det_fwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, VP]),
-    'pvraft_linear_wgrad_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_linear_wgrad_det': (C.c_int, [VP, VP, C.c_int64, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP]),
-    'pvraft_linear_bwd_small_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_linear_bwd_small_det': (C.c_int, [VP, VP, VP, C.c_int64, C.c_int, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP, VP]),
-    'pvraft_gn_act_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_gn_act_bwd_det': (C.c_int, [VP, VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int64, C.c_int, VP, VP, VP,
-                                        VP, VP, VP, VP, VP, VP]),
-    'pvraft_edge_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
-    'pvraft_edge_bwd_det': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_corr_init_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
-    'pvraft_corr_init_bwd_det': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
-    'pvraft_corr_init_nm_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
-    'pvraft_corr_init_nm_bwd_det': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
 }
 EXPORTS = tuple(_SIGNATURES)
 

@@ -69,6 +69,7 @@ extern "C" int pvraft_sizeof(int which) {
         case 3: return (int)sizeof(pvraft_flowout_args);
         case 4: return (int)sizeof(pvraft_tc_linear_args);
         case 5: return (int)sizeof(pvraft_knn_branch_args);
+        case 6: return (int)sizeof(pvraft_update_chain_args);
         default: return -1;
     }
 }

@@ -249,15 +249,13 @@ static void launch_split(const float* x, long long n, float* hi, float* lo, cuda
 
 using namespace pvraft;
 
-extern "C" int64_t pvraft_corr_matmul_nm_workspace_bytes(int B, int N, int M, int C) {
+extern "C" int64_t pvraft_corr_matmul_workspace_bytes(int B, int N, int M, int C) {
     if (B <= 0 || N <= 0 || M <= 0 || C <= 0) return 0;
     return (int64_t)2 * B * ((int64_t)N + M) * C * (int64_t)sizeof(float);   // hi/lo copies of both feature maps
 }
 
-extern "C" int64_t pvraft_corr_matmul_workspace_bytes(int B, int N, int C) { return pvraft_corr_matmul_nm_workspace_bytes(B, N, N, C); }
-
-extern "C" int pvraft_corr_matmul_nm_fwd(const float* fmap1, const float* fmap2, int B, int N, int M, int C, float* corr, void* workspace,
-                                         void* stream) {
+extern "C" int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, int B, int N, int M, int C, float* corr, void* workspace,
+                                      void* stream) {
     if (!fmap1 || !fmap2 || !corr || !workspace) return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul: null pointer");
     if (B <= 0 || N <= 0 || M <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul: bad shape");
     if (N % kTileM || M % kTileN || C % kBlockK)
@@ -276,11 +274,6 @@ extern "C" int pvraft_corr_matmul_nm_fwd(const float* fmap1, const float* fmap2,
     return launch_gemm(a_hi, a_lo, b_hi, b_lo, B, N, M, C, 0, N / kTileM, 0, M / kTileN, corr, M, st);
 }
 
-extern "C" int pvraft_corr_matmul_fwd(const float* fmap1, const float* fmap2, int B, int N, int C, float* corr, void* workspace,
-                                      void* stream) {
-    return pvraft_corr_matmul_nm_fwd(fmap1, fmap2, B, N, N, C, corr, workspace, stream);
-}
-
 extern "C" int pvraft_tf32_split_fwd(const float* x, int64_t n, float* hi, float* lo, void* stream) {
     if (!x || !hi || !lo || n <= 0) return fail(PVRAFT_ERR_BAD_ARG, "tf32_split: bad argument");
     if (n % 4 || ((uintptr_t)x | (uintptr_t)hi | (uintptr_t)lo) % 16)
@@ -289,8 +282,8 @@ extern "C" int pvraft_tf32_split_fwd(const float* x, int64_t n, float* hi, float
     return check_launch("tf32_split");
 }
 
-extern "C" int pvraft_corr_matmul_window_nm_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
-                                                int M, int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream) {
+extern "C" int pvraft_corr_matmul_window_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
+                                             int M, int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream) {
     if (!a_hi || !a_lo || !b_hi || !b_lo || !corr) return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul_window: null pointer");
     if (B <= 0 || N <= 0 || M <= 0 || C <= 0 || rows <= 0 || cols <= 0 || r0 < 0 || c0 < 0)
         return fail(PVRAFT_ERR_BAD_ARG, "corr_matmul_window: bad shape");
@@ -306,9 +299,4 @@ extern "C" int pvraft_corr_matmul_window_nm_fwd(const float* a_hi, const float* 
     if ((long long)B * N > 0x7fffffffLL || (long long)B * M > 0x7fffffffLL)
         return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul_window: B*N=%lld / B*M=%lld operand rows", (long long)B * N, (long long)B * M);
     return launch_gemm(a_hi, a_lo, b_hi, b_lo, B, N, M, C, r0, tiles_m, c0, tiles_n, corr, ldc, (cudaStream_t)stream);
-}
-
-extern "C" int pvraft_corr_matmul_window_fwd(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N,
-                                             int C, int r0, int rows, int c0, int cols, float* corr, int64_t ldc, void* stream) {
-    return pvraft_corr_matmul_window_nm_fwd(a_hi, a_lo, b_hi, b_lo, B, N, N, C, r0, rows, c0, cols, corr, ldc, stream);
 }

@@ -731,7 +731,6 @@ template <bool DET>
 static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half, const float* xyz2_pad, const float* coords, int B, int N,
                            int M, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
                            int8_t* dbg_cube, void* ws, void* stream) {
-    if (DET && moments && !ws) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: the deterministic form needs its workspace");
     if (!corr_val || !corr_idx || !xyz2_pad || !coords || !vox || !knn_sel) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: null pointer");
     if (B <= 0 || N <= 0 || M <= 0) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup: B=%d N=%d M=%d", B, N, M);
     if (levels < 1 || levels > 4) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_lookup: levels=%d (1..4 supported)", levels);
@@ -794,70 +793,24 @@ static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half
     return fx_flush_f64(static_cast<const unsigned long long*>(ws), B, 15, PVRAFT_MOMENTS, PVRAFT_MOMENTS, moments, st);
 }
 
-extern "C" int pvraft_corr_lookup_nm_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad,
-                                         const float* coords, int B, int N, int M, int K, int levels, float base_scale,
-                                         float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
-                                         int8_t* dbg_cube, void* stream) {
-    return corr_lookup_any<false>(corr_val, corr_idx, false, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld, knn_sel,
-                                  knn_slot, moments, dbg_cube, nullptr, stream);
-}
-
-extern "C" int pvraft_corr_lookup_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad,
-                                      const float* coords, int B, int N, int K, int levels, float base_scale,
-                                      float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
-                                      int8_t* dbg_cube, void* stream) {
-    return pvraft_corr_lookup_nm_fwd(corr_val, corr_idx, xyz2_pad, coords, B, N, N, K, levels, base_scale, vox, vox_ld, knn_sel,
-                                     knn_slot, moments, dbg_cube, stream);
-}
-
-extern "C" int pvraft_corr_lookup_bf16_nm_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
-                                              const float* coords, int B, int N, int M, int K, int levels, float base_scale,
-                                              float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
-                                              int8_t* dbg_cube, void* stream) {
-    return corr_lookup_any<false>(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld,
-                                  knn_sel, knn_slot, moments, dbg_cube, nullptr, stream);
+extern "C" int pvraft_corr_lookup_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords, int B,
+                                      int N, int M, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
+                                      int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* det_workspace, void* stream) {
+    auto f = det_workspace ? corr_lookup_any<true> : corr_lookup_any<false>;
+    return f(corr_val, corr_idx, false, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld, knn_sel, knn_slot, moments, dbg_cube,
+             det_workspace, stream);
 }
 
 extern "C" int pvraft_corr_lookup_bf16_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
-                                           const float* coords, int B, int N, int K, int levels, float base_scale,
-                                           float* vox, int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments,
-                                           int8_t* dbg_cube, void* stream) {
-    return pvraft_corr_lookup_bf16_nm_fwd(corr_val_bf16, corr_idx_u16, xyz2_pad, coords, B, N, N, K, levels, base_scale, vox, vox_ld,
-                                          knn_sel, knn_slot, moments, dbg_cube, stream);
+                                           const float* coords, int B, int N, int M, int K, int levels, float base_scale, float* vox,
+                                           int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
+                                           void* det_workspace, void* stream) {
+    auto f = det_workspace ? corr_lookup_any<true> : corr_lookup_any<false>;
+    return f(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld, knn_sel, knn_slot, moments,
+             dbg_cube, det_workspace, stream);
 }
 
 extern "C" int64_t pvraft_corr_lookup_det_workspace_bytes(int B) { return (int64_t)B * PVRAFT_MOMENTS * kFxWords * 8; }
-
-extern "C" int pvraft_corr_lookup_nm_det_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords,
-                                             int B, int N, int M, int K, int levels, float base_scale, float* vox, int vox_ld,
-                                             float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace,
-                                             void* stream) {
-    return corr_lookup_any<true>(corr_val, corr_idx, false, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld, knn_sel,
-                                 knn_slot, moments, dbg_cube, workspace, stream);
-}
-
-extern "C" int pvraft_corr_lookup_det_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords, int B,
-                                          int N, int K, int levels, float base_scale, float* vox, int vox_ld, float* knn_sel,
-                                          int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace, void* stream) {
-    return pvraft_corr_lookup_nm_det_fwd(corr_val, corr_idx, xyz2_pad, coords, B, N, N, K, levels, base_scale, vox, vox_ld, knn_sel,
-                                         knn_slot, moments, dbg_cube, workspace, stream);
-}
-
-extern "C" int pvraft_corr_lookup_bf16_nm_det_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
-                                                  const float* coords, int B, int N, int M, int K, int levels, float base_scale, float* vox,
-                                                  int vox_ld, float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube,
-                                                  void* workspace, void* stream) {
-    return corr_lookup_any<true>(corr_val_bf16, corr_idx_u16, true, xyz2_pad, coords, B, N, M, K, levels, base_scale, vox, vox_ld,
-                                 knn_sel, knn_slot, moments, dbg_cube, workspace, stream);
-}
-
-extern "C" int pvraft_corr_lookup_bf16_det_fwd(const uint16_t* corr_val_bf16, const uint16_t* corr_idx_u16, const float* xyz2_pad,
-                                               const float* coords, int B, int N, int K, int levels, float base_scale, float* vox, int vox_ld,
-                                               float* knn_sel, int32_t* knn_slot, double* moments, int8_t* dbg_cube, void* workspace,
-                                               void* stream) {
-    return pvraft_corr_lookup_bf16_nm_det_fwd(corr_val_bf16, corr_idx_u16, xyz2_pad, coords, B, N, N, K, levels, base_scale, vox, vox_ld,
-                                              knn_sel, knn_slot, moments, dbg_cube, workspace, stream);
-}
 
 // fp32 correlation values -> bf16 (round to nearest even), int32 candidate ids -> uint16: the 4-byte-per-candidate state
 __global__ void k_state_pack_bf16(const float* __restrict__ val, const int32_t* __restrict__ idx, long long n, uint16_t* __restrict__ val_out,

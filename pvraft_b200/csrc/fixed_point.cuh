@@ -1,5 +1,5 @@
 // Exact fixed-point accumulation for the deterministic instantiations of the reducing kernels (the library's form of
-// torch.use_deterministic_algorithms(True); include/pvraft_b200.h, "Deterministic entry points").
+// torch.use_deterministic_algorithms(True); include/pvraft_b200.h, "Deterministic mode").
 //
 // A slot holds a signed Q64.64 number -- value = (hi * 2^64 + lo) * 2^-64 in 128-bit two's complement -- plus a flag word:
 // three 64-bit words.  A contribution enters as fx_from(v): |v| truncated toward zero to a multiple of 2^-64.  From then on

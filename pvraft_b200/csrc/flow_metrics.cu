@@ -62,28 +62,24 @@ __global__ void __launch_bounds__(256) k_flow_l1_bwd(const float* __restrict__ e
 
 using namespace pvraft;
 
-extern "C" int pvraft_flow_metrics_fwd(const float* est, const float* gt, const float* mask, int64_t points, double* acc, void* stream) {
+extern "C" int pvraft_flow_metrics_fwd(const float* est, const float* gt, const float* mask, int64_t points, double* acc, void* det_workspace,
+                                       void* stream) {
     if (!est || !gt || !acc || points <= 0) return fail(PVRAFT_ERR_BAD_ARG, "flow_metrics: bad argument");
     long long blocks = (points + 255) / 256;
-    const long long cap = (long long)sm_count() * 8;
+    const long long cap = det_workspace ? kDetCtas : (long long)sm_count() * 8;
     if (blocks > cap) blocks = cap;
-    k_flow_metrics<false><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(est, gt, mask, points, acc);
-    return check_launch("flow_metrics");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!det_workspace) {
+        k_flow_metrics<false><<<(unsigned)blocks, 256, 0, st>>>(est, gt, mask, points, acc);
+        return check_launch("flow_metrics");
+    }
+    k_flow_metrics<true><<<(unsigned)blocks, 256, 0, st>>>(est, gt, mask, points, static_cast<double*>(det_workspace));
+    const int rc = check_launch("flow_metrics");
+    if (rc) return rc;
+    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, 6, 6, 0, acc, st);
 }
 
 extern "C" int64_t pvraft_flow_metrics_det_workspace_bytes(void) { return 6 * kFxWords * 8; }
-
-extern "C" int pvraft_flow_metrics_det_fwd(const float* est, const float* gt, const float* mask, int64_t points, double* acc, void* workspace,
-                                           void* stream) {
-    if (!est || !gt || !acc || !workspace || points <= 0) return fail(PVRAFT_ERR_BAD_ARG, "flow_metrics_det: bad argument");
-    long long blocks = (points + 255) / 256;
-    if (blocks > kDetCtas) blocks = kDetCtas;
-    cudaStream_t st = (cudaStream_t)stream;
-    k_flow_metrics<true><<<(unsigned)blocks, 256, 0, st>>>(est, gt, mask, points, static_cast<double*>(workspace));
-    int rc = check_launch("flow_metrics_det");
-    if (rc) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(workspace), 1, 6, 6, 0, acc, st);
-}
 
 extern "C" int pvraft_flow_l1_bwd(const float* est, const float* gt, const float* mask, int64_t points, const double* acc, const float* g,
                                   float weight, float* d_est, void* stream) {

@@ -766,7 +766,7 @@ using namespace pvraft;
 
 template <bool DET>
 static int linear_fwd(const pvraft_linear_args* a, void* ws, void* stream) {
-    if (!a || !a->in || !a->weight || !a->out || (DET && a->out_stats && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "linear: null pointer");
+    if (!a || !a->in || !a->weight || !a->out) return fail(PVRAFT_ERR_BAD_ARG, "linear: null pointer");
     if (a->B <= 0 || a->N <= 0 || a->cin <= 0 || a->cout <= 0) return fail(PVRAFT_ERR_BAD_ARG, "linear: bad shape");
     if (a->cout > 128 || a->cin > 256) return fail(PVRAFT_ERR_UNSUPPORTED, "linear: cin=%d cout=%d (max 256/128)", a->cin, a->cout);
     if (a->in_mode != PVRAFT_IN_PLAIN) {
@@ -791,11 +791,11 @@ static int linear_fwd(const pvraft_linear_args* a, void* ws, void* stream) {
     return fx_flush_f64(static_cast<const unsigned long long*>(ws), 1, (long long)a->B * 16, (long long)a->B * 16, 0, a->out_stats, (cudaStream_t)stream);
 }
 
-extern "C" int pvraft_linear_fwd(const pvraft_linear_args* a, void* stream) { return linear_fwd<false>(a, nullptr, stream); }
+extern "C" int pvraft_linear_fwd(const pvraft_linear_args* a, void* det_workspace, void* stream) {
+    return det_workspace ? linear_fwd<true>(a, det_workspace, stream) : linear_fwd<false>(a, nullptr, stream);
+}
 
 extern "C" int64_t pvraft_linear_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
-
-extern "C" int pvraft_linear_det_fwd(const pvraft_linear_args* a, void* workspace, void* stream) { return linear_fwd<true>(a, workspace, stream); }
 
 extern "C" int pvraft_gn_act_fwd(const float* in, const double* stats, const float* gamma, const float* beta, double count,
                                  int act, float slope, int B, int N, int C, int transpose_out, float* out, const float* slope_dev,

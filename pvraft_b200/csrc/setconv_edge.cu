@@ -201,7 +201,7 @@ using namespace pvraft;
 template <bool DET>
 static int setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin, int B, int N, int C,
                             float* ymax, float* ymin, double* stats, const int32_t* order, void* ws, void* stream) {
-    if (!fc1p || !nbr || !edge_feats || !w_fc1 || !ymax || !ymin || !stats || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: null pointer");
+    if (!fc1p || !nbr || !edge_feats || !w_fc1 || !ymax || !ymin || !stats) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: null pointer");
     if (B <= 0 || N <= 0 || cin <= 0) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: bad shape");
     if (C <= 0 || C > 128 || C % PVRAFT_GN_GROUPS) return fail(PVRAFT_ERR_UNSUPPORTED, "setconv_edge: C=%d (multiple of 8, <= 128)", C);
     const long long total = (long long)B * N;
@@ -219,14 +219,10 @@ static int setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* 
 }
 
 extern "C" int pvraft_setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
-                                       int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order, void* stream) {
-    return setconv_edge_fwd<false>(fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order, nullptr, stream);
+                                       int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order,
+                                       void* det_workspace, void* stream) {
+    auto f = det_workspace ? setconv_edge_fwd<true> : setconv_edge_fwd<false>;
+    return f(fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order, det_workspace, stream);
 }
 
 extern "C" int64_t pvraft_setconv_edge_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
-
-extern "C" int pvraft_setconv_edge_det_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
-                                           int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order, void* workspace,
-                                           void* stream) {
-    return setconv_edge_fwd<true>(fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order, workspace, stream);
-}

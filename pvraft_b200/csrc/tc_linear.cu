@@ -947,7 +947,7 @@ extern "C" int pvraft_tc_weight_split(const float* w, int rows, int cols, int ld
 
 template <bool DET>
 static int tc_linear_fwd(const pvraft_tc_linear_args* a, void* ws, void* stream) {
-    if (!a || !a->in[0] || !a->w_hi || !a->w_lo || !a->out || (DET && a->out_stats && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: null pointer");
+    if (!a || !a->in[0] || !a->w_hi || !a->w_lo || !a->out) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: null pointer");
     if (a->B <= 0 || a->N <= 0 || a->n_pad < 16 || a->n_pad > 128 || a->n_pad % 16) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: bad shape (n_pad=%d)", a->n_pad);
     if (a->N % kTcM) return fail(PVRAFT_ERR_UNSUPPORTED, "tc_linear: points per sample (%d) must be a multiple of 128", a->N);
     int K = 0;
@@ -1031,13 +1031,11 @@ static int tc_linear_fwd(const pvraft_tc_linear_args* a, void* ws, void* stream)
     return fx_flush_f64(static_cast<const unsigned long long*>(ws), 1, (long long)a->B * 16, (long long)a->B * 16, 0, a->out_stats, (cudaStream_t)stream);
 }
 
-extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* stream) { return tc_linear_fwd<false>(a, nullptr, stream); }
+extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* det_workspace, void* stream) {
+    return det_workspace ? tc_linear_fwd<true>(a, det_workspace, stream) : tc_linear_fwd<false>(a, nullptr, stream);
+}
 
 extern "C" int64_t pvraft_tc_linear_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
-
-extern "C" int pvraft_tc_linear_det_fwd(const pvraft_tc_linear_args* a, void* workspace, void* stream) {
-    return tc_linear_fwd<true>(a, workspace, stream);
-}
 
 extern "C" int pvraft_update_chain_fwd(const pvraft_update_chain_args* a, void* stream) {
     if (!a || !a->y1 || !a->y1_stats || !a->gn_gamma || !a->gn_beta || !a->kfeat || !a->cflow || !a->flow || !a->net || !a->inp ||

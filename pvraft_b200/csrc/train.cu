@@ -7,9 +7,9 @@
 // arithmetic step of forward and backward is one of the kernels of this library.  Layout conventions as in the forward
 // kernels: per-point features point-major [B,rows,C]; "rows" is N for per-point layers and N*32 for per-edge layers.
 // Reductions into parameter gradients use fp32 / fp64 atomics (order-nondeterministic, like ATen's own CUDA backward) in
-// the default instantiations.  The DET instantiations (the *_det entry points) add exact fixed-point values instead
-// (fixed_point.cuh) and size their grids from the shapes alone, so their results are bitwise reproducible; their
-// accumulator arguments then point at the caller's fixed-point workspace.
+// the default instantiations.  The DET instantiations (what an entry point runs when given a det_workspace) add exact
+// fixed-point values instead (fixed_point.cuh) and size their grids from the shapes alone, so their results are bitwise
+// reproducible; their accumulator arguments then point at the caller's fixed-point workspace.
 #include "fixed_point.cuh"
 
 namespace pvraft {
@@ -770,7 +770,7 @@ using namespace pvraft;
 template <bool DET>
 static int linear_wgrad(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db, void* ws,
                         void* stream) {
-    if (!x || !dy || !dW || rows <= 0 || cin <= 0 || cout <= 0 || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "linear_wgrad: bad argument");
+    if (!x || !dy || !dW || rows <= 0 || cin <= 0 || cout <= 0) return fail(PVRAFT_ERR_BAD_ARG, "linear_wgrad: bad argument");
     if (cin > 256 || cout > 128) return fail(PVRAFT_ERR_UNSUPPORTED, "linear_wgrad: cin=%d cout=%d (max 256/128)", cin, cout);
     const int cin_p = (cin + 3) & ~3;
     if (8 * (cin_p >> 2) > 2 * kWgThreads) return fail(PVRAFT_ERR_UNSUPPORTED, "linear_wgrad: cin=%d", cin);
@@ -797,23 +797,19 @@ static int linear_wgrad(const float* x, const float* dy, int64_t rows, int cin, 
 }
 
 extern "C" int pvraft_linear_wgrad(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
-                                   void* stream) {
-    return linear_wgrad<false>(x, dy, rows, cin, cout, dW, dw_ld, db, nullptr, stream);
+                                   void* det_workspace, void* stream) {
+    auto f = det_workspace ? linear_wgrad<true> : linear_wgrad<false>;
+    return f(x, dy, rows, cin, cout, dW, dw_ld, db, det_workspace, stream);
 }
 
 extern "C" int64_t pvraft_linear_wgrad_det_workspace_bytes(int cin, int cout) {
     return (int64_t)((int64_t)cout * cin + cout) * kFxWords * 8;
 }
 
-extern "C" int pvraft_linear_wgrad_det(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
-                                       void* workspace, void* stream) {
-    return linear_wgrad<true>(x, dy, rows, cin, cout, dW, dw_ld, db, workspace, stream);
-}
-
 template <bool DET>
 static int linear_bwd_small(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld, float* dW, int dw_ld,
                             float* db, float* dx, void* ws, void* stream) {
-    if (!x || !dy || !W || !dW || rows <= 0 || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "linear_bwd_small: bad argument");
+    if (!x || !dy || !W || !dW || rows <= 0) return fail(PVRAFT_ERR_BAD_ARG, "linear_bwd_small: bad argument");
     const int lpr = cout / 16;
     if (cin < 1 || cin > 4 || cout % 16 || !(lpr == 1 || lpr == 2 || lpr == 3 || lpr == 4 || lpr == 6 || lpr == 8))
         return fail(PVRAFT_ERR_UNSUPPORTED, "linear_bwd_small: cin=%d cout=%d (cin <= 4, cout in {16,32,48,64,96,128})", cin, cout);
@@ -846,24 +842,20 @@ static int linear_bwd_small(const float* x, const float* dy, const float* W, int
 }
 
 extern "C" int pvraft_linear_bwd_small(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld, float* dW,
-                                       int dw_ld, float* db, float* dx, void* stream) {
-    return linear_bwd_small<false>(x, dy, W, rows, cin, cout, w_ld, dW, dw_ld, db, dx, nullptr, stream);
+                                       int dw_ld, float* db, float* dx, void* det_workspace, void* stream) {
+    auto f = det_workspace ? linear_bwd_small<true> : linear_bwd_small<false>;
+    return f(x, dy, W, rows, cin, cout, w_ld, dW, dw_ld, db, dx, det_workspace, stream);
 }
 
 extern "C" int64_t pvraft_linear_bwd_small_det_workspace_bytes(int cin, int cout) {
     return (int64_t)((int64_t)cout * cin + cout) * kFxWords * 8;
 }
 
-extern "C" int pvraft_linear_bwd_small_det(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld,
-                                           float* dW, int dw_ld, float* db, float* dx, void* workspace, void* stream) {
-    return linear_bwd_small<true>(x, dy, W, rows, cin, cout, w_ld, dW, dw_ld, db, dx, workspace, stream);
-}
-
 template <bool DET>
 static int gn_act_bwd(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta, double count, int act,
                       float slope, int B, int64_t rows, int C, double* gsum, double* dgamma, double* dbeta, double* dslope, float* dx,
                       const float* slope_dev, const uint8_t* arg, void* ws, void* stream) {
-    if (!x || !dy || !stats || !gamma || !beta || !gsum || !dgamma || !dbeta || !dx || (DET && !ws)) return fail(PVRAFT_ERR_BAD_ARG, "gn_act_bwd: null pointer");
+    if (!x || !dy || !stats || !gamma || !beta || !gsum || !dgamma || !dbeta || !dx) return fail(PVRAFT_ERR_BAD_ARG, "gn_act_bwd: null pointer");
     if (C > 256 || C % PVRAFT_GN_GROUPS || B <= 0 || rows <= 0) return fail(PVRAFT_ERR_UNSUPPORTED, "gn_act_bwd: C=%d", C);
     if (arg && rows % PVRAFT_KNN) return fail(PVRAFT_ERR_BAD_ARG, "gn_act_bwd: the max-pooled form needs rows %% 32 == 0");
     GnBwdParams p{x, dy, stats, gamma, beta, count, act, slope, (long long)rows, B, C, gsum, dgamma, dbeta, dslope, dx, slope_dev, arg};
@@ -907,21 +899,13 @@ static int gn_act_bwd(const float* x, const float* dy, const double* stats, cons
 
 extern "C" int pvraft_gn_act_bwd(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta, double count,
                                  int act, float slope, int B, int64_t rows, int C, double* gsum, double* dgamma, double* dbeta,
-                                 double* dslope, float* dx, const float* slope_dev, const uint8_t* arg, void* stream) {
-    return gn_act_bwd<false>(x, dy, stats, gamma, beta, count, act, slope, B, rows, C, gsum, dgamma, dbeta, dslope, dx, slope_dev, arg,
-                             nullptr, stream);
+                                 double* dslope, float* dx, const float* slope_dev, const uint8_t* arg, void* det_workspace, void* stream) {
+    auto f = det_workspace ? gn_act_bwd<true> : gn_act_bwd<false>;
+    return f(x, dy, stats, gamma, beta, count, act, slope, B, rows, C, gsum, dgamma, dbeta, dslope, dx, slope_dev, arg, det_workspace, stream);
 }
 
 extern "C" int64_t pvraft_gn_act_bwd_det_workspace_bytes(int B, int C) {
     return (int64_t)((int64_t)B * 16 + 2 * (int64_t)C + 1) * kFxWords * 8;
-}
-
-extern "C" int pvraft_gn_act_bwd_det(const float* x, const float* dy, const double* stats, const float* gamma, const float* beta,
-                                     double count, int act, float slope, int B, int64_t rows, int C, double* gsum, double* dgamma,
-                                     double* dbeta, double* dslope, float* dx, const float* slope_dev, const uint8_t* arg, void* workspace,
-                                     void* stream) {
-    return gn_act_bwd<true>(x, dy, stats, gamma, beta, count, act, slope, B, rows, C, gsum, dgamma, dbeta, dslope, dx, slope_dev, arg,
-                            workspace, stream);
 }
 
 extern "C" int pvraft_gn_act_maxk_fwd(const float* x, const double* stats, const float* gamma, const float* beta, double count, int act,
@@ -935,46 +919,40 @@ extern "C" int pvraft_gn_act_maxk_fwd(const float* x, const double* stats, const
     return check_launch("gn_act_maxk");
 }
 
-extern "C" int pvraft_edge_fwd(const float* P, const int32_t* nbr, float* E, int B, int N, int C, double* stats, void* stream) {
+extern "C" int pvraft_edge_fwd(const float* P, const int32_t* nbr, float* E, int B, int N, int C, double* stats, void* det_workspace,
+                               void* stream) {
     if (!P || !nbr || !E || B <= 0 || N <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "edge_fwd: bad argument");
     if (stats && C % PVRAFT_GN_GROUPS) return fail(PVRAFT_ERR_BAD_ARG, "edge_fwd: statistics need C %% 8 == 0");
-    const long long pts = (long long)B * N;
-    k_edge_fwd<false><<<(unsigned)((pts + 7) / 8), 256, 0, (cudaStream_t)stream>>>(P, nbr, E, B, N, C, stats);
-    return check_launch("edge_fwd");
-}
-
-extern "C" int64_t pvraft_edge_det_fwd_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
-
-extern "C" int pvraft_edge_det_fwd(const float* P, const int32_t* nbr, float* E, int B, int N, int C, double* stats, void* workspace,
-                                   void* stream) {
-    if (!P || !nbr || !E || B <= 0 || N <= 0 || C <= 0 || (stats && !workspace)) return fail(PVRAFT_ERR_BAD_ARG, "edge_det_fwd: bad argument");
-    if (stats && C % PVRAFT_GN_GROUPS) return fail(PVRAFT_ERR_BAD_ARG, "edge_det_fwd: statistics need C %% 8 == 0");
-    const long long pts = (long long)B * N;
+    const unsigned blocks = (unsigned)(((long long)B * N + 7) / 8);
     cudaStream_t st = (cudaStream_t)stream;
-    k_edge_fwd<true><<<(unsigned)((pts + 7) / 8), 256, 0, st>>>(P, nbr, E, B, N, C, stats ? static_cast<double*>(workspace) : nullptr);
-    int rc = check_launch("edge_det_fwd");
+    if (!det_workspace) {
+        k_edge_fwd<false><<<blocks, 256, 0, st>>>(P, nbr, E, B, N, C, stats);
+        return check_launch("edge_fwd");
+    }
+    k_edge_fwd<true><<<blocks, 256, 0, st>>>(P, nbr, E, B, N, C, stats ? static_cast<double*>(det_workspace) : nullptr);
+    const int rc = check_launch("edge_fwd");
     if (rc || !stats) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(workspace), 1, (long long)B * 16, (long long)B * 16, 0, stats, st);
+    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, (long long)B * 16, (long long)B * 16, 0, stats, st);
 }
 
-extern "C" int pvraft_edge_bwd(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* stream) {
+extern "C" int64_t pvraft_edge_fwd_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
+
+extern "C" int pvraft_edge_bwd(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* det_workspace, void* stream) {
     if (!dT || !nbr || !dP || B <= 0 || N <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "edge_bwd: bad argument");
     const long long pts = (long long)B * N;
-    k_edge_bwd<false><<<(unsigned)((pts + 7) / 8), 256, 0, (cudaStream_t)stream>>>(dT, nbr, B, N, C, dP);
-    return check_launch("edge_bwd");
+    const unsigned blocks = (unsigned)((pts + 7) / 8);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!det_workspace) {
+        k_edge_bwd<false><<<blocks, 256, 0, st>>>(dT, nbr, B, N, C, dP);
+        return check_launch("edge_bwd");
+    }
+    k_edge_bwd<true><<<blocks, 256, 0, st>>>(dT, nbr, B, N, C, static_cast<float*>(det_workspace));
+    const int rc = check_launch("edge_bwd");
+    if (rc) return rc;
+    return fx_flush_f32(static_cast<const unsigned long long*>(det_workspace), 1, pts * C, pts * C, 0, dP, st);
 }
 
 extern "C" int64_t pvraft_edge_bwd_det_workspace_bytes(int B, int N, int C) { return (int64_t)B * N * C * kFxWords * 8; }
-
-extern "C" int pvraft_edge_bwd_det(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* workspace, void* stream) {
-    if (!dT || !nbr || !dP || !workspace || B <= 0 || N <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "edge_bwd_det: bad argument");
-    const long long pts = (long long)B * N;
-    cudaStream_t st = (cudaStream_t)stream;
-    k_edge_bwd<true><<<(unsigned)((pts + 7) / 8), 256, 0, st>>>(dT, nbr, B, N, C, static_cast<float*>(workspace));
-    int rc = check_launch("edge_bwd_det");
-    if (rc) return rc;
-    return fx_flush_f32(static_cast<const unsigned long long*>(workspace), 1, pts * C, pts * C, 0, dP, st);
-}
 
 extern "C" int pvraft_maxk_fwd(const float* x, int64_t pts, int C, float* y, uint8_t* arg, void* stream) {
     if (!x || !y || !arg || pts <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "maxk_fwd: bad argument");
@@ -991,9 +969,9 @@ extern "C" int pvraft_maxk_bwd(const float* dy, const uint8_t* arg, int64_t pts,
     return check_launch("maxk_bwd");
 }
 
-extern "C" int pvraft_corr_lookup_nm_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
-                                         const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int M, int K, int levels,
-                                         float base_scale, float* d_corr, void* stream) {
+extern "C" int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
+                                      const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int M, int K, int levels,
+                                      float base_scale, float* d_corr, void* stream) {
     if (!corr_idx || !xyz2_pad || !coords || !knn_slot || !g_vox || !g_sel || !d_corr) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup_bwd: null pointer");
     if (B <= 0 || N <= 0 || M <= 0 || K < 32 || levels < 1 || levels > 4 || vox_ld < levels * 27)
         return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup_bwd: bad shape");
@@ -1014,17 +992,10 @@ extern "C" int pvraft_corr_lookup_nm_bwd(const int32_t* corr_idx, const float* x
     return check_launch("corr_lookup_bwd");
 }
 
-extern "C" int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
-                                      const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int K, int levels, float base_scale,
-                                      float* d_corr, void* stream) {
-    return pvraft_corr_lookup_nm_bwd(corr_idx, xyz2_pad, coords, knn_slot, g_vox, vox_ld, g_sel, B, N, N, K, levels, base_scale, d_corr,
-                                     stream);
-}
-
 template <bool DET>
 static int corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M, int C, int K,
                          float* d_fmap1, float* d_fmap2, void* ws, void* stream) {
-    if (!g || !idx || !fmap1 || !fmap2 || !d_fmap1 || !d_fmap2 || B <= 0 || N <= 0 || M <= 0 || K <= 0 || (DET && !ws))
+    if (!g || !idx || !fmap1 || !fmap2 || !d_fmap1 || !d_fmap2 || B <= 0 || N <= 0 || M <= 0 || K <= 0)
         return fail(PVRAFT_ERR_BAD_ARG, "corr_init_bwd: bad argument");
     float* kd2 = DET ? static_cast<float*>(ws) : d_fmap2;
     const long long rows = (long long)B * N;
@@ -1044,26 +1015,10 @@ static int corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1,
     return fx_flush_f32(static_cast<const unsigned long long*>(ws), 1, rows2 * C, rows2 * C, 0, d_fmap2, st);
 }
 
-extern "C" int pvraft_corr_init_nm_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M, int C,
-                                       int K, float* d_fmap1, float* d_fmap2, void* stream) {
-    return corr_init_bwd<false>(g, idx, fmap1, fmap2, B, N, M, C, K, d_fmap1, d_fmap2, nullptr, stream);
+extern "C" int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M, int C,
+                                    int K, float* d_fmap1, float* d_fmap2, void* det_workspace, void* stream) {
+    auto f = det_workspace ? corr_init_bwd<true> : corr_init_bwd<false>;
+    return f(g, idx, fmap1, fmap2, B, N, M, C, K, d_fmap1, d_fmap2, det_workspace, stream);
 }
 
-extern "C" int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C, int K,
-                                    float* d_fmap1, float* d_fmap2, void* stream) {
-    return pvraft_corr_init_nm_bwd(g, idx, fmap1, fmap2, B, N, N, C, K, d_fmap1, d_fmap2, stream);
-}
-
-extern "C" int64_t pvraft_corr_init_nm_bwd_det_workspace_bytes(int B, int M, int C) { return (int64_t)B * M * C * kFxWords * 8; }
-
-extern "C" int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int N, int C) { return pvraft_corr_init_nm_bwd_det_workspace_bytes(B, N, C); }
-
-extern "C" int pvraft_corr_init_nm_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M,
-                                           int C, int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream) {
-    return corr_init_bwd<true>(g, idx, fmap1, fmap2, B, N, M, C, K, d_fmap1, d_fmap2, workspace, stream);
-}
-
-extern "C" int pvraft_corr_init_bwd_det(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int C,
-                                        int K, float* d_fmap1, float* d_fmap2, void* workspace, void* stream) {
-    return pvraft_corr_init_nm_bwd_det(g, idx, fmap1, fmap2, B, N, N, C, K, d_fmap1, d_fmap2, workspace, stream);
-}
+extern "C" int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int M, int C) { return (int64_t)B * M * C * kFxWords * 8; }

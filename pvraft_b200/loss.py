@@ -15,12 +15,9 @@ def _gt(batch):
 
 def _metrics(est, gt, mask):
     acc = torch.zeros(8, dtype=torch.float64, device=est.device)
-    args = (ops._p(est), ops._p(gt), ops._p(mask), est.numel() // 3, acc.data_ptr())
-    if ops.deterministic():
-        ws = ops._det_workspace(lib().pvraft_flow_metrics_det_workspace_bytes(), est.device)
-        ops._count(lib().pvraft_flow_metrics_det_fwd(*args, ops._p(ws, torch.uint8), ops._stream()), 'flow_metrics_det')
-    else:
-        ops._count(lib().pvraft_flow_metrics_fwd(*args, ops._stream()), 'flow_metrics')
+    ws = ops._det_workspace(lib().pvraft_flow_metrics_det_workspace_bytes, device=est.device)
+    ops._count(lib().pvraft_flow_metrics_fwd(ops._p(est), ops._p(gt), ops._p(mask), est.numel() // 3, acc.data_ptr(), ops._p(ws, torch.uint8),
+                                             ops._stream()), 'flow_metrics')
     return acc
 
 

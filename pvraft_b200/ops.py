@@ -49,14 +49,17 @@ def _count(rc, what):
 
 def deterministic():
     """True while torch.use_deterministic_algorithms(True) is in effect.  The wrappers that reduce floating-point values
-    then call the library's deterministic entry points (include/pvraft_b200.h, "Deterministic entry points"), whose
-    results are bitwise reproducible; read at every call, so the flag can change between calls."""
+    then hand the library a det_workspace (include/pvraft_b200.h, "Deterministic mode"), which makes their results bitwise
+    reproducible; read at every call, so the flag can change between calls."""
     return torch.are_deterministic_algorithms_enabled()
 
 
-def _det_workspace(nbytes, device):
-    """The zero-filled fixed-point workspace of one deterministic call."""
-    return torch.zeros(int(nbytes), dtype=torch.uint8, device=device)
+def _det_workspace(size_fn, *size_args, device):
+    """The det_workspace argument of a reducing entry point: while deterministic() is on, a zero-filled buffer of
+    size_fn(*size_args) bytes (size_fn: the entry point's pvraft_*_det_workspace_bytes query); None otherwise."""
+    if not deterministic():
+        return None
+    return torch.zeros(int(size_fn(*size_args)), dtype=torch.uint8, device=device)
 
 
 _TLS = threading.local()   # .arena = [buffer [n,B,8,2] f64, next free block]: zeroed accumulators handed out inside a
@@ -121,8 +124,8 @@ def corr_matmul(fmap1_pm, fmap2_pm):
     if fmap2_pm.shape != (b, m, c):
         raise ValueError(f'corr_matmul: feature maps {tuple(fmap1_pm.shape)} and {tuple(fmap2_pm.shape)}')
     corr = torch.empty(b, n, m, dtype=torch.float32, device=fmap1_pm.device)
-    ws = torch.empty(int(lib().pvraft_corr_matmul_nm_workspace_bytes(b, n, m, c)), dtype=torch.uint8, device=fmap1_pm.device)
-    _count(lib().pvraft_corr_matmul_nm_fwd(_p(fmap1_pm), _p(fmap2_pm), b, n, m, c, _p(corr), _p(ws, torch.uint8), _stream()),
+    ws = torch.empty(int(lib().pvraft_corr_matmul_workspace_bytes(b, n, m, c)), dtype=torch.uint8, device=fmap1_pm.device)
+    _count(lib().pvraft_corr_matmul_fwd(_p(fmap1_pm), _p(fmap2_pm), b, n, m, c, _p(corr), _p(ws, torch.uint8), _stream()),
            'corr_matmul')
     return corr
 
@@ -236,7 +239,7 @@ def corr_build(fmap1_pm, fmap2_pm, k, plan=None):
         split = [_p(ws_a[0, s]), _p(ws_a[1, s]), _p(ws_b[0, s]), _p(ws_b[1, s])]
         for r0, nr in plan.row_blocks:
             for j, (c0, nc) in enumerate(plan.windows):
-                _count(lib().pvraft_corr_matmul_window_nm_fwd(*split, 1, npad, mpad, c, r0, nr, c0, nc, _p(slab), plan.ld, _stream()),
+                _count(lib().pvraft_corr_matmul_window_fwd(*split, 1, npad, mpad, c, r0, nr, c0, nc, _p(slab), plan.ld, _stream()),
                        'corr_matmul_window')
                 _count(lib().pvraft_corr_topk_window_fwd(_p(slab), nr, nc, plan.ld, k, c0, None, _p(cand_val) + 4 * j * k,
                                                          _p(cand_idx, torch.int32) + 4 * j * k, wk, _stream()), 'corr_topk_window')
@@ -294,17 +297,11 @@ def corr_lookup(corr_val, corr_idx, xyz2_pad, coords, levels, base_scale, vox=No
     slots = torch.empty(b, n, KNN, dtype=torch.int32, device=dev) if want_slots else None
     cube = torch.empty(b, n, k, levels, dtype=torch.int8, device=dev) if want_cube else None
     half = corr_val.dtype == torch.bfloat16   # reduced-precision state: bf16 values + uint16 ids (stored as int16)
-    args = ((_p(corr_val, torch.bfloat16), _p(corr_idx, torch.int16)) if half else (_p(corr_val), _p(corr_idx, torch.int32))) + \
-        (_p(xyz2_pad), _p(coords), b, n, m, k, levels, float(base_scale), _p(vox), vox.shape[-1], _p(knn_sel), _p(slots, torch.int32),
-         _p(moments, torch.float64), _p(cube, torch.int8))
-    if deterministic():
-        ws = _det_workspace(lib().pvraft_corr_lookup_det_workspace_bytes(b), dev)
-        fn = lib().pvraft_corr_lookup_bf16_nm_det_fwd if half else lib().pvraft_corr_lookup_nm_det_fwd
-        _count(fn(*args, _p(ws, torch.uint8), _stream()), 'corr_lookup_det')
-    elif half:
-        _count(lib().pvraft_corr_lookup_bf16_nm_fwd(*args, _stream()), 'corr_lookup_bf16')
-    else:
-        _count(lib().pvraft_corr_lookup_nm_fwd(*args, _stream()), 'corr_lookup')
+    state = (_p(corr_val, torch.bfloat16), _p(corr_idx, torch.int16)) if half else (_p(corr_val), _p(corr_idx, torch.int32))
+    fn = lib().pvraft_corr_lookup_bf16_fwd if half else lib().pvraft_corr_lookup_fwd
+    ws = _det_workspace(lib().pvraft_corr_lookup_det_workspace_bytes, b, device=dev)
+    _count(fn(*state, _p(xyz2_pad), _p(coords), b, n, m, k, levels, float(base_scale), _p(vox), vox.shape[-1], _p(knn_sel),
+              _p(slots, torch.int32), _p(moments, torch.float64), _p(cube, torch.int8), _p(ws, torch.uint8), _stream()), 'corr_lookup')
     return dict(vox=vox, knn_sel=knn_sel, moments=moments, knn_slot=slots, cube=cube)
 
 
@@ -320,11 +317,8 @@ def linear(x, weight, bias=None, *, cin=None, w_ld=0, w_cin=0, in_mode=IN_PLAIN,
     a = _lib.LinearArgs(_p(x), _p(in_min), _p(in_stats, torch.float64), _p(in_gamma), _p(in_beta), float(in_count),
                         in_mode, in_act, float(in_slope), _p(weight), int(w_ld), int(w_cin), _p(bias), _p(residual), out_act,
                         _p(out), _p(out_stats, torch.float64), b, n, cin, cout)
-    if out_stats is not None and deterministic():
-        ws = _det_workspace(lib().pvraft_linear_det_workspace_bytes(b), x.device)
-        _count(lib().pvraft_linear_det_fwd(C.byref(a), _p(ws, torch.uint8), _stream()), 'linear_det')
-    else:
-        _count(lib().pvraft_linear_fwd(C.byref(a), _stream()), 'linear')
+    ws = _det_workspace(lib().pvraft_linear_det_workspace_bytes, b, device=x.device) if out_stats is not None else None
+    _count(lib().pvraft_linear_fwd(C.byref(a), _p(ws, torch.uint8), _stream()), 'linear')
     return out
 
 
@@ -460,11 +454,8 @@ def tc_linear(sources, w, bias=None, *, in_min=None, in_stats=None, in_gamma=Non
     a.params_settled = 1 if pending == 0 else 0
     if pending:
         _TLS.unsettled = pending - 1
-    if out_stats is not None and deterministic():
-        ws = _det_workspace(lib().pvraft_tc_linear_det_workspace_bytes(b), out.device)
-        _count(lib().pvraft_tc_linear_det_fwd(C.byref(a), _p(ws, torch.uint8), _stream()), 'tc_linear_det')
-    else:
-        _count(lib().pvraft_tc_linear_fwd(C.byref(a), _stream()), 'tc_linear')
+    ws = _det_workspace(lib().pvraft_tc_linear_det_workspace_bytes, b, device=out.device) if out_stats is not None else None
+    _count(lib().pvraft_tc_linear_fwd(C.byref(a), _p(ws, torch.uint8), _stream()), 'tc_linear')
     return out
 
 
@@ -530,13 +521,9 @@ def setconv_edge(fc1p, nbr, edge_feats, w_fc1, cin, stats, ymax=None, ymin=None,
         ymax = torch.empty_like(fc1p)
     if ymin is None:
         ymin = torch.empty_like(fc1p)
-    args = (_p(fc1p), _p(nbr, torch.int32), _p(edge_feats), _p(w_fc1), cin, b, n, c, _p(ymax), _p(ymin), _p(stats, torch.float64),
-            _p(order, torch.int32))
-    if deterministic():
-        ws = _det_workspace(lib().pvraft_setconv_edge_det_workspace_bytes(b), fc1p.device)
-        _count(lib().pvraft_setconv_edge_det_fwd(*args, _p(ws, torch.uint8), _stream()), 'setconv_edge_det')
-    else:
-        _count(lib().pvraft_setconv_edge_fwd(*args, _stream()), 'setconv_edge')
+    ws = _det_workspace(lib().pvraft_setconv_edge_det_workspace_bytes, b, device=fc1p.device)
+    _count(lib().pvraft_setconv_edge_fwd(_p(fc1p), _p(nbr, torch.int32), _p(edge_feats), _p(w_fc1), cin, b, n, c, _p(ymax), _p(ymin),
+                                         _p(stats, torch.float64), _p(order, torch.int32), _p(ws, torch.uint8), _stream()), 'setconv_edge')
     return ymax, ymin
 
 
@@ -558,24 +545,18 @@ def knn(xyz, query, k, mode=0, want_rel=False, use_sweep=True):
 def linear_wgrad(x, dy, dw, db=None):
     """dw [cout,cin] += dy^T x, db [cout] += column sums of dy (both zeroed by the caller); x [B,R,cin], dy [B,R,cout]."""
     rows = x.shape[0] * x.shape[1]
-    args = (_p(x), _p(dy), rows, x.shape[-1], dy.shape[-1], _p(dw), dw.shape[-1], _p(db))
-    if deterministic():
-        ws = _det_workspace(lib().pvraft_linear_wgrad_det_workspace_bytes(x.shape[-1], dy.shape[-1]), x.device)
-        _count(lib().pvraft_linear_wgrad_det(*args, _p(ws, torch.uint8), _stream()), 'linear_wgrad_det')
-    else:
-        _count(lib().pvraft_linear_wgrad(*args, _stream()), 'linear_wgrad')
+    ws = _det_workspace(lib().pvraft_linear_wgrad_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
+    _count(lib().pvraft_linear_wgrad(_p(x), _p(dy), rows, x.shape[-1], dy.shape[-1], _p(dw), dw.shape[-1], _p(db), _p(ws, torch.uint8),
+                                     _stream()), 'linear_wgrad')
 
 
 def linear_bwd_small(x, dy, w, dw, db=None, want_dx=False):
     """cin <= 4, cout in {16,32,48,64,96,128}: dw += dy^T x, db += column sums, and dx = dy w (returned, or None) in one pass over dy."""
     rows = x.shape[0] * x.shape[1]
     dx = torch.empty_like(x) if want_dx else None
-    args = (_p(x), _p(dy), _p(w), rows, x.shape[-1], dy.shape[-1], w.shape[-1], _p(dw), dw.shape[-1], _p(db), _p(dx))
-    if deterministic():
-        ws = _det_workspace(lib().pvraft_linear_bwd_small_det_workspace_bytes(x.shape[-1], dy.shape[-1]), x.device)
-        _count(lib().pvraft_linear_bwd_small_det(*args, _p(ws, torch.uint8), _stream()), 'linear_bwd_small_det')
-    else:
-        _count(lib().pvraft_linear_bwd_small(*args, _stream()), 'linear_bwd_small')
+    ws = _det_workspace(lib().pvraft_linear_bwd_small_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
+    _count(lib().pvraft_linear_bwd_small(_p(x), _p(dy), _p(w), rows, x.shape[-1], dy.shape[-1], w.shape[-1], _p(dw), dw.shape[-1], _p(db),
+                                         _p(dx), _p(ws, torch.uint8), _stream()), 'linear_bwd_small')
     return dx
 
 
@@ -596,35 +577,26 @@ def gn_act_bwd(x, dy, stats, gamma, beta, count, act, slope, want_dslope=False, 
     scratch = torch.zeros(b * 16 + 2 * c + 1, dtype=torch.float64, device=dev)   # gsum | dgamma | dbeta | dslope
     gsum, dgamma, dbeta, dslope = scratch[:b * 16], scratch[b * 16:b * 16 + c], scratch[b * 16 + c:b * 16 + 2 * c], scratch[-1:]
     dx = torch.empty_like(x)
-    args = (_p(x), _p(dy), _p(stats, torch.float64), _p(gamma), _p(beta), float(count), act, float(slope), b, rows, c, gsum.data_ptr(),
-            dgamma.data_ptr(), dbeta.data_ptr(), dslope.data_ptr() if want_dslope else None, _p(dx), _p(slope_dev), _p(arg, torch.uint8))
-    if deterministic():
-        ws = _det_workspace(lib().pvraft_gn_act_bwd_det_workspace_bytes(b, c), dev)
-        _count(lib().pvraft_gn_act_bwd_det(*args, _p(ws, torch.uint8), _stream()), 'gn_act_bwd_det')
-    else:
-        _count(lib().pvraft_gn_act_bwd(*args, _stream()), 'gn_act_bwd')
+    ws = _det_workspace(lib().pvraft_gn_act_bwd_det_workspace_bytes, b, c, device=dev)
+    _count(lib().pvraft_gn_act_bwd(_p(x), _p(dy), _p(stats, torch.float64), _p(gamma), _p(beta), float(count), act, float(slope), b, rows, c,
+                                   gsum.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), dslope.data_ptr() if want_dslope else None, _p(dx),
+                                   _p(slope_dev), _p(arg, torch.uint8), _p(ws, torch.uint8), _stream()), 'gn_act_bwd')
     return dx, dgamma.float(), dbeta.float(), (dslope.float() if want_dslope else None)
 
 
 def edge_fwd(p, nbr, e, stats=None):
     """e [B,N*32,C] <- p[nbr] - p[centre] + e in place; stats [B,8,2] f64 accumulated."""
     b, n, c = p.shape
-    args = (_p(p), _p(nbr, torch.int32), _p(e), b, n, c, _p(stats, torch.float64))
-    if stats is not None and deterministic():
-        ws = _det_workspace(lib().pvraft_edge_det_fwd_workspace_bytes(b), p.device)
-        _count(lib().pvraft_edge_det_fwd(*args, _p(ws, torch.uint8), _stream()), 'edge_det_fwd')
-    else:
-        _count(lib().pvraft_edge_fwd(*args, _stream()), 'edge_fwd')
+    ws = _det_workspace(lib().pvraft_edge_fwd_det_workspace_bytes, b, device=p.device) if stats is not None else None
+    _count(lib().pvraft_edge_fwd(_p(p), _p(nbr, torch.int32), _p(e), b, n, c, _p(stats, torch.float64), _p(ws, torch.uint8), _stream()),
+           'edge_fwd')
     return e
 
 
 def edge_bwd(dt, nbr, dp):
     b, n, c = dp.shape
-    if deterministic():
-        ws = _det_workspace(lib().pvraft_edge_bwd_det_workspace_bytes(b, n, c), dp.device)
-        _count(lib().pvraft_edge_bwd_det(_p(dt), _p(nbr, torch.int32), b, n, c, _p(dp), _p(ws, torch.uint8), _stream()), 'edge_bwd_det')
-    else:
-        _count(lib().pvraft_edge_bwd(_p(dt), _p(nbr, torch.int32), b, n, c, _p(dp), _stream()), 'edge_bwd')
+    ws = _det_workspace(lib().pvraft_edge_bwd_det_workspace_bytes, b, n, c, device=dp.device)
+    _count(lib().pvraft_edge_bwd(_p(dt), _p(nbr, torch.int32), b, n, c, _p(dp), _p(ws, torch.uint8), _stream()), 'edge_bwd')
     return dp
 
 
@@ -653,8 +625,8 @@ def corr_lookup_bwd(corr_idx, xyz2_pad, coords, slots, g_vox, g_sel, levels, bas
     b, n, k = corr_idx.shape
     m = _table_rows(xyz2_pad, b)
     d_corr = torch.empty(b, n, k, dtype=torch.float32, device=corr_idx.device)
-    _count(lib().pvraft_corr_lookup_nm_bwd(_p(corr_idx, torch.int32), _p(xyz2_pad), _p(coords), _p(slots, torch.int32), _p(g_vox),
-                                           g_vox.shape[-1], _p(g_sel), b, n, m, k, levels, float(base_scale), _p(d_corr), _stream()),
+    _count(lib().pvraft_corr_lookup_bwd(_p(corr_idx, torch.int32), _p(xyz2_pad), _p(coords), _p(slots, torch.int32), _p(g_vox),
+                                        g_vox.shape[-1], _p(g_sel), b, n, m, k, levels, float(base_scale), _p(d_corr), _stream()),
            'corr_lookup_bwd')
     return d_corr
 
@@ -667,12 +639,9 @@ def corr_init_bwd(g, idx, fmap1, fmap2):
         raise ValueError(f'corr_init_bwd: feature maps {tuple(fmap1.shape)} and {tuple(fmap2.shape)}')
     d1 = torch.empty_like(fmap1)
     d2 = torch.zeros_like(fmap2)
-    args = (_p(g), _p(idx, torch.int32), _p(fmap1), _p(fmap2), b, n, m, c, g.shape[-1], _p(d1), _p(d2))
-    if deterministic():
-        ws = _det_workspace(lib().pvraft_corr_init_nm_bwd_det_workspace_bytes(b, m, c), fmap1.device)
-        _count(lib().pvraft_corr_init_nm_bwd_det(*args, _p(ws, torch.uint8), _stream()), 'corr_init_bwd_det')
-    else:
-        _count(lib().pvraft_corr_init_nm_bwd(*args, _stream()), 'corr_init_bwd')
+    ws = _det_workspace(lib().pvraft_corr_init_bwd_det_workspace_bytes, b, m, c, device=fmap1.device)
+    _count(lib().pvraft_corr_init_bwd(_p(g), _p(idx, torch.int32), _p(fmap1), _p(fmap2), b, n, m, c, g.shape[-1], _p(d1), _p(d2),
+                                      _p(ws, torch.uint8), _stream()), 'corr_init_bwd')
     return d1, d2
 
 

@@ -510,9 +510,9 @@ def test_lookup_static_split_without_moments(dev, sm_count):
     sel = torch.empty(b, n, 32, 4, dtype=torch.float32, device=dev)
     slots = torch.empty(b, n, 32, dtype=torch.int32, device=dev)
     cube = torch.empty(b, n, k, levels, dtype=torch.int8, device=dev)
-    rc = lib().pvraft_corr_lookup_fwd(ops._p(cb.corr_val), ops._p(cb.corr_idx, torch.int32), ops._p(cb._xyz2p), ops._p(cd), b, n, k,
+    rc = lib().pvraft_corr_lookup_fwd(ops._p(cb.corr_val), ops._p(cb.corr_idx, torch.int32), ops._p(cb._xyz2p), ops._p(cd), b, n, n, k,
                                       levels, scale, ops._p(vox), ld, ops._p(sel), ops._p(slots, torch.int32), None,
-                                      ops._p(cube, torch.int8), ops._stream())
+                                      ops._p(cube, torch.int8), None, ops._stream())
     assert rc == 0
     out = dict(vox=vox, knn_sel=sel, knn_slot=slots, cube=cube)
     e = check_lookup(cb, out, coords, torch.arange(n), levels, scale, moments=False)

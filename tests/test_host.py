@@ -27,18 +27,18 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(handle, name), f'{name} is declared in the header but not exported'
     assert declared == set(_lib.EXPORTS), 'ctypes binding and header disagree'
     lib = _lib.lib()
-    assert lib.pvraft_version() == 100
+    assert lib.pvraft_version() == 200
     for which, struct in enumerate([_lib.LinearArgs, _lib.CorrFeatArgs, _lib.GruArgs, _lib.FlowOutArgs, _lib.TcLinearArgs,
-                                    _lib.KnnBranchArgs]):
+                                    _lib.KnnBranchArgs, _lib.UpdateChainArgs]):
         assert lib.pvraft_sizeof(which) == ctypes.sizeof(struct), f'struct {struct.__name__} layout drifted'
 
 
 def test_argument_errors_are_reported_without_a_gpu():
     from pvraft_b200 import _lib
     lib = _lib.lib()
-    rc = lib.pvraft_corr_lookup_fwd(None, None, None, None, 1, 64, 64, 3, 0.25, None, 0, None, None, None, None, None)
+    rc = lib.pvraft_corr_lookup_fwd(None, None, None, None, 1, 64, 64, 64, 3, 0.25, None, 0, None, None, None, None, None, None)
     assert rc == -1 and b'null' in lib.pvraft_last_error_string()
-    rc = lib.pvraft_corr_lookup_fwd(16, 16, 16, 16, 1, 64, 96, 3, 0.25, 16, 0, 16, None, None, None, None)
+    rc = lib.pvraft_corr_lookup_fwd(16, 16, 16, 16, 1, 64, 64, 96, 3, 0.25, 16, 0, 16, None, None, None, None, None)
     assert rc == -2 and b'truncate_k=96' in lib.pvraft_last_error_string()
     rc = lib.pvraft_knn_fwd(8, 8, 1, 16, 16, 33, 0, 8, None, None, None)
     assert rc == -2
