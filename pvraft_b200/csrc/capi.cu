@@ -1,8 +1,8 @@
-// Error plumbing + device queries of the C ABI (include/pvraft_b200.h).
+// Error plumbing + device queries of the C ABI (include/pvraft_b200.h), and the tensor-map encoder of the TMA kernels.
 #include <stdarg.h>
 #include <string.h>
 
-#include "common.cuh"
+#include "tma.cuh"
 
 namespace pvraft {
 
@@ -40,6 +40,32 @@ int sm_count() {
         cached_dev = dev;
     }
     return cached;
+}
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+int make_tensor_map(CUtensorMap* map, const float* base, long long rows, int cols, long long ld, int box_rows, const char* op) {
+    // through the driver entry point (no link-time dependency on libcuda), looked up once: the initialisation of a
+    // function-local static is thread-safe, and the library is called from several host threads (nn.DataParallel)
+    static const EncodeTiledFn encode = []() -> EncodeTiledFn {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+            return reinterpret_cast<EncodeTiledFn>(p);
+        return nullptr;
+    }();
+    if (!encode) return fail(PVRAFT_ERR_UNSUPPORTED, "%s: cuTensorMapEncodeTiled is not available from this driver", op);
+    const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
+    const cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
+    const cuuint32_t estr[2] = {1, 1};
+    const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(PVRAFT_ERR_UNSUPPORTED, "%s: cuTensorMapEncodeTiled failed (%d)", op, (int)r);
+    return 0;
 }
 
 }  // namespace pvraft

@@ -99,6 +99,21 @@ __device__ __forceinline__ ActCoef act_coef(int act, float slope) {
 }
 __device__ __forceinline__ float apply_act(float x, const ActCoef& c) { return fmaf(c.slope, fminf(x, 0.f), fmaxf(x, c.lo)); }
 
+// prologue of four consecutive channels: the folded GroupNorm affine, then the activation
+__device__ __forceinline__ float4 tc_gn_act4(float4 x, const float4& sc, const float4& sh, const ActCoef& act) {
+    x.x = apply_act(fmaf(x.x, sc.x, sh.x), act);
+    x.y = apply_act(fmaf(x.y, sc.y, sh.y), act);
+    x.z = apply_act(fmaf(x.z, sc.z, sh.z), act);
+    x.w = apply_act(fmaf(x.w, sc.w, sh.w), act);
+    return x;
+}
+
+// ConvGRU gates of the tensor-core kernels (tc_linear.cu, update_chain.cu)
+__device__ __forceinline__ float tsigmoid(float x) { return 1.f / (1.f + expf(-x)); }
+// ConvGRU state update h' = (1 - z) h + z tanh(q) (model/update.py:37-39); one definition for every kernel that applies it, so
+// that the multiply-add contraction is the same everywhere
+__device__ __forceinline__ float tgru_blend(float z, float h, float q_pre) { return (1.f - z) * h + z * tanhf(q_pre); }
+
 // Contiguous split of `total` items over `parts` workers: worker w gets [begin, end).
 __host__ __device__ __forceinline__ void split_range(long long total, int parts, int w, long long& begin, long long& end) {
     const long long per = (total + parts - 1) / parts;

@@ -8,8 +8,7 @@
 // hi*hi + lo*hi + hi*lo (the classic 3xTF32 scheme, error ~2^-21 relative per product; the dropped lo*lo term is
 // ~2^-22).  The kernel is persistent (one CTA per SM walks 128 x 128 output tiles); roles and pipeline are described at
 // k_corr_gemm below.  The division by sqrt(C) is a true division, as on the reference's CPU path.
-#include <cuda.h>
-
+#include "tma.cuh"
 #include "wgmma.cuh"
 
 namespace pvraft {
@@ -20,34 +19,6 @@ constexpr int kOperandBytes = kTileM * kBlockK * 4;         // 16 KB
 constexpr int kStageBytes = 4 * kOperandBytes;              // A_hi, A_lo, B_hi, B_lo
 constexpr int kStages = 3;
 constexpr int kConsumerWarps = 8;
-
-__device__ __forceinline__ unsigned su32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init_(void* bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(su32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx_(void* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(su32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_(void* bar, unsigned parity) {
-    asm volatile(
-        "{\n\t.reg .pred P1;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t}" ::"r"(su32(bar)),
-        "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_(void* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(su32(bar)) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, void* bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(su32(dst)),
-                 "l"(map), "r"(su32(bar)), "r"(c0), "r"(c1)
-                 : "memory");
-}
 
 struct GemmParams {
     float* corr;   // [B, tiles_m * 128, ldc]: rows [r0, r0 + 128 tiles_m) x columns [c0, c0 + 128 tiles_n) of every sample
@@ -78,21 +49,19 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
             const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, const GemmParams p) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    // 1024-byte alignment (SWIZZLE_128B) by pointer arithmetic on the shared array: an integer round trip would lose the
-    // address space and turn every shared-memory access into a generic LD/ST
-    unsigned char* tiles = smem_raw + ((1024u - ((unsigned)__cvta_generic_to_shared(smem_raw) & 1023u)) & 1023u);
+    unsigned char* tiles = SMEM_ALIGN_1024(smem_raw);
     __shared__ __align__(8) unsigned long long s_full[kStages], s_empty[kStages];
     const int warp = warp_id(), lane = lane_id();
     const int num_kb = p.C / kBlockK;
     const long long my_tiles = blockIdx.x < p.n_tiles ? (p.n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
 
     if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b_lo) : "memory");
-        for (int s = 0; s < kStages; ++s) { mbar_init_(&s_full[s], 1); mbar_init_(&s_empty[s], kConsumerWarps); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        prefetch_tensormap(&map_a_hi);
+        prefetch_tensormap(&map_a_lo);
+        prefetch_tensormap(&map_b_hi);
+        prefetch_tensormap(&map_b_lo);
+        for (int s = 0; s < kStages; ++s) { mbar_init(&s_full[s], 1); mbar_init(&s_empty[s], kConsumerWarps); }
+        fence_mbarrier_init();
     }
     __syncthreads();
     const int tiles_per_batch = p.tiles_m * p.tiles_n;
@@ -108,9 +77,9 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
                 const int tile_m = r / p.tiles_n, tile_n = r - tile_m * p.tiles_n;
                 const int row_a = b * p.N + p.r0 + tile_m * kTileM, row_b = b * p.M + p.c0 + tile_n * kTileN;
                 for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait_(&s_empty[s], phase ^ 1u);
+                    mbar_wait(&s_empty[s], phase ^ 1u);
                     unsigned char* st = tiles + (size_t)s * kStageBytes;
-                    mbar_expect_tx_(&s_full[s], kStageBytes);
+                    mbar_expect_tx(&s_full[s], kStageBytes);
                     tma_load_2d(st + 0 * kOperandBytes, &map_a_hi, &s_full[s], kb * kBlockK, row_a);
                     tma_load_2d(st + 1 * kOperandBytes, &map_a_lo, &s_full[s], kb * kBlockK, row_a);
                     tma_load_2d(st + 2 * kOperandBytes, &map_b_hi, &s_full[s], kb * kBlockK, row_b);
@@ -133,7 +102,7 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
         const int b = (int)(t / tiles_per_batch), r = (int)(t - (long long)b * tiles_per_batch);
         const int tile_m = r / p.tiles_n, tile_n = r - tile_m * p.tiles_n;
         for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait_(&s_full[s], phase);
+            mbar_wait(&s_full[s], phase);
             unsigned char* st = tiles + (size_t)s * kStageBytes;
             const unsigned long long a_hi = wgmma_desc(st + 0 * kOperandBytes + a_off), a_lo = wgmma_desc(st + 1 * kOperandBytes + a_off);
             const unsigned long long b_hi = wgmma_desc(st + 2 * kOperandBytes), b_lo = wgmma_desc(st + 3 * kOperandBytes);
@@ -147,13 +116,13 @@ k_corr_gemm(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant_
             }
             wgmma_commit();
             wgmma_wait<1>();                       // the previous k-block's MMAs have retired: its stage may be refilled
-            if (prev_s >= 0 && lane == 0) mbar_arrive_(&s_empty[prev_s]);
+            if (prev_s >= 0 && lane == 0) mbar_arrive(&s_empty[prev_s]);
             prev_s = s;
             if (++s == kStages) { s = 0; phase ^= 1u; }
         }
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
-        if (lane == 0) mbar_arrive_(&s_empty[prev_s]);
+        if (lane == 0) mbar_arrive(&s_empty[prev_s]);
         prev_s = -1;
         // corr / sqrt(C) as a true (correctly rounded) division (model/corr.py:99)
         const int row = tile_m * kTileM + half * 64 + wq * 16 + (lane >> 2);
@@ -186,45 +155,17 @@ __global__ void k_tf32_split(const float* __restrict__ x, long long n, float* __
     *reinterpret_cast<float4*>(lo + i) = make_float4(l[0], l[1], l[2], l[3]);
 }
 
-// ---- host: tensor maps through the driver entry point (no link-time dependency on libcuda) ----------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-    return fn;
-}
-
-// [rows, C] fp32 row-major, box = 128 rows x 32 columns, 128-byte swizzle
-static int make_map(CUtensorMap* m, const float* base, long long rows, int C) {
-    EncodeTiledFn fn = encode_fn();
-    if (!fn) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul: cuTensorMapEncodeTiled is not available from this driver");
-    const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)C * sizeof(float)};
-    const cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)kTileM};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(PVRAFT_ERR_UNSUPPORTED, "corr_matmul: cuTensorMapEncodeTiled failed (%d)", (int)r);
-    return 0;
-}
-
 // Rows [r0, r0 + 128 tiles_m) x columns [c0, c0 + 128 tiles_n) of every sample, from split operands A [B*N, C] and
 // B [B*M, C] (hi/lo of both maps), into corr [B, 128 tiles_m, ldc]
 static int launch_gemm(const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo, int B, int N, int M, int C, int r0,
                        int tiles_m, int c0, int tiles_n, float* corr, long long ldc, cudaStream_t st) {
     int rc;
     CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
-    if ((rc = make_map(&ma_hi, a_hi, (long long)B * N, C)) || (rc = make_map(&ma_lo, a_lo, (long long)B * N, C)) ||
-        (rc = make_map(&mb_hi, b_hi, (long long)B * M, C)) || (rc = make_map(&mb_lo, b_lo, (long long)B * M, C)))
+    const long long rows_a = (long long)B * N, rows_b = (long long)B * M;
+    if ((rc = make_tensor_map(&ma_hi, a_hi, rows_a, C, C, kTileM, "corr_matmul")) ||
+        (rc = make_tensor_map(&ma_lo, a_lo, rows_a, C, C, kTileM, "corr_matmul")) ||
+        (rc = make_tensor_map(&mb_hi, b_hi, rows_b, C, C, kTileN, "corr_matmul")) ||
+        (rc = make_tensor_map(&mb_lo, b_lo, rows_b, C, C, kTileN, "corr_matmul")))
         return rc;
     GemmParams p{};
     p.corr = corr; p.N = N; p.M = M; p.C = C;

@@ -26,6 +26,7 @@
 #include <math.h>
 
 #include "fixed_point.cuh"
+#include "tma.cuh"
 
 namespace pvraft {
 
@@ -75,31 +76,6 @@ __device__ __forceinline__ unsigned cell_code(float dx, float dy, float dz, floa
     const bool ok = fmaxf(fmaxf(fabsf(qx), fabsf(qy)), fabsf(qz)) <= 1.f;
     const int cell = (int)fmaf(qx, 9.f, fmaf(qy, 3.f, qz + 13.f));
     return ok ? (unsigned)cell : 0xFFu;
-}
-
-// ---- mbarrier / bulk-copy (TMA) primitives ----------------------------------------------------------
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(void* bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(void* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(void* bar, unsigned parity) {
-    asm volatile(
-        "{\n\t.reg .pred P1;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t}" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, void* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
 }
 
 // bring a row of `bytes` bytes into L2 (64 B per lane per step); it is read sparsely (valid + kNN slots) afterwards
@@ -185,7 +161,7 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
 
     if (active_warp && lane == 0) mbar_init(s_bar, 1);
     if (threadIdx.x == 0) mbar_init(&s_tabbar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
     __syncthreads();
 
     // Work distribution.  With a moment buffer (zeroed by the caller) and at least one CTA per sample, the CTAs of a sample

@@ -1,4 +1,5 @@
-// Hopper warpgroup MMA (wgmma) on TF32 operands in shared memory, shared by corr_gemm.cu and tc_linear.cu.
+// Hopper warpgroup MMA (wgmma) on TF32 operands in shared memory, shared by corr_gemm.cu, tc_linear.cu and update_chain.cu,
+// and the 3xTF32 pieces of the two tensor-core layer kernels (tc_linear.cu, update_chain.cu).
 //
 // Both operands are K-major tiles written by TMA with SWIZZLE_128B: rows of 32 fp32 (128 bytes), 8-row swizzle atoms of
 // 1024 bytes, the tile 1024-byte aligned.  One wgmma.m64nNk8 multiplies 64 rows of A by N rows of B over K = 8 (32 bytes of
@@ -103,6 +104,36 @@ __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], unsigned long lo
         "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(da), "l"(db), "r"(accumulate));
+}
+
+// ---- 3xTF32 operands of the tensor-core layers: x = hi + lo, x . w ~ hi . w_hi + lo . w_hi + hi . w_lo ---------------------
+constexpr int kTcM = 128, kTcKB = 32;         // tile rows (points), k-block channels (one 128-byte swizzle row)
+constexpr int kTcABytes = kTcM * kTcKB * 4;   // 16 KB: one activation box
+
+// round-to-nearest (ties away from zero) to the 10-bit TF32 mantissa with two full-rate integer ops; identical to
+// cvt.rna.tf32.f32 for finite values (the conversion instruction runs at a fraction of the ALU rate)
+__device__ __forceinline__ float tf32_rna(float x) {
+    return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
+}
+// one k-block (32 channels) of a warpgroup's 64 x N accumulator: 3xTF32, four K = 8 slices
+template <int N>
+__device__ __forceinline__ void tc_mma_kblock(float (&acc)[64], unsigned long long a_hi, unsigned long long a_lo, unsigned long long b_hi,
+                                              unsigned long long b_lo, int kb) {
+#pragma unroll
+    for (int k = 0; k < kTcKB / 8; ++k) {
+        wgmma_tf32<N>(acc, wgmma_desc_k(a_hi, k), wgmma_desc_k(b_hi, k), (kb | k) != 0);
+        wgmma_tf32<N>(acc, wgmma_desc_k(a_lo, k), wgmma_desc_k(b_hi, k), 1);
+        wgmma_tf32<N>(acc, wgmma_desc_k(a_hi, k), wgmma_desc_k(b_lo, k), 1);
+    }
+}
+// 3xTF32 operand split of one 16-byte chunk at byte offset `off` of an operand stage: hi = tf32(x) at stage + off, lo =
+// tf32(x - hi) at the same offset of the lo box behind it
+__device__ __forceinline__ void tc_split_store(unsigned char* stage, int off, const float4& x) {
+    float4 hi, lo;
+    hi.x = tf32_rna(x.x); hi.y = tf32_rna(x.y); hi.z = tf32_rna(x.z); hi.w = tf32_rna(x.w);
+    lo.x = tf32_rna(x.x - hi.x); lo.y = tf32_rna(x.y - hi.y); lo.z = tf32_rna(x.z - hi.z); lo.w = tf32_rna(x.w - hi.w);
+    *reinterpret_cast<float4*>(stage + off) = hi;
+    *reinterpret_cast<float4*>(stage + kTcABytes + off) = lo;
 }
 
 }  // namespace pvraft
