@@ -526,12 +526,21 @@ PVRAFT_API int pvraft_maxk_fwd(const float* x, int64_t pts, int C, float* y, uin
 PVRAFT_API int pvraft_maxk_bwd(const float* dy, const uint8_t* arg, int64_t pts, int C, float* dx, void* stream);
 
 /* Backward of pvraft_corr_lookup_fwd w.r.t. corr_val (model/corr.py:47-66,84; indices and coordinates carry no gradient:
- * corr.py:52-62 is under no_grad and RAFTSceneFlow.py:41 detaches the coordinates):
+ * corr.py:52-62 is under no_grad and RAFTSceneFlow.py:41 detaches the coordinates; the gradient w.r.t. the gather table
+ * is pvraft_corr_lookup_xyz_bwd):
  *   g_vox [B,N,vox_ld], g_sel [B,N,32,4] (channel 0 used), knn_slot [B,N,32] from the forward, xyz2_pad [B,M,4]
  *   -> d_corr [B,N,K] (overwritten).  The means' divisor is clamp(count, 1, N), as in the forward. */
 PVRAFT_API int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2_pad, const float* coords, const int32_t* knn_slot,
                                       const float* g_vox, int vox_ld, const float* g_sel, int B, int N, int M, int K, int levels,
                                       float base_scale, float* d_corr, void* stream);
+/* Backward of pvraft_corr_lookup_fwd's kNN 4-vectors w.r.t. the gather table (model/corr.py:42,88-89: knn_xyz =
+ * truncate_xyz2[slot] - coords; the voxel branch's index math carries no gradient):
+ *   corr_idx [B,N,K] (stored order, ids < M), knn_slot [B,N,32] from the forward, g_sel [B,N,32,4] (channels 1..3 used)
+ *   -> d_xyz2[b, corr_idx[b,n,knn_slot[b,n,j]], c] += g_sel[b,n,j,1+c]   (d_xyz2 [B,M,3] ACCUMULATED, zeroed by the caller).
+ * 32 <= K <= M. */
+PVRAFT_API int pvraft_corr_lookup_xyz_bwd(const int32_t* corr_idx, const int32_t* knn_slot, const float* g_sel, int B, int N, int M, int K,
+                                          float* d_xyz2, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_corr_lookup_xyz_bwd_det_workspace_bytes(int B, int M);
 
 /* Backward of the truncated correlation (model/corr.py:95-100 + the top-k gather of :37-38), sparse over the K kept entries:
  *   g [B,N,K], idx [B,N,K] (same stored order, ids < M), fmap1 [B,N,C], fmap2 [B,M,C] point-major

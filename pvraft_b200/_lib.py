@@ -124,6 +124,8 @@ _SIGNATURES = {
     'pvraft_maxk_bwd': (C.c_int, [VP, VP, C.c_int64, C.c_int, VP, VP]),
     'pvraft_corr_lookup_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_int, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                          VP, VP]),
+    'pvraft_corr_lookup_xyz_bwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_corr_lookup_xyz_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
     'pvraft_corr_init_bwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
     'pvraft_corr_init_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
     'pvraft_flow_metrics_fwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, VP]),

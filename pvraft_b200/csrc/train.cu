@@ -712,6 +712,30 @@ __global__ void __launch_bounds__(256) k_lookup_bwd(const LookupBwdParams p) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// Correlation lookup, backward w.r.t. the gather table (model/corr.py:42,88-89: knn_xyz = truncate_xyz2[slot] - coords, the
+// coordinates detached):  d xyz2[b, corr_idx[b,n,knn_slot[b,n,j]], c] += g_sel[b,n,j,1+c].
+// One warp per query point, lane = selected neighbour; ids read in the stored (reordered) row order, as k_lookup_bwd does.
+// DET: d_xyz2 is the fixed-point workspace [B,M,3].
+// ---------------------------------------------------------------------------------------------------------------------
+template <bool DET>
+__global__ void __launch_bounds__(256) k_lookup_xyz_bwd(const int32_t* __restrict__ corr_idx, const int32_t* __restrict__ knn_slot,
+                                                        const float* __restrict__ g_sel, int B, int N, int M, int K,
+                                                        float* __restrict__ d_xyz2) {
+    const int lane = lane_id(), w = warp_id();
+    const long long pt = (long long)blockIdx.x * 8 + w;
+    if (pt >= (long long)B * N) return;
+    const int b = (int)(pt / N);
+    const int slot = __ldg(knn_slot + pt * PVRAFT_KNN + lane);
+    const size_t row = ((size_t)b * M + __ldg(corr_idx + pt * K + slot)) * 3;
+    const float* g = g_sel + (pt * PVRAFT_KNN + lane) * 4 + 1;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(d_xyz2) + (row + c) * kFxWords, (double)__ldg(g + c));
+        else atomicAdd(d_xyz2 + row + c, __ldg(g + c));
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // Truncated correlation, backward (model/corr.py:95-100 then the top-k gather of :37-38), sparse: only the K kept entries
 // of a row carry gradient, so the dense N x M gradient of the reference is never formed (f2, d_f2: M rows per sample):
 //   d f1[b,n,:] = (1/sqrt(C)) sum_k g[b,n,k] f2[b,idx[b,n,k],:]      d f2[b,m,:] += (1/sqrt(C)) g[b,n,k] f1[b,n,:]  (m = idx[b,n,k])
@@ -991,6 +1015,26 @@ extern "C" int pvraft_corr_lookup_bwd(const int32_t* corr_idx, const float* xyz2
     k_lookup_bwd<<<(unsigned)((pts + 7) / 8), 256, 0, (cudaStream_t)stream>>>(p);
     return check_launch("corr_lookup_bwd");
 }
+
+extern "C" int pvraft_corr_lookup_xyz_bwd(const int32_t* corr_idx, const int32_t* knn_slot, const float* g_sel, int B, int N, int M, int K,
+                                          float* d_xyz2, void* det_workspace, void* stream) {
+    if (!corr_idx || !knn_slot || !g_sel || !d_xyz2) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup_xyz_bwd: null pointer");
+    if (B <= 0 || N <= 0 || M <= 0 || K < PVRAFT_KNN || K > M) return fail(PVRAFT_ERR_BAD_ARG, "corr_lookup_xyz_bwd: bad shape");
+    const long long pts = (long long)B * N;
+    const unsigned blocks = (unsigned)((pts + 7) / 8);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!det_workspace) {
+        k_lookup_xyz_bwd<false><<<blocks, 256, 0, st>>>(corr_idx, knn_slot, g_sel, B, N, M, K, d_xyz2);
+        return check_launch("corr_lookup_xyz_bwd");
+    }
+    k_lookup_xyz_bwd<true><<<blocks, 256, 0, st>>>(corr_idx, knn_slot, g_sel, B, N, M, K, static_cast<float*>(det_workspace));
+    const int rc = check_launch("corr_lookup_xyz_bwd");
+    if (rc) return rc;
+    const long long vals = (long long)B * M * 3;
+    return fx_flush_f32(static_cast<const unsigned long long*>(det_workspace), 1, vals, vals, 0, d_xyz2, st);
+}
+
+extern "C" int64_t pvraft_corr_lookup_xyz_bwd_det_workspace_bytes(int B, int M) { return (int64_t)B * M * 3 * kFxWords * 8; }
 
 template <bool DET>
 static int corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M, int C, int K,

@@ -10,6 +10,31 @@ import torch
 from . import ops
 
 
+class EdgeFeatsFn(torch.autograd.Function):
+    """(xyz [B,N,3], nbr [B,N,k] int32, rel [B,N,k,3]) -> rel = xyz[nbr] - xyz, differentiable w.r.t. xyz
+    (model/flot/graph.py:72; the adjacency carries no gradient).  The forward returns `rel` as given -- the kNN kernel writes
+    it with the adjacency -- and the backward is pvraft_edge_bwd with C = 3: d xyz[nbr] += d rel, d xyz -= sum_j d rel."""
+
+    @staticmethod
+    def forward(ctx, xyz, nbr, rel):
+        ctx.save_for_backward(nbr)
+        ctx.shape = xyz.shape
+        return rel
+
+    @staticmethod
+    def backward(ctx, d_rel):
+        nbr, = ctx.saved_tensors
+        b, n, k = nbr.shape
+        dp = torch.zeros(ctx.shape, dtype=torch.float32, device=d_rel.device)
+        ops.edge_bwd(d_rel.reshape(b, n * k, 3).contiguous(), nbr, dp)
+        return dp, None, None
+
+
+def edge_feats(xyz, nbr, rel):
+    """Edge features of the adjacency nbr that gradients reach xyz through; rel: their values, xyz[nbr] - xyz."""
+    return EdgeFeatsFn.apply(xyz, nbr, rel)
+
+
 class Graph:
     def __init__(self, nbr, edge_feats, k_neighbors, size, order=None):
         self.nbr = nbr                    # int32 [B,N,k] local ids
@@ -43,6 +68,8 @@ class Graph:
             raise ValueError(f'need at least {nb_neighbors} points per cloud, got {n}')
         pc = pcloud.detach().contiguous().float()
         nbr, rel = ops.knn(pc, pc, nb_neighbors, mode=0, want_rel=True)
+        if torch.is_grad_enabled() and pcloud.requires_grad:
+            rel = edge_feats(pcloud.float(), nbr, rel)
         # spatially coherent processing order for the edge kernel (changes no result: the 8 warps of a CTA then gather
         # overlapping neighbourhoods, which L1 serves)
         order = ops.point_order(pc) if n >= 64 else None

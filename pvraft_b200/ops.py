@@ -631,6 +631,17 @@ def corr_lookup_bwd(corr_idx, xyz2_pad, coords, slots, g_vox, g_sel, levels, bas
     return d_corr
 
 
+def corr_lookup_xyz_bwd(corr_idx, slots, g_sel, d_xyz2):
+    """d_xyz2 [B,M,3] (zeroed by the caller) += the gradient of the kNN 4-vectors g_sel [B,N*32,4] w.r.t. the second cloud's
+    rows, through the state's ids corr_idx [B,N,K] and the forward's slots [B,N,32]."""
+    b, n, k = corr_idx.shape
+    m = d_xyz2.shape[1]
+    ws = _det_workspace(lib().pvraft_corr_lookup_xyz_bwd_det_workspace_bytes, b, m, device=d_xyz2.device)
+    _count(lib().pvraft_corr_lookup_xyz_bwd(_p(corr_idx, torch.int32), _p(slots, torch.int32), _p(g_sel), b, n, m, k, _p(d_xyz2),
+                                            _p(ws, torch.uint8), _stream()), 'corr_lookup_xyz_bwd')
+    return d_xyz2
+
+
 def corr_init_bwd(g, idx, fmap1, fmap2):
     """g, idx [B,N,K], fmap1 [B,N,C], fmap2 [B,M,C] -> (d fmap1 [B,N,C], d fmap2 [B,M,C])."""
     b, n, c = fmap1.shape

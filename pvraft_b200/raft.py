@@ -19,11 +19,14 @@ from .refine import FlotRefine
 from .update import UpdateBlock
 
 
-def _records_grad(module):
-    """True when the caller differentiates through this forward (tools/engine.py:140-143): the training path of train.py runs;
-    otherwise (torch.no_grad(), or nothing requires grad) the fused inference kernels do."""
+def _records_grad(module, p):
+    """True when the caller differentiates through this forward (tools/engine.py:140-143), w.r.t. a parameter or an input
+    cloud of p: the training path of train.py runs; otherwise (torch.no_grad(), or nothing requires grad) the fused
+    inference kernels do."""
     if not torch.is_grad_enabled():
         return False
+    if p[0].requires_grad or p[1].requires_grad:   # (inside an nn.DataParallel replica: the scattered inputs keep requires_grad)
+        return True
     for m in module.modules():
         # nn.DataParallel replicas keep their (non-leaf) parameter copies in `_former_parameters`; `.parameters()` is empty there
         for t in list(m._parameters.values()) + list(getattr(m, '_former_parameters', {}).values()):
@@ -108,7 +111,7 @@ class _RaftBase(nn.Module):
         if not p[0].is_cuda:
             raise ops._lib.PvraftError('pvraft_b200 kernels need CUDA tensors (no CPU fallback exists)')
         with torch.cuda.device(p[0].device):        # the library launches on the current device
-            if _records_grad(self):
+            if _records_grad(self, p):
                 return self._forward_train(p, num_iters)
             graph = self.use_cuda_graph
             if graph is None:    # automatic (never inside an nn.DataParallel replica thread)
@@ -238,8 +241,14 @@ class RSF_refine(_RaftBase):
 
     def _forward_train(self, p, num_iters=12):
         """model/RAFTSceneFlowRefine.py:22-48: everything up to the last flow under no_grad (the fused inference kernels),
-        the refiner -- the only part tools/engine_refine.py trains -- layer by layer with gradients."""
+        the refiner -- the only part tools/engine_refine.py trains -- layer by layer with gradients.  The refiner's input
+        flow is coords2 - xyz1 with coords2 computed under no_grad, so xyz1 receives minus the flow's gradient and xyz2 none."""
+        x1 = p[0].float()
+        if x1.requires_grad and self.corr_block.state_dtype != torch.float32:
+            raise NotImplementedError("training differentiates through the fp32 state: call model.set_precision('fp32')")
         with torch.no_grad():
             xyz1, _, graph, graph_context, net, inp = self._encode(p)
             flow, _ = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=False)
+        if x1.requires_grad:
+            flow = flow + (x1.detach() - x1)          # the same values; d xyz1 = -d flow
         return train.flot_refine(self.refine_block, flow, graph)

@@ -11,12 +11,15 @@ The forward runs layer by layer -- the fused inference kernels keep no activatio
     EdgeFn          SetConv edge stage        pvraft_edge_fwd / pvraft_edge_bwd          (model/flot/gconv.py:65-73)
     MaxKFn          max over 32 neighbours    pvraft_maxk_fwd / pvraft_maxk_bwd          (gconv.py:80, model/corr.py:92)
     CorrInitFn      truncated correlation     wgmma GEMM + top-k + reorder / pvraft_corr_init_bwd (sparse)   (corr.py:31-42,95-100)
-    CorrLookupFn    voxel means + kNN gather  pvraft_corr_lookup_fwd / pvraft_corr_lookup_bwd                  (corr.py:47-66,75-91)
+    CorrLookupFn    voxel means + kNN gather  pvraft_corr_lookup_fwd / pvraft_corr_lookup_bwd (+ pvraft_corr_lookup_xyz_bwd)  (corr.py:47-66,75-91)
+    EdgeFeatsFn     graph edge features       the kNN kernel's output / pvraft_edge_bwd with C = 3            (graph.py:72; in graph.py)
 
 PyTorch is the tape (which Function follows which) and the allocator; the glue between Functions that the reference also
 writes as single ATen calls (cat / split / relu / sigmoid / tanh / add / mul on [B,N,64..192] tensors: model/update.py:18-20,
-32-39, model/corr.py:45) stays ATen.  Gradients w.r.t. the coordinates are not needed: the reference detaches `coords2`
-every iteration (model/RAFTSceneFlow.py:41) and derives every index under no_grad (model/corr.py:52-62).
+32-39, model/corr.py:45) stays ATen.  The input clouds stay attached, so gradients reach them as in the reference: through
+the flows (coords2 - xyz1), the encoders' first SetConv (the cloud is its signal), the graphs' edge features and, for xyz2,
+the kNN 4-vectors of every lookup.  `coords2` carries none: the reference detaches it every iteration
+(model/RAFTSceneFlow.py:41) and derives every index under no_grad (model/corr.py:52-62).
 All tensors are point-major [B,rows,C] (rows = N per-point, N*32 per-edge).
 """
 import os
@@ -222,10 +225,11 @@ class CorrInitFn(torch.autograd.Function):
 
 class CorrLookupFn(torch.autograd.Function):
     """corr_val [B,N1,K] (+ ids, gather table [B,N2,4], query coordinates [B,N1,3]) -> voxel means [B,N1,levels*27],
-    kNN 4-vectors [B,N1*32,4]."""
+    kNN 4-vectors [B,N1*32,4].  xyz2 [B,N2,3], the cloud the gather table was padded from (ops.xyz_pad), receives the
+    gradient of the kNN 4-vectors' coordinate channels when it requires grad (model/corr.py:88-89)."""
 
     @staticmethod
-    def forward(ctx, corr_val, corr_idx, xyz2p, coords, levels, base_scale):
+    def forward(ctx, corr_val, corr_idx, xyz2p, coords, levels, base_scale, xyz2=None):
         coords = coords.contiguous()
         out = ops.corr_lookup(corr_val, corr_idx, xyz2p, coords, levels, base_scale, want_slots=True, vox_ld=levels * 27)
         ctx.save_for_backward(corr_idx, xyz2p, coords, out['knn_slot'])
@@ -237,8 +241,13 @@ class CorrLookupFn(torch.autograd.Function):
     def backward(ctx, g_vox, g_sel):
         corr_idx, xyz2p, coords, slots = ctx.saved_tensors
         levels, base_scale = ctx.cfg
-        return ops.corr_lookup_bwd(corr_idx, xyz2p, coords, slots, g_vox.contiguous(), g_sel.contiguous(), levels, base_scale), \
-            None, None, None, None, None
+        g_sel = g_sel.contiguous()
+        d_corr = ops.corr_lookup_bwd(corr_idx, xyz2p, coords, slots, g_vox.contiguous(), g_sel, levels, base_scale)
+        d_xyz2 = None
+        if len(ctx.needs_input_grad) > 6 and ctx.needs_input_grad[6]:      # xyz2 given, and it requires grad
+            b, m, _ = xyz2p.shape
+            d_xyz2 = ops.corr_lookup_xyz_bwd(corr_idx, slots, g_sel, torch.zeros(b, m, 3, dtype=torch.float32, device=g_sel.device))
+        return d_corr, None, None, None, None, None, d_xyz2
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -306,8 +315,8 @@ def rsf_forward(model, p, num_iters):
     """RSF.forward with gradients (model/RAFTSceneFlow.py:22-50) -> list of num_iters flows [B,N1,3]."""
     cb = model.corr_block
     ops.check_pair(p[0], p[1], cb.truncate_k)
-    xyz1 = p[0].detach().contiguous().float()
-    xyz2 = p[1].detach().contiguous().float()
+    xyz1 = p[0].contiguous().float()                                           # attached: gradients reach the inputs
+    xyz2 = p[1].contiguous().float()
     b, n, _ = xyz1.shape
     if cb.state_dtype != torch.float32:
         raise NotImplementedError("training differentiates through the fp32 state: call model.set_precision('fp32')")
@@ -330,7 +339,7 @@ def rsf_forward(model, p, num_iters):
     preds = []
     for _ in range(num_iters):
         coords2 = coords2.detach()                                             # :41
-        vox, sel = CorrLookupFn.apply(corr_val, corr_idx, xyz2p, coords2, cb.num_levels, cb.base_scale)
+        vox, sel = CorrLookupFn.apply(corr_val, corr_idx, xyz2p, coords2, cb.num_levels, cb.base_scale, xyz2)
         corr = corr_features(cb, vox, sel)                                     # :42
         flow = coords2 - xyz1                                                  # :43
         net, delta = update_block(model.update_block, net, inp, corr, flow, graph1)   # :44
