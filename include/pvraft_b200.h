@@ -218,12 +218,16 @@ PVRAFT_API int pvraft_linear_fwd(const pvraft_linear_args* a, void* det_workspac
 PVRAFT_API int64_t pvraft_linear_det_workspace_bytes(int B);
 
 /* ------------------------------------------------------------------------------------------------
- * The same fused layer on the Hopper tensor cores (TMA + wgmma), fp32-accurate through a 3xTF32 operand split.
+ * The same fused layer on the Hopper tensor cores (TMA + wgmma), in one of two operand formats:
+ *   - 3xTF32 (w_hi, w_lo set): fp32-accurate through a hi/lo operand split;
+ *   - bf16 (w_bf16 set): activations (after the prologue) and weights rounded to bf16 (nearest even), fp32 accumulation.
+ *     Prologue, epilogue, GroupNorm statistics and every tensor in memory stay fp32.
  * Up to three activation sources are concatenated along K (e.g. [h | inp | motion] of the ConvGRU,
  * model/update.py:32,36); the GroupNorm(+max/min selection)+activation prologue and the bias / ReLU / residual /
  * GroupNorm-statistics epilogue match pvraft_linear_fwd; two extra epilogues implement the ConvGRU gates
  * (model/update.py:34-39).  Requirements: points per sample N % 128 == 0; every source has a multiple of 32
- * channels; weights pre-split with pvraft_tc_weight_split into hi/lo [n_pad, K] (n_pad = cout rounded up to 16, <= 128).
+ * channels; weights pre-split with pvraft_tc_weight_split into hi/lo [n_pad, K] (n_pad = cout rounded up to 16, <= 128), or
+ * converted with pvraft_tc_weight_bf16 into bf16 [n_pad, K].
  * --------------------------------------------------------------------------------------------- */
 typedef enum pvraft_tc_epilogue {
     PVRAFT_TC_PLAIN = 0,   /* out = act(acc + bias) (+ residual), optional output statistics                  */
@@ -268,9 +272,11 @@ typedef struct pvraft_tc_linear_args {
     const float* coords2;   /* FLOW: [B,N,3] or NULL */
     float* coords2_out;     /* FLOW: [B,N,3] or NULL (may alias coords2) */
     float* flow_out;        /* FLOW: [B,N,3] or NULL */
-    int params_settled;     /* nonzero: w_hi, w_lo, bias, bias2, w3, b3 were last written at least three launches ago on this
-                               stream (or before a synchronisation).  The kernel is launched with programmatic stream
+    int params_settled;     /* nonzero: w_hi, w_lo (or w_bf16), bias, bias2, w3, b3 were last written at least three launches ago
+                               on this stream (or before a synchronisation).  The kernel is launched with programmatic stream
                                serialization and then fetches them while the previous kernel drains.  0 is always safe. */
+    const uint16_t* w_bf16; /* [n_pad, K] bf16 weights, or NULL.  Set: bf16 operands, and w_hi, w_lo must be NULL
+                               (PVRAFT_ERR_BAD_ARG otherwise) */
 } pvraft_tc_linear_args;
 
 /* det_workspace: pvraft_tc_linear_det_workspace_bytes(B) bytes or NULL ("Deterministic mode"; it orders out_stats). */
@@ -285,7 +291,8 @@ PVRAFT_API int64_t pvraft_tc_linear_det_workspace_bytes(int B);
  *   z, r   = sigmoid(W_zr [net | inp | motion] + [b_z | b_r])     (ConvGRU, model/update.py:34-35)
  *   net_out = (1 - z) net + z tanh(W_q [r*net | inp | motion] + b_q)   (model/update.py:36-39)
  *   p_out  = W_fc1[:, :64] net_out                                 (flow-head SetConv fc1 pre-transform, no bias)
- * Weights pre-split with pvraft_tc_weight_split into hi/lo, [n_pad, K] row-major, in this order:
+ * Weights pre-split with pvraft_tc_weight_split into hi/lo, [n_pad, K] row-major -- or, for bf16 operands, converted with
+ * pvraft_tc_weight_bf16 into w_bf16 (then the same bits as the five bf16 pvraft_tc_linear_fwd calls) -- in this order:
  *   0 W_cc [64,192], 1 W_m [64,128] (61 rows + zero padding), 2 [W_z; W_r] [128,192], 3 W_q [64,192], 4 W_fc1 [64,64].
  * Requirements: N % 128 == 0, hidden = context = 64, y1_channels = 128 (PVRAFT_ERR_UNSUPPORTED otherwise); net_out != net.
  * No reductions: the results do not depend on the launch configuration.
@@ -312,6 +319,7 @@ typedef struct pvraft_update_chain_args {
     float* net_out;          /* [B,N,hidden] */
     float* p_out;            /* [B,N,64] */
     int B, N, hidden, context, y1_channels;
+    const uint16_t* w_bf16[5];  /* bf16 weights, or all NULL: all five set selects bf16 operands, with w_hi, w_lo all NULL */
 } pvraft_update_chain_args;
 
 PVRAFT_API int pvraft_update_chain_fwd(const pvraft_update_chain_args* a, void* stream);
@@ -319,6 +327,9 @@ PVRAFT_API int pvraft_update_chain_fwd(const pvraft_update_chain_args* a, void* 
  * written zero-padded as [rows_pad, cols_pad]. */
 PVRAFT_API int pvraft_tc_weight_split(const float* w, int rows, int cols, int ld, int col0, int rows_pad, int cols_pad,
                            float* hi, float* lo, void* stream);
+/* bf16(w) (round to nearest even) of the same window, written zero-padded as [rows_pad, cols_pad]: the w_bf16 operand. */
+PVRAFT_API int pvraft_tc_weight_bf16(const float* w, int rows, int cols, int ld, int col0, int rows_pad, int cols_pad,
+                          uint16_t* out, void* stream);
 
 /* out[B,N,C] (or channel-major [B,C,N] when transpose_out != 0) = act(GN(in)) -- the trailing
  * GroupNorm+LeakyReLU of SetConv (model/flot/gconv.py:33,82-83) when nothing follows it. */

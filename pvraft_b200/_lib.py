@@ -35,7 +35,7 @@ class TcLinearArgs(C.Structure):
                 ('w_lo', VP), ('n_pad', C.c_int), ('cout', C.c_int), ('bias', VP), ('bias2', VP), ('out_act', C.c_int),
                 ('residual', VP), ('out', VP), ('out2', VP), ('h', VP), ('z', VP), ('out_stats', VP), ('epilogue', C.c_int),
                 ('B', C.c_int), ('N', C.c_int), ('tail', VP), ('w3', VP), ('b3', VP), ('coords1', VP), ('coords2', VP),
-                ('coords2_out', VP), ('flow_out', VP), ('params_settled', C.c_int)]
+                ('coords2_out', VP), ('flow_out', VP), ('params_settled', C.c_int), ('w_bf16', VP)]
 
 
 class UpdateChainArgs(C.Structure):
@@ -43,7 +43,7 @@ class UpdateChainArgs(C.Structure):
                 ('gn_slope', C.c_float), ('kfeat', VP), ('cflow', VP), ('flow', VP), ('net', VP), ('inp', VP),
                 ('w_hi', VP * 5), ('w_lo', VP * 5), ('b_cc', VP), ('b_m', VP), ('b_z', VP), ('b_r', VP), ('b_q', VP),
                 ('net_out', VP), ('p_out', VP), ('B', C.c_int), ('N', C.c_int), ('hidden', C.c_int), ('context', C.c_int),
-                ('y1_channels', C.c_int)]
+                ('y1_channels', C.c_int), ('w_bf16', VP * 5)]
 
 
 class KnnBranchArgs(C.Structure):
@@ -97,6 +97,7 @@ _SIGNATURES = {
     'pvraft_tc_linear_det_workspace_bytes': (C.c_int64, [C.c_int]),
     'pvraft_update_chain_fwd': (C.c_int, [C.POINTER(UpdateChainArgs), VP]),
     'pvraft_tc_weight_split':(C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_tc_weight_bf16': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP]),
     'pvraft_gn_act_fwd': (C.c_int, [VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int,
                                     C.c_int, VP, VP, VP]),
     'pvraft_corr_feature_fwd': (C.c_int, [C.POINTER(CorrFeatArgs), VP]),

@@ -46,7 +46,9 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-int make_tensor_map(CUtensorMap* map, const float* base, long long rows, int cols, long long ld, int box_rows, const char* op) {
+// a 2-D row-major tensor [rows, cols] with row stride ld (elements), loaded as boxes of [box_rows, 32] elements
+static int encode_2d(CUtensorMap* map, CUtensorMapDataType dtype, int esize, CUtensorMapSwizzle swizzle, const void* base, long long rows,
+                     int cols, long long ld, int box_rows, const char* op) {
     // through the driver entry point (no link-time dependency on libcuda), looked up once: the initialisation of a
     // function-local static is thread-safe, and the library is called from several host threads (nn.DataParallel)
     static const EncodeTiledFn encode = []() -> EncodeTiledFn {
@@ -58,14 +60,21 @@ int make_tensor_map(CUtensorMap* map, const float* base, long long rows, int col
     }();
     if (!encode) return fail(PVRAFT_ERR_UNSUPPORTED, "%s: cuTensorMapEncodeTiled is not available from this driver", op);
     const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
+    const cuuint64_t strides[1] = {(cuuint64_t)ld * esize};
     const cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
     const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const CUresult r = encode(map, dtype, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(PVRAFT_ERR_UNSUPPORTED, "%s: cuTensorMapEncodeTiled failed (%d)", op, (int)r);
     return 0;
+}
+
+int make_tensor_map(CUtensorMap* map, const float* base, long long rows, int cols, long long ld, int box_rows, const char* op) {
+    return encode_2d(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, CU_TENSOR_MAP_SWIZZLE_128B, base, rows, cols, ld, box_rows, op);
+}
+
+int make_tensor_map_bf16(CUtensorMap* map, const uint16_t* base, long long rows, int cols, long long ld, int box_rows, const char* op) {
+    return encode_2d(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, CU_TENSOR_MAP_SWIZZLE_64B, base, rows, cols, ld, box_rows, op);
 }
 
 }  // namespace pvraft

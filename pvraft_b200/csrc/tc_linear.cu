@@ -1,4 +1,4 @@
-// Per-point linear layers on the Hopper tensor cores (wgmma), fp32-accurate (3xTF32), with the GroupNorm / activation
+// Per-point linear layers on the Hopper tensor cores (wgmma), fp32-accurate (3xTF32) or on bf16 operands, with the GroupNorm / activation
 // prologue and the bias / activation / residual / GroupNorm-statistics / GRU-gate epilogues fused around the MMA.
 //
 //   out[M x N] = epilogue( prologue(A)[M x K] . W[N x K]^T )          M = B*Npts points, N = cout, K = cin
@@ -17,6 +17,9 @@
 //                bias / activation / residual -> transpose through shared memory -> coalesced stores; GroupNorm (sum,
 //                sum^2) of the output combined across the warps into one double atomic per (group, moment) and tile;
 //                ConvGRU-gate, cat-tail and flow-head (64 -> 3 + RAFT coordinate update) variants
+// BF16 (the 'bf16-compute' mode of the RAFT loop): the transformed activations are rounded to bf16 (nearest even) and stored
+// in the lo half of the stage, one 64-row tile per warpgroup at the group's offset; the weights arrive as bf16 boxes
+// [N x 32] (SWIZZLE_64B, pvraft_tc_weight_bf16); 2 x wgmma.m64nNk16.bf16 per k-block, fp32 accumulation and epilogues.
 // Launched with programmatic stream serialization: the prologue overlaps the previous kernel's tail (griddepcontrol.wait
 // precedes the first global read).  Replaces the k_linear / k_gru / k_corrfeat / k_flowout CUDA-core kernels whenever
 // Npts % 128 == 0 and every source has a multiple of 32 channels.
@@ -328,8 +331,9 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, float* __restrict
 __host__ __device__ __forceinline__ int tc_acc_pitch(int n) { return ((n + 31) & ~31) + 4; }
 
 // A CTA walks tiles blockIdx.x, +gridDim.x, ...; the operand ring runs across tile boundaries.
-// NT = p.N (the padded cout): the wgmma shape is part of the instruction
-template <int NT, bool DET>
+// NT = p.N (the padded cout): the wgmma shape is part of the instruction.  BF16: bf16 operands (map_w_hi holds the bf16
+// weights, map_w_lo is not read)
+template <int NT, bool DET, bool BF16>
 __global__ void __launch_bounds__(kTcThreads, 1)
 k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
             const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
@@ -337,15 +341,17 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* tiles = SMEM_ALIGN_1024(smem_raw);
     // stage layout: [A hi 16K][A lo 16K][W hi N*128][W lo N*128, only when the weights are streamed];
-    // resident weights live behind the ring as num_kb x [W hi][W lo]
-    const int w_bytes = p.N * kTcKB * 4;
+    // resident weights live behind the ring as num_kb x [W hi][W lo].
+    // BF16: [A raw 16K][A bf16: 4K at the start of each group's 8K of the lo half][W N*64, only when streamed]
+    constexpr int w_boxes = BF16 ? 1 : 2;
+    const int w_bytes = p.N * kTcKB * (BF16 ? 2 : 4);
     const int w_off = 2 * kTcABytes;
-    const int stage_bytes = w_off + (p.w_resident ? 0 : 2 * w_bytes);
+    const int stage_bytes = w_off + (p.w_resident ? 0 : w_boxes * w_bytes);
     const int S = p.stages;
     const int num_kb = p.K / kTcKB;
     const int acc_pitch = tc_acc_pitch(NT);
     unsigned char* w_res = tiles + (size_t)S * stage_bytes;
-    float* s_scale = reinterpret_cast<float*>(w_res + (p.w_resident ? (size_t)num_kb * 2 * w_bytes : 0));   // [2 groups][scale K | shift K]
+    float* s_scale = reinterpret_cast<float*>(w_res + (p.w_resident ? (size_t)num_kb * w_boxes * w_bytes : 0));   // [2 groups][scale K | shift K]
     float* s_bias = s_scale + 4 * p.K;                                            // [2 * N]
     float* s_acc = s_bias + 2 * p.N;                                              // [128 rows][acc_pitch] accumulator tile
     float* s_estage = s_acc + (size_t)kTcM * acc_pitch;                           // GRU epilogues: [8 warps][32][20] staging
@@ -359,7 +365,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
 
     if (warp == kTcProducerWarp && lane == 0) {
         prefetch_tensormap(&map_w_hi);
-        prefetch_tensormap(&map_w_lo);
+        if constexpr (!BF16) prefetch_tensormap(&map_w_lo);
         prefetch_tensormap(&map_a0);
         for (int s = 0; s < S; ++s) { mbar_init(&s_full[s], 1); mbar_init(&s_empty[s], 8); }   // 8 MMA warps release a stage
         mbar_init(&s_acc_full, 8);     // 8 MMA warps deposit the accumulator tile
@@ -373,10 +379,10 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
     // the steady state of a forward, whose weights are split once): the SMs that finished the previous kernel early then
     // hold their weights when the dependency resolves.  Every read of an ACTIVATION is below the wait.
     auto load_weights = [&]() {   // the whole weight matrix (hi and lo) once per CTA
-        mbar_expect_tx(&s_w_full, (unsigned)(num_kb * 2 * w_bytes));
+        mbar_expect_tx(&s_w_full, (unsigned)(num_kb * w_boxes * w_bytes));
         for (int kb = 0; kb < num_kb; ++kb) {
-            tma_load_2d(w_res + (size_t)kb * 2 * w_bytes, &map_w_hi, &s_w_full, kb * kTcKB, 0);
-            tma_load_2d(w_res + (size_t)kb * 2 * w_bytes + w_bytes, &map_w_lo, &s_w_full, kb * kTcKB, 0);
+            tma_load_2d(w_res + (size_t)kb * w_boxes * w_bytes, &map_w_hi, &s_w_full, kb * kTcKB, 0);
+            if constexpr (!BF16) tma_load_2d(w_res + (size_t)kb * 2 * w_bytes + w_bytes, &map_w_lo, &s_w_full, kb * kTcKB, 0);
         }
     };
     auto load_bias = [&]() {   // by the epilogue threads 0..255
@@ -403,7 +409,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
         // ===== TMA producer: raw activation boxes (and the weights) =====
         if (lane == 0) {
             if (p.w_resident && !p.settled) load_weights();
-            const unsigned tx = (unsigned)(kTcABytes * (p.minmax ? 2 : 1) + (p.w_resident ? 0 : 2 * w_bytes));
+            const unsigned tx = (unsigned)(kTcABytes * (p.minmax ? 2 : 1) + (p.w_resident ? 0 : w_boxes * w_bytes));
             TcCursor cw;
             for (int step = 0; step < total_steps; ++step, cw.next(num_kb, S)) {
                 const int s = cw.s, kb = cw.kb;
@@ -419,7 +425,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
                 if (p.minmax) tma_load_2d(st + kTcABytes, &map_min, &s_full[s], kb * kTcKB, row0);
                 if (!p.w_resident) {
                     tma_load_2d(st + w_off, &map_w_hi, &s_full[s], kb * kTcKB, 0);
-                    tma_load_2d(st + w_off + w_bytes, &map_w_lo, &s_full[s], kb * kTcKB, 0);
+                    if constexpr (!BF16) tma_load_2d(st + w_off + w_bytes, &map_w_lo, &s_full[s], kb * kTcKB, 0);
                 }
             }
         }
@@ -465,6 +471,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
             if (p.in_stats != nullptr) gn_table();
             mbar_wait(&s_full[s], cp.phase);   // the raw box(es) of this k-block have landed
             unsigned char* st = tiles + (size_t)s * stage_bytes;
+            float4 xb[4];   // BF16: the transformed chunks, stored once the group has read the whole box
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const int c = t + i * 128, r = grp * 64 + (c >> 3), lc = c & 7;
@@ -485,18 +492,32 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
                     x.z = apply_act(fmaf(x.z, sc.z, sh.z), iact);
                     x.w = apply_act(fmaf(x.w, sc.w, sh.w), iact);
                 }
+                if constexpr (BF16) {
+                    xb[i] = x;
+                    continue;
+                }
                 float4 hi, lo;
                 hi.x = tf32_rna(x.x); hi.y = tf32_rna(x.y); hi.z = tf32_rna(x.z); hi.w = tf32_rna(x.w);
                 lo.x = tf32_rna(x.x - hi.x); lo.y = tf32_rna(x.y - hi.y); lo.z = tf32_rna(x.z - hi.z); lo.w = tf32_rna(x.w - hi.w);
                 *reinterpret_cast<float4*>(st + off) = hi;   // in place: raw -> hi; the lo half of the stage held the min array
                 *reinterpret_cast<float4*>(st + kTcABytes + off) = lo;
             }
+            if constexpr (BF16) {
+                // the bf16 tile overwrites min-array rows of this group that its other threads may not have read yet
+                if (p.minmax) asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int c = t + i * 128;
+                    tc_bf16_store(st + kTcABytes + a_off, c >> 3, c & 7, xb[i]);
+                }
+            }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma (async proxy)
             asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");   // the group's 64 rows are in place
-            const unsigned char* wb = p.w_resident ? w_res + (size_t)kb * 2 * w_bytes : st + w_off;
+            const unsigned char* wb = p.w_resident ? w_res + (size_t)kb * w_boxes * w_bytes : st + w_off;
             wgmma_fence_regs(acc);
             wgmma_fence();
-            tc_mma_kblock<NT>(acc, wgmma_desc(st + a_off), wgmma_desc(st + kTcABytes + a_off), wgmma_desc(wb), wgmma_desc(wb + w_bytes), kb);
+            if constexpr (BF16) tc_mma_kblock_bf16<NT>(acc, wgmma_desc_bf16(st + kTcABytes + a_off), wgmma_desc_bf16(wb), kb);
+            else tc_mma_kblock<NT>(acc, wgmma_desc(st + a_off), wgmma_desc(st + kTcABytes + a_off), wgmma_desc(wb), wgmma_desc(wb + w_bytes), kb);
             wgmma_commit();
             wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
             if (prev_s >= 0 && lane == 0) mbar_arrive(&s_empty[prev_s]);
@@ -546,6 +567,17 @@ __global__ void k_weight_split(const float* __restrict__ w, int rows, int cols, 
     lo[i] = tf32_rna(x - h);
 }
 
+// bf16(w) (round to nearest even) of a [rows, ld] weight window [rows, cols] written as [rows_pad, cols_pad] (zero padded)
+__global__ void k_weight_bf16(const float* __restrict__ w, int rows, int cols, int ld, int col0, int rows_pad, int cols_pad,
+                              __nv_bfloat16* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= rows_pad * cols_pad) return;
+    const int r = i / cols_pad, c = i - r * cols_pad;
+    float x = 0.f;
+    if (r < rows && c < cols) x = __ldg(w + (size_t)r * ld + col0 + c);
+    out[i] = __float2bfloat16_rn(x);
+}
+
 }  // namespace pvraft
 
 using namespace pvraft;
@@ -558,9 +590,20 @@ extern "C" int pvraft_tc_weight_split(const float* w, int rows, int cols, int ld
     return check_launch("tc_weight_split");
 }
 
-template <bool DET>
+extern "C" int pvraft_tc_weight_bf16(const float* w, int rows, int cols, int ld, int col0, int rows_pad, int cols_pad, uint16_t* out,
+                                     void* stream) {
+    if (!w || !out || rows <= 0 || cols <= 0 || rows_pad < rows || cols_pad < cols) return fail(PVRAFT_ERR_BAD_ARG, "tc_weight_bf16: bad argument");
+    const int n = rows_pad * cols_pad;
+    k_weight_bf16<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(w, rows, cols, ld > 0 ? ld : cols, col0, rows_pad, cols_pad,
+                                                                      reinterpret_cast<__nv_bfloat16*>(out));
+    return check_launch("tc_weight_bf16");
+}
+
+template <bool DET, bool BF16>
 static int tc_linear_fwd(const pvraft_tc_linear_args* a, void* ws, void* stream) {
-    if (!a || !a->in[0] || !a->w_hi || !a->w_lo || !a->out) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: null pointer");
+    if (!a || !a->in[0] || !a->out) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: null pointer");
+    if (BF16 ? (a->w_hi || a->w_lo) : (!a->w_hi || !a->w_lo))
+        return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: pass either w_hi and w_lo (3xTF32) or w_bf16 (bf16), not both");
     if (a->B <= 0 || a->N <= 0 || a->n_pad < 16 || a->n_pad > 128 || a->n_pad % 16) return fail(PVRAFT_ERR_BAD_ARG, "tc_linear: bad shape (n_pad=%d)", a->n_pad);
     if (a->N % kTcM) return fail(PVRAFT_ERR_UNSUPPORTED, "tc_linear: points per sample (%d) must be a multiple of 128", a->N);
     int K = 0;
@@ -597,9 +640,13 @@ static int tc_linear_fwd(const pvraft_tc_linear_args* a, void* ws, void* stream)
     p.w3 = a->w3; p.b3 = a->b3; p.coords1 = a->coords1; p.coords2 = a->coords2; p.coords2_out = a->coords2_out; p.flow_out = a->flow_out;
     p.out_ld = a->tail ? a->cout + 3 : a->cout;
     p.settled = a->params_settled ? 1 : 0;
-    if ((rc = make_tensor_map(&mw_hi, a->w_hi, a->n_pad, K, K, a->n_pad, "tc_linear")) ||
-        (rc = make_tensor_map(&mw_lo, a->w_lo, a->n_pad, K, K, a->n_pad, "tc_linear")))
+    if (BF16) {   // the unused lo slot repeats the bf16 map (a tensor map must be valid even if never dereferenced)
+        if ((rc = make_tensor_map_bf16(&mw_hi, a->w_bf16, a->n_pad, K, K, a->n_pad, "tc_linear"))) return rc;
+        mw_lo = mw_hi;
+    } else if ((rc = make_tensor_map(&mw_hi, a->w_hi, a->n_pad, K, K, a->n_pad, "tc_linear")) ||
+               (rc = make_tensor_map(&mw_lo, a->w_lo, a->n_pad, K, K, a->n_pad, "tc_linear"))) {
         return rc;
+    }
     CUtensorMap ma[3], mmin;
     for (int s = 0; s < 3; ++s) {   // unused slots repeat source 0 (a tensor map must be valid even if never dereferenced)
         const int q = a->in[s] ? s : 0;
@@ -607,13 +654,13 @@ static int tc_linear_fwd(const pvraft_tc_linear_args* a, void* ws, void* stream)
     }
     if ((rc = make_tensor_map(&mmin, a->in_min ? a->in_min : a->in[0], M, a->in_channels[0], a->in_channels[0], kTcM, "tc_linear"))) return rc;
     const size_t a_stage = (size_t)2 * kTcABytes;
-    const size_t w_all = (size_t)(K / kTcKB) * 2 * a->n_pad * kTcKB * 4;          // hi + lo of the whole weight matrix
+    const size_t w_kb = (size_t)(BF16 ? 2 : 8) * a->n_pad * kTcKB;               // one k-block of weights: hi + lo, or bf16
+    const size_t w_all = (size_t)(K / kTcKB) * w_kb;                               // the whole weight matrix
     const bool gru = a->epilogue == TC_EPI_GRU_ZR || a->epilogue == TC_EPI_GRU_Q;
     const size_t fixed = (size_t)(4 * K + 2 * a->n_pad + kTcM * tc_acc_pitch(a->n_pad) + (gru ? 8 * 32 * kTcPitch16 : 0) + 4 * 128 * 2) * sizeof(float) + 1024 + 64;
     const size_t budget = (size_t)kSmemBudget - 2048 /* static barriers */ - fixed;
     // Weights stay resident in shared memory when that still leaves a ring of >= 3 activation stages (re-streaming the
     // same few KB per tile from every SM hot-spots a handful of L2 slices); otherwise they travel with the k-blocks.
-    const size_t w_kb = (size_t)2 * a->n_pad * kTcKB * 4;
     const int stages_res = w_all < budget ? (int)((budget - w_all) / a_stage) : 0;
     const int stages_str = (int)(budget / (a_stage + w_kb));
     p.w_resident = (stages_res >= 3 || stages_res >= stages_str) ? 1 : 0;
@@ -623,16 +670,16 @@ static int tc_linear_fwd(const pvraft_tc_linear_args* a, void* ws, void* stream)
     if (stages < 2) return fail(PVRAFT_ERR_SMEM, "tc_linear: K=%d, n_pad=%d leave room for only %d operand stage(s) (2 needed)", K, a->n_pad, stages);
     p.stages = stages;
     const size_t smem = stages * stage + (p.w_resident ? w_all : 0) + fixed;
-    decltype(&k_tc_linear<16, DET>) kernel = nullptr;
+    decltype(&k_tc_linear<16, DET, BF16>) kernel = nullptr;
     switch (a->n_pad) {
-        case 16: kernel = k_tc_linear<16, DET>; break;
-        case 32: kernel = k_tc_linear<32, DET>; break;
-        case 48: kernel = k_tc_linear<48, DET>; break;
-        case 64: kernel = k_tc_linear<64, DET>; break;
-        case 80: kernel = k_tc_linear<80, DET>; break;
-        case 96: kernel = k_tc_linear<96, DET>; break;
-        case 112: kernel = k_tc_linear<112, DET>; break;
-        default: kernel = k_tc_linear<128, DET>; break;
+        case 16: kernel = k_tc_linear<16, DET, BF16>; break;
+        case 32: kernel = k_tc_linear<32, DET, BF16>; break;
+        case 48: kernel = k_tc_linear<48, DET, BF16>; break;
+        case 64: kernel = k_tc_linear<64, DET, BF16>; break;
+        case 80: kernel = k_tc_linear<80, DET, BF16>; break;
+        case 96: kernel = k_tc_linear<96, DET, BF16>; break;
+        case 112: kernel = k_tc_linear<112, DET, BF16>; break;
+        default: kernel = k_tc_linear<128, DET, BF16>; break;
     }
     if ((rc = opt_in_smem(kernel, smem))) return rc;
     const long long n_tiles = (M + kTcM - 1) / kTcM;
@@ -646,7 +693,9 @@ static int tc_linear_fwd(const pvraft_tc_linear_args* a, void* ws, void* stream)
 }
 
 extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* det_workspace, void* stream) {
-    return det_workspace ? tc_linear_fwd<true>(a, det_workspace, stream) : tc_linear_fwd<false>(a, nullptr, stream);
+    if (a && a->w_bf16)
+        return det_workspace ? tc_linear_fwd<true, true>(a, det_workspace, stream) : tc_linear_fwd<false, true>(a, nullptr, stream);
+    return det_workspace ? tc_linear_fwd<true, false>(a, det_workspace, stream) : tc_linear_fwd<false, false>(a, nullptr, stream);
 }
 
 extern "C" int64_t pvraft_tc_linear_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }

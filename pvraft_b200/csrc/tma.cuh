@@ -11,6 +11,8 @@ namespace pvraft {
 // [rows, cols] fp32 row-major (row stride ld floats) -> `map`: boxes of box_rows x 32 columns (one 128-byte swizzle row),
 // SWIZZLE_128B.  Error messages start with `op` (definition in capi.cu).
 int make_tensor_map(CUtensorMap* map, const float* base, long long rows, int cols, long long ld, int box_rows, const char* op);
+// the same for a bf16 tensor (row stride ld elements): boxes of box_rows x 32 columns (one 64-byte swizzle row), SWIZZLE_64B
+int make_tensor_map_bf16(CUtensorMap* map, const uint16_t* base, long long rows, int cols, long long ld, int box_rows, const char* op);
 
 // ---- device ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }

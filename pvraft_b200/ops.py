@@ -83,6 +83,25 @@ class stats_arena:
         return False
 
 
+class bf16_compute:
+    """Scope in which tc_weights returns the bf16 operand form of a layer's weights by default, so that every tensor-core
+    layer (tc_linear, update_chain) launched inside it runs on bf16 operands with fp32 accumulation.  The RAFT loop enters it
+    in the 'bf16-compute' precision mode (RSF.set_precision); the encoders and the refiner run outside it.  Per thread, like
+    stats_arena."""
+
+    def __init__(self, enabled=True):
+        self.enabled = bool(enabled)
+
+    def __enter__(self):
+        self.prev = getattr(_TLS, 'bf16', False)
+        _TLS.bf16 = self.enabled
+        return self
+
+    def __exit__(self, *exc):
+        _TLS.bf16 = self.prev
+        return False
+
+
 def new_stats(b, device, n=1):
     """Zeroed GroupNorm accumulators: n x [B,8,2] doubles (one cudaMemset for all of them)."""
     arena = getattr(_TLS, 'arena', None)
@@ -326,15 +345,18 @@ _TC_WEIGHTS = {}
 TC_PLAIN, TC_GRU_ZR, TC_GRU_Q, TC_FLOW = 0, 1, 2, 3
 
 
-def tc_weights(weights, col0=0, cols=None, k_pad=None, kcat=False, transposed=None):
-    """tf32 hi/lo split of a (stack of) [cout, cin(,1,1)] weight(s) -> (hi, lo) [n_pad, k_pad], cached per parameter
-    version (inference weights are static, so this runs once; the training path re-splits after every optimizer step).
-    transposed=(r0, r1): the split of W^T[r0:r1, :] instead -- the operand of dx = dy . W for input columns r0..r1."""
+def tc_weights(weights, col0=0, cols=None, k_pad=None, kcat=False, transposed=None, bf16=None):
+    """tf32 hi/lo split of a (stack of) [cout, cin(,1,1)] weight(s) -> (hi, lo, n_pad, rows), hi and lo [n_pad, k_pad],
+    cached per parameter version (inference weights are static, so this runs once; the training path re-splits after every
+    optimizer step).  transposed=(r0, r1): the split of W^T[r0:r1, :] instead -- the operand of dx = dy . W for input
+    columns r0..r1.  bf16=True (default: inside a `bf16_compute` scope): the bf16 form (w, None, n_pad, rows) instead, w
+    [n_pad, k_pad] torch.bfloat16 rounded to nearest even, cached separately."""
     if torch.is_tensor(weights):
         weights = (weights,)
+    bf16 = bool(getattr(_TLS, 'bf16', False)) if bf16 is None else bool(bf16)
     # keyed by the identity of the source tensor OBJECTS (validated through weak references and version counters):
     # a data_ptr key would go stale when the allocator hands a freed weight's address to a new tensor
-    key = tuple(id(w) for w in weights) + (col0, cols, k_pad, kcat, transposed)
+    key = tuple(id(w) for w in weights) + (col0, cols, k_pad, kcat, transposed, bf16)
     hit = _TC_WEIGHTS.get(key)
     if hit is not None:
         refs, versions, ptrs, result = hit
@@ -353,12 +375,19 @@ def tc_weights(weights, col0=0, cols=None, k_pad=None, kcat=False, transposed=No
     n_pad = (rows + 15) // 16 * 16
     # (the split kernel writes every entry of the rows it is given, padding columns included: zero-fill only for padding rows)
     alloc = torch.empty if n_pad == rows else torch.zeros
-    hi = alloc(n_pad, kp, dtype=torch.float32, device=mats[0].device)
-    lo = alloc(n_pad, kp, dtype=torch.float32, device=mats[0].device)
+    if bf16:
+        hi, lo = alloc(n_pad, kp, dtype=torch.bfloat16, device=mats[0].device), None
+    else:
+        hi = alloc(n_pad, kp, dtype=torch.float32, device=mats[0].device)
+        lo = alloc(n_pad, kp, dtype=torch.float32, device=mats[0].device)
     r0 = 0
     for m in mats:
-        check(lib().pvraft_tc_weight_split(_p(m.contiguous()), m.shape[0], ncols, ld, col0, m.shape[0], kp,
-                                           hi[r0:].data_ptr(), lo[r0:].data_ptr(), _stream()), 'tc_weight_split')
+        if bf16:
+            check(lib().pvraft_tc_weight_bf16(_p(m.contiguous()), m.shape[0], ncols, ld, col0, m.shape[0], kp, hi[r0:].data_ptr(),
+                                              _stream()), 'tc_weight_bf16')
+        else:
+            check(lib().pvraft_tc_weight_split(_p(m.contiguous()), m.shape[0], ncols, ld, col0, m.shape[0], kp,
+                                               hi[r0:].data_ptr(), lo[r0:].data_ptr(), _stream()), 'tc_weight_split')
         r0 += m.shape[0]
     if len(_TC_WEIGHTS) > 512:
         _TC_WEIGHTS.clear()
@@ -428,8 +457,8 @@ def tc_linear(sources, w, bias=None, *, in_min=None, in_stats=None, in_gamma=Non
               bias2=None, out2=None, h=None, z=None, cout=None, tail=None, w3=None, b3=None, coords1=None, coords2=None,
               coords2_out=None, flow_out=None):
     """Fused layer on the Hopper tensor cores (wgmma).  sources: list of [B,N,C_i] tensors concatenated along K (the
-    GroupNorm prologue applies to sources[0]); w = (hi, lo, n_pad, rows) from tc_weights(); tail [B,N,3] fills the
-    output columns cout..cout+2."""
+    GroupNorm prologue applies to sources[0]); w = (hi, lo, n_pad, rows) from tc_weights() -- its bf16 form runs the layer on
+    bf16 operands; tail [B,N,3] fills the output columns cout..cout+2."""
     hi, lo, n_pad, rows = w
     b, n, _ = sources[0].shape
     cout = rows if cout is None else cout
@@ -441,7 +470,11 @@ def tc_linear(sources, w, bias=None, *, in_min=None, in_stats=None, in_gamma=Non
         a.in_channels[i] = src.shape[-1]
     a.in_min, a.in_stats, a.in_gamma, a.in_beta = _p(in_min), _p(in_stats, torch.float64), _p(in_gamma), _p(in_beta)
     a.in_count, a.in_act, a.in_slope = float(in_count), in_act, float(in_slope)
-    a.w_hi, a.w_lo, a.n_pad, a.cout = _p(hi), _p(lo), n_pad, cout
+    if lo is None:
+        a.w_bf16 = _p(hi, torch.bfloat16)
+    else:
+        a.w_hi, a.w_lo = _p(hi), _p(lo)
+    a.n_pad, a.cout = n_pad, cout
     a.bias, a.bias2, a.out_act, a.residual = _p(bias), _p(bias2), out_act, _p(residual)
     a.out, a.out2, a.h, a.z = _p(out), _p(out2), _p(h), _p(z)
     a.out_stats, a.epilogue, a.B, a.N = _p(out_stats, torch.float64), epilogue, b, n
@@ -466,7 +499,8 @@ def update_chain(y1, gn, kfeat, cflow, flow, net, inp, weights, biases):
     """MotionEncoder + ConvGRU + flow-head fc1 pre-transform of one RAFT iteration in one launch (include/pvraft_b200.h,
     pvraft_update_chain_fwd): the same bits as the five tc_linear launches it replaces.  gn: y1's prologue (in_stats,
     in_gamma, in_beta, in_count, in_slope as for tc_linear); weights: five tc_weights() results in the order cc, motion,
-    [z|r], q, fc1; biases: (b_cc, b_m, b_z, b_r, b_q).  Returns (net' [B,N,64], P [B,N,64])."""
+    [z|r], q, fc1, all five in the 3xTF32 or all five in the bf16 form; biases: (b_cc, b_m, b_z, b_r, b_q).
+    Returns (net' [B,N,64], P [B,N,64])."""
     b, n, _ = net.shape
     net_out, p_out = torch.empty_like(net), torch.empty_like(net)
     a = _lib.UpdateChainArgs()
@@ -474,7 +508,10 @@ def update_chain(y1, gn, kfeat, cflow, flow, net, inp, weights, biases):
     a.gn_gamma, a.gn_beta, a.gn_count, a.gn_slope = _p(gn['in_gamma']), _p(gn['in_beta']), float(gn['in_count']), float(gn['in_slope'])
     a.kfeat, a.cflow, a.flow, a.net, a.inp = _p(kfeat), _p(cflow), _p(flow), _p(net), _p(inp)
     for i, (hi, lo, _, _) in enumerate(weights):
-        a.w_hi[i], a.w_lo[i] = _p(hi), _p(lo)
+        if lo is None:
+            a.w_bf16[i] = _p(hi, torch.bfloat16)
+        else:
+            a.w_hi[i], a.w_lo[i] = _p(hi), _p(lo)
     a.b_cc, a.b_m, a.b_z, a.b_r, a.b_q = (_p(x) for x in biases)
     a.net_out, a.p_out = _p(net_out), _p(p_out)
     a.B, a.N, a.hidden, a.context, a.y1_channels = b, n, net.shape[-1], inp.shape[-1], y1.shape[-1]

@@ -49,6 +49,7 @@ class _RaftBase(nn.Module):
     # graph is only valid for the parameter values it was captured with: every entry records (version, data_ptr) of all
     # parameters and is re-captured when any of them changed (optimizer step, load_state_dict, .to()).
     use_cuda_graph = {'1': True, '0': False}.get(os.environ.get('PVRAFT_CUDA_GRAPH', ''), None)
+    bf16_compute = False   # set_precision('bf16-compute'): the RAFT loop's tensor-core layers on bf16 operands
 
     def reset_graphs(self):
         self.__dict__.pop('_graphs', None)
@@ -57,10 +58,17 @@ class _RaftBase(nn.Module):
     def set_precision(self, mode):
         """'fp32' (default): the reference's arithmetic.  'bf16': the reduced-precision STATE mode of BASELINE.json configs[2] --
         the truncated correlation is kept as bf16 values + uint16 candidate ids (4 B instead of 8 B per candidate and iteration,
-        the lookup kernel's whole HBM stream); coordinates, index math and every layer stay fp32.  Inference only."""
-        if mode not in ('fp32', 'bf16'):
-            raise ValueError("precision must be 'fp32' or 'bf16'")
-        self.corr_block.state_dtype = torch.bfloat16 if mode == 'bf16' else torch.float32
+        the lookup kernel's whole HBM stream); coordinates, index math and every layer stay fp32.  'bf16-compute': the bf16
+        state, and every tensor-core layer of the RAFT loop (out_conv[0], the update chain or its five layers, the flow
+        head's SetConv fc2 / fc3 and its FLOW layer) on bf16 operands -- activations after the prologue and weights rounded to
+        nearest even -- with fp32 accumulation; prologues, epilogues, GroupNorm statistics, coordinates and every tensor in
+        memory stay fp32.  The encoders, the correlation build and the refiner stay fp32, so everything before the loop is
+        bitwise that of 'bf16'; at N % 128 != 0 the loop runs on the CUDA-core kernels and the mode equals 'bf16'.  Both bf16
+        modes are inference only (RSF_refine trains its fp32 refiner behind the no-grad loop)."""
+        if mode not in ('fp32', 'bf16', 'bf16-compute'):
+            raise ValueError("precision must be 'fp32', 'bf16' or 'bf16-compute'")
+        self.corr_block.state_dtype = torch.float32 if mode == 'fp32' else torch.bfloat16
+        self.bf16_compute = mode == 'bf16-compute'   # (in __dict__: nn.DataParallel replicas inherit it)
         self.reset_graphs()
         return self
 
@@ -164,8 +172,9 @@ class _RaftBase(nn.Module):
         use_tc = ops.tc_supported(n)
         # (hoisting the constant context part of the GRU pre-activations out of the loop -- K = 128 per iteration instead of 192 --
         #  was measured slower in round 1, 22.15 vs 21.72 ms per forward: the two extra per-point reads outweigh the shorter GEMM)
-        # per iteration: the lookup moments, the lookup-feature GroupNorm sums and the three SetConv sums; one memset
-        with ops.stats_arena(b, xyz1.device, 5 * num_iters):
+        # per iteration: the lookup moments, the lookup-feature GroupNorm sums and the three SetConv sums; one memset.
+        # 'bf16-compute': the loop's tensor-core layers take the bf16 form of their weights (ops.bf16_compute)
+        with ops.stats_arena(b, xyz1.device, 5 * num_iters), ops.bf16_compute(self.bf16_compute):
             return self._iterate_body(xyz1, graph_context, net, inp, num_iters, keep_all, coords2, flow, preds, me, use_tc)
 
     def _iterate_body(self, xyz1, graph_context, net, inp, num_iters, keep_all, coords2, flow, preds, me, use_tc):
