@@ -500,6 +500,14 @@ PVRAFT_API int pvraft_point_order_fwd(const float* xyz, int B, int N, int32_t* p
 PVRAFT_API int pvraft_linear_wgrad(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
                                    void* det_workspace, void* stream);
 PVRAFT_API int64_t pvraft_linear_wgrad_det_workspace_bytes(int cin, int cout);
+/* The same gradients on the tensor cores with bf16 operands (the 'bf16-mixed' training mode): the autograd of nn.Conv1d(k=1)
+ * in model/update.py and model/flot/gconv.py, for the per-point layers of the RAFT loop.
+ *   x [rows,cin], dy [rows,cout]  ->  dW[o,i] += sum_r bf16(dy[r,o]) bf16(x[r,i])  (round to nearest even, fp32 accumulation;
+ *   row stride dw_ld floats, 0 = cin),  db[o] += sum_r dy[r,o]  (fp32, from the unrounded dy; or NULL).
+ * rows >= 1; cin in {32,64,...,192} and cout in {32,64,96,128} (PVRAFT_ERR_UNSUPPORTED otherwise). */
+PVRAFT_API int pvraft_tc_wgrad_bf16(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
+                                    void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_tc_wgrad_bf16_det_workspace_bytes(int cin, int cout);
 
 /* GroupNorm(8) + activation backward (model/corr.py:17-18,25-26; model/flot/gconv.py:27-36 via autograd in the reference):
  *   x, dy [B,rows,C]; stats [B,8,2] raw sums of x (as produced in the forward); count = rows * C/8; act/slope as pvraft_gn_act_fwd

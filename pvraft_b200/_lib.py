@@ -111,6 +111,8 @@ _SIGNATURES = {
     'pvraft_knn_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
     'pvraft_linear_wgrad': (C.c_int, [VP, VP, C.c_int64, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP]),
     'pvraft_linear_wgrad_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
+    'pvraft_tc_wgrad_bf16': (C.c_int, [VP, VP, C.c_int64, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP]),
+    'pvraft_tc_wgrad_bf16_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
     'pvraft_gn_act_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int64, C.c_int, VP, VP, VP, VP,
                                     VP, VP, VP, VP, VP]),
     'pvraft_gn_act_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),

@@ -102,6 +102,11 @@ class bf16_compute:
         return False
 
 
+def bf16_compute_active():
+    """True inside an enabled `bf16_compute` scope on this thread."""
+    return bool(getattr(_TLS, 'bf16', False))
+
+
 def new_stats(b, device, n=1):
     """Zeroed GroupNorm accumulators: n x [B,8,2] doubles (one cudaMemset for all of them)."""
     arena = getattr(_TLS, 'arena', None)
@@ -353,7 +358,7 @@ def tc_weights(weights, col0=0, cols=None, k_pad=None, kcat=False, transposed=No
     [n_pad, k_pad] torch.bfloat16 rounded to nearest even, cached separately."""
     if torch.is_tensor(weights):
         weights = (weights,)
-    bf16 = bool(getattr(_TLS, 'bf16', False)) if bf16 is None else bool(bf16)
+    bf16 = bf16_compute_active() if bf16 is None else bool(bf16)
     # keyed by the identity of the source tensor OBJECTS (validated through weak references and version counters):
     # a data_ptr key would go stale when the allocator hands a freed weight's address to a new tensor
     key = tuple(id(w) for w in weights) + (col0, cols, k_pad, kcat, transposed, bf16)
@@ -585,6 +590,16 @@ def linear_wgrad(x, dy, dw, db=None):
     ws = _det_workspace(lib().pvraft_linear_wgrad_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
     _count(lib().pvraft_linear_wgrad(_p(x), _p(dy), rows, x.shape[-1], dy.shape[-1], _p(dw), dw.shape[-1], _p(db), _p(ws, torch.uint8),
                                      _stream()), 'linear_wgrad')
+
+
+def tc_wgrad_bf16(x, dy, dw, db=None):
+    """linear_wgrad on the tensor cores with bf16 operands (round to nearest even, fp32 accumulation): dw [cout,cin] +=
+    bf16(dy)^T bf16(x), db [cout] += column sums of the unrounded dy; x [B,R,cin], dy [B,R,cout], cin in {32..192} and
+    cout in {32..128} multiples of 32."""
+    rows = x.shape[0] * x.shape[1]
+    ws = _det_workspace(lib().pvraft_tc_wgrad_bf16_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
+    _count(lib().pvraft_tc_wgrad_bf16(_p(x), _p(dy), rows, x.shape[-1], dy.shape[-1], _p(dw), dw.shape[-1], _p(db), _p(ws, torch.uint8),
+                                      _stream()), 'tc_wgrad_bf16')
 
 
 def linear_bwd_small(x, dy, w, dw, db=None, want_dx=False):

@@ -49,7 +49,7 @@ class _RaftBase(nn.Module):
     # graph is only valid for the parameter values it was captured with: every entry records (version, data_ptr) of all
     # parameters and is re-captured when any of them changed (optimizer step, load_state_dict, .to()).
     use_cuda_graph = {'1': True, '0': False}.get(os.environ.get('PVRAFT_CUDA_GRAPH', ''), None)
-    bf16_compute = False   # set_precision('bf16-compute'): the RAFT loop's tensor-core layers on bf16 operands
+    bf16_compute = False   # set_precision('bf16-compute' / 'bf16-mixed'): the RAFT loop's tensor-core layers on bf16 operands
 
     def reset_graphs(self):
         self.__dict__.pop('_graphs', None)
@@ -64,11 +64,18 @@ class _RaftBase(nn.Module):
         nearest even -- with fp32 accumulation; prologues, epilogues, GroupNorm statistics, coordinates and every tensor in
         memory stay fp32.  The encoders, the correlation build and the refiner stay fp32, so everything before the loop is
         bitwise that of 'bf16'; at N % 128 != 0 the loop runs on the CUDA-core kernels and the mode equals 'bf16'.  Both bf16
-        modes are inference only (RSF_refine trains its fp32 refiner behind the no-grad loop)."""
-        if mode not in ('fp32', 'bf16', 'bf16-compute'):
-            raise ValueError("precision must be 'fp32', 'bf16' or 'bf16-compute'")
-        self.corr_block.state_dtype = torch.float32 if mode == 'fp32' else torch.bfloat16
-        self.bf16_compute = mode == 'bf16-compute'   # (in __dict__: nn.DataParallel replicas inherit it)
+        modes are inference only (RSF_refine trains its fp32 refiner behind the no-grad loop).
+        'bf16-mixed': mixed-precision training.  The correlation state stays fp32 and the loop's tensor-core layers run on
+        bf16 operands with fp32 accumulation, in inference as in 'bf16-compute' and in a training step too: there every
+        per-point layer of the loop whose shape suits the tensor cores (train.bf16_layer_plan) takes bf16 wgmma for its
+        output, its input gradient and its weight gradient.  The weights stay fp32 (the optimizer's master copy); the
+        encoders, the correlation build and lookup, GroupNorm, the edge-level layers, the loss and the refiner keep their
+        fp32 forms, so everything before the loop is bitwise 'fp32'.  Input gradients work; at N % 128 != 0 nothing runs on
+        the tensor cores and the mode equals 'fp32'."""
+        if mode not in ('fp32', 'bf16', 'bf16-compute', 'bf16-mixed'):
+            raise ValueError("precision must be 'fp32', 'bf16', 'bf16-compute' or 'bf16-mixed'")
+        self.corr_block.state_dtype = torch.float32 if mode in ('fp32', 'bf16-mixed') else torch.bfloat16
+        self.bf16_compute = mode in ('bf16-compute', 'bf16-mixed')   # (in __dict__: nn.DataParallel replicas inherit it)
         self.reset_graphs()
         return self
 

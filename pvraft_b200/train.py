@@ -6,6 +6,7 @@ The forward runs layer by layer -- the fused inference kernels keep no activatio
 `torch.autograd.Function` whose forward AND backward are kernels of libpvraft_b200.so:
 
     LinearFn        1x1 convolution           pvraft_linear_fwd (y, and dx = dy.W through the transposed weight) + pvraft_linear_wgrad
+                                              ('bf16-mixed' loop layers: pvraft_tc_linear_fwd on bf16 + pvraft_tc_wgrad_bf16)
     GnActFn         GroupNorm(8) + act        pvraft_gn_act_fwd / pvraft_gn_act_bwd
     GnActMaxFn      ... + max over 32 rows    pvraft_gn_act_maxk_fwd / pvraft_gn_act_bwd (arg form: no dense max gradient)
     EdgeFn          SetConv edge stage        pvraft_edge_fwd / pvraft_edge_bwd          (model/flot/gconv.py:65-73)
@@ -45,6 +46,16 @@ def _tc_train():
     return _TC_TRAIN == '1' or (_TC_TRAIN == 'auto' and torch.cuda.is_current_stream_capturing())
 
 
+def bf16_layer_plan(n_points, cin, cout, want_stats=False):
+    """Kernels of a per-point layer [B, n_points, cin] -> cout: (forward, dx, dW), each True where its shape suits the
+    tensor-core kernel -- bf16 wgmma inside the RAFT loop of a 'bf16-mixed' training step, 3xTF32 for forward and dx in a
+    captured fp32 step (no dW kernel there) -- and False where it keeps its fp32 CUDA-core kernel.  The forward follows
+    the shape rule of the tensor-core path (N % 128 == 0, cin % 32 == 0, cout <= 128; GroupNorm sums need cout % 32 == 0);
+    dx also needs cout % 32 == 0 (the transposed weight's K), dW cout % 32 == 0 and cin <= 192 (pvraft_tc_wgrad_bf16)."""
+    fwd = ops.tc_supported(n_points, cin) and cout <= 128 and (not want_stats or cout % 32 == 0)
+    return fwd, fwd and cout % 32 == 0, fwd and cout % 32 == 0 and cin <= 192
+
+
 class LinearFn(torch.autograd.Function):
     """y[B,R,cout] = x[B,R,cin] . W^T (+ b); optionally also the GroupNorm sums [B,8,2] of y (not differentiable: the
     consumer GnActFn differentiates through the statistics itself)."""
@@ -56,11 +67,16 @@ class LinearFn(torch.autograd.Function):
         stats = _zeros64(x.shape[0], 8, 2, device=x.device) if want_stats else None
         cout, cin = w2.shape
         # per-point layers whose shapes fit go to the wgmma kernel (3xTF32: fp32-accurate), forward and dx; the weight is
-        # split once per parameter version, i.e. once per optimizer step however many iterations use the layer
-        ctx.tc = _tc_train() and x.dim() == 3 and ops.tc_supported(x.shape[1], cin) and cout <= 128 and (not want_stats or cout % 32 == 0)
+        # split once per parameter version, i.e. once per optimizer step however many iterations use the layer.
+        # Inside the RAFT loop of 'bf16-mixed' (an ops.bf16_compute scope) they go there in eager steps too, on bf16
+        # operands, and so does their weight gradient.  The backward runs on autograd's device thread, which does not see
+        # the scope: the format is recorded here.
+        fwd_tc, ctx.dx_tc, ctx.dw_tc = bf16_layer_plan(x.shape[1], cin, cout, want_stats) if x.dim() == 3 else (False,) * 3
+        ctx.bf16 = fwd_tc and ops.bf16_compute_active()
+        ctx.tc = ctx.bf16 or (_tc_train() and fwd_tc)
         ctx.w_ref = w
         if ctx.tc:
-            y = ops.tc_linear([x], ops.tc_weights(w), None if b is None else b.detach(), out_stats=stats)
+            y = ops.tc_linear([x], ops.tc_weights(w, bf16=ctx.bf16), None if b is None else b.detach(), out_stats=stats)
         else:
             y = ops.linear(x, w2, b, out_stats=stats)
         ctx.save_for_backward(x, w2)
@@ -84,8 +100,9 @@ class LinearFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             # dx = dy . W: the same kernel with the transposed weight, 128 output columns (the kernel's limit) at a time
             cout, cin = w2.shape
-            if ctx.tc and cout % 32 == 0:
-                parts = [ops.tc_linear([dy], ops.tc_weights(ctx.w_ref, transposed=(c0, min(c0 + 128, cin)))) for c0 in range(0, cin, 128)]
+            if ctx.tc and ctx.dx_tc:
+                parts = [ops.tc_linear([dy], ops.tc_weights(ctx.w_ref, transposed=(c0, min(c0 + 128, cin)), bf16=ctx.bf16))
+                         for c0 in range(0, cin, 128)]
             else:
                 parts = [ops.linear(dy, w2[:, c0:min(c0 + 128, cin)].t().contiguous()) for c0 in range(0, cin, 128)]
             dx = parts[0] if len(parts) == 1 else torch.cat(parts, -1)
@@ -93,7 +110,10 @@ class LinearFn(torch.autograd.Function):
         if ctx.needs_input_grad[1] or (ctx.has_bias and ctx.needs_input_grad[2]):
             dw = torch.zeros_like(w2)
             db = torch.zeros(w2.shape[0], dtype=torch.float32, device=w2.device) if ctx.has_bias else None
-            ops.linear_wgrad(x, dy, dw, db)
+            if ctx.bf16 and ctx.dw_tc:
+                ops.tc_wgrad_bf16(x, dy, dw, db)
+            else:
+                ops.linear_wgrad(x, dy, dw, db)
             dw = dw.reshape(ctx.w_shape)
         return dx, dw, db, None
 
@@ -337,12 +357,14 @@ def rsf_forward(model, p, num_iters):
     inp = torch.relu(fct1[..., model.hidden_dim:])
     coords2 = xyz1.clone()
     preds = []
-    for _ in range(num_iters):
-        coords2 = coords2.detach()                                             # :41
-        vox, sel = CorrLookupFn.apply(corr_val, corr_idx, xyz2p, coords2, cb.num_levels, cb.base_scale, xyz2)
-        corr = corr_features(cb, vox, sel)                                     # :42
-        flow = coords2 - xyz1                                                  # :43
-        net, delta = update_block(model.update_block, net, inp, corr, flow, graph1)   # :44
-        coords2 = coords2 + delta                                              # :45
-        preds.append(coords2 - xyz1)                                           # :46
+    # 'bf16-mixed': the loop's per-point layers on bf16 wgmma (LinearFn, bf16_layer_plan); the lookup stays fp32
+    with ops.bf16_compute(model.bf16_compute):
+        for _ in range(num_iters):
+            coords2 = coords2.detach()                                         # :41
+            vox, sel = CorrLookupFn.apply(corr_val, corr_idx, xyz2p, coords2, cb.num_levels, cb.base_scale, xyz2)
+            corr = corr_features(cb, vox, sel)                                 # :42
+            flow = coords2 - xyz1                                              # :43
+            net, delta = update_block(model.update_block, net, inp, corr, flow, graph1)   # :44
+            coords2 = coords2 + delta                                          # :45
+            preds.append(coords2 - xyz1)                                       # :46
     return preds
