@@ -581,6 +581,36 @@ PVRAFT_API int64_t pvraft_flow_metrics_det_workspace_bytes(void);
 PVRAFT_API int pvraft_flow_l1_bwd(const float* est, const float* gt, const float* mask, int64_t points, const double* acc, const float* g,
                        float weight, float* d_est, void* stream);
 
+/* Self-supervised losses (no counterpart in the reference, which trains on ground truth only): the Chamfer distance between
+ * the first cloud moved by the flow and the second cloud, and the smoothness of the flow over the first cloud's kNN graph.
+ * S = n*B samples (n predictions of a batch of B, stacked); sample s pairs with batch entry s % B, so the second cloud and the
+ * graph are never copied per prediction.  ||v||^2 is (vx*vx + vy*vy) + vz*vz of the fp32 difference vector, rounded to
+ * nearest at every step, never contracted.  Null pointers, S < 1, B < 1, S % B != 0, N < 1, M < 1 and k outside 1..32 return
+ * PVRAFT_ERR_BAD_ARG before any launch.
+ *   pvraft_chamfer_fwd: a [S,N,3] (W = P1 + flow), b [B,M,3] (P2)
+ *       -> nn_ab [S,N] int32: argmin_j ||a[s,i] - b[s%B,j]||^2;  nn_ba [S,M] int32: argmin_i ||a[s,i] - b[s%B,j]||^2
+ *          (exact ties: the lowest index), and acc [S,2] double, ZEROED by the caller, accumulates the sums of the minima
+ *          (acc[s,0] over i, acc[s,1] over j): C_s = acc[s,0] / N + acc[s,1] / M.  A brute-force search: 2 S N M pairs.
+ *   pvraft_chamfer_bwd: g [S] the DEVICE upstream gradient of C_s
+ *       -> d_a [S,N,3] += 2 g_s/N (a_i - b_nn(i)) and, for every j, d_a[nn_ba(j)] += 2 g_s/M (a_nn(j) - b_j);  d_b [B,M,3] the
+ *          negated terms at the other end of each pair (or NULL).  Both ACCUMULATED, zeroed by the caller.
+ *   pvraft_flow_smooth_fwd: f [S,N,3], nbr [B,N,k] int32 local ids (sample s uses nbr[s % B])
+ *       -> acc [S] double (ZEROED by the caller) += sum_i sum_e ||f[s,nbr[i,e]] - f[s,i]||:  S_s = acc[s] / (N k).
+ *   pvraft_flow_smooth_bwd: g [S] DEVICE -> d_f [S,N,3] (ACCUMULATED, zeroed by the caller): for every edge (i, j = nbr[i,e]),
+ *       u = g_s/(N k) (f_j - f_i)/||f_j - f_i|| (0 where f_j = f_i), d_f[j] += u, d_f[i] -= u. */
+PVRAFT_API int pvraft_chamfer_fwd(const float* a, const float* b, int S, int B, int N, int M, int32_t* nn_ab, int32_t* nn_ba, double* acc,
+                                  void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_chamfer_fwd_det_workspace_bytes(int S);
+PVRAFT_API int pvraft_chamfer_bwd(const float* a, const float* b, const int32_t* nn_ab, const int32_t* nn_ba, const float* g, int S, int B,
+                                  int N, int M, float* d_a, float* d_b, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_chamfer_bwd_det_workspace_bytes(int S, int B, int N, int M);
+PVRAFT_API int pvraft_flow_smooth_fwd(const float* f, const int32_t* nbr, int S, int B, int N, int k, double* acc, void* det_workspace,
+                                      void* stream);
+PVRAFT_API int64_t pvraft_flow_smooth_fwd_det_workspace_bytes(int S);
+PVRAFT_API int pvraft_flow_smooth_bwd(const float* f, const int32_t* nbr, const float* g, int S, int B, int N, int k, float* d_f,
+                                      void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_flow_smooth_bwd_det_workspace_bytes(int S, int N);
+
 /* sizeof() of the argument structs as compiled into the library (0 = linear, 1 = corrfeat, 2 = gru, 3 = flowout,
  * 4 = tc_linear, 5 = knn_branch, 6 = update_chain; -1 otherwise): lets a foreign-language binding verify its struct layout
  * at load time. */

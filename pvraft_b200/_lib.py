@@ -134,6 +134,14 @@ _SIGNATURES = {
     'pvraft_flow_metrics_fwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, VP]),
     'pvraft_flow_metrics_det_workspace_bytes': (C.c_int64, []),
     'pvraft_flow_l1_bwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, C.c_float, VP, VP]),
+    'pvraft_chamfer_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP]),
+    'pvraft_chamfer_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_chamfer_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
+    'pvraft_chamfer_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    'pvraft_flow_smooth_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_flow_smooth_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_flow_smooth_bwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_flow_smooth_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
     'pvraft_sizeof': (C.c_int, [C.c_int]),
     'pvraft_transpose_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, VP]),
 }

@@ -708,6 +708,79 @@ def corr_init_bwd(g, idx, fmap1, fmap2):
     return d1, d2
 
 
+def _loss_batch(what, x, b_rows, m=None):
+    """The shape rules of the self-supervised loss kernels: x [S,N,3] with S a multiple of the batch size b_rows."""
+    if x.dim() != 3 or x.shape[-1] != 3 or x.shape[0] < 1 or x.shape[1] < 1:
+        raise ValueError(f'{what}: expected [S,N,3], got {tuple(x.shape)}')
+    if b_rows < 1 or x.shape[0] % b_rows:
+        raise ValueError(f'{what}: {x.shape[0]} samples are not a whole number of batches of {b_rows}')
+    if m is not None and m < 1:
+        raise ValueError(f'{what}: the second cloud is empty')
+
+
+def chamfer(a, b):
+    """a [S,N,3] (the first clouds moved by the flows), b [B,M,3] (the second clouds; sample s searches b[s % B]) ->
+    (acc [S,2] f64: the sums over a's points of their least squared distance to b, and over b's points of theirs to a;
+    nn_ab [S,N] int32, nn_ba [S,M] int32: the nearest points, lowest index on ties).  Both directions in one launch."""
+    if b.dim() != 3 or b.shape[-1] != 3:
+        raise ValueError(f'chamfer: expected b [B,M,3], got {tuple(b.shape)}')
+    s, n, _ = a.shape
+    bb, m = int(b.shape[0]), int(b.shape[1])
+    _loss_batch('chamfer', a, bb, m)
+    acc = torch.zeros(s, 2, dtype=torch.float64, device=a.device)
+    nn_ab = torch.empty(s, n, dtype=torch.int32, device=a.device)
+    nn_ba = torch.empty(s, m, dtype=torch.int32, device=a.device)
+    ws = _det_workspace(lib().pvraft_chamfer_fwd_det_workspace_bytes, s, device=a.device)
+    _count(lib().pvraft_chamfer_fwd(_p(a), _p(b), s, bb, n, m, _p(nn_ab, torch.int32), _p(nn_ba, torch.int32), _p(acc, torch.float64),
+                                    _p(ws, torch.uint8), _stream()), 'chamfer_fwd')
+    return acc, nn_ab, nn_ba
+
+
+def chamfer_bwd(a, b, nn_ab, nn_ba, g, want_db=True):
+    """Gradients of C_s = acc[s,0]/N + acc[s,1]/M (chamfer) with the indices held fixed, for the upstream gradient g [S]
+    (on the device) -> (d_a [S,N,3], d_b [B,M,3] or None)."""
+    s, n, _ = a.shape
+    bb, m = int(b.shape[0]), int(b.shape[1])
+    _loss_batch('chamfer_bwd', a, bb, m)
+    if g.shape != (s,):
+        raise ValueError(f'chamfer_bwd: expected g [{s}], got {tuple(g.shape)}')
+    d_a = torch.zeros_like(a)
+    d_b = torch.zeros_like(b) if want_db else None
+    ws = _det_workspace(lib().pvraft_chamfer_bwd_det_workspace_bytes, s, bb, n, m, device=a.device)
+    _count(lib().pvraft_chamfer_bwd(_p(a), _p(b), _p(nn_ab, torch.int32), _p(nn_ba, torch.int32), _p(g), s, bb, n, m, _p(d_a), _p(d_b),
+                                    _p(ws, torch.uint8), _stream()), 'chamfer_bwd')
+    return d_a, d_b
+
+
+def _smooth_args(what, f, nbr):
+    if nbr.dim() != 3 or nbr.shape[1] != f.shape[1] or not 1 <= nbr.shape[2] <= KNN:
+        raise ValueError(f'{what}: expected nbr [B,{f.shape[1]},k] with 1 <= k <= {KNN}, got {tuple(nbr.shape)}')
+    _loss_batch(what, f, int(nbr.shape[0]))
+    return f.shape[0], int(nbr.shape[0]), f.shape[1], int(nbr.shape[2])
+
+
+def flow_smooth(f, nbr):
+    """f [S,N,3], nbr [B,N,k] int32 (sample s uses nbr[s % B]) -> acc [S] f64: sum over the edges of ||f_j - f_i||."""
+    s, bb, n, k = _smooth_args('flow_smooth', f, nbr)
+    acc = torch.zeros(s, dtype=torch.float64, device=f.device)
+    ws = _det_workspace(lib().pvraft_flow_smooth_fwd_det_workspace_bytes, s, device=f.device)
+    _count(lib().pvraft_flow_smooth_fwd(_p(f), _p(nbr, torch.int32), s, bb, n, k, _p(acc, torch.float64), _p(ws, torch.uint8), _stream()),
+           'flow_smooth_fwd')
+    return acc
+
+
+def flow_smooth_bwd(f, nbr, g):
+    """Gradient of S_s = acc[s] / (N k) (flow_smooth) for the upstream gradient g [S] (on the device) -> d_f [S,N,3]."""
+    s, bb, n, k = _smooth_args('flow_smooth_bwd', f, nbr)
+    if g.shape != (s,):
+        raise ValueError(f'flow_smooth_bwd: expected g [{s}], got {tuple(g.shape)}')
+    d_f = torch.zeros_like(f)
+    ws = _det_workspace(lib().pvraft_flow_smooth_bwd_det_workspace_bytes, s, n, device=f.device)
+    _count(lib().pvraft_flow_smooth_bwd(_p(f), _p(nbr, torch.int32), _p(g), s, bb, n, k, _p(d_f), _p(ws, torch.uint8), _stream()),
+           'flow_smooth_bwd')
+    return d_f
+
+
 def device_info():
     sm, smem = C.c_int(0), C.c_int(0)
     check(lib().pvraft_device_info(C.byref(sm), C.byref(smem)), 'device_info')
