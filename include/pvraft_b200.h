@@ -611,6 +611,21 @@ PVRAFT_API int pvraft_flow_smooth_bwd(const float* f, const int32_t* nbr, const 
                                       void* det_workspace, void* stream);
 PVRAFT_API int64_t pvraft_flow_smooth_bwd_det_workspace_bytes(int S, int N);
 
+/* Flow propagation along a scan sequence (no counterpart in the reference, which estimates one pair at a time): carries a
+ * flow defined on one cloud onto the points of another, the warm start of the next pair under a constant-velocity
+ * assumption (pvraft_b200.stream.SceneFlowStream).
+ *   xyz_prev [B,M,3], flow_prev [B,M,3] (the flow on xyz_prev's points), xyz [B,N,3]
+ *   -> for every query q of xyz, the k nearest of the moved points W = xyz_prev + flow_prev (formed in the kernel, one fp32
+ *      add per coordinate), ranked by ||q - W_j||^2 = (dx*dx + dy*dy) + dz*dz of the fp32 difference vector, rounded to
+ *      nearest at every step, never contracted, on (distance, index): exact ties go to the lowest index.
+ *      flow_out [B,N,3]: sum_j w_j flow_prev[j] / sum_j w_j with w_j = 1 / (sqrt_rn(d_j) + 1e-8), summed in fp32 nearest first;
+ *      idx_out [B,N,k] int32 (or NULL): the neighbours, nearest first.
+ * A brute-force search of B N M pairs.  No det_workspace: no value is accumulated with atomics, and every sum runs in a fixed
+ * order inside one thread, so the result is bitwise reproducible as it is.  Null inputs or flow_out, B, M or N < 1, and k
+ * outside 1..min(8, M) return PVRAFT_ERR_BAD_ARG before any launch. */
+PVRAFT_API int pvraft_flow_propagate_fwd(const float* xyz_prev, const float* flow_prev, const float* xyz, int B, int M, int N, int k,
+                                         float* flow_out, int32_t* idx_out, void* stream);
+
 /* sizeof() of the argument structs as compiled into the library (0 = linear, 1 = corrfeat, 2 = gru, 3 = flowout,
  * 4 = tc_linear, 5 = knn_branch, 6 = update_chain; -1 otherwise): lets a foreign-language binding verify its struct layout
  * at load time. */

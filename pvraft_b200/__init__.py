@@ -7,7 +7,8 @@ from .graph import Graph
 from .pointconv import knn_point, square_distance
 from .raft import RSF, RSF_refine
 from .refine import FlotRefine
+from .stream import SceneFlowStream
 from .update import ConvGRU, ConvRNN, FlowHead, MotionEncoder, UpdateBlock
 
 __all__ = ['RSF', 'RSF_refine', 'CorrBlock', 'UpdateBlock', 'MotionEncoder', 'ConvGRU', 'ConvRNN', 'FlowHead',
-           'FlotEncoder', 'FlotRefine', 'SetConv', 'Graph', 'knn_point', 'square_distance']
+           'FlotEncoder', 'FlotRefine', 'SetConv', 'Graph', 'knn_point', 'square_distance', 'SceneFlowStream']

@@ -12,6 +12,7 @@
 // and argmin in registers while the other cloud streams through shared memory in double-buffered tiles; one launch searches
 // both directions (blockIdx.z) for every prediction of a sequence (blockIdx.y = sample s, which searches b[s % B]).
 #include "fixed_point.cuh"
+#include "nn_search.cuh"
 
 namespace pvraft {
 
@@ -20,12 +21,6 @@ constexpr int kNnQueries = 4;                          // queries per thread, he
 constexpr int kNnPerCta = kNnThreads * kNnQueries;
 constexpr int kNnTile = 256;                           // searched points per shared-memory tile (two tiles)
 constexpr int kNnStage = kNnTile / kNnThreads;         // points each thread stages per tile
-
-// the squared length of the fp32 difference q - p, with no FMA contraction
-__device__ __forceinline__ float diff_sq(float qx, float qy, float qz, const float4& p) {
-    const float dx = __fsub_rn(qx, p.x), dy = __fsub_rn(qy, p.y), dz = __fsub_rn(qz, p.z);
-    return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-}
 
 // a [S,N,3], b [B,M,3].  z = 0: every a-point of sample s queries b[s % B] -> nn_ab [S,N], acc[2s] += sum of the minima;
 // z = 1: every b-point queries a[s] -> nn_ba [S,M], acc[2s + 1].  DET: acc is the [2S] fixed-point workspace.  What a warp

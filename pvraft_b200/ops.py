@@ -781,6 +781,39 @@ def flow_smooth_bwd(f, nbr, g):
     return d_f
 
 
+PROPAGATE_MAX_K = 8   # neighbours pvraft_flow_propagate_fwd averages over at most
+
+
+def flow_propagate(xyz_prev, flow_prev, xyz, k=3, want_idx=False):
+    """Carry a flow defined on one cloud onto another under a constant-velocity assumption: flow_prev [B,M,3] on the points
+    xyz_prev [B,M,3] -> flow [B,N,3] on xyz [B,N,3], the inverse-distance-weighted mean flow of the k nearest moved points
+    xyz_prev + flow_prev of every point of xyz (include/pvraft_b200.h, pvraft_flow_propagate_fwd).  want_idx: also the
+    neighbours [B,N,k] int32, nearest first (exact distance ties: the lowest index).  Bitwise reproducible in any mode."""
+    for name, t in (('xyz_prev', xyz_prev), ('flow_prev', flow_prev), ('xyz', xyz)):
+        if not torch.is_tensor(t) or t.dim() != 3 or t.shape[-1] != 3 or t.shape[0] < 1 or t.shape[1] < 1:
+            raise ValueError(f'flow_propagate: expected {name} [B,n,3] with B, n >= 1, got '
+                             f'{tuple(t.shape) if torch.is_tensor(t) else type(t)}')
+        if t.dtype != torch.float32:
+            raise ValueError(f'flow_propagate: {name} must be float32, got {t.dtype}')
+    b, m = int(xyz_prev.shape[0]), int(xyz_prev.shape[1])
+    if flow_prev.shape != xyz_prev.shape:
+        raise ValueError(f'flow_propagate: flow_prev {tuple(flow_prev.shape)} must match xyz_prev {tuple(xyz_prev.shape)}')
+    if xyz.shape[0] != b:
+        raise ValueError(f'flow_propagate: xyz {tuple(xyz.shape)} and xyz_prev {tuple(xyz_prev.shape)} differ in batch size')
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(PROPAGATE_MAX_K, m):
+        raise ValueError(f'flow_propagate: k={k!r} must be an integer in 1..min({PROPAGATE_MAX_K}, M={m})')
+    for t in (xyz_prev, flow_prev, xyz):
+        if not t.is_cuda:
+            raise _lib.PvraftError('pvraft_b200 kernels need CUDA tensors (no CPU fallback exists)')
+    n = int(xyz.shape[1])
+    xyz_prev, flow_prev, xyz = xyz_prev.contiguous(), flow_prev.contiguous(), xyz.contiguous()
+    out = torch.empty(b, n, 3, dtype=torch.float32, device=xyz.device)
+    idx = torch.empty(b, n, k, dtype=torch.int32, device=xyz.device) if want_idx else None
+    _count(lib().pvraft_flow_propagate_fwd(_p(xyz_prev), _p(flow_prev), _p(xyz), b, m, n, k, _p(out), _p(idx, torch.int32), _stream()),
+           'flow_propagate_fwd')
+    return (out, idx) if want_idx else out
+
+
 def device_info():
     sm, smem = C.c_int(0), C.c_int(0)
     check(lib().pvraft_device_info(C.byref(sm), C.byref(smem)), 'device_info')

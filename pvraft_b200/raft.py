@@ -35,6 +35,22 @@ def _records_grad(module, p):
     return False
 
 
+def _check_flow_init(p, flow_init):
+    """flow_init of forward(): None, or a tensor [B,N1,3] -> its detached, contiguous fp32 form (a constant: RAFT's warm start
+    passes no gradient to it)."""
+    if flow_init is None:
+        return None
+    want = (int(p[0].shape[0]), int(p[0].shape[1]), 3) if p[0].dim() == 3 else None
+    if not torch.is_tensor(flow_init) or want is None or tuple(flow_init.shape) != want:
+        got = tuple(flow_init.shape) if torch.is_tensor(flow_init) else type(flow_init).__name__
+        raise ValueError(f'flow_init must be a tensor [B,N1,3] = {want} shaped like the first cloud, got {got}')
+    if not flow_init.is_floating_point():
+        raise ValueError(f'flow_init must be a floating-point tensor, got {flow_init.dtype}')
+    if not flow_init.is_cuda:
+        raise ops._lib.PvraftError('pvraft_b200 kernels need CUDA tensors (no CPU fallback exists): flow_init is on the CPU')
+    return flow_init.detach().contiguous().float()
+
+
 class _RaftBase(nn.Module):
     # CUDA-graph replay of the whole forward (encoders, correlation build, all iterations): the eager path costs ~28 us of
     # host time per launch (python + ctypes + tensor-map encodes), which bounds small batches (B <= 2: ~0.5 ms per
@@ -52,8 +68,8 @@ class _RaftBase(nn.Module):
     bf16_compute = False   # set_precision('bf16-compute' / 'bf16-mixed'): the RAFT loop's tensor-core layers on bf16 operands
 
     def reset_graphs(self):
-        self.__dict__.pop('_graphs', None)
-        self.__dict__.pop('_seen', None)
+        for name in ('_graphs', '_seen', '_stream_graphs', '_stream_seen'):   # (the last two: SceneFlowStream's)
+            self.__dict__.pop(name, None)
 
     def set_precision(self, mode):
         """'fp32' (default): the reference's arithmetic.  'bf16': the reduced-precision STATE mode of BASELINE.json configs[2] --
@@ -79,55 +95,68 @@ class _RaftBase(nn.Module):
         self.reset_graphs()
         return self
 
-    def _graph_key(self, xyz1, xyz2, num_iters):
+    def _graph_key(self, xyz1, xyz2, num_iters, warm=False):
         # a graph records the kernels of one setting of torch.use_deterministic_algorithms: never replayed under the other.
         # A pair of clouds of different sizes adds the second cloud's shape (pairs that share N1 and differ in N2 run on
-        # different buffers); a pair of equal sizes keeps the short key.
+        # different buffers); a pair of equal sizes keeps the short key.  A warm-started forward (flow_init) records only
+        # that it is one: the starting flow is a static input like the clouds, so new values replay the same graph.
         key = (tuple(xyz1.shape), xyz1.device, int(num_iters), ops.deterministic())
-        return key if xyz2.shape == xyz1.shape else key + (tuple(xyz2.shape),)
+        key = key if xyz2.shape == xyz1.shape else key + (tuple(xyz2.shape),)
+        return key + ('flow_init',) if warm else key
 
     def _stamp(self):
         return tuple((q._version, q.data_ptr()) for q in self.parameters())
 
-    def _graphed(self, p, num_iters):
+    def _graphed(self, p, num_iters, flow_init=None):
         xyz1, xyz2 = p[0].detach().contiguous().float(), p[1].detach().contiguous().float()
+        inputs = [xyz1, xyz2] if flow_init is None else [xyz1, xyz2, flow_init]
         graphs = self.__dict__.setdefault('_graphs', {})
-        key = self._graph_key(xyz1, xyz2, num_iters)
+        key = self._graph_key(xyz1, xyz2, num_iters, flow_init is not None)
         entry = graphs.get(key)
         stamp = self._stamp()
         if entry is not None and entry[3] != stamp:
             entry = None                                   # weights changed since the capture: stale derived constants
         if entry is None:
-            static_in = [torch.empty_like(xyz1), torch.empty_like(xyz2)]
-            static_in[0].copy_(xyz1)
-            static_in[1].copy_(xyz2)
+            static_in = [torch.empty_like(t) for t in inputs]
+            for s, t in zip(static_in, inputs):
+                s.copy_(t)
+
+            def run():
+                return self._forward_impl(static_in[:2], num_iters, static_in[2] if len(static_in) > 2 else None)
+
             side = torch.cuda.Stream(device=xyz1.device)   # warm-up off the capture stream: weight splits, derived constants
             side.wait_stream(torch.cuda.current_stream(xyz1.device))
             with torch.cuda.stream(side):
                 for _ in range(2):
-                    self._forward_impl(static_in, num_iters)
+                    run()
             torch.cuda.current_stream(xyz1.device).wait_stream(side)
             graph = torch.cuda.CUDAGraph()
             l0 = ops.launch_count
             with torch.cuda.graph(graph):
-                static_out = self._forward_impl(static_in, num_iters)
+                static_out = run()
             graphs.pop(key, None)
             while len(graphs) >= 8:                        # oldest capture out (its private memory pool goes with it)
                 graphs.pop(next(iter(graphs)))
             entry = graphs[key] = (graph, static_in, static_out, stamp, ops.launch_count - l0)
         graph, static_in, static_out, _, n_kernels = entry
-        static_in[0].copy_(xyz1)
-        static_in[1].copy_(xyz2)
+        for s, t in zip(static_in, inputs):
+            s.copy_(t)
         graph.replay()
         ops.launch_count += n_kernels            # the library's kernels inside the replayed graph
         return static_out.clone() if torch.is_tensor(static_out) else [t.clone() for t in static_out]
 
-    def forward(self, p, num_iters=12):
+    def forward(self, p, num_iters=12, flow_init=None):
+        """p = [xyz1 [B,N1,3], xyz2 [B,N2,3]] -> the reference's outputs.  flow_init [B,N1,3] (optional): RAFT's warm start,
+        the loop starts at coords2 = xyz1 + flow_init instead of xyz1.  It is a constant: detached, it receives no gradient.
+        None runs the reference's loop; a zero flow_init gives the same bits."""
+        flow_init = _check_flow_init(p, flow_init)
         if not p[0].is_cuda:
             raise ops._lib.PvraftError('pvraft_b200 kernels need CUDA tensors (no CPU fallback exists)')
         with torch.cuda.device(p[0].device):        # the library launches on the current device
+            if flow_init is not None and flow_init.device != p[0].device:
+                raise ops._lib.PvraftError(f'flow_init is on {flow_init.device}, the clouds on {p[0].device}')
             if _records_grad(self, p):
-                return self._forward_train(p, num_iters)
+                return self._forward_train(p, num_iters, flow_init)
             graph = self.use_cuda_graph
             if graph is None:    # automatic (never inside an nn.DataParallel replica thread)
                 if getattr(self, '_is_replica', False):
@@ -136,14 +165,14 @@ class _RaftBase(nn.Module):
                     graph = True     # host-bound from the first call
                 else:                # larger batches: once the same shape has come back with the same weights
                     seen = self.__dict__.setdefault('_seen', {})
-                    key, stamp = self._graph_key(p[0], p[1], num_iters), self._stamp()
+                    key, stamp = self._graph_key(p[0], p[1], num_iters, flow_init is not None), self._stamp()
                     graph = seen.get(key) == stamp
                     if len(seen) > 64:
                         seen.clear()
                     seen[key] = stamp
             if graph:
-                return self._graphed(p, num_iters)
-            return self._forward_impl(p, num_iters)
+                return self._graphed(p, num_iters, flow_init)
+            return self._forward_impl(p, num_iters, flow_init)
 
     def _encode(self, p):
         xyz1, xyz2 = p[0], p[1]
@@ -161,8 +190,18 @@ class _RaftBase(nn.Module):
                           None if graph2.order is None else graph2.order[:b])   # pc1's graph
         else:
             # clouds of different sizes: one encoder pass per cloud (the kernels take one N per launch)
-            fmap1, graph = self.feature_extractor(xyz1, point_major=True)   # pc1's graph
-            fmap2, _ = self.feature_extractor(xyz2, point_major=True)
+            fmap1, graph = self._encode_cloud(xyz1)                     # pc1's graph
+            fmap2, _ = self._encode_cloud(xyz2)
+        return self._pair(xyz1, xyz2, fmap1, graph, fmap2)
+
+    def _encode_cloud(self, xyz):
+        """The part of the pre-loop work that sees one cloud alone: its feature map [B,N,128] and its kNN graph (with the
+        Morton order).  Nothing in it depends on which side of a pair the cloud is on, so a scan sequence encodes every scan
+        once (SceneFlowStream)."""
+        return self.feature_extractor(xyz, point_major=True)
+
+    def _pair(self, xyz1, xyz2, fmap1, graph, fmap2):
+        """The pre-loop work that needs both clouds, from their feature maps and pc1's graph -> the loop's inputs."""
         self.corr_block.init_module_pm(fmap1, fmap2, xyz2)               # :29
         # the reference rebuilds the same pc1 graph for the context encoder (:31); reuse it
         fct1, graph_context = self.context_extractor(xyz1, graph=graph, point_major=True)
@@ -170,10 +209,14 @@ class _RaftBase(nn.Module):
         inp = torch.relu(fct1[..., self.hidden_dim:]).contiguous()
         return xyz1, xyz2, graph, graph_context, net, inp
 
-    def _iterate(self, xyz1, graph_context, net, inp, num_iters, keep_all):
+    def _iterate(self, xyz1, graph_context, net, inp, num_iters, keep_all, flow_init=None):
         b, n, _ = xyz1.shape
-        coords2 = xyz1.clone()
-        flow = torch.zeros_like(xyz1)
+        if flow_init is None:
+            coords2 = xyz1.clone()
+            flow = torch.zeros_like(xyz1)
+        else:                                     # warm start: the loop starts at xyz1 + flow_init
+            coords2 = xyz1 + flow_init
+            flow = coords2 - xyz1                 # the first iteration's flow input, as :43 computes it
         preds = []
         me = self.update_block.motion_encoder
         use_tc = ops.tc_supported(n)
@@ -229,13 +272,17 @@ class RSF(_RaftBase):
                                     resolution=3, truncate_k=args.truncate_k)
         self.update_block = UpdateBlock(hidden_dim=self.hidden_dim)
 
-    def _forward_impl(self, p, num_iters=12):
-        xyz1, _, _, graph_context, net, inp = self._encode(p)
-        _, preds = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=True)
+    def _forward_impl(self, p, num_iters=12, flow_init=None):
+        return self._run(self._encode(p), num_iters, flow_init)
+
+    def _run(self, encoded, num_iters, flow_init=None):
+        """The loop on _pair's outputs -> the list of num_iters flows."""
+        xyz1, _, _, graph_context, net, inp = encoded
+        _, preds = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=True, flow_init=flow_init)
         return preds
 
-    def _forward_train(self, p, num_iters=12):
-        return train.rsf_forward(self, p, num_iters)
+    def _forward_train(self, p, num_iters=12, flow_init=None):
+        return train.rsf_forward(self, p, num_iters, flow_init)
 
 
 class RSF_refine(_RaftBase):
@@ -250,12 +297,16 @@ class RSF_refine(_RaftBase):
         self.update_block = UpdateBlock(hidden_dim=self.hidden_dim)
         self.refine_block = FlotRefine()
 
-    def _forward_impl(self, p, num_iters=12):
-        xyz1, _, graph, graph_context, net, inp = self._encode(p)
-        flow, _ = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=False)
+    def _forward_impl(self, p, num_iters=12, flow_init=None):
+        return self._run(self._encode(p), num_iters, flow_init)
+
+    def _run(self, encoded, num_iters, flow_init=None):
+        """The loop and the refiner on _pair's outputs -> the refined flow."""
+        xyz1, _, graph, graph_context, net, inp = encoded
+        flow, _ = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=False, flow_init=flow_init)
         return self.refine_block(flow, graph)      # RAFTSceneFlowRefine.py:46
 
-    def _forward_train(self, p, num_iters=12):
+    def _forward_train(self, p, num_iters=12, flow_init=None):
         """model/RAFTSceneFlowRefine.py:22-48: everything up to the last flow under no_grad (the fused inference kernels),
         the refiner -- the only part tools/engine_refine.py trains -- layer by layer with gradients.  The refiner's input
         flow is coords2 - xyz1 with coords2 computed under no_grad, so xyz1 receives minus the flow's gradient and xyz2 none."""
@@ -264,7 +315,7 @@ class RSF_refine(_RaftBase):
             raise NotImplementedError("training differentiates through the fp32 state: call model.set_precision('fp32')")
         with torch.no_grad():
             xyz1, _, graph, graph_context, net, inp = self._encode(p)
-            flow, _ = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=False)
+            flow, _ = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=False, flow_init=flow_init)
         if x1.requires_grad:
             flow = flow + (x1.detach() - x1)          # the same values; d xyz1 = -d flow
         return train.flot_refine(self.refine_block, flow, graph)

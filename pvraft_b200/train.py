@@ -331,8 +331,9 @@ def flot_refine(m, flow, graph):
     return flow + linear(x, m.fc.weight, m.fc.bias)
 
 
-def rsf_forward(model, p, num_iters):
-    """RSF.forward with gradients (model/RAFTSceneFlow.py:22-50) -> list of num_iters flows [B,N1,3]."""
+def rsf_forward(model, p, num_iters, flow_init=None):
+    """RSF.forward with gradients (model/RAFTSceneFlow.py:22-50) -> list of num_iters flows [B,N1,3].  flow_init [B,N1,3]
+    (detached, fp32): the loop starts at xyz1 + flow_init (RAFT's warm start; no gradient reaches it)."""
     cb = model.corr_block
     ops.check_pair(p[0], p[1], cb.truncate_k)
     xyz1 = p[0].contiguous().float()                                           # attached: gradients reach the inputs
@@ -355,7 +356,7 @@ def rsf_forward(model, p, num_iters):
     fct1 = flot_encoder(model.context_extractor, xyz1, graph1)                 # :31 (same cloud, same graph)
     net = torch.tanh(fct1[..., :model.hidden_dim])                             # :33-35
     inp = torch.relu(fct1[..., model.hidden_dim:])
-    coords2 = xyz1.clone()
+    coords2 = xyz1.clone() if flow_init is None else xyz1 + flow_init          # (detached at the top of every iteration)
     preds = []
     # 'bf16-mixed': the loop's per-point layers on bf16 wgmma (LinearFn, bf16_layer_plan); the lookup stays fp32
     with ops.bf16_compute(model.bf16_compute):
