@@ -3,18 +3,65 @@
 // materialising the reference's [B, C+3, 32, N] edge tensor.
 //
 // fc1 is linear and bias-free, so  W.[x_j - x_i, e] = P_j - P_i + W_e.e  with  P = W[:, :cin].x  computed
-// once per point by pvraft_linear_fwd; this kernel only gathers the 32 rows P_j (L2-resident table).
+// once per point by pvraft_linear_fwd; this kernel only gathers the 32 rows P_j.
 // GroupNorm + LeakyReLU is monotone per channel, so max_e lrelu(GN(y_e)) = lrelu(GN(max_e y_e)) when the
 // folded GN scale is >= 0 and lrelu(GN(min_e y_e)) otherwise: the kernel emits both the per-channel max
 // and min of the raw y, plus the double-precision (sum, sum^2) of all N*32*C raw values per group.
 //
-// One warp per point; lane l owns the adjacent channel pairs (2l, 2l+1) + 64q: a neighbour row is one 8-byte load per lane
-// and pair, and the per-edge scalars (neighbour id, edge vector) are read back as ONE broadcast 16-byte shared-memory load.
+// Persistent and warp-specialised, one CTA per SM.  A CTA walks tiles of kEdgeTile consecutive positions of the processing
+// order (one sample per tile).  The builder warps prepare tile t + 1 while the consumer warps compute tile t: they
+// deduplicate the tile's neighbour and centre ids in a shared-memory hash (a Morton tile of 32 points makes ~1000 references
+// to ~200 distinct rows) and bulk-copy every distinct row P_j into the idle half of a double-buffered table.  The consumer
+// warps run one warp per point exactly as a plain gather would: lane l owns the adjacent channel pairs (2l, 2l+1) + 64q, a
+// neighbour row is one 8-byte shared-memory load per lane and pair, and the per-edge scalars (row offset, edge vector) are
+// read back as ONE broadcast 16-byte shared-memory load.  A tile with more distinct rows than the table holds is gathered
+// from global memory instead (an unordered cloud), with the same arithmetic: the results never depend on the order.
 #include "fixed_point.cuh"
+#include "tma.cuh"
 
 namespace pvraft {
 
-constexpr int kEdgeThreads = 256;
+constexpr int kEdgeTile = 32;                                  // points per tile
+constexpr int kEdgeConsumerWarps = 16;                         // at most: one point per warp at a time
+// Warps per role, from the channel pairs per lane and the form.  The builders' chain per tile (hash rounds, then the copies)
+// is what the consumers wait for: 8 builder warps halve it against 4 (M = 4 references per lane instead of 8) where the
+// register budget of one CTA per SM allows it without spills.  Registers: 80 (1 pair, 16 + 8 warps), 96 (1 pair DET,
+// 16 + 4), 128 (2 pairs, 12 + 4), 168 (2 pairs DET, 8 + 4).
+__host__ __device__ constexpr int edge_consumer_warps(int pairs, bool det) { return pairs == 1 ? kEdgeConsumerWarps : det ? 8 : 12; }
+__host__ __device__ constexpr int edge_builder_warps(int pairs, bool det) { return pairs == 1 && !det ? 8 : 4; }
+__host__ __device__ constexpr int edge_threads(int pairs, bool det) { return (edge_consumer_warps(pairs, det) + edge_builder_warps(pairs, det)) * 32; }
+constexpr int kEdgeRefs = kEdgeTile * 33;                      // row references of a tile: 32 neighbours + the centre per point
+constexpr int kEdgeHashBits = 11, kEdgeHash = 1 << kEdgeHashBits;   // > kEdgeRefs: linear probing always reaches an empty key
+constexpr int kEdgeTableFloats = 22528;                        // one table buffer: rows = min(kEdgeRefs, this / C)
+// named barriers (0 is __syncthreads): the consumers among themselves, "buffer free" (consumers arrive, builders wait), the builders
+constexpr int kBarConsumers = 1, kBarEmpty = 2, kBarBuilders = 4;
+
+
+inline int edge_table_rows(int C) { return kEdgeTableFloats / C < kEdgeRefs ? kEdgeTableFloats / C : kEdgeRefs; }
+
+// shared memory after the two table buffers [2][rows][C]
+struct EdgeSmem {
+    int key[2][kEdgeHash];                 // row id, -1 = empty
+    short slot[2][kEdgeHash];              // table slot of key[h] (>= rows: the tile overflowed)
+    short ref[2][kEdgeTile * 32];          // key index of neighbour e of point p, at p * 32 + e
+    short ctr[2][kEdgeTile];               // key index of the centre of point p
+    int row[2][kEdgeRefs];                 // row id of table slot r
+    int count[2];                          // distinct rows of the tile
+    unsigned long long full[2];            // mbarrier: the tile's hash, references and rows are in place
+    float4 edge[kEdgeConsumerWarps][32];   // (row offset bits, ex, ey, ez) of a consumer warp's point
+    double part[kEdgeConsumerWarps][16];   // per-warp GroupNorm partials (group, moment)
+    unsigned long long fx[16 * kFxWords];  // DET: the CTA's fixed-point (group, moment) sums
+};
+
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void cp_async16(void* dst, const void* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+// one arrival on the mbarrier once every cp.async this thread has issued so far has landed
+__device__ __forceinline__ void cp_async_arrive(void* bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 
 // elementwise arithmetic on channel pairs held as one 64-bit value: each component is one IEEE round-to-nearest operation
 // (the _rn intrinsics are never contracted into an FMA)
@@ -45,19 +92,170 @@ __device__ __forceinline__ unsigned long long sub2(unsigned long long a, unsigne
     return pk(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y));
 }
 
+template <bool TABLE>
+__device__ __forceinline__ float2 ld_row(const float* p) {
+    if constexpr (TABLE) return *reinterpret_cast<const float2*>(p);   // LDS.64 from the shared table
+    else return __ldg(reinterpret_cast<const float2*>(p));
+}
+
+// one point: y_e = (P_j - P_i) + W_e.e over the 32 edges in order 0..31 -> per-channel max, min, sum and sum of squares.
+// rows: the shared table (TABLE) or the sample's P; se: the warp's (row offset, edge vector) list; ctr: the centre row P_i
+template <int PAIRS, bool TABLE>
+__device__ __forceinline__ void edge_point(const float* rows, const float4* se, const float* ctr, const int (&coff)[PAIRS],
+                                           const unsigned long long (&wx2)[PAIRS], const unsigned long long (&wy2)[PAIRS],
+                                           const unsigned long long (&wz2)[PAIRS], float2 (&mx)[PAIRS], float2 (&mn)[PAIRS],
+                                           unsigned long long (&s1)[PAIRS], unsigned long long (&s2)[PAIRS]) {
+    unsigned long long pi[PAIRS];
+#pragma unroll
+    for (int q = 0; q < PAIRS; ++q) {
+        const float2 t = ld_row<TABLE>(ctr + coff[q]);
+        pi[q] = pk(t.x, t.y);
+        mx[q] = make_float2(-INFINITY, -INFINITY); mn[q] = make_float2(INFINITY, INFINITY);
+        s1[q] = pk(0.f, 0.f); s2[q] = pk(0.f, 0.f);
+    }
+#pragma unroll 8
+    for (int e = 0; e < 32; ++e) {
+        const float4 ed = se[e];
+        const float* row = rows + __float_as_int(ed.x);
+        const unsigned long long ex = pk(ed.y, ed.y), ey = pk(ed.z, ed.z), ez = pk(ed.w, ed.w);
+#pragma unroll
+        for (int q = 0; q < PAIRS; ++q) {
+            const float2 pj = ld_row<TABLE>(row + coff[q]);
+            // y = (P_j - P_i) + fma(w_z, e_z, fma(w_y, e_y, w_x * e_x)), both channels of the pair at once
+            const unsigned long long t = fma2(wz2[q], ez, fma2(wy2[q], ey, mul2(wx2[q], ex)));
+            const unsigned long long y2 = add2(sub2(pk(pj.x, pj.y), pi[q]), t);
+            const float2 y = upk(y2);
+            mx[q].x = fmaxf(mx[q].x, y.x); mx[q].y = fmaxf(mx[q].y, y.y);
+            mn[q].x = fminf(mn[q].x, y.x); mn[q].y = fminf(mn[q].y, y.y);
+            s1[q] = add2(s1[q], y2);
+            s2[q] = fma2(y2, y2, s2[q]);
+        }
+    }
+}
+
+// warp-collective: puts the rows id[0..K) of every lane (-1: nothing) into the tile's hash and returns their key indices in h.
+// The K compare-and-swaps of a lane are in flight together; each round's new keys take the next table slots (one warp scan,
+// one shared atomic).
+template <int K>
+__device__ __forceinline__ void edge_insert(const int (&id)[K], int (&h)[K], EdgeSmem& s, int buf, int rows) {
+    const int lane = lane_id();
+    unsigned pending = 0;
+#pragma unroll
+    for (int m = 0; m < K; ++m) {
+        h[m] = (int)(((unsigned)id[m] * 0x9E3779B1u) >> (32 - kEdgeHashBits));
+        if (id[m] >= 0) pending |= 1u << m;
+    }
+    while (__any_sync(kFull, pending)) {
+        int old[K];
+#pragma unroll
+        for (int m = 0; m < K; ++m)
+            if (pending >> m & 1u) old[m] = atomicCAS(&s.key[buf][h[m]], -1, id[m]);
+        unsigned fresh = 0;
+#pragma unroll
+        for (int m = 0; m < K; ++m)
+            if (pending >> m & 1u) {
+                if (old[m] == -1) fresh |= 1u << m;
+                if (old[m] == -1 || old[m] == id[m]) pending &= ~(1u << m);
+                else h[m] = (h[m] + 1) & (kEdgeHash - 1);
+            }
+        const int nf = __popc(fresh);
+        int incl = nf;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(kFull, incl, o);
+            if (lane >= o) incl += v;
+        }
+        const int total = __shfl_sync(kFull, incl, 31);
+        if (total) {
+            int first = 0;
+            if (lane == 31) first = atomicAdd(&s.count[buf], total);
+            int sl = __shfl_sync(kFull, first, 31) + incl - nf;
+#pragma unroll
+            for (int m = 0; m < K; ++m)
+                if (fresh >> m & 1u) {
+                    s.slot[buf][h[m]] = (short)sl;
+                    if (sl < rows) s.row[buf][sl] = id[m];
+                    ++sl;
+                }
+        }
+    }
+}
+
 // DET: every point's per-channel (sum, sum^2) over its 32 edges enters a per-lane fixed-point register sum, and those enter the
 // [B,16] fixed-point workspace `stats` points at then (fixed_point.cuh): the sums do not depend on which CTA took which points
 template <int PAIRS, bool DET>
-__global__ void __launch_bounds__(kEdgeThreads, DET ? 2 : (PAIRS == 1 ? 6 : 4)) k_setconv_edge_pairs(const float* __restrict__ fc1p, const int32_t* __restrict__ nbr,
+__global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pairs(const float* __restrict__ fc1p, const int32_t* __restrict__ nbr,
                                                                      const float* __restrict__ edge_feats, const float* __restrict__ w_fc1,
                                                                      int cin, int B, int N, int C, float* __restrict__ ymax,
                                                                      float* __restrict__ ymin, double* __restrict__ stats,
-                                                                     const int32_t* __restrict__ order) {
-    __shared__ double s_part[kEdgeThreads / 32][128][2];
-    __shared__ __align__(16) float4 s_edge[kEdgeThreads / 32][32];   // (neighbour id bits, ex, ey, ez) of the warp's point
+                                                                     const int32_t* __restrict__ order, int rows) {
+    constexpr int CW = edge_consumer_warps(PAIRS, DET), kConsumers = CW * 32, kThreads = edge_threads(PAIRS, DET);
+    constexpr int BW = edge_builder_warps(PAIRS, DET), kBuilders = BW * 32;
+    static_assert(kEdgeTile % BW == 0 && kEdgeTile <= kBuilders && CW <= kEdgeConsumerWarps, "work split");
+    extern __shared__ __align__(128) unsigned char smem[];
+    float* tables = reinterpret_cast<float*>(smem);   // [2][rows][C]
+    EdgeSmem& s = *reinterpret_cast<EdgeSmem*>(smem + (size_t)2 * rows * C * sizeof(float));
     pdl_trigger();   // the next kernel may be staged while this one drains
-    pdl_wait();      // (launched with PDL: nothing above touches global memory)
-    const int lane = lane_id(), w = warp_id(), nwarps = kEdgeThreads / 32;
+    if (threadIdx.x == 0) {
+        mbar_init(&s.full[0], 2 * kBuilders);   // per builder thread: its hash / reference stores, then its row copies
+        mbar_init(&s.full[1], 2 * kBuilders);
+        fence_mbarrier_init();
+    }
+    __syncthreads();
+    pdl_wait();      // (launched with PDL: nothing above touches global memory; P is the previous launch's output)
+    const int lane = lane_id(), w = warp_id();
+    const int tps = (N + kEdgeTile - 1) / kEdgeTile;   // tiles per sample
+    long long t_begin, t_end;
+    split_range((long long)B * tps, gridDim.x, blockIdx.x, t_begin, t_end);
+    const int ntiles = (int)(t_end - t_begin);
+
+    if (w >= CW) {   // ---- builders: tile k into buffer k & 1 ----
+        const int bt = threadIdx.x - kConsumers, bw = bt >> 5;
+        const int chunks = C / 4, rows_per_copy = 32 / chunks, copy_row = lane / chunks, copy_chunk = lane - copy_row * chunks;
+        constexpr int M = kEdgeTile / BW;
+        for (int k = 0; k < ntiles; ++k) {
+            const int buf = k & 1;
+            const long long t = t_begin + k;
+            const int b = (int)(t / tps), start = (int)(t - (long long)b * tps) * kEdgeTile, len = min(kEdgeTile, N - start);
+            // this thread's references, read before the buffer is free: neighbour `lane` of the points bw, bw + 4, ..., and
+            // (warp 0) the centre of point `lane`
+            const long long s0 = (long long)b * N;
+            int id[M + 1], h[M + 1];
+#pragma unroll
+            for (int m = 0; m < M; ++m) {
+                const int p = bw + BW * m;
+                id[m] = p < len ? (order ? __ldg(order + s0 + start + p) : start + p) : -1;
+            }
+            id[M] = bw == 0 && lane < len ? (order ? __ldg(order + s0 + start + lane) : start + lane) : -1;
+#pragma unroll
+            for (int m = 0; m < M; ++m)
+                if (id[m] >= 0) id[m] = __ldg(nbr + (s0 + id[m]) * 32 + lane);
+            if (k >= 2) bar_sync(kBarEmpty + buf, kThreads);   // the consumers are done with tile k - 2
+            for (int j = bt; j < kEdgeHash; j += kBuilders) s.key[buf][j] = -1;
+            if (bt == 0) s.count[buf] = 0;
+            bar_sync(kBarBuilders, kBuilders);
+            edge_insert<M + 1>(id, h, s, buf, rows);
+#pragma unroll
+            for (int m = 0; m < M; ++m)
+                if (id[m] >= 0) s.ref[buf][(bw + BW * m) * 32 + lane] = (short)h[m];
+            if (id[M] >= 0) s.ctr[buf][lane] = (short)h[M];
+            mbar_arrive(&s.full[buf]);
+            bar_sync(kBarBuilders, kBuilders);   // every row id is in place
+            // the distinct rows -> the table: a warp copies rows_per_copy rows of C / 4 16-byte chunks per instruction; an
+            // overflowing tile copies nothing (its consumers gather from global memory)
+            const int n = s.count[buf];
+            if (n <= rows) {
+                const float* P = fc1p + (size_t)b * N * C;
+                float* table = tables + (size_t)buf * rows * C;
+                for (int r = bw * rows_per_copy + copy_row; copy_row < rows_per_copy && r < n; r += BW * rows_per_copy)
+                    cp_async16(table + (size_t)r * C + 4 * copy_chunk, P + (size_t)s.row[buf][r] * C + 4 * copy_chunk);
+            }
+            cp_async_arrive(&s.full[buf]);   // (when this thread's copies have landed)
+        }
+        return;
+    }
+
+    // ---- consumers: one warp per point ----
     const int ld = cin + 3;
     float2 wx[PAIRS], wy[PAIRS], wz[PAIRS];
 #pragma unroll
@@ -70,66 +268,111 @@ __global__ void __launch_bounds__(kEdgeThreads, DET ? 2 : (PAIRS == 1 ? 6 : 4)) 
     unsigned long long wx2[PAIRS], wy2[PAIRS], wz2[PAIRS];
 #pragma unroll
     for (int q = 0; q < PAIRS; ++q) { wx2[q] = pk(wx[q].x, wx[q].y); wy2[q] = pk(wy[q].x, wy[q].y); wz2[q] = pk(wz[q].x, wz[q].y); }
-    const long long total = (long long)B * N;
-    long long pt_begin, pt_end;
-    split_range(total, gridDim.x, blockIdx.x, pt_begin, pt_end);   // (handing SM-mates adjacent ranges was measured: no gain)
-    long long seg = pt_begin;
-    while (seg < pt_end) {
-        const int b = (int)(seg / N);
-        long long seg_end = (long long)(b + 1) * N;
-        if (seg_end > pt_end) seg_end = pt_end;
-        double dS[PAIRS][2], dSS[PAIRS][2];
+    bool on[PAIRS];   // C need not fill the last group of 64 channels (encoder layers: 16, 48, 96)
+    int coff[PAIRS];
 #pragma unroll
-        for (int q = 0; q < PAIRS; ++q) { dS[q][0] = dS[q][1] = 0.0; dSS[q][0] = dSS[q][1] = 0.0; }
-        Fx fS[PAIRS][2], fSS[PAIRS][2];
+    for (int q = 0; q < PAIRS; ++q) { on[q] = 2 * lane + 64 * q < C; coff[q] = on[q] ? 2 * lane + 64 * q : 0; }
+    const int gsz = C / PVRAFT_GN_GROUPS;
+    double dS[PAIRS][2], dSS[PAIRS][2];
+    Fx fS[PAIRS][2], fSS[PAIRS][2];
+    auto reset = [&]() {
+#pragma unroll
+        for (int q = 0; q < PAIRS; ++q)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                dS[q][h] = dSS[q][h] = 0.0;
+                if constexpr (DET) fS[q][h] = fSS[q][h] = Fx{0ull, 0ull, 0u};
+            }
+    };
+    // the consumers' partials of sample b -> one global addition per (group, moment) and CTA
+    auto flush = [&](int b) {
         if constexpr (DET) {
+            bar_sync(kBarConsumers, kConsumers);
+            if (threadIdx.x < 16 * kFxWords) s.fx[threadIdx.x] = 0ull;
+            bar_sync(kBarConsumers, kConsumers);
 #pragma unroll
             for (int q = 0; q < PAIRS; ++q)
 #pragma unroll
-                for (int h = 0; h < 2; ++h) fS[q][h] = fSS[q][h] = Fx{0ull, 0ull, 0u};
+                for (int h = 0; h < 2; ++h)
+                    if (on[q]) {
+                        const int g = (2 * lane + 64 * q + h) / gsz;
+                        fx_atomic(s.fx + (g * 2) * kFxWords, fS[q][h]);
+                        fx_atomic(s.fx + (g * 2 + 1) * kFxWords, fSS[q][h]);
+                    }
+            bar_sync(kBarConsumers, kConsumers);
+            if (threadIdx.x < 16) {
+                const Fx v{s.fx[threadIdx.x * kFxWords], s.fx[threadIdx.x * kFxWords + 1], (unsigned)s.fx[threadIdx.x * kFxWords + 2]};
+                fx_atomic(reinterpret_cast<unsigned long long*>(stats) + ((size_t)b * 16 + threadIdx.x) * kFxWords, v);
+            }
+        } else {
+            bar_sync(kBarConsumers, kConsumers);   // (the previous flush has read s.part)
+#pragma unroll
+            for (int g = 0; g < PVRAFT_GN_GROUPS; ++g) {
+                double a = 0.0, a2 = 0.0;
+#pragma unroll
+                for (int q = 0; q < PAIRS; ++q)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        if (on[q] && (2 * lane + 64 * q + h) / gsz == g) { a += dS[q][h]; a2 += dSS[q][h]; }
+#pragma unroll
+                for (int o = 16; o; o >>= 1) { a += __shfl_xor_sync(kFull, a, o); a2 += __shfl_xor_sync(kFull, a2, o); }
+                if (lane == 0) { s.part[w][2 * g] = a; s.part[w][2 * g + 1] = a2; }
+            }
+            bar_sync(kBarConsumers, kConsumers);
+            if (threadIdx.x < 16) {
+                double acc = 0.0;
+                for (int ww = 0; ww < CW; ++ww) acc += s.part[ww][threadIdx.x];
+                if (acc != 0.0) atomicAdd(stats + (size_t)b * 16 + threadIdx.x, acc);
+            }
         }
-        bool on[PAIRS];   // C need not fill the last group of 64 channels (encoder layers: 16, 48, 96)
-        int coff[PAIRS];
+        reset();
+    };
+    reset();
+    int cur = -1;   // the sample whose partials the registers hold
+    for (int k = 0; k < ntiles; ++k) {
+        const int buf = k & 1;
+        const long long t = t_begin + k;
+        const int b = (int)(t / tps), start = (int)(t - (long long)b * tps) * kEdgeTile, len = min(kEdgeTile, N - start);
+        if (b != cur) {
+            if (cur >= 0) flush(cur);
+            cur = b;
+        }
+        // the global reads that do not need the table, issued before waiting for it: the ids and edge vectors of the warp's points
+        constexpr int U = (kEdgeTile + CW - 1) / CW;
+        int pid[U];
+        float3 pe[U];
 #pragma unroll
-        for (int q = 0; q < PAIRS; ++q) { on[q] = 2 * lane + 64 * q < C; coff[q] = on[q] ? 2 * lane + 64 * q : 0; }
+        for (int u = 0; u < U; ++u) {
+            const int p = w + u * CW;
+            pid[u] = p < len ? (order ? __ldg(order + (long long)b * N + start + p) : start + p) : 0;
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            // lane e parks neighbour e: its row offset and edge feature x_j - x_i (graph.edge_feats, gconv.py:66)
+            const float* ef = edge_feats + (((size_t)b * N + pid[u]) * 32 + lane) * 3;
+            pe[u] = w + u * CW < len ? make_float3(__ldg(ef), __ldg(ef + 1), __ldg(ef + 2)) : make_float3(0.f, 0.f, 0.f);
+        }
+        mbar_wait(&s.full[buf], (unsigned)(k >> 1) & 1u);
+        const bool in_table = s.count[buf] <= rows;
         const float* P = fc1p + (size_t)b * N * C;
-        for (long long r = seg + w; r < seg_end; r += nwarps) {
-            // processing order: with `order` (a space-filling-curve rank -> point table) the 8 warps of a CTA work on spatial
-            // neighbours at the same time, whose 32-neighbourhoods overlap: their gathers hit the same rows in L1
-            const int i = order ? __ldg(order + r) : (int)(r - (long long)b * N);
+        const float* table = tables + (size_t)buf * rows * C;
+#pragma unroll 1
+        for (int p = w; p < len; p += CW) {
+            const int i = pid[0];
+            const float3 e = pe[0];
+#pragma unroll
+            for (int u = 0; u + 1 < U; ++u) { pid[u] = pid[u + 1]; pe[u] = pe[u + 1]; }
             const long long pt = (long long)b * N + i;
-            // lane e parks neighbour e: id and edge feature x_j - x_i (graph.edge_feats, gconv.py:66)
-            const float* ef = edge_feats + ((size_t)pt * 32 + lane) * 3;
+            const int off = in_table ? s.slot[buf][s.ref[buf][p * 32 + lane]] * C : __ldg(nbr + pt * 32 + lane) * C;
             __syncwarp();
-            s_edge[w][lane] = make_float4(__int_as_float(__ldg(nbr + pt * 32 + lane) * C), __ldg(ef), __ldg(ef + 1), __ldg(ef + 2));
+            s.edge[w][lane] = make_float4(__int_as_float(off), e.x, e.y, e.z);
             __syncwarp();
-            unsigned long long pi[PAIRS], s1[PAIRS], s2[PAIRS];
             float2 mx[PAIRS], mn[PAIRS];
-#pragma unroll
-            for (int q = 0; q < PAIRS; ++q) {
-                const float2 t = __ldg(reinterpret_cast<const float2*>(P + (size_t)i * C + coff[q]));
-                pi[q] = pk(t.x, t.y);
-                mx[q] = make_float2(-INFINITY, -INFINITY); mn[q] = make_float2(INFINITY, INFINITY);
-                s1[q] = pk(0.f, 0.f); s2[q] = pk(0.f, 0.f);
-            }
-#pragma unroll 8
-            for (int e = 0; e < 32; ++e) {
-                const float4 ed = s_edge[w][e];
-                const float* row = P + __float_as_int(ed.x);
-                const unsigned long long ex = pk(ed.y, ed.y), ey = pk(ed.z, ed.z), ez = pk(ed.w, ed.w);
-#pragma unroll
-                for (int q = 0; q < PAIRS; ++q) {
-                    const float2 pj = __ldg(reinterpret_cast<const float2*>(row + coff[q]));
-                    // y = (P_j - P_i) + fma(w_z, e_z, fma(w_y, e_y, w_x * e_x)), both channels of the pair at once
-                    const unsigned long long t = fma2(wz2[q], ez, fma2(wy2[q], ey, mul2(wx2[q], ex)));
-                    const unsigned long long y2 = add2(sub2(pk(pj.x, pj.y), pi[q]), t);
-                    const float2 y = upk(y2);
-                    mx[q].x = fmaxf(mx[q].x, y.x); mx[q].y = fmaxf(mx[q].y, y.y);
-                    mn[q].x = fminf(mn[q].x, y.x); mn[q].y = fminf(mn[q].y, y.y);
-                    s1[q] = add2(s1[q], y2);
-                    s2[q] = fma2(y2, y2, s2[q]);
-                }
-            }
+            unsigned long long s1[PAIRS], s2[PAIRS];
+            if (in_table)
+                edge_point<PAIRS, true>(table, s.edge[w], table + s.slot[buf][s.ctr[buf][p]] * C, coff, wx2, wy2, wz2, mx, mn, s1, s2);
+            else
+                edge_point<PAIRS, false>(P, s.edge[w], P + (size_t)i * C, coff, wx2, wy2, wz2, mx, mn, s1, s2);
 #pragma unroll
             for (int q = 0; q < PAIRS; ++q) {
                 const size_t o = (size_t)pt * C + coff[q];
@@ -142,56 +385,14 @@ __global__ void __launch_bounds__(kEdgeThreads, DET ? 2 : (PAIRS == 1 ? 6 : 4)) 
                     fx_add(fS[q][0], fx_from((double)a1.x)); fx_add(fS[q][1], fx_from((double)a1.y));
                     fx_add(fSS[q][0], fx_from((double)a2.x)); fx_add(fSS[q][1], fx_from((double)a2.y));
                 } else {
-                dS[q][0] += (double)a1.x; dS[q][1] += (double)a1.y;
-                dSS[q][0] += (double)a2.x; dSS[q][1] += (double)a2.y;
+                    dS[q][0] += (double)a1.x; dS[q][1] += (double)a1.y;
+                    dSS[q][0] += (double)a2.x; dSS[q][1] += (double)a2.y;
                 }
             }
         }
-        if constexpr (DET) {   // lanes -> the CTA's shared slots -> one global addition per (group, moment)
-            __shared__ unsigned long long s_fx[16 * kFxWords];
-            __syncthreads();
-            if (threadIdx.x < 16 * kFxWords) s_fx[threadIdx.x] = 0ull;
-            __syncthreads();
-            const int gsz = C / PVRAFT_GN_GROUPS;
-#pragma unroll
-            for (int q = 0; q < PAIRS; ++q)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (on[q]) {
-                        const int g = (2 * lane + 64 * q + h) / gsz;
-                        fx_atomic(s_fx + (g * 2) * kFxWords, fS[q][h]);
-                        fx_atomic(s_fx + (g * 2 + 1) * kFxWords, fSS[q][h]);
-                    }
-            __syncthreads();
-            if (threadIdx.x < 16) {
-                const Fx v{s_fx[threadIdx.x * kFxWords], s_fx[threadIdx.x * kFxWords + 1], (unsigned)s_fx[threadIdx.x * kFxWords + 2]};
-                fx_atomic(reinterpret_cast<unsigned long long*>(stats) + ((size_t)b * 16 + threadIdx.x) * kFxWords, v);
-            }
-            seg = seg_end;
-            continue;
-        }
-        // block reduction of the per-channel partials -> per-group sums -> one atomic per (group, moment)
-        __syncthreads();
-#pragma unroll
-        for (int q = 0; q < PAIRS; ++q) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                if (on[q]) {
-                    s_part[w][2 * lane + 64 * q + h][0] = dS[q][h];
-                    s_part[w][2 * lane + 64 * q + h][1] = dSS[q][h];
-                }
-            }
-        }
-        __syncthreads();
-        if (threadIdx.x < 16) {
-            const int g = threadIdx.x >> 1, m = threadIdx.x & 1, gsz = C / PVRAFT_GN_GROUPS;
-            double acc = 0.0;
-            for (int c = g * gsz; c < (g + 1) * gsz; ++c)
-                for (int ww = 0; ww < nwarps; ++ww) acc += s_part[ww][c][m];
-            if (acc != 0.0) atomicAdd(stats + (size_t)b * 16 + threadIdx.x, acc);
-        }
-        seg = seg_end;
+        if (k + 2 < ntiles) bar_arrive(kBarEmpty + buf, kThreads);   // the builders may refill this buffer with tile k + 2
     }
+    if (cur >= 0) flush(cur);
 }
 
 }  // namespace pvraft
@@ -204,16 +405,20 @@ static int setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* 
     if (!fc1p || !nbr || !edge_feats || !w_fc1 || !ymax || !ymin || !stats) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: null pointer");
     if (B <= 0 || N <= 0 || cin <= 0) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: bad shape");
     if (C <= 0 || C > 128 || C % PVRAFT_GN_GROUPS) return fail(PVRAFT_ERR_UNSUPPORTED, "setconv_edge: C=%d (multiple of 8, <= 128)", C);
-    const long long total = (long long)B * N;
-    long long g = (long long)sm_count() * 8;
-    const long long need = (total + (kEdgeThreads / 32) - 1) / (kEdgeThreads / 32);
-    if (g > need) g = need;
-    const int grid = (int)(g < 1 ? 1 : g);
+    if (reinterpret_cast<uintptr_t>(fc1p) % 16) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: fc1p must be 16-byte aligned (rows are bulk-copied)");
+    const int rows = edge_table_rows(C);
+    const size_t smem = (size_t)2 * rows * C * sizeof(float) + sizeof(EdgeSmem);
+    const long long tiles = (long long)B * ((N + kEdgeTile - 1) / kEdgeTile);
+    long long g = sm_count();
+    if (g > tiles) g = tiles;
+    const int grid = (int)g;
     cudaStream_t st = (cudaStream_t)stream;
     double* kstats = DET ? static_cast<double*>(ws) : stats;
-    if (C <= 64) launch_pdl(k_setconv_edge_pairs<1, DET>, grid, kEdgeThreads, 0, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, kstats, order);
-    else launch_pdl(k_setconv_edge_pairs<2, DET>, grid, kEdgeThreads, 0, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, kstats, order);
-    const int rc = check_launch("setconv_edge");
+    const auto kernel = C <= 64 ? k_setconv_edge_pairs<1, DET> : k_setconv_edge_pairs<2, DET>;
+    int rc;
+    if ((rc = opt_in_smem(kernel, smem))) return rc;
+    launch_pdl(kernel, grid, edge_threads(C <= 64 ? 1 : 2, DET), smem, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, kstats, order, rows);
+    rc = check_launch("setconv_edge");
     if (rc || !DET) return rc;
     return fx_flush_f64(static_cast<const unsigned long long*>(ws), 1, (long long)B * 16, (long long)B * 16, 0, stats, st);
 }

@@ -1,45 +1,83 @@
-"""Does a spatially coherent point order help the SetConv edge kernel (gathers of neighbour rows)?
-python tools/bench_edge.py"""
-import os, sys
+"""Standalone time of the SetConv edge kernel (ops.setconv_edge) at the shapes a forward launches it at, with CUDA events.
+python tools/bench_edge.py [--launches 50] [--det]
+
+Inputs are the real ones: the 32-NN graph from ops.knn and the Morton processing order from ops.point_order over the bench
+clouds.  Shapes (bench default, B = 8, N = 8192):
+  loop      B = 8,  C = 64, cin = 64  (flow-head SetConv, 32 launches per forward)
+  feat1..3  B = 16, C = 16 / 48 / 96, cin = 3 / 32 / 64  (feature encoder over both clouds)
+  ctx1..3   B = 8,  same channels  (context encoder over pc1)
+Each shape is timed with the Morton order and with order = None (index order)."""
+import argparse
+import os
+import subprocess
+import sys
+
 import torch
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import bench
-from pvraft_b200 import ops, Graph
-dev = torch.device('cuda:0')
-b, n, c = 8, 8192, 64
-pc, _ = [t.to(dev) for t in bench.synthetic_clouds(b, n, 1234)]
+import bench  # noqa: E402
+from pvraft_b200 import ops, Graph  # noqa: E402
 
 
-def morton_order(p):
-    lo, hi = p.amin(1, keepdim=True), p.amax(1, keepdim=True)
-    q = ((p - lo) / (hi - lo).clamp_min(1e-9) * 1023.0).long().clamp_(0, 1023)
-    def spread(v):
-        v = (v | (v << 16)) & 0x030000FF
-        v = (v | (v << 8)) & 0x0300F00F
-        v = (v | (v << 4)) & 0x030C30C3
-        v = (v | (v << 2)) & 0x09249249
-        return v
-    code = spread(q[..., 0]) | (spread(q[..., 1]) << 1) | (spread(q[..., 2]) << 2)
-    return code.argsort(1)
+def card_line():
+    try:
+        r = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                           stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=30)
+        return r.stdout.strip().splitlines()[0]
+    except Exception as e:   # the timing below does not depend on it
+        return f'(nvidia-smi unavailable: {e})'
 
 
-def run(points, label):
-    g = Graph.construct_graph(points, 32)
-    x = torch.randn(b, n, c, device=dev)
-    w = torch.randn(c, c + 3, device=dev)
-    st = torch.zeros(b, 8, 2, dtype=torch.float64, device=dev)
-    big = torch.randn(8192, 8192, device=dev)
-    for _ in range(3):
-        ops.setconv_edge(x, g.nbr, g._rel, w, c, st)
-    for _ in range(2): big @ big
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(20):
-        ops.setconv_edge(x, g.nbr, g._rel, w, c, st)
-    e.record(); torch.cuda.synchronize()
-    print(label, 'setconv_edge %.1f us' % (s.elapsed_time(e) * 1e3 / 20))
+def time_edge(p, g, w, cin, order, launches, det):
+    b = p.shape[0]
+    st = torch.zeros(b, 8, 2, dtype=torch.float64, device=p.device)
+    ymax, ymin = torch.empty_like(p), torch.empty_like(p)
+    run = lambda: ops.setconv_edge(p, g.nbr, g._rel, w, cin, st, ymax, ymin, order=order)
+    prev = torch.are_deterministic_algorithms_enabled()
+    torch.use_deterministic_algorithms(det)
+    try:
+        for _ in range(5):
+            run()
+        torch.cuda.synchronize()
+        times = []
+        for _ in range(5):
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for _ in range(launches):
+                run()
+            e.record()
+            torch.cuda.synchronize()
+            times.append(s.elapsed_time(e) * 1e3 / launches)
+    finally:
+        torch.use_deterministic_algorithms(prev)
+    return sorted(times)[len(times) // 2], min(times), max(times)
 
 
-run(pc, 'input order ')
-perm = morton_order(pc)
-run(torch.gather(pc, 1, perm.unsqueeze(-1).expand(-1, -1, 3)).contiguous(), 'morton order')
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--launches', type=int, default=50, help='launches per timed window (5 windows, median reported)')
+    ap.add_argument('--det', action='store_true', help='also time the deterministic form')
+    a = ap.parse_args()
+    dev = torch.device('cuda:0')
+    print('card:', card_line())
+    b, n = 8, 8192
+    pc1, pc2 = [t.to(dev) for t in bench.synthetic_clouds(b, n, 1234)]
+    both = torch.cat([pc1, pc2], 0).contiguous()
+    g8, g16 = Graph.construct_graph(pc1, 32), Graph.construct_graph(both, 32)
+    shapes = [('loop ', g8, 64, 64)] + [(f'feat{i + 1}', g16, c, cin) for i, (c, cin) in enumerate([(16, 3), (48, 32), (96, 64)])] \
+        + [(f'ctx{i + 1} ', g8, c, cin) for i, (c, cin) in enumerate([(16, 3), (48, 32), (96, 64)])]
+    torch.manual_seed(0)
+    for label, g, c, cin in shapes:
+        bb = g.nbr.shape[0]
+        p = torch.randn(bb, n, c, device=dev)
+        w = torch.randn(c, cin + 3, device=dev)
+        for det in ([False, True] if a.det else [False]):
+            for oname, order in (('morton', g.order), ('index ', None)):
+                med, lo, hi = time_edge(p, g, w, cin, order, a.launches, det)
+                gathers = bb * n * 32 * c * 4 / 1e9   # neighbour-row bytes the gathers read per launch
+                print(f'{label} B={bb:2d} C={c:3d} {"DET " if det else ""}{oname}: {med:8.1f} us  (min {lo:.1f}, max {hi:.1f}; '
+                      f'{gathers * 1e3:.0f} MB of neighbour rows, {gathers / (med * 1e-6) / 1e3:.2f} TB/s)', flush=True)
+
+
+if __name__ == '__main__':
+    main()
