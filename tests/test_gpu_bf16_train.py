@@ -19,6 +19,7 @@ import torch
 
 from conftest import default_weights
 from oracle import pvraft_oracle as O
+from train_helpers import sequence_loss
 
 pytestmark = pytest.mark.gpu
 
@@ -58,11 +59,6 @@ def make_model(dev, k=128, refine=False, seed=0, mode='bf16-mixed'):
 def clouds(b, n, seed, dev, scale=0.4):
     pc1, pc2 = O.synthetic_clouds(b, n, seed=seed)
     return (pc1 * scale).to(dev), (pc2 * scale).to(dev)
-
-
-def sequence_loss(flows, gt, gamma=0.8):
-    n = len(flows)
-    return sum(gamma ** (n - i - 1) * (flows[i] - gt).abs().sum(-1).mean() for i in range(n))
 
 
 def step(m, pc1, pc2, iters, inputs=False):

@@ -16,8 +16,9 @@ import torch
 from conftest import default_weights
 from oracle import pvraft_oracle as O
 from test_gpu_deterministic import same_bits
-from test_gpu_input_grads import deterministic, oracle_adjacency
-from test_gpu_train import compare_grads, leaf, sequence_loss
+from test_gpu_input_grads import deterministic
+from test_gpu_train import leaf
+from train_helpers import compare_grads, oracle_adjacency, sequence_loss
 
 pytestmark = pytest.mark.gpu
 K, ITERS = 128, 3

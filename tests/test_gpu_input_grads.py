@@ -3,7 +3,7 @@
     * the lookup's table gradient (pvraft_corr_lookup_xyz_bwd) and the graph's edge features (pvraft_edge_bwd with C = 3)
       against float64 autograd, in the default and the deterministic mode;
     * the whole model against autograd through the CPU oracle on the oracle's adjacency, with the bounds of
-      test_gpu_train.compare_grads, for RSF (equal and unequal clouds, N % 128 != 0) and RSF_refine;
+      train_helpers.compare_grads, for RSF (equal and unequal clouds, N % 128 != 0) and RSF_refine;
     * frozen weights, bitwise repeatability in deterministic mode, and a captured frozen-weight step.
 """
 import contextlib
@@ -16,8 +16,9 @@ from conftest import default_weights, rel_err
 import unequal_oracle as U
 from oracle import pvraft_oracle as O
 from test_gpu_deterministic import same_bits
-from test_gpu_train import compare_grads, leaf, sequence_loss
+from test_gpu_train import leaf
 from test_gpu_unequal_clouds import unequal_state
+from train_helpers import compare_grads, oracle_adjacency, sequence_loss
 
 pytestmark = pytest.mark.gpu
 
@@ -133,29 +134,6 @@ def test_graph_edge_features_backward(dev, det):
 # ----------------------------------------------------------------------------------------------------------------------
 # whole model against the oracle
 # ----------------------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def oracle_adjacency():
-    """kNN ties at the 32nd distance are either-valid: the model runs on the oracle's adjacency, handed in as `nbr`; the edge
-    features stay differentiable w.r.t. the cloud through graph.edge_feats."""
-    from pvraft_b200 import Graph, graph as G
-
-    def from_oracle(pcloud, k):
-        b, n, _ = pcloud.shape
-        og = O.construct_graph(pcloud.detach().float().cpu(), k)
-        nbr = (og.edges.reshape(b, n, k) - (torch.arange(b) * n).view(b, 1, 1)).to(torch.int32).to(pcloud.device)
-        rel = og.edge_feats.reshape(b, n, k, 3).to(pcloud.device).contiguous()
-        if torch.is_grad_enabled() and pcloud.requires_grad:
-            rel = G.edge_feats(pcloud.float(), nbr, rel)
-        return Graph(nbr, rel, k, [b * n, b * n])
-
-    orig = G.Graph.__dict__['construct_graph']
-    G.Graph.construct_graph = staticmethod(from_oracle)
-    try:
-        yield
-    finally:
-        G.Graph.construct_graph = orig
-
-
 @pytest.mark.parametrize('n1, n2, k', [(1024, 1024, 128), (384, 640, 64), (1000, 1000, 128)])
 def test_rsf_input_gradients_match_oracle(dev, n1, n2, k):
     """A 3-iteration step at B = 2: with trainable weights every parameter and both clouds, with frozen weights both clouds

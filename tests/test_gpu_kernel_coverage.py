@@ -29,6 +29,7 @@ import torch
 
 from conftest import default_weights, rel_err
 from oracle import pvraft_oracle as O
+from train_helpers import randomise_affine
 
 pytestmark = pytest.mark.gpu
 
@@ -622,21 +623,6 @@ def test_knn_branch_instantiation_follows_the_slope(dev):
             want = ('<false>', 'ILb0E') if slope > 1 else ('<true>', 'ILb1E')    # demangled or mangled name
             assert names and all(any(w in nm for w in want) for nm in names), (slope, host, names)
     print('knn_branch kernels by slope:', seen)
-
-
-def randomise_affine(model, seed, slopes):
-    """GroupNorm affines drawn at random (some negative scales), as tests/golden/make_golden.py does, and the two PReLU slopes
-    of the correlation block (out_conv.2, knn_conv.2) set to `slopes`."""
-    g = torch.Generator().manual_seed(seed)
-    with torch.no_grad():
-        for name, p in model.named_parameters():
-            if '.gn' in name or 'out_conv.1.' in name or 'knn_conv.1.' in name:
-                if name.endswith('weight'):
-                    p.copy_(torch.randn(p.shape, generator=g) * 0.5 + 0.8)
-                else:
-                    p.copy_(torch.randn(p.shape, generator=g) * 0.2)
-        model.corr_block.out_conv[2].weight.fill_(slopes[0])
-        model.corr_block.knn_conv[2].weight.fill_(slopes[1])
 
 
 @pytest.mark.parametrize('slopes', [(-0.3, 1.7), (1.7, -0.3)])

@@ -15,7 +15,7 @@ import torch
 
 from conftest import default_weights, rel_err
 from oracle import pvraft_oracle as O
-from test_gpu_train import compare_grads, oracle_adjacency
+from train_helpers import compare_grads, oracle_adjacency
 
 pytestmark = pytest.mark.gpu
 

@@ -7,7 +7,6 @@ autograd through the CPU oracle.  Tolerances (max-abs difference / max-abs refer
 (the per-tensor bound is looser because discrete routing decisions -- arg-max over the 32 neighbours, the sign of the L1 loss at
 flow = target, top-K membership at near-ties -- may flip between two fp32 evaluations and move a gradient contribution).
 """
-import contextlib
 import types
 
 import pytest
@@ -16,6 +15,7 @@ import torch.nn.functional as F
 
 from conftest import default_weights, rel_err
 from oracle import pvraft_oracle as O
+from train_helpers import compare_grads, oracle_adjacency, sequence_loss
 
 pytestmark = pytest.mark.gpu
 
@@ -238,49 +238,6 @@ def test_corr_init_fn_backward(dev, b, n, c, k):
 # ----------------------------------------------------------------------------------------------------------------------
 # whole model
 # ----------------------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def oracle_adjacency():
-    """kNN ties at the 32nd distance are either-valid (SURVEY H1): compare gradients on the oracle's adjacency."""
-    from pvraft_b200 import Graph, graph as G
-
-    def from_oracle(pcloud, k):
-        b, n, _ = pcloud.shape
-        og = O.construct_graph(pcloud.detach().cpu(), k)
-        nbr = (og.edges.reshape(b, n, k) - (torch.arange(b) * n).view(b, 1, 1)).to(torch.int32)
-        return Graph(nbr.to(pcloud.device), og.edge_feats.reshape(b, n, k, 3).to(pcloud.device).contiguous(), k, [b * n, b * n])
-
-    orig = G.Graph.__dict__['construct_graph']
-    G.Graph.construct_graph = staticmethod(from_oracle)
-    try:
-        yield
-    finally:
-        G.Graph.construct_graph = orig
-
-
-def sequence_loss(flows, gt, gamma=0.8):
-    """tools/loss.py:4-13 with an all-ones mask: sum_i gamma^(n-i-1) * mean |flow_i - gt| (compute_loss, loss.py:16-40)."""
-    n = len(flows)
-    return sum(gamma ** (n - i - 1) * (flows[i] - gt).abs().sum(-1).mean() for i in range(n))
-
-
-def compare_grads(got, want, tol_l2, tol_max):
-    worst_l2, worst_max, dot, na, nb = ('', 0.0), ('', 0.0), 0.0, 0.0, 0.0
-    for k, w in want.items():
-        a, w = got[k].double().cpu(), w.double()
-        assert a.shape == w.shape, k
-        e2 = float((a - w).norm() / w.norm().clamp_min(1e-30))
-        em = float((a - w).abs().max() / w.abs().max().clamp_min(1e-30))
-        worst_l2 = (k, e2) if e2 > worst_l2[1] else worst_l2
-        worst_max = (k, em) if em > worst_max[1] else worst_max
-        dot += float((a * w).sum()); na += float((a * a).sum()); nb += float((w * w).sum())
-    cos = dot / (na * nb) ** 0.5
-    print(f'gradient parity over {len(want)} tensors: worst relative L2 {worst_l2[0]} {worst_l2[1]:.2e}, worst max-abs/max-abs '
-          f'{worst_max[0]} {worst_max[1]:.2e}, cosine of the full gradient {cos:.8f}')
-    assert worst_l2[1] < tol_l2, worst_l2
-    assert worst_max[1] < tol_max, worst_max
-    assert cos > 0.99999, cos
-
-
 def test_rsf_gradients_match_oracle(dev):
     """SURVEY 8c item 4: a 3-iteration training step, N=1024, B=2 -- every one of the 95 parameters."""
     from pvraft_b200 import RSF

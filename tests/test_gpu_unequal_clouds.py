@@ -20,7 +20,8 @@ from conftest import load_golden, rel_err
 import unequal_oracle as U
 from oracle import pvraft_oracle as O
 from test_gpu_large_clouds import same_bits
-from test_gpu_train import compare_grads, leaf, oracle_adjacency, sequence_loss
+from test_gpu_train import leaf
+from train_helpers import compare_grads, oracle_adjacency, sequence_loss
 
 pytestmark = pytest.mark.gpu
 
