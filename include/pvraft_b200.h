@@ -611,6 +611,44 @@ PVRAFT_API int pvraft_flow_smooth_bwd(const float* f, const int32_t* nbr, const 
                                       void* det_workspace, void* stream);
 PVRAFT_API int64_t pvraft_flow_smooth_bwd_det_workspace_bytes(int S, int N);
 
+/* The Laplacian regularity term of the self-supervised loss (PointPWC-Net's third term): the local shape of W = P1 + flow
+ * should match the local shape of P2 around the same place.  Same sample stacking as above (sample s pairs with batch entry
+ * s % B); graphs are int32 local ids of k_lap neighbours that include the point itself (pvraft_knn_fwd, mode 0); squared
+ * distances in the difference form of pvraft_chamfer_fwd.  Null pointers, S < 1, B < 1, S % B != 0, N < 1, M < 1, k_lap
+ * outside 2..min(32, N) and k_int outside 1..min(8, M) return PVRAFT_ERR_BAD_ARG before any launch.
+ *   pvraft_cloud_laplacian_fwd: x [B,N,3], nbr [B,N,k] (2 <= k <= min(32, N))
+ *       -> out [B,N,3]: L(x)_i = sum_e (x[nbr[i,e]] - x_i) / (k - 1), fp32 summed in edge order (a self edge adds 0).  Every
+ *          output is written once: no det_workspace.
+ *   pvraft_cloud_laplacian_bwd: g_l [B,N,3] -> d_x [B,N,3] (ACCUMULATED, zeroed by the caller): c = g_l[i] / (k - 1),
+ *       d_x[nbr[i,e]] += c for every edge with nbr[i,e] != i, d_x[i] -= c per such edge.
+ *   pvraft_laplacian_fwd: w [S,N,3] (W), p2 [B,M,3], l2 [B,M,3] (pvraft_cloud_laplacian_fwd of p2 over its own graph),
+ *       g1 [B,N,k_lap] (P1's graph)
+ *       -> nn_idx [S,N,k_int] int32: the k_int nearest of w[s,i] in p2[s%B] ranked on (||w_i - p2_j||^2, j), nearest first
+ *          (an unfilled slot, possible only with non-finite coordinates, reads -1);
+ *          res [S,N,3]: Lhat_i - L(w)_i with Lhat_i = sum_r w_r l2[j_r] / sum_r w_r, w_r = 1 / (d_r + 1e-8) on the SQUARED
+ *          distance d_r (fp32, nearest first), and L(w) over g1;
+ *          acc [S] double (ZEROED by the caller) += sum_i ||res_i||^2, each point's term in double:  R_s = acc[s] / N.
+ *          A brute-force search of S N M pairs.
+ *   pvraft_laplacian_bwd: g [S] the DEVICE upstream gradient of R_s, the forward's nn_idx and res, neighbours held fixed;
+ *       e_i = 2 g_s / N res_i ->
+ *          d_w [S,N,3]: -e_i/(k_lap-1) at every neighbour j != i of g1(i) and +e_i/(k_lap-1) per such edge at i, plus at i
+ *          sum_r (dLhat/dd_r . e_i) 2 (w_i - p2_{j_r}) with dLhat/dd_r = -(w_r / sum w)^2 sum_q w_q (l2_{j_r} - l2_{j_q});
+ *          d_p2 [B,M,3] (or NULL): the negated distance terms at p2_{j_r};  d_l2 [B,M,3] (or NULL): (w_r / sum w) e_i at j_r.
+ *          All ACCUMULATED, zeroed by the caller; d_l2 reaches p2 through pvraft_cloud_laplacian_bwd.
+ * Accumulation: acc in double atomics, the gradients in fp32 atomics (order varies run to run); with a det_workspace all in
+ * the fixed-point form ("Deterministic mode"). */
+PVRAFT_API int pvraft_cloud_laplacian_fwd(const float* x, const int32_t* nbr, int B, int N, int k, float* out, void* stream);
+PVRAFT_API int pvraft_cloud_laplacian_bwd(const float* g_l, const int32_t* nbr, int B, int N, int k, float* d_x, void* det_workspace,
+                                          void* stream);
+PVRAFT_API int64_t pvraft_cloud_laplacian_bwd_det_workspace_bytes(int B, int N);
+PVRAFT_API int pvraft_laplacian_fwd(const float* w, const float* p2, const float* l2, const int32_t* g1, int S, int B, int N, int M, int k_lap,
+                                    int k_int, int32_t* nn_idx, float* res, double* acc, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_laplacian_fwd_det_workspace_bytes(int S);
+PVRAFT_API int pvraft_laplacian_bwd(const float* w, const float* p2, const float* l2, const int32_t* g1, const int32_t* nn_idx, const float* res,
+                                    const float* g, int S, int B, int N, int M, int k_lap, int k_int, float* d_w, float* d_p2, float* d_l2,
+                                    void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_laplacian_bwd_det_workspace_bytes(int S, int B, int N, int M);
+
 /* Flow propagation along a scan sequence (no counterpart in the reference, which estimates one pair at a time): carries a
  * flow defined on one cloud onto the points of another, the warm start of the next pair under a constant-velocity
  * assumption (pvraft_b200.stream.SceneFlowStream).

@@ -142,7 +142,15 @@ _SIGNATURES = {
     'pvraft_flow_smooth_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
     'pvraft_flow_smooth_bwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_flow_smooth_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_flow_propagate_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_cloud_laplacian_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP]),
+    'pvraft_cloud_laplacian_bwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_cloud_laplacian_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
+    'pvraft_laplacian_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP]),
+    'pvraft_laplacian_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_laplacian_bwd': (C.c_int, [VP, VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP,
+                                       VP]),
+    'pvraft_laplacian_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    'pvraft_flow_propagate_fwd':(C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_sizeof': (C.c_int, [C.c_int]),
     'pvraft_transpose_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, VP]),
 }

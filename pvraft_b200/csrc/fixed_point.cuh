@@ -61,6 +61,13 @@ __device__ __forceinline__ void fx_atomic(unsigned long long* slot, const Fx& v)
 
 __device__ __forceinline__ void fx_atomic(unsigned long long* slot, double v) { fx_atomic(slot, fx_from(v)); }
 
+// dst[i] += v: an fp32 atomic, or (DET) an exact addition into slot i of the fixed-point workspace dst
+template <bool DET>
+__device__ __forceinline__ void scatter_add(float* dst, long long i, float v) {
+    if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dst) + i * kFxWords, (double)v);
+    else atomicAdd(dst + i, v);
+}
+
 __device__ __forceinline__ double fx_value(const unsigned long long* slot) {
     if (slot[2]) return __longlong_as_double(0x7ff8000000000000ll);
     unsigned long long lo = slot[0], hi = slot[1];
@@ -89,5 +96,13 @@ int fx_flush_f32(const unsigned long long* acc, long long rows, long long cols, 
 
 // grid caps of the deterministic instantiations: constants, so that the rows a CTA or thread sums depend on the shapes only
 constexpr long long kDetCtas = 256;
+
+// CTAs of 256 threads for a grid-stride scatter over `items`: capped by kDetCtas in the deterministic form, by 8 per SM
+// otherwise
+inline long long scatter_blocks(long long items, bool det) {
+    long long blocks = (items + 255) / 256;
+    const long long cap = det ? kDetCtas : (long long)sm_count() * 8;
+    return blocks > cap ? cap : blocks;
+}
 
 }  // namespace pvraft

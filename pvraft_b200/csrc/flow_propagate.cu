@@ -25,25 +25,6 @@ constexpr int kPrMaxK = 8;
 constexpr int kPrNone = 0x7fffffff;                    // index of an unfilled slot: loses every (distance, index) tie
 static_assert(kPrTile == kPrThreads, "each thread stages one point per tile");
 
-// insert (d, j) into the ascending list best / arg of length K; the caller has checked d < best[K - 1]
-template <int K>
-__device__ __forceinline__ void kbest_insert(float (&best)[K], int (&arg)[K], float d, int j) {
-#pragma unroll
-    for (int i = K - 1; i > 0; --i) {
-        if (best[i - 1] > d) {
-            best[i] = best[i - 1];
-            arg[i] = arg[i - 1];
-        } else if (best[i] > d) {
-            best[i] = d;
-            arg[i] = j;
-        }
-    }
-    if (best[0] > d) {
-        best[0] = d;
-        arg[0] = j;
-    }
-}
-
 // xyz_prev, flow_prev [B,M,3], xyz [B,N,3] -> flow_out [B,N,3], idx_out [B,N,K] (or NULL); grid (ceil(N / kPrPerCta), B)
 template <int K>
 __global__ void __launch_bounds__(kPrThreads) k_flow_propagate(const float* __restrict__ xyz_prev, const float* __restrict__ flow_prev,

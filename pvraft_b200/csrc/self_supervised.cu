@@ -111,12 +111,6 @@ __global__ void __launch_bounds__(kNnThreads) k_chamfer_nn(const float* __restri
     }
 }
 
-template <bool DET>
-__device__ __forceinline__ void scatter_add(float* dst, long long i, float v) {
-    if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dst) + i * kFxWords, (double)v);
-    else atomicAdd(dst + i, v);
-}
-
 // Items [0, S*N): d_a[s,i] += v, d_b[s%B, nn_ab] -= v with v = 2 g_s / N (a_i - b_nn); items [S*N, S*N + S*M):
 // d_a[s, nn_ba] += v, d_b[s%B, j] -= v with v = 2 g_s / M (a_nn - b_j).  d_b may be NULL.  DET: d_a and d_b are the
 // fixed-point workspaces; every value added is one item's.
@@ -207,12 +201,6 @@ __global__ void __launch_bounds__(256) k_flow_smooth_bwd(const float* __restrict
 }
 
 static bool bad_batch(int S, int B, int N) { return S < 1 || B < 1 || S % B != 0 || N < 1; }
-
-static long long scatter_blocks(long long items, bool det) {
-    long long blocks = (items + 255) / 256;
-    const long long cap = det ? kDetCtas : (long long)sm_count() * 8;
-    return blocks > cap ? cap : blocks;
-}
 
 }  // namespace pvraft
 

@@ -781,6 +781,84 @@ def flow_smooth_bwd(f, nbr, g):
     return d_f
 
 
+LAPLACIAN_MAX_K_INT = 8   # neighbours pvraft_laplacian_fwd interpolates from at most
+
+
+def _graph_args(what, x, nbr):
+    """x [B,N,3], nbr [B,N,k] int32 with 2 <= k <= min(32, N): the rules of the Laplacian graphs."""
+    if x.dim() != 3 or x.shape[-1] != 3 or x.shape[0] < 1 or x.shape[1] < 1:
+        raise ValueError(f'{what}: expected [B,N,3], got {tuple(x.shape)}')
+    if nbr.dim() != 3 or tuple(nbr.shape[:2]) != tuple(x.shape[:2]) or not 2 <= nbr.shape[2] <= min(KNN, x.shape[1]):
+        raise ValueError(f'{what}: expected nbr [{x.shape[0]},{x.shape[1]},k] with 2 <= k <= min({KNN}, N), got {tuple(nbr.shape)}')
+    return int(x.shape[0]), int(x.shape[1]), int(nbr.shape[2])
+
+
+def cloud_laplacian(x, nbr):
+    """x [B,N,3], nbr [B,N,k] int32 (a kNN graph that includes each point) -> L(x) [B,N,3],
+    L(x)_i = sum_e (x[nbr[i,e]] - x_i) / (k - 1)."""
+    b, n, k = _graph_args('cloud_laplacian', x, nbr)
+    out = torch.empty_like(x)
+    _count(lib().pvraft_cloud_laplacian_fwd(_p(x), _p(nbr, torch.int32), b, n, k, _p(out), _stream()), 'cloud_laplacian_fwd')
+    return out
+
+
+def cloud_laplacian_bwd(g_l, nbr, d_x):
+    """d_x [B,N,3] += the gradient of L(x) (cloud_laplacian) for the upstream gradient g_l [B,N,3]; returns d_x."""
+    b, n, k = _graph_args('cloud_laplacian_bwd', g_l, nbr)
+    if d_x.shape != g_l.shape:
+        raise ValueError(f'cloud_laplacian_bwd: d_x {tuple(d_x.shape)} does not match g_l {tuple(g_l.shape)}')
+    ws = _det_workspace(lib().pvraft_cloud_laplacian_bwd_det_workspace_bytes, b, n, device=g_l.device)
+    _count(lib().pvraft_cloud_laplacian_bwd(_p(g_l), _p(nbr, torch.int32), b, n, k, _p(d_x), _p(ws, torch.uint8), _stream()),
+           'cloud_laplacian_bwd')
+    return d_x
+
+
+def _laplacian_args(what, w, p2, l2, g1, k_int):
+    if p2.dim() != 3 or p2.shape[-1] != 3 or l2.shape != p2.shape:
+        raise ValueError(f'{what}: expected p2 and l2 [B,M,3], got {tuple(p2.shape)} and {tuple(l2.shape)}')
+    bb, m = int(p2.shape[0]), int(p2.shape[1])
+    _loss_batch(what, w, bb, m)
+    s, n = int(w.shape[0]), int(w.shape[1])
+    if g1.dim() != 3 or tuple(g1.shape[:2]) != (bb, n) or not 2 <= g1.shape[2] <= min(KNN, n):
+        raise ValueError(f'{what}: expected g1 [{bb},{n},k_lap] with 2 <= k_lap <= min({KNN}, N), got {tuple(g1.shape)}')
+    if isinstance(k_int, bool) or not isinstance(k_int, int) or not 1 <= k_int <= min(LAPLACIAN_MAX_K_INT, m):
+        raise ValueError(f'{what}: k_int={k_int!r} must be an integer in 1..min({LAPLACIAN_MAX_K_INT}, M={m})')
+    return s, bb, n, m, int(g1.shape[2])
+
+
+def laplacian(w, p2, l2, g1, k_int):
+    """w [S,N,3] (the first clouds moved by the flows), p2 [B,M,3] and its Laplacian l2 = cloud_laplacian(p2, g2), g1 [B,N,k_lap]
+    (the first cloud's graph; sample s uses entry s % B) -> (acc [S] f64: sum_i ||Lhat_i - L(w)_i||^2 with Lhat_i the
+    inverse-squared-distance interpolation of l2 over the k_int nearest points of p2; nn_idx [S,N,k_int] int32, nearest first,
+    lowest index on ties; res [S,N,3] = Lhat - L(w)).  R_s = acc[s] / N."""
+    s, bb, n, m, kl = _laplacian_args('laplacian', w, p2, l2, g1, k_int)
+    acc = torch.zeros(s, dtype=torch.float64, device=w.device)
+    nn_idx = torch.empty(s, n, k_int, dtype=torch.int32, device=w.device)
+    res = torch.empty_like(w)
+    ws = _det_workspace(lib().pvraft_laplacian_fwd_det_workspace_bytes, s, device=w.device)
+    _count(lib().pvraft_laplacian_fwd(_p(w), _p(p2), _p(l2), _p(g1, torch.int32), s, bb, n, m, kl, k_int, _p(nn_idx, torch.int32), _p(res),
+                                      _p(acc, torch.float64), _p(ws, torch.uint8), _stream()), 'laplacian_fwd')
+    return acc, nn_idx, res
+
+
+def laplacian_bwd(w, p2, l2, g1, nn_idx, res, g, want_dp2=True):
+    """Gradients of R_s = acc[s] / N (laplacian) with nn_idx held fixed, for the upstream gradient g [S] (on the device) ->
+    (d_w [S,N,3], d_p2 [B,M,3] (the distance part; None unless want_dp2), d_l2 [B,M,3] (None unless want_dp2)).  d_l2 reaches p2
+    through cloud_laplacian_bwd."""
+    s, bb, n, m, kl = _laplacian_args('laplacian_bwd', w, p2, l2, g1, int(nn_idx.shape[-1]) if nn_idx.dim() == 3 else -1)
+    if tuple(nn_idx.shape[:2]) != (s, n) or res.shape != w.shape:
+        raise ValueError(f'laplacian_bwd: nn_idx {tuple(nn_idx.shape)} and res {tuple(res.shape)} do not match w {tuple(w.shape)}')
+    if g.shape != (s,):
+        raise ValueError(f'laplacian_bwd: expected g [{s}], got {tuple(g.shape)}')
+    d_w = torch.zeros_like(w)
+    d_p2 = torch.zeros_like(p2) if want_dp2 else None
+    d_l2 = torch.zeros_like(p2) if want_dp2 else None
+    ws = _det_workspace(lib().pvraft_laplacian_bwd_det_workspace_bytes, s, bb, n, m, device=w.device)
+    _count(lib().pvraft_laplacian_bwd(_p(w), _p(p2), _p(l2), _p(g1, torch.int32), _p(nn_idx, torch.int32), _p(res), _p(g), s, bb, n, m, kl,
+                                      int(nn_idx.shape[-1]), _p(d_w), _p(d_p2), _p(d_l2), _p(ws, torch.uint8), _stream()), 'laplacian_bwd')
+    return d_w, d_p2, d_l2
+
+
 PROPAGATE_MAX_K = 8   # neighbours pvraft_flow_propagate_fwd averages over at most
 
 
