@@ -473,8 +473,9 @@ PVRAFT_API int pvraft_flow_out_fwd(const pvraft_flowout_args* a, void* stream);
  * with q.x = fma(qz,xz, fma(qy,xy, qx*xx)) and |.|^2 = (x*x+y*y)+z*z.  1 <= k <= 32, N >= k.
  * Ties at the k-th place: lowest candidate id.
  * workspace: pvraft_knn_workspace_bytes(B, N) bytes of device scratch (16-byte aligned) enable the
- * uniform-grid search (N <= 16384); with workspace == NULL (or larger N) the brute-force kernel runs.  Both
- * return the same set.
+ * uniform-grid search for N >= 64 (the index sorted in shared memory up to N = 16384, by pvraft_grid_index_fwd's
+ * counting sort above); with workspace == NULL (or N < 64) the brute-force kernel runs.  Both return the same
+ * neighbours in the same order.
  * --------------------------------------------------------------------------------------------- */
 PVRAFT_API int64_t pvraft_knn_workspace_bytes(int B, int N);
 PVRAFT_API int pvraft_knn_fwd(const float* xyz, const float* query, int B, int N, int S, int k, int mode, int32_t* idx,
@@ -485,6 +486,19 @@ PVRAFT_API int pvraft_knn_fwd(const float* xyz, const float* query, int B, int N
  * RAFT driver uses it to make the SetConv gathers of consecutive points overlap in L1/L2.  64 <= N <= 16384;
  * workspace: pvraft_knn_workspace_bytes(B, N) bytes. */
 PVRAFT_API int pvraft_point_order_fwd(const float* xyz, int B, int N, int32_t* perm, void* workspace, void* stream);
+
+/* Uniform-grid index of S clouds of any size (no counterpart in the reference), the search structure of the kNN graphs
+ * beyond 16384 points and of the *_grid_fwd searches below.  Built on the device with no host synchronisation (capturable):
+ * per sample the bounding box, cells of edge h ~ cbrt(3 * volume / N) (at most max(32768, N) cells and 1024 along an axis),
+ * and the points counting-sorted by cell id.
+ *   xyz [S,N,3], offset [S,N,3] or NULL: the index is of xyz + offset (one fp32 add per coordinate), e.g. W = P + flow.
+ *   workspace: pvraft_grid_index_workspace_bytes(S, N) bytes, 16-byte aligned; it holds, every block 16-byte aligned:
+ *   float4 pts[S*N] (x, y, z, |p|^2 in cell order) | int32 ids[S*N] (the original ids) | int32 key[S*N] | int32 rank[S*N] |
+ *   int32 cell_start[S * (cells + 1)] | per-sample grid parameters | scratch.  The order of the points inside a cell varies
+ *   from run to run (an atomic histogram); every search on the index ranks on (distance, id), so its results do not.
+ * Null pointers, S or N < 1 return PVRAFT_ERR_BAD_ARG, S > 65535 PVRAFT_ERR_UNSUPPORTED. */
+PVRAFT_API int64_t pvraft_grid_index_workspace_bytes(int S, int N);
+PVRAFT_API int pvraft_grid_index_fwd(const float* xyz, const float* offset, int S, int N, void* workspace, void* stream);
 
 /* ================================================================================================
  * Gradient contract (SURVEY.md section 8b): what tools/engine.py:131-147 differentiates through.
@@ -603,6 +617,13 @@ PVRAFT_API int pvraft_chamfer_fwd(const float* a, const float* b, int S, int B, 
 PVRAFT_API int64_t pvraft_chamfer_fwd_det_workspace_bytes(int S);
 PVRAFT_API int pvraft_chamfer_bwd(const float* a, const float* b, const int32_t* nn_ab, const int32_t* nn_ba, const float* g, int S, int B,
                                   int N, int M, float* d_a, float* d_b, void* det_workspace, void* stream);
+/* The same pvraft_chamfer_fwd results (nn_ab, nn_ba bitwise; acc up to summation order) from a search on uniform-grid
+ * indices of b and of a instead of 2 S N M pairs.  workspace: pvraft_chamfer_grid_workspace_bytes(S, B, N, M) bytes,
+ * 16-byte aligned (the indices: pvraft_grid_index_workspace_bytes(B, M) + pvraft_grid_index_workspace_bytes(S, N));
+ * det_workspace: pvraft_chamfer_fwd_det_workspace_bytes(S) bytes or NULL. */
+PVRAFT_API int64_t pvraft_chamfer_grid_workspace_bytes(int S, int B, int N, int M);
+PVRAFT_API int pvraft_chamfer_grid_fwd(const float* a, const float* b, int S, int B, int N, int M, int32_t* nn_ab, int32_t* nn_ba,
+                                       double* acc, void* workspace, void* det_workspace, void* stream);
 PVRAFT_API int64_t pvraft_chamfer_bwd_det_workspace_bytes(int S, int B, int N, int M);
 PVRAFT_API int pvraft_flow_smooth_fwd(const float* f, const int32_t* nbr, int S, int B, int N, int k, double* acc, void* det_workspace,
                                       void* stream);
@@ -644,6 +665,12 @@ PVRAFT_API int64_t pvraft_cloud_laplacian_bwd_det_workspace_bytes(int B, int N);
 PVRAFT_API int pvraft_laplacian_fwd(const float* w, const float* p2, const float* l2, const int32_t* g1, int S, int B, int N, int M, int k_lap,
                                     int k_int, int32_t* nn_idx, float* res, double* acc, void* det_workspace, void* stream);
 PVRAFT_API int64_t pvraft_laplacian_fwd_det_workspace_bytes(int S);
+/* The same pvraft_laplacian_fwd results (nn_idx and res bitwise; acc up to summation order) from a search on a uniform-grid
+ * index of p2.  workspace: pvraft_grid_index_workspace_bytes(B, M) bytes, 16-byte aligned; det_workspace:
+ * pvraft_laplacian_fwd_det_workspace_bytes(S) bytes or NULL. */
+PVRAFT_API int pvraft_laplacian_grid_fwd(const float* w, const float* p2, const float* l2, const int32_t* g1, int S, int B, int N, int M,
+                                         int k_lap, int k_int, int32_t* nn_idx, float* res, double* acc, void* workspace,
+                                         void* det_workspace, void* stream);
 PVRAFT_API int pvraft_laplacian_bwd(const float* w, const float* p2, const float* l2, const int32_t* g1, const int32_t* nn_idx, const float* res,
                                     const float* g, int S, int B, int N, int M, int k_lap, int k_int, float* d_w, float* d_p2, float* d_l2,
                                     void* det_workspace, void* stream);
@@ -663,6 +690,11 @@ PVRAFT_API int64_t pvraft_laplacian_bwd_det_workspace_bytes(int S, int B, int N,
  * outside 1..min(8, M) return PVRAFT_ERR_BAD_ARG before any launch. */
 PVRAFT_API int pvraft_flow_propagate_fwd(const float* xyz_prev, const float* flow_prev, const float* xyz, int B, int M, int N, int k,
                                          float* flow_out, int32_t* idx_out, void* stream);
+/* The same pvraft_flow_propagate_fwd results, bitwise, from a search on a uniform-grid index of W = xyz_prev + flow_prev
+ * (built with flow_prev as its offset: the same fp32 add).  workspace: pvraft_grid_index_workspace_bytes(B, M) bytes,
+ * 16-byte aligned.  No det_workspace, for the same reason. */
+PVRAFT_API int pvraft_flow_propagate_grid_fwd(const float* xyz_prev, const float* flow_prev, const float* xyz, int B, int M, int N, int k,
+                                              float* flow_out, int32_t* idx_out, void* workspace, void* stream);
 
 /* sizeof() of the argument structs as compiled into the library (0 = linear, 1 = corrfeat, 2 = gru, 3 = flowout,
  * 4 = tc_linear, 5 = knn_branch, 6 = update_chain; -1 otherwise): lets a foreign-language binding verify its struct layout

@@ -151,6 +151,13 @@ _SIGNATURES = {
                                        VP]),
     'pvraft_laplacian_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     'pvraft_flow_propagate_fwd':(C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
+    'pvraft_flow_propagate_grid_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
+    'pvraft_grid_index_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
+    'pvraft_grid_index_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, VP, VP]),
+    'pvraft_chamfer_grid_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    'pvraft_chamfer_grid_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_laplacian_grid_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP,
+                                            VP]),
     'pvraft_sizeof': (C.c_int, [C.c_int]),
     'pvraft_transpose_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, VP]),
 }

@@ -11,7 +11,7 @@
 // index order, so a strict comparison keeps the (distance, index) order.  At the end the eight lists of a query are merged
 // on (distance, index) in shared memory by one thread, which also forms the weighted mean, nearest first.  There are no
 // atomics and no reduction whose order depends on timing: the result is a function of the inputs.
-#include "nn_search.cuh"
+#include "grid_index.cuh"
 
 namespace pvraft {
 
@@ -24,6 +24,31 @@ constexpr int kPrSlice = kPrTile / kPrWarps;           // points of a tile each 
 constexpr int kPrMaxK = 8;
 constexpr int kPrNone = 0x7fffffff;                    // index of an unfilled slot: loses every (distance, index) tie
 static_assert(kPrTile == kPrThreads, "each thread stages one point per tile");
+
+// The per-query step after the search, shared by k_flow_propagate and k_flow_propagate_grid: from the k nearest (nd, nx) of
+// a query, nearest first, write its flow and neighbours at row `row`.
+// w_j = 1 / (sqrt(d_j) + 1e-8); flow = sum_j w_j flow_prev[j] / sum_j w_j, summed nearest first.  An unfilled slot (only
+// possible when non-finite coordinates leave fewer than K comparable points) contributes nothing and reads back as -1.
+template <int K>
+__device__ __forceinline__ void propagate_point(const float (&nd)[K], const int (&nx)[K], const float* fp, int M, long long row,
+                                                float* flow_out, int32_t* idx_out) {
+    float sw = 0.f, sx = 0.f, sy = 0.f, sz = 0.f;
+#pragma unroll
+    for (int r = 0; r < K; ++r) {
+        const int j = nx[r];
+        const bool ok = j < M;
+        if (idx_out) idx_out[row * K + r] = ok ? j : -1;
+        if (!ok) continue;
+        const float w = __fdiv_rn(1.f, __fadd_rn(__fsqrt_rn(nd[r]), 1e-8f));
+        sx = __fadd_rn(sx, __fmul_rn(w, __ldg(fp + 3ll * j)));
+        sy = __fadd_rn(sy, __fmul_rn(w, __ldg(fp + 3ll * j + 1)));
+        sz = __fadd_rn(sz, __fmul_rn(w, __ldg(fp + 3ll * j + 2)));
+        sw = __fadd_rn(sw, w);
+    }
+    flow_out[3 * row] = __fdiv_rn(sx, sw);
+    flow_out[3 * row + 1] = __fdiv_rn(sy, sw);
+    flow_out[3 * row + 2] = __fdiv_rn(sz, sw);
+}
 
 // xyz_prev, flow_prev [B,M,3], xyz [B,N,3] -> flow_out [B,N,3], idx_out [B,N,K] (or NULL); grid (ceil(N / kPrPerCta), B)
 template <int K>
@@ -134,31 +159,48 @@ __global__ void __launch_bounds__(kPrThreads) k_flow_propagate(const float* __re
             }
     }
 
-    // w_j = 1 / (sqrt(d_j) + 1e-8); flow = sum_j w_j flow_prev[j] / sum_j w_j, summed nearest first.  An unfilled slot (only
-    // possible when non-finite coordinates leave fewer than K comparable points) contributes nothing and reads back as -1.
-    float sw = 0.f, sx = 0.f, sy = 0.f, sz = 0.f;
-    const long long row = (long long)b * N + q;
-#pragma unroll
-    for (int r = 0; r < K; ++r) {
-        const int j = nx[r];
-        const bool ok = j < M;
-        if (idx_out) idx_out[row * K + r] = ok ? j : -1;
-        if (!ok) continue;
-        const float w = __fdiv_rn(1.f, __fadd_rn(__fsqrt_rn(nd[r]), 1e-8f));
-        sx = __fadd_rn(sx, __fmul_rn(w, __ldg(fp + 3ll * j)));
-        sy = __fadd_rn(sy, __fmul_rn(w, __ldg(fp + 3ll * j + 1)));
-        sz = __fadd_rn(sz, __fmul_rn(w, __ldg(fp + 3ll * j + 2)));
-        sw = __fadd_rn(sw, w);
-    }
-    flow_out[3 * row] = __fdiv_rn(sx, sw);
-    flow_out[3 * row + 1] = __fdiv_rn(sy, sw);
-    flow_out[3 * row + 2] = __fdiv_rn(sz, sw);
+    propagate_point<K>(nd, nx, fp, M, (long long)b * N + q, flow_out, idx_out);
 }
 
 template <int K>
 static void launch_propagate(dim3 grid, cudaStream_t st, const float* xyz_prev, const float* flow_prev, const float* xyz, int M, int N,
                              float* flow_out, int32_t* idx_out) {
     k_flow_propagate<K><<<grid, kPrThreads, 0, st>>>(xyz_prev, flow_prev, xyz, M, N, flow_out, idx_out);
+}
+
+// The grid form of k_flow_propagate: the same search on the index `ix` of W = xyz_prev + flow_prev (built with flow_prev as
+// its offset, the same fp32 add), the same propagate_point.  One warp per query, kGqPerWarp consecutive queries per warp.
+template <int K>
+__global__ void __launch_bounds__(kGqThreads) k_flow_propagate_grid(const float* __restrict__ flow_prev, const float* __restrict__ xyz, int M, int N,
+                                                                     GridIndex ix, float* __restrict__ flow_out, int32_t* __restrict__ idx_out) {
+    const int b = blockIdx.y;
+    const int q0 = (blockIdx.x * kGqWarps + warp_id()) * kGqPerWarp;
+    if (q0 >= N) return;   // uniform over the warp; no barrier follows
+    const float* fp = flow_prev + (long long)b * M * 3;
+    const float* qp = xyz + (long long)b * N * 3;
+    const float4* P = ix.pts + (long long)b * M;
+    const int32_t* I = ix.ids + (long long)b * M;
+    const int32_t* CS = ix.cell_start + (long long)b * (ix.cells + 1);
+    const GridParams gp = ix.params[b];
+    for (int q = q0; q < min(q0 + kGqPerWarp, N); ++q) {
+        float bd;
+        int bi;
+        grid_knn_diff(P, I, CS, gp, __ldg(qp + 3ll * q), __ldg(qp + 3ll * q + 1), __ldg(qp + 3ll * q + 2), K, bd, bi);
+        float nd[K];
+        int nx[K];
+#pragma unroll
+        for (int r = 0; r < K; ++r) {
+            nd[r] = __shfl_sync(kFull, bd, r);
+            nx[r] = __shfl_sync(kFull, bi, r);
+        }
+        if (lane_id() == 0) propagate_point<K>(nd, nx, fp, M, (long long)b * N + q, flow_out, idx_out);
+    }
+}
+
+template <int K>
+static void launch_propagate_grid(dim3 grid, cudaStream_t st, const float* flow_prev, const float* xyz, int M, int N, const GridIndex& ix,
+                                  float* flow_out, int32_t* idx_out) {
+    k_flow_propagate_grid<K><<<grid, kGqThreads, 0, st>>>(flow_prev, xyz, M, N, ix, flow_out, idx_out);
 }
 
 }  // namespace pvraft
@@ -183,4 +225,27 @@ extern "C" int pvraft_flow_propagate_fwd(const float* xyz_prev, const float* flo
         default: launch_propagate<8>(grid, st, xyz_prev, flow_prev, xyz, M, N, flow_out, idx_out); break;
     }
     return check_launch("flow_propagate_fwd");
+}
+
+extern "C" int pvraft_flow_propagate_grid_fwd(const float* xyz_prev, const float* flow_prev, const float* xyz, int B, int M, int N, int k,
+                                              float* flow_out, int32_t* idx_out, void* workspace, void* stream) {
+    if (!xyz_prev || !flow_prev || !xyz || !flow_out || !workspace || B < 1 || M < 1 || N < 1 || k < 1 || k > kPrMaxK || k > M)
+        return fail(PVRAFT_ERR_BAD_ARG, "flow_propagate_grid_fwd: bad argument");
+    if (B > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "flow_propagate_grid_fwd: B = %d samples (at most 65535)", B);
+    cudaStream_t st = (cudaStream_t)stream;
+    GridIndex ix;
+    const int rc = grid_index_build(xyz_prev, flow_prev, B, M, workspace, st, &ix);
+    if (rc) return rc;
+    const dim3 grid((unsigned)((N + kGqPerCta - 1) / kGqPerCta), (unsigned)B);
+    switch (k) {
+        case 1: launch_propagate_grid<1>(grid, st, flow_prev, xyz, M, N, ix, flow_out, idx_out); break;
+        case 2: launch_propagate_grid<2>(grid, st, flow_prev, xyz, M, N, ix, flow_out, idx_out); break;
+        case 3: launch_propagate_grid<3>(grid, st, flow_prev, xyz, M, N, ix, flow_out, idx_out); break;
+        case 4: launch_propagate_grid<4>(grid, st, flow_prev, xyz, M, N, ix, flow_out, idx_out); break;
+        case 5: launch_propagate_grid<5>(grid, st, flow_prev, xyz, M, N, ix, flow_out, idx_out); break;
+        case 6: launch_propagate_grid<6>(grid, st, flow_prev, xyz, M, N, ix, flow_out, idx_out); break;
+        case 7: launch_propagate_grid<7>(grid, st, flow_prev, xyz, M, N, ix, flow_out, idx_out); break;
+        default: launch_propagate_grid<8>(grid, st, flow_prev, xyz, M, N, ix, flow_out, idx_out); break;
+    }
+    return check_launch("flow_propagate_grid_fwd");
 }

@@ -12,8 +12,9 @@
 //                 slack of the distance formula: a few hundred candidates are scored per query instead of the whole cloud.
 // Distances reproduce the reference's expanded form bit-for-bit on the CPU oracle: |q|^2 and |x|^2 as
 // (x*x+y*y)+z*z, q.x as fma(z,z',fma(y,y',x*x')); ranking is on (distance, original id), so the result does not
-// depend on the visiting order.  Clouds too large for the shared-memory sort fall back to the brute-force kernel.
-#include "common.cuh"
+// depend on the visiting order.  Clouds too large for the shared-memory sort get the same index from the multi-CTA counting
+// sort of grid_index.cu, and the same k_knn_grid searches it, one launch per sample.
+#include "grid_index.cuh"
 
 namespace pvraft {
 
@@ -21,41 +22,10 @@ constexpr int kKnnThreads = 256;
 constexpr int kKnnTile = 2048;      // candidates per shared-memory tile of the brute-force kernel
 constexpr int kSortMaxN = 16384;    // (key, id) pairs of the in-smem sort: 8 B * 16384 = 128 KB
 
-__device__ __forceinline__ float sqnorm(float x, float y, float z) {
-    return __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z));
-}
-
-// (distance, id) ordering: smaller distance first, ties -> smaller id first
-__device__ __forceinline__ bool worse(float d1, int i1, float d2, int i2) { return d1 > d2 || (d1 == d2 && i1 > i2); }
-
 __device__ __forceinline__ float ref_distance(int mode, float qx, float qy, float qz, float qn, const float4 p) {
     const float dot = __fmaf_rn(qz, p.z, __fmaf_rn(qy, p.y, __fmul_rn(qx, p.x)));
     if (mode == 0) return __fsub_rn(__fadd_rn(qn, p.w), __fmul_rn(2.f, dot));   // graph.py:53-57
     return __fadd_rn(__fadd_rn(__fmul_rn(-2.f, dot), qn), p.w);                  // pointconv.py:21-24
-}
-
-// The warp keeps its current k best SORTED across the lanes (lane i = i-th best, lanes >= k hold +inf sentinels), so an
-// insertion is one ballot + one shuffle-up instead of a full warp reduction for the new k-th distance.
-// insert the candidates flagged in `cand` (one per lane: d, id); tau / tau_i = the current k-th (distance, id)
-__device__ __forceinline__ void insert_candidates(unsigned cand, float d, int id, float& bd, int& bi, float& tau, int& tau_i, int k) {
-    const int lane = lane_id();
-    while (cand) {
-        const int src = __ffs(cand) - 1;
-        cand &= cand - 1;
-        const float cd = __shfl_sync(kFull, d, src);
-        const int cid = __shfl_sync(kFull, id, src);
-        if (worse(cd, cid, tau, tau_i)) continue;   // tau may have tightened since the ballot
-        const unsigned behind = __ballot_sync(kFull, worse(bd, bi, cd, cid));   // a suffix of the lanes: they move up by one
-        const float nd = __shfl_up_sync(kFull, bd, 1);
-        const int ni = __shfl_up_sync(kFull, bi, 1);
-        if ((behind >> lane) & 1u) {
-            const bool first = lane == 0 || !((behind >> (lane - 1)) & 1u);
-            bd = first ? cd : nd;
-            bi = first ? cid : ni;
-        }
-        tau = __shfl_sync(kFull, bd, k - 1);
-        tau_i = __shfl_sync(kFull, bi, k - 1);
-    }
 }
 
 __device__ __forceinline__ void write_result(const float* __restrict__ X, float qx, float qy, float qz, int lane, int k, int bi,
@@ -122,18 +92,6 @@ __global__ void __launch_bounds__(kKnnThreads) k_knn(const float* __restrict__ x
 constexpr int kMaxCells = 32768;
 constexpr int kMaxGridDim = 64;
 constexpr float kCellOcc = 3.0f;   // (the time is flat between 1.5 and 16 points per cell: insertions dominate, not the scan)
-
-struct GridParams {      // one per sample, written by k_grid_sort
-    float gmin[3], h[3], inv_h[3];
-    int G[3];
-    float margin;        // absolute safety margin of the face-distance bound (cell assignment is done in fp32)
-    float max_norm;      // largest |p|^2 of the sample (rounding slack of the expanded distance form)
-};
-
-__device__ __forceinline__ int cell_coord(float v, float gmin, float inv_h, int G) {
-    const int c = (int)floorf((v - gmin) * inv_h);
-    return c < 0 ? 0 : (c >= G ? G - 1 : c);
-}
 
 // `morton` != 0: the sort key is the Morton (Z-order) interleave of the cell coordinates instead of the linear cell id, and only
 // `ids` (the permutation) is of interest to the caller: a spatially coherent point order (pvraft_point_order_fwd).
@@ -319,7 +277,8 @@ __global__ void __launch_bounds__(kKnnThreads) k_knn_grid(const float* __restric
 using namespace pvraft;
 
 extern "C" int64_t pvraft_knn_workspace_bytes(int B, int N) {
-    if (B <= 0 || N <= 0 || N > kSortMaxN) return 0;   // brute force needs no workspace
+    if (B <= 0 || N <= 0) return 0;
+    if (N > kSortMaxN) return grid_index_bytes(B, N);
     return (int64_t)B * N * (int64_t)(sizeof(float4) + sizeof(int32_t) + sizeof(unsigned)) +
            (int64_t)B * (kMaxCells + 1) * (int64_t)sizeof(int32_t) + (int64_t)B * (int64_t)sizeof(GridParams) + 512;
 }
@@ -351,6 +310,21 @@ extern "C" int pvraft_knn_fwd(const float* xyz, const float* query, int B, int N
         if ((rc = check_launch("knn grid cells"))) return rc;
         k_knn_grid<<<grid, kKnnThreads, 0, st>>>(xyz, sorted, ids, cell_start, params, query, N, S, k, mode, idx, rel);
         return check_launch("knn grid");
+    }
+    if (workspace && N > kSortMaxN) {
+        // the index of grid_index.cu: its cell_start rows are grid_index_cells(N) + 1 long, not kMaxCells + 1, so k_knn_grid
+        // runs once per sample on that sample's slices (blockIdx.y = 0)
+        GridIndex ix;
+        int rc;
+        if ((rc = grid_index_build(xyz, nullptr, B, N, workspace, st, &ix))) return rc;
+        for (int b = 0; b < B; ++b) {
+            const size_t pts = (size_t)b * N, qs = (size_t)b * S;
+            k_knn_grid<<<dim3(grid.x, 1), kKnnThreads, 0, st>>>(xyz + pts * 3, ix.pts + pts, ix.ids + pts,
+                                                                 ix.cell_start + (size_t)b * (ix.cells + 1), ix.params + b, query + qs * 3, N,
+                                                                 S, k, mode, idx + qs * k, rel ? rel + qs * k * 3 : nullptr);
+            if ((rc = check_launch("knn grid"))) return rc;
+        }
+        return 0;
     }
     k_knn<<<grid, kKnnThreads, 0, st>>>(xyz, query, N, S, k, mode, idx, rel);
     return check_launch("knn");

@@ -23,7 +23,7 @@
 //                  dd_m/dW_i = 2 (W_i - P2_m) = -dd_m/dP2_m.
 //   k_cloud_laplacian_bwd carries dL2 into P2 over G2.
 #include "fixed_point.cuh"
-#include "nn_search.cuh"
+#include "grid_index.cuh"
 
 namespace pvraft {
 
@@ -92,6 +92,37 @@ __global__ void __launch_bounds__(256) k_cloud_laplacian_bwd(const float* __rest
         scatter_add<DET>(d_x, 3 * p + 1, oy);
         scatter_add<DET>(d_x, 3 * p + 2, oz);
     }
+}
+
+// The per-query step of k_laplacian_grid after its search, the same formula, order and rounding as k_laplacian_fwd's (which
+// keeps its own copy, so that its machine code is unchanged): from the k_int nearest (nd, nx) of w_q, nearest first, write
+// nn_idx and the residual of row `row` and return its squared length in double.
+// Lhat = sum_r w_r L2[j_r] / sum_r w_r, summed in fp32 nearest first.  An unfilled slot (only possible when non-finite
+// coordinates leave fewer than K comparable points) contributes nothing and reads back as -1.
+template <int K>
+__device__ __forceinline__ double laplacian_point(const float (&nd)[K], const int (&nx)[K], const float* ws,
+                                                  const float* lp, const int32_t* g1_q, int kl, int M, long long row,
+                                                  int q, int32_t* nn_idx, float* res) {
+    float sw = 0.f, sx = 0.f, sy = 0.f, sz = 0.f;
+#pragma unroll
+    for (int r = 0; r < K; ++r) {
+        const int j = nx[r];
+        const bool ok = j < M;
+        nn_idx[row * K + r] = ok ? j : -1;
+        if (!ok) continue;
+        const float wr = __fdiv_rn(1.f, __fadd_rn(nd[r], 1e-8f));
+        sx = __fadd_rn(sx, __fmul_rn(wr, __ldg(lp + 3ll * j)));
+        sy = __fadd_rn(sy, __fmul_rn(wr, __ldg(lp + 3ll * j + 1)));
+        sz = __fadd_rn(sz, __fmul_rn(wr, __ldg(lp + 3ll * j + 2)));
+        sw = __fadd_rn(sw, wr);
+    }
+    const float3 lw = laplacian_at(ws, g1_q, kl, q);
+    const float rx = __fsub_rn(__fdiv_rn(sx, sw), lw.x), ry = __fsub_rn(__fdiv_rn(sy, sw), lw.y),
+                rz = __fsub_rn(__fdiv_rn(sz, sw), lw.z);
+    res[3 * row] = rx;
+    res[3 * row + 1] = ry;
+    res[3 * row + 2] = rz;
+    return ((double)rx * (double)rx + (double)ry * (double)ry) + (double)rz * (double)rz;
 }
 
 // w [S,N,3], p2 and l2 [B,M,3], g1 [B,N,kl] (sample s uses entry s % B) -> nn_idx [S,N,K], res [S,N,3] = Lhat - L(w),
@@ -237,6 +268,42 @@ __global__ void __launch_bounds__(kLpThreads) k_laplacian_fwd(const float* __res
     }
 }
 
+// The grid form of k_laplacian_fwd: the same search on the index `ix` of p2 (B samples), the same laplacian_point.  One warp
+// per query (kGqPerWarp consecutive queries per warp); lane 0 forms each query's result and sums its queries' terms in order.
+template <int K, bool DET>
+__global__ void __launch_bounds__(kGqThreads) k_laplacian_grid(const float* __restrict__ w, const float* __restrict__ l2,
+                                                                const int32_t* __restrict__ g1, int B, int N, int M, int kl, GridIndex ix,
+                                                                int32_t* __restrict__ nn_idx, float* __restrict__ res, double* __restrict__ acc) {
+    const int s = blockIdx.y, b = s % B;
+    const int lane = lane_id();
+    const int q0 = (blockIdx.x * kGqWarps + warp_id()) * kGqPerWarp;
+    if (q0 >= N) return;   // uniform over the warp; no barrier follows
+    const float* ws = w + (long long)s * N * 3;
+    const float* lp = l2 + (long long)b * M * 3;
+    const float4* P = ix.pts + (long long)b * M;
+    const int32_t* I = ix.ids + (long long)b * M;
+    const int32_t* CS = ix.cell_start + (long long)b * (ix.cells + 1);
+    const GridParams gp = ix.params[b];
+    double part = 0.0;
+    for (int q = q0; q < min(q0 + kGqPerWarp, N); ++q) {
+        float bd;
+        int bi;
+        grid_knn_diff(P, I, CS, gp, __ldg(ws + 3ll * q), __ldg(ws + 3ll * q + 1), __ldg(ws + 3ll * q + 2), K, bd, bi);
+        float nd[K];
+        int nx[K];
+#pragma unroll
+        for (int r = 0; r < K; ++r) {
+            nd[r] = __shfl_sync(kFull, bd, r);
+            nx[r] = __shfl_sync(kFull, bi, r);
+        }
+        if (lane == 0) part += laplacian_point<K>(nd, nx, ws, lp, g1 + ((long long)b * N + q) * kl, kl, M, (long long)s * N + q, q, nn_idx, res);
+    }
+    if (lane == 0 && part != 0.0) {
+        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + (long long)s * kFxWords, part);
+        else atomicAdd(acc + s, part);
+    }
+}
+
 // One thread per point (s, i) of W: d_w [S,N,3] (over G1 and at i), d_p2 [B,M,3] (the distance part; or NULL) and
 // d_l2 [B,M,3] (or NULL), all accumulated, for the upstream gradient g [S] on the device.  k (<= kLpMaxK) slots of nn_idx
 // per point; a slot of -1 contributes nothing.  DET: the destinations are fixed-point workspaces.
@@ -331,6 +398,13 @@ static void launch_fwd(dim3 grid, cudaStream_t st, bool det, const float* w, con
     else k_laplacian_fwd<K, false><<<grid, kLpThreads, 0, st>>>(w, p2, l2, g1, B, N, M, kl, nn_idx, res, acc);
 }
 
+template <int K>
+static void launch_grid(dim3 grid, cudaStream_t st, bool det, const float* w, const float* l2, const int32_t* g1, int B, int N, int M, int kl,
+                        const GridIndex& ix, int32_t* nn_idx, float* res, double* acc) {
+    if (det) k_laplacian_grid<K, true><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, kl, ix, nn_idx, res, acc);
+    else k_laplacian_grid<K, false><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, kl, ix, nn_idx, res, acc);
+}
+
 static bool bad_graph(int k, int n) { return k < 2 || k > kLpMaxGraph || k > n; }
 
 static bool bad_term(int S, int B, int N, int M, int k_lap, int k_int) {
@@ -392,6 +466,34 @@ extern "C" int pvraft_laplacian_fwd(const float* w, const float* p2, const float
 }
 
 extern "C" int64_t pvraft_laplacian_fwd_det_workspace_bytes(int S) { return S < 1 ? 0 : (int64_t)S * kFxWords * 8; }
+
+extern "C" int pvraft_laplacian_grid_fwd(const float* w, const float* p2, const float* l2, const int32_t* g1, int S, int B, int N, int M,
+                                         int k_lap, int k_int, int32_t* nn_idx, float* res, double* acc, void* workspace, void* det_workspace,
+                                         void* stream) {
+    if (!w || !p2 || !l2 || !g1 || !nn_idx || !res || !acc || !workspace || bad_term(S, B, N, M, k_lap, k_int))
+        return fail(PVRAFT_ERR_BAD_ARG, "laplacian_grid_fwd: bad argument");
+    if (S > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "laplacian_grid_fwd: S = %d samples (at most 65535)", S);
+    cudaStream_t st = (cudaStream_t)stream;
+    GridIndex ix;
+    int rc = grid_index_build(p2, nullptr, B, M, workspace, st, &ix);
+    if (rc) return rc;
+    const dim3 grid((unsigned)((N + kGqPerCta - 1) / kGqPerCta), (unsigned)S);
+    const bool det = det_workspace != nullptr;
+    double* sums = det ? static_cast<double*>(det_workspace) : acc;
+    switch (k_int) {
+        case 1: launch_grid<1>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
+        case 2: launch_grid<2>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
+        case 3: launch_grid<3>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
+        case 4: launch_grid<4>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
+        case 5: launch_grid<5>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
+        case 6: launch_grid<6>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
+        case 7: launch_grid<7>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
+        default: launch_grid<8>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
+    }
+    rc = check_launch("laplacian_grid_fwd");
+    if (rc || !det) return rc;
+    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, S, S, 0, acc, st);
+}
 
 extern "C" int pvraft_laplacian_bwd(const float* w, const float* p2, const float* l2, const int32_t* g1, const int32_t* nn_idx, const float* res,
                                     const float* g, int S, int B, int N, int M, int k_lap, int k_int, float* d_w, float* d_p2, float* d_l2,

@@ -12,7 +12,7 @@
 // and argmin in registers while the other cloud streams through shared memory in double-buffered tiles; one launch searches
 // both directions (blockIdx.z) for every prediction of a sequence (blockIdx.y = sample s, which searches b[s % B]).
 #include "fixed_point.cuh"
-#include "nn_search.cuh"
+#include "grid_index.cuh"
 
 namespace pvraft {
 
@@ -105,6 +105,41 @@ __global__ void __launch_bounds__(kNnThreads) k_chamfer_nn(const float* __restri
         }
     }
     sum = warp_sum(sum);
+    if (lane_id() == 0 && sum != 0.0) {
+        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + (2ll * s + dir) * kFxWords, sum);
+        else atomicAdd(acc + 2 * s + dir, sum);
+    }
+}
+
+// The grid form of k_chamfer_nn: the same nn_ab, nn_ba and minima, searched on the index ib of b (B samples) for z = 0 and
+// the index ia of a (S samples) for z = 1.  One warp per query, kGqPerWarp consecutive queries per warp; lane 0 sums the
+// warp's minima in query order, so what a warp sums is fixed by the shapes.  A query with no finite distance gets index 0
+// and an infinite minimum, as in k_chamfer_nn.
+template <bool DET>
+__global__ void __launch_bounds__(kGqThreads) k_chamfer_grid(const float* __restrict__ a, const float* __restrict__ b, int B, int N, int M,
+                                                              GridIndex ib, GridIndex ia, int32_t* __restrict__ nn_ab, int32_t* __restrict__ nn_ba,
+                                                              double* __restrict__ acc) {
+    const int s = blockIdx.y, dir = blockIdx.z;
+    const int nq = dir ? M : N, nc = dir ? N : M;
+    const int q0 = (blockIdx.x * kGqWarps + warp_id()) * kGqPerWarp;
+    if (q0 >= nq) return;   // uniform over the warp; no barrier follows
+    const float* qry = dir ? b + (long long)(s % B) * M * 3 : a + (long long)s * N * 3;
+    int32_t* out = dir ? nn_ba + (long long)s * M : nn_ab + (long long)s * N;
+    const int t = dir ? s : s % B;   // the searched sample of its index
+    const float4* P = (dir ? ia.pts : ib.pts) + (long long)t * nc;
+    const int32_t* I = (dir ? ia.ids : ib.ids) + (long long)t * nc;
+    const int32_t* CS = (dir ? ia.cell_start : ib.cell_start) + (long long)t * ((dir ? ia.cells : ib.cells) + 1);
+    const GridParams gp = (dir ? ia.params : ib.params)[t];
+    double sum = 0.0;
+    for (int q = q0; q < min(q0 + kGqPerWarp, nq); ++q) {
+        float bd;
+        int bi;
+        grid_knn_diff(P, I, CS, gp, __ldg(qry + 3ll * q), __ldg(qry + 3ll * q + 1), __ldg(qry + 3ll * q + 2), 1, bd, bi);
+        if (lane_id() == 0) {
+            out[q] = bi < nc ? bi : 0;
+            sum += (double)bd;
+        }
+    }
     if (lane_id() == 0 && sum != 0.0) {
         if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + (2ll * s + dir) * kFxWords, sum);
         else atomicAdd(acc + 2 * s + dir, sum);
@@ -224,6 +259,33 @@ extern "C" int pvraft_chamfer_fwd(const float* a, const float* b, int S, int B, 
 }
 
 extern "C" int64_t pvraft_chamfer_fwd_det_workspace_bytes(int S) { return S < 1 ? 0 : 2ll * S * kFxWords * 8; }
+
+extern "C" int64_t pvraft_chamfer_grid_workspace_bytes(int S, int B, int N, int M) {
+    if (S < 1 || B < 1 || N < 1 || M < 1) return 0;
+    return grid_index_bytes(B, M) + grid_index_bytes(S, N);
+}
+
+extern "C" int pvraft_chamfer_grid_fwd(const float* a, const float* b, int S, int B, int N, int M, int32_t* nn_ab, int32_t* nn_ba, double* acc,
+                                       void* workspace, void* det_workspace, void* stream) {
+    if (!a || !b || !nn_ab || !nn_ba || !acc || !workspace || bad_batch(S, B, N) || M < 1)
+        return fail(PVRAFT_ERR_BAD_ARG, "chamfer_grid_fwd: bad argument");
+    if (S > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "chamfer_grid_fwd: S = %d samples (at most 65535)", S);
+    cudaStream_t st = (cudaStream_t)stream;
+    GridIndex ib, ia;
+    int rc = grid_index_build(b, nullptr, B, M, workspace, st, &ib);
+    if (!rc) rc = grid_index_build(a, nullptr, S, N, static_cast<char*>(workspace) + grid_index_bytes(B, M), st, &ia);
+    if (rc) return rc;
+    const int nmax = N > M ? N : M;
+    const dim3 grid((unsigned)((nmax + kGqPerCta - 1) / kGqPerCta), (unsigned)S, 2);
+    if (!det_workspace) {
+        k_chamfer_grid<false><<<grid, kGqThreads, 0, st>>>(a, b, B, N, M, ib, ia, nn_ab, nn_ba, acc);
+        return check_launch("chamfer_grid_fwd");
+    }
+    k_chamfer_grid<true><<<grid, kGqThreads, 0, st>>>(a, b, B, N, M, ib, ia, nn_ab, nn_ba, static_cast<double*>(det_workspace));
+    rc = check_launch("chamfer_grid_fwd");
+    if (rc) return rc;
+    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, 2ll * S, 2ll * S, 0, acc, st);
+}
 
 extern "C" int pvraft_chamfer_bwd(const float* a, const float* b, const int32_t* nn_ab, const int32_t* nn_ba, const float* g, int S, int B,
                                   int N, int M, float* d_a, float* d_b, void* det_workspace, void* stream) {

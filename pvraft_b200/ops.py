@@ -423,12 +423,15 @@ def derived(tensors, tag, fn):
     return value
 
 
+KNN_SORT_MAX_N = 16384   # largest cloud the kNN grid sorts in shared memory (csrc/knn.cu); beyond it a counting sort builds the grid
+
+
 def point_order(points):
     """[B,N,3] -> [B,N] int32: Morton order over the cells of the kNN grid, from the library's in-shared-memory sort
     (one launch; the torch formulation below costs ~40 launches)."""
     b, n, _ = points.shape
     ws_bytes = int(lib().pvraft_knn_workspace_bytes(b, n))
-    if ws_bytes <= 0 or n < 64:
+    if ws_bytes <= 0 or n < 64 or n > KNN_SORT_MAX_N:
         return morton_order(points).to(torch.int32).contiguous()
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=points.device)
     perm = torch.empty(b, n, dtype=torch.int32, device=points.device)
@@ -718,10 +721,32 @@ def _loss_batch(what, x, b_rows, m=None):
         raise ValueError(f'{what}: the second cloud is empty')
 
 
-def chamfer(a, b):
+# Per op, searched clouds of at least this many points are searched on a uniform-grid index (pvraft_*_grid_fwd) instead of by
+# brute force.  Both forms return the same neighbours in the same order, so the choice only changes the time.  Measured with
+# tools/grid_search_cost.py on an H100 80GB HBM3 at 700 W (DESIGN.md 4.4): at N = M = 8192 the grid form of Chamfer (S = 8)
+# and of the Laplacian term take 0.52 / 0.42 ms against 0.54 / 0.60 ms, while the propagation (B = 1, k = 3) takes 0.24 ms
+# against 0.12 ms; at 32 768 every grid form is at least 2x faster.
+GRID_SEARCH_MIN_POINTS = {'chamfer': 8192, 'laplacian': 8192, 'flow_propagate': 32768}
+
+
+def use_grid_search(op, searched, use_grid=None):
+    """True when the nearest-neighbour op `op` ('chamfer', 'laplacian', 'flow_propagate') runs its grid form for a searched
+    cloud of `searched` points.  `use_grid` True / False forces the grid / brute-force form; it exists for tests and
+    measurement, and the models and losses leave it None."""
+    if use_grid is not None:
+        return bool(use_grid)
+    return searched >= GRID_SEARCH_MIN_POINTS[op]
+
+
+def _workspace(nbytes, device):
+    return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
+
+
+def chamfer(a, b, use_grid=None):
     """a [S,N,3] (the first clouds moved by the flows), b [B,M,3] (the second clouds; sample s searches b[s % B]) ->
     (acc [S,2] f64: the sums over a's points of their least squared distance to b, and over b's points of theirs to a;
-    nn_ab [S,N] int32, nn_ba [S,M] int32: the nearest points, lowest index on ties).  Both directions in one launch."""
+    nn_ab [S,N] int32, nn_ba [S,M] int32: the nearest points, lowest index on ties).  Both directions in one launch.
+    The grid form runs when the larger cloud has GRID_SEARCH_MIN_POINTS['chamfer'] points (`use_grid`: see use_grid_search)."""
     if b.dim() != 3 or b.shape[-1] != 3:
         raise ValueError(f'chamfer: expected b [B,M,3], got {tuple(b.shape)}')
     s, n, _ = a.shape
@@ -731,6 +756,11 @@ def chamfer(a, b):
     nn_ab = torch.empty(s, n, dtype=torch.int32, device=a.device)
     nn_ba = torch.empty(s, m, dtype=torch.int32, device=a.device)
     ws = _det_workspace(lib().pvraft_chamfer_fwd_det_workspace_bytes, s, device=a.device)
+    if use_grid_search('chamfer', max(n, m), use_grid):
+        gw = _workspace(lib().pvraft_chamfer_grid_workspace_bytes(s, bb, n, m), a.device)
+        _count(lib().pvraft_chamfer_grid_fwd(_p(a), _p(b), s, bb, n, m, _p(nn_ab, torch.int32), _p(nn_ba, torch.int32), _p(acc, torch.float64),
+                                             _p(gw, torch.uint8), _p(ws, torch.uint8), _stream()), 'chamfer_grid_fwd')
+        return acc, nn_ab, nn_ba
     _count(lib().pvraft_chamfer_fwd(_p(a), _p(b), s, bb, n, m, _p(nn_ab, torch.int32), _p(nn_ba, torch.int32), _p(acc, torch.float64),
                                     _p(ws, torch.uint8), _stream()), 'chamfer_fwd')
     return acc, nn_ab, nn_ba
@@ -826,16 +856,23 @@ def _laplacian_args(what, w, p2, l2, g1, k_int):
     return s, bb, n, m, int(g1.shape[2])
 
 
-def laplacian(w, p2, l2, g1, k_int):
+def laplacian(w, p2, l2, g1, k_int, use_grid=None):
     """w [S,N,3] (the first clouds moved by the flows), p2 [B,M,3] and its Laplacian l2 = cloud_laplacian(p2, g2), g1 [B,N,k_lap]
     (the first cloud's graph; sample s uses entry s % B) -> (acc [S] f64: sum_i ||Lhat_i - L(w)_i||^2 with Lhat_i the
     inverse-squared-distance interpolation of l2 over the k_int nearest points of p2; nn_idx [S,N,k_int] int32, nearest first,
-    lowest index on ties; res [S,N,3] = Lhat - L(w)).  R_s = acc[s] / N."""
+    lowest index on ties; res [S,N,3] = Lhat - L(w)).  R_s = acc[s] / N.  The grid form runs when p2 has
+    GRID_SEARCH_MIN_POINTS['laplacian'] points (`use_grid`: see use_grid_search)."""
     s, bb, n, m, kl = _laplacian_args('laplacian', w, p2, l2, g1, k_int)
     acc = torch.zeros(s, dtype=torch.float64, device=w.device)
     nn_idx = torch.empty(s, n, k_int, dtype=torch.int32, device=w.device)
     res = torch.empty_like(w)
     ws = _det_workspace(lib().pvraft_laplacian_fwd_det_workspace_bytes, s, device=w.device)
+    if use_grid_search('laplacian', m, use_grid):
+        gw = _workspace(lib().pvraft_grid_index_workspace_bytes(bb, m), w.device)
+        _count(lib().pvraft_laplacian_grid_fwd(_p(w), _p(p2), _p(l2), _p(g1, torch.int32), s, bb, n, m, kl, k_int, _p(nn_idx, torch.int32),
+                                               _p(res), _p(acc, torch.float64), _p(gw, torch.uint8), _p(ws, torch.uint8), _stream()),
+               'laplacian_grid_fwd')
+        return acc, nn_idx, res
     _count(lib().pvraft_laplacian_fwd(_p(w), _p(p2), _p(l2), _p(g1, torch.int32), s, bb, n, m, kl, k_int, _p(nn_idx, torch.int32), _p(res),
                                       _p(acc, torch.float64), _p(ws, torch.uint8), _stream()), 'laplacian_fwd')
     return acc, nn_idx, res
@@ -862,11 +899,12 @@ def laplacian_bwd(w, p2, l2, g1, nn_idx, res, g, want_dp2=True):
 PROPAGATE_MAX_K = 8   # neighbours pvraft_flow_propagate_fwd averages over at most
 
 
-def flow_propagate(xyz_prev, flow_prev, xyz, k=3, want_idx=False):
+def flow_propagate(xyz_prev, flow_prev, xyz, k=3, want_idx=False, use_grid=None):
     """Carry a flow defined on one cloud onto another under a constant-velocity assumption: flow_prev [B,M,3] on the points
     xyz_prev [B,M,3] -> flow [B,N,3] on xyz [B,N,3], the inverse-distance-weighted mean flow of the k nearest moved points
     xyz_prev + flow_prev of every point of xyz (include/pvraft_b200.h, pvraft_flow_propagate_fwd).  want_idx: also the
-    neighbours [B,N,k] int32, nearest first (exact distance ties: the lowest index).  Bitwise reproducible in any mode."""
+    neighbours [B,N,k] int32, nearest first (exact distance ties: the lowest index).  Bitwise reproducible in any mode.  The
+    grid form (the same bits) runs when xyz_prev has GRID_SEARCH_MIN_POINTS['flow_propagate'] points (`use_grid`: see use_grid_search)."""
     for name, t in (('xyz_prev', xyz_prev), ('flow_prev', flow_prev), ('xyz', xyz)):
         if not torch.is_tensor(t) or t.dim() != 3 or t.shape[-1] != 3 or t.shape[0] < 1 or t.shape[1] < 1:
             raise ValueError(f'flow_propagate: expected {name} [B,n,3] with B, n >= 1, got '
@@ -887,6 +925,11 @@ def flow_propagate(xyz_prev, flow_prev, xyz, k=3, want_idx=False):
     xyz_prev, flow_prev, xyz = xyz_prev.contiguous(), flow_prev.contiguous(), xyz.contiguous()
     out = torch.empty(b, n, 3, dtype=torch.float32, device=xyz.device)
     idx = torch.empty(b, n, k, dtype=torch.int32, device=xyz.device) if want_idx else None
+    if use_grid_search('flow_propagate', m, use_grid):
+        gw = _workspace(lib().pvraft_grid_index_workspace_bytes(b, m), xyz.device)
+        _count(lib().pvraft_flow_propagate_grid_fwd(_p(xyz_prev), _p(flow_prev), _p(xyz), b, m, n, k, _p(out), _p(idx, torch.int32),
+                                                    _p(gw, torch.uint8), _stream()), 'flow_propagate_grid_fwd')
+        return (out, idx) if want_idx else out
     _count(lib().pvraft_flow_propagate_fwd(_p(xyz_prev), _p(flow_prev), _p(xyz), b, m, n, k, _p(out), _p(idx, torch.int32), _stream()),
            'flow_propagate_fwd')
     return (out, idx) if want_idx else out
