@@ -18,7 +18,9 @@
 //     correlations to the cell's shared-memory accumulator one rank at a time -> the sums equal a sequential
 //     scatter_add over the stored row bit for bit, at a cost that grows with the fullest cell, not with the list;
 //   * the 32 nearest candidates: exact threshold on the fp32 distance bits -- a 128-bin shared-memory histogram
-//     brackets it, a short bisection with warp-wide population counts finishes (no sort), ties -> lowest slot;
+//     brackets it, a short bisection with warp-wide population counts finishes (no sort); the 32 are emitted in
+//     (lane, element) order, and when the 32nd distance T ties, every candidate < T comes first, then those == T in
+//     (lane, element) order up to 32 -- the lowest slots only for K <= 128, where a lane's elements are consecutive slots;
 //   * double-precision first/second moments of the kNN 4-vectors, from which the consumer derives the
 //     GroupNorm statistics of knn_conv's output without materialising its [B,64,N,32] tensor.
 // Index-deciding arithmetic is bit-faithful to the reference's fp32 op sequence: separate rn
