@@ -1,4 +1,4 @@
-// A uniform-grid index of point clouds of any size, and the exact k-nearest search on it in the difference form.
+// A uniform-grid index of point clouds of any size, and the exact k-nearest search on it.
 //
 // The index of S clouds of N points (grid_index_build, csrc/grid_index.cu) is what k_knn_grid reads: per sample the points
 // as float4 (x, y, z, |p|^2) sorted by linear cell id (x fastest), their original ids, cell_start[c] = number of points in
@@ -76,42 +76,54 @@ GridIndex grid_index_carve(void* workspace, int S, int N);
 // (grid_index_bytes(S, N) bytes, 16-byte aligned).  No host synchronisation: capturable into a CUDA graph.
 int grid_index_build(const float* xyz, const float* offset, int S, int N, void* workspace, cudaStream_t st, GridIndex* ix);
 
-// ---- the k-nearest search in the difference form --------------------------------------------------------------------------
+// ---- the k-nearest search on the index -------------------------------------------------------------------------------------
 constexpr int kGridNone = 0x7fffff00;   // ids of the list's unfilled slots (kGridNone + lane): larger than any point id
 
-// score the sorted range [begin, end) of the index against q (one warp), for grid_knn_diff
-__device__ __forceinline__ void grid_scan_diff(const float4* __restrict__ P, const int32_t* __restrict__ I, int begin, int end, float qx, float qy,
-                                               float qz, int k, float& bd, int& bi, float& tau, int& tau_i) {
+// A distance form is a policy with three members:
+//   dist(qx, qy, qz, p)  the distance of the query q to the index point p (x, y, z, |p|^2);
+//   kFiniteOnly          the admission rule (admitted): a candidate (d, id) enters when it is not worse than the list's k-th
+//                        entry (tau, tau_i) and, if kFiniteOnly, d is finite.  A compile-time flag, and admitted returns
+//                        the ballot itself: with a bool-returning predicate call inside the ballot, ptxas (nvcc 12.9)
+//                        spills up to 36 more bytes in k_laplacian_grid and gives k_knn_grid 4 more registers;
+//   stop(b, tau)         whether no unvisited point can enter once every one is at least b > 0 away along some axis.
+
+// the lanes whose candidate (d, id) exists (`in`) and enters a list whose k-th entry is (tau, tau_i), under Form's admission
+// rule
+template <class Form>
+__device__ __forceinline__ unsigned admitted(bool in, float d, int id, float tau, int tau_i) {
+    return __ballot_sync(kFull, in && (!Form::kFiniteOnly || d < INFINITY) && !worse(d, id, tau, tau_i));
+}
+
+// score the sorted range [begin, end) of the index against q (one warp)
+template <class Form>
+__device__ __forceinline__ void grid_scan(const Form& form, const float4* __restrict__ P, const int32_t* __restrict__ I, int begin, int end,
+                                          float qx, float qy, float qz, int k, float& bd, int& bi, float& tau, int& tau_i) {
     const int lane = lane_id();
     for (int i0 = begin; i0 < end; i0 += 32) {
         const int i = i0 + lane;
         float d = INFINITY;
         int id = 0x7fffffff;
         if (i < end) {
-            d = diff_sq(qx, qy, qz, __ldg(P + i));
+            d = form.dist(qx, qy, qz, __ldg(P + i));
             id = __ldg(I + i);
         }
-        const unsigned cand = __ballot_sync(kFull, i < end && d < INFINITY && !worse(d, id, tau, tau_i));
+        const unsigned cand = admitted<Form>(i < end, d, id, tau, tau_i);
         insert_candidates(cand, d, id, bd, bi, tau, tau_i, k);
     }
 }
 
-// One warp finds the k (<= 32) nearest points of q in one sample of the index, ranked on (diff_sq(q, p), id) -- the order of
-// the brute-force searches of nn_search.cuh, whatever order the points are visited in.  Only finite distances enter the list
-// (the brute-force searches admit a point only below a finite or infinite running k-th distance, which +inf and NaN never
-// are).  On return lane r < k holds the r-th nearest (bd, bi); a slot no point filled holds (+inf, kGridNone + r).
+// One warp finds the k (<= 32) nearest points of q in one sample of the index (P, I, CS, gp), ranked on (form.dist, id),
+// whatever order the points are visited in.  On return lane r < k holds the r-th nearest (bd, bi); a slot no point filled
+// holds (+inf, kGridNone + r).
 //
-// The visit is k_knn_grid's: shells of cells of growing Chebyshev radius r around q's cell.  The stopping rule must be exact
-// for the computed fp32 distance.  After shell r, every unvisited point p lies outside the box of cells [c - r, c + r], so on
-// some axis a, |q_a - p_a| >= bound, the distance from q to the nearest face of the box with cells behind it; `margin`
-// covers the fp32 error of the face position and of the cell assignment (k_knn_grid), so b = bound - margin is a lower
-// bound on |q_a - p_a| in exact arithmetic.  Rounding to nearest is monotone, and b is an fp32 number, so the computed
-// |dx_a| = fl(|q_a - p_a|) >= b and fl(dx_a * dx_a) >= fl(b * b).  Every other term of diff_sq is >= 0 and each rounded sum
-// of non-negative terms is >= each of its terms, so the computed distance of p is >= fl(b * b): the bound carries the
-// rounding of all three products and both sums with no slack term.  The search stops when fl(b * b) > tau, STRICTLY: every
-// unvisited point then has a distance above the k-th, so none can enter, not even on an equal distance with a lower id.
-__device__ __forceinline__ void grid_knn_diff(const float4* __restrict__ P, const int32_t* __restrict__ I, const int32_t* __restrict__ CS,
-                                              const GridParams& gp, float qx, float qy, float qz, int k, float& bd, int& bi) {
+// The visit: shells of cells of growing Chebyshev radius r around q's cell.  After shell r, every unvisited point p lies
+// outside the box of cells [c - r, c + r], so on some axis a, |q_a - p_a| >= bound, the distance from q to the nearest face of
+// the box with cells behind it; `margin` covers the fp32 error of the face position and of the cell assignment, so
+// b = bound - margin is a lower bound on |q_a - p_a| in exact arithmetic.  The form's stop(b, tau) turns it into a bound on
+// the distance.
+template <class Form>
+__device__ __forceinline__ void grid_knn(const Form& form, const float4* __restrict__ P, const int32_t* __restrict__ I,
+                                         const int32_t* __restrict__ CS, const GridParams& gp, float qx, float qy, float qz, int k, float& bd, int& bi) {
     const int lane = lane_id();
     const float qv[3] = {qx, qy, qz};
     int c[3];
@@ -121,9 +133,7 @@ __device__ __forceinline__ void grid_knn_diff(const float4* __restrict__ P, cons
     bi = kGridNone + lane;
     float tau = INFINITY;
     int tau_i = kGridNone + k - 1;
-    auto scan = [&](int begin, int end) {   // score the sorted range [begin, end)
-        grid_scan_diff(P, I, begin, end, qx, qy, qz, k, bd, bi, tau, tau_i);
-    };
+    auto scan = [&](int begin, int end) { grid_scan(form, P, I, begin, end, qx, qy, qz, k, bd, bi, tau, tau_i); };
     const int rmax = max(max(gp.G[0], gp.G[1]), gp.G[2]);
     for (int r = 0; r < rmax; ++r) {
         const int x0 = max(c[0] - r, 0), x1 = min(c[0] + r, gp.G[0] - 1);
@@ -139,6 +149,7 @@ __device__ __forceinline__ void grid_knn_diff(const float4* __restrict__ P, cons
                 }
             }
         }
+        // distance from the query to the nearest face of the visited box that still has cells behind it
         float bound = INFINITY;
 #pragma unroll
         for (int a = 0; a < 3; ++a) {
@@ -147,8 +158,27 @@ __device__ __forceinline__ void grid_knn_diff(const float4* __restrict__ P, cons
         }
         if (bound == INFINITY) break;                 // the box covers the whole grid
         const float b = bound - gp.margin;
-        if (b > 0.f && __fmul_rn(b, b) > tau) break;
+        if (b > 0.f && form.stop(b, tau)) break;
     }
+}
+
+// The difference form diff_sq, the order of the brute-force searches of nn_search.cuh.  Only finite distances enter the list
+// (the brute-force searches admit a point only below a finite or infinite running k-th distance, which +inf and NaN never
+// are).  The stopping rule is exact for the computed fp32 distance: rounding to nearest is monotone, and b is an fp32 number,
+// so the computed |dx_a| = fl(|q_a - p_a|) >= b and fl(dx_a * dx_a) >= fl(b * b).  Every other term of diff_sq is >= 0 and
+// each rounded sum of non-negative terms is >= each of its terms, so the computed distance of p is >= fl(b * b): the bound
+// carries the rounding of all three products and both sums with no slack term.  The search stops when fl(b * b) > tau,
+// STRICTLY: every unvisited point then has a distance above the k-th, so none can enter, not even on an equal distance with a
+// lower id.
+struct DiffForm {
+    __device__ __forceinline__ float dist(float qx, float qy, float qz, const float4& p) const { return diff_sq(qx, qy, qz, p); }
+    static constexpr bool kFiniteOnly = true;
+    __device__ __forceinline__ bool stop(float b, float tau) const { return __fmul_rn(b, b) > tau; }
+};
+
+__device__ __forceinline__ void grid_knn_diff(const float4* __restrict__ P, const int32_t* __restrict__ I, const int32_t* __restrict__ CS,
+                                              const GridParams& gp, float qx, float qy, float qz, int k, float& bd, int& bi) {
+    grid_knn(DiffForm(), P, I, CS, gp, qx, qy, qz, k, bd, bi);
 }
 
 }  // namespace pvraft

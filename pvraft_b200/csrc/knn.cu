@@ -6,14 +6,15 @@
 //   k_grid_sort   one CTA per sample: bounding box -> uniform grid (~3 points per cell), points sorted by cell id with a
 //                 bitonic sort in shared memory -> float4 (x,y,z,|p|^2) in cell order + original ids
 //   k_grid_cells  cell_start[c] by binary search in the sorted cell ids
-//   k_knn_grid    one warp per query: shells of cells of growing radius around the query's cell; the warp keeps the current
-//                 k best as one (distance, id) pair per lane plus the running k-th distance tau, a candidate enters only
-//                 if it beats tau, and the search stops once the unvisited space is farther than tau plus the rounding
-//                 slack of the distance formula: a few hundred candidates are scored per query instead of the whole cloud.
+//   k_knn_grid    one warp per query: grid_knn (grid_index.cuh), shells of cells of growing radius around the query's cell; the
+//                 warp keeps the current k best as one (distance, id) pair per lane plus the running k-th distance tau, a
+//                 candidate enters only if it beats tau, and the search stops once the unvisited space is farther than tau plus
+//                 the rounding slack of the distance formula: a few hundred candidates are scored per query instead of the
+//                 whole cloud.
 // Distances reproduce the reference's expanded form bit-for-bit on the CPU oracle: |q|^2 and |x|^2 as
 // (x*x+y*y)+z*z, q.x as fma(z,z',fma(y,y',x*x')); ranking is on (distance, original id), so the result does not
 // depend on the visiting order.  Clouds too large for the shared-memory sort get the same index from the multi-CTA counting
-// sort of grid_index.cu, and the same k_knn_grid searches it, one launch per sample.
+// sort of grid_index.cu, and the same k_knn_grid searches it.
 #include "grid_index.cuh"
 
 namespace pvraft {
@@ -27,6 +28,18 @@ __device__ __forceinline__ float ref_distance(int mode, float qx, float qy, floa
     if (mode == 0) return __fsub_rn(__fadd_rn(qn, p.w), __fmul_rn(2.f, dot));   // graph.py:53-57
     return __fadd_rn(__fadd_rn(__fmul_rn(-2.f, dot), qn), p.w);                  // pointconv.py:21-24
 }
+
+// The distance form (grid_index.cuh) of the kNN graph: ref_distance, every candidate not worse than the k-th admitted (NaN
+// included; k_knn uses the same dist and admitted), and a stop once bound^2 exceeds the k-th distance by more than the
+// rounding slack of the expanded form, which depends on |q|^2 and the sample's largest |p|^2.
+struct ExpandedForm {
+    int mode;
+    float qn;
+    float slack;
+    __device__ __forceinline__ float dist(float qx, float qy, float qz, const float4& p) const { return ref_distance(mode, qx, qy, qz, qn, p); }
+    static constexpr bool kFiniteOnly = false;
+    __device__ __forceinline__ bool stop(float b, float tau) const { return b * b > tau + slack; }
+};
 
 __device__ __forceinline__ void write_result(const float* __restrict__ X, float qx, float qy, float qz, int lane, int k, int bi,
                                              size_t out_row, int32_t* __restrict__ out, float* __restrict__ rel) {
@@ -57,11 +70,11 @@ __global__ void __launch_bounds__(kKnnThreads) k_knn(const float* __restrict__ x
         const float* Q = query + ((size_t)b * S + q) * 3;
         qx = __ldg(Q); qy = __ldg(Q + 1); qz = __ldg(Q + 2);
     }
-    const float qn = sqnorm(qx, qy, qz);
+    const ExpandedForm form{mode, sqnorm(qx, qy, qz), 0.f};   // no stopping test: every point is scored
     float bd = INFINITY;                 // sorted list of (distance, id): +inf sentinels with ascending ids
-    int bi = 0x7fffff00 + lane;
+    int bi = kGridNone + lane;
     float tau = INFINITY;
-    int tau_i = 0x7fffff00 + k - 1;
+    int tau_i = kGridNone + k - 1;
     for (int base = 0; base < N; base += kKnnTile) {
         const int cnt = min(kKnnTile, N - base);
         __syncthreads();
@@ -75,8 +88,8 @@ __global__ void __launch_bounds__(kKnnThreads) k_knn(const float* __restrict__ x
             const int i = i0 + lane;
             float d = INFINITY;
             const int id = base + i;
-            if (i < cnt) d = ref_distance(mode, qx, qy, qz, qn, s_pts[i]);
-            const unsigned cand = __ballot_sync(kFull, i < cnt && !worse(d, id, tau, tau_i));
+            if (i < cnt) d = form.dist(qx, qy, qz, s_pts[i]);
+            const unsigned cand = admitted<ExpandedForm>(i < cnt, d, id, tau, tau_i);
             insert_candidates(cand, d, id, bd, bi, tau, tau_i, k);
         }
     }
@@ -203,73 +216,37 @@ __global__ void k_grid_cells(const unsigned* __restrict__ keys, int N, int32_t* 
     cell_start[(size_t)b * (kMaxCells + 1) + c] = lo;
 }
 
-// One warp per query: shells of cells of growing Chebyshev radius around the query's cell.  After shell r every
-// unvisited point lies outside the box of cells [c - r, c + r], i.e. at least `bound` away from the query; the search
-// stops when bound^2 exceeds the current k-th distance by more than the rounding slack of the expanded distance form.
-__global__ void __launch_bounds__(kKnnThreads) k_knn_grid(const float* __restrict__ xyz, const float4* __restrict__ sorted,
-                                                          const int32_t* __restrict__ ids, const int32_t* __restrict__ cell_start,
-                                                          const GridParams* __restrict__ params, const float* __restrict__ query,
+// One warp per query on the index `ix` of xyz (B samples): grid_knn in the expanded form.
+__global__ void __launch_bounds__(kKnnThreads) k_knn_grid(const float* __restrict__ xyz, GridIndex ix, const float* __restrict__ query,
                                                           int N, int S, int k, int mode, int32_t* __restrict__ out, float* __restrict__ rel) {
     const int b = blockIdx.y;
-    const int lane = lane_id(), w = warp_id();
-    const int q = blockIdx.x * (kKnnThreads / 32) + w;
+    const int q = blockIdx.x * (kKnnThreads / 32) + warp_id();
     if (q >= S) return;
-    const float* X = xyz + (size_t)b * N * 3;
-    const float4* P = sorted + (size_t)b * N;
-    const int32_t* I = ids + (size_t)b * N;
-    const int32_t* CS = cell_start + (size_t)b * (kMaxCells + 1);
-    const GridParams gp = params[b];
+    const float4* P = ix.pts + (size_t)b * N;
+    const int32_t* I = ix.ids + (size_t)b * N;
+    const int32_t* CS = ix.cell_start + b * (ix.cells + 1ll);
+    const GridParams gp = ix.params[b];
     const float* Q = query + ((size_t)b * S + q) * 3;
     const float qv[3] = {__ldg(Q), __ldg(Q + 1), __ldg(Q + 2)};
     const float qn = sqnorm(qv[0], qv[1], qv[2]);
-    const float slack = 4e-6f * (qn + gp.max_norm) + 1e-30f;
-    int c[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) c[a] = cell_coord(qv[a], gp.gmin[a], gp.inv_h[a], gp.G[a]);
-    float bd = INFINITY;                 // sorted list of (distance, id): +inf sentinels with ascending ids
-    int bi = 0x7fffff00 + lane;
-    float tau = INFINITY;
-    int tau_i = 0x7fffff00 + k - 1;
-    auto scan = [&](int begin, int end) {   // score the sorted range [begin, end)
-        for (int i0 = begin; i0 < end; i0 += 32) {
-            const int i = i0 + lane;
-            float d = INFINITY;
-            int id = 0x7fffffff;
-            if (i < end) {
-                d = ref_distance(mode, qv[0], qv[1], qv[2], qn, __ldg(P + i));
-                id = __ldg(I + i);
-            }
-            const unsigned cand = __ballot_sync(kFull, i < end && !worse(d, id, tau, tau_i));
-            insert_candidates(cand, d, id, bd, bi, tau, tau_i, k);
-        }
-    };
-    const int rmax = max(max(gp.G[0], gp.G[1]), gp.G[2]);
-    for (int r = 0; r < rmax; ++r) {
-        const int x0 = max(c[0] - r, 0), x1 = min(c[0] + r, gp.G[0] - 1);
-        for (int z = max(c[2] - r, 0); z <= min(c[2] + r, gp.G[2] - 1); ++z) {
-            const bool z_face = (z == c[2] - r) || (z == c[2] + r);
-            for (int y = max(c[1] - r, 0); y <= min(c[1] + r, gp.G[1] - 1); ++y) {
-                const int row = (z * gp.G[1] + y) * gp.G[0];
-                if (z_face || y == c[1] - r || y == c[1] + r) {
-                    scan(__ldg(CS + row + x0), __ldg(CS + row + x1 + 1));   // the whole run along x is new
-                } else {   // only the two end cells of the run are on the shell
-                    if (c[0] - r >= 0) scan(__ldg(CS + row + c[0] - r), __ldg(CS + row + c[0] - r + 1));
-                    if (c[0] + r < gp.G[0] && r > 0) scan(__ldg(CS + row + c[0] + r), __ldg(CS + row + c[0] + r + 1));
-                }
-            }
-        }
-        // distance from the query to the nearest face of the visited box that still has cells behind it
-        float bound = INFINITY;
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            if (c[a] - r > 0) bound = fminf(bound, qv[a] - (gp.gmin[a] + (float)(c[a] - r) * gp.h[a]));
-            if (c[a] + r < gp.G[a] - 1) bound = fminf(bound, (gp.gmin[a] + (float)(c[a] + r + 1) * gp.h[a]) - qv[a]);
-        }
-        if (bound == INFINITY) break;                 // the box covers the whole grid
-        bound -= gp.margin;
-        if (bound > 0.f && bound * bound > tau + slack) break;
-    }
-    write_result(X, qv[0], qv[1], qv[2], lane, k, bi, (size_t)b * S + q, out, rel);
+    const ExpandedForm form{mode, qn, 4e-6f * (qn + gp.max_norm) + 1e-30f};
+    float bd;
+    int bi;
+    grid_knn(form, P, I, CS, gp, qv[0], qv[1], qv[2], k, bd, bi);
+    write_result(xyz + (size_t)b * N * 3, qv[0], qv[1], qv[2], lane_id(), k, bi, (size_t)b * S + q, out, rel);
+}
+
+// The index of k_grid_sort in `workspace` (pvraft_knn_workspace_bytes): float4 sorted[B*N] | int32 ids[B*N] | uint32 keys[B*N]
+// | int32 cell_start[B*(kMaxCells+1)] | GridParams[B] (16-byte aligned).  `keys` is k_grid_sort's sort key of each point.
+static GridIndex knn_index_carve(void* workspace, int B, int N, unsigned*& keys) {
+    GridIndex ix;
+    ix.pts = reinterpret_cast<float4*>(workspace);
+    ix.ids = reinterpret_cast<int32_t*>(ix.pts + (size_t)B * N);
+    keys = reinterpret_cast<unsigned*>(ix.ids + (size_t)B * N);
+    ix.cell_start = reinterpret_cast<int32_t*>(keys + (size_t)B * N);
+    ix.params = reinterpret_cast<GridParams*>((reinterpret_cast<uintptr_t>(ix.cell_start + (size_t)B * (kMaxCells + 1)) + 15) & ~(uintptr_t)15);
+    ix.cells = kMaxCells;
+    return ix;
 }
 
 }  // namespace pvraft
@@ -292,42 +269,27 @@ extern "C" int pvraft_knn_fwd(const float* xyz, const float* query, int B, int N
     if (B > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "knn: B=%d", B);
     cudaStream_t st = (cudaStream_t)stream;
     dim3 grid((S + kKnnThreads / 32 - 1) / (kKnnThreads / 32), B);
+    GridIndex ix;
+    int rc;
     if (workspace && N <= kSortMaxN && N >= 64) {
         int NP = 1;
         while (NP < N) NP <<= 1;
-        // workspace layout: float4 sorted[B*N] | int32 ids[B*N] | uint32 keys[B*N] | int32 cell_start[B*(kMaxCells+1)] | GridParams[B]
-        float4* sorted = reinterpret_cast<float4*>(workspace);
-        int32_t* ids = reinterpret_cast<int32_t*>(sorted + (size_t)B * N);
-        unsigned* keys = reinterpret_cast<unsigned*>(ids + (size_t)B * N);
-        int32_t* cell_start = reinterpret_cast<int32_t*>(keys + (size_t)B * N);
-        GridParams* params = reinterpret_cast<GridParams*>((reinterpret_cast<uintptr_t>(cell_start + (size_t)B * (kMaxCells + 1)) + 15) & ~(uintptr_t)15);
+        unsigned* keys;
+        ix = knn_index_carve(workspace, B, N, keys);
         const size_t smem = (size_t)NP * sizeof(unsigned long long);
-        int rc;
         if ((rc = opt_in_smem(k_grid_sort, smem))) return rc;
-        k_grid_sort<<<B, 1024, smem, st>>>(xyz, N, NP, kCellOcc, 0, params, sorted, ids, keys);
+        k_grid_sort<<<B, 1024, smem, st>>>(xyz, N, NP, kCellOcc, 0, ix.params, ix.pts, ix.ids, keys);
         if ((rc = check_launch("knn grid sort"))) return rc;
-        k_grid_cells<<<dim3((kMaxCells + 1 + 255) / 256, B), 256, 0, st>>>(keys, N, cell_start);
+        k_grid_cells<<<dim3((kMaxCells + 1 + 255) / 256, B), 256, 0, st>>>(keys, N, ix.cell_start);
         if ((rc = check_launch("knn grid cells"))) return rc;
-        k_knn_grid<<<grid, kKnnThreads, 0, st>>>(xyz, sorted, ids, cell_start, params, query, N, S, k, mode, idx, rel);
-        return check_launch("knn grid");
-    }
-    if (workspace && N > kSortMaxN) {
-        // the index of grid_index.cu: its cell_start rows are grid_index_cells(N) + 1 long, not kMaxCells + 1, so k_knn_grid
-        // runs once per sample on that sample's slices (blockIdx.y = 0)
-        GridIndex ix;
-        int rc;
+    } else if (workspace && N > kSortMaxN) {
         if ((rc = grid_index_build(xyz, nullptr, B, N, workspace, st, &ix))) return rc;
-        for (int b = 0; b < B; ++b) {
-            const size_t pts = (size_t)b * N, qs = (size_t)b * S;
-            k_knn_grid<<<dim3(grid.x, 1), kKnnThreads, 0, st>>>(xyz + pts * 3, ix.pts + pts, ix.ids + pts,
-                                                                 ix.cell_start + (size_t)b * (ix.cells + 1), ix.params + b, query + qs * 3, N,
-                                                                 S, k, mode, idx + qs * k, rel ? rel + qs * k * 3 : nullptr);
-            if ((rc = check_launch("knn grid"))) return rc;
-        }
-        return 0;
+    } else {
+        k_knn<<<grid, kKnnThreads, 0, st>>>(xyz, query, N, S, k, mode, idx, rel);
+        return check_launch("knn");
     }
-    k_knn<<<grid, kKnnThreads, 0, st>>>(xyz, query, N, S, k, mode, idx, rel);
-    return check_launch("knn");
+    k_knn_grid<<<grid, kKnnThreads, 0, st>>>(xyz, ix, query, N, S, k, mode, idx, rel);
+    return check_launch("knn grid");
 }
 
 extern "C" int pvraft_point_order_fwd(const float* xyz, int B, int N, int32_t* perm, void* workspace, void* stream) {
@@ -336,18 +298,14 @@ extern "C" int pvraft_point_order_fwd(const float* xyz, int B, int N, int32_t* p
     cudaStream_t st = (cudaStream_t)stream;
     int NP = 1;
     while (NP < N) NP <<= 1;
-    // same workspace layout as pvraft_knn_fwd; the permutation is the `ids` array of the sort
-    float4* sorted = reinterpret_cast<float4*>(workspace);
-    int32_t* ids = reinterpret_cast<int32_t*>(sorted + (size_t)B * N);
-    unsigned* keys = reinterpret_cast<unsigned*>(ids + (size_t)B * N);
-    int32_t* cell_start = reinterpret_cast<int32_t*>(keys + (size_t)B * N);
-    GridParams* params = reinterpret_cast<GridParams*>((reinterpret_cast<uintptr_t>(cell_start + (size_t)B * (kMaxCells + 1)) + 15) & ~(uintptr_t)15);
+    unsigned* keys;
+    const GridIndex ix = knn_index_carve(workspace, B, N, keys);   // the permutation is the `ids` array of the sort
     const size_t smem = (size_t)NP * sizeof(unsigned long long);
     int rc;
     if ((rc = opt_in_smem(k_grid_sort, smem))) return rc;
-    k_grid_sort<<<B, 1024, smem, st>>>(xyz, N, NP, kCellOcc, 1, params, sorted, ids, keys);
+    k_grid_sort<<<B, 1024, smem, st>>>(xyz, N, NP, kCellOcc, 1, ix.params, ix.pts, ix.ids, keys);
     if ((rc = check_launch("point order sort"))) return rc;
-    const cudaError_t e = cudaMemcpyAsync(perm, ids, (size_t)B * N * sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
+    const cudaError_t e = cudaMemcpyAsync(perm, ix.ids, (size_t)B * N * sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
     if (e != cudaSuccess) return fail((int)e, "point_order: copy failed: %s", cudaGetErrorString(e));
     return 0;
 }

@@ -7,10 +7,8 @@
 //            squared distance (the weighting of PointPWC-Net's curvature interpolation; not k_flow_propagate's 1/(sqrt(d)+1e-8))
 //   R_s    = (1/N) sum_i ||Lhat_i - L(W)_i||^2,  L(W) over G1 = knn(P1, P1, k_lap): neighbours of the un-moved cloud, values of W
 //
-// k_laplacian_fwd does the search in the structure of k_flow_propagate: the difference form of nn_search.cuh ranked on
-// (distance, index), kLpPerCta queries per CTA held in registers by every warp while P2 streams through double-buffered
-// shared-memory tiles, warp w searching the w-th slice of each tile with a sorted K-best list per query, and the eight lists
-// merged on (distance, index) in shared memory at the end.  The thread that owns a query then interpolates L2, gathers L(W)_i
+// k_laplacian_fwd searches P2 with the tiled brute-force K-best search of nn_search.cuh (tiled_kbest), the difference form
+// ranked on (distance, index), as k_flow_propagate does.  The thread that owns a query then interpolates L2, gathers L(W)_i
 // over G1, writes the residual Lhat_i - L(W)_i and its neighbours for the backward pass, and adds its squared length (in
 // double) to the sample's sum; DET: into the fixed-point workspace, each warp's sum being a function of the shapes.
 //
@@ -27,17 +25,8 @@
 
 namespace pvraft {
 
-constexpr int kLpWarps = 8;
-constexpr int kLpThreads = kLpWarps * kWarp;
-constexpr int kLpQueries = 2;                          // queries per lane, held in registers
-constexpr int kLpPerCta = kWarp * kLpQueries;          // queries per CTA, searched by every warp
-constexpr int kLpTile = 256;                           // searched points per shared-memory tile (two tiles)
-constexpr int kLpSlice = kLpTile / kLpWarps;           // points of a tile each warp searches
 constexpr int kLpMaxK = 8;                             // interpolation neighbours k_int
 constexpr int kLpMaxGraph = 32;                        // graph neighbours k_lap (the kNN kernel's limit)
-constexpr int kLpNone = 0x7fffffff;                    // index of an unfilled slot: loses every (distance, index) tie
-static_assert(kLpTile == kLpThreads, "each thread stages one point per tile");
-static_assert(kLpPerCta % kWarp == 0, "the merging threads are whole warps");
 
 // L(x)_i over the graph row nbr_i (k ids into x): the fp32 differences summed in edge order, then divided by k - 1.  A self
 // edge adds an exact zero.
@@ -94,9 +83,8 @@ __global__ void __launch_bounds__(256) k_cloud_laplacian_bwd(const float* __rest
     }
 }
 
-// The per-query step of k_laplacian_grid after its search, the same formula, order and rounding as k_laplacian_fwd's (which
-// keeps its own copy, so that its machine code is unchanged): from the k_int nearest (nd, nx) of w_q, nearest first, write
-// nn_idx and the residual of row `row` and return its squared length in double.
+// The per-query step after the search, shared by k_laplacian_fwd and k_laplacian_grid: from the k_int nearest (nd, nx) of
+// w_q, nearest first, write nn_idx and the residual of row `row` and return its squared length in double.
 // Lhat = sum_r w_r L2[j_r] / sum_r w_r, summed in fp32 nearest first.  An unfilled slot (only possible when non-finite
 // coordinates leave fewer than K comparable points) contributes nothing and reads back as -1.
 template <int K>
@@ -126,143 +114,25 @@ __device__ __forceinline__ double laplacian_point(const float (&nd)[K], const in
 }
 
 // w [S,N,3], p2 and l2 [B,M,3], g1 [B,N,kl] (sample s uses entry s % B) -> nn_idx [S,N,K], res [S,N,3] = Lhat - L(w),
-// acc[s] += sum_i ||res_i||^2; grid (ceil(N / kLpPerCta), S).  DET: acc is the [S] fixed-point workspace.
+// acc[s] += sum_i ||res_i||^2; grid (ceil(N / kKbPerCta), S).  DET: acc is the [S] fixed-point workspace.
+// K = 2 fits in 32 registers with no spills, 8 CTAs per SM; unasked, ptxas (nvcc 12.9) gives it 40 and 6 CTAs.  The other K
+// are left to ptxas: a minimum of 1 CTA per SM raises them.
 template <int K, bool DET>
-__global__ void __launch_bounds__(kLpThreads) k_laplacian_fwd(const float* __restrict__ w, const float* __restrict__ p2, const float* __restrict__ l2,
+__global__ void __launch_bounds__(kKbThreads, K == 2 ? 8 : 0) k_laplacian_fwd(const float* __restrict__ w, const float* __restrict__ p2, const float* __restrict__ l2,
                                                                const int32_t* __restrict__ g1, int B, int N, int M, int kl,
                                                                int32_t* __restrict__ nn_idx, float* __restrict__ res, double* __restrict__ acc) {
-    __shared__ float4 tile[2][kLpTile];
-    __shared__ float md[kLpWarps][K][kLpPerCta];       // every warp's k-best lists, [warp][rank][query]
-    __shared__ int mi[kLpWarps][K][kLpPerCta];
     const int s = blockIdx.y, b = s % B;
     const float* ws = w + (long long)s * N * 3;
-    const float* cp = p2 + (long long)b * M * 3;
-    const float* lp = l2 + (long long)b * M * 3;
-    const int q0 = blockIdx.x * kLpPerCta;
-    const int lane = lane_id(), warp = warp_id();
-
-    float qx[kLpQueries], qy[kLpQueries], qz[kLpQueries], best[kLpQueries][K];
-    int arg[kLpQueries][K];
-#pragma unroll
-    for (int i = 0; i < kLpQueries; ++i) {
-        const int q = q0 + i * kWarp + lane;
-        const bool ok = q < N;
-        qx[i] = ok ? __ldg(ws + 3ll * q) : 0.f;
-        qy[i] = ok ? __ldg(ws + 3ll * q + 1) : 0.f;
-        qz[i] = ok ? __ldg(ws + 3ll * q + 2) : 0.f;
-#pragma unroll
-        for (int r = 0; r < K; ++r) {
-            best[i][r] = INFINITY;
-            arg[i][r] = kLpNone;
-        }
-    }
-
-    // the next tile is fetched into registers while the current one is searched; points past the end read as NaN, whose
-    // distance never compares below a list entry
-    float st[3];
-    auto fetch = [&](int t) {
-        const int p = t * kLpTile + threadIdx.x;
-        const bool ok = p < M;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) st[c] = ok ? __ldg(cp + 3ll * p + c) : NAN;
-    };
-    auto store = [&](int buf) { tile[buf][threadIdx.x] = make_float4(st[0], st[1], st[2], 0.f); };
-
-    const int tiles = (M + kLpTile - 1) / kLpTile;
-    fetch(0);
-    store(0);
-    __syncthreads();
-    for (int t = 0; t < tiles; ++t) {
-        const bool more = t + 1 < tiles;
-        if (more) fetch(t + 1);
-        const float4* tl = tile[t & 1] + warp * kLpSlice;
-        const int base = t * kLpTile + warp * kLpSlice;
-#pragma unroll 8
-        for (int j = 0; j < kLpSlice; ++j) {
-            const float4 p = tl[j];   // the same address in every lane: a broadcast
-#pragma unroll
-            for (int i = 0; i < kLpQueries; ++i) {
-                const float d = diff_sq(qx[i], qy[i], qz[i], p);
-                if (d < best[i][K - 1]) kbest_insert<K>(best[i], arg[i], d, base + j);
-            }
-        }
-        if (more) store((t + 1) & 1);   // the buffer searched in iteration t - 1, released by its barrier
-        __syncthreads();
-    }
-
-#pragma unroll
-    for (int i = 0; i < kLpQueries; ++i)
-#pragma unroll
-        for (int r = 0; r < K; ++r) {
-            md[warp][r][i * kWarp + lane] = best[i][r];
-            mi[warp][r][i * kWarp + lane] = arg[i][r];
-        }
-    __syncthreads();
-    const int t = threadIdx.x, q = q0 + t;
-    if (t >= kLpPerCta) return;   // whole warps; the rest stay for the warp sum
-
+    float nd[K];
+    int nx[K];
+    if (!tiled_kbest<K, false>(ws, N, p2 + (long long)b * M * 3, nullptr, M, nd, nx)) return;   // whole warps; the rest stay for the warp sum
+    const int q = blockIdx.x * kKbPerCta + threadIdx.x;
     double part = 0.0;
-    if (q < N) {
-        // merge the warps' lists: each is ascending in (distance, index), so K times the least head wins
-        float hd[kLpWarps];
-        int hx[kLpWarps], pos[kLpWarps];
-#pragma unroll
-        for (int v = 0; v < kLpWarps; ++v) {
-            pos[v] = 0;
-            hd[v] = md[v][0][t];
-            hx[v] = mi[v][0][t];
-        }
-        float nd[K];
-        int nx[K];
-#pragma unroll
-        for (int r = 0; r < K; ++r) {
-            int bw = 0;
-            float bd = hd[0];
-            int bx = hx[0];
-#pragma unroll
-            for (int v = 1; v < kLpWarps; ++v)
-                if (hd[v] < bd || (hd[v] == bd && hx[v] < bx)) {
-                    bw = v;
-                    bd = hd[v];
-                    bx = hx[v];
-                }
-            nd[r] = bd;
-            nx[r] = bx;
-#pragma unroll
-            for (int v = 0; v < kLpWarps; ++v)
-                if (v == bw) {
-                    ++pos[v];
-                    hd[v] = pos[v] < K ? md[v][pos[v]][t] : INFINITY;
-                    hx[v] = pos[v] < K ? mi[v][pos[v]][t] : kLpNone;
-                }
-        }
-
-        // Lhat = sum_r w_r L2[j_r] / sum_r w_r, summed in fp32 nearest first.  An unfilled slot (only possible when
-        // non-finite coordinates leave fewer than K comparable points) contributes nothing and reads back as -1.
-        float sw = 0.f, sx = 0.f, sy = 0.f, sz = 0.f;
-        const long long row = (long long)s * N + q;
-#pragma unroll
-        for (int r = 0; r < K; ++r) {
-            const int j = nx[r];
-            const bool ok = j < M;
-            nn_idx[row * K + r] = ok ? j : -1;
-            if (!ok) continue;
-            const float wr = __fdiv_rn(1.f, __fadd_rn(nd[r], 1e-8f));
-            sx = __fadd_rn(sx, __fmul_rn(wr, __ldg(lp + 3ll * j)));
-            sy = __fadd_rn(sy, __fmul_rn(wr, __ldg(lp + 3ll * j + 1)));
-            sz = __fadd_rn(sz, __fmul_rn(wr, __ldg(lp + 3ll * j + 2)));
-            sw = __fadd_rn(sw, wr);
-        }
-        const float3 lw = laplacian_at(ws, g1 + ((long long)b * N + q) * kl, kl, q);
-        const float rx = __fsub_rn(__fdiv_rn(sx, sw), lw.x), ry = __fsub_rn(__fdiv_rn(sy, sw), lw.y),
-                    rz = __fsub_rn(__fdiv_rn(sz, sw), lw.z);
-        res[3 * row] = rx;
-        res[3 * row + 1] = ry;
-        res[3 * row + 2] = rz;
-        part = ((double)rx * (double)rx + (double)ry * (double)ry) + (double)rz * (double)rz;
-    }
+    if (q < N)
+        part = laplacian_point<K>(nd, nx, ws, l2 + (long long)b * M * 3, g1 + ((long long)b * N + q) * kl, kl, M, (long long)s * N + q, q,
+                                  nn_idx, res);
     part = warp_sum(part);
-    if (lane == 0 && part != 0.0) {
+    if (lane_id() == 0 && part != 0.0) {
         if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + (long long)s * kFxWords, part);
         else atomicAdd(acc + s, part);
     }
@@ -391,20 +261,6 @@ __global__ void __launch_bounds__(256) k_laplacian_bwd(const float* __restrict__
     }
 }
 
-template <int K>
-static void launch_fwd(dim3 grid, cudaStream_t st, bool det, const float* w, const float* p2, const float* l2, const int32_t* g1, int B,
-                       int N, int M, int kl, int32_t* nn_idx, float* res, double* acc) {
-    if (det) k_laplacian_fwd<K, true><<<grid, kLpThreads, 0, st>>>(w, p2, l2, g1, B, N, M, kl, nn_idx, res, acc);
-    else k_laplacian_fwd<K, false><<<grid, kLpThreads, 0, st>>>(w, p2, l2, g1, B, N, M, kl, nn_idx, res, acc);
-}
-
-template <int K>
-static void launch_grid(dim3 grid, cudaStream_t st, bool det, const float* w, const float* l2, const int32_t* g1, int B, int N, int M, int kl,
-                        const GridIndex& ix, int32_t* nn_idx, float* res, double* acc) {
-    if (det) k_laplacian_grid<K, true><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, kl, ix, nn_idx, res, acc);
-    else k_laplacian_grid<K, false><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, kl, ix, nn_idx, res, acc);
-}
-
 static bool bad_graph(int k, int n) { return k < 2 || k > kLpMaxGraph || k > n; }
 
 static bool bad_term(int S, int B, int N, int M, int k_lap, int k_int) {
@@ -446,20 +302,15 @@ extern "C" int pvraft_laplacian_fwd(const float* w, const float* p2, const float
     if (!w || !p2 || !l2 || !g1 || !nn_idx || !res || !acc || bad_term(S, B, N, M, k_lap, k_int))
         return fail(PVRAFT_ERR_BAD_ARG, "laplacian_fwd: bad argument");
     if (S > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "laplacian_fwd: S = %d samples (at most 65535)", S);
-    const dim3 grid((unsigned)((N + kLpPerCta - 1) / kLpPerCta), (unsigned)S);
+    const dim3 grid((unsigned)((N + kKbPerCta - 1) / kKbPerCta), (unsigned)S);
     cudaStream_t st = (cudaStream_t)stream;
     const bool det = det_workspace != nullptr;
     double* sums = det ? static_cast<double*>(det_workspace) : acc;
-    switch (k_int) {
-        case 1: launch_fwd<1>(grid, st, det, w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums); break;
-        case 2: launch_fwd<2>(grid, st, det, w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums); break;
-        case 3: launch_fwd<3>(grid, st, det, w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums); break;
-        case 4: launch_fwd<4>(grid, st, det, w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums); break;
-        case 5: launch_fwd<5>(grid, st, det, w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums); break;
-        case 6: launch_fwd<6>(grid, st, det, w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums); break;
-        case 7: launch_fwd<7>(grid, st, det, w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums); break;
-        default: launch_fwd<8>(grid, st, det, w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums); break;
-    }
+    dispatch_k<kLpMaxK>(k_int, [&](auto kc) {
+        constexpr int K = decltype(kc)::value;
+        if (det) k_laplacian_fwd<K, true><<<grid, kKbThreads, 0, st>>>(w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums);
+        else k_laplacian_fwd<K, false><<<grid, kKbThreads, 0, st>>>(w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums);
+    });
     const int rc = check_launch("laplacian_fwd");
     if (rc || !det) return rc;
     return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, S, S, 0, acc, st);
@@ -480,16 +331,11 @@ extern "C" int pvraft_laplacian_grid_fwd(const float* w, const float* p2, const 
     const dim3 grid((unsigned)((N + kGqPerCta - 1) / kGqPerCta), (unsigned)S);
     const bool det = det_workspace != nullptr;
     double* sums = det ? static_cast<double*>(det_workspace) : acc;
-    switch (k_int) {
-        case 1: launch_grid<1>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
-        case 2: launch_grid<2>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
-        case 3: launch_grid<3>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
-        case 4: launch_grid<4>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
-        case 5: launch_grid<5>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
-        case 6: launch_grid<6>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
-        case 7: launch_grid<7>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
-        default: launch_grid<8>(grid, st, det, w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums); break;
-    }
+    dispatch_k<kLpMaxK>(k_int, [&](auto kc) {
+        constexpr int K = decltype(kc)::value;
+        if (det) k_laplacian_grid<K, true><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums);
+        else k_laplacian_grid<K, false><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums);
+    });
     rc = check_launch("laplacian_grid_fwd");
     if (rc || !det) return rc;
     return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, S, S, 0, acc, st);
