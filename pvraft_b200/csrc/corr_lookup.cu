@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
         const float4* tab_g = p.tab + (size_t)b * p.M;
         int* counter = dyn ? reinterpret_cast<int*>(p.moments + (size_t)b * PVRAFT_MOMENTS + 15) : nullptr;
         if constexpr (DET)   // slot 15 of the sample's fixed-point moments
-            counter = dyn ? reinterpret_cast<int*>(reinterpret_cast<unsigned long long*>(p.moments) + ((size_t)b * PVRAFT_MOMENTS + 15) * kFxWords) : nullptr;
+            counter = dyn ? reinterpret_cast<int*>((fx_slots(p.moments) + ((size_t)b * PVRAFT_MOMENTS + 15)).base) : nullptr;
         auto claim_chunk = [&]() -> long long {   // first point of the next unclaimed chunk of this sample
             int c = 0;
             if (lane == 0) c = atomicAdd(counter, kChunk);
@@ -522,7 +522,7 @@ __global__ void __launch_bounds__(kLookupThreads, 1) k_corr_lookup(const LookupP
             if (DET && p.moments) {
                 const int which = (lane >> 1) & 15;
                 if ((lane & 1) == 0 && which < 15)
-                    fx_atomic(reinterpret_cast<unsigned long long*>(p.moments) + ((size_t)b * PVRAFT_MOMENTS + which) * kFxWords, fmom);
+                    add(fx_slots(p.moments), (size_t)b * PVRAFT_MOMENTS + which, fmom);
             } else if (p.moments) {
                 // (moments_reduce_scatter, written out)
                 double v[16];
@@ -768,7 +768,7 @@ static int corr_lookup_any(const void* corr_val, const void* corr_idx, bool half
 #undef PVRAFT_LOOKUP_CASE
 #undef PVRAFT_LOOKUP_CASE_H
     if (rc || !DET || !moments) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(ws), B, 15, PVRAFT_MOMENTS, PVRAFT_MOMENTS, moments, st);
+    return fx_flush(fx_slots(ws), B, 15, PVRAFT_MOMENTS, PVRAFT_MOMENTS, moments, st);
 }
 
 extern "C" int pvraft_corr_lookup_fwd(const float* corr_val, const int32_t* corr_idx, const float* xyz2_pad, const float* coords, int B,
@@ -788,7 +788,7 @@ extern "C" int pvraft_corr_lookup_bf16_fwd(const uint16_t* corr_val_bf16, const 
              dbg_cube, det_workspace, stream);
 }
 
-extern "C" int64_t pvraft_corr_lookup_det_workspace_bytes(int B) { return (int64_t)B * PVRAFT_MOMENTS * kFxWords * 8; }
+extern "C" int64_t pvraft_corr_lookup_det_workspace_bytes(int B) { return fx_bytes((long long)B * PVRAFT_MOMENTS); }
 
 // fp32 correlation values -> bf16 (round to nearest even), int32 candidate ids -> uint16: the 4-byte-per-candidate state
 __global__ void k_state_pack_bf16(const float* __restrict__ val, const int32_t* __restrict__ idx, long long n, uint16_t* __restrict__ val_out,

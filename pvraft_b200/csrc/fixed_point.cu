@@ -14,21 +14,19 @@ __global__ void k_fx_flush(const unsigned long long* __restrict__ acc, long long
 }
 
 template <typename T>
-static int fx_flush(const unsigned long long* acc, long long rows, long long cols, long long acc_ld, long long ld, T* out, cudaStream_t st) {
+static int flush(const unsigned long long* acc, long long rows, long long cols, long long acc_ld, long long ld, T* out, cudaStream_t st) {
     const long long n = rows * cols;
     if (n <= 0) return PVRAFT_OK;
     k_fx_flush<T><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(acc, rows, cols, acc_ld, ld, out);
     return check_launch("fx_flush");
 }
 
-int fx_flush_f64(const unsigned long long* acc, long long rows, long long cols, long long acc_ld, long long ld, double* out,
-                 cudaStream_t st) {
-    return fx_flush(acc, rows, cols, acc_ld, ld, out, st);
+int fx_flush(FxSlots acc, long long rows, long long cols, long long acc_ld, long long ld, double* out, cudaStream_t st) {
+    return flush(acc.base, rows, cols, acc_ld, ld, out, st);
 }
 
-int fx_flush_f32(const unsigned long long* acc, long long rows, long long cols, long long acc_ld, long long ld, float* out,
-                 cudaStream_t st) {
-    return fx_flush(acc, rows, cols, acc_ld, ld, out, st);
+int fx_flush(FxSlots acc, long long rows, long long cols, long long acc_ld, long long ld, float* out, cudaStream_t st) {
+    return flush(acc.base, rows, cols, acc_ld, ld, out, st);
 }
 
 }  // namespace pvraft

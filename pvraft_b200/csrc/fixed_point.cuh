@@ -14,7 +14,18 @@
 // fx_value then rounds the exact 128-bit sum to double once (round to nearest even); the flush adds that double to the
 // destination, which rounds once more (in fp32 for fp32 destinations).  The range is |sum| < 2^63; a contribution that is
 // not finite or has |v| >= 2^62 sets the flag, and the slot reads back as NaN.
+//
+// The shared code every reducing kernel uses:
+//   FxSlots, Acc<DET, T>  a typed destination: a kernel declares its accumulating parameters Acc<DET, T> -- T* in the default
+//                         instantiation, FxSlots (slots of the caller's workspace) in the DET one -- and adds with add(dst, i, v),
+//                         an atomicAdd or an exact fixed-point addition.  Structs whose layout the default kernels share carry
+//                         the workspace in their T* field and convert it with fx_slots().
+//   fx_stage_zero/flush   a CTA's slots staged in shared memory: zeroed, and later added into the global slots (empty ones
+//                         skipped), by the CTA or by the first `nt` threads of it.
+//   FxCarve               the host's description of a workspace as consecutive named slot ranges; the size query of an entry
+//                         point and its launcher run the same description.  fx_flush adds the slots into the real destination.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 
 namespace pvraft {
@@ -61,11 +72,39 @@ __device__ __forceinline__ void fx_atomic(unsigned long long* slot, const Fx& v)
 
 __device__ __forceinline__ void fx_atomic(unsigned long long* slot, double v) { fx_atomic(slot, fx_from(v)); }
 
-// dst[i] += v: an fp32 atomic, or (DET) an exact addition into slot i of the fixed-point workspace dst
-template <bool DET>
-__device__ __forceinline__ void scatter_add(float* dst, long long i, float v) {
-    if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dst) + i * kFxWords, (double)v);
-    else atomicAdd(dst + i, v);
+__device__ __forceinline__ Fx fx_load(const unsigned long long* slot) { return Fx{slot[0], slot[1], (unsigned)slot[2]}; }
+
+// kFxWords-word slots in global or shared memory: slot i starts at base + i * kFxWords
+struct FxSlots {
+    unsigned long long* base;
+    __host__ __device__ explicit operator bool() const { return base != nullptr; }
+};
+__host__ __device__ __forceinline__ FxSlots operator+(FxSlots s, long long i) { return FxSlots{s.base + i * kFxWords}; }
+// the workspace carried in a T* field of a struct that the default instantiation shares
+__host__ __device__ __forceinline__ FxSlots fx_slots(const void* ws) {
+    return FxSlots{static_cast<unsigned long long*>(const_cast<void*>(ws))};
+}
+
+// an accumulating parameter: the real destination, or (DET) slots of the fixed-point workspace
+template <bool DET, typename T = float>
+using Acc = std::conditional_t<DET, FxSlots, T* __restrict__>;
+
+// dst[i] += v: an atomic, or an exact addition into slot i
+__device__ __forceinline__ void add(float* dst, long long i, float v) { atomicAdd(dst + i, v); }
+__device__ __forceinline__ void add(double* dst, long long i, double v) { atomicAdd(dst + i, v); }
+__device__ __forceinline__ void add(FxSlots dst, long long i, double v) { fx_atomic(dst.base + i * kFxWords, v); }
+__device__ __forceinline__ void add(FxSlots dst, long long i, const Fx& v) { fx_atomic(dst.base + i * kFxWords, v); }
+
+// a CTA's n slots staged in shared memory (s), handled by its threads below nt: zero them before the first shared add, and
+// add them into the n global slots g, skipping empty ones, after the last (each behind a barrier of those threads)
+__device__ __forceinline__ void fx_stage_zero(FxSlots s, int n, int nt = blockDim.x) {
+    for (int i = threadIdx.x; i < n * kFxWords; i += nt) s.base[i] = 0ull;
+}
+__device__ __forceinline__ void fx_stage_flush(FxSlots s, int n, FxSlots g, int nt = blockDim.x) {
+    for (int i = threadIdx.x; i < n; i += nt) {
+        const Fx v = fx_load(s.base + i * kFxWords);
+        if (v.lo || v.hi || v.bad) fx_atomic(g.base + i * kFxWords, v);
+    }
 }
 
 __device__ __forceinline__ double fx_value(const unsigned long long* slot) {
@@ -91,9 +130,47 @@ __device__ __forceinline__ double fx_value(const unsigned long long* slot) {
 }
 
 // out[r * ld + c] += value of slot (r * acc_ld + c), for r < rows, c < cols (a separate launch after the accumulating kernel)
-int fx_flush_f64(const unsigned long long* acc, long long rows, long long cols, long long acc_ld, long long ld, double* out, cudaStream_t st);
-int fx_flush_f32(const unsigned long long* acc, long long rows, long long cols, long long acc_ld, long long ld, float* out, cudaStream_t st);
+int fx_flush(FxSlots acc, long long rows, long long cols, long long acc_ld, long long ld, double* out, cudaStream_t st);
+int fx_flush(FxSlots acc, long long rows, long long cols, long long acc_ld, long long ld, float* out, cudaStream_t st);
+// out[i] += value of slot i, for i < n
+template <typename T>
+inline int fx_flush(FxSlots acc, long long n, T* out, cudaStream_t st) { return fx_flush(acc, 1, n, n, 0, out, st); }
 
+inline int64_t fx_bytes(long long slots) { return slots * kFxWords * 8; }
+
+// Host: a workspace carved into consecutive slot ranges, in the order of the take() calls.  Carving a null workspace only
+// counts, so that an entry point's size query and its launcher share one description.
+struct FxCarve {
+    unsigned long long* base;
+    long long slots = 0;
+    explicit FxCarve(void* ws) : base(static_cast<unsigned long long*>(ws)) {}
+    FxSlots take(long long n) {
+        const FxSlots r{base ? base + slots * kFxWords : nullptr};
+        slots += n;
+        return r;
+    }
+    int64_t bytes() const { return fx_bytes(slots); }
+};
+
+// The [B,16] GroupNorm statistics (slot b * 16 + 2 * group + moment) of k_linear, k_tc_linear, k_setconv_edge_pairs and
+// k_edge_fwd
+inline int64_t gn_stats_ws_bytes(int B) { return fx_bytes(16ll * B); }
+inline int gn_stats_flush(void* ws, int B, double* stats, cudaStream_t st) { return fx_flush(fx_slots(ws), 16ll * B, stats, st); }
+
+// The weight gradients of k_linear_wgrad, k_linear_bwd_small and k_tc_wgrad: [cout][cin] weight slots | [cout] bias slots
+struct WgradWs {
+    FxSlots w, b;
+    int64_t bytes;
+};
+inline WgradWs wgrad_ws(void* ws, int cin, int cout) {
+    FxCarve c(ws);
+    return {c.take((long long)cout * cin), c.take(cout), c.bytes()};
+}
+// dW[o * ld + i] += slot (o, i), db[o] += slot o (db may be null)
+inline int wgrad_flush(const WgradWs& L, int cin, int cout, int ld, float* dW, float* db, cudaStream_t st) {
+    const int rc = fx_flush(L.w, cout, cin, cin, ld, dW, st);
+    return rc || !db ? rc : fx_flush(L.b, cout, db, st);
+}
 // grid caps of the deterministic instantiations: constants, so that the rows a CTA or thread sums depend on the shapes only
 constexpr long long kDetCtas = 256;
 

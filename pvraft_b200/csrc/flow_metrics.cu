@@ -12,7 +12,7 @@ namespace pvraft {
 // fixed-point workspace `acc` points at then (fixed_point.cuh)
 template <bool DET>
 __global__ void __launch_bounds__(256) k_flow_metrics(const float* __restrict__ est, const float* __restrict__ gt, const float* __restrict__ mask,
-                                                      long long points, double* __restrict__ acc) {
+                                                      long long points, Acc<DET, double> acc) {
     __shared__ double s_acc[6];
     if (threadIdx.x < 6) s_acc[threadIdx.x] = 0.0;
     __syncthreads();
@@ -33,15 +33,15 @@ __global__ void __launch_bounds__(256) k_flow_metrics(const float* __restrict__ 
 #pragma unroll
     for (int i = 0; i < 6; ++i) {
         const float s = warp_sum(v[i]);
-        if constexpr (DET) {
-            if (lane_id() == 0 && s != 0.f) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + i * kFxWords, (double)s);
-        } else {
-            if (lane_id() == 0 && s != 0.f) atomicAdd(&s_acc[i], (double)s);
+        if (lane_id() == 0 && s != 0.f) {
+            if constexpr (DET) add(acc, i, s);
+            else atomicAdd(&s_acc[i], (double)s);
         }
     }
-    if constexpr (DET) return;
-    __syncthreads();
-    if (threadIdx.x < 6 && s_acc[threadIdx.x] != 0.0) atomicAdd(acc + threadIdx.x, s_acc[threadIdx.x]);
+    if constexpr (!DET) {
+        __syncthreads();
+        if (threadIdx.x < 6 && s_acc[threadIdx.x] != 0.0) atomicAdd(acc + threadIdx.x, s_acc[threadIdx.x]);
+    }
 }
 
 // d/d est of  weight * mean_{valid points, 3 components} |est - gt|  times the upstream gradient g (device scalar)
@@ -73,13 +73,12 @@ extern "C" int pvraft_flow_metrics_fwd(const float* est, const float* gt, const 
         k_flow_metrics<false><<<(unsigned)blocks, 256, 0, st>>>(est, gt, mask, points, acc);
         return check_launch("flow_metrics");
     }
-    k_flow_metrics<true><<<(unsigned)blocks, 256, 0, st>>>(est, gt, mask, points, static_cast<double*>(det_workspace));
+    k_flow_metrics<true><<<(unsigned)blocks, 256, 0, st>>>(est, gt, mask, points, fx_slots(det_workspace));
     const int rc = check_launch("flow_metrics");
-    if (rc) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, 6, 6, 0, acc, st);
+    return rc ? rc : fx_flush(fx_slots(det_workspace), 6, acc, st);
 }
 
-extern "C" int64_t pvraft_flow_metrics_det_workspace_bytes(void) { return 6 * kFxWords * 8; }
+extern "C" int64_t pvraft_flow_metrics_det_workspace_bytes(void) { return fx_bytes(6); }
 
 extern "C" int pvraft_flow_l1_bwd(const float* est, const float* gt, const float* mask, int64_t points, const double* acc, const float* g,
                                   float weight, float* d_est, void* stream) {

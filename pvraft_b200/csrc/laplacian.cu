@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(256) k_cloud_laplacian(const float* __restrict
 // -c per such edge at i.  DET: d_x is the fixed-point workspace.
 template <bool DET>
 __global__ void __launch_bounds__(256) k_cloud_laplacian_bwd(const float* __restrict__ g_l, const int32_t* __restrict__ nbr, int N, int k,
-                                                             long long points, float* __restrict__ d_x) {
+                                                             long long points, Acc<DET> d_x) {
     const float den = (float)(k - 1);
     for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < points; p += (long long)gridDim.x * blockDim.x) {
         const long long b = p / N, i = p - b * N;
@@ -70,16 +70,16 @@ __global__ void __launch_bounds__(256) k_cloud_laplacian_bwd(const float* __rest
             const long long j = __ldg(nbr + p * k + e);
             if (j == i) continue;
             const long long r = 3 * (b * N + j);
-            scatter_add<DET>(d_x, r, cx);
-            scatter_add<DET>(d_x, r + 1, cy);
-            scatter_add<DET>(d_x, r + 2, cz);
+            add(d_x, r, cx);
+            add(d_x, r + 1, cy);
+            add(d_x, r + 2, cz);
             ox -= cx;
             oy -= cy;
             oz -= cz;
         }
-        scatter_add<DET>(d_x, 3 * p, ox);
-        scatter_add<DET>(d_x, 3 * p + 1, oy);
-        scatter_add<DET>(d_x, 3 * p + 2, oz);
+        add(d_x, 3 * p, ox);
+        add(d_x, 3 * p + 1, oy);
+        add(d_x, 3 * p + 2, oz);
     }
 }
 
@@ -120,7 +120,7 @@ __device__ __forceinline__ double laplacian_point(const float (&nd)[K], const in
 template <int K, bool DET>
 __global__ void __launch_bounds__(kKbThreads, K == 2 ? 8 : 0) k_laplacian_fwd(const float* __restrict__ w, const float* __restrict__ p2, const float* __restrict__ l2,
                                                                const int32_t* __restrict__ g1, int B, int N, int M, int kl,
-                                                               int32_t* __restrict__ nn_idx, float* __restrict__ res, double* __restrict__ acc) {
+                                                               int32_t* __restrict__ nn_idx, float* __restrict__ res, Acc<DET, double> acc) {
     const int s = blockIdx.y, b = s % B;
     const float* ws = w + (long long)s * N * 3;
     float nd[K];
@@ -132,10 +132,7 @@ __global__ void __launch_bounds__(kKbThreads, K == 2 ? 8 : 0) k_laplacian_fwd(co
         part = laplacian_point<K>(nd, nx, ws, l2 + (long long)b * M * 3, g1 + ((long long)b * N + q) * kl, kl, M, (long long)s * N + q, q,
                                   nn_idx, res);
     part = warp_sum(part);
-    if (lane_id() == 0 && part != 0.0) {
-        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + (long long)s * kFxWords, part);
-        else atomicAdd(acc + s, part);
-    }
+    if (lane_id() == 0 && part != 0.0) add(acc, s, part);
 }
 
 // The grid form of k_laplacian_fwd: the same search on the index `ix` of p2 (B samples), the same laplacian_point.  One warp
@@ -143,7 +140,7 @@ __global__ void __launch_bounds__(kKbThreads, K == 2 ? 8 : 0) k_laplacian_fwd(co
 template <int K, bool DET>
 __global__ void __launch_bounds__(kGqThreads) k_laplacian_grid(const float* __restrict__ w, const float* __restrict__ l2,
                                                                 const int32_t* __restrict__ g1, int B, int N, int M, int kl, GridIndex ix,
-                                                                int32_t* __restrict__ nn_idx, float* __restrict__ res, double* __restrict__ acc) {
+                                                                int32_t* __restrict__ nn_idx, float* __restrict__ res, Acc<DET, double> acc) {
     const int s = blockIdx.y, b = s % B;
     const int lane = lane_id();
     const int q0 = (blockIdx.x * kGqWarps + warp_id()) * kGqPerWarp;
@@ -168,10 +165,7 @@ __global__ void __launch_bounds__(kGqThreads) k_laplacian_grid(const float* __re
         }
         if (lane == 0) part += laplacian_point<K>(nd, nx, ws, lp, g1 + ((long long)b * N + q) * kl, kl, M, (long long)s * N + q, q, nn_idx, res);
     }
-    if (lane == 0 && part != 0.0) {
-        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + (long long)s * kFxWords, part);
-        else atomicAdd(acc + s, part);
-    }
+    if (lane == 0 && part != 0.0) add(acc, s, part);
 }
 
 // One thread per point (s, i) of W: d_w [S,N,3] (over G1 and at i), d_p2 [B,M,3] (the distance part; or NULL) and
@@ -181,8 +175,8 @@ template <bool DET>
 __global__ void __launch_bounds__(256) k_laplacian_bwd(const float* __restrict__ w, const float* __restrict__ p2, const float* __restrict__ l2,
                                                        const int32_t* __restrict__ g1, const int32_t* __restrict__ nn_idx,
                                                        const float* __restrict__ res, const float* __restrict__ g, int B, int N, int M,
-                                                       int kl, int k, long long points, float* __restrict__ d_w, float* __restrict__ d_p2,
-                                                       float* __restrict__ d_l2) {
+                                                       int kl, int k, long long points, Acc<DET> d_w, Acc<DET> d_p2,
+                                                       Acc<DET> d_l2) {
     const float den = (float)(kl - 1);
     for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < points; p += (long long)gridDim.x * blockDim.x) {
         const int s = (int)(p / N), b = s % B;
@@ -198,9 +192,9 @@ __global__ void __launch_bounds__(256) k_laplacian_bwd(const float* __restrict__
             const long long j = __ldg(ni + e);
             if (j == i) continue;
             const long long r = 3 * ((long long)s * N + j);
-            scatter_add<DET>(d_w, r, -cx);
-            scatter_add<DET>(d_w, r + 1, -cy);
-            scatter_add<DET>(d_w, r + 2, -cz);
+            add(d_w, r, -cx);
+            add(d_w, r + 1, -cy);
+            add(d_w, r + 2, -cz);
             ox += cx;
             oy += cy;
             oz += cz;
@@ -245,19 +239,19 @@ __global__ void __launch_bounds__(256) k_laplacian_bwd(const float* __restrict__
             oz += vz;
             const long long r = 3 * ((long long)b * M + jj[m]);
             if (d_p2) {
-                scatter_add<DET>(d_p2, r, -vx);
-                scatter_add<DET>(d_p2, r + 1, -vy);
-                scatter_add<DET>(d_p2, r + 2, -vz);
+                add(d_p2, r, -vx);
+                add(d_p2, r + 1, -vy);
+                add(d_p2, r + 2, -vz);
             }
             if (d_l2) {
-                scatter_add<DET>(d_l2, r, om * ex);
-                scatter_add<DET>(d_l2, r + 1, om * ey);
-                scatter_add<DET>(d_l2, r + 2, om * ez);
+                add(d_l2, r, om * ex);
+                add(d_l2, r + 1, om * ey);
+                add(d_l2, r + 2, om * ez);
             }
         }
-        scatter_add<DET>(d_w, 3 * p, ox);
-        scatter_add<DET>(d_w, 3 * p + 1, oy);
-        scatter_add<DET>(d_w, 3 * p + 2, oz);
+        add(d_w, 3 * p, ox);
+        add(d_w, 3 * p + 1, oy);
+        add(d_w, 3 * p + 2, oz);
     }
 }
 
@@ -289,13 +283,12 @@ extern "C" int pvraft_cloud_laplacian_bwd(const float* g_l, const int32_t* nbr, 
         k_cloud_laplacian_bwd<false><<<blocks, 256, 0, st>>>(g_l, nbr, N, k, points, d_x);
         return check_launch("cloud_laplacian_bwd");
     }
-    k_cloud_laplacian_bwd<true><<<blocks, 256, 0, st>>>(g_l, nbr, N, k, points, static_cast<float*>(det_workspace));
+    k_cloud_laplacian_bwd<true><<<blocks, 256, 0, st>>>(g_l, nbr, N, k, points, fx_slots(det_workspace));
     const int rc = check_launch("cloud_laplacian_bwd");
-    if (rc) return rc;
-    return fx_flush_f32(static_cast<const unsigned long long*>(det_workspace), 1, 3 * points, 3 * points, 0, d_x, st);
+    return rc ? rc : fx_flush(fx_slots(det_workspace), 3 * points, d_x, st);
 }
 
-extern "C" int64_t pvraft_cloud_laplacian_bwd_det_workspace_bytes(int B, int N) { return B < 1 || N < 1 ? 0 : 3ll * B * N * kFxWords * 8; }
+extern "C" int64_t pvraft_cloud_laplacian_bwd_det_workspace_bytes(int B, int N) { return B < 1 || N < 1 ? 0 : fx_bytes(3ll * B * N); }
 
 extern "C" int pvraft_laplacian_fwd(const float* w, const float* p2, const float* l2, const int32_t* g1, int S, int B, int N, int M, int k_lap,
                                     int k_int, int32_t* nn_idx, float* res, double* acc, void* det_workspace, void* stream) {
@@ -305,18 +298,16 @@ extern "C" int pvraft_laplacian_fwd(const float* w, const float* p2, const float
     const dim3 grid((unsigned)((N + kKbPerCta - 1) / kKbPerCta), (unsigned)S);
     cudaStream_t st = (cudaStream_t)stream;
     const bool det = det_workspace != nullptr;
-    double* sums = det ? static_cast<double*>(det_workspace) : acc;
     dispatch_k<kLpMaxK>(k_int, [&](auto kc) {
         constexpr int K = decltype(kc)::value;
-        if (det) k_laplacian_fwd<K, true><<<grid, kKbThreads, 0, st>>>(w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums);
-        else k_laplacian_fwd<K, false><<<grid, kKbThreads, 0, st>>>(w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, sums);
+        if (det) k_laplacian_fwd<K, true><<<grid, kKbThreads, 0, st>>>(w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, fx_slots(det_workspace));
+        else k_laplacian_fwd<K, false><<<grid, kKbThreads, 0, st>>>(w, p2, l2, g1, B, N, M, k_lap, nn_idx, res, acc);
     });
     const int rc = check_launch("laplacian_fwd");
-    if (rc || !det) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, S, S, 0, acc, st);
+    return rc || !det ? rc : fx_flush(fx_slots(det_workspace), S, acc, st);
 }
 
-extern "C" int64_t pvraft_laplacian_fwd_det_workspace_bytes(int S) { return S < 1 ? 0 : (int64_t)S * kFxWords * 8; }
+extern "C" int64_t pvraft_laplacian_fwd_det_workspace_bytes(int S) { return S < 1 ? 0 : fx_bytes(S); }
 
 extern "C" int pvraft_laplacian_grid_fwd(const float* w, const float* p2, const float* l2, const int32_t* g1, int S, int B, int N, int M,
                                          int k_lap, int k_int, int32_t* nn_idx, float* res, double* acc, void* workspace, void* det_workspace,
@@ -330,15 +321,23 @@ extern "C" int pvraft_laplacian_grid_fwd(const float* w, const float* p2, const 
     if (rc) return rc;
     const dim3 grid((unsigned)((N + kGqPerCta - 1) / kGqPerCta), (unsigned)S);
     const bool det = det_workspace != nullptr;
-    double* sums = det ? static_cast<double*>(det_workspace) : acc;
     dispatch_k<kLpMaxK>(k_int, [&](auto kc) {
         constexpr int K = decltype(kc)::value;
-        if (det) k_laplacian_grid<K, true><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums);
-        else k_laplacian_grid<K, false><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, sums);
+        if (det) k_laplacian_grid<K, true><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, fx_slots(det_workspace));
+        else k_laplacian_grid<K, false><<<grid, kGqThreads, 0, st>>>(w, l2, g1, B, N, M, k_lap, ix, nn_idx, res, acc);
     });
     rc = check_launch("laplacian_grid_fwd");
-    if (rc || !det) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, S, S, 0, acc, st);
+    return rc || !det ? rc : fx_flush(fx_slots(det_workspace), S, acc, st);
+}
+
+// laplacian_bwd's workspace: [3 S N] slots for d_w | [3 B M] for d_p2 | [3 B M] for d_l2
+struct LaplacianBwdWs {
+    FxSlots d_w, d_p2, d_l2;
+    int64_t bytes;
+};
+static LaplacianBwdWs laplacian_bwd_ws(void* ws, int S, int B, int N, int M) {
+    FxCarve c(ws);
+    return {c.take(3ll * S * N), c.take(3ll * B * M), c.take(3ll * B * M), c.bytes()};
 }
 
 extern "C" int pvraft_laplacian_bwd(const float* w, const float* p2, const float* l2, const int32_t* g1, const int32_t* nn_idx, const float* res,
@@ -354,23 +353,16 @@ extern "C" int pvraft_laplacian_bwd(const float* w, const float* p2, const float
         k_laplacian_bwd<false><<<blocks, 256, 0, st>>>(w, p2, l2, g1, nn_idx, res, g, B, N, M, k_lap, k_int, points, d_w, d_p2, d_l2);
         return check_launch("laplacian_bwd");
     }
-    // workspace: [3 S N | 3 B M | 3 B M] slots for d_w, d_p2, d_l2
-    const long long nw = 3 * points, nb = 3ll * B * M;
-    unsigned long long* ws = static_cast<unsigned long long*>(det_workspace);
-    float* ws_w = reinterpret_cast<float*>(ws);
-    float* ws_p2 = reinterpret_cast<float*>(ws + nw * kFxWords);
-    float* ws_l2 = reinterpret_cast<float*>(ws + (nw + nb) * kFxWords);
-    k_laplacian_bwd<true><<<blocks, 256, 0, st>>>(w, p2, l2, g1, nn_idx, res, g, B, N, M, k_lap, k_int, points, ws_w, d_p2 ? ws_p2 : nullptr,
-                                                  d_l2 ? ws_l2 : nullptr);
+    const LaplacianBwdWs L = laplacian_bwd_ws(det_workspace, S, B, N, M);
+    k_laplacian_bwd<true><<<blocks, 256, 0, st>>>(w, p2, l2, g1, nn_idx, res, g, B, N, M, k_lap, k_int, points, L.d_w,
+                                                  d_p2 ? L.d_p2 : FxSlots{}, d_l2 ? L.d_l2 : FxSlots{});
     int rc = check_launch("laplacian_bwd");
-    if (rc) return rc;
-    rc = fx_flush_f32(ws, 1, nw, nw, 0, d_w, st);
-    if (!rc && d_p2) rc = fx_flush_f32(reinterpret_cast<const unsigned long long*>(ws_p2), 1, nb, nb, 0, d_p2, st);
-    if (!rc && d_l2) rc = fx_flush_f32(reinterpret_cast<const unsigned long long*>(ws_l2), 1, nb, nb, 0, d_l2, st);
+    if (!rc) rc = fx_flush(L.d_w, 3 * points, d_w, st);
+    if (!rc && d_p2) rc = fx_flush(L.d_p2, 3ll * B * M, d_p2, st);
+    if (!rc && d_l2) rc = fx_flush(L.d_l2, 3ll * B * M, d_l2, st);
     return rc;
 }
 
 extern "C" int64_t pvraft_laplacian_bwd_det_workspace_bytes(int S, int B, int N, int M) {
-    if (S < 1 || B < 1 || N < 1 || M < 1) return 0;
-    return (3ll * S * N + 6ll * B * M) * kFxWords * 8;
+    return S < 1 || B < 1 || N < 1 || M < 1 ? 0 : laplacian_bwd_ws(nullptr, S, B, N, M).bytes;
 }

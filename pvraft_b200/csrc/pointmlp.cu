@@ -64,27 +64,24 @@ __device__ __forceinline__ void flush_stats(double* s_g /*[16] smem*/, double* g
 
 // DET form (fixed_point.cuh): after every tile, each thread's sums over its points of the tile enter the CTA's fixed-point
 // slots s_fx [16]; when the CTA leaves a sample these are added to the sample's slots of the [B,16] workspace
-__device__ __forceinline__ void tile_stats_fx(unsigned long long* s_fx, double* dS, double* dSS, const int* ch, int n, int cout) {
+__device__ __forceinline__ void tile_stats_fx(FxSlots s_fx, double* dS, double* dSS, const int* ch, int n, int cout) {
     const int gsz = cout / PVRAFT_GN_GROUPS;
     for (int i = 0; i < n; ++i) {
         if (ch[i] < cout && (dS[i] != 0.0 || dSS[i] != 0.0)) {
             const int g = ch[i] / gsz;
-            fx_atomic(s_fx + (g * 2) * kFxWords, dS[i]);
-            fx_atomic(s_fx + (g * 2 + 1) * kFxWords, dSS[i]);
+            add(s_fx, g * 2, dS[i]);
+            add(s_fx, g * 2 + 1, dSS[i]);
         }
         dS[i] = 0.0;
         dSS[i] = 0.0;
     }
 }
 
-__device__ __forceinline__ void flush_stats_fx(unsigned long long* s_fx, unsigned long long* gfx /*[16] slots of the sample*/) {
+__device__ __forceinline__ void flush_stats_fx(FxSlots s_fx, FxSlots gfx /*[16] slots of the sample*/) {
     __syncthreads();
-    if (threadIdx.x < 16) {
-        const Fx v{s_fx[threadIdx.x * kFxWords], s_fx[threadIdx.x * kFxWords + 1], (unsigned)s_fx[threadIdx.x * kFxWords + 2]};
-        fx_atomic(gfx + threadIdx.x * kFxWords, v);
-    }
+    fx_stage_flush(s_fx, 16, gfx);
     __syncthreads();
-    if (threadIdx.x < 16 * kFxWords) s_fx[threadIdx.x] = 0ull;
+    fx_stage_zero(s_fx, 16);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -155,9 +152,8 @@ __global__ void __launch_bounds__(kMlpThreads, 2) k_linear(const LinearParams P)
     float* s_shift = s_scale + P.KD;
     float* s_act = s_shift + P.KD;
     double* s_g = reinterpret_cast<double*>(s_act + kTP * P.AS);   // [16]  (DET: [16] fixed-point slots; a.out_stats is the workspace)
-    unsigned long long* s_fx = reinterpret_cast<unsigned long long*>(s_g);
-    if constexpr (DET)
-        if (threadIdx.x < 16 * kFxWords) s_fx[threadIdx.x] = 0ull;
+    const FxSlots s_fx = fx_slots(s_g);
+    if constexpr (DET) fx_stage_zero(s_fx, 16);
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
 
     const int w_cin = a.w_cin > 0 ? a.w_cin : a.cin;
@@ -175,7 +171,7 @@ __global__ void __launch_bounds__(kMlpThreads, 2) k_linear(const LinearParams P)
         const int b = it.sample(), p0 = it.p0(), npts = it.npts();
         if (b != cur_b) {
             if constexpr (DET) {
-                if (a.out_stats && cur_b >= 0) flush_stats_fx(s_fx, reinterpret_cast<unsigned long long*>(a.out_stats) + (size_t)cur_b * 16 * kFxWords);
+                if (a.out_stats && cur_b >= 0) flush_stats_fx(s_fx, fx_slots(a.out_stats) + cur_b * 16);
             } else {
             if (a.out_stats && cur_b >= 0) flush_stats(s_g, a.out_stats + (size_t)cur_b * 16, dS, dSS, ch, P.passes * 4, a.cout);
             }
@@ -246,7 +242,7 @@ __global__ void __launch_bounds__(kMlpThreads, 2) k_linear(const LinearParams P)
             if (a.out_stats) tile_stats_fx(s_fx, dS, dSS, ch, P.passes * 4, a.cout);
     }
     if constexpr (DET) {
-        if (a.out_stats && cur_b >= 0) flush_stats_fx(s_fx, reinterpret_cast<unsigned long long*>(a.out_stats) + (size_t)cur_b * 16 * kFxWords);
+        if (a.out_stats && cur_b >= 0) flush_stats_fx(s_fx, fx_slots(a.out_stats) + cur_b * 16);
         return;
     }
     if (a.out_stats && cur_b >= 0) flush_stats(s_g, a.out_stats + (size_t)cur_b * 16, dS, dSS, ch, P.passes * 4, a.cout);
@@ -788,14 +784,14 @@ static int linear_fwd(const pvraft_linear_args* a, void* ws, void* stream) {
     k_linear<DET><<<tile_grid(k_linear<DET>, a->B, a->N, smem), kMlpThreads, smem, (cudaStream_t)stream>>>(P);
     rc = check_launch("linear");
     if (rc || !DET || !a->out_stats) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(ws), 1, (long long)a->B * 16, (long long)a->B * 16, 0, a->out_stats, (cudaStream_t)stream);
+    return gn_stats_flush(ws, a->B, a->out_stats, (cudaStream_t)stream);
 }
 
 extern "C" int pvraft_linear_fwd(const pvraft_linear_args* a, void* det_workspace, void* stream) {
     return det_workspace ? linear_fwd<true>(a, det_workspace, stream) : linear_fwd<false>(a, nullptr, stream);
 }
 
-extern "C" int64_t pvraft_linear_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
+extern "C" int64_t pvraft_linear_det_workspace_bytes(int B) { return gn_stats_ws_bytes(B); }
 
 extern "C" int pvraft_gn_act_fwd(const float* in, const double* stats, const float* gamma, const float* beta, double count,
                                  int act, float slope, int B, int N, int C, int transpose_out, float* out, const float* slope_dev,

@@ -27,7 +27,7 @@ constexpr int kNnStage = kNnTile / kNnThreads;         // points each thread sta
 // sums (its lanes' kNnQueries minima) is fixed by the shapes.
 template <bool DET>
 __global__ void __launch_bounds__(kNnThreads) k_chamfer_nn(const float* __restrict__ a, const float* __restrict__ b, int B, int N, int M,
-                                                          int32_t* __restrict__ nn_ab, int32_t* __restrict__ nn_ba, double* __restrict__ acc) {
+                                                          int32_t* __restrict__ nn_ab, int32_t* __restrict__ nn_ba, Acc<DET, double> acc) {
     __shared__ float4 tile[2][kNnTile];
     const int s = blockIdx.y, dir = blockIdx.z;
     const float* pa = a + (long long)s * N * 3;
@@ -105,10 +105,7 @@ __global__ void __launch_bounds__(kNnThreads) k_chamfer_nn(const float* __restri
         }
     }
     sum = warp_sum(sum);
-    if (lane_id() == 0 && sum != 0.0) {
-        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + (2ll * s + dir) * kFxWords, sum);
-        else atomicAdd(acc + 2 * s + dir, sum);
-    }
+    if (lane_id() == 0 && sum != 0.0) add(acc + 2 * s, dir, sum);
 }
 
 // The grid form of k_chamfer_nn: the same nn_ab, nn_ba and minima, searched on the index ib of b (B samples) for z = 0 and
@@ -118,7 +115,7 @@ __global__ void __launch_bounds__(kNnThreads) k_chamfer_nn(const float* __restri
 template <bool DET>
 __global__ void __launch_bounds__(kGqThreads) k_chamfer_grid(const float* __restrict__ a, const float* __restrict__ b, int B, int N, int M,
                                                               GridIndex ib, GridIndex ia, int32_t* __restrict__ nn_ab, int32_t* __restrict__ nn_ba,
-                                                              double* __restrict__ acc) {
+                                                              Acc<DET, double> acc) {
     const int s = blockIdx.y, dir = blockIdx.z;
     const int nq = dir ? M : N, nc = dir ? N : M;
     const int q0 = (blockIdx.x * kGqWarps + warp_id()) * kGqPerWarp;
@@ -140,10 +137,7 @@ __global__ void __launch_bounds__(kGqThreads) k_chamfer_grid(const float* __rest
             sum += (double)bd;
         }
     }
-    if (lane_id() == 0 && sum != 0.0) {
-        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + (2ll * s + dir) * kFxWords, sum);
-        else atomicAdd(acc + 2 * s + dir, sum);
-    }
+    if (lane_id() == 0 && sum != 0.0) add(acc + 2 * s, dir, sum);
 }
 
 // Items [0, S*N): d_a[s,i] += v, d_b[s%B, nn_ab] -= v with v = 2 g_s / N (a_i - b_nn); items [S*N, S*N + S*M):
@@ -152,7 +146,7 @@ __global__ void __launch_bounds__(kGqThreads) k_chamfer_grid(const float* __rest
 template <bool DET>
 __global__ void __launch_bounds__(256) k_chamfer_bwd(const float* __restrict__ a, const float* __restrict__ b, const int32_t* __restrict__ nn_ab,
                                                      const int32_t* __restrict__ nn_ba, const float* __restrict__ g, int B, int N, int M,
-                                                     long long items_a, long long items, float* __restrict__ d_a, float* __restrict__ d_b) {
+                                                     long long items_a, long long items, Acc<DET> d_a, Acc<DET> d_b) {
     for (long long it = (long long)blockIdx.x * blockDim.x + threadIdx.x; it < items; it += (long long)gridDim.x * blockDim.x) {
         long long ia, ib;
         float c;
@@ -171,8 +165,8 @@ __global__ void __launch_bounds__(256) k_chamfer_bwd(const float* __restrict__ a
 #pragma unroll
         for (int x = 0; x < 3; ++x) {
             const float v = c * (__ldg(a + 3 * ia + x) - __ldg(b + 3 * ib + x));
-            scatter_add<DET>(d_a, 3 * ia + x, v);
-            if (d_b) scatter_add<DET>(d_b, 3 * ib + x, -v);
+            add(d_a, 3 * ia + x, v);
+            if (d_b) add(d_b, 3 * ib + x, -v);
         }
     }
 }
@@ -182,7 +176,7 @@ __global__ void __launch_bounds__(256) k_chamfer_bwd(const float* __restrict__ a
 // capped by a constant, so what a warp sums is fixed by the shapes.
 template <bool DET>
 __global__ void __launch_bounds__(256) k_flow_smooth_fwd(const float* __restrict__ f, const int32_t* __restrict__ nbr, int B, int N, int k,
-                                                         double* __restrict__ acc) {
+                                                         Acc<DET, double> acc) {
     const int s = blockIdx.y;
     const float* fs = f + (long long)s * N * 3;
     const int32_t* ns = nbr + (long long)(s % B) * N * k;
@@ -196,17 +190,14 @@ __global__ void __launch_bounds__(256) k_flow_smooth_fwd(const float* __restrict
         }
     }
     sum = warp_sum(sum);
-    if (lane_id() == 0 && sum != 0.0) {
-        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(acc) + (long long)s * kFxWords, sum);
-        else atomicAdd(acc + s, sum);
-    }
+    if (lane_id() == 0 && sum != 0.0) add(acc, s, sum);
 }
 
 // d_f[s,j] += u, d_f[s,i] -= u for every edge (i, j = nbr[i,e]), u = g_s / (N k) (f_j - f_i) / ||f_j - f_i|| (0 where f_j = f_i,
 // self edges included).  One thread per point: the scattered +u per edge, then the point's own -sum_e u (edge order).
 template <bool DET>
 __global__ void __launch_bounds__(256) k_flow_smooth_bwd(const float* __restrict__ f, const int32_t* __restrict__ nbr, const float* __restrict__ g,
-                                                         int B, int N, int k, long long points, float* __restrict__ d_f) {
+                                                         int B, int N, int k, long long points, Acc<DET> d_f) {
     for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < points; p += (long long)gridDim.x * blockDim.x) {
         const int s = (int)(p / N);
         const long long i = p - (long long)s * N;
@@ -222,16 +213,16 @@ __global__ void __launch_bounds__(256) k_flow_smooth_bwd(const float* __restrict
             if (!(n2 > 0.f)) continue;
             const float r = scale / sqrtf(n2);
             const float ux = dx * r, uy = dy * r, uz = dz * r;
-            scatter_add<DET>(d_f, 3 * j, ux);
-            scatter_add<DET>(d_f, 3 * j + 1, uy);
-            scatter_add<DET>(d_f, 3 * j + 2, uz);
+            add(d_f, 3 * j, ux);
+            add(d_f, 3 * j + 1, uy);
+            add(d_f, 3 * j + 2, uz);
             ox -= ux;
             oy -= uy;
             oz -= uz;
         }
-        scatter_add<DET>(d_f, 3 * p, ox);
-        scatter_add<DET>(d_f, 3 * p + 1, oy);
-        scatter_add<DET>(d_f, 3 * p + 2, oz);
+        add(d_f, 3 * p, ox);
+        add(d_f, 3 * p + 1, oy);
+        add(d_f, 3 * p + 2, oz);
     }
 }
 
@@ -252,13 +243,12 @@ extern "C" int pvraft_chamfer_fwd(const float* a, const float* b, int S, int B, 
         k_chamfer_nn<false><<<grid, kNnThreads, 0, st>>>(a, b, B, N, M, nn_ab, nn_ba, acc);
         return check_launch("chamfer_fwd");
     }
-    k_chamfer_nn<true><<<grid, kNnThreads, 0, st>>>(a, b, B, N, M, nn_ab, nn_ba, static_cast<double*>(det_workspace));
+    k_chamfer_nn<true><<<grid, kNnThreads, 0, st>>>(a, b, B, N, M, nn_ab, nn_ba, fx_slots(det_workspace));
     const int rc = check_launch("chamfer_fwd");
-    if (rc) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, 2ll * S, 2ll * S, 0, acc, st);
+    return rc ? rc : fx_flush(fx_slots(det_workspace), 2ll * S, acc, st);
 }
 
-extern "C" int64_t pvraft_chamfer_fwd_det_workspace_bytes(int S) { return S < 1 ? 0 : 2ll * S * kFxWords * 8; }
+extern "C" int64_t pvraft_chamfer_fwd_det_workspace_bytes(int S) { return S < 1 ? 0 : fx_bytes(2ll * S); }
 
 extern "C" int64_t pvraft_chamfer_grid_workspace_bytes(int S, int B, int N, int M) {
     if (S < 1 || B < 1 || N < 1 || M < 1) return 0;
@@ -281,10 +271,19 @@ extern "C" int pvraft_chamfer_grid_fwd(const float* a, const float* b, int S, in
         k_chamfer_grid<false><<<grid, kGqThreads, 0, st>>>(a, b, B, N, M, ib, ia, nn_ab, nn_ba, acc);
         return check_launch("chamfer_grid_fwd");
     }
-    k_chamfer_grid<true><<<grid, kGqThreads, 0, st>>>(a, b, B, N, M, ib, ia, nn_ab, nn_ba, static_cast<double*>(det_workspace));
+    k_chamfer_grid<true><<<grid, kGqThreads, 0, st>>>(a, b, B, N, M, ib, ia, nn_ab, nn_ba, fx_slots(det_workspace));
     rc = check_launch("chamfer_grid_fwd");
-    if (rc) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, 2ll * S, 2ll * S, 0, acc, st);
+    return rc ? rc : fx_flush(fx_slots(det_workspace), 2ll * S, acc, st);
+}
+
+// chamfer_bwd's workspace: [3 S N] slots for d_a | [3 B M] for d_b
+struct ChamferBwdWs {
+    FxSlots d_a, d_b;
+    int64_t bytes;
+};
+static ChamferBwdWs chamfer_bwd_ws(void* ws, int S, int B, int N, int M) {
+    FxCarve c(ws);
+    return {c.take(3ll * S * N), c.take(3ll * B * M), c.bytes()};
 }
 
 extern "C" int pvraft_chamfer_bwd(const float* a, const float* b, const int32_t* nn_ab, const int32_t* nn_ba, const float* g, int S, int B,
@@ -298,20 +297,15 @@ extern "C" int pvraft_chamfer_bwd(const float* a, const float* b, const int32_t*
         k_chamfer_bwd<false><<<blocks, 256, 0, st>>>(a, b, nn_ab, nn_ba, g, B, N, M, items_a, items, d_a, d_b);
         return check_launch("chamfer_bwd");
     }
-    const long long na = 3 * items_a, nb = 3ll * B * M;
-    float* ws_a = static_cast<float*>(det_workspace);
-    float* ws_b = reinterpret_cast<float*>(static_cast<unsigned long long*>(det_workspace) + na * kFxWords);
-    k_chamfer_bwd<true><<<blocks, 256, 0, st>>>(a, b, nn_ab, nn_ba, g, B, N, M, items_a, items, ws_a, d_b ? ws_b : nullptr);
+    const ChamferBwdWs L = chamfer_bwd_ws(det_workspace, S, B, N, M);
+    k_chamfer_bwd<true><<<blocks, 256, 0, st>>>(a, b, nn_ab, nn_ba, g, B, N, M, items_a, items, L.d_a, d_b ? L.d_b : FxSlots{});
     int rc = check_launch("chamfer_bwd");
-    if (rc) return rc;
-    rc = fx_flush_f32(reinterpret_cast<const unsigned long long*>(ws_a), 1, na, na, 0, d_a, st);
-    if (rc || !d_b) return rc;
-    return fx_flush_f32(reinterpret_cast<const unsigned long long*>(ws_b), 1, nb, nb, 0, d_b, st);
+    if (rc || (rc = fx_flush(L.d_a, 3ll * S * N, d_a, st)) || !d_b) return rc;
+    return fx_flush(L.d_b, 3ll * B * M, d_b, st);
 }
 
 extern "C" int64_t pvraft_chamfer_bwd_det_workspace_bytes(int S, int B, int N, int M) {
-    if (S < 1 || B < 1 || N < 1 || M < 1) return 0;
-    return (3ll * S * N + 3ll * B * M) * kFxWords * 8;
+    return S < 1 || B < 1 || N < 1 || M < 1 ? 0 : chamfer_bwd_ws(nullptr, S, B, N, M).bytes;
 }
 
 extern "C" int pvraft_flow_smooth_fwd(const float* f, const int32_t* nbr, int S, int B, int N, int k, double* acc, void* det_workspace,
@@ -326,13 +320,12 @@ extern "C" int pvraft_flow_smooth_fwd(const float* f, const int32_t* nbr, int S,
         k_flow_smooth_fwd<false><<<grid, 256, 0, st>>>(f, nbr, B, N, k, acc);
         return check_launch("flow_smooth_fwd");
     }
-    k_flow_smooth_fwd<true><<<grid, 256, 0, st>>>(f, nbr, B, N, k, static_cast<double*>(det_workspace));
+    k_flow_smooth_fwd<true><<<grid, 256, 0, st>>>(f, nbr, B, N, k, fx_slots(det_workspace));
     const int rc = check_launch("flow_smooth_fwd");
-    if (rc) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, S, S, 0, acc, st);
+    return rc ? rc : fx_flush(fx_slots(det_workspace), S, acc, st);
 }
 
-extern "C" int64_t pvraft_flow_smooth_fwd_det_workspace_bytes(int S) { return S < 1 ? 0 : (int64_t)S * kFxWords * 8; }
+extern "C" int64_t pvraft_flow_smooth_fwd_det_workspace_bytes(int S) { return S < 1 ? 0 : fx_bytes(S); }
 
 extern "C" int pvraft_flow_smooth_bwd(const float* f, const int32_t* nbr, const float* g, int S, int B, int N, int k, float* d_f,
                                       void* det_workspace, void* stream) {
@@ -345,10 +338,9 @@ extern "C" int pvraft_flow_smooth_bwd(const float* f, const int32_t* nbr, const 
         k_flow_smooth_bwd<false><<<blocks, 256, 0, st>>>(f, nbr, g, B, N, k, points, d_f);
         return check_launch("flow_smooth_bwd");
     }
-    k_flow_smooth_bwd<true><<<blocks, 256, 0, st>>>(f, nbr, g, B, N, k, points, static_cast<float*>(det_workspace));
+    k_flow_smooth_bwd<true><<<blocks, 256, 0, st>>>(f, nbr, g, B, N, k, points, fx_slots(det_workspace));
     const int rc = check_launch("flow_smooth_bwd");
-    if (rc) return rc;
-    return fx_flush_f32(static_cast<const unsigned long long*>(det_workspace), 1, 3 * points, 3 * points, 0, d_f, st);
+    return rc ? rc : fx_flush(fx_slots(det_workspace), 3 * points, d_f, st);
 }
 
-extern "C" int64_t pvraft_flow_smooth_bwd_det_workspace_bytes(int S, int N) { return S < 1 || N < 1 ? 0 : 3ll * S * N * kFxWords * 8; }
+extern "C" int64_t pvraft_flow_smooth_bwd_det_workspace_bytes(int S, int N) { return S < 1 || N < 1 ? 0 : fx_bytes(3ll * S * N); }

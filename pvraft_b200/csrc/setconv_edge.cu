@@ -187,7 +187,7 @@ template <int PAIRS, bool DET>
 __global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pairs(const float* __restrict__ fc1p, const int32_t* __restrict__ nbr,
                                                                      const float* __restrict__ edge_feats, const float* __restrict__ w_fc1,
                                                                      int cin, int B, int N, int C, float* __restrict__ ymax,
-                                                                     float* __restrict__ ymin, double* __restrict__ stats,
+                                                                     float* __restrict__ ymin, Acc<DET, double> stats,
                                                                      const int32_t* __restrict__ order, int rows) {
     constexpr int CW = edge_consumer_warps(PAIRS, DET), kConsumers = CW * 32, kThreads = edge_threads(PAIRS, DET);
     constexpr int BW = edge_builder_warps(PAIRS, DET), kBuilders = BW * 32;
@@ -287,8 +287,9 @@ __global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pa
     // the consumers' partials of sample b -> one global addition per (group, moment) and CTA
     auto flush = [&](int b) {
         if constexpr (DET) {
+            const FxSlots sfx{s.fx};
             bar_sync(kBarConsumers, kConsumers);
-            if (threadIdx.x < 16 * kFxWords) s.fx[threadIdx.x] = 0ull;
+            fx_stage_zero(sfx, 16, kConsumers);
             bar_sync(kBarConsumers, kConsumers);
 #pragma unroll
             for (int q = 0; q < PAIRS; ++q)
@@ -296,14 +297,11 @@ __global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pa
                 for (int h = 0; h < 2; ++h)
                     if (on[q]) {
                         const int g = (2 * lane + 64 * q + h) / gsz;
-                        fx_atomic(s.fx + (g * 2) * kFxWords, fS[q][h]);
-                        fx_atomic(s.fx + (g * 2 + 1) * kFxWords, fSS[q][h]);
+                        add(sfx, g * 2, fS[q][h]);
+                        add(sfx, g * 2 + 1, fSS[q][h]);
                     }
             bar_sync(kBarConsumers, kConsumers);
-            if (threadIdx.x < 16) {
-                const Fx v{s.fx[threadIdx.x * kFxWords], s.fx[threadIdx.x * kFxWords + 1], (unsigned)s.fx[threadIdx.x * kFxWords + 2]};
-                fx_atomic(reinterpret_cast<unsigned long long*>(stats) + ((size_t)b * 16 + threadIdx.x) * kFxWords, v);
-            }
+            fx_stage_flush(sfx, 16, stats + b * 16, kConsumers);
         } else {
             bar_sync(kBarConsumers, kConsumers);   // (the previous flush has read s.part)
 #pragma unroll
@@ -413,14 +411,16 @@ static int setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* 
     if (g > tiles) g = tiles;
     const int grid = (int)g;
     cudaStream_t st = (cudaStream_t)stream;
-    double* kstats = DET ? static_cast<double*>(ws) : stats;
+    Acc<DET, double> kstats;   // DET: the [B,16] workspace
+    if constexpr (DET) kstats = fx_slots(ws);
+    else kstats = stats;
     const auto kernel = C <= 64 ? k_setconv_edge_pairs<1, DET> : k_setconv_edge_pairs<2, DET>;
     int rc;
     if ((rc = opt_in_smem(kernel, smem))) return rc;
     launch_pdl(kernel, grid, edge_threads(C <= 64 ? 1 : 2, DET), smem, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, kstats, order, rows);
     rc = check_launch("setconv_edge");
     if (rc || !DET) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(ws), 1, (long long)B * 16, (long long)B * 16, 0, stats, st);
+    return gn_stats_flush(ws, B, stats, st);
 }
 
 extern "C" int pvraft_setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
@@ -430,4 +430,4 @@ extern "C" int pvraft_setconv_edge_fwd(const float* fc1p, const int32_t* nbr, co
     return f(fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order, det_workspace, stream);
 }
 
-extern "C" int64_t pvraft_setconv_edge_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
+extern "C" int64_t pvraft_setconv_edge_det_workspace_bytes(int B) { return gn_stats_ws_bytes(B); }

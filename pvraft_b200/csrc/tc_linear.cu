@@ -211,18 +211,18 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, float* __restrict
                 }
                 if ((t & (gsz - 1)) == 0 && t < p.cout) {
                     if constexpr (DET) {
-                        unsigned long long* fx = reinterpret_cast<unsigned long long*>(p.out_stats) + ((size_t)sample * 16 + (t / gsz) * 2) * kFxWords;
-                        fx_atomic(fx, a1);
-                        fx_atomic(fx + kFxWords, a2);
+                        const FxSlots fx = fx_slots(p.out_stats) + (sample * 16 + (t / gsz) * 2);
+                        add(fx, 0, a1);
+                        add(fx, 1, a2);
                     } else {
                     atomicAdd(p.out_stats + (size_t)sample * 16 + (t / gsz) * 2 + 0, a1);
                     atomicAdd(p.out_stats + (size_t)sample * 16 + (t / gsz) * 2 + 1, a2);
                     }
                 }
             } else if (DET && t < p.cout) {
-                unsigned long long* fx = reinterpret_cast<unsigned long long*>(p.out_stats) + ((size_t)sample * 16 + (t / gsz) * 2) * kFxWords;
-                fx_atomic(fx, a1);
-                fx_atomic(fx + kFxWords, a2);
+                const FxSlots fx = fx_slots(p.out_stats) + (sample * 16 + (t / gsz) * 2);
+                add(fx, 0, a1);
+                add(fx, 1, a2);
             } else if (t < p.cout) {
                 atomicAdd(p.out_stats + (size_t)sample * 16 + (t / gsz) * 2 + 0, a1);
                 atomicAdd(p.out_stats + (size_t)sample * 16 + (t / gsz) * 2 + 1, a2);
@@ -689,7 +689,7 @@ static int tc_linear_fwd(const pvraft_tc_linear_args* a, void* ws, void* stream)
     if (le != cudaSuccess) return fail((int)le, "tc_linear: launch failed: %s", cudaGetErrorString(le));
     rc = check_launch("tc_linear");
     if (rc || !DET || !a->out_stats) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(ws), 1, (long long)a->B * 16, (long long)a->B * 16, 0, a->out_stats, (cudaStream_t)stream);
+    return gn_stats_flush(ws, a->B, a->out_stats, (cudaStream_t)stream);
 }
 
 extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* det_workspace, void* stream) {
@@ -698,4 +698,4 @@ extern "C" int pvraft_tc_linear_fwd(const pvraft_tc_linear_args* a, void* det_wo
     return det_workspace ? tc_linear_fwd<true, false>(a, det_workspace, stream) : tc_linear_fwd<false, false>(a, nullptr, stream);
 }
 
-extern "C" int64_t pvraft_tc_linear_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
+extern "C" int64_t pvraft_tc_linear_det_workspace_bytes(int B) { return gn_stats_ws_bytes(B); }

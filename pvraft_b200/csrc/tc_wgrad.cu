@@ -27,8 +27,7 @@ constexpr int kWgTcMaxSlabs = 128;    // cap of the slab count (a constant: the 
 // NT = cout (32, 64, 96 or 128): the wgmma width
 template <int NT, bool DET>
 __global__ void __launch_bounds__(kWgTcThreads) k_tc_wgrad(const float* __restrict__ x, const float* __restrict__ dy, long long rows,
-                                                            int cin, long long slab_rows, float* __restrict__ dW, int dw_ld,
-                                                            float* __restrict__ db) {
+                                                            int cin, long long slab_rows, Acc<DET> dW, int dw_ld, Acc<DET> db) {
     constexpr int kA = 64 * kWgTcRows * 2;        // bf16 x^T tile [64 channels][32 rows]
     constexpr int kB = NT * kWgTcRows * 2;        // bf16 dy^T tile [NT channels][32 rows]
     constexpr int kChans = 64 + NT;               // channels a step loads: the CTA's 64 of x, then all NT of dy
@@ -39,7 +38,7 @@ __global__ void __launch_bounds__(kWgTcThreads) k_tc_wgrad(const float* __restri
     float* s_db = reinterpret_cast<float*>(tiles + 2 * (kA + kB));   // [8 row groups][NT] partial column sums of dy
     const int t = threadIdx.x;
     const int c0 = blockIdx.y * 64;               // first input channel of this CTA
-    const bool bias_cta = db != nullptr && blockIdx.y == 0;
+    const bool bias_cta = db && blockIdx.y == 0;
     const long long r_begin = (long long)blockIdx.x * slab_rows;
     const long long r_end = min(rows, r_begin + slab_rows);
     const int steps = r_end > r_begin ? (int)((r_end - r_begin + kWgTcRows - 1) / kWgTcRows) : 0;
@@ -111,10 +110,7 @@ __global__ void __launch_bounds__(kWgTcThreads) k_tc_wgrad(const float* __restri
         for (int e = 0; e < 4; ++e) {
             const int i = i0 + (e >> 1) * 8, o = 8 * j + 2 * (lane & 3) + (e & 1);
             const float a = acc[4 * j + e];
-            if (i < cin && a != 0.f) {
-                if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dW) + ((size_t)o * cin + i) * kFxWords, (double)a);
-                else atomicAdd(dW + (size_t)o * dw_ld + i, a);
-            }
+            if (i < cin && a != 0.f) add(dW, (size_t)o * dw_ld + i, a);
         }
     }
     if (!bias_cta) return;
@@ -131,10 +127,7 @@ __global__ void __launch_bounds__(kWgTcThreads) k_tc_wgrad(const float* __restri
         float b = 0.f;
 #pragma unroll
         for (int g = 0; g < 8; ++g) b += s_db[g * NT + t];
-        if (b != 0.f) {
-            if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(db) + (size_t)t * kFxWords, (double)b);
-            else atomicAdd(db + t, b);
-        }
+        if (b != 0.f) add(db, t, b);
     }
 }
 
@@ -156,10 +149,11 @@ static int tc_wgrad(const float* x, const float* dy, int64_t rows, int cin, int 
     const size_t smem = 1024 + 2 * (size_t)(64 + cout) * kWgTcRows * 2 + (size_t)8 * cout * sizeof(float);
     const int ld = dw_ld > 0 ? dw_ld : cin;
     cudaStream_t st = (cudaStream_t)stream;
-    unsigned long long* fx = static_cast<unsigned long long*>(ws);
-    unsigned long long* fxb = DET ? fx + (size_t)cout * cin * kFxWords : nullptr;
-    float* out_w = DET ? reinterpret_cast<float*>(fx) : dW;
-    float* out_b = DET ? (db ? reinterpret_cast<float*>(fxb) : nullptr) : db;
+    const WgradWs L = wgrad_ws(ws, cin, cout);
+    Acc<DET> out_w, out_b;   // DET: the weight slots are [cout][cin], leading dimension cin
+    int out_ld = ld;
+    if constexpr (DET) { out_w = L.w; out_b = db ? L.b : FxSlots{}; out_ld = cin; }
+    else { out_w = dW; out_b = db; }
     decltype(&k_tc_wgrad<32, DET>) kernel = nullptr;
     switch (cout) {
         case 32: kernel = k_tc_wgrad<32, DET>; break;
@@ -169,13 +163,9 @@ static int tc_wgrad(const float* x, const float* dy, int64_t rows, int cin, int 
     }
     int rc;
     if ((rc = opt_in_smem(kernel, smem))) return rc;
-    kernel<<<grid, kWgTcThreads, smem, st>>>(x, dy, rows, cin, slab_rows, out_w, ld, out_b);
-    if ((rc = check_launch("tc_wgrad_bf16"))) return rc;
-    if constexpr (DET) {
-        if ((rc = fx_flush_f32(fx, cout, cin, cin, ld, dW, st))) return rc;
-        return db ? fx_flush_f32(fxb, 1, cout, cout, cout, db, st) : 0;
-    }
-    return 0;
+    kernel<<<grid, kWgTcThreads, smem, st>>>(x, dy, rows, cin, slab_rows, out_w, out_ld, out_b);
+    if ((rc = check_launch("tc_wgrad_bf16")) || !DET) return rc;
+    return wgrad_flush(L, cin, cout, ld, dW, db, st);
 }
 
 extern "C" int pvraft_tc_wgrad_bf16(const float* x, const float* dy, int64_t rows, int cin, int cout, float* dW, int dw_ld, float* db,
@@ -184,6 +174,4 @@ extern "C" int pvraft_tc_wgrad_bf16(const float* x, const float* dy, int64_t row
     return f(x, dy, rows, cin, cout, dW, dw_ld, db, det_workspace, stream);
 }
 
-extern "C" int64_t pvraft_tc_wgrad_bf16_det_workspace_bytes(int cin, int cout) {
-    return (int64_t)((int64_t)cout * cin + cout) * kFxWords * 8;
-}
+extern "C" int64_t pvraft_tc_wgrad_bf16_det_workspace_bytes(int cin, int cout) { return wgrad_ws(nullptr, cin, cout).bytes; }

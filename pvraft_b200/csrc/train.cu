@@ -9,7 +9,7 @@
 // Reductions into parameter gradients use fp32 / fp64 atomics (order-nondeterministic, like ATen's own CUDA backward) in
 // the default instantiations.  The DET instantiations (what an entry point runs when given a det_workspace) add exact
 // fixed-point values instead (fixed_point.cuh) and size their grids from the shapes alone, so their results are bitwise
-// reproducible; their accumulator arguments then point at the caller's fixed-point workspace.
+// reproducible; their accumulating parameters (Acc<DET, T>) are then slots of the caller's fixed-point workspace.
 #include "fixed_point.cuh"
 
 namespace pvraft {
@@ -25,7 +25,7 @@ constexpr int kWgThreads = 256;
 
 template <bool DET>
 __global__ void __launch_bounds__(kWgThreads) k_linear_wgrad(const float* __restrict__ x, const float* __restrict__ dy, long long rows,
-                                                             int cin, int cout, float* __restrict__ dW, int dw_ld, float* __restrict__ db) {
+                                                             int cin, int cout, Acc<DET> dW, int dw_ld, Acc<DET> db) {
     extern __shared__ __align__(16) float smem_wg[];
     const int cin_p = (cin + 3) & ~3;
     const int xs_ld = cin_p + 4;                 // +4 floats: consecutive rows start in different bank groups
@@ -91,15 +91,9 @@ __global__ void __launch_bounds__(kWgThreads) k_linear_wgrad(const float* __rest
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int ii = ib * 4 + i;
-                    if (ii < cin && acc[t][o * 4 + i] != 0.f) {
-                        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dW) + ((size_t)oo * cin + ii) * kFxWords, (double)acc[t][o * 4 + i]);
-                        else atomicAdd(dW + (size_t)oo * dw_ld + ii, acc[t][o * 4 + i]);
-                    }
+                    if (ii < cin && acc[t][o * 4 + i] != 0.f) add(dW, (size_t)oo * dw_ld + ii, acc[t][o * 4 + i]);
                 }
-                if (db && ib == 0 && accb[t][o] != 0.f) {
-                    if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(db) + (size_t)oo * kFxWords, (double)accb[t][o]);
-                    else atomicAdd(db + oo, accb[t][o]);
-                }
+                if (db && ib == 0 && accb[t][o] != 0.f) add(db, oo, accb[t][o]);
             }
         }
     }
@@ -113,8 +107,8 @@ __global__ void __launch_bounds__(kWgThreads) k_linear_wgrad(const float* __rest
 // ---------------------------------------------------------------------------------------------------------------------
 template <int LPR, bool DET>
 __global__ void __launch_bounds__(256) k_linear_bwd_small(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ W,
-                                                          long long rows, int cin, int w_ld, float* __restrict__ dW, int dw_ld,
-                                                          float* __restrict__ db, float* __restrict__ dx) {
+                                                          long long rows, int cin, int w_ld, Acc<DET> dW, int dw_ld, Acc<DET> db,
+                                                          float* __restrict__ dx) {
     constexpr int COUT = 16 * LPR, RPW = 32 / LPR;   // LPR = 3 or 6 leaves two lanes of the warp idle
     __shared__ float4 s_w[COUT];
     __shared__ float s_acc[COUT][5];
@@ -204,12 +198,11 @@ __global__ void __launch_bounds__(256) k_linear_bwd_small(const float* __restric
             }
         }
         if (rr == 0) {
-            if constexpr (DET) {   // every warp's sums straight into the fixed-point slots [COUT][cin] | [COUT]
-                unsigned long long* fx = reinterpret_cast<unsigned long long*>(dW);
+            if constexpr (DET) {   // every warp's sums straight into the fixed-point slots
 #pragma unroll
                 for (int k = 0; k < 4; ++k)
-                    if (k < cin) fx_atomic(fx + ((size_t)(q * 16 + o) * cin + k) * kFxWords, (double)acc[o][k]);
-                if (db) fx_atomic(reinterpret_cast<unsigned long long*>(db) + (size_t)(q * 16 + o) * kFxWords, (double)accb[o]);
+                    if (k < cin) add(dW, (size_t)(q * 16 + o) * dw_ld + k, acc[o][k]);
+                if (db) add(db, q * 16 + o, accb[o]);
             } else {
 #pragma unroll
                 for (int k = 0; k < 4; ++k) atomicAdd(&s_acc[q * 16 + o][k], acc[o][k]);
@@ -223,8 +216,8 @@ __global__ void __launch_bounds__(256) k_linear_bwd_small(const float* __restric
         const int o = i / 5, k = i - o * 5;
         const float v = s_acc[o][k];
         if (v == 0.f) continue;
-        if (k < 4) { if (k < cin) atomicAdd(dW + (size_t)o * dw_ld + k, v); }
-        else if (db) atomicAdd(db + o, v);
+        if (k < 4) { if (k < cin) add(dW, (size_t)o * dw_ld + k, v); }
+        else if (db) add(db, o, v);
     }
 }
 
@@ -234,7 +227,8 @@ __global__ void __launch_bounds__(256) k_linear_bwd_small(const float* __restric
 //   dxh = g * gamma                                    dslope    += sum_{t<0} dy * t   (t = xh*gamma+beta; PReLU only)
 //   dx  = rstd * (dxh - mean_g(dxh) - xh * mean_g(dxh * xh))
 // pass 1 (k_gn_bwd_reduce) accumulates the per-(sample, group) sums and the parameter gradients in double; pass 2
-// (k_gn_bwd_apply) writes dx.  A thread keeps one channel (blockDim = C * rows-per-pass), so its group is fixed.
+// (k_gn_bwd_apply, k_gn_bwd_apply_arg) writes dx.  A thread keeps one channel (blockDim = C * rows-per-pass), so its group
+// is fixed.
 // ---------------------------------------------------------------------------------------------------------------------
 struct GnBwdParams {
     const float* x;
@@ -247,7 +241,7 @@ struct GnBwdParams {
     float slope;
     long long rows;        // rows per sample
     int B, C;
-    double* gsum;          // [B,8,2]: sum dxh, sum dxh*xh
+    double* gsum;          // [B,8,2]: sum dxh, sum dxh*xh   (pass 1 of DET: these four point at workspace slots)
     double* dgamma;        // [C]
     double* dbeta;         // [C]
     double* dslope;        // [1] or null
@@ -265,51 +259,53 @@ __device__ __forceinline__ void gn_mean_rstd(const double* st, double count, flo
     rstd = (float)rsqrt(var + 1e-5);
 }
 
-// DET: a CTA's fixed-point slots -> the workspace [B*16 gsum | C dgamma | C dbeta | 1 dslope] (p.gsum points at it)
-__device__ __forceinline__ void gn_bwd_flush_fx(const GnBwdParams& p, const unsigned long long* s_fx, int b) {
-    unsigned long long* ws = reinterpret_cast<unsigned long long*>(p.gsum);
-    for (int i = threadIdx.x; i < 16 + 2 * p.C + 1; i += blockDim.x) {
-        const Fx v{s_fx[i * kFxWords], s_fx[i * kFxWords + 1], (unsigned)s_fx[i * kFxWords + 2]};
-        if (!v.lo && !v.hi && !v.bad) continue;
-        fx_atomic(ws + (size_t)(i < 16 ? b * 16 + i : p.B * 16 + (i - 16)) * kFxWords, v);
-    }
-}
-
-template <bool DET>
+// Pass 1 for both row sources.  ARG = false: the rows of dy [B,rows,C].  ARG = true (the activation was followed by a max
+// over each point's 32 consecutive rows, GnActMaxFn): only the arg-max row of a (point, channel) carries gradient, so the
+// pass gathers ONE x per (point, channel) -- 1/32 of the tensor.  A thread's sums enter the CTA's shared sums (DET: shared
+// fixed-point slots), which are added once per CTA into the destinations (DET: their slots in the workspace, p.gsum,
+// p.dgamma, p.dbeta and p.dslope pointing at them).
+template <bool ARG, bool DET>
 __global__ void __launch_bounds__(256) k_gn_bwd_reduce(const GnBwdParams pp) {
     GnBwdParams p = pp;
     if (p.slope_dev) p.slope = __ldg(p.slope_dev);
     __shared__ double s_g[8][2];
-    __shared__ double s_par[3];   // unused slots keep the layout simple
+    __shared__ double s_par;
     __shared__ double s_ch[2][256];   // dgamma | dbeta of this CTA: ONE global atomic per channel and CTA
-    unsigned long long* s_fx = nullptr;   // DET: [16 gsum | C dgamma | C dbeta | dslope] fixed-point slots of this CTA
-    if constexpr (DET) { __shared__ unsigned long long s_fx_[(16 + 2 * 256 + 1) * kFxWords]; s_fx = s_fx_; }
+    FxSlots s_fx{};   // DET: [16 gsum | C dgamma | C dbeta | dslope] fixed-point slots of this CTA
+    if constexpr (DET) { __shared__ unsigned long long s_fx_[(16 + 2 * 256 + 1) * kFxWords]; s_fx.base = s_fx_; }
     const int b = blockIdx.y;
     const int C = p.C, gsz = C / PVRAFT_GN_GROUPS;
-    const int rpp = blockDim.x / C;   // rows per pass
+    const int rpp = blockDim.x / C;   // rows (ARG: points) per pass
     const int c = threadIdx.x % C, rl = threadIdx.x / C;
-    const bool live = rl < rpp;
     if (threadIdx.x < 16) (&s_g[0][0])[threadIdx.x] = 0.0;
-    if (threadIdx.x < 3) s_par[threadIdx.x] = 0.0;
+    if (threadIdx.x == 0) s_par = 0.0;
     s_ch[0][threadIdx.x] = 0.0;
     s_ch[1][threadIdx.x] = 0.0;
-    if constexpr (DET)
-        for (int i = threadIdx.x; i < (16 + 2 * C + 1) * kFxWords; i += blockDim.x) s_fx[i] = 0ull;
+    if constexpr (DET) fx_stage_zero(s_fx, 16 + 2 * C + 1);
     __syncthreads();
     const int g = c / gsz;
     float mean, rstd;
     gn_mean_rstd(p.stats + ((size_t)b * 8 + g) * 2, p.count, mean, rstd);
     const float ga = __ldg(p.gamma + c), be = __ldg(p.beta + c);
-    double a0 = 0.0, a1 = 0.0, dg = 0.0, dbt = 0.0, dsl = 0.0;
-    float f0 = 0.f, f1 = 0.f, fg = 0.f, fb = 0.f, fs = 0.f;
-    int pend = 0;
-    if (live) {
-        const long long base = (long long)b * p.rows;
-        for (long long r = (long long)blockIdx.x * rpp + rl; r < p.rows; r += (long long)gridDim.x * rpp) {
-            const size_t at = (size_t)(base + r) * C + c;
-            const float xh = (__ldg(p.x + at) - mean) * rstd;
+    if (rl < rpp) {
+        double a0 = 0.0, a1 = 0.0, dg = 0.0, dbt = 0.0, dsl = 0.0;
+        float f0 = 0.f, f1 = 0.f, fg = 0.f, fb = 0.f, fs = 0.f;
+        int pend = 0;
+        const long long n = ARG ? p.rows >> 5 : p.rows, base = (long long)b * n;
+        for (long long r = (long long)blockIdx.x * rpp + rl; r < n; r += (long long)gridDim.x * rpp) {
+            float xv, d;
+            if constexpr (ARG) {
+                const size_t pc = (size_t)(base + r) * C + c;
+                const int a = __ldg(p.arg + pc);
+                d = __ldg(p.dy + pc);
+                xv = __ldg(p.x + ((size_t)(base + r) * PVRAFT_KNN + a) * C + c);
+            } else {
+                const size_t at = (size_t)(base + r) * C + c;
+                xv = __ldg(p.x + at);
+                d = __ldg(p.dy + at);
+            }
+            const float xh = (xv - mean) * rstd;
             const float t = fmaf(xh, ga, be);
-            const float d = __ldg(p.dy + at);
             float gq = d;
             if (p.act == PVRAFT_ACT_RELU) gq = t > 0.f ? d : 0.f;
             else if (p.act == PVRAFT_ACT_LRELU) { gq = t >= 0.f ? d : d * p.slope; if (t < 0.f) fs += d * t; }
@@ -319,22 +315,25 @@ __global__ void __launch_bounds__(256) k_gn_bwd_reduce(const GnBwdParams pp) {
         }
         a0 += f0; a1 += f1; dg += fg; dbt += fb; dsl += fs;
         if constexpr (DET) {
-            fx_atomic(s_fx + (g * 2) * kFxWords, a0);
-            fx_atomic(s_fx + (g * 2 + 1) * kFxWords, a1);
-            fx_atomic(s_fx + (16 + c) * kFxWords, dg);
-            fx_atomic(s_fx + (16 + C + c) * kFxWords, dbt);
-            if (p.dslope && dsl != 0.0) fx_atomic(s_fx + (16 + 2 * C) * kFxWords, dsl);
+            add(s_fx, g * 2, a0);
+            add(s_fx, g * 2 + 1, a1);
+            add(s_fx, 16 + c, dg);
+            add(s_fx, 16 + C + c, dbt);
+            if (p.dslope && dsl != 0.0) add(s_fx, 16 + 2 * C, dsl);
         } else {
-        atomicAdd(&s_g[g][0], a0);
-        atomicAdd(&s_g[g][1], a1);
-        atomicAdd(&s_ch[0][c], dg);
-        atomicAdd(&s_ch[1][c], dbt);
-        if (p.dslope && dsl != 0.0) atomicAdd(&s_par[0], dsl);
+            atomicAdd(&s_g[g][0], a0);
+            atomicAdd(&s_g[g][1], a1);
+            atomicAdd(&s_ch[0][c], dg);
+            atomicAdd(&s_ch[1][c], dbt);
+            if (p.dslope && dsl != 0.0) atomicAdd(&s_par, dsl);
         }
     }
     __syncthreads();
     if constexpr (DET) {
-        gn_bwd_flush_fx(p, s_fx, b);
+        fx_stage_flush(s_fx, 16, fx_slots(p.gsum) + b * 16);
+        fx_stage_flush(s_fx + 16, C, fx_slots(p.dgamma));
+        fx_stage_flush(s_fx + (16 + C), C, fx_slots(p.dbeta));
+        if (p.dslope) fx_stage_flush(s_fx + (16 + 2 * C), 1, fx_slots(p.dslope));
         return;
     }
     if (threadIdx.x < 16) {
@@ -345,7 +344,7 @@ __global__ void __launch_bounds__(256) k_gn_bwd_reduce(const GnBwdParams pp) {
         if (s_ch[0][threadIdx.x] != 0.0) atomicAdd(p.dgamma + threadIdx.x, s_ch[0][threadIdx.x]);
         if (s_ch[1][threadIdx.x] != 0.0) atomicAdd(p.dbeta + threadIdx.x, s_ch[1][threadIdx.x]);
     }
-    if (threadIdx.x == 0 && p.dslope && s_par[0] != 0.0) atomicAdd(p.dslope, s_par[0]);
+    if (threadIdx.x == 0 && p.dslope && s_par != 0.0) atomicAdd(p.dslope, s_par);
 }
 
 __global__ void __launch_bounds__(256) k_gn_bwd_apply(const GnBwdParams pp) {
@@ -374,82 +373,7 @@ __global__ void __launch_bounds__(256) k_gn_bwd_apply(const GnBwdParams pp) {
     }
 }
 
-// The same two passes when the activation was followed by a max over each point's 32 consecutive rows (GnActMaxFn): only the
-// arg-max row of a (point, channel) carries gradient, so pass 1 gathers ONE x per (point, channel) -- 1/32 of the tensor -- and
-// pass 2 streams x -> dx in 16-byte pieces with the point's (arg, dy) held in registers across its 32 rows.
-template <bool DET>
-__global__ void __launch_bounds__(256) k_gn_bwd_reduce_arg(const GnBwdParams pp) {
-    GnBwdParams p = pp;
-    if (p.slope_dev) p.slope = __ldg(p.slope_dev);
-    __shared__ double s_g[8][2];
-    __shared__ double s_par;
-    __shared__ double s_ch[2][256];
-    unsigned long long* s_fx = nullptr;   // DET: as in k_gn_bwd_reduce
-    if constexpr (DET) { __shared__ unsigned long long s_fx_[(16 + 2 * 256 + 1) * kFxWords]; s_fx = s_fx_; }
-    const int b = blockIdx.y;
-    const int C = p.C, gsz = C / PVRAFT_GN_GROUPS;
-    const int ppp = blockDim.x / C;   // points per pass
-    const int c = threadIdx.x % C, rl = threadIdx.x / C;
-    if (threadIdx.x < 16) (&s_g[0][0])[threadIdx.x] = 0.0;
-    if (threadIdx.x == 0) s_par = 0.0;
-    s_ch[0][threadIdx.x] = 0.0;
-    s_ch[1][threadIdx.x] = 0.0;
-    if constexpr (DET)
-        for (int i = threadIdx.x; i < (16 + 2 * C + 1) * kFxWords; i += blockDim.x) s_fx[i] = 0ull;
-    __syncthreads();
-    const int g = c / gsz;
-    float mean, rstd;
-    gn_mean_rstd(p.stats + ((size_t)b * 8 + g) * 2, p.count, mean, rstd);
-    const float ga = __ldg(p.gamma + c), be = __ldg(p.beta + c);
-    if (rl < ppp) {
-        double a0 = 0.0, a1 = 0.0, dg = 0.0, dbt = 0.0, dsl = 0.0;
-        float f0 = 0.f, f1 = 0.f, fg = 0.f, fb = 0.f, fs = 0.f;
-        int pend = 0;
-        const long long pts = p.rows >> 5, pbase = (long long)b * pts;
-        for (long long pt = (long long)blockIdx.x * ppp + rl; pt < pts; pt += (long long)gridDim.x * ppp) {
-            const size_t pc = (size_t)(pbase + pt) * C + c;
-            const int a = __ldg(p.arg + pc);
-            const float d = __ldg(p.dy + pc);
-            const float xh = (__ldg(p.x + ((size_t)(pbase + pt) * PVRAFT_KNN + a) * C + c) - mean) * rstd;
-            const float t = fmaf(xh, ga, be);
-            float gq = d;
-            if (p.act == PVRAFT_ACT_RELU) gq = t > 0.f ? d : 0.f;
-            else if (p.act == PVRAFT_ACT_LRELU) { gq = t >= 0.f ? d : d * p.slope; if (t < 0.f) fs += d * t; }
-            const float dxh = gq * ga;
-            f0 += dxh; f1 += dxh * xh; fg += gq * xh; fb += gq;
-            if (++pend == 32) { a0 += f0; a1 += f1; dg += fg; dbt += fb; dsl += fs; f0 = f1 = fg = fb = fs = 0.f; pend = 0; }
-        }
-        a0 += f0; a1 += f1; dg += fg; dbt += fb; dsl += fs;
-        if constexpr (DET) {
-            fx_atomic(s_fx + (g * 2) * kFxWords, a0);
-            fx_atomic(s_fx + (g * 2 + 1) * kFxWords, a1);
-            fx_atomic(s_fx + (16 + c) * kFxWords, dg);
-            fx_atomic(s_fx + (16 + C + c) * kFxWords, dbt);
-            if (p.dslope && dsl != 0.0) fx_atomic(s_fx + (16 + 2 * C) * kFxWords, dsl);
-        } else {
-        atomicAdd(&s_g[g][0], a0);
-        atomicAdd(&s_g[g][1], a1);
-        atomicAdd(&s_ch[0][c], dg);
-        atomicAdd(&s_ch[1][c], dbt);
-        if (p.dslope && dsl != 0.0) atomicAdd(&s_par, dsl);
-        }
-    }
-    __syncthreads();
-    if constexpr (DET) {
-        gn_bwd_flush_fx(p, s_fx, b);
-        return;
-    }
-    if (threadIdx.x < 16) {
-        const double v = (&s_g[0][0])[threadIdx.x];
-        if (v != 0.0) atomicAdd(p.gsum + (size_t)b * 16 + threadIdx.x, v);
-    }
-    if (threadIdx.x < C) {
-        if (s_ch[0][threadIdx.x] != 0.0) atomicAdd(p.dgamma + threadIdx.x, s_ch[0][threadIdx.x]);
-        if (s_ch[1][threadIdx.x] != 0.0) atomicAdd(p.dbeta + threadIdx.x, s_ch[1][threadIdx.x]);
-    }
-    if (threadIdx.x == 0 && p.dslope && s_par != 0.0) atomicAdd(p.dslope, s_par);
-}
-
+// Pass 2 of the max-pooled form: x -> dx in 16-byte pieces, with the point's (arg, dy) held in registers across its 32 rows.
 __global__ void __launch_bounds__(256) k_gn_bwd_apply_arg(const GnBwdParams pp) {
     GnBwdParams p = pp;
     if (p.slope_dev) p.slope = __ldg(p.slope_dev);
@@ -532,16 +456,15 @@ __global__ void __launch_bounds__(256) k_gn_act_maxk(const float* __restrict__ x
 // ---------------------------------------------------------------------------------------------------------------------
 template <bool DET>
 __global__ void __launch_bounds__(256) k_edge_fwd(const float* __restrict__ P, const int32_t* __restrict__ nbr, float* __restrict__ E,
-                                                  int B, int N, int C, double* __restrict__ stats) {
+                                                  int B, int N, int C, Acc<DET, double> stats) {
     __shared__ double s_g[16];
     const int lane = lane_id(), w = warp_id();
     const long long pt = (long long)blockIdx.x * 8 + w;
     const int b0 = (int)(((long long)blockIdx.x * 8) / N);   // a CTA's 8 points may straddle two samples
-    unsigned long long* s_fx = nullptr;   // DET: fixed-point [16] of the CTA's first sample; `stats` is the [B,16] workspace
-    if constexpr (DET) { __shared__ unsigned long long s_fx_[16 * kFxWords]; s_fx = s_fx_; }
+    FxSlots s_fx{};   // DET: fixed-point [16] of the CTA's first sample; `stats` is the [B,16] workspace
+    if constexpr (DET) { __shared__ unsigned long long s_fx_[16 * kFxWords]; s_fx.base = s_fx_; }
     if (threadIdx.x < 16) s_g[threadIdx.x] = 0.0;
-    if constexpr (DET)
-        if (threadIdx.x < 16 * kFxWords) s_fx[threadIdx.x] = 0ull;
+    if constexpr (DET) fx_stage_zero(s_fx, 16);
     __syncthreads();
     const int gsz = C / PVRAFT_GN_GROUPS;
     if (pt < (long long)B * N) {
@@ -559,11 +482,12 @@ __global__ void __launch_bounds__(256) k_edge_fwd(const float* __restrict__ P, c
                 s += t;
                 ss += t * t;
             }
-            if (DET && stats) {   // one (point, channel) sum of 32 neighbours per contribution
-                unsigned long long* gfx = reinterpret_cast<unsigned long long*>(stats) + (size_t)b * 16 * kFxWords;
-                unsigned long long* dst = b == b0 ? s_fx : gfx;
-                fx_atomic(dst + ((c / gsz) * 2) * kFxWords, (double)s);
-                fx_atomic(dst + ((c / gsz) * 2 + 1) * kFxWords, (double)ss);
+            if constexpr (DET) {   // one (point, channel) sum of 32 neighbours per contribution
+                if (stats) {
+                    const FxSlots dst = b == b0 ? s_fx : stats + b * 16;
+                    add(dst, (c / gsz) * 2, s);
+                    add(dst, (c / gsz) * 2 + 1, ss);
+                }
             } else if (stats) {
                 if (b == b0) {
                     atomicAdd(&s_g[(c / gsz) * 2], (double)s);
@@ -577,34 +501,29 @@ __global__ void __launch_bounds__(256) k_edge_fwd(const float* __restrict__ P, c
     }
     __syncthreads();
     if constexpr (DET) {
-        if (stats && threadIdx.x < 16) {
-            const Fx v{s_fx[threadIdx.x * kFxWords], s_fx[threadIdx.x * kFxWords + 1], (unsigned)s_fx[threadIdx.x * kFxWords + 2]};
-            fx_atomic(reinterpret_cast<unsigned long long*>(stats) + ((size_t)b0 * 16 + threadIdx.x) * kFxWords, v);
-        }
-        return;
+        if (stats) fx_stage_flush(s_fx, 16, stats + b0 * 16);
+    } else if (stats && threadIdx.x < 16 && s_g[threadIdx.x] != 0.0) {
+        atomicAdd(stats + (size_t)b0 * 16 + threadIdx.x, s_g[threadIdx.x]);
     }
-    if (stats && threadIdx.x < 16 && s_g[threadIdx.x] != 0.0) atomicAdd(stats + (size_t)b0 * 16 + threadIdx.x, s_g[threadIdx.x]);
 }
 
 template <bool DET>
 __global__ void __launch_bounds__(256) k_edge_bwd(const float* __restrict__ dT, const int32_t* __restrict__ nbr, int B, int N, int C,
-                                                  float* __restrict__ dP) {
+                                                  Acc<DET> dP) {
     const int lane = lane_id(), w = warp_id();
     const long long pt = (long long)blockIdx.x * 8 + w;
     if (pt >= (long long)B * N) return;
     const int b = (int)(pt / N);
-    float* dPb = dP + (size_t)b * N * C;
+    const auto dPb = dP + (size_t)b * N * C;
     for (int c = lane; c < C; c += 32) {
         float s = 0.f;
         for (int j = 0; j < PVRAFT_KNN; ++j) {
             const int nb = __ldg(nbr + pt * PVRAFT_KNN + j);
             const float g = __ldg(dT + ((size_t)pt * PVRAFT_KNN + j) * C + c);
             s += g;
-            if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dP) + ((size_t)b * N * C + (size_t)nb * C + c) * kFxWords, (double)g);
-            else atomicAdd(dPb + (size_t)nb * C + c, g);
+            add(dPb + (size_t)nb * C, c, g);
         }
-        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(dP) + ((size_t)pt * C + c) * kFxWords, -(double)s);
-        else atomicAdd(dP + (size_t)pt * C + c, -s);
+        add(dP + (size_t)pt * C, c, -s);
     }
 }
 
@@ -715,12 +634,11 @@ __global__ void __launch_bounds__(256) k_lookup_bwd(const LookupBwdParams p) {
 // Correlation lookup, backward w.r.t. the gather table (model/corr.py:42,88-89: knn_xyz = truncate_xyz2[slot] - coords, the
 // coordinates detached):  d xyz2[b, corr_idx[b,n,knn_slot[b,n,j]], c] += g_sel[b,n,j,1+c].
 // One warp per query point, lane = selected neighbour; ids read in the stored (reordered) row order, as k_lookup_bwd does.
-// DET: d_xyz2 is the fixed-point workspace [B,M,3].
 // ---------------------------------------------------------------------------------------------------------------------
 template <bool DET>
 __global__ void __launch_bounds__(256) k_lookup_xyz_bwd(const int32_t* __restrict__ corr_idx, const int32_t* __restrict__ knn_slot,
                                                         const float* __restrict__ g_sel, int B, int N, int M, int K,
-                                                        float* __restrict__ d_xyz2) {
+                                                        Acc<DET> d_xyz2) {
     const int lane = lane_id(), w = warp_id();
     const long long pt = (long long)blockIdx.x * 8 + w;
     if (pt >= (long long)B * N) return;
@@ -729,10 +647,7 @@ __global__ void __launch_bounds__(256) k_lookup_xyz_bwd(const int32_t* __restric
     const size_t row = ((size_t)b * M + __ldg(corr_idx + pt * K + slot)) * 3;
     const float* g = g_sel + (pt * PVRAFT_KNN + lane) * 4 + 1;
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        if constexpr (DET) fx_atomic(reinterpret_cast<unsigned long long*>(d_xyz2) + (row + c) * kFxWords, (double)__ldg(g + c));
-        else atomicAdd(d_xyz2 + row + c, __ldg(g + c));
-    }
+    for (int c = 0; c < 3; ++c) add(d_xyz2, row + c, __ldg(g + c));
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -744,14 +659,14 @@ __global__ void __launch_bounds__(256) k_lookup_xyz_bwd(const int32_t* __restric
 template <int CPL, bool DET>
 __global__ void __launch_bounds__(256) k_corr_init_bwd(const float* __restrict__ g, const int32_t* __restrict__ idx, const float* __restrict__ f1,
                                                        const float* __restrict__ f2, int B, int N, int M, int K, float scale,
-                                                       float* __restrict__ d_f1, float* __restrict__ d_f2) {
+                                                       float* __restrict__ d_f1, Acc<DET> d_f2) {
     constexpr int C = CPL * 32;
     const int lane = lane_id(), w = warp_id();
     const long long row = (long long)blockIdx.x * 8 + w;
     if (row >= (long long)B * N) return;
     const int b = (int)(row / N);
     const float* f2b = f2 + (size_t)b * M * C;
-    float* d2b = d_f2 + (size_t)b * M * C;
+    const auto d2b = d_f2 + (size_t)b * M * C;
     float a[CPL], acc[CPL];
 #pragma unroll
     for (int i = 0; i < CPL; ++i) { a[i] = __ldg(f1 + row * C + lane * CPL + i) * scale; acc[i] = 0.f; }
@@ -763,14 +678,7 @@ __global__ void __launch_bounds__(256) k_corr_init_bwd(const float* __restrict__
             const float gj = __shfl_sync(kFull, gk, j);
             const int m = __shfl_sync(kFull, ik, j);
             if (gj == 0.f) continue;
-            if constexpr (DET) {   // d_f2 is the fixed-point workspace [B,M,C]
-                unsigned long long* fx = reinterpret_cast<unsigned long long*>(d_f2) + ((size_t)b * M + m) * C * kFxWords;
-#pragma unroll
-                for (int i = 0; i < CPL; ++i) {
-                    acc[i] = fmaf(gj, __ldg(f2b + (size_t)m * C + lane * CPL + i), acc[i]);
-                    fx_atomic(fx + (size_t)(lane * CPL + i) * kFxWords, (double)(gj * a[i]));
-                }
-            } else if constexpr (CPL == 4) {   // the model's C = 128: one 128-bit load and one vector reduction per lane
+            if constexpr (!DET && CPL == 4) {   // the model's C = 128: one 128-bit load and one vector reduction per lane
                 const float4 v = __ldg(reinterpret_cast<const float4*>(f2b + (size_t)m * C) + lane);
                 acc[0] = fmaf(gj, v.x, acc[0]); acc[1] = fmaf(gj, v.y, acc[1]); acc[2] = fmaf(gj, v.z, acc[2]); acc[3] = fmaf(gj, v.w, acc[3]);
                 atomicAdd(reinterpret_cast<float4*>(d2b + (size_t)m * C) + lane, make_float4(gj * a[0], gj * a[1], gj * a[2], gj * a[3]));
@@ -778,7 +686,7 @@ __global__ void __launch_bounds__(256) k_corr_init_bwd(const float* __restrict__
 #pragma unroll
                 for (int i = 0; i < CPL; ++i) {
                     acc[i] = fmaf(gj, __ldg(f2b + (size_t)m * C + lane * CPL + i), acc[i]);
-                    atomicAdd(d2b + (size_t)m * C + lane * CPL + i, gj * a[i]);
+                    add(d2b, (size_t)m * C + lane * CPL + i, gj * a[i]);
                 }
             }
         }
@@ -807,14 +715,11 @@ static int linear_wgrad(const float* x, const float* dy, int64_t rows, int cin, 
     dim3 grid((unsigned)workers, (unsigned)((cout + 31) / 32));
     const int ld = dw_ld > 0 ? dw_ld : cin;
     cudaStream_t st = (cudaStream_t)stream;
-    if constexpr (DET) {
-        unsigned long long* fx = static_cast<unsigned long long*>(ws);
-        unsigned long long* fxb = fx + (size_t)cout * cin * kFxWords;
-        k_linear_wgrad<true><<<grid, kWgThreads, smem, st>>>(x, dy, rows, cin, cout, reinterpret_cast<float*>(fx), ld,
-                                                             db ? reinterpret_cast<float*>(fxb) : nullptr);
+    if constexpr (DET) {   // the weight slots are [cout][cin]: leading dimension cin
+        const WgradWs L = wgrad_ws(ws, cin, cout);
+        k_linear_wgrad<true><<<grid, kWgThreads, smem, st>>>(x, dy, rows, cin, cout, L.w, cin, db ? L.b : FxSlots{});
         if ((rc = check_launch("linear_wgrad"))) return rc;
-        if ((rc = fx_flush_f32(fx, cout, cin, cin, ld, dW, st))) return rc;
-        return db ? fx_flush_f32(fxb, 1, cout, cout, cout, db, st) : 0;
+        return wgrad_flush(L, cin, cout, ld, dW, db, st);
     }
     k_linear_wgrad<false><<<grid, kWgThreads, smem, st>>>(x, dy, rows, cin, cout, dW, ld, db);
     return check_launch("linear_wgrad");
@@ -826,9 +731,7 @@ extern "C" int pvraft_linear_wgrad(const float* x, const float* dy, int64_t rows
     return f(x, dy, rows, cin, cout, dW, dw_ld, db, det_workspace, stream);
 }
 
-extern "C" int64_t pvraft_linear_wgrad_det_workspace_bytes(int cin, int cout) {
-    return (int64_t)((int64_t)cout * cin + cout) * kFxWords * 8;
-}
+extern "C" int64_t pvraft_linear_wgrad_det_workspace_bytes(int cin, int cout) { return wgrad_ws(nullptr, cin, cout).bytes; }
 
 template <bool DET>
 static int linear_bwd_small(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld, float* dW, int dw_ld,
@@ -845,11 +748,12 @@ static int linear_bwd_small(const float* x, const float* dy, const float* W, int
     if (ctas > cap) ctas = cap;
     const int wl = w_ld > 0 ? w_ld : cin, dl = dw_ld > 0 ? dw_ld : cin;
     cudaStream_t st = (cudaStream_t)stream;
-    unsigned long long* fx = static_cast<unsigned long long*>(ws);
-    unsigned long long* fxb = DET ? fx + (size_t)cout * cin * kFxWords : nullptr;
-    float* kdW = DET ? reinterpret_cast<float*>(fx) : dW;
-    float* kdb = DET ? (db ? reinterpret_cast<float*>(fxb) : nullptr) : db;
-#define PVRAFT_LBS(L) k_linear_bwd_small<L, DET><<<(unsigned)ctas, 256, 0, st>>>(x, dy, W, rows, cin, wl, kdW, dl, kdb, dx)
+    const WgradWs L = wgrad_ws(ws, cin, cout);
+    Acc<DET> kdW, kdb;   // DET: the weight slots are [cout][cin], leading dimension cin
+    int kdl = dl;
+    if constexpr (DET) { kdW = L.w; kdb = db ? L.b : FxSlots{}; kdl = cin; }
+    else { kdW = dW; kdb = db; }
+#define PVRAFT_LBS(LPR) k_linear_bwd_small<LPR, DET><<<(unsigned)ctas, 256, 0, st>>>(x, dy, W, rows, cin, wl, kdW, kdl, kdb, dx)
     switch (lpr) {
         case 1: PVRAFT_LBS(1); break;
         case 2: PVRAFT_LBS(2); break;
@@ -861,8 +765,7 @@ static int linear_bwd_small(const float* x, const float* dy, const float* W, int
 #undef PVRAFT_LBS
     int rc = check_launch("linear_bwd_small");
     if (rc || !DET) return rc;
-    if ((rc = fx_flush_f32(fx, cout, cin, cin, dl, dW, st))) return rc;
-    return db ? fx_flush_f32(fxb, 1, cout, cout, cout, db, st) : 0;
+    return wgrad_flush(L, cin, cout, dl, dW, db, st);
 }
 
 extern "C" int pvraft_linear_bwd_small(const float* x, const float* dy, const float* W, int64_t rows, int cin, int cout, int w_ld, float* dW,
@@ -871,8 +774,16 @@ extern "C" int pvraft_linear_bwd_small(const float* x, const float* dy, const fl
     return f(x, dy, W, rows, cin, cout, w_ld, dW, dw_ld, db, dx, det_workspace, stream);
 }
 
-extern "C" int64_t pvraft_linear_bwd_small_det_workspace_bytes(int cin, int cout) {
-    return (int64_t)((int64_t)cout * cin + cout) * kFxWords * 8;
+extern "C" int64_t pvraft_linear_bwd_small_det_workspace_bytes(int cin, int cout) { return wgrad_ws(nullptr, cin, cout).bytes; }
+
+// gn_act_bwd's workspace: [B*16 gsum | C dgamma | C dbeta | 1 dslope]
+struct GnBwdWs {
+    FxSlots gsum, dgamma, dbeta, dslope;
+    int64_t bytes;
+};
+static GnBwdWs gn_bwd_ws(void* ws, int B, int C) {
+    FxCarve c(ws);
+    return {c.take(16ll * B), c.take(C), c.take(C), c.take(1), c.bytes()};
 }
 
 template <bool DET>
@@ -884,18 +795,21 @@ static int gn_act_bwd(const float* x, const float* dy, const double* stats, cons
     if (arg && rows % PVRAFT_KNN) return fail(PVRAFT_ERR_BAD_ARG, "gn_act_bwd: the max-pooled form needs rows %% 32 == 0");
     GnBwdParams p{x, dy, stats, gamma, beta, count, act, slope, (long long)rows, B, C, gsum, dgamma, dbeta, dslope, dx, slope_dev, arg};
     GnBwdParams pr = p;   // the reducing pass: DET accumulates into the fixed-point workspace, flushed before the apply pass
-    if (DET) pr.gsum = static_cast<double*>(ws);
+    const GnBwdWs L = gn_bwd_ws(ws, B, C);
+    if (DET) {
+        pr.gsum = reinterpret_cast<double*>(L.gsum.base);
+        pr.dgamma = reinterpret_cast<double*>(L.dgamma.base);
+        pr.dbeta = reinterpret_cast<double*>(L.dbeta.base);
+        pr.dslope = dslope ? reinterpret_cast<double*>(L.dslope.base) : nullptr;
+    }
     const long long cap = ((DET ? kDetCtas * 4 : (long long)sm_count() * 8) + B - 1) / B;
     cudaStream_t st = (cudaStream_t)stream;
     auto flush = [&]() -> int {
         if (!DET) return 0;
-        const unsigned long long* fx = static_cast<const unsigned long long*>(ws);
         int rc;
-        if ((rc = fx_flush_f64(fx, 1, (long long)B * 16, (long long)B * 16, 0, gsum, st))) return rc;
-        fx += (size_t)B * 16 * kFxWords;
-        if ((rc = fx_flush_f64(fx, 1, C, C, 0, dgamma, st))) return rc;
-        if ((rc = fx_flush_f64(fx + (size_t)C * kFxWords, 1, C, C, 0, dbeta, st))) return rc;
-        return dslope ? fx_flush_f64(fx + (size_t)2 * C * kFxWords, 1, 1, 1, 0, dslope, st) : 0;
+        if ((rc = fx_flush(L.gsum, 16ll * B, gsum, st)) || (rc = fx_flush(L.dgamma, C, dgamma, st)) || (rc = fx_flush(L.dbeta, C, dbeta, st)))
+            return rc;
+        return dslope ? fx_flush(L.dslope, 1, dslope, st) : 0;
     };
     if (arg) {
         const long long pts = rows / PVRAFT_KNN;
@@ -903,7 +817,7 @@ static int gn_act_bwd(const float* x, const float* dy, const double* stats, cons
         long long wr = (pts + ppp_r * 16 - 1) / (ppp_r * 16), wa = (pts + ppp_a - 1) / ppp_a;   // >= 16 points per reducing thread
         if (wr > cap) wr = cap;
         if (wa > cap) wa = cap;
-        k_gn_bwd_reduce_arg<DET><<<dim3((unsigned)wr, (unsigned)B), 256, 0, st>>>(pr);
+        k_gn_bwd_reduce<true, DET><<<dim3((unsigned)wr, (unsigned)B), 256, 0, st>>>(pr);
         int rc = check_launch("gn_bwd_reduce_arg");
         if (rc || (rc = flush())) return rc;
         k_gn_bwd_apply_arg<<<dim3((unsigned)wa, (unsigned)B), 256, 0, st>>>(p);
@@ -914,7 +828,7 @@ static int gn_act_bwd(const float* x, const float* dy, const double* stats, cons
     if (workers > cap) workers = cap;
     if (wr > cap) wr = cap;
     dim3 grid((unsigned)workers, (unsigned)B);
-    k_gn_bwd_reduce<DET><<<dim3((unsigned)wr, (unsigned)B), 256, 0, st>>>(pr);
+    k_gn_bwd_reduce<false, DET><<<dim3((unsigned)wr, (unsigned)B), 256, 0, st>>>(pr);
     int rc = check_launch("gn_bwd_reduce");
     if (rc || (rc = flush())) return rc;
     k_gn_bwd_apply<<<grid, 256, 0, st>>>(p);
@@ -928,9 +842,7 @@ extern "C" int pvraft_gn_act_bwd(const float* x, const float* dy, const double* 
     return f(x, dy, stats, gamma, beta, count, act, slope, B, rows, C, gsum, dgamma, dbeta, dslope, dx, slope_dev, arg, det_workspace, stream);
 }
 
-extern "C" int64_t pvraft_gn_act_bwd_det_workspace_bytes(int B, int C) {
-    return (int64_t)((int64_t)B * 16 + 2 * (int64_t)C + 1) * kFxWords * 8;
-}
+extern "C" int64_t pvraft_gn_act_bwd_det_workspace_bytes(int B, int C) { return gn_bwd_ws(nullptr, B, C).bytes; }
 
 extern "C" int pvraft_gn_act_maxk_fwd(const float* x, const double* stats, const float* gamma, const float* beta, double count, int act,
                                       float slope, int B, int64_t pts_per_sample, int C, float* y, uint8_t* arg, const float* slope_dev,
@@ -953,13 +865,13 @@ extern "C" int pvraft_edge_fwd(const float* P, const int32_t* nbr, float* E, int
         k_edge_fwd<false><<<blocks, 256, 0, st>>>(P, nbr, E, B, N, C, stats);
         return check_launch("edge_fwd");
     }
-    k_edge_fwd<true><<<blocks, 256, 0, st>>>(P, nbr, E, B, N, C, stats ? static_cast<double*>(det_workspace) : nullptr);
+    k_edge_fwd<true><<<blocks, 256, 0, st>>>(P, nbr, E, B, N, C, stats ? fx_slots(det_workspace) : FxSlots{});
     const int rc = check_launch("edge_fwd");
     if (rc || !stats) return rc;
-    return fx_flush_f64(static_cast<const unsigned long long*>(det_workspace), 1, (long long)B * 16, (long long)B * 16, 0, stats, st);
+    return gn_stats_flush(det_workspace, B, stats, st);
 }
 
-extern "C" int64_t pvraft_edge_fwd_det_workspace_bytes(int B) { return (int64_t)B * 16 * kFxWords * 8; }
+extern "C" int64_t pvraft_edge_fwd_det_workspace_bytes(int B) { return gn_stats_ws_bytes(B); }
 
 extern "C" int pvraft_edge_bwd(const float* dT, const int32_t* nbr, int B, int N, int C, float* dP, void* det_workspace, void* stream) {
     if (!dT || !nbr || !dP || B <= 0 || N <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "edge_bwd: bad argument");
@@ -970,13 +882,12 @@ extern "C" int pvraft_edge_bwd(const float* dT, const int32_t* nbr, int B, int N
         k_edge_bwd<false><<<blocks, 256, 0, st>>>(dT, nbr, B, N, C, dP);
         return check_launch("edge_bwd");
     }
-    k_edge_bwd<true><<<blocks, 256, 0, st>>>(dT, nbr, B, N, C, static_cast<float*>(det_workspace));
+    k_edge_bwd<true><<<blocks, 256, 0, st>>>(dT, nbr, B, N, C, fx_slots(det_workspace));
     const int rc = check_launch("edge_bwd");
-    if (rc) return rc;
-    return fx_flush_f32(static_cast<const unsigned long long*>(det_workspace), 1, pts * C, pts * C, 0, dP, st);
+    return rc ? rc : fx_flush(fx_slots(det_workspace), pts * C, dP, st);
 }
 
-extern "C" int64_t pvraft_edge_bwd_det_workspace_bytes(int B, int N, int C) { return (int64_t)B * N * C * kFxWords * 8; }
+extern "C" int64_t pvraft_edge_bwd_det_workspace_bytes(int B, int N, int C) { return fx_bytes((long long)B * N * C); }
 
 extern "C" int pvraft_maxk_fwd(const float* x, int64_t pts, int C, float* y, uint8_t* arg, void* stream) {
     if (!x || !y || !arg || pts <= 0 || C <= 0) return fail(PVRAFT_ERR_BAD_ARG, "maxk_fwd: bad argument");
@@ -1027,21 +938,21 @@ extern "C" int pvraft_corr_lookup_xyz_bwd(const int32_t* corr_idx, const int32_t
         k_lookup_xyz_bwd<false><<<blocks, 256, 0, st>>>(corr_idx, knn_slot, g_sel, B, N, M, K, d_xyz2);
         return check_launch("corr_lookup_xyz_bwd");
     }
-    k_lookup_xyz_bwd<true><<<blocks, 256, 0, st>>>(corr_idx, knn_slot, g_sel, B, N, M, K, static_cast<float*>(det_workspace));
+    k_lookup_xyz_bwd<true><<<blocks, 256, 0, st>>>(corr_idx, knn_slot, g_sel, B, N, M, K, fx_slots(det_workspace));
     const int rc = check_launch("corr_lookup_xyz_bwd");
-    if (rc) return rc;
-    const long long vals = (long long)B * M * 3;
-    return fx_flush_f32(static_cast<const unsigned long long*>(det_workspace), 1, vals, vals, 0, d_xyz2, st);
+    return rc ? rc : fx_flush(fx_slots(det_workspace), 3ll * B * M, d_xyz2, st);
 }
 
-extern "C" int64_t pvraft_corr_lookup_xyz_bwd_det_workspace_bytes(int B, int M) { return (int64_t)B * M * 3 * kFxWords * 8; }
+extern "C" int64_t pvraft_corr_lookup_xyz_bwd_det_workspace_bytes(int B, int M) { return fx_bytes(3ll * B * M); }
 
 template <bool DET>
 static int corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M, int C, int K,
                          float* d_fmap1, float* d_fmap2, void* ws, void* stream) {
     if (!g || !idx || !fmap1 || !fmap2 || !d_fmap1 || !d_fmap2 || B <= 0 || N <= 0 || M <= 0 || K <= 0)
         return fail(PVRAFT_ERR_BAD_ARG, "corr_init_bwd: bad argument");
-    float* kd2 = DET ? static_cast<float*>(ws) : d_fmap2;
+    Acc<DET> kd2;   // DET: the workspace [B,M,C]
+    if constexpr (DET) kd2 = fx_slots(ws);
+    else kd2 = d_fmap2;
     const long long rows = (long long)B * N;
     const unsigned blocks = (unsigned)((rows + 7) / 8);
     const float scale = 1.0f / sqrtf((float)C);
@@ -1053,10 +964,8 @@ static int corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1,
         case 256: k_corr_init_bwd<8, DET><<<blocks, 256, 0, st>>>(g, idx, fmap1, fmap2, B, N, M, K, scale, d_fmap1, kd2); break;
         default: return fail(PVRAFT_ERR_UNSUPPORTED, "corr_init_bwd: C=%d (32, 64, 128, 256)", C);
     }
-    int rc = check_launch("corr_init_bwd");
-    if (rc || !DET) return rc;
-    const long long rows2 = (long long)B * M;
-    return fx_flush_f32(static_cast<const unsigned long long*>(ws), 1, rows2 * C, rows2 * C, 0, d_fmap2, st);
+    const int rc = check_launch("corr_init_bwd");
+    return rc || !DET ? rc : fx_flush(fx_slots(ws), (long long)B * M * C, d_fmap2, st);
 }
 
 extern "C" int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const float* fmap1, const float* fmap2, int B, int N, int M, int C,
@@ -1065,4 +974,4 @@ extern "C" int pvraft_corr_init_bwd(const float* g, const int32_t* idx, const fl
     return f(g, idx, fmap1, fmap2, B, N, M, C, K, d_fmap1, d_fmap2, det_workspace, stream);
 }
 
-extern "C" int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int M, int C) { return (int64_t)B * M * C * kFxWords * 8; }
+extern "C" int64_t pvraft_corr_init_bwd_det_workspace_bytes(int B, int M, int C) { return fx_bytes((long long)B * M * C); }
