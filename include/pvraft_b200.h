@@ -676,6 +676,42 @@ PVRAFT_API int pvraft_laplacian_bwd(const float* w, const float* p2, const float
                                     void* det_workspace, void* stream);
 PVRAFT_API int64_t pvraft_laplacian_bwd_det_workspace_bytes(int S, int B, int N, int M);
 
+/* The forward-backward consistency of a pair of flows (UnFlow's term and occlusion test, for scene flow): W = P1 + f12 moved
+ * by the reverse flow found there should land back on P1.  Same sample stacking as above (sample s pairs with batch entry
+ * s % B of p2 and with prediction s of f21); the search and the interpolation are pvraft_laplacian_fwd's, bit for bit, with
+ * the reverse flow as the interpolated field.  Null pointers, S < 1, B < 1, S % B != 0, N < 1, M < 1, k outside
+ * 1..min(8, M), and alpha or beta negative or not finite return PVRAFT_ERR_BAD_ARG before any launch.
+ *   pvraft_flow_consistency_fwd: w [S,N,3] (W = P1 + f12), f12 [S,N,3], p2 [B,M,3], f21 [S,M,3]
+ *       -> nn_idx [S,N,k] int32: the k nearest of w[s,i] in p2[s%B] ranked on (||w_i - p2_j||^2, j), nearest first (an
+ *          unfilled slot, possible only with non-finite coordinates, reads -1);
+ *          res [S,N,3]: r_i = f12_i + bhat_i, bhat_i = sum_r w_r f21[s,j_r] / sum_r w_r, w_r = 1 / (d_r + 1e-8) on the SQUARED
+ *          distance d_r (fp32, nearest first);
+ *          ok [S,N] uint8: ||r_i||^2 < alpha (||f12_i||^2 + ||bhat_i||^2) + beta, each squared length in double;
+ *          acc [S] double (ZEROED by the caller) += sum_i ||r_i||^2, each point's term in double:  F_s = acc[s] / N.
+ *          A brute-force search of S N M pairs.
+ *   pvraft_flow_consistency_bwd: g [S] the DEVICE upstream gradient of F_s, the forward's nn_idx and res, neighbours held
+ *       fixed; e_i = 2 g_s / N r_i ->
+ *          d_f12 [S,N,3] = e_i and d_w [S,N,3] = sum_r (dbhat/dd_r . e_i) 2 (w_i - p2_{j_r}), dbhat/dd_r = -(w_r / sum w)^2
+ *          sum_q w_q (f21_{j_r} - f21_{j_q}): both WRITTEN, every element once;
+ *          d_p2 [B,M,3] (or NULL): the negated distance terms at p2_{j_r};  d_f21 [S,M,3]: (w_r / sum w) e_i at j_r.  Both
+ *          ACCUMULATED, zeroed by the caller.
+ * Accumulation: acc in double atomics, d_p2 and d_f21 in fp32 atomics (order varies run to run); with a det_workspace in the
+ * fixed-point form ("Deterministic mode"). */
+PVRAFT_API int pvraft_flow_consistency_fwd(const float* w, const float* f12, const float* p2, const float* f21, int S, int B, int N, int M,
+                                           int k, float alpha, float beta, int32_t* nn_idx, float* res, uint8_t* ok, double* acc,
+                                           void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_flow_consistency_fwd_det_workspace_bytes(int S);
+/* The same pvraft_flow_consistency_fwd results (nn_idx, res and ok bitwise; acc up to summation order) from a search on a
+ * uniform-grid index of p2.  workspace: pvraft_grid_index_workspace_bytes(B, M) bytes, 16-byte aligned; det_workspace:
+ * pvraft_flow_consistency_fwd_det_workspace_bytes(S) bytes or NULL. */
+PVRAFT_API int pvraft_flow_consistency_grid_fwd(const float* w, const float* f12, const float* p2, const float* f21, int S, int B, int N,
+                                                int M, int k, float alpha, float beta, int32_t* nn_idx, float* res, uint8_t* ok,
+                                                double* acc, void* workspace, void* det_workspace, void* stream);
+PVRAFT_API int pvraft_flow_consistency_bwd(const float* w, const float* p2, const float* f21, const int32_t* nn_idx, const float* res,
+                                           const float* g, int S, int B, int N, int M, int k, float* d_w, float* d_f12, float* d_p2,
+                                           float* d_f21, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_flow_consistency_bwd_det_workspace_bytes(int S, int B, int M);
+
 /* Flow propagation along a scan sequence (no counterpart in the reference, which estimates one pair at a time): carries a
  * flow defined on one cloud onto the points of another, the warm start of the next pair under a constant-velocity
  * assumption (pvraft_b200.stream.SceneFlowStream).

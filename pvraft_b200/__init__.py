@@ -4,6 +4,7 @@ from .corr import CorrBlock
 from .extractor import FlotEncoder
 from .gconv import SetConv
 from .graph import Graph
+from .loss import flow_consistency
 from .pointconv import knn_point, square_distance
 from .raft import RSF, RSF_refine
 from .refine import FlotRefine
@@ -11,4 +12,5 @@ from .stream import SceneFlowStream
 from .update import ConvGRU, ConvRNN, FlowHead, MotionEncoder, UpdateBlock
 
 __all__ = ['RSF', 'RSF_refine', 'CorrBlock', 'UpdateBlock', 'MotionEncoder', 'ConvGRU', 'ConvRNN', 'FlowHead',
-           'FlotEncoder', 'FlotRefine', 'SetConv', 'Graph', 'knn_point', 'square_distance', 'SceneFlowStream']
+           'FlotEncoder', 'FlotRefine', 'SetConv', 'Graph', 'knn_point', 'square_distance', 'SceneFlowStream',
+           'flow_consistency']

@@ -158,6 +158,14 @@ _SIGNATURES = {
     'pvraft_chamfer_grid_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP]),
     'pvraft_laplacian_grid_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP,
                                             VP]),
+    'pvraft_flow_consistency_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, VP, VP,
+                                              VP, VP, VP, VP]),
+    'pvraft_flow_consistency_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_flow_consistency_grid_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, VP,
+                                                   VP, VP, VP, VP, VP, VP]),
+    'pvraft_flow_consistency_bwd': (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP,
+                                              VP]),
+    'pvraft_flow_consistency_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
     'pvraft_sizeof': (C.c_int, [C.c_int]),
     'pvraft_transpose_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, VP]),
 }

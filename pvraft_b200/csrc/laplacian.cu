@@ -14,18 +14,14 @@
 //
 // Backward, with the neighbours held fixed: e_i = dR/d(residual_i) = 2 g_s / N (Lhat_i - L(W)_i).
 //   through L(W):  -e_i / (k_lap - 1) at every neighbour j != i of G1(i), +e_i / (k_lap - 1) per such edge at i;
-//   through Lhat:  dLhat/dL2[j_m] = w_m / sum w, and dLhat/dd_m = -(w_m^2 / sum w) (L2_m - Lhat) = -(w_m / sum w)^2 sum_r w_r
-//                  (L2_m - L2_r).  Evaluating L2_m - Lhat as that weighted sum of differences keeps it accurate when one
-//                  weight dominates (a duplicated point: d = 0, w = 1e8), where Lhat and L2_m agree to nearly every bit and
-//                  their difference, multiplied by w_m^2 / sum w ~ 1e8, would be rounding noise.
-//                  dd_m/dW_i = 2 (W_i - P2_m) = -dd_m/dP2_m.
+//   through Lhat:  the backward of the interpolation (idw_bwd in idw.cuh, with the field L2).
 //   k_cloud_laplacian_bwd carries dL2 into P2 over G2.
-#include "fixed_point.cuh"
 #include "grid_index.cuh"
+#include "idw.cuh"
 
 namespace pvraft {
 
-constexpr int kLpMaxK = 8;                             // interpolation neighbours k_int
+constexpr int kLpMaxK = kIdwMaxK;                      // interpolation neighbours k_int
 constexpr int kLpMaxGraph = 32;                        // graph neighbours k_lap (the kNN kernel's limit)
 
 // L(x)_i over the graph row nbr_i (k ids into x): the fp32 differences summed in edge order, then divided by k - 1.  A self
@@ -85,28 +81,15 @@ __global__ void __launch_bounds__(256) k_cloud_laplacian_bwd(const float* __rest
 
 // The per-query step after the search, shared by k_laplacian_fwd and k_laplacian_grid: from the k_int nearest (nd, nx) of
 // w_q, nearest first, write nn_idx and the residual of row `row` and return its squared length in double.
-// Lhat = sum_r w_r L2[j_r] / sum_r w_r, summed in fp32 nearest first.  An unfilled slot (only possible when non-finite
-// coordinates leave fewer than K comparable points) contributes nothing and reads back as -1.
+// Lhat is the interpolation of L2 (idw_sums in idw.cuh).
 template <int K>
 __device__ __forceinline__ double laplacian_point(const float (&nd)[K], const int (&nx)[K], const float* ws,
                                                   const float* lp, const int32_t* g1_q, int kl, int M, long long row,
                                                   int q, int32_t* nn_idx, float* res) {
-    float sw = 0.f, sx = 0.f, sy = 0.f, sz = 0.f;
-#pragma unroll
-    for (int r = 0; r < K; ++r) {
-        const int j = nx[r];
-        const bool ok = j < M;
-        nn_idx[row * K + r] = ok ? j : -1;
-        if (!ok) continue;
-        const float wr = __fdiv_rn(1.f, __fadd_rn(nd[r], 1e-8f));
-        sx = __fadd_rn(sx, __fmul_rn(wr, __ldg(lp + 3ll * j)));
-        sy = __fadd_rn(sy, __fmul_rn(wr, __ldg(lp + 3ll * j + 1)));
-        sz = __fadd_rn(sz, __fmul_rn(wr, __ldg(lp + 3ll * j + 2)));
-        sw = __fadd_rn(sw, wr);
-    }
+    const float4 t = idw_sums<K>(nd, nx, lp, M, nn_idx + row * K);
     const float3 lw = laplacian_at(ws, g1_q, kl, q);
-    const float rx = __fsub_rn(__fdiv_rn(sx, sw), lw.x), ry = __fsub_rn(__fdiv_rn(sy, sw), lw.y),
-                rz = __fsub_rn(__fdiv_rn(sz, sw), lw.z);
+    const float rx = __fsub_rn(__fdiv_rn(t.x, t.w), lw.x), ry = __fsub_rn(__fdiv_rn(t.y, t.w), lw.y),
+                rz = __fsub_rn(__fdiv_rn(t.z, t.w), lw.z);
     res[3 * row] = rx;
     res[3 * row + 1] = ry;
     res[3 * row + 2] = rz;
@@ -201,54 +184,8 @@ __global__ void __launch_bounds__(256) k_laplacian_bwd(const float* __restrict__
         }
 
         // through Lhat_i
-        const float wx = __ldg(w + 3 * p), wy = __ldg(w + 3 * p + 1), wz = __ldg(w + 3 * p + 2);
-        int jj[kLpMaxK];
-        float wt[kLpMaxK], dx[kLpMaxK], dy[kLpMaxK], dz[kLpMaxK], lx[kLpMaxK], ly[kLpMaxK], lz[kLpMaxK];
-        float sw = 0.f;
-#pragma unroll
-        for (int r = 0; r < kLpMaxK; ++r) {
-            jj[r] = r < k ? __ldg(nn_idx + p * k + r) : -1;
-            wt[r] = dx[r] = dy[r] = dz[r] = lx[r] = ly[r] = lz[r] = 0.f;
-            if (jj[r] < 0) continue;
-            const long long m = 3 * ((long long)b * M + jj[r]);
-            dx[r] = __fsub_rn(wx, __ldg(p2 + m));
-            dy[r] = __fsub_rn(wy, __ldg(p2 + m + 1));
-            dz[r] = __fsub_rn(wz, __ldg(p2 + m + 2));
-            lx[r] = __ldg(l2 + m);
-            ly[r] = __ldg(l2 + m + 1);
-            lz[r] = __ldg(l2 + m + 2);
-            const float d = __fadd_rn(__fadd_rn(__fmul_rn(dx[r], dx[r]), __fmul_rn(dy[r], dy[r])), __fmul_rn(dz[r], dz[r]));
-            wt[r] = __fdiv_rn(1.f, __fadd_rn(d, 1e-8f));   // the forward's weight, bit for bit
-            sw = __fadd_rn(sw, wt[r]);
-        }
-#pragma unroll
-        for (int m = 0; m < kLpMaxK; ++m) {
-            if (jj[m] < 0) continue;
-            float tx = 0.f, ty = 0.f, tz = 0.f;   // sum_r w_r (L2_m - L2_r) = sum w (L2_m - Lhat)
-#pragma unroll
-            for (int r = 0; r < kLpMaxK; ++r) {
-                tx += wt[r] * (lx[m] - lx[r]);
-                ty += wt[r] * (ly[m] - ly[r]);
-                tz += wt[r] * (lz[m] - lz[r]);
-            }
-            const float om = __fdiv_rn(wt[m], sw);
-            const float gd = -2.f * om * om * ((ex * tx + ey * ty) + ez * tz);   // dR/dd_m times dd_m/d(W_i - P2_m) = 2 (W_i - P2_m)
-            const float vx = gd * dx[m], vy = gd * dy[m], vz = gd * dz[m];
-            ox += vx;
-            oy += vy;
-            oz += vz;
-            const long long r = 3 * ((long long)b * M + jj[m]);
-            if (d_p2) {
-                add(d_p2, r, -vx);
-                add(d_p2, r + 1, -vy);
-                add(d_p2, r + 2, -vz);
-            }
-            if (d_l2) {
-                add(d_l2, r, om * ex);
-                add(d_l2, r + 1, om * ey);
-                add(d_l2, r + 2, om * ez);
-            }
-        }
+        idw_bwd<DET>(__ldg(w + 3 * p), __ldg(w + 3 * p + 1), __ldg(w + 3 * p + 2), p2, l2, nn_idx, p, k, b, b, M, ex, ey, ez, ox, oy, oz,
+                     d_p2, d_l2);
         add(d_w, 3 * p, ox);
         add(d_w, 3 * p + 1, oy);
         add(d_w, 3 * p + 2, oz);

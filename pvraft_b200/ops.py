@@ -725,7 +725,8 @@ def _loss_batch(what, x, b_rows, m=None):
 # brute force.  Both forms return the same neighbours in the same order, so the choice only changes the time.  Measured with
 # tools/grid_search_cost.py on an H100 80GB HBM3 at 700 W (DESIGN.md 4.4): at N = M = 8192 the grid form of Chamfer (S = 8)
 # and of the Laplacian term take 0.52 / 0.42 ms against 0.54 / 0.60 ms, while the propagation (B = 1, k = 3) takes 0.24 ms
-# against 0.12 ms; at 32 768 every grid form is at least 2x faster.
+# against 0.12 ms; at 32 768 every grid form is at least 2x faster.  flow_consistency runs the Laplacian's search and takes
+# its threshold (DESIGN.md 4.8).
 GRID_SEARCH_MIN_POINTS = {'chamfer': 8192, 'laplacian': 8192, 'flow_propagate': 32768}
 
 
@@ -894,6 +895,67 @@ def laplacian_bwd(w, p2, l2, g1, nn_idx, res, g, want_dp2=True):
     _count(lib().pvraft_laplacian_bwd(_p(w), _p(p2), _p(l2), _p(g1, torch.int32), _p(nn_idx, torch.int32), _p(res), _p(g), s, bb, n, m, kl,
                                       int(nn_idx.shape[-1]), _p(d_w), _p(d_p2), _p(d_l2), _p(ws, torch.uint8), _stream()), 'laplacian_bwd')
     return d_w, d_p2, d_l2
+
+
+CONSISTENCY_MAX_K = 8   # neighbours pvraft_flow_consistency_fwd interpolates the reverse flow from at most
+
+
+def _consistency_args(what, w, p2, f21, k, n_f12=None):
+    if p2.dim() != 3 or p2.shape[-1] != 3:
+        raise ValueError(f'{what}: expected p2 [B,M,3], got {tuple(p2.shape)}')
+    bb, m = int(p2.shape[0]), int(p2.shape[1])
+    _loss_batch(what, w, bb, m)
+    s, n = int(w.shape[0]), int(w.shape[1])
+    if f21.dim() != 3 or tuple(f21.shape) != (s, m, 3):
+        raise ValueError(f'{what}: expected f21 [{s},{m},3], got {tuple(f21.shape)}')
+    if n_f12 is not None and tuple(n_f12.shape) != tuple(w.shape):
+        raise ValueError(f'{what}: f12 {tuple(n_f12.shape)} does not match w {tuple(w.shape)}')
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(CONSISTENCY_MAX_K, m):
+        raise ValueError(f'{what}: k={k!r} must be an integer in 1..min({CONSISTENCY_MAX_K}, M={m})')
+    return s, bb, n, m
+
+
+def flow_consistency(w, f12, p2, f21, k, alpha, beta, use_grid=None):
+    """w [S,N,3] (the first clouds moved by the forward flows f12 [S,N,3]), p2 [B,M,3] (sample s searches p2[s % B]) and the
+    reverse flows f21 [S,M,3] -> (acc [S] f64: sum_i ||r_i||^2; nn_idx [S,N,k] int32, nearest first, lowest index on ties;
+    res [S,N,3]: r_i = f12_i + bhat_i, bhat_i the inverse-squared-distance interpolation of f21 over the k nearest points of
+    p2; ok [S,N] uint8: ||r_i||^2 < alpha (||f12_i||^2 + ||bhat_i||^2) + beta).  F_s = acc[s] / N.  The grid form runs when p2
+    has GRID_SEARCH_MIN_POINTS['laplacian'] points, the threshold of the same search (`use_grid`: see use_grid_search)."""
+    s, bb, n, m = _consistency_args('flow_consistency', w, p2, f21, k, f12)
+    if not (0.0 <= float(alpha) < float('inf')) or not (0.0 <= float(beta) < float('inf')):
+        raise ValueError(f'flow_consistency: alpha={alpha!r} and beta={beta!r} must be finite and not negative')
+    acc = torch.zeros(s, dtype=torch.float64, device=w.device)
+    nn_idx = torch.empty(s, n, k, dtype=torch.int32, device=w.device)
+    res = torch.empty_like(w)
+    ok = torch.empty(s, n, dtype=torch.uint8, device=w.device)
+    ws = _det_workspace(lib().pvraft_flow_consistency_fwd_det_workspace_bytes, s, device=w.device)
+    args = (_p(w), _p(f12), _p(p2), _p(f21), s, bb, n, m, k, float(alpha), float(beta), _p(nn_idx, torch.int32), _p(res),
+            _p(ok, torch.uint8), _p(acc, torch.float64))
+    if use_grid_search('laplacian', m, use_grid):
+        gw = _workspace(lib().pvraft_grid_index_workspace_bytes(bb, m), w.device)
+        _count(lib().pvraft_flow_consistency_grid_fwd(*args, _p(gw, torch.uint8), _p(ws, torch.uint8), _stream()), 'flow_consistency_grid_fwd')
+    else:
+        _count(lib().pvraft_flow_consistency_fwd(*args, _p(ws, torch.uint8), _stream()), 'flow_consistency_fwd')
+    return acc, nn_idx, res, ok
+
+
+def flow_consistency_bwd(w, p2, f21, nn_idx, res, g, want_dp2=True):
+    """Gradients of F_s = acc[s] / N (flow_consistency) with nn_idx held fixed, for the upstream gradient g [S] (on the
+    device) -> (d_w [S,N,3], d_f12 [S,N,3], d_p2 [B,M,3] (the distance part; None unless want_dp2), d_f21 [S,M,3])."""
+    k = int(nn_idx.shape[-1]) if nn_idx.dim() == 3 else -1
+    s, bb, n, m = _consistency_args('flow_consistency_bwd', w, p2, f21, k)
+    if tuple(nn_idx.shape[:2]) != (s, n) or res.shape != w.shape:
+        raise ValueError(f'flow_consistency_bwd: nn_idx {tuple(nn_idx.shape)} and res {tuple(res.shape)} do not match w {tuple(w.shape)}')
+    if g.shape != (s,):
+        raise ValueError(f'flow_consistency_bwd: expected g [{s}], got {tuple(g.shape)}')
+    d_w = torch.empty_like(w)
+    d_f12 = torch.empty_like(w)
+    d_p2 = torch.zeros_like(p2) if want_dp2 else None
+    d_f21 = torch.zeros_like(f21)
+    ws = _det_workspace(lib().pvraft_flow_consistency_bwd_det_workspace_bytes, s, bb, m, device=w.device)
+    _count(lib().pvraft_flow_consistency_bwd(_p(w), _p(p2), _p(f21), _p(nn_idx, torch.int32), _p(res), _p(g), s, bb, n, m, k, _p(d_w),
+                                             _p(d_f12), _p(d_p2), _p(d_f21), _p(ws, torch.uint8), _stream()), 'flow_consistency_bwd')
+    return d_w, d_f12, d_p2, d_f21
 
 
 PROPAGATE_MAX_K = 8   # neighbours pvraft_flow_propagate_fwd averages over at most

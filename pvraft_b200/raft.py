@@ -51,6 +51,13 @@ def _check_flow_init(p, flow_init):
     return flow_init.detach().contiguous().float()
 
 
+def _clone(out):
+    """A copy of a graph's static output: a tensor, a list of tensors, or the (forward, backward) pair of either."""
+    if torch.is_tensor(out):
+        return out.clone()
+    return type(out)(_clone(t) for t in out) if isinstance(out, tuple) else [_clone(t) for t in out]
+
+
 class _RaftBase(nn.Module):
     # CUDA-graph replay of the whole forward (encoders, correlation build, all iterations): the eager path costs ~28 us of
     # host time per launch (python + ctypes + tensor-map encodes), which bounds small batches (B <= 2: ~0.5 ms per
@@ -95,23 +102,25 @@ class _RaftBase(nn.Module):
         self.reset_graphs()
         return self
 
-    def _graph_key(self, xyz1, xyz2, num_iters, warm=False):
+    def _graph_key(self, xyz1, xyz2, num_iters, warm=False, bidirectional=False):
         # a graph records the kernels of one setting of torch.use_deterministic_algorithms: never replayed under the other.
         # A pair of clouds of different sizes adds the second cloud's shape (pairs that share N1 and differ in N2 run on
         # different buffers); a pair of equal sizes keeps the short key.  A warm-started forward (flow_init) records only
-        # that it is one: the starting flow is a static input like the clouds, so new values replay the same graph.
+        # that it is one: the starting flow is a static input like the clouds, so new values replay the same graph.  A
+        # bidirectional forward records its flag.
         key = (tuple(xyz1.shape), xyz1.device, int(num_iters), ops.deterministic())
         key = key if xyz2.shape == xyz1.shape else key + (tuple(xyz2.shape),)
-        return key + ('flow_init',) if warm else key
+        key = key + ('flow_init',) if warm else key
+        return key + ('bidirectional',) if bidirectional else key
 
     def _stamp(self):
         return tuple((q._version, q.data_ptr()) for q in self.parameters())
 
-    def _graphed(self, p, num_iters, flow_init=None):
+    def _graphed(self, p, num_iters, flow_init=None, bidirectional=False):
         xyz1, xyz2 = p[0].detach().contiguous().float(), p[1].detach().contiguous().float()
         inputs = [xyz1, xyz2] if flow_init is None else [xyz1, xyz2, flow_init]
         graphs = self.__dict__.setdefault('_graphs', {})
-        key = self._graph_key(xyz1, xyz2, num_iters, flow_init is not None)
+        key = self._graph_key(xyz1, xyz2, num_iters, flow_init is not None, bidirectional)
         entry = graphs.get(key)
         stamp = self._stamp()
         if entry is not None and entry[3] != stamp:
@@ -122,7 +131,7 @@ class _RaftBase(nn.Module):
                 s.copy_(t)
 
             def run():
-                return self._forward_impl(static_in[:2], num_iters, static_in[2] if len(static_in) > 2 else None)
+                return self._forward_impl(static_in[:2], num_iters, static_in[2] if len(static_in) > 2 else None, bidirectional)
 
             side = torch.cuda.Stream(device=xyz1.device)   # warm-up off the capture stream: weight splits, derived constants
             side.wait_stream(torch.cuda.current_stream(xyz1.device))
@@ -143,12 +152,24 @@ class _RaftBase(nn.Module):
             s.copy_(t)
         graph.replay()
         ops.launch_count += n_kernels            # the library's kernels inside the replayed graph
-        return static_out.clone() if torch.is_tensor(static_out) else [t.clone() for t in static_out]
+        return _clone(static_out)
 
-    def forward(self, p, num_iters=12, flow_init=None):
+    def forward(self, p, num_iters=12, flow_init=None, bidirectional=False):
         """p = [xyz1 [B,N1,3], xyz2 [B,N2,3]] -> the reference's outputs.  flow_init [B,N1,3] (optional): RAFT's warm start,
         the loop starts at coords2 = xyz1 + flow_init instead of xyz1.  It is a constant: detached, it receives no gradient.
-        None runs the reference's loop; a zero flow_init gives the same bits."""
+        None runs the reference's loop; a zero flow_init gives the same bits.
+        bidirectional=True: the flow in both directions, (forward, backward) = (model(p), model([xyz2, xyz1])) in one call
+        (_encode_both): for RSF two lists of num_iters flows [B,N1,3] and [B,N2,3], for RSF_refine the two refined flows.
+        Under torch.use_deterministic_algorithms(True) each equals its one-direction call bitwise when N1 = N2 is a multiple
+        of 128 or N1 != N2.  It cannot be warm-started: flow_init must be None."""
+        if bidirectional:
+            if flow_init is not None:
+                raise ValueError('a bidirectional forward cannot be warm-started: flow_init must be None')
+            ops.check_pair(p[0], p[1], self.corr_block.truncate_k)   # both directions, before any launch
+            ops.check_pair(p[1], p[0], self.corr_block.truncate_k)
+            if self.corr_block.state_dtype != torch.float32 and max(p[0].shape[1], p[1].shape[1]) > 65536:
+                raise ValueError(f'uint16 candidate ids need both clouds of a bidirectional forward to have at most 65536 points, '
+                                 f'got N1={p[0].shape[1]} and N2={p[1].shape[1]}')
         flow_init = _check_flow_init(p, flow_init)
         if not p[0].is_cuda:
             raise ops._lib.PvraftError('pvraft_b200 kernels need CUDA tensors (no CPU fallback exists)')
@@ -156,7 +177,7 @@ class _RaftBase(nn.Module):
             if flow_init is not None and flow_init.device != p[0].device:
                 raise ops._lib.PvraftError(f'flow_init is on {flow_init.device}, the clouds on {p[0].device}')
             if _records_grad(self, p):
-                return self._forward_train(p, num_iters, flow_init)
+                return self._forward_train(p, num_iters, flow_init, bidirectional)
             graph = self.use_cuda_graph
             if graph is None:    # automatic (never inside an nn.DataParallel replica thread)
                 if getattr(self, '_is_replica', False):
@@ -165,14 +186,44 @@ class _RaftBase(nn.Module):
                     graph = True     # host-bound from the first call
                 else:                # larger batches: once the same shape has come back with the same weights
                     seen = self.__dict__.setdefault('_seen', {})
-                    key, stamp = self._graph_key(p[0], p[1], num_iters, flow_init is not None), self._stamp()
+                    key, stamp = self._graph_key(p[0], p[1], num_iters, flow_init is not None, bidirectional), self._stamp()
                     graph = seen.get(key) == stamp
                     if len(seen) > 64:
                         seen.clear()
                     seen[key] = stamp
             if graph:
-                return self._graphed(p, num_iters, flow_init)
-            return self._forward_impl(p, num_iters, flow_init)
+                return self._graphed(p, num_iters, flow_init, bidirectional)
+            return self._forward_impl(p, num_iters, flow_init, bidirectional)
+
+    def _forward_impl(self, p, num_iters=12, flow_init=None, bidirectional=False):
+        if not bidirectional:
+            return self._run(self._encode(p), num_iters, flow_init)
+        outs = [self._run(e, num_iters) for e in self._encode_both(p)]
+        if len(outs) == 2:
+            return tuple(outs)
+        out, b = outs[0], int(p[0].shape[0])
+        if torch.is_tensor(out):
+            return out[:b], out[b:]
+        return [f[:b] for f in out], [f[b:] for f in out]
+
+    def _encode_both(self, p):
+        """Yields _pair's outputs for both directions (forward has checked both); the caller runs each before taking the
+        next, because _pair leaves the correlation state on corr_block.  Clouds of equal sizes: one 2B stack (xyz1 =
+        cat[x1, x2] against cat[x2, x1]) on the encoder's 2B pass, whose graph is kept whole -- each cloud's own graph, for
+        the context encoder, the loop's SetConv and the refiner -- so one correlation build, one context pass and one loop
+        serve both directions.  Different sizes: each cloud encoded once, then one _pair per direction."""
+        xyz1 = p[0].detach().contiguous().float()
+        xyz2 = p[1].detach().contiguous().float()
+        if xyz1.shape == xyz2.shape:
+            b = xyz1.shape[0]
+            both = torch.cat([xyz1, xyz2], 0)
+            fmap, graph = self.feature_extractor(both, point_major=True)
+            yield self._pair(both, torch.cat([xyz2, xyz1], 0), fmap, graph, torch.cat([fmap[b:], fmap[:b]], 0))
+            return
+        fmap1, graph1 = self._encode_cloud(xyz1)
+        fmap2, graph2 = self._encode_cloud(xyz2)
+        yield self._pair(xyz1, xyz2, fmap1, graph1, fmap2)
+        yield self._pair(xyz2, xyz1, fmap2, graph2, fmap1)
 
     def _encode(self, p):
         xyz1, xyz2 = p[0], p[1]
@@ -272,17 +323,14 @@ class RSF(_RaftBase):
                                     resolution=3, truncate_k=args.truncate_k)
         self.update_block = UpdateBlock(hidden_dim=self.hidden_dim)
 
-    def _forward_impl(self, p, num_iters=12, flow_init=None):
-        return self._run(self._encode(p), num_iters, flow_init)
-
     def _run(self, encoded, num_iters, flow_init=None):
         """The loop on _pair's outputs -> the list of num_iters flows."""
         xyz1, _, _, graph_context, net, inp = encoded
         _, preds = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=True, flow_init=flow_init)
         return preds
 
-    def _forward_train(self, p, num_iters=12, flow_init=None):
-        return train.rsf_forward(self, p, num_iters, flow_init)
+    def _forward_train(self, p, num_iters=12, flow_init=None, bidirectional=False):
+        return train.rsf_forward(self, p, num_iters, flow_init, bidirectional)
 
 
 class RSF_refine(_RaftBase):
@@ -297,25 +345,43 @@ class RSF_refine(_RaftBase):
         self.update_block = UpdateBlock(hidden_dim=self.hidden_dim)
         self.refine_block = FlotRefine()
 
-    def _forward_impl(self, p, num_iters=12, flow_init=None):
-        return self._run(self._encode(p), num_iters, flow_init)
-
     def _run(self, encoded, num_iters, flow_init=None):
         """The loop and the refiner on _pair's outputs -> the refined flow."""
         xyz1, _, graph, graph_context, net, inp = encoded
         flow, _ = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=False, flow_init=flow_init)
         return self.refine_block(flow, graph)      # RAFTSceneFlowRefine.py:46
 
-    def _forward_train(self, p, num_iters=12, flow_init=None):
+    def _forward_train(self, p, num_iters=12, flow_init=None, bidirectional=False):
         """model/RAFTSceneFlowRefine.py:22-48: everything up to the last flow under no_grad (the fused inference kernels),
         the refiner -- the only part tools/engine_refine.py trains -- layer by layer with gradients.  The refiner's input
-        flow is coords2 - xyz1 with coords2 computed under no_grad, so xyz1 receives minus the flow's gradient and xyz2 none."""
-        x1 = p[0].float()
-        if x1.requires_grad and self.corr_block.state_dtype != torch.float32:
+        flow is coords2 - xyz1 with coords2 computed under no_grad, so xyz1 receives minus the flow's gradient and xyz2 none.
+        Bidirectional: the same per direction (the refiner on the 2B stack when the sizes are equal); each cloud receives
+        minus the gradient of the refiner input flow that starts on it."""
+        starts = (p[0], p[1]) if bidirectional else (p[0],)       # the clouds the refiner's input flows start on
+        if any(x.requires_grad for x in starts) and self.corr_block.state_dtype != torch.float32:
             raise NotImplementedError("training differentiates through the fp32 state: call model.set_precision('fp32')")
         with torch.no_grad():
-            xyz1, _, graph, graph_context, net, inp = self._encode(p)
-            flow, _ = self._iterate(xyz1, graph_context, net, inp, num_iters, keep_all=False, flow_init=flow_init)
-        if x1.requires_grad:
-            flow = flow + (x1.detach() - x1)          # the same values; d xyz1 = -d flow
-        return train.flot_refine(self.refine_block, flow, graph)
+            encoded = self._encode_both(p) if bidirectional else [self._encode(p)]   # (each direction's loop runs before the next _pair)
+            loops = [(e[0], e[2], self._iterate(e[0], e[3], e[4], e[5], num_iters, keep_all=False, flow_init=flow_init)[0])
+                     for e in encoded]
+        if not bidirectional:
+            x1 = p[0].float()
+            flow, graph = loops[0][2], loops[0][1]
+            if x1.requires_grad:
+                flow = flow + (x1.detach() - x1)      # the same values; d xyz1 = -d flow
+            return train.flot_refine(self.refine_block, flow, graph)
+        x1, x2 = p[0].float(), p[1].float()
+        if len(loops) == 1:                           # the 2B stack: cat[x1, x2] starts the flows
+            b = int(p[0].shape[0])
+            start = torch.cat([x1, x2], 0)
+            flow = loops[0][2]
+            if start.requires_grad:
+                flow = flow + (start.detach() - start)
+            out = train.flot_refine(self.refine_block, flow, loops[0][1])
+            return out[:b], out[b:]
+        outs = []
+        for (_, graph, flow), x in zip(loops, (x1, x2)):
+            if x.requires_grad:
+                flow = flow + (x.detach() - x)
+            outs.append(train.flot_refine(self.refine_block, flow, graph))
+        return tuple(outs)

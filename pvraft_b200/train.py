@@ -331,11 +331,16 @@ def flot_refine(m, flow, graph):
     return flow + linear(x, m.fc.weight, m.fc.bias)
 
 
-def rsf_forward(model, p, num_iters, flow_init=None):
+def rsf_forward(model, p, num_iters, flow_init=None, bidirectional=False):
     """RSF.forward with gradients (model/RAFTSceneFlow.py:22-50) -> list of num_iters flows [B,N1,3].  flow_init [B,N1,3]
-    (detached, fp32): the loop starts at xyz1 + flow_init (RAFT's warm start; no gradient reaches it)."""
+    (detached, fp32): the loop starts at xyz1 + flow_init (RAFT's warm start; no gradient reaches it).
+    bidirectional: (forward, backward), the lists of model(p) and model([xyz2, xyz1]).  Clouds of equal sizes run as one 2B
+    stack on the encoder's 2B pass, its graph kept whole: CorrInitFn on (cat[f1, f2], cat[f2, f1]), whose backward reaches
+    both feature maps through the stacking, and one context pass and loop.  Different sizes: one pass per direction."""
     cb = model.corr_block
     ops.check_pair(p[0], p[1], cb.truncate_k)
+    if bidirectional:
+        ops.check_pair(p[1], p[0], cb.truncate_k)
     xyz1 = p[0].contiguous().float()                                           # attached: gradients reach the inputs
     xyz2 = p[1].contiguous().float()
     b, n, _ = xyz1.shape
@@ -345,12 +350,25 @@ def rsf_forward(model, p, num_iters, flow_init=None):
         both = torch.cat([xyz1, xyz2], 0)
         g_both = Graph.construct_graph(both, 32)                               # :25-26 (one batch of 2B clouds)
         fmap = flot_encoder(model.feature_extractor, both, g_both)
+        if bidirectional:
+            preds = _rsf_loop(model, both, torch.cat([xyz2, xyz1], 0), fmap, g_both, torch.cat([fmap[b:], fmap[:b]], 0), num_iters)
+            return [f[:b] for f in preds], [f[b:] for f in preds]
         graph1 = Graph(g_both.nbr[:b].contiguous(), g_both._rel[:b].contiguous(), 32, [b * n] * 2)   # (the training path does not use .order)
         fmap1, fmap2 = fmap[:b], fmap[b:]
     else:                                                                      # clouds of different sizes: one pass per cloud
         graph1 = Graph.construct_graph(xyz1, 32)
         fmap1 = flot_encoder(model.feature_extractor, xyz1, graph1)
-        fmap2 = flot_encoder(model.feature_extractor, xyz2, Graph.construct_graph(xyz2, 32))
+        graph2 = Graph.construct_graph(xyz2, 32)
+        fmap2 = flot_encoder(model.feature_extractor, xyz2, graph2)
+        if bidirectional:
+            return (_rsf_loop(model, xyz1, xyz2, fmap1, graph1, fmap2, num_iters),
+                    _rsf_loop(model, xyz2, xyz1, fmap2, graph2, fmap1, num_iters))
+    return _rsf_loop(model, xyz1, xyz2, fmap1, graph1, fmap2, num_iters, flow_init)
+
+
+def _rsf_loop(model, xyz1, xyz2, fmap1, graph1, fmap2, num_iters, flow_init=None):
+    """The part of rsf_forward after the feature encoder: correlation, context and the loop -> the list of flows."""
+    cb = model.corr_block
     corr_val, corr_idx = CorrInitFn.apply(fmap1, fmap2, cb.truncate_k, cb)     # :29
     xyz2p = ops.xyz_pad(xyz2)
     fct1 = flot_encoder(model.context_extractor, xyz1, graph1)                 # :31 (same cloud, same graph)
