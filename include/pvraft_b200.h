@@ -431,12 +431,23 @@ PVRAFT_API int pvraft_gru_fwd(const pvraft_gru_args* a, void* stream);
  *   order [B,N] int32 or NULL: the LOCAL point processed r-th in every sample (pvraft_point_order_fwd: a Morton rank table).
  *   It changes no result, only which points a CTA works on at the same time, so that their overlapping neighbourhoods are
  *   gathered from L1 instead of L2.
+ *   plan: the gather plan of (nbr, order), pvraft_edge_plan_fwd (16-byte aligned).  The kernel copies each tile's distinct rows
+ *   into shared memory from it, or gathers the tile from global memory when it has more distinct rows than the table holds at
+ *   this C; either way the results are the same bits.
  *   det_workspace: pvraft_setconv_edge_det_workspace_bytes(B) bytes or NULL ("Deterministic mode").
  * --------------------------------------------------------------------------------------------- */
 PVRAFT_API int pvraft_setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
                                        int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order,
-                                       void* det_workspace, void* stream);
+                                       const void* plan, void* det_workspace, void* stream);
 PVRAFT_API int64_t pvraft_setconv_edge_det_workspace_bytes(int B);
+
+/* Gather plan of a kNN graph for pvraft_setconv_edge_fwd, independent of the features and of C: per tile of 32 consecutive
+ * positions of the processing order (never straddling two samples), the distinct rows its 32 x 32 neighbour references and
+ * 32 centres name, in slot order, and the slot of every reference.  nbr [B,N,32] int32, order [B,N] int32 or NULL (as for
+ * pvraft_setconv_edge_fwd) -> plan, pvraft_edge_plan_bytes(B, N) bytes, sample-major: the plan of the first b samples of a
+ * batch is its first pvraft_edge_plan_bytes(b, N) bytes.  Record layout in csrc/edge_plan.cuh. */
+PVRAFT_API int pvraft_edge_plan_fwd(const int32_t* nbr, const int32_t* order, int B, int N, void* plan, void* stream);
+PVRAFT_API int64_t pvraft_edge_plan_bytes(int B, int N);
 
 /* ------------------------------------------------------------------------------------------------
  * FlowHead output stage + RAFT coordinate update.  Replaces model/update.py:69,71-72 (conv1, cat,

@@ -104,8 +104,10 @@ _SIGNATURES = {
     'pvraft_knn_branch_fwd': (C.c_int, [C.POINTER(KnnBranchArgs), VP]),
     'pvraft_point_order_fwd': (C.c_int, [VP, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_gru_fwd': (C.c_int, [C.POINTER(GruArgs), VP]),
-    'pvraft_setconv_edge_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP]),
+    'pvraft_setconv_edge_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP, VP]),
     'pvraft_setconv_edge_det_workspace_bytes': (C.c_int64, [C.c_int]),
+    'pvraft_edge_plan_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, VP, VP]),
+    'pvraft_edge_plan_bytes': (C.c_int64, [C.c_int, C.c_int]),
     'pvraft_flow_out_fwd': (C.c_int, [C.POINTER(FlowOutArgs), VP]),
     'pvraft_knn_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
     'pvraft_knn_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),

@@ -9,52 +9,44 @@
 // and min of the raw y, plus the double-precision (sum, sum^2) of all N*32*C raw values per group.
 //
 // Persistent and warp-specialised, one CTA per SM.  A CTA walks tiles of kEdgeTile consecutive positions of the processing
-// order (one sample per tile).  The builder warps prepare tile t + 1 while the consumer warps compute tile t: they
-// deduplicate the tile's neighbour and centre ids in a shared-memory hash (a Morton tile of 32 points makes ~1000 references
-// to ~200 distinct rows) and bulk-copy every distinct row P_j into the idle half of a double-buffered table.  The consumer
-// warps run one warp per point exactly as a plain gather would: lane l owns the adjacent channel pairs (2l, 2l+1) + 64q, a
-// neighbour row is one 8-byte shared-memory load per lane and pair, and the per-edge scalars (row offset, edge vector) are
-// read back as ONE broadcast 16-byte shared-memory load.  A tile with more distinct rows than the table holds is gathered
-// from global memory instead (an unordered cloud), with the same arithmetic: the results never depend on the order.
+// order (edge_plan.cuh), driven by the graph's gather plan (edge_plan.cu): the producer warps bulk-copy tile t + 1's row ids
+// and reference slots, then its distinct rows P_j, into the idle half of a double-buffered table while the consumer warps
+// compute tile t.  The consumers run one warp per point exactly as a plain gather would: lane l owns the adjacent channel
+// pairs (2l, 2l+1) + 64q, a neighbour row is one 8-byte shared-memory load per lane and pair, and the per-edge scalars (row
+// offset, edge vector) are read back as ONE broadcast 16-byte shared-memory load.  A tile with more distinct rows than the
+// table holds is gathered from global memory instead (an unordered cloud), with the same arithmetic: the results never
+// depend on the order nor on the plan.
+#include "edge_plan.cuh"
 #include "fixed_point.cuh"
 #include "tma.cuh"
 
 namespace pvraft {
 
-constexpr int kEdgeTile = 32;                                  // points per tile
-constexpr int kEdgeConsumerWarps = 16;                         // at most: one point per warp at a time
-// Warps per role, from the channel pairs per lane and the form.  The builders' chain per tile (hash rounds, then the copies)
-// is what the consumers wait for: 8 builder warps halve it against 4 (M = 4 references per lane instead of 8) where the
-// register budget of one CTA per SM allows it without spills.  Registers: 80 (1 pair, 16 + 8 warps), 96 (1 pair DET,
-// 16 + 4), 128 (2 pairs, 12 + 4), 168 (2 pairs DET, 8 + 4).
-__host__ __device__ constexpr int edge_consumer_warps(int pairs, bool det) { return pairs == 1 ? kEdgeConsumerWarps : det ? 8 : 12; }
-__host__ __device__ constexpr int edge_builder_warps(int pairs, bool det) { return pairs == 1 && !det ? 8 : 4; }
-__host__ __device__ constexpr int edge_threads(int pairs, bool det) { return (edge_consumer_warps(pairs, det) + edge_builder_warps(pairs, det)) * 32; }
-constexpr int kEdgeRefs = kEdgeTile * 33;                      // row references of a tile: 32 neighbours + the centre per point
-constexpr int kEdgeHashBits = 11, kEdgeHash = 1 << kEdgeHashBits;   // > kEdgeRefs: linear probing always reaches an empty key
+// Warps per role and form, within the register budget of one CTA per SM and without spills (registers: DESIGN 4.2).  Four
+// producer warps issue a tile's row copies, where the budget has room for them beside the consumers; points are dealt to
+// the consumers round-robin across tiles, so a count that does not divide kEdgeTile still balances.
+constexpr int kEdgeConsumerWarps = 24;                         // at most
+__host__ __device__ constexpr int edge_consumer_warps(int pairs, bool det) { return pairs == 1 ? (det ? 16 : 24) : (det ? 8 : 12); }
+constexpr int kEdgeProducerWarps = 4;
+__host__ __device__ constexpr int edge_threads(int pairs, bool det) { return (edge_consumer_warps(pairs, det) + kEdgeProducerWarps) * 32; }
 constexpr int kEdgeTableFloats = 22528;                        // one table buffer: rows = min(kEdgeRefs, this / C)
-// named barriers (0 is __syncthreads): the consumers among themselves, "buffer free" (consumers arrive, builders wait), the builders
-constexpr int kBarConsumers = 1, kBarEmpty = 2, kBarBuilders = 4;
+// named barriers (0 is __syncthreads): the consumers among themselves, "buffer free" (consumers arrive, the producers wait)
+constexpr int kBarConsumers = 1, kBarEmpty = 2;
 
 
 inline int edge_table_rows(int C) { return kEdgeTableFloats / C < kEdgeRefs ? kEdgeTableFloats / C : kEdgeRefs; }
 
 // shared memory after the two table buffers [2][rows][C]
 struct EdgeSmem {
-    int key[2][kEdgeHash];                 // row id, -1 = empty
-    short slot[2][kEdgeHash];              // table slot of key[h] (>= rows: the tile overflowed)
-    short ref[2][kEdgeTile * 32];          // key index of neighbour e of point p, at p * 32 + e
-    short ctr[2][kEdgeTile];               // key index of the centre of point p
-    int row[2][kEdgeRefs];                 // row id of table slot r
-    int count[2];                          // distinct rows of the tile
-    unsigned long long full[2];            // mbarrier: the tile's hash, references and rows are in place
+    alignas(16) int row[2][kEdgeRefs];     // row id of table slot r (the plan's ids)
+    alignas(16) uint16_t slot[2][kEdgeRefs];   // table slot of each reference (the plan's slots)
+    unsigned long long meta[2];            // mbarrier: the tile's ids and slots are in place
+    unsigned long long full[2];            // mbarrier: the tile's rows are in place
     float4 edge[kEdgeConsumerWarps][32];   // (row offset bits, ex, ey, ez) of a consumer warp's point
     double part[kEdgeConsumerWarps][16];   // per-warp GroupNorm partials (group, moment)
     unsigned long long fx[16 * kFxWords];  // DET: the CTA's fixed-point (group, moment) sums
 };
 
-__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-__device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
@@ -62,6 +54,8 @@ __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
 __device__ __forceinline__ void cp_async_arrive(void* bar) {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // elementwise arithmetic on channel pairs held as one 64-bit value: each component is one IEEE round-to-nearest operation
 // (the _rn intrinsics are never contracted into an FMA)
@@ -133,54 +127,6 @@ __device__ __forceinline__ void edge_point(const float* rows, const float4* se, 
     }
 }
 
-// warp-collective: puts the rows id[0..K) of every lane (-1: nothing) into the tile's hash and returns their key indices in h.
-// The K compare-and-swaps of a lane are in flight together; each round's new keys take the next table slots (one warp scan,
-// one shared atomic).
-template <int K>
-__device__ __forceinline__ void edge_insert(const int (&id)[K], int (&h)[K], EdgeSmem& s, int buf, int rows) {
-    const int lane = lane_id();
-    unsigned pending = 0;
-#pragma unroll
-    for (int m = 0; m < K; ++m) {
-        h[m] = (int)(((unsigned)id[m] * 0x9E3779B1u) >> (32 - kEdgeHashBits));
-        if (id[m] >= 0) pending |= 1u << m;
-    }
-    while (__any_sync(kFull, pending)) {
-        int old[K];
-#pragma unroll
-        for (int m = 0; m < K; ++m)
-            if (pending >> m & 1u) old[m] = atomicCAS(&s.key[buf][h[m]], -1, id[m]);
-        unsigned fresh = 0;
-#pragma unroll
-        for (int m = 0; m < K; ++m)
-            if (pending >> m & 1u) {
-                if (old[m] == -1) fresh |= 1u << m;
-                if (old[m] == -1 || old[m] == id[m]) pending &= ~(1u << m);
-                else h[m] = (h[m] + 1) & (kEdgeHash - 1);
-            }
-        const int nf = __popc(fresh);
-        int incl = nf;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int v = __shfl_up_sync(kFull, incl, o);
-            if (lane >= o) incl += v;
-        }
-        const int total = __shfl_sync(kFull, incl, 31);
-        if (total) {
-            int first = 0;
-            if (lane == 31) first = atomicAdd(&s.count[buf], total);
-            int sl = __shfl_sync(kFull, first, 31) + incl - nf;
-#pragma unroll
-            for (int m = 0; m < K; ++m)
-                if (fresh >> m & 1u) {
-                    s.slot[buf][h[m]] = (short)sl;
-                    if (sl < rows) s.row[buf][sl] = id[m];
-                    ++sl;
-                }
-        }
-    }
-}
-
 // DET: every point's per-channel (sum, sum^2) over its 32 edges enters a per-lane fixed-point register sum, and those enter the
 // [B,16] fixed-point workspace `stats` points at then (fixed_point.cuh): the sums do not depend on which CTA took which points
 template <int PAIRS, bool DET>
@@ -188,69 +134,59 @@ __global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pa
                                                                      const float* __restrict__ edge_feats, const float* __restrict__ w_fc1,
                                                                      int cin, int B, int N, int C, float* __restrict__ ymax,
                                                                      float* __restrict__ ymin, Acc<DET, double> stats,
-                                                                     const int32_t* __restrict__ order, int rows) {
+                                                                     const int32_t* __restrict__ order, const unsigned char* __restrict__ plan,
+                                                                     int rows) {
     constexpr int CW = edge_consumer_warps(PAIRS, DET), kConsumers = CW * 32, kThreads = edge_threads(PAIRS, DET);
-    constexpr int BW = edge_builder_warps(PAIRS, DET), kBuilders = BW * 32;
-    static_assert(kEdgeTile % BW == 0 && kEdgeTile <= kBuilders && CW <= kEdgeConsumerWarps, "work split");
+    constexpr int PW = kEdgeProducerWarps;
+    static_assert(CW <= kEdgeConsumerWarps, "work split");
     extern __shared__ __align__(128) unsigned char smem[];
     float* tables = reinterpret_cast<float*>(smem);   // [2][rows][C]
     EdgeSmem& s = *reinterpret_cast<EdgeSmem*>(smem + (size_t)2 * rows * C * sizeof(float));
     pdl_trigger();   // the next kernel may be staged while this one drains
     if (threadIdx.x == 0) {
-        mbar_init(&s.full[0], 2 * kBuilders);   // per builder thread: its hash / reference stores, then its row copies
-        mbar_init(&s.full[1], 2 * kBuilders);
+        for (int i = 0; i < 2; ++i) {
+            mbar_init(&s.meta[i], 1);    // the producer's expect_tx, then the bulk copies' bytes
+            mbar_init(&s.full[i], PW * 32);   // per producer thread: the landing of its row copies
+        }
         fence_mbarrier_init();
     }
     __syncthreads();
     pdl_wait();      // (launched with PDL: nothing above touches global memory; P is the previous launch's output)
     const int lane = lane_id(), w = warp_id();
-    const int tps = (N + kEdgeTile - 1) / kEdgeTile;   // tiles per sample
+    const int tps = edge_tiles_per_sample(N);
     long long t_begin, t_end;
     split_range((long long)B * tps, gridDim.x, blockIdx.x, t_begin, t_end);
     const int ntiles = (int)(t_end - t_begin);
 
-    if (w >= CW) {   // ---- builders: tile k into buffer k & 1 ----
-        const int bt = threadIdx.x - kConsumers, bw = bt >> 5;
+    if (w >= CW) {   // ---- producers: tile k into buffer k & 1 ----
+        const int pw = w - CW;
         const int chunks = C / 4, rows_per_copy = 32 / chunks, copy_row = lane / chunks, copy_chunk = lane - copy_row * chunks;
-        constexpr int M = kEdgeTile / BW;
+        const int* count = reinterpret_cast<const int*>(plan + kEdgePlanCount);   // (of tile t at t * kEdgePlanBytes / 4)
+        int n = ntiles > 0 ? __ldg(count + t_begin * (kEdgePlanBytes / 4)) : 0;
         for (int k = 0; k < ntiles; ++k) {
             const int buf = k & 1;
             const long long t = t_begin + k;
-            const int b = (int)(t / tps), start = (int)(t - (long long)b * tps) * kEdgeTile, len = min(kEdgeTile, N - start);
-            // this thread's references, read before the buffer is free: neighbour `lane` of the points bw, bw + 4, ..., and
-            // (warp 0) the centre of point `lane`
-            const long long s0 = (long long)b * N;
-            int id[M + 1], h[M + 1];
-#pragma unroll
-            for (int m = 0; m < M; ++m) {
-                const int p = bw + BW * m;
-                id[m] = p < len ? (order ? __ldg(order + s0 + start + p) : start + p) : -1;
-            }
-            id[M] = bw == 0 && lane < len ? (order ? __ldg(order + s0 + start + lane) : start + lane) : -1;
-#pragma unroll
-            for (int m = 0; m < M; ++m)
-                if (id[m] >= 0) id[m] = __ldg(nbr + (s0 + id[m]) * 32 + lane);
+            const int b = (int)(t / tps);
+            const unsigned char* rec = plan + t * kEdgePlanBytes;
+            const bool in_table = n <= rows;   // an overflowing tile copies no rows (its consumers gather from global memory)
             if (k >= 2) bar_sync(kBarEmpty + buf, kThreads);   // the consumers are done with tile k - 2
-            for (int j = bt; j < kEdgeHash; j += kBuilders) s.key[buf][j] = -1;
-            if (bt == 0) s.count[buf] = 0;
-            bar_sync(kBarBuilders, kBuilders);
-            edge_insert<M + 1>(id, h, s, buf, rows);
-#pragma unroll
-            for (int m = 0; m < M; ++m)
-                if (id[m] >= 0) s.ref[buf][(bw + BW * m) * 32 + lane] = (short)h[m];
-            if (id[M] >= 0) s.ctr[buf][lane] = (short)h[M];
-            mbar_arrive(&s.full[buf]);
-            bar_sync(kBarBuilders, kBuilders);   // every row id is in place
-            // the distinct rows -> the table: a warp copies rows_per_copy rows of C / 4 16-byte chunks per instruction; an
-            // overflowing tile copies nothing (its consumers gather from global memory)
-            const int n = s.count[buf];
-            if (n <= rows) {
-                const float* P = fc1p + (size_t)b * N * C;
-                float* table = tables + (size_t)buf * rows * C;
-                for (int r = bw * rows_per_copy + copy_row; copy_row < rows_per_copy && r < n; r += BW * rows_per_copy)
-                    cp_async16(table + (size_t)r * C + 4 * copy_chunk, P + (size_t)s.row[buf][r] * C + 4 * copy_chunk);
+            if (pw == 0 && lane == 0) {
+                const unsigned id_bytes = in_table ? (unsigned)(n * 4 + 15) & ~15u : 0u;
+                mbar_expect_tx(&s.meta[buf], id_bytes + kEdgeRefs * 2);
+                if (id_bytes) bulk_g2s(s.row[buf], rec, id_bytes, &s.meta[buf]);
+                bulk_g2s(s.slot[buf], rec + kEdgePlanSlots, kEdgeRefs * 2, &s.meta[buf]);
+            }
+            if (in_table && copy_row < rows_per_copy) {
+                // the distinct rows -> the table: a warp copies rows_per_copy rows of C / 4 16-byte chunks per instruction
+                mbar_wait(&s.meta[buf], (unsigned)(k >> 1) & 1u);
+                const float* P = fc1p + (size_t)b * N * C + 4 * copy_chunk;
+                float* table = tables + (size_t)buf * rows * C + 4 * copy_chunk;
+#pragma unroll 1
+                for (int r = pw * rows_per_copy + copy_row; r < n; r += PW * rows_per_copy)
+                    cp_async16(table + (size_t)r * C, P + (size_t)s.row[buf][r] * C);
             }
             cp_async_arrive(&s.full[buf]);   // (when this thread's copies have landed)
+            if (k + 1 < ntiles) n = __ldg(count + (t + 1) * (kEdgePlanBytes / 4));
         }
         return;
     }
@@ -327,6 +263,7 @@ __global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pa
     };
     reset();
     int cur = -1;   // the sample whose partials the registers hold
+    int deal = 0;   // the consumer warp that takes the next point: points are dealt round-robin across tiles
     for (int k = 0; k < ntiles; ++k) {
         const int buf = k & 1;
         const long long t = t_begin + k;
@@ -335,40 +272,43 @@ __global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pa
             if (cur >= 0) flush(cur);
             cur = b;
         }
+        const int p0 = w >= deal ? w - deal : w - deal + CW;   // this warp's first point of the tile
+        deal = (deal + len) % CW;
         // the global reads that do not need the table, issued before waiting for it: the ids and edge vectors of the warp's points
         constexpr int U = (kEdgeTile + CW - 1) / CW;
         int pid[U];
         float3 pe[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            const int p = w + u * CW;
+            const int p = p0 + u * CW;
             pid[u] = p < len ? (order ? __ldg(order + (long long)b * N + start + p) : start + p) : 0;
         }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             // lane e parks neighbour e: its row offset and edge feature x_j - x_i (graph.edge_feats, gconv.py:66)
             const float* ef = edge_feats + (((size_t)b * N + pid[u]) * 32 + lane) * 3;
-            pe[u] = w + u * CW < len ? make_float3(__ldg(ef), __ldg(ef + 1), __ldg(ef + 2)) : make_float3(0.f, 0.f, 0.f);
+            pe[u] = p0 + u * CW < len ? make_float3(__ldg(ef), __ldg(ef + 1), __ldg(ef + 2)) : make_float3(0.f, 0.f, 0.f);
         }
+        const bool in_table = __ldg(reinterpret_cast<const int*>(plan + t * kEdgePlanBytes + kEdgePlanCount)) <= rows;
+        mbar_wait(&s.meta[buf], (unsigned)(k >> 1) & 1u);
         mbar_wait(&s.full[buf], (unsigned)(k >> 1) & 1u);
-        const bool in_table = s.count[buf] <= rows;
         const float* P = fc1p + (size_t)b * N * C;
         const float* table = tables + (size_t)buf * rows * C;
 #pragma unroll 1
-        for (int p = w; p < len; p += CW) {
+        for (int p = p0; p < len; p += CW) {
             const int i = pid[0];
             const float3 e = pe[0];
 #pragma unroll
             for (int u = 0; u + 1 < U; ++u) { pid[u] = pid[u + 1]; pe[u] = pe[u + 1]; }
             const long long pt = (long long)b * N + i;
-            const int off = in_table ? s.slot[buf][s.ref[buf][p * 32 + lane]] * C : __ldg(nbr + pt * 32 + lane) * C;
+            const int off = (in_table ? (int)s.slot[buf][p * 32 + lane] : __ldg(nbr + pt * 32 + lane)) * C;
             __syncwarp();
             s.edge[w][lane] = make_float4(__int_as_float(off), e.x, e.y, e.z);
             __syncwarp();
             float2 mx[PAIRS], mn[PAIRS];
             unsigned long long s1[PAIRS], s2[PAIRS];
             if (in_table)
-                edge_point<PAIRS, true>(table, s.edge[w], table + s.slot[buf][s.ctr[buf][p]] * C, coff, wx2, wy2, wz2, mx, mn, s1, s2);
+                edge_point<PAIRS, true>(table, s.edge[w], table + s.slot[buf][kEdgeTile * 32 + p] * C, coff, wx2, wy2, wz2, mx, mn, s1, s2);
             else
                 edge_point<PAIRS, false>(P, s.edge[w], P + (size_t)i * C, coff, wx2, wy2, wz2, mx, mn, s1, s2);
 #pragma unroll
@@ -388,7 +328,7 @@ __global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pa
                 }
             }
         }
-        if (k + 2 < ntiles) bar_arrive(kBarEmpty + buf, kThreads);   // the builders may refill this buffer with tile k + 2
+        if (k + 2 < ntiles) bar_arrive(kBarEmpty + buf, kThreads);   // the producers may refill this buffer with tile k + 2
     }
     if (cur >= 0) flush(cur);
 }
@@ -399,14 +339,15 @@ using namespace pvraft;
 
 template <bool DET>
 static int setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin, int B, int N, int C,
-                            float* ymax, float* ymin, double* stats, const int32_t* order, void* ws, void* stream) {
-    if (!fc1p || !nbr || !edge_feats || !w_fc1 || !ymax || !ymin || !stats) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: null pointer");
+                            float* ymax, float* ymin, double* stats, const int32_t* order, const void* plan, void* ws, void* stream) {
+    if (!fc1p || !nbr || !edge_feats || !w_fc1 || !ymax || !ymin || !stats || !plan) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: null pointer");
     if (B <= 0 || N <= 0 || cin <= 0) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: bad shape");
     if (C <= 0 || C > 128 || C % PVRAFT_GN_GROUPS) return fail(PVRAFT_ERR_UNSUPPORTED, "setconv_edge: C=%d (multiple of 8, <= 128)", C);
     if (reinterpret_cast<uintptr_t>(fc1p) % 16) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: fc1p must be 16-byte aligned (rows are bulk-copied)");
+    if (reinterpret_cast<uintptr_t>(plan) % 16) return fail(PVRAFT_ERR_BAD_ARG, "setconv_edge: plan must be 16-byte aligned");
     const int rows = edge_table_rows(C);
     const size_t smem = (size_t)2 * rows * C * sizeof(float) + sizeof(EdgeSmem);
-    const long long tiles = (long long)B * ((N + kEdgeTile - 1) / kEdgeTile);
+    const long long tiles = (long long)B * edge_tiles_per_sample(N);
     long long g = sm_count();
     if (g > tiles) g = tiles;
     const int grid = (int)g;
@@ -417,7 +358,8 @@ static int setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* 
     const auto kernel = C <= 64 ? k_setconv_edge_pairs<1, DET> : k_setconv_edge_pairs<2, DET>;
     int rc;
     if ((rc = opt_in_smem(kernel, smem))) return rc;
-    launch_pdl(kernel, grid, edge_threads(C <= 64 ? 1 : 2, DET), smem, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, kstats, order, rows);
+    launch_pdl(kernel, grid, edge_threads(C <= 64 ? 1 : 2, DET), smem, st, fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, kstats, order,
+               static_cast<const unsigned char*>(plan), rows);
     rc = check_launch("setconv_edge");
     if (rc || !DET) return rc;
     return gn_stats_flush(ws, B, stats, st);
@@ -425,9 +367,9 @@ static int setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* 
 
 extern "C" int pvraft_setconv_edge_fwd(const float* fc1p, const int32_t* nbr, const float* edge_feats, const float* w_fc1, int cin,
                                        int B, int N, int C, float* ymax, float* ymin, double* stats, const int32_t* order,
-                                       void* det_workspace, void* stream) {
+                                       const void* plan, void* det_workspace, void* stream) {
     auto f = det_workspace ? setconv_edge_fwd<true> : setconv_edge_fwd<false>;
-    return f(fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order, det_workspace, stream);
+    return f(fc1p, nbr, edge_feats, w_fc1, cin, B, N, C, ymax, ymin, stats, order, plan, det_workspace, stream);
 }
 
 extern "C" int64_t pvraft_setconv_edge_det_workspace_bytes(int B) { return gn_stats_ws_bytes(B); }

@@ -56,7 +56,8 @@ class SetConv(torch.nn.Module):
             p = ops.tc_linear([x], ops.tc_weights(self.fc1.weight, col0=0, cols=cin), **pro)
         else:
             p = ops.linear(x, _w(self.fc1.weight), cin=cin, w_ld=cin + 3, cout=mid, in_mode=IN_GN if deferred else ops.IN_PLAIN, **pro)
-        ymax, ymin = ops.setconv_edge(p, graph.nbr, graph._rel, _w(self.fc1.weight), cin, stats[0], order=getattr(graph, 'order', None))
+        ymax, ymin = ops.setconv_edge(p, graph.nbr, graph._rel, _w(self.fc1.weight), cin, stats[0], order=graph.order,
+                                      plan=graph.plan)
         gsz1, gsz = mid // 8, cout // 8
         pro1 = dict(in_min=ymin, in_stats=stats[0], in_gamma=_w(self.gn1.weight), in_beta=_w(self.gn1.bias),
                     in_count=float(n) * 32 * gsz1, in_act=ACT_LRELU, in_slope=0.1)

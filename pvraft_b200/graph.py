@@ -36,13 +36,22 @@ def edge_feats(xyz, nbr, rel):
 
 
 class Graph:
-    def __init__(self, nbr, edge_feats, k_neighbors, size, order=None):
+    def __init__(self, nbr, edge_feats, k_neighbors, size, order=None, plan=None):
         self.nbr = nbr                    # int32 [B,N,k] local ids
         self._rel = edge_feats            # f32 [B,N,k,3]
         self.order = order                # int32 [B,N] or None: processing order of the SetConv edge kernel (a Morton rank table)
         self.k_neighbors = k_neighbors
         self.size = tuple(size)
         self._edges = None
+        self._plan = plan
+
+    @property
+    def plan(self):
+        """The SetConv edge kernel's gather plan of (nbr, order) (ops.edge_plan), built on first use: every SetConv on this
+        graph, whatever its channel count, runs from it."""
+        if self._plan is None:
+            self._plan = ops.edge_plan(self.nbr, self.order)
+        return self._plan
 
     @property
     def edges(self):

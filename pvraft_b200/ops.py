@@ -560,15 +560,33 @@ def flow_out(args):
     _count(lib().pvraft_flow_out_fwd(C.byref(args), _stream()), 'flow_out')
 
 
-def setconv_edge(fc1p, nbr, edge_feats, w_fc1, cin, stats, ymax=None, ymin=None, order=None):
+def edge_plan(nbr, order=None):
+    """The SetConv edge kernel's gather plan of the kNN graph nbr [B,N,32] processed in `order` ([B,N] or None):
+    uint8 [B, tiles per sample, record bytes], sample-major, so plan[:b] is the plan of nbr[:b] (csrc/edge_plan.cuh)."""
+    b, n, _ = nbr.shape
+    rec = int(lib().pvraft_edge_plan_bytes(1, 1))
+    tiles = int(lib().pvraft_edge_plan_bytes(1, n)) // rec
+    plan = torch.empty(b, tiles, rec, dtype=torch.uint8, device=nbr.device)
+    _count(lib().pvraft_edge_plan_fwd(_p(nbr, torch.int32), _p(order, torch.int32), b, n, _p(plan, torch.uint8), _stream()),
+           'edge_plan')
+    return plan
+
+
+def setconv_edge(fc1p, nbr, edge_feats, w_fc1, cin, stats, ymax=None, ymin=None, order=None, plan=None):
+    """plan: edge_plan(nbr, order), built here when not given (a Graph keeps its own)."""
     b, n, c = fc1p.shape
     if ymax is None:
         ymax = torch.empty_like(fc1p)
     if ymin is None:
         ymin = torch.empty_like(fc1p)
+    if plan is None:
+        plan = edge_plan(nbr, order)
+    elif plan.shape[0] != b or plan.numel() != int(lib().pvraft_edge_plan_bytes(b, n)):
+        raise ValueError(f'edge plan of shape {tuple(plan.shape)} does not belong to a graph of {b} x {n} points')
     ws = _det_workspace(lib().pvraft_setconv_edge_det_workspace_bytes, b, device=fc1p.device)
     _count(lib().pvraft_setconv_edge_fwd(_p(fc1p), _p(nbr, torch.int32), _p(edge_feats), _p(w_fc1), cin, b, n, c, _p(ymax), _p(ymin),
-                                         _p(stats, torch.float64), _p(order, torch.int32), _p(ws, torch.uint8), _stream()), 'setconv_edge')
+                                         _p(stats, torch.float64), _p(order, torch.int32), _p(plan, torch.uint8), _p(ws, torch.uint8),
+                                         _stream()), 'setconv_edge')
     return ymax, ymin
 
 

@@ -238,7 +238,7 @@ class _RaftBase(nn.Module):
             fmap, graph2 = self.feature_extractor(both, point_major=True)
             fmap1, fmap2 = fmap[:b], fmap[b:]
             graph = Graph(graph2.nbr[:b], graph2._rel[:b], graph2.k_neighbors, [b * xyz1.shape[1]] * 2,
-                          None if graph2.order is None else graph2.order[:b])   # pc1's graph
+                          None if graph2.order is None else graph2.order[:b], graph2.plan[:b])   # pc1's graph
         else:
             # clouds of different sizes: one encoder pass per cloud (the kernels take one N per launch)
             fmap1, graph = self._encode_cloud(xyz1)                     # pc1's graph

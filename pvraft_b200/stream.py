@@ -25,7 +25,7 @@ _MAX_GRAPHS = 8
 
 def _scan_state(fmap, graph):
     """What a stream keeps of an encoded scan besides its points: the feature map and the kNN graph's tensors."""
-    state = {'fmap': fmap, 'nbr': graph.nbr, 'rel': graph._rel}
+    state = {'fmap': fmap, 'nbr': graph.nbr, 'rel': graph._rel, 'plan': graph.plan}
     if graph.order is not None:
         state['order'] = graph.order
     return state
@@ -53,7 +53,7 @@ class SceneFlowStream:
         self.reset()
 
     def reset(self):
-        self._scan = None   # the last scan: {'xyz', 'fmap', 'nbr', 'rel'[, 'order']}
+        self._scan = None   # the last scan: {'xyz', 'fmap', 'nbr', 'rel', 'plan'[, 'order']}
         self._stamp = None  # the model's parameters when that scan was encoded
         self._last = None   # the last pair: (its first cloud, its final flow on that cloud)
 
@@ -100,7 +100,7 @@ class SceneFlowStream:
             return None, new
         xyz1 = s['xyz1']
         b, n1, _ = xyz1.shape
-        graph1 = Graph(s['nbr1'], s['rel1'], ops.KNN, [b * n1] * 2, s.get('order1'))
+        graph1 = Graph(s['nbr1'], s['rel1'], ops.KNN, [b * n1] * 2, s.get('order1'), s['plan1'])
         flow_init = ops.flow_propagate(s['src_xyz'], s['src_flow'], xyz1, self.k) if 'src_xyz' in s else None
         return m._run(m._pair(xyz1, s['xyz'], s['fmap1'], graph1, fmap), self.num_iters, flow_init), new
 

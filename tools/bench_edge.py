@@ -6,7 +6,8 @@ clouds.  Shapes (bench default, B = 8, N = 8192):
   loop      B = 8,  C = 64, cin = 64  (flow-head SetConv, 32 launches per forward)
   feat1..3  B = 16, C = 16 / 48 / 96, cin = 3 / 32 / 64  (feature encoder over both clouds)
   ctx1..3   B = 8,  same channels  (context encoder over pc1)
-Each shape is timed with the Morton order and with order = None (index order)."""
+Each shape is timed with the Morton order and with order = None (index order), each from its graph's gather plan
+(ops.edge_plan, built once per graph and not counted in the launch); the plan build itself is timed once per graph."""
 import argparse
 import os
 import subprocess
@@ -28,11 +29,7 @@ def card_line():
         return f'(nvidia-smi unavailable: {e})'
 
 
-def time_edge(p, g, w, cin, order, launches, det):
-    b = p.shape[0]
-    st = torch.zeros(b, 8, 2, dtype=torch.float64, device=p.device)
-    ymax, ymin = torch.empty_like(p), torch.empty_like(p)
-    run = lambda: ops.setconv_edge(p, g.nbr, g._rel, w, cin, st, ymax, ymin, order=order)
+def time_launches(run, launches, det=False):
     prev = torch.are_deterministic_algorithms_enabled()
     torch.use_deterministic_algorithms(det)
     try:
@@ -53,6 +50,13 @@ def time_edge(p, g, w, cin, order, launches, det):
     return sorted(times)[len(times) // 2], min(times), max(times)
 
 
+def time_edge(p, g, w, cin, order, plan, launches, det):
+    b = p.shape[0]
+    st = torch.zeros(b, 8, 2, dtype=torch.float64, device=p.device)
+    ymax, ymin = torch.empty_like(p), torch.empty_like(p)
+    return time_launches(lambda: ops.setconv_edge(p, g.nbr, g._rel, w, cin, st, ymax, ymin, order=order, plan=plan), launches, det)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--launches', type=int, default=50, help='launches per timed window (5 windows, median reported)')
@@ -64,6 +68,12 @@ def main():
     pc1, pc2 = [t.to(dev) for t in bench.synthetic_clouds(b, n, 1234)]
     both = torch.cat([pc1, pc2], 0).contiguous()
     g8, g16 = Graph.construct_graph(pc1, 32), Graph.construct_graph(both, 32)
+    plans = {}
+    for gname, g in (('B=8 ', g8), ('B=16', g16)):
+        for oname, order in (('morton', g.order), ('index ', None)):
+            plans[id(g), oname] = ops.edge_plan(g.nbr, order)
+            med, lo, hi = time_launches(lambda: ops.edge_plan(g.nbr, order), a.launches)
+            print(f'edge_plan {gname} {oname}: {med:8.1f} us  (min {lo:.1f}, max {hi:.1f})', flush=True)
     shapes = [('loop ', g8, 64, 64)] + [(f'feat{i + 1}', g16, c, cin) for i, (c, cin) in enumerate([(16, 3), (48, 32), (96, 64)])] \
         + [(f'ctx{i + 1} ', g8, c, cin) for i, (c, cin) in enumerate([(16, 3), (48, 32), (96, 64)])]
     torch.manual_seed(0)
@@ -73,7 +83,7 @@ def main():
         w = torch.randn(c, cin + 3, device=dev)
         for det in ([False, True] if a.det else [False]):
             for oname, order in (('morton', g.order), ('index ', None)):
-                med, lo, hi = time_edge(p, g, w, cin, order, a.launches, det)
+                med, lo, hi = time_edge(p, g, w, cin, order, plans[id(g), oname], a.launches, det)
                 gathers = bb * n * 32 * c * 4 / 1e9   # neighbour-row bytes the gathers read per launch
                 print(f'{label} B={bb:2d} C={c:3d} {"DET " if det else ""}{oname}: {med:8.1f} us  (min {lo:.1f}, max {hi:.1f}; '
                       f'{gathers * 1e3:.0f} MB of neighbour rows, {gathers / (med * 1e-6) / 1e3:.2f} TB/s)', flush=True)
