@@ -20,6 +20,8 @@
  *   - GroupNorm statistics travel as raw double-precision sums ("stats": [B,8,2] = per sample,
  *     per group (sum, sum of squares)); producers ACCUMULATE with atomics, so the caller zeroes
  *     them (cudaMemsetAsync) before the producing call (in a fixed order with a det_workspace, see "Deterministic mode").
+ *     Every producer keeps the sums accurate enough for var = sum x^2 / n - mean^2 to hold the variance to about 1e-7
+ *     relative even when a group's mean is thousands of times its spread (fp32 partials are formed about a pivot value).
  *   - Weights are passed in the reference's own state_dict layouts ([Cout,Cin(,1(,1))] row-major).
  *   - Deterministic mode (what pvraft_b200 runs while torch.are_deterministic_algorithms_enabled() is true).  Every entry
  *     point that reduces floating-point values takes `void* det_workspace` as its last argument before `stream`.  NULL runs

@@ -80,6 +80,23 @@ __device__ __forceinline__ GnAffine gn_affine(const double* stats_bg /* (sum,sum
     return a;
 }
 
+// GroupNorm raw sums of n fp32 values y without the fp32 error that gn_affine's var = sum y^2 / n - mean^2 would expose:
+// plain fp32 partials of y^2 carry ~2^-24 mean^2, which stays standing next to the variance (a relative 2^-24 r^2 for a
+// group whose mean is r times its spread).  So sum y^2 is formed from the fp32 sum of squares about a pivot p, one of the
+// values, whose error is ~2^-24 of the spread: sum y^2 = sum (y - p)^2 + p (2 sum y - n p), in double (pivot_sumsq).  sum y
+// itself comes from a compensated fp32 sum (kahan_add: the pair s - err holds it to ~2^-48), so that the mean is as exact as
+// double accumulation would make it.
+__device__ __forceinline__ void kahan_add(float& s, float& err, float y) {
+    const float v = y - err, t = s + v;
+    err = (t - s) - v;
+    s = t;
+}
+__device__ __forceinline__ double kahan_value(float s, float err) { return (double)s - (double)err; }
+__device__ __forceinline__ double pivot_sumsq(double sum_y, float p, float sdd, int n) {
+    const double dp = p;
+    return fma(dp, 2.0 * sum_y - (double)n * dp, (double)sdd);
+}
+
 __device__ __forceinline__ float apply_act(float x, int act, float slope) {
     if (act == PVRAFT_ACT_RELU) return fmaxf(x, 0.f);
     if (act == PVRAFT_ACT_LRELU) return x >= 0.f ? x : slope * x;

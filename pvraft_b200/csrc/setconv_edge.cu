@@ -6,7 +6,8 @@
 // once per point by pvraft_linear_fwd; this kernel only gathers the 32 rows P_j.
 // GroupNorm + LeakyReLU is monotone per channel, so max_e lrelu(GN(y_e)) = lrelu(GN(max_e y_e)) when the
 // folded GN scale is >= 0 and lrelu(GN(min_e y_e)) otherwise: the kernel emits both the per-channel max
-// and min of the raw y, plus the double-precision (sum, sum^2) of all N*32*C raw values per group.
+// and min of the raw y, plus the double-precision (sum, sum^2) of all N*32*C raw values per group (each point's 32 edges
+// summed in fp32 about its first edge's value and converted exactly: pivot_sumsq, csrc/common.cuh).
 //
 // Persistent and warp-specialised, one CTA per SM.  A CTA walks tiles of kEdgeTile consecutive positions of the processing
 // order (edge_plan.cuh), driven by the graph's gather plan (edge_plan.cu): the producer warps bulk-copy tile t + 1's row ids
@@ -92,37 +93,47 @@ __device__ __forceinline__ float2 ld_row(const float* p) {
     else return __ldg(reinterpret_cast<const float2*>(p));
 }
 
-// one point: y_e = (P_j - P_i) + W_e.e over the 32 edges in order 0..31 -> per-channel max, min, sum and sum of squares.
+// y = (P_j - P_i) + fma(w_z, e_z, fma(w_y, e_y, w_x * e_x)) of one edge, both channels of a pair at once.  ed: the edge's
+// (row offset, edge vector); pi: the centre's pair
+template <bool TABLE>
+__device__ __forceinline__ unsigned long long edge_y2(const float* rows, const float4& ed, int coff, unsigned long long pi,
+                                                      unsigned long long wx2, unsigned long long wy2, unsigned long long wz2) {
+    const float2 pj = ld_row<TABLE>(rows + __float_as_int(ed.x) + coff);
+    const unsigned long long t = fma2(wz2, pk(ed.w, ed.w), fma2(wy2, pk(ed.z, ed.z), mul2(wx2, pk(ed.y, ed.y))));
+    return add2(sub2(pk(pj.x, pj.y), pi), t);
+}
+
+// one point: y_e = (P_j - P_i) + W_e.e over the 32 edges in order 0..31 -> per-channel max, min, and the sum and sum of
+// squares of y_e - piv with the pivot piv = y_0 (pivot_sumsq).  The sum is of y_e - piv too, uncompensated: a compensated
+// sum does not fit the register budget of the one-pair form (it spills), so a point's mean carries ~2^-24 of its spread.
 // rows: the shared table (TABLE) or the sample's P; se: the warp's (row offset, edge vector) list; ctr: the centre row P_i
 template <int PAIRS, bool TABLE>
 __device__ __forceinline__ void edge_point(const float* rows, const float4* se, const float* ctr, const int (&coff)[PAIRS],
                                            const unsigned long long (&wx2)[PAIRS], const unsigned long long (&wy2)[PAIRS],
                                            const unsigned long long (&wz2)[PAIRS], float2 (&mx)[PAIRS], float2 (&mn)[PAIRS],
-                                           unsigned long long (&s1)[PAIRS], unsigned long long (&s2)[PAIRS]) {
+                                           unsigned long long (&piv)[PAIRS], unsigned long long (&s1)[PAIRS],
+                                           unsigned long long (&s2)[PAIRS]) {
     unsigned long long pi[PAIRS];
 #pragma unroll
     for (int q = 0; q < PAIRS; ++q) {
         const float2 t = ld_row<TABLE>(ctr + coff[q]);
         pi[q] = pk(t.x, t.y);
+        piv[q] = edge_y2<TABLE>(rows, se[0], coff[q], pi[q], wx2[q], wy2[q], wz2[q]);
         mx[q] = make_float2(-INFINITY, -INFINITY); mn[q] = make_float2(INFINITY, INFINITY);
         s1[q] = pk(0.f, 0.f); s2[q] = pk(0.f, 0.f);
     }
 #pragma unroll 8
     for (int e = 0; e < 32; ++e) {
         const float4 ed = se[e];
-        const float* row = rows + __float_as_int(ed.x);
-        const unsigned long long ex = pk(ed.y, ed.y), ey = pk(ed.z, ed.z), ez = pk(ed.w, ed.w);
 #pragma unroll
         for (int q = 0; q < PAIRS; ++q) {
-            const float2 pj = ld_row<TABLE>(row + coff[q]);
-            // y = (P_j - P_i) + fma(w_z, e_z, fma(w_y, e_y, w_x * e_x)), both channels of the pair at once
-            const unsigned long long t = fma2(wz2[q], ez, fma2(wy2[q], ey, mul2(wx2[q], ex)));
-            const unsigned long long y2 = add2(sub2(pk(pj.x, pj.y), pi[q]), t);
+            const unsigned long long y2 = edge_y2<TABLE>(rows, ed, coff[q], pi[q], wx2[q], wy2[q], wz2[q]);
             const float2 y = upk(y2);
             mx[q].x = fmaxf(mx[q].x, y.x); mx[q].y = fmaxf(mx[q].y, y.y);
             mn[q].x = fminf(mn[q].x, y.x); mn[q].y = fminf(mn[q].y, y.y);
-            s1[q] = add2(s1[q], y2);
-            s2[q] = fma2(y2, y2, s2[q]);
+            const unsigned long long d2 = sub2(y2, piv[q]);
+            s1[q] = add2(s1[q], d2);
+            s2[q] = fma2(d2, d2, s2[q]);
         }
     }
 }
@@ -306,11 +317,11 @@ __global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pa
             s.edge[w][lane] = make_float4(__int_as_float(off), e.x, e.y, e.z);
             __syncwarp();
             float2 mx[PAIRS], mn[PAIRS];
-            unsigned long long s1[PAIRS], s2[PAIRS];
+            unsigned long long piv[PAIRS], s1[PAIRS], s2[PAIRS];
             if (in_table)
-                edge_point<PAIRS, true>(table, s.edge[w], table + s.slot[buf][kEdgeTile * 32 + p] * C, coff, wx2, wy2, wz2, mx, mn, s1, s2);
+                edge_point<PAIRS, true>(table, s.edge[w], table + s.slot[buf][kEdgeTile * 32 + p] * C, coff, wx2, wy2, wz2, mx, mn, piv, s1, s2);
             else
-                edge_point<PAIRS, false>(P, s.edge[w], P + (size_t)i * C, coff, wx2, wy2, wz2, mx, mn, s1, s2);
+                edge_point<PAIRS, false>(P, s.edge[w], P + (size_t)i * C, coff, wx2, wy2, wz2, mx, mn, piv, s1, s2);
 #pragma unroll
             for (int q = 0; q < PAIRS; ++q) {
                 const size_t o = (size_t)pt * C + coff[q];
@@ -318,13 +329,15 @@ __global__ void __launch_bounds__(edge_threads(PAIRS, DET), 1) k_setconv_edge_pa
                     *reinterpret_cast<float2*>(ymax + o) = mx[q];
                     *reinterpret_cast<float2*>(ymin + o) = mn[q];
                 }
-                const float2 a1 = upk(s1[q]), a2 = upk(s2[q]);
+                const float2 pv = upk(piv[q]), a1 = upk(s1[q]), a2 = upk(s2[q]);
+                const double t1[2] = {fma(32.0, (double)pv.x, (double)a1.x), fma(32.0, (double)pv.y, (double)a1.y)};
+                const double t2[2] = {pivot_sumsq(t1[0], pv.x, a2.x, 32), pivot_sumsq(t1[1], pv.y, a2.y, 32)};
                 if constexpr (DET) {
-                    fx_add(fS[q][0], fx_from((double)a1.x)); fx_add(fS[q][1], fx_from((double)a1.y));
-                    fx_add(fSS[q][0], fx_from((double)a2.x)); fx_add(fSS[q][1], fx_from((double)a2.y));
+                    fx_add(fS[q][0], fx_from(t1[0])); fx_add(fS[q][1], fx_from(t1[1]));
+                    fx_add(fSS[q][0], fx_from(t2[0])); fx_add(fSS[q][1], fx_from(t2[1]));
                 } else {
-                    dS[q][0] += (double)a1.x; dS[q][1] += (double)a1.y;
-                    dSS[q][0] += (double)a2.x; dSS[q][1] += (double)a2.y;
+                    dS[q][0] += t1[0]; dS[q][1] += t1[1];
+                    dSS[q][0] += t2[0]; dSS[q][1] += t2[1];
                 }
             }
         }

@@ -173,15 +173,20 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, float* __restrict
                     for (int i = 0; i < 8; ++i) *reinterpret_cast<float4*>(obase + i * ostep + c0) = t[i];
                 }
                 if (want_stats) {
-                    // lane = column: (sum, sum^2) of this warp's 32 rows, read down the staged tile (conflict-free)
-                    float s1 = 0.f, s2 = 0.f;
+                    // lane = column: (sum, sum^2) of this warp's 32 rows, read down the staged tile (conflict-free): the
+                    // compensated sum, the squares about the column's first row (pivot_sumsq); the double sums then
+                    // replace the block's first four rows
+                    const float piv = stg[lane];
+                    float s1 = 0.f, e1 = 0.f, s2 = 0.f;
 #pragma unroll
                     for (int r = 0; r < 32; ++r) {
-                        const float a = stg[r * pitch + lane];
-                        s1 += a;
-                        s2 = fmaf(a, a, s2);
+                        const float a = stg[r * pitch + lane], d = a - piv;
+                        kahan_add(s1, e1, a);
+                        s2 = fmaf(d, d, s2);
                     }
-                    *reinterpret_cast<float2*>(s_part + (size_t)(quad * 128 + c0 + lane) * 2) = make_float2(s1, s2);
+                    const double a1 = kahan_value(s1, e1), a2 = pivot_sumsq(a1, piv, s2, 32);
+                    __syncwarp();
+                    *reinterpret_cast<double2*>(stg + (lane >> 3) * pitch + (lane & 7) * 4) = make_double2(a1, a2);
                 }
             } else {
                 float* o = p.out + (size_t)row * p.out_ld + c0;
@@ -197,11 +202,13 @@ __device__ __forceinline__ void tc_epilogue(const TcParams& p, float* __restrict
             const int t = (half * 4 + quad) * 32 + lane;   // 0..255; threads 0..N-1 own one column each
             double a1 = 0.0, a2 = 0.0;
             if (t < p.N) {
+                // column t's partial of the warp of lane quadrant w: in that warp's staged block of chunk t & ~31
+                const float* part = s_acc + (size_t)((t & 31) >> 3) * pitch + (t & ~31) + (t & 7) * 4;
 #pragma unroll
                 for (int w = 0; w < 4; ++w) {
-                    const float2 pr = *reinterpret_cast<const float2*>(s_part + (size_t)(w * 128 + t) * 2);
-                    a1 += (double)pr.x;
-                    a2 += (double)pr.y;
+                    const double2 pr = *reinterpret_cast<const double2*>(part + (size_t)w * 32 * pitch);
+                    a1 += pr.x;
+                    a2 += pr.y;
                 }
             }
             if ((gsz & (gsz - 1)) == 0 && gsz <= 32) {   // groups are aligned runs of gsz lanes
@@ -355,7 +362,7 @@ k_tc_linear(const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant_
     float* s_bias = s_scale + 4 * p.K;                                            // [2 * N]
     float* s_acc = s_bias + 2 * p.N;                                              // [128 rows][acc_pitch] accumulator tile
     float* s_estage = s_acc + (size_t)kTcM * acc_pitch;                           // GRU epilogues: [8 warps][32][20] staging
-    float* s_part = s_estage + (p.epi == TC_EPI_GRU_ZR || p.epi == TC_EPI_GRU_Q ? 8 * 32 * kTcPitch16 : 0);   // [4 warps][128 columns][2]
+    float* s_part = s_estage + (p.epi == TC_EPI_GRU_ZR || p.epi == TC_EPI_GRU_Q ? 8 * 32 * kTcPitch16 : 0);   // FLOW: [128 rows][4] exchange | w3
     __shared__ __align__(8) unsigned long long s_full[kTcMaxStages], s_empty[kTcMaxStages];
     __shared__ __align__(8) unsigned long long s_acc_full, s_acc_empty, s_w_full;
     const int warp = warp_id(), lane = lane_id();

@@ -473,15 +473,18 @@ __global__ void __launch_bounds__(256) k_edge_fwd(const float* __restrict__ P, c
         const float* pc = P + (size_t)pt * C;
         for (int c = lane; c < C; c += 32) {
             const float ctr = __ldg(pc + c);
-            float s = 0.f, ss = 0.f;
+            float piv = 0.f, ps = 0.f, pe = 0.f, pss = 0.f;   // compensated sum, squares about the first neighbour's value
             for (int j = 0; j < PVRAFT_KNN; ++j) {
                 const int nb = __ldg(nbr + pt * PVRAFT_KNN + j);
                 float* e = E + ((size_t)pt * PVRAFT_KNN + j) * C + c;
                 const float t = (__ldg(Pb + (size_t)nb * C + c) - ctr) + *e;
                 *e = t;
-                s += t;
-                ss += t * t;
+                if (j == 0) piv = t;
+                const float d = t - piv;
+                kahan_add(ps, pe, t);
+                pss = fmaf(d, d, pss);
             }
+            const double s = kahan_value(ps, pe), ss = pivot_sumsq(s, piv, pss, PVRAFT_KNN);
             if constexpr (DET) {   // one (point, channel) sum of 32 neighbours per contribution
                 if (stats) {
                     const FxSlots dst = b == b0 ? s_fx : stats + b * 16;
@@ -490,11 +493,11 @@ __global__ void __launch_bounds__(256) k_edge_fwd(const float* __restrict__ P, c
                 }
             } else if (stats) {
                 if (b == b0) {
-                    atomicAdd(&s_g[(c / gsz) * 2], (double)s);
-                    atomicAdd(&s_g[(c / gsz) * 2 + 1], (double)ss);
+                    atomicAdd(&s_g[(c / gsz) * 2], s);
+                    atomicAdd(&s_g[(c / gsz) * 2 + 1], ss);
                 } else {
-                    atomicAdd(stats + (size_t)b * 16 + (c / gsz) * 2, (double)s);
-                    atomicAdd(stats + (size_t)b * 16 + (c / gsz) * 2 + 1, (double)ss);
+                    atomicAdd(stats + (size_t)b * 16 + (c / gsz) * 2, s);
+                    atomicAdd(stats + (size_t)b * 16 + (c / gsz) * 2 + 1, ss);
                 }
             }
         }
