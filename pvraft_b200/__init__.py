@@ -8,9 +8,10 @@ from .loss import flow_consistency
 from .pointconv import knn_point, square_distance
 from .raft import RSF, RSF_refine
 from .refine import FlotRefine
+from .rigid import RigidMotion, rigid_motion
 from .stream import SceneFlowStream
 from .update import ConvGRU, ConvRNN, FlowHead, MotionEncoder, UpdateBlock
 
 __all__ = ['RSF', 'RSF_refine', 'CorrBlock', 'UpdateBlock', 'MotionEncoder', 'ConvGRU', 'ConvRNN', 'FlowHead',
            'FlotEncoder', 'FlotRefine', 'SetConv', 'Graph', 'knn_point', 'square_distance', 'SceneFlowStream',
-           'flow_consistency']
+           'flow_consistency', 'rigid_motion', 'RigidMotion']
