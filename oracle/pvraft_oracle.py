@@ -15,6 +15,7 @@ Weights are a flat dict keyed exactly like the reference `state_dict()`
 (e.g. 'corr_block.out_conv.0.weight'), so a reference checkpoint can be fed in directly.
 
 Layout conventions follow the reference: coordinates / flows [B,N,3]; feature maps [B,C,N].
+Every function follows its inputs' dtype and device, so tests/grad_replay.py also runs it in float64 on the GPU.
 """
 from __future__ import annotations
 
@@ -60,14 +61,26 @@ def group_norm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups:
     return xn * gamma.view(bshape) + beta.view(bshape)
 
 
-def prelu(x: torch.Tensor, a: torch.Tensor) -> torch.Tensor:
+# `layer` (the GroupNorm or 1x1 convolution that feeds an activation) and neighbour_max's `layer` name where the forward
+# takes a discrete decision -- an activation's branch, an arg-max -- so that tests/grad_replay.py can substitute the
+# decisions another run took.  They change nothing here.
+def prelu(x: torch.Tensor, a: torch.Tensor, layer: Optional[str] = None) -> torch.Tensor:
     """nn.PReLU() with a single shared slope (model/corr.py:18,26)."""
     return torch.where(x >= 0, x, a.view(-1)[0] * x)
 
 
-def leaky_relu(x: torch.Tensor, slope: float = 0.1) -> torch.Tensor:
+def leaky_relu(x: torch.Tensor, slope: float = 0.1, layer: Optional[str] = None) -> torch.Tensor:
     """LeakyReLU(0.1), model/flot/gconv.py:36."""
     return torch.where(x >= 0, x, slope * x)
+
+
+def relu(x: torch.Tensor, layer: Optional[str] = None) -> torch.Tensor:
+    return torch.relu(x)
+
+
+def neighbour_max(x: torch.Tensor, dim: int, layer: str) -> torch.Tensor:
+    """Max over the 32 neighbours along `dim` (gconv.py:80, corr.py:92); `layer` names the GroupNorm that feeds it."""
+    return x.max(dim=dim).values
 
 
 # --------------------------------------------------------------------------------------
@@ -128,12 +141,12 @@ def set_conv(P: Params, prefix: str, signal: torch.Tensor, graph: Graph) -> torc
     x = torch.cat([edge.reshape(-1, c), graph.edge_feats], -1)              # gconv.py:66
     x = x.reshape(b, n, k, c + 3).permute(0, 3, 2, 1)                       # [B,C+3,k,N] gconv.py:67-68
     x = pointwise_linear(x, P[prefix + '.fc1.weight'])
-    x = leaky_relu(group_norm(x, P[prefix + '.gn1.weight'], P[prefix + '.gn1.bias']))
-    x = x.max(dim=2).values                                                 # [B,mid,N]
+    x = leaky_relu(group_norm(x, P[prefix + '.gn1.weight'], P[prefix + '.gn1.bias']), layer=prefix + '.gn1')
+    x = neighbour_max(x, 2, prefix + '.gn1')                                # [B,mid,N]
     x = pointwise_linear(x, P[prefix + '.fc2.weight'])
-    x = leaky_relu(group_norm(x, P[prefix + '.gn2.weight'], P[prefix + '.gn2.bias']))
+    x = leaky_relu(group_norm(x, P[prefix + '.gn2.weight'], P[prefix + '.gn2.bias']), layer=prefix + '.gn2')
     x = pointwise_linear(x, P[prefix + '.fc3.weight'])
-    x = leaky_relu(group_norm(x, P[prefix + '.gn3.weight'], P[prefix + '.gn3.bias']))
+    x = leaky_relu(group_norm(x, P[prefix + '.gn3.weight'], P[prefix + '.gn3.bias']), layer=prefix + '.gn3')
     return x.transpose(1, 2)                                                # [B,N,Cout]
 
 
@@ -167,7 +180,8 @@ class CorrState(NamedTuple):
 
 
 def calculate_corr(fmap1: torch.Tensor, fmap2: torch.Tensor) -> torch.Tensor:
-    """model/corr.py:95-100: fmap1^T fmap2 / sqrt(C)."""
+    """model/corr.py:95-100: fmap1^T fmap2 / sqrt(C).  The divisor is the reference's fp32 sqrt(C) in every dtype: a 0-dim
+    fp32 tensor does not demote float64 maps, so a float64 reference divides by sqrt(C) rounded to fp32 too."""
     c = fmap1.shape[1]
     corr = torch.matmul(fmap1.transpose(1, 2), fmap2)
     return corr / torch.sqrt(torch.tensor(c).float())
@@ -208,8 +222,8 @@ def voxel_means(state: CorrState, coords: torch.Tensor, num_levels: int, base_sc
         r = base_scale * (2 ** lvl)
         cube, valid = voxel_cube_index(state, coords, r)
         w = valid.to(state.truncated_corr.dtype)
-        s = torch.zeros(b, n, cells, device=coords.device).scatter_add_(2, cube, state.truncated_corr * w)
-        c = torch.zeros(b, n, cells, device=coords.device).scatter_add_(2, cube, w)
+        s = torch.zeros(b, n, cells, dtype=w.dtype, device=coords.device).scatter_add_(2, cube, state.truncated_corr * w)
+        c = torch.zeros(b, n, cells, dtype=w.dtype, device=coords.device).scatter_add_(2, cube, w)
         feats.append((s / torch.clamp(c, 1, n)).transpose(1, 2))
     return torch.cat(feats, dim=1).contiguous()
 
@@ -220,7 +234,7 @@ def voxel_feature(P: Params, state: CorrState, coords: torch.Tensor, num_levels:
     x = voxel_means(state, coords, num_levels, base_scale)
     x = pointwise_linear(x, P[prefix + '.out_conv.0.weight'], P[prefix + '.out_conv.0.bias'])
     x = prelu(group_norm(x, P[prefix + '.out_conv.1.weight'], P[prefix + '.out_conv.1.bias']),
-              P[prefix + '.out_conv.2.weight'])
+              P[prefix + '.out_conv.2.weight'], layer=prefix + '.out_conv.1')
     return pointwise_linear(x, P[prefix + '.out_conv.3.weight'], P[prefix + '.out_conv.3.bias'])
 
 
@@ -250,8 +264,8 @@ def knn_feature(P: Params, state: CorrState, coords: torch.Tensor, knn: int = KN
     x = knn_gather(state, coords, knn_select(state, coords, knn))
     x = pointwise_linear(x, P[prefix + '.knn_conv.0.weight'], P[prefix + '.knn_conv.0.bias'])
     x = prelu(group_norm(x, P[prefix + '.knn_conv.1.weight'], P[prefix + '.knn_conv.1.bias']),
-              P[prefix + '.knn_conv.2.weight'])
-    x = x.max(dim=3).values
+              P[prefix + '.knn_conv.2.weight'], layer=prefix + '.knn_conv.1')
+    x = neighbour_max(x, 3, prefix + '.knn_conv.1')
     return pointwise_linear(x, P[prefix + '.knn_out.weight'], P[prefix + '.knn_out.bias'])
 
 
@@ -268,9 +282,9 @@ def corr_lookup(P: Params, state: CorrState, coords: torch.Tensor, num_levels: i
 def motion_encoder(P: Params, flow: torch.Tensor, corr: torch.Tensor, prefix: str) -> torch.Tensor:
     """model/update.py:15-21 -> [B,64,N] (61 learned channels ++ the 3 flow channels)."""
     ft = flow.transpose(1, 2)
-    cor = torch.relu(pointwise_linear(corr, P[prefix + '.conv_corr.weight'], P[prefix + '.conv_corr.bias']))
-    flo = torch.relu(pointwise_linear(ft, P[prefix + '.conv_flow.weight'], P[prefix + '.conv_flow.bias']))
-    out = torch.relu(pointwise_linear(torch.cat([cor, flo], 1), P[prefix + '.conv.weight'], P[prefix + '.conv.bias']))
+    cor = relu(pointwise_linear(corr, P[prefix + '.conv_corr.weight'], P[prefix + '.conv_corr.bias']), prefix + '.conv_corr')
+    flo = relu(pointwise_linear(ft, P[prefix + '.conv_flow.weight'], P[prefix + '.conv_flow.bias']), prefix + '.conv_flow')
+    out = relu(pointwise_linear(torch.cat([cor, flo], 1), P[prefix + '.conv.weight'], P[prefix + '.conv.bias']), prefix + '.conv')
     return torch.cat([out, ft], dim=1)
 
 
@@ -287,7 +301,8 @@ def flow_head(P: Params, x: torch.Tensor, graph: Graph, prefix: str) -> torch.Te
     """model/update.py:68-72 -> [B,3,N]."""
     a = pointwise_linear(x, P[prefix + '.conv1.weight'], P[prefix + '.conv1.bias'])
     s = set_conv(P, prefix + '.setconv', x.transpose(1, 2), graph).transpose(1, 2)
-    y = torch.relu(pointwise_linear(torch.cat([s, a], 1), P[prefix + '.out_conv.0.weight'], P[prefix + '.out_conv.0.bias']))
+    y = relu(pointwise_linear(torch.cat([s, a], 1), P[prefix + '.out_conv.0.weight'], P[prefix + '.out_conv.0.bias']),
+             prefix + '.out_conv.0')
     return pointwise_linear(y, P[prefix + '.out_conv.2.weight'], P[prefix + '.out_conv.2.bias'])
 
 
@@ -318,7 +333,7 @@ def prepare(P: Params, xyz1: torch.Tensor, xyz2: torch.Tensor, truncate_k: int) 
     state = corr_init(fmap1, fmap2, xyz2, truncate_k)
     fct1, gctx = flot_encoder(P, 'context_extractor', xyz1)
     net, inp = torch.split(fct1, [64, 64], dim=1)
-    return LoopInputs(state, torch.tanh(net), torch.relu(inp), gctx, g1)
+    return LoopInputs(state, torch.tanh(net), relu(inp, 'context_extractor'), gctx, g1)
 
 
 def raft_loop(P: Params, li: LoopInputs, xyz1: torch.Tensor, num_iters: int, num_levels: int,

@@ -8,11 +8,18 @@ record of how they were made.
 The only thing added to the reference is a shim for its one absent third-party import,
 `torch_scatter.scatter_add` (model/corr.py:50), with torch-scatter's documented semantics
 (sum-scatter along `dim`, output width max(index)+1).
+
+The gradient fixtures (ref_grads_rsf.npz, ref_grads_refine.npz) run the reference in float64 with autograd.  Its backward
+into the input clouds fails under current torch ("modified by an inplace operation: [torch.LongTensor]"): graph.py:72
+indexes the cloud with a view of `neighbors` that graph.py:77-79 then offsets in place.  The forward therefore runs under
+torch.autograd.graph.saved_tensors_hooks(pack=clone), which saves a copy of every tensor autograd keeps, so the in-place
+offset no longer reaches the saved index.  That is a runtime hook; the reference's source is untouched.
 """
 import copy
 import os
 import sys
 import types
+import zlib
 
 import numpy as np
 import torch
@@ -108,6 +115,71 @@ def trace_forward(model, pc1, pc2, iters):
     return {k: (v.detach().cpu().numpy() if torch.is_tensor(v) else v) for k, v in out.items()}
 
 
+def sequence_loss(flows, gt, gamma=0.8):
+    """tools/loss.py:4-13 with an all-ones mask (the form tests/train_helpers.py uses)."""
+    n = len(flows)
+    return sum(gamma ** (n - i - 1) * (flows[i] - gt).abs().sum(-1).mean() for i in range(n))
+
+
+def local_adjacency(graph, b, n):
+    """Graph.edges (global ids b*N + j) -> local ids [B,N,k] int16, each row sorted (a set: the order is not a decision)."""
+    e = graph.edges.reshape(b, n, -1) - (torch.arange(b) * n).view(b, 1, 1)
+    return np.sort(e.numpy(), -1).astype(np.int16)
+
+
+SKETCH = 128
+
+
+def grad_sketch(name, g):
+    """A float64 gradient -> what the fixtures keep of it: the tensor itself (flattened) when it has at most SKETCH
+    elements, else S g = V g / sqrt(SKETCH), V [SKETCH, numel] standard normal from a generator seeded by the tensor's
+    name.  S is a fixed random (Johnson-Lindenstrauss) sketch: for any a, ||S a - S g|| / ||S g|| estimates the relative
+    L2 error ||a - g|| / ||g|| within a factor 1 +- 0.2 (a few standard deviations of a chi distribution with SKETCH
+    degrees of freedom), in float64, at 1 KiB per tensor instead of 8 bytes per element."""
+    g = torch.as_tensor(g).detach().to(torch.float64).reshape(-1)
+    if g.numel() <= SKETCH:
+        return g.numpy()
+    gen = torch.Generator().manual_seed(zlib.crc32(name.encode()))
+    return (torch.randn(SKETCH, g.numel(), generator=gen, dtype=torch.float64) @ g / SKETCH ** 0.5).numpy()
+
+
+def reference_gradients(rsf, rsf_refine, pc1, pc2, iters):
+    """Fixtures 6 and 7: float64 gradients of the unmodified reference.
+
+    6: RSF, the sequence loss over `iters` flows -> every parameter gradient, d xyz1, d xyz2, the adjacency of both
+       clouds' graphs and the top-K ids of the correlation (as sets: rows sorted).
+    7: RSF_refine, the mean L1 error of the refined flow -> the refine_block gradients and d xyz1 (the loop runs under
+       no_grad, RAFTSceneFlowRefine.py:23; xyz1 reaches the loss through coords2 - coords1 only).
+    Each gradient is kept as 's/<name>', its float64 grad_sketch."""
+    hook = torch.autograd.graph.saved_tensors_hooks(lambda t: t.clone(), lambda t: t)
+    b, n, _ = pc1.shape
+    gt = pc2 - pc1
+    out = []
+    for model in (rsf, rsf_refine):
+        x1, x2 = pc1.clone().requires_grad_(True), pc2.clone().requires_grad_(True)
+        with hook:
+            pred = model([x1, x2], iters)
+        loss = sequence_loss(pred, gt) if isinstance(pred, list) else (pred - gt).abs().sum(-1).mean()
+        loss.backward()
+        grads = {k: p.grad for k, p in model.named_parameters() if p.grad is not None}
+        grads['xyz1'] = x1.grad
+        if isinstance(pred, list):
+            grads['xyz2'] = x2.grad
+        z = {'loss': np.float64(float(loss.detach()))}
+        for k, g in grads.items():
+            z['s/' + k] = grad_sketch(k, g)
+        if isinstance(pred, list):
+            with torch.no_grad():
+                fmap1, g1 = model.feature_extractor(pc1)
+                fmap2, g2 = model.feature_extractor(pc2)
+                corr = model.corr_block.calculate_corr(fmap1, fmap2)
+                top = torch.topk(corr, k=model.corr_block.truncate_k, dim=2, sorted=True).indices
+            z.update(nbr1=local_adjacency(g1, b, n), nbr2=local_adjacency(g2, b, n),
+                     topk=np.sort(top.numpy(), -1).astype(np.int16))
+        out.append(z)
+    return out
+
+
 def main():
     if not REF or not os.path.isdir(REF):
         sys.exit('set PVRAFT_REFERENCE to the reference tree (weiyithu/PV-RAFT)')
@@ -132,6 +204,17 @@ def main():
     small.update(tr)
     small.update(np_state(model.state_dict()))
     np.savez_compressed(os.path.join(HERE, 'small_rsf_refine.npz'), **small)
+
+    # ---- fixtures 6 and 7: float64 reference gradients with fixture 1's weights and clouds ----
+    sd = {k: v.double() for k, v in model.state_dict().items()}
+    rsf = RSF(args).double()
+    rsf.load_state_dict({k: v for k, v in sd.items() if not k.startswith('refine_block.')})
+    ref64 = RSF_refine(args).double()
+    ref64.load_state_dict(sd)
+    g_rsf, g_refine = reference_gradients(rsf, ref64, pc1.double(), pc2.double(), 3)
+    assert len([k for k in g_rsf if k.startswith('s/')]) == 95 + 2 and len([k for k in g_refine if k.startswith('s/')]) == 29 + 1
+    np.savez_compressed(os.path.join(HERE, 'ref_grads_rsf.npz'), **g_rsf)
+    np.savez_compressed(os.path.join(HERE, 'ref_grads_refine.npz'), **g_refine)
 
     # ---- fixture 2: default-init RSF, N=1024, K=512, 4 iters; outputs only -----------------
     args = types.SimpleNamespace(corr_levels=3, base_scales=0.25, truncate_k=512)
