@@ -745,58 +745,7 @@ PVRAFT_API int pvraft_flow_propagate_fwd(const float* xyz_prev, const float* flo
 PVRAFT_API int pvraft_flow_propagate_grid_fwd(const float* xyz_prev, const float* flow_prev, const float* xyz, int B, int M, int N, int k,
                                               float* flow_out, int32_t* idx_out, void* workspace, void* stream);
 
-/* A robust rigid fit of a flow (the sensor's ego-motion; no counterpart in the reference): RANSAC over minimal samples and a
- * Horn/Kabsch refit, such that xyz1 R^T + t ~ xyz1 + flow on the inliers.  y = x + f is formed in fp32 (one rounded add per
- * coordinate) wherever it appears.  No host synchronisation; every output element is written.
- *   Sampling: hypothesis h < H draws r = 0, 1, 2: j_r = splitmix64((seed << 32) | (h << 2) | r) mod n_allowed, an index into
- *       the sample's ascending list of allowed points (mask[b,i] != 0; all N points with mask NULL), where splitmix64(k) =
- *       mix(k + 0x9e3779b97f4a7c15), mix(z) = z3 ^ (z3 >> 31), z2 = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9,
- *       z3 = (z2 ^ (z2 >> 27)) * 0x94d049bb133111eb (uint64 arithmetic).  The key leaves out the sample index: a batched
- *       call equals per-sample calls.  The triple is REJECTED (never redrawn) when n_allowed = 0, two j_r are equal, it is
- *       near-collinear: NOT |a x b|^2 > 1e-6 |a|^2 |b|^2 (a = x1 - x0, b = x2 - x0; coincident points are rejected too), or
- *       one of its pairwise distances (0-1, 0-2, 1-2) changes by more than 2 threshold: NOT | ||x_i - x_j|| - ||y_i - y_j|| |
- *       <= 2 threshold.  Both tests in double on the fp32 coordinates, each operation rounded to nearest, none contracted
- *       (|u|^2 = (u0 u0 + u1 u1) + u2 u2, cross products as a1 b2 - a2 b1, ...).
- *   Minimal fit: Horn's closed form about the triple's centroids (c_x, c_y): the eigenvector of the largest eigenvalue of
- *       the 4x4 N(S), S = sum (x - c_x)(y - c_y)^T, by cyclic Jacobi sweeps in double; a proper rotation always.  The model
- *       (R, c_x, c_y) is stored in fp32.
- *   Score: count of allowed points with ||r||^2 <= threshold^2 (fp32 threshold * threshold), r = R (x - c_x) - (y - c_y),
- *       in fp32: d = x - c_x, e = y - c_y, r_k = ((R_k0 d_0 + R_k1 d_1) + R_k2 d_2) - e_k, ||r||^2 = (r_0^2 + r_1^2) + r_2^2,
- *       each operation rounded to nearest, none contracted.  Integer counts; the best hypothesis has the most inliers, the
- *       lowest h on ties.
- *   Refit, `rounds` times: the inliers are the allowed points within the threshold (the same test) of the current model --
- *       the best hypothesis, then the previous round's (R, x-bar, y-bar) -- and get the unweighted Horn fit from their
- *       moments (n, sum dx, sum dy, sum dx dy^T) in double about the current model's (c_x, c_y); x-bar = c_x + sum dx / n,
- *       t = y-bar - R x-bar.  The last round's inliers are inliers_out.
- *   Degenerate: n < 3, or lambda0 - lambda1 <= 1e-5 lambda0 (the top two eigenvalues of N(S): collinear or coincident
- *       inliers): R = I, t = y-bar - x-bar (0 with no inlier), degenerate = 1.  A sample none of whose hypotheses is accepted
- *       takes every allowed point as an inlier in every round and is degenerate.
- *   pvraft_rigid_motion_fwd: xyz1, flow [B,N,3], mask [B,N] uint8 or NULL -> R [B,3,3] and t [B,3] fp32, inliers [B,N] uint8,
- *       count [B] int32, degenerate [B] uint8, state [B,32] double (pvraft_rigid_motion_bwd's input: eigenvectors at [4j, 4j+4),
- *       eigenvalues [16, 20) (the top first), x-bar [20, 23), y-bar [23, 26), n, degenerate); optional (NULL to skip):
- *       triples [B,H,3] int32, the drawn point indices (-1 with no allowed point), hyp_count [B,H] int32, the counts (-1 for
- *       a rejected triple).  workspace: pvraft_rigid_motion_workspace_bytes(B, N, H, rounds) bytes, 16-byte aligned, no
- *       initialisation needed; det_workspace: pvraft_rigid_motion_fwd_det_workspace_bytes(B, rounds) bytes or NULL
- *       ("Deterministic mode": the moments in fixed point, so R and t are the same bits from run to run).  The counts,
- *       the selection and the inlier sets are integer decisions and do not depend on the mode except through R and t.
- *   pvraft_rigid_motion_bwd: dR [B,3,3], dt [B,3] the DEVICE upstream gradients, the forward's inliers and state, the
- *       inlier set held fixed -> d_xyz1, d_flow [B,N,3], every element WRITTEN once (zero off the inliers): dt gives
- *       d y-bar += dt, d x-bar -= R^T dt, dR -= dt x-bar^T; dR -> dq through R(q); dq -> dN = sym(sum_{j>=1} v_j v_j^T dq
- *       v_0^T / (lambda0 - lambda_j)); dN -> dS; per inlier dx_i = dS (y_i - y-bar) + d x-bar / n, dy_i = dS^T (x_i - x-bar)
- *       + d y-bar / n; d_flow = dy, d_xyz1 = dx + dy.  Degenerate samples propagate the translation only.  No atomics: the
- *       result is bitwise reproducible as it is.
- * Null required pointers, B < 1, N < 3, B N >= 2^31, H outside 1..4096, rounds outside 1..8, a threshold that is not
- * finite and > 0, and seed < 0 return PVRAFT_ERR_BAD_ARG before any launch; B > 65535 PVRAFT_ERR_UNSUPPORTED. */
-PVRAFT_API int pvraft_rigid_motion_fwd(const float* xyz1, const float* flow, const uint8_t* mask, int B, int N, float threshold, int H,
-                                       int rounds, int seed, float* R, float* t, uint8_t* inliers, int32_t* count, uint8_t* degenerate,
-                                       double* state, int32_t* triples, int32_t* hyp_count, void* workspace, void* det_workspace,
-                                       void* stream);
-PVRAFT_API int64_t pvraft_rigid_motion_workspace_bytes(int B, int N, int H, int rounds);
-PVRAFT_API int64_t pvraft_rigid_motion_fwd_det_workspace_bytes(int B, int rounds);
-PVRAFT_API int pvraft_rigid_motion_bwd(const float* xyz1, const float* flow, const uint8_t* inliers, const double* state, const float* dR,
-                                       const float* dt, int B, int N, float* d_xyz1, float* d_flow, void* stream);
-
-/* Euclidean clustering (single linkage; no counterpart in the reference), the objects of pvraft_rigid_objects_fwd.  Integer
+/* Euclidean clustering (single linkage; no counterpart in the reference), the segments of pvraft_rigid_objects_fwd.  Integer
  * decisions only: the outputs are the same bits in every mode and from run to run, so there is no det_workspace.
  *   Edges: points i != j of one sample are adjacent when both take part -- mask[b,i] != 0 (every point with mask NULL) and
  *       all three coordinates finite -- and diff_sq(x_i, x_j) <= fl(radius * radius), diff_sq the fp32 difference form of
@@ -818,26 +767,62 @@ PVRAFT_API int pvraft_euclidean_clusters_fwd(const float* xyz, const float* flow
                                              int32_t* sizes, void* workspace, void* stream);
 PVRAFT_API int64_t pvraft_euclidean_clusters_workspace_bytes(int B, int N);
 
-/* One rigid fit per object (no counterpart in the reference): labels [B,N] int32 (as pvraft_euclidean_clusters_fwd writes
- * them; a value outside 0 .. O - 1 is no object), O objects per sample.  Object o of sample b is fitted exactly as
- * pvraft_rigid_motion_fwd fits sample 0 of xyz1[b], flow[b] with mask = (labels[b] == o), B = 1 and the same threshold, H,
- * rounds and seed: the sampler over the object's ascending member list, the rejection, the scoring, the selection, the
- * refits and the degenerate rule.  In the deterministic mode every window of 256 point ids adds the same partial moments as
- * that call does, into fixed point, so R, t, count, degenerate, state and the inliers are the same bits; otherwise they
- * agree to the rounding of the double moment sums.  An object with no member gets R = I, t = 0, count 0, degenerate 1.
- * The scoring takes (members) x H residual tests, not O N H.
- *   pvraft_rigid_objects_fwd: -> R [B,O,3,3], t [B,O,3] fp32, inliers [B,N] uint8 (an inlier of its own object's fit), count
- *       [B,O] int32, degenerate [B,O] uint8, state [B,O,32] double (the layout of pvraft_rigid_motion_fwd's).  workspace:
+/* A robust rigid fit of a flow (no counterpart in the reference): RANSAC over minimal samples and a Horn/Kabsch refit, such
+ * that xyz1 R^T + t ~ xyz1 + flow on the inliers, once per SEGMENT.  Sample b has O segments: segment (b, o) is the points
+ * with labels[b,i] == o (a value outside 0 .. O - 1 is in no segment); with labels NULL (only with O = 1) segment (b, 0) is
+ * every point of the sample.  pvraft_b200.rigid_motion, the sensor's ego-motion, is O = 1 (labels[b,i] = 0 where its mask
+ * allows the point, -1 elsewhere, or NULL without a mask); pvraft_b200.rigid_objects one segment per object, with the labels
+ * pvraft_euclidean_clusters_fwd writes.  Every segment is fitted as the same call with B = 1, O = 1 and labels =
+ * (labels[b] == o ? 0 : -1) fits it: below, "allowed" means a member of the segment.  y = x + f is formed in fp32 (one
+ * rounded add per coordinate) wherever it appears.  No host synchronisation; every output element is written.
+ *   Sampling: hypothesis h < H draws r = 0, 1, 2: j_r = splitmix64((seed << 32) | (h << 2) | r) mod n_allowed, an index into
+ *       the segment's ascending list of allowed points, where splitmix64(k) = mix(k + 0x9e3779b97f4a7c15), mix(z) = z3 ^
+ *       (z3 >> 31), z2 = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9, z3 = (z2 ^ (z2 >> 27)) * 0x94d049bb133111eb (uint64
+ *       arithmetic).  The key leaves out the sample and the segment index: a batched call equals per-sample calls.  The
+ *       triple is REJECTED (never redrawn) when n_allowed = 0, two j_r are equal, it is near-collinear: NOT |a x b|^2 >
+ *       1e-6 |a|^2 |b|^2 (a = x1 - x0, b = x2 - x0; coincident points are rejected too), or one of its pairwise distances
+ *       (0-1, 0-2, 1-2) changes by more than 2 threshold: NOT | ||x_i - x_j|| - ||y_i - y_j|| | <= 2 threshold.  Both tests
+ *       in double on the fp32 coordinates, each operation rounded to nearest, none contracted (|u|^2 = (u0 u0 + u1 u1) +
+ *       u2 u2, cross products as a1 b2 - a2 b1, ...).
+ *   Minimal fit: Horn's closed form about the triple's centroids (c_x, c_y): the eigenvector of the largest eigenvalue of
+ *       the 4x4 N(S), S = sum (x - c_x)(y - c_y)^T, by cyclic Jacobi sweeps in double; a proper rotation always.  The model
+ *       (R, c_x, c_y) is stored in fp32.
+ *   Score: count of allowed points with ||r||^2 <= threshold^2 (fp32 threshold * threshold), r = R (x - c_x) - (y - c_y),
+ *       in fp32: d = x - c_x, e = y - c_y, r_k = ((R_k0 d_0 + R_k1 d_1) + R_k2 d_2) - e_k, ||r||^2 = (r_0^2 + r_1^2) + r_2^2,
+ *       each operation rounded to nearest, none contracted.  Integer counts; the best hypothesis has the most inliers, the
+ *       lowest h on ties.  The scoring takes (allowed points) x H residual tests, not O N H.
+ *   Refit, `rounds` times: the inliers are the allowed points within the threshold (the same test) of the current model --
+ *       the best hypothesis, then the previous round's (R, x-bar, y-bar) -- and get the unweighted Horn fit from their
+ *       moments (n, sum dx, sum dy, sum dx dy^T) in double about the current model's (c_x, c_y); x-bar = c_x + sum dx / n,
+ *       t = y-bar - R x-bar.  The last round's inliers are inliers_out.  The moments are summed per window of 256 point ids
+ *       and the windows' partial sums added, so in the deterministic mode a segment's R, t, count, degenerate, state and
+ *       inliers are the same bits as those of its B = 1, O = 1 call.
+ *   Degenerate: n < 3, or lambda0 - lambda1 <= 1e-5 lambda0 (the top two eigenvalues of N(S): collinear or coincident
+ *       inliers): R = I, t = y-bar - x-bar (0 with no inlier), degenerate = 1.  A segment none of whose hypotheses is
+ *       accepted takes every allowed point as an inlier in every round and is degenerate; a segment with no member gets
+ *       R = I, t = 0, count 0, degenerate 1.
+ *   pvraft_rigid_objects_fwd: xyz1, flow [B,N,3], labels [B,N] int32 or NULL (O = 1) -> R [B,O,3,3] and t [B,O,3] fp32,
+ *       inliers [B,N] uint8 (an inlier of its own segment's fit), count [B,O] int32, degenerate [B,O] uint8, state [B,O,32]
+ *       double (pvraft_rigid_objects_bwd's input: eigenvectors at [4j, 4j+4), eigenvalues [16, 20) (the top first), x-bar
+ *       [20, 23), y-bar [23, 26), n, degenerate); optional (NULL to skip): triples [B O,H,3] int32, the drawn point indices
+ *       (-1 with no allowed point), hyp_count [B O,H] int32, the counts (-1 for a rejected triple).  workspace:
  *       pvraft_rigid_objects_workspace_bytes(B, N, O, H, rounds) bytes, 16-byte aligned, no initialisation needed;
- *       det_workspace: pvraft_rigid_objects_fwd_det_workspace_bytes(B, O, rounds) bytes or NULL.
- *   pvraft_rigid_objects_bwd: dR [B,O,3,3], dt [B,O,3] on the device, the forward's labels, inliers and state -> d_xyz1,
- *       d_flow [B,N,3]: pvraft_rigid_motion_bwd's formula per object, the inlier sets held fixed; a point belongs to at most
- *       one object, so every element is WRITTEN once (zero off the inliers), with no atomics.
- * Null required pointers, B < 1, N < 1, B N >= 2^31, O outside 1..256, H outside 1..4096, rounds outside 1..8, a threshold
- * that is not finite and > 0, and seed < 0 return PVRAFT_ERR_BAD_ARG before any launch; B O > 65535 PVRAFT_ERR_UNSUPPORTED. */
+ *       det_workspace: pvraft_rigid_objects_fwd_det_workspace_bytes(B, O, rounds) bytes or NULL ("Deterministic mode": the
+ *       moments in fixed point, so R and t are the same bits from run to run).  The counts, the selection and the inlier
+ *       sets are integer decisions and do not depend on the mode except through R and t.
+ *   pvraft_rigid_objects_bwd: dR [B,O,3,3], dt [B,O,3] the DEVICE upstream gradients, the forward's labels, inliers and
+ *       state, the inlier sets held fixed -> d_xyz1, d_flow [B,N,3], every element WRITTEN once (zero off the inliers): dt
+ *       gives d y-bar += dt, d x-bar -= R^T dt, dR -= dt x-bar^T; dR -> dq through R(q); dq -> dN = sym(sum_{j>=1} v_j v_j^T
+ *       dq v0^T / (lambda0 - lambda_j)); dN -> dS; per inlier dx_i = dS (y_i - y-bar) + d x-bar / n, dy_i = dS^T (x_i -
+ *       x-bar) + d y-bar / n; d_flow = dy, d_xyz1 = dx + dy.  Degenerate segments propagate the translation only.  A point
+ *       belongs to at most one segment, so there are no atomics: the result is bitwise reproducible as it is.
+ * Null required pointers, labels NULL with O != 1, B < 1, N < 1, B N >= 2^31, O outside 1..256, H outside 1..4096, rounds
+ * outside 1..8, a threshold that is not finite and > 0, and seed < 0 return PVRAFT_ERR_BAD_ARG before any launch; B O > 65535
+ * PVRAFT_ERR_UNSUPPORTED. */
 PVRAFT_API int pvraft_rigid_objects_fwd(const float* xyz1, const float* flow, const int32_t* labels, int B, int N, int O, float threshold,
                                         int H, int rounds, int seed, float* R, float* t, uint8_t* inliers, int32_t* count,
-                                        uint8_t* degenerate, double* state, void* workspace, void* det_workspace, void* stream);
+                                        uint8_t* degenerate, double* state, int32_t* triples, int32_t* hyp_count, void* workspace,
+                                        void* det_workspace, void* stream);
 PVRAFT_API int64_t pvraft_rigid_objects_workspace_bytes(int B, int N, int O, int H, int rounds);
 PVRAFT_API int64_t pvraft_rigid_objects_fwd_det_workspace_bytes(int B, int O, int rounds);
 PVRAFT_API int pvraft_rigid_objects_bwd(const float* xyz1, const float* flow, const int32_t* labels, const uint8_t* inliers,

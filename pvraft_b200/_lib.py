@@ -168,16 +168,11 @@ _SIGNATURES = {
     'pvraft_flow_consistency_bwd': (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP,
                                               VP]),
     'pvraft_flow_consistency_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
-    'pvraft_rigid_motion_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP, VP,
-                                          VP, VP, VP, VP]),
-    'pvraft_rigid_motion_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
-    'pvraft_rigid_motion_fwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_rigid_motion_bwd': (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, VP, VP, VP]),
     'pvraft_euclidean_clusters_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int, VP, VP, VP, VP,
                                                 VP]),
     'pvraft_euclidean_clusters_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
     'pvraft_rigid_objects_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP,
-                                           VP, VP, VP, VP, VP]),
+                                           VP, VP, VP, VP, VP, VP, VP]),
     'pvraft_rigid_objects_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     'pvraft_rigid_objects_fwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
     'pvraft_rigid_objects_bwd': (C.c_int, [VP, VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),

@@ -3,24 +3,26 @@
 // per coordinate) everywhere below.
 //
 //   sampling   hypothesis h draws r = 0, 1, 2: j_r = splitmix64((seed << 32) | (h << 2) | r) mod n_allowed, an index into the
-//              sample's ascending list of allowed points (k_rigid_allowed; the identity without a mask).  The key leaves out
-//              the sample, so a sample's result does not depend on the rest of the batch.  A triple is rejected, never
+//              segment's ascending member list (the identity without labels).  The key leaves out the sample and the
+//              segment, so a segment's result does not depend on the rest of the batch.  A triple is rejected, never
 //              redrawn (triple_rejected, in double, every operation rounded and none contracted).
 //   minimal    Horn's closed form about the triple's own centroids (horn_fit: the top eigenvector of the 4x4 N(S) by cyclic
 //              Jacobi sweeps in double), stored as (R, c_x, c_y) in fp32; the residual is R (x - c_x) - (y - c_y) (residual2).
-//   score      k_rigid_score: every (hypothesis, allowed point) pair, ||residual||^2 <= threshold^2 in fp32, counted with
+//   score      k_rigid_score: every (hypothesis, member) pair, ||residual||^2 <= threshold^2 in fp32, counted with
 //              ballots into integers, so the counts and the selection (k_rigid_select: most inliers, lowest h on ties) are
 //              the same bits in any mode.
 //   refit      `rounds` times: k_rigid_moments takes (count, sum dx, sum dy, sum dx dy^T) in double about the current
-//              model's (c_x, c_y) over the allowed points within the threshold of it (DET: fixed-point slots), and
-//              k_rigid_solve (one thread per sample) runs the same Horn solve; its (R, x-bar, y-bar) is the next round's model.
+//              model's (c_x, c_y) over the members within the threshold of it (DET: fixed-point slots), and
+//              k_rigid_solve (one thread per segment) runs the same Horn solve; its (R, x-bar, y-bar) is the next round's model.
 //   degenerate count < 3, or an eigen-gap lambda0 - lambda1 <= kGapTol lambda0: R = I, t = y-bar - x-bar.  A sample none of
 //              whose hypotheses is accepted takes every allowed point as its inliers in every round and is degenerate.
 //
-// The kernels fit SEGMENTS (RmSegs): rigid_motion is one segment per sample; rigid_objects (the end of this file) one per
-// (sample, object), each fitted exactly as rigid_motion fits that sample with mask = (labels == object).
+// A fit is O SEGMENTS per sample: segment (b, o) is the points with labels[b, i] == o, or, with labels NULL (O = 1), every
+// point of the sample.  rigid_motion is O = 1 (labels = where(mask, 0, -1), or NULL without a mask), rigid_objects one
+// segment per object.  The grouping (k_rigid_allowed for O = 1, k_ro_group_* otherwise) gives both the same RmSegs, and
+// every kernel after it has one form.
 //
-// Backward (k_rigid_bwd, one thread per point, each gradient written once): the inlier set held fixed, from the per-sample
+// Backward (k_rigid_bwd, one thread per point, each gradient written once): the inlier set held fixed, from the per-segment
 // double state the forward saves (eigenvectors, eigenvalues, centroids, count):
 //   dt -> d y-bar += dt, d x-bar -= R^T dt, dR -= dt x-bar^T;  dR -> dq through R(q);  dq -> dN = sym(sum_{j>=1} v_j v_j^T dq
 //   v_0^T / (lambda0 - lambda_j));  dN -> dS;  dx_i = dS (y_i - y-bar) + d x-bar / n, dy_i = dS^T (x_i - x-bar) + d y-bar / n.
@@ -28,7 +30,7 @@
 
 namespace pvraft {
 
-constexpr int kRmState = 32;          // doubles per sample in the saved state
+constexpr int kRmState = 32;          // doubles per segment in the saved state
 constexpr int kRmModel = 16;          // floats per model: R (9, row-major), c_x (3), c_y (3), flag
 constexpr int kRmMoments = 16;        // n, sum dx (3), sum dy (3), sum dx dy^T (9, row-major)
 constexpr int kRmMaxH = 4096;
@@ -183,20 +185,20 @@ __device__ __forceinline__ bool triple_rejected(const double (&x)[3][3], const d
     return false;
 }
 
-// The allowed points of each sample in ascending order: allowed [B,N] (the first nallow[s] entries of row s), one CTA of
-// kRmScan threads per sample
+// The O = 1 grouping: the members (labels == 0) of each sample in ascending order -> list [B,N] (the first n[s] entries of
+// row s), one CTA of kRmScan threads per sample
 constexpr int kRmScan = 1024;
-__global__ void __launch_bounds__(kRmScan) k_rigid_allowed(const uint8_t* __restrict__ mask, int N, int32_t* __restrict__ allowed,
-                                                           int32_t* __restrict__ nallow) {
+__global__ void __launch_bounds__(kRmScan) k_rigid_allowed(const int32_t* __restrict__ labels, int N, int32_t* __restrict__ list,
+                                                           int32_t* __restrict__ nmem) {
     __shared__ int warp_tot[kRmScan / kWarp];
     __shared__ int base_sh;
     const int s = blockIdx.x, lane = lane_id(), wid = warp_id();
-    const uint8_t* m = mask + (long long)s * N;
-    int32_t* out = allowed + (long long)s * N;
+    const int32_t* l = labels + (long long)s * N;
+    int32_t* out = list + (long long)s * N;
     if (threadIdx.x == 0) base_sh = 0;
     for (int c0 = 0; c0 < N; c0 += kRmScan) {
         const int i = c0 + threadIdx.x;
-        const bool on = i < N && m[i] != 0;
+        const bool on = i < N && l[i] == 0;
         const unsigned bal = __ballot_sync(kFull, on);
         __syncthreads();   // base_sh of the previous chunk is final; warp_tot free
         if (lane == 0) warp_tot[wid] = __popc(bal);
@@ -212,13 +214,12 @@ __global__ void __launch_bounds__(kRmScan) k_rigid_allowed(const uint8_t* __rest
         }
     }
     __syncthreads();
-    if (threadIdx.x == 0) nallow[s] = base_sh;
+    if (threadIdx.x == 0) nmem[s] = base_sh;
 }
 
-// The point sets one launch fits, one per SEGMENT: segment g is a subset of sample g / per, and its members, ascending, are
-// list[first(g), first(g) + count(g)), first(g) = start[g] (g N with start NULL) -- or, with list NULL, all N points of the
-// sample.  rigid_motion: one segment per sample (per = 1), list = the allowed list (k_rigid_allowed) or NULL without a mask;
-// rigid_objects: per = max_objects segments per sample, one per object, from the stable grouping of k_ro_group_*.
+// The segments of one fit: segment g is a subset of sample g / per, and its members, ascending, are list[first(g), first(g) +
+// count(g)), first(g) = start[g] (g N with start NULL: k_rigid_allowed) -- or, with list NULL (no labels), all N points of
+// the sample.
 struct RmSegs {
     const int32_t* list;    // [B,N] member ids, or NULL
     const int32_t* start;   // [G] offset of each segment's members in list, or NULL
@@ -295,16 +296,16 @@ __global__ void __launch_bounds__(128) k_rigid_hypotheses(const float* __restric
 }
 
 // Inlier counts of every (hypothesis, member) pair.  A CTA holds kScHyp hypotheses in shared memory (read as broadcasts) and
-// kScPer points per thread in registers; per hypothesis and warp a ballot and a popcount, lane j of each warp keeps
-// hypothesis j's count, then one shared and one global integer atomic.  Without `items` (one segment per sample, list NULL):
-// grid (ceil(N / kScPoints), ceil(H / kScHyp), B), CTA x takes points [x kScPoints, (x + 1) kScPoints) that pass the mask.
-// With items [B,stride] (nitems [B] of them per sample): grid (stride, ceil(H / kScHyp), B), CTA x takes item x = (j << 8) | o
-// -- members [j kScPoints, (j + 1) kScPoints) of segment (sample, o) -- so the work is the members' number times H.
+// kScPer members per thread in registers; per hypothesis and warp a ballot and a popcount, lane j of each warp keeps
+// hypothesis j's count, then one shared and one global integer atomic.  Without `items` (one segment per sample): grid
+// (ceil(N / kScPoints), ceil(H / kScHyp), B), CTA x takes members [x kScPoints, (x + 1) kScPoints) of segment s.  With items
+// [B,stride] (nitems [B] of them per sample): grid (stride, ceil(H / kScHyp), B), CTA x takes item x = (j << 8) | o --
+// members [j kScPoints, (j + 1) kScPoints) of segment (sample, o) -- so the work is the members' number times H.
 constexpr int kScThreads = 256, kScPer = 4, kScPoints = kScThreads * kScPer, kScHyp = 32;
-__global__ void __launch_bounds__(kScThreads) k_rigid_score(const float* __restrict__ x, const float* __restrict__ f,
-                                                            const uint8_t* __restrict__ mask, RmSegs sg, const int32_t* __restrict__ items,
-                                                            const int32_t* __restrict__ nitems, int stride, int H, float thr2,
-                                                            const float* __restrict__ hyp, int32_t* __restrict__ hcnt) {
+__global__ void __launch_bounds__(kScThreads) k_rigid_score(const float* __restrict__ x, const float* __restrict__ f, RmSegs sg,
+                                                            const int32_t* __restrict__ items, const int32_t* __restrict__ nitems,
+                                                            int stride, int H, float thr2, const float* __restrict__ hyp,
+                                                            int32_t* __restrict__ hcnt) {
     __shared__ float sh[kScHyp][kRmModel];
     __shared__ int cnt[kScHyp];
     const int s = blockIdx.z, h0 = blockIdx.y * kScHyp, lane = lane_id(), N = sg.N;
@@ -316,6 +317,7 @@ __global__ void __launch_bounds__(kScThreads) k_rigid_score(const float* __restr
         base = (w >> 8) * kScPoints;
     }
     const int n_g = sg.count(g);
+    if (base >= n_g) return;   // no member left: uniform over the CTA
     for (int i = threadIdx.x; i < kScHyp * kRmModel; i += kScThreads) {
         const int hh = h0 + i / kRmModel;
         sh[i / kRmModel][i % kRmModel] = hh < H ? __ldg(hyp + ((long long)g * H + h0) * kRmModel + i) : 0.f;
@@ -327,7 +329,7 @@ __global__ void __launch_bounds__(kScThreads) k_rigid_score(const float* __restr
     for (int k = 0; k < kScPer; ++k) {
         const int j = base + k * kScThreads + threadIdx.x;
         const int i = j < n_g ? sg.member(g, j) : 0;
-        ok[k] = j < n_g && (!mask || mask[(long long)s * N + i] != 0);
+        ok[k] = j < n_g;
         const long long o = ((long long)s * N + i) * 3;
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
@@ -399,17 +401,18 @@ __global__ void __launch_bounds__(kSelThreads) k_rigid_select(const float* __res
 // when it is a member and (flag 0, or residual2 under g's model <= thr2); (1, dx, dy, dx dy^T) with dx = x - c_x, dy = y - c_y
 // in double summed per warp (xor butterfly), then over the CTA's warps in order, and added once per (window, segment) into
 // acc [G,kRmMoments] (DET: fixed-point slots).  Without `items` (one segment per sample): grid (ceil(N / kMomThreads), B),
-// membership the mask, inliers [B,N] written for every point.  With items [B,N] (nitems [B] per sample; item (c << 8) | o:
-// the window c of point ids [c kMomThreads, (c + 1) kMomThreads), of segment (sample, o), membership labels == o): grid
-// (any, B), each CTA taking items x, x + gridDim.x, ...; inliers written for members only.  A window's partial sum is the
-// same value either way, so in the DET form a segment's moments are those of the one-segment launch with mask = (labels == o).
+// membership labels == 0 (every point with labels NULL), inliers [B,N] written for every point.  With items [B,N] (nitems
+// [B] per sample; item (c << 8) | o: the window c of point ids [c kMomThreads, (c + 1) kMomThreads), of segment (sample, o),
+// membership labels == o): grid (any, B), each CTA taking items x, x + gridDim.x, ...; inliers written for members only.
+// A window's partial sum is the same value either way, so in the DET form a segment's moments are those of the one-segment
+// launch with labels = where(labels == o, 0, -1).
 constexpr int kMomThreads = 256;
 template <bool DET>
 __global__ void __launch_bounds__(kMomThreads) k_rigid_moments(const float* __restrict__ x, const float* __restrict__ f,
-                                                               const uint8_t* __restrict__ mask, const int32_t* __restrict__ labels,
-                                                               const int32_t* __restrict__ items, const int32_t* __restrict__ nitems,
-                                                               int per, int N, float thr2, const float* __restrict__ model,
-                                                               uint8_t* __restrict__ inliers, Acc<DET, double> acc) {
+                                                               const int32_t* __restrict__ labels, const int32_t* __restrict__ items,
+                                                               const int32_t* __restrict__ nitems, int per, int N, float thr2,
+                                                               const float* __restrict__ model, uint8_t* __restrict__ inliers,
+                                                               Acc<DET, double> acc) {
     __shared__ double part[kMomThreads / kWarp][kRmMoments];
     const int s = blockIdx.y;
     const int n_items = items ? nitems[s] : 1;
@@ -428,7 +431,7 @@ __global__ void __launch_bounds__(kMomThreads) k_rigid_moments(const float* __re
         for (int k = 0; k < kRmMoments; ++k) v[k] = 0.0;
         if (i < N) {
             const long long p = (long long)s * N + i;
-            const bool member = items ? labels[p] == o : (!mask || mask[p] != 0);
+            const bool member = !labels || labels[p] == o;
             const float x0 = __ldg(x + 3 * p), x1 = __ldg(x + 3 * p + 1), x2 = __ldg(x + 3 * p + 2);
             const float y0 = __fadd_rn(x0, __ldg(f + 3 * p)), y1 = __fadd_rn(x1, __ldg(f + 3 * p + 1)), y2 = __fadd_rn(x2, __ldg(f + 3 * p + 2));
             const bool in = member && (m[15] == 0.f || residual2(m, x0, x1, x2, y0, y1, y2) <= thr2);
@@ -463,8 +466,8 @@ __global__ void __launch_bounds__(kMomThreads) k_rigid_moments(const float* __re
     }
 }
 
-// One thread per sample: the Horn solve of one round's moments -> R [B,3,3], t [B,3], count [B], degenerate [B], state
-// [B,kRmState] and the next round's model.  DET: the moments are read from the fixed-point slots.
+// One thread per segment: the Horn solve of one round's moments -> R [G,3,3], t [G,3], count [G], degenerate [G], state
+// [G,kRmState] and the next round's model.  DET: the moments are read from the fixed-point slots.
 template <bool DET>
 __global__ void __launch_bounds__(64) k_rigid_solve(const double* __restrict__ mom, FxSlots slots, int B, float* __restrict__ model,
                                                     float* __restrict__ Rout, float* __restrict__ tout, int32_t* __restrict__ count,
@@ -533,7 +536,7 @@ __global__ void __launch_bounds__(64) k_rigid_solve(const double* __restrict__ m
 }
 
 // One thread per point: d_xyz1 and d_flow [B,N,3], every element written once (zero off the inliers).  The point's segment:
-// its sample (labels NULL), or (sample, labels[p]) with `per` segments per sample; the state, dR and dt are per segment.
+// (sample, labels[p]) with `per` segments per sample, or its sample with labels NULL; the state, dR and dt are per segment.
 __global__ void __launch_bounds__(256) k_rigid_bwd(const float* __restrict__ x, const float* __restrict__ f,
                                                    const uint8_t* __restrict__ inliers, const int32_t* __restrict__ labels, int per,
                                                    const double* __restrict__ state, const float* __restrict__ dR,
@@ -622,112 +625,9 @@ __global__ void __launch_bounds__(256) k_rigid_bwd(const float* __restrict__ x, 
     }
 }
 
-// the forward's workspace: allowed [B,N] i32 | nallow [B] i32 | hyp [B,H,16] f32 | hcnt [B,H] i32 | model [B,16] f32 |
-// mom [rounds,B,16] f64, each range 16-byte aligned
-struct RigidWs {
-    int32_t* allowed;
-    int32_t* nallow;
-    float* hyp;
-    int32_t* hcnt;
-    float* model;
-    double* mom;
-    int64_t bytes;
-};
-static RigidWs rigid_ws(void* ws, int B, int N, int H, int rounds) {
-    char* base = static_cast<char*>(ws);
-    int64_t off = 0;
-    auto take = [&](int64_t bytes) {
-        char* p = base ? base + off : nullptr;
-        off += (bytes + 15) / 16 * 16;
-        return p;
-    };
-    RigidWs L;
-    L.allowed = reinterpret_cast<int32_t*>(take(4ll * B * N));
-    L.nallow = reinterpret_cast<int32_t*>(take(4ll * B));
-    L.hyp = reinterpret_cast<float*>(take(4ll * B * H * kRmModel));
-    L.hcnt = reinterpret_cast<int32_t*>(take(4ll * B * H));
-    L.model = reinterpret_cast<float*>(take(4ll * B * kRmModel));
-    L.mom = reinterpret_cast<double*>(take(8ll * rounds * B * kRmMoments));
-    L.bytes = off;
-    return L;
-}
-
-// The `rounds` refits of G = B per segments: moments over mgrid, then the Horn solve of every segment
-static int rigid_refits(const float* xyz1, const float* flow, const uint8_t* mask, const int32_t* labels, const int32_t* items,
-                        const int32_t* nitems, int per, int B, int N, int rounds, float thr2, dim3 mgrid, float* model, double* mom0,
-                        float* R, float* t, uint8_t* inliers, int32_t* count, uint8_t* degenerate, double* state, void* det_workspace,
-                        cudaStream_t st, const char* what) {
-    const int G = B * per;
-    const unsigned sblocks = (unsigned)((G + 63) / 64);
-    for (int r = 0; r < rounds; ++r) {
-        double* mom = mom0 + (long long)r * G * kRmMoments;
-        if (det_workspace) {
-            const FxSlots slots = fx_slots(det_workspace) + (long long)r * G * kRmMoments;
-            k_rigid_moments<true><<<mgrid, kMomThreads, 0, st>>>(xyz1, flow, mask, labels, items, nitems, per, N, thr2, model, inliers, slots);
-            k_rigid_solve<true><<<sblocks, 64, 0, st>>>(mom, slots, G, model, R, t, count, degenerate, state);
-        } else {
-            k_rigid_moments<false><<<mgrid, kMomThreads, 0, st>>>(xyz1, flow, mask, labels, items, nitems, per, N, thr2, model, inliers, mom);
-            k_rigid_solve<false><<<sblocks, 64, 0, st>>>(mom, FxSlots{}, G, model, R, t, count, degenerate, state);
-        }
-    }
-    return check_launch(what);
-}
-
-static bool bad_sizes(int B, int N, int H, int rounds) {
-    return B < 1 || N < 3 || H < 1 || H > kRmMaxH || rounds < 1 || rounds > kRmMaxRounds || (long long)B * N > 0x7fffffffll;
-}
-
-}  // namespace pvraft
-
-using namespace pvraft;
-
-extern "C" int64_t pvraft_rigid_motion_workspace_bytes(int B, int N, int H, int rounds) {
-    return bad_sizes(B, N, H, rounds) ? 0 : rigid_ws(nullptr, B, N, H, rounds).bytes;
-}
-
-extern "C" int64_t pvraft_rigid_motion_fwd_det_workspace_bytes(int B, int rounds) {
-    return B < 1 || rounds < 1 || rounds > kRmMaxRounds ? 0 : fx_bytes((long long)rounds * B * kRmMoments);
-}
-
-extern "C" int pvraft_rigid_motion_fwd(const float* xyz1, const float* flow, const uint8_t* mask, int B, int N, float threshold, int H,
-                                       int rounds, int seed, float* R, float* t, uint8_t* inliers, int32_t* count, uint8_t* degenerate,
-                                       double* state, int32_t* triples, int32_t* hyp_count, void* workspace, void* det_workspace,
-                                       void* stream) {
-    if (!xyz1 || !flow || !R || !t || !inliers || !count || !degenerate || !state || !workspace || bad_sizes(B, N, H, rounds) ||
-        !(threshold > 0.f) || isinf(threshold) || seed < 0)
-        return fail(PVRAFT_ERR_BAD_ARG, "rigid_motion_fwd: bad argument");
-    if (B > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "rigid_motion_fwd: B = %d samples (at most 65535)", B);
-    cudaStream_t st = (cudaStream_t)stream;
-    const RigidWs L = rigid_ws(workspace, B, N, H, rounds);
-    const float thr2 = threshold * threshold;
-    if (mask) k_rigid_allowed<<<B, kRmScan, 0, st>>>(mask, N, L.allowed, L.nallow);
-    // the score reads the mask itself, in point order; the sampler and the selection the allowed list
-    const RmSegs sg{mask ? L.allowed : nullptr, nullptr, L.nallow, N, 1};
-    const RmSegs dense{nullptr, nullptr, nullptr, N, 1};
-    k_rigid_hypotheses<<<dim3((unsigned)((H + 127) / 128), (unsigned)B), 128, 0, st>>>(xyz1, flow, sg, H, (unsigned long long)seed,
-                                                                                      threshold, L.hyp, L.hcnt, triples);
-    k_rigid_score<<<dim3((unsigned)((N + kScPoints - 1) / kScPoints), (unsigned)((H + kScHyp - 1) / kScHyp), (unsigned)B), kScThreads, 0,
-                    st>>>(xyz1, flow, mask, dense, nullptr, nullptr, 0, H, thr2, L.hyp, L.hcnt);
-    k_rigid_select<<<B, kSelThreads, 0, st>>>(xyz1, flow, sg, H, B, rounds, L.hyp, L.hcnt, L.model, L.mom, hyp_count);
-    return rigid_refits(xyz1, flow, mask, nullptr, nullptr, nullptr, 1, B, N, rounds, thr2, dim3((unsigned)((N + kMomThreads - 1) / kMomThreads),
-                        (unsigned)B), L.model, L.mom, R, t, inliers, count, degenerate, state, det_workspace, st, "rigid_motion_fwd");
-}
-
-extern "C" int pvraft_rigid_motion_bwd(const float* xyz1, const float* flow, const uint8_t* inliers, const double* state, const float* dR,
-                                       const float* dt, int B, int N, float* d_xyz1, float* d_flow, void* stream) {
-    if (!xyz1 || !flow || !inliers || !state || !dR || !dt || !d_xyz1 || !d_flow || B < 1 || N < 3 || (long long)B * N > 0x7fffffffll)
-        return fail(PVRAFT_ERR_BAD_ARG, "rigid_motion_bwd: bad argument");
-    const long long points = (long long)B * N;
-    const unsigned blocks = (unsigned)scatter_blocks(points, false);
-    k_rigid_bwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(xyz1, flow, inliers, nullptr, 1, state, dR, dt, N, points, d_xyz1, d_flow);
-    return check_launch("rigid_motion_bwd");
-}
-
-namespace pvraft {
-
-// ---- one fit per object ---------------------------------------------------------------------------------------------------
-// The segments of rigid_objects: the points of each sample grouped stably by label (labels [B,N], -1 or out of [0, O): no
-// object) in windows of kRoChunk point ids, with integer counts only:
+// ---- the grouping for O > 1 ------------------------------------------------------------------------------------------------
+// The points of each sample grouped stably by label (labels [B,N], -1 or out of [0, O): no segment) in windows of kRoChunk
+// point ids, with integer counts only:
 //   k_ro_group_count    per window, the number of points of each object -> cnt [B,C,O] (C = ceil(N / kRoChunk))
 //   k_ro_group_scan     one CTA per sample, thread o per object: n[g] and start[g] = s N + (members of the objects before
 //                       o); pre [B,C,O] = where window c's members of o go in the sample's list; the moment items (c << 8) | o of every window
@@ -828,9 +728,10 @@ __global__ void __launch_bounds__(kRoChunk) k_ro_group_scatter(const int32_t* __
     list[(long long)s * N + __ldg(pre + ((long long)s * C + c) * O + l) + before] = i;
 }
 
-// the workspace of rigid_objects: list [B,N] | start [G] | n [G] | cnt [B,C,O] | pre [B,C,O] | moment items [B,N] |
-// nm [B] | score items [B,S] | ns [B] | hyp [G,H,16] f32 | hcnt [G,H] | model [G,16] f32 | mom [rounds,G,16] f64
-struct ObjWs {
+// the forward's workspace: list [B,N] | start [G] | n [G] | cnt [B,C,O] | pre [B,C,O] | moment items [B,N] | nm [B] |
+// score items [B,S] | ns [B] | hyp [G,H,16] f32 | hcnt [G,H] | model [G,16] f32 | mom [rounds,G,16] f64, each range 16-byte
+// aligned (O = 1 uses list and n only of the grouping's ranges)
+struct FitWs {
     int32_t *list, *start, *n, *cnt, *pre, *mitems, *nm, *sitems, *ns;
     float* hyp;
     int32_t* hcnt;
@@ -839,7 +740,7 @@ struct ObjWs {
     int C, S;
     int64_t bytes;
 };
-static ObjWs objects_ws(void* ws, int B, int N, int O, int H, int rounds) {
+static FitWs fit_ws(void* ws, int B, int N, int O, int H, int rounds) {
     char* base = static_cast<char*>(ws);
     int64_t off = 0;
     auto take = [&](int64_t bytes) {
@@ -847,7 +748,7 @@ static ObjWs objects_ws(void* ws, int B, int N, int O, int H, int rounds) {
         off += (bytes + 15) / 16 * 16;
         return p;
     };
-    ObjWs L;
+    FitWs L;
     const long long G = (long long)B * O;
     L.C = (N + kRoChunk - 1) / kRoChunk;
     L.S = (N + kScPoints - 1) / kScPoints + O;
@@ -868,15 +769,17 @@ static ObjWs objects_ws(void* ws, int B, int N, int O, int H, int rounds) {
     return L;
 }
 
-static bool bad_objects(int B, int N, int O, int H, int rounds) {
+static bool bad_sizes(int B, int N, int O, int H, int rounds) {
     return B < 1 || N < 1 || O < 1 || O > kRoMaxObjects || H < 1 || H > kRmMaxH || rounds < 1 || rounds > kRmMaxRounds ||
            (long long)B * N > 0x7fffffffll;
 }
 
 }  // namespace pvraft
 
+using namespace pvraft;
+
 extern "C" int64_t pvraft_rigid_objects_workspace_bytes(int B, int N, int O, int H, int rounds) {
-    return bad_objects(B, N, O, H, rounds) ? 0 : objects_ws(nullptr, B, N, O, H, rounds).bytes;
+    return bad_sizes(B, N, O, H, rounds) ? 0 : fit_ws(nullptr, B, N, O, H, rounds).bytes;
 }
 
 extern "C" int64_t pvraft_rigid_objects_fwd_det_workspace_bytes(int B, int O, int rounds) {
@@ -885,34 +788,59 @@ extern "C" int64_t pvraft_rigid_objects_fwd_det_workspace_bytes(int B, int O, in
 
 extern "C" int pvraft_rigid_objects_fwd(const float* xyz1, const float* flow, const int32_t* labels, int B, int N, int O, float threshold,
                                         int H, int rounds, int seed, float* R, float* t, uint8_t* inliers, int32_t* count,
-                                        uint8_t* degenerate, double* state, void* workspace, void* det_workspace, void* stream) {
-    if (!xyz1 || !flow || !labels || !R || !t || !inliers || !count || !degenerate || !state || !workspace ||
-        bad_objects(B, N, O, H, rounds) || !(threshold > 0.f) || isinf(threshold) || seed < 0)
+                                        uint8_t* degenerate, double* state, int32_t* triples, int32_t* hyp_count, void* workspace,
+                                        void* det_workspace, void* stream) {
+    if (!xyz1 || !flow || (!labels && O != 1) || !R || !t || !inliers || !count || !degenerate || !state || !workspace ||
+        bad_sizes(B, N, O, H, rounds) || !(threshold > 0.f) || isinf(threshold) || seed < 0)
         return fail(PVRAFT_ERR_BAD_ARG, "rigid_objects_fwd: bad argument");
     if ((long long)B * O > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "rigid_objects_fwd: B * O = %lld fits (at most 65535)", (long long)B * O);
     cudaStream_t st = (cudaStream_t)stream;
-    const ObjWs L = objects_ws(workspace, B, N, O, H, rounds);
+    const FitWs L = fit_ws(workspace, B, N, O, H, rounds);
     const int G = B * O;
     const float thr2 = threshold * threshold;
-    cudaError_t e = cudaMemsetAsync(inliers, 0, (size_t)B * N, st);
-    if (e != cudaSuccess) return fail((int)e, "rigid_objects_fwd: memset failed: %s", cudaGetErrorString(e));
-    k_ro_group_count<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.cnt);
-    k_ro_group_scan<<<B, kRoMaxObjects, 0, st>>>(L.cnt, N, O, L.C, L.S, L.pre, L.start, L.n, L.mitems, L.nm, L.sitems, L.ns);
-    k_ro_group_scatter<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.pre, L.list);
-    const RmSegs sg{L.list, L.start, L.n, N, O};
+    // O = 1: the member list in one launch (none without labels), and the score and moment kernels' one-segment grids;
+    // O > 1: the stable grouping, and work items that cover each segment's members
+    const int32_t *sitems = nullptr, *nsitems = nullptr, *mitems = nullptr, *nmitems = nullptr;
+    unsigned score_x = (unsigned)((N + kScPoints - 1) / kScPoints), mom_x = (unsigned)L.C;
+    if (O == 1) {
+        if (labels) k_rigid_allowed<<<B, kRmScan, 0, st>>>(labels, N, L.list, L.n);
+    } else {
+        cudaError_t e = cudaMemsetAsync(inliers, 0, (size_t)B * N, st);   // the moments write the members' inliers only
+        if (e != cudaSuccess) return fail((int)e, "rigid_objects_fwd: memset failed: %s", cudaGetErrorString(e));
+        k_ro_group_count<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.cnt);
+        k_ro_group_scan<<<B, kRoMaxObjects, 0, st>>>(L.cnt, N, O, L.C, L.S, L.pre, L.start, L.n, L.mitems, L.nm, L.sitems, L.ns);
+        k_ro_group_scatter<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.pre, L.list);
+        sitems = L.sitems, nsitems = L.ns, mitems = L.mitems, nmitems = L.nm;
+        score_x = (unsigned)L.S;
+        mom_x += (unsigned)O;
+    }
+    const RmSegs sg{labels ? L.list : nullptr, O > 1 ? L.start : nullptr, L.n, N, O};
     k_rigid_hypotheses<<<dim3((unsigned)((H + 127) / 128), (unsigned)G), 128, 0, st>>>(xyz1, flow, sg, H, (unsigned long long)seed,
-                                                                                      threshold, L.hyp, L.hcnt, nullptr);
-    k_rigid_score<<<dim3((unsigned)L.S, (unsigned)((H + kScHyp - 1) / kScHyp), (unsigned)B), kScThreads, 0, st>>>(
-        xyz1, flow, nullptr, sg, L.sitems, L.ns, L.S, H, thr2, L.hyp, L.hcnt);
-    k_rigid_select<<<G, kSelThreads, 0, st>>>(xyz1, flow, sg, H, G, rounds, L.hyp, L.hcnt, L.model, L.mom, nullptr);
-    return rigid_refits(xyz1, flow, nullptr, labels, L.mitems, L.nm, O, B, N, rounds, thr2, dim3((unsigned)(L.C + O), (unsigned)B), L.model,
-                        L.mom, R, t, inliers, count, degenerate, state, det_workspace, st, "rigid_objects_fwd");
+                                                                                      threshold, L.hyp, L.hcnt, triples);
+    k_rigid_score<<<dim3(score_x, (unsigned)((H + kScHyp - 1) / kScHyp), (unsigned)B), kScThreads, 0, st>>>(
+        xyz1, flow, sg, sitems, nsitems, L.S, H, thr2, L.hyp, L.hcnt);
+    k_rigid_select<<<G, kSelThreads, 0, st>>>(xyz1, flow, sg, H, G, rounds, L.hyp, L.hcnt, L.model, L.mom, hyp_count);
+    const unsigned sblocks = (unsigned)((G + 63) / 64);
+    for (int r = 0; r < rounds; ++r) {
+        double* mom = L.mom + (long long)r * G * kRmMoments;
+        if (det_workspace) {
+            const FxSlots slots = fx_slots(det_workspace) + (long long)r * G * kRmMoments;
+            k_rigid_moments<true><<<dim3(mom_x, (unsigned)B), kMomThreads, 0, st>>>(xyz1, flow, labels, mitems, nmitems, O, N, thr2, L.model,
+                                                                                  inliers, slots);
+            k_rigid_solve<true><<<sblocks, 64, 0, st>>>(mom, slots, G, L.model, R, t, count, degenerate, state);
+        } else {
+            k_rigid_moments<false><<<dim3(mom_x, (unsigned)B), kMomThreads, 0, st>>>(xyz1, flow, labels, mitems, nmitems, O, N, thr2, L.model,
+                                                                                   inliers, mom);
+            k_rigid_solve<false><<<sblocks, 64, 0, st>>>(mom, FxSlots{}, G, L.model, R, t, count, degenerate, state);
+        }
+    }
+    return check_launch("rigid_objects_fwd");
 }
 
 extern "C" int pvraft_rigid_objects_bwd(const float* xyz1, const float* flow, const int32_t* labels, const uint8_t* inliers,
                                         const double* state, const float* dR, const float* dt, int B, int N, int O, float* d_xyz1,
                                         float* d_flow, void* stream) {
-    if (!xyz1 || !flow || !labels || !inliers || !state || !dR || !dt || !d_xyz1 || !d_flow || B < 1 || N < 1 || O < 1 ||
+    if (!xyz1 || !flow || (!labels && O != 1) || !inliers || !state || !dR || !dt || !d_xyz1 || !d_flow || B < 1 || N < 1 || O < 1 ||
         O > kRoMaxObjects || (long long)B * N > 0x7fffffffll)
         return fail(PVRAFT_ERR_BAD_ARG, "rigid_objects_bwd: bad argument");
     const long long points = (long long)B * N;

@@ -1015,49 +1015,8 @@ def flow_propagate(xyz_prev, flow_prev, xyz, k=3, want_idx=False, use_grid=None)
     return (out, idx) if want_idx else out
 
 
-RIGID_MAX_HYPOTHESES = 4096   # pvraft_rigid_motion_fwd scores at most this many minimal samples per call
+RIGID_MAX_HYPOTHESES = 4096   # pvraft_rigid_objects_fwd scores at most this many minimal samples per segment
 RIGID_MAX_ROUNDS = 8
-
-
-def rigid_motion(x, f, mask, threshold, hypotheses, rounds, seed, want_samples=False):
-    """x, f [B,N,3] f32 (the first cloud and its flow), mask [B,N] uint8 or None -> (R [B,3,3], t [B,3], inliers [B,N] uint8,
-    count [B] int32, degenerate [B] uint8, state [B,32] f64 for rigid_motion_bwd), plus (triples [B,H,3] int32, hypothesis
-    counts [B,H] int32, -1 for a rejected triple) with want_samples.  The RANSAC + Horn refit of include/pvraft_b200.h,
-    pvraft_rigid_motion_fwd; the arguments are checked by pvraft_b200.rigid_motion."""
-    b, n = int(x.shape[0]), int(x.shape[1])
-    dev = x.device
-    R = torch.empty(b, 3, 3, dtype=torch.float32, device=dev)
-    t = torch.empty(b, 3, dtype=torch.float32, device=dev)
-    inl = torch.empty(b, n, dtype=torch.uint8, device=dev)
-    count = torch.empty(b, dtype=torch.int32, device=dev)
-    degen = torch.empty(b, dtype=torch.uint8, device=dev)
-    state = torch.empty(b, 32, dtype=torch.float64, device=dev)
-    triples = torch.empty(b, hypotheses, 3, dtype=torch.int32, device=dev) if want_samples else None
-    hcount = torch.empty(b, hypotheses, dtype=torch.int32, device=dev) if want_samples else None
-    ws = _workspace(lib().pvraft_rigid_motion_workspace_bytes(b, n, hypotheses, rounds), dev)
-    det = _det_workspace(lib().pvraft_rigid_motion_fwd_det_workspace_bytes, b, rounds, device=dev)
-    _count(lib().pvraft_rigid_motion_fwd(_p(x), _p(f), _p(mask, torch.uint8), b, n, float(threshold), hypotheses, rounds, seed, _p(R),
-                                         _p(t), _p(inl, torch.uint8), _p(count, torch.int32), _p(degen, torch.uint8),
-                                         _p(state, torch.float64), _p(triples, torch.int32), _p(hcount, torch.int32),
-                                         _p(ws, torch.uint8), _p(det, torch.uint8), _stream()), 'rigid_motion_fwd')
-    out = (R, t, inl, count, degen, state)
-    return out + (triples, hcount) if want_samples else out
-
-
-def rigid_motion_bwd(x, f, inliers, state, dR, dt):
-    """Gradients of rigid_motion's R and t with the inlier set held fixed, for the upstream dR [B,3,3] and dt [B,3] (on the
-    device) -> (d_x, d_f) [B,N,3], every element written once."""
-    b, n = int(x.shape[0]), int(x.shape[1])
-    if f.shape != x.shape or tuple(inliers.shape) != (b, n) or tuple(state.shape) != (b, 32) or tuple(dR.shape) != (b, 3, 3) or \
-            tuple(dt.shape) != (b, 3):
-        raise ValueError(f'rigid_motion_bwd: shapes x {tuple(x.shape)}, f {tuple(f.shape)}, inliers {tuple(inliers.shape)}, state '
-                         f'{tuple(state.shape)}, dR {tuple(dR.shape)}, dt {tuple(dt.shape)} do not agree')
-    d_x, d_f = torch.empty_like(x), torch.empty_like(x)
-    _count(lib().pvraft_rigid_motion_bwd(_p(x), _p(f), _p(inliers, torch.uint8), _p(state, torch.float64), _p(dR), _p(dt), b, n, _p(d_x),
-                                         _p(d_f), _stream()), 'rigid_motion_bwd')
-    return d_x, d_f
-
-
 RIGID_MAX_OBJECTS = 256   # pvraft_euclidean_clusters_fwd / pvraft_rigid_objects_fwd keep at most this many objects per sample
 
 
@@ -1078,10 +1037,13 @@ def euclidean_clusters(x, f, mask, radius, flow_radius, min_points, max_objects)
     return labels, num, sizes
 
 
-def rigid_objects(x, f, labels, objects, threshold, hypotheses, rounds, seed):
-    """x, f [B,N,3] f32, labels [B,N] int32 (euclidean_clusters) -> (R [B,O,3,3], t [B,O,3], inliers [B,N] uint8, count [B,O]
-    int32, degenerate [B,O] uint8, state [B,O,32] f64 for rigid_objects_bwd), O = objects: rigid_motion's fit once per object
-    (include/pvraft_b200.h, pvraft_rigid_objects_fwd)."""
+def rigid_objects(x, f, labels, objects, threshold, hypotheses, rounds, seed, want_samples=False):
+    """x, f [B,N,3] f32 (the first cloud and its flow), labels [B,N] int32 (segment o of sample b: labels[b] == o), or None
+    with objects = 1 (every point in segment 0) -> (R [B,O,3,3], t [B,O,3], inliers [B,N] uint8, count [B,O] int32,
+    degenerate [B,O] uint8, state [B,O,32] f64 for rigid_objects_bwd), O = objects, plus (triples [B O,H,3] int32,
+    hypothesis counts [B O,H] int32, -1 for a rejected triple) with want_samples.  The RANSAC + Horn refit of each segment
+    (include/pvraft_b200.h, pvraft_rigid_objects_fwd); the arguments are checked by pvraft_b200.rigid_motion and
+    pvraft_b200.rigid_objects."""
     b, n, o = int(x.shape[0]), int(x.shape[1]), int(objects)
     dev = x.device
     R = torch.empty(b, o, 3, 3, dtype=torch.float32, device=dev)
@@ -1090,23 +1052,27 @@ def rigid_objects(x, f, labels, objects, threshold, hypotheses, rounds, seed):
     count = torch.empty(b, o, dtype=torch.int32, device=dev)
     degen = torch.empty(b, o, dtype=torch.uint8, device=dev)
     state = torch.empty(b, o, 32, dtype=torch.float64, device=dev)
+    triples = torch.empty(b * o, hypotheses, 3, dtype=torch.int32, device=dev) if want_samples else None
+    hcount = torch.empty(b * o, hypotheses, dtype=torch.int32, device=dev) if want_samples else None
     ws = _workspace(lib().pvraft_rigid_objects_workspace_bytes(b, n, o, hypotheses, rounds), dev)
     det = _det_workspace(lib().pvraft_rigid_objects_fwd_det_workspace_bytes, b, o, rounds, device=dev)
     _count(lib().pvraft_rigid_objects_fwd(_p(x), _p(f), _p(labels, torch.int32), b, n, o, float(threshold), hypotheses, rounds, seed,
                                           _p(R), _p(t), _p(inl, torch.uint8), _p(count, torch.int32), _p(degen, torch.uint8),
-                                          _p(state, torch.float64), _p(ws, torch.uint8), _p(det, torch.uint8), _stream()),
-           'rigid_objects_fwd')
-    return R, t, inl, count, degen, state
+                                          _p(state, torch.float64), _p(triples, torch.int32), _p(hcount, torch.int32),
+                                          _p(ws, torch.uint8), _p(det, torch.uint8), _stream()), 'rigid_objects_fwd')
+    out = (R, t, inl, count, degen, state)
+    return out + (triples, hcount) if want_samples else out
 
 
 def rigid_objects_bwd(x, f, labels, inliers, state, dR, dt):
     """Gradients of rigid_objects' R and t with the labels and inlier sets held fixed, for the upstream dR [B,O,3,3] and dt
-    [B,O,3] -> (d_x, d_f) [B,N,3], every element written once."""
+    [B,O,3] (on the device) -> (d_x, d_f) [B,N,3], every element written once."""
     b, n, o = int(x.shape[0]), int(x.shape[1]), int(state.shape[1])
-    if f.shape != x.shape or tuple(labels.shape) != (b, n) or tuple(inliers.shape) != (b, n) or tuple(state.shape) != (b, o, 32) or \
-            tuple(dR.shape) != (b, o, 3, 3) or tuple(dt.shape) != (b, o, 3):
-        raise ValueError(f'rigid_objects_bwd: shapes x {tuple(x.shape)}, f {tuple(f.shape)}, labels {tuple(labels.shape)}, inliers '
-                         f'{tuple(inliers.shape)}, state {tuple(state.shape)}, dR {tuple(dR.shape)}, dt {tuple(dt.shape)} do not agree')
+    if f.shape != x.shape or (labels is not None and tuple(labels.shape) != (b, n)) or tuple(inliers.shape) != (b, n) or \
+            tuple(state.shape) != (b, o, 32) or tuple(dR.shape) != (b, o, 3, 3) or tuple(dt.shape) != (b, o, 3):
+        raise ValueError(f'rigid_objects_bwd: shapes x {tuple(x.shape)}, f {tuple(f.shape)}, labels '
+                         f'{None if labels is None else tuple(labels.shape)}, inliers {tuple(inliers.shape)}, state '
+                         f'{tuple(state.shape)}, dR {tuple(dR.shape)}, dt {tuple(dt.shape)} do not agree')
     d_x, d_f = torch.empty_like(x), torch.empty_like(x)
     _count(lib().pvraft_rigid_objects_bwd(_p(x), _p(f), _p(labels, torch.int32), _p(inliers, torch.uint8), _p(state, torch.float64),
                                           _p(dR), _p(dt), b, n, o, _p(d_x), _p(d_f), _stream()), 'rigid_objects_bwd')

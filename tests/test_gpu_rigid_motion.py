@@ -184,14 +184,18 @@ def fit(dev, x, f, mask=None, **kw):
 
 
 def raw(dev, x, f, mask=None, threshold=0.1, hypotheses=256, rounds=2, seed=0):
+    """The one-segment fit rigid_motion makes, with the sampler's triples and counts: (R, t, inliers, count, degenerate,
+    state, triples [B,H,3], hypothesis counts [B,H])."""
     from pvraft_b200 import ops
-    m = None if mask is None else mask.to(dev).contiguous().view(torch.uint8)
-    return ops.rigid_motion(x.to(dev).contiguous(), f.to(dev).contiguous(), m, threshold, hypotheses, rounds, seed, want_samples=True)
+    lab = None if mask is None else torch.add(mask.to(dev), -1).int()
+    R, t, inl, count, degen, state, triples, hcount = ops.rigid_objects(x.to(dev).contiguous(), f.to(dev).contiguous(), lab, 1, threshold,
+                                                                        hypotheses, rounds, seed, want_samples=True)
+    return R[:, 0], t[:, 0], inl, count[:, 0], degen[:, 0], state[:, 0], triples, hcount
 
 
 # ---- 1. sampler ----------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize('masked', [False, True])
-def test_sampler_bit_exact(dev, masked):
+def test_one_segment_sampler_bit_exact(dev, masked):
     g = torch.Generator().manual_seed(1)
     b, n, hc, thr, seed = 2, 3000, 1024, 0.1, 12345
     x = torch.rand(b, n, 3, generator=g) * 10
@@ -219,7 +223,7 @@ def test_sampler_bit_exact(dev, masked):
 
 
 # ---- 2. counts and selection ---------------------------------------------------------------------------------------------
-def test_counts_and_selection_against_float64(dev):
+def test_one_segment_counts_and_selection_against_float64(dev):
     g = torch.Generator().manual_seed(2)
     n, hc, thr = 4000, 512, 0.5
     x64 = torch.rand(n, 3, generator=g, dtype=torch.float64) * 5
@@ -411,7 +415,7 @@ def batch_case(g, b=4, n=5000):
     return torch.stack(xs), torch.stack(fs)
 
 
-def test_deterministic_repeatable_and_batched_equals_per_sample(dev, det):
+def test_one_segment_deterministic_repeatable_and_batched_equals_per_sample(dev, det):
     g = torch.Generator().manual_seed(8)
     x, f = batch_case(g)
     mask = torch.rand(x.shape[:2], generator=g) < 0.9
@@ -428,7 +432,7 @@ def test_deterministic_repeatable_and_batched_equals_per_sample(dev, det):
     assert all(same_bits(p, q) for p, q in zip(ra, rb))
 
 
-def test_default_mode_agrees_with_deterministic_mode(dev):
+def test_one_segment_default_mode_agrees_with_deterministic_mode(dev):
     g = torch.Generator().manual_seed(9)
     x, f = batch_case(g)
     a = raw(dev, x, f, threshold=0.05)

@@ -18,14 +18,14 @@ def r16(v):
     return (v + 15) // 16 * 16
 
 
-def test_header_declares_and_lib_binds_the_entry_points():
+def test_header_declares_and_lib_binds_the_clustering_and_fit_entry_points():
     from pvraft_b200 import _lib
     with open(os.path.join(ROOT, 'include', 'pvraft_b200.h')) as f:
         header = f.read()
     for name in NAMES:
         assert re.search(r'PVRAFT_API int(64_t)? ' + name + r'\(', header), name
         assert name in _lib.EXPORTS
-    assert [len(_lib._SIGNATURES[n][1]) for n in NAMES] == [14, 2, 19, 5, 3, 13]
+    assert [len(_lib._SIGNATURES[n][1]) for n in NAMES] == [14, 2, 21, 5, 3, 13]
     from pvraft_b200 import build
     assert 'clusters.cu' in build.SOURCES
 
@@ -52,7 +52,7 @@ def test_workspace_sizes():
         assert lib.pvraft_euclidean_clusters_workspace_bytes(*bad) == 0, bad
 
 
-def test_entry_points_refuse_bad_arguments():
+def test_clustering_and_fit_entry_points_refuse_bad_arguments():
     from pvraft_b200 import _lib
     lib = _lib.lib()
 
@@ -60,7 +60,7 @@ def test_entry_points_refuse_bad_arguments():
         return lib.pvraft_euclidean_clusters_fwd(x, f, mask, B, N, radius, fr, minp, O, lab, num, sizes, ws, None)
 
     def fwd(x=P, f=P, lab=P, B=2, N=64, O=8, thr=0.1, H=256, rounds=2, seed=0, R=P, t=P, inl=P, cnt=P, deg=P, st=P, ws=P):
-        return lib.pvraft_rigid_objects_fwd(x, f, lab, B, N, O, thr, H, rounds, seed, R, t, inl, cnt, deg, st, ws, None, None)
+        return lib.pvraft_rigid_objects_fwd(x, f, lab, B, N, O, thr, H, rounds, seed, R, t, inl, cnt, deg, st, None, None, ws, None, None)
 
     def bwd(x=P, f=P, lab=P, inl=P, st=P, dR=P, dt=P, B=2, N=64, O=8, dx=P, df=P):
         return lib.pvraft_rigid_objects_bwd(x, f, lab, inl, st, dR, dt, B, N, O, dx, df, None)

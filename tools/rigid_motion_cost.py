@@ -1,6 +1,6 @@
-"""Cost of the rigid-motion fit (pvraft_b200.rigid_motion): CUDA-event times of the forward and of forward + backward at
-B in {1, 8}, N in {8192, 32768, 131072}, H in {256, 1024} hypotheses, rounds = 2, on LiDAR-like scenes (ego-motion, two
-moving objects, 1 cm noise, threshold 0.05), and the score kernel's own time from torch.profiler in a separate pass, as
+"""Cost of the rigid-motion fit (pvraft_b200.rigid_motion): CUDA-event times of the forward, of the forward with a mask that
+allows 9 points in 10, and of forward + backward at B in {1, 8}, N in {8192, 32768, 131072}, H in {256, 1024} hypotheses,
+rounds = 2, on LiDAR-like scenes (ego-motion, two moving objects, 1 cm noise, threshold 0.05), and the score kernel's own time from torch.profiler in a separate pass, as
 point-hypothesis tests per second (B N H over its time).  Every time is a median over `--calls` calls.  Prints the card name
 and power limit read in the same run.  `python tools/rigid_motion_cost.py [--calls 20]`."""
 import argparse
@@ -53,21 +53,26 @@ def main():
             x, f = scene(b, n, dev)
             xg, fg = x.clone().requires_grad_(True), f.clone().requires_grad_(True)
             gR, gt = torch.randn(b, 3, 3, device=dev), torch.randn(b, 3, device=dev)
+            mask = (torch.arange(n, device=dev) % 10 != 0).expand(b, n).contiguous()
             for h in (256, 1024):
                 def fwd():
                     pvraft_b200.rigid_motion(x, f, threshold=0.05, hypotheses=h, rounds=2)
+
+                def fwd_masked():
+                    pvraft_b200.rigid_motion(x, f, mask=mask, threshold=0.05, hypotheses=h, rounds=2)
 
                 def fwd_bwd():
                     out = pvraft_b200.rigid_motion(xg, fg, threshold=0.05, hypotheses=h, rounds=2)
                     torch.autograd.grad((out.rotation * gR).sum() + (out.translation * gt).sum(), (xg, fg))
 
                 t_f = _median_ms(fwd, a.calls, 5)
+                t_m = _median_ms(fwd_masked, a.calls, 5)
                 t_fb = _median_ms(fwd_bwd, a.calls, 5)
-                rows.append((b, n, h, t_f, t_fb, x, f))
-    print(' B       N     H   forward ms   fwd+bwd ms   score kernel ms   tests/s')
-    for b, n, h, t_f, t_fb, x, f in rows:
+                rows.append((b, n, h, t_f, t_m, t_fb, x, f))
+    print(' B       N     H   forward ms   masked fwd ms   fwd+bwd ms   score kernel ms   tests/s')
+    for b, n, h, t_f, t_m, t_fb, x, f in rows:
         sc = score_seconds(x, f, h, a.calls)
-        print(f'{b:2d} {n:7d} {h:5d} {t_f:12.3f} {t_fb:12.3f} {sc * 1e3:17.4f} {b * n * h / sc:9.3e}')
+        print(f'{b:2d} {n:7d} {h:5d} {t_f:12.3f} {t_m:15.3f} {t_fb:12.3f} {sc * 1e3:17.4f} {b * n * h / sc:9.3e}')
 
 
 if __name__ == '__main__':
