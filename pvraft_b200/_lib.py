@@ -1,20 +1,31 @@
-"""ctypes binding of the C ABI declared in include/pvraft_b200.h.
+"""ctypes binding of the C ABI, derived from its declarations in include/pvraft_b200.h.
 
-The shared library is mandatory: importing the package never falls back to PyTorch ops or to the
-CPU oracle -- a missing/unbuildable `libpvraft_b200.so` raises at first use.
+The header is read at import: every `PVRAFT_API` function and every argument struct is bound from what the header says,
+so the binding cannot drift from the declarations the library is compiled against.  This is not a C parser: after
+comments and preprocessor lines are removed, the header may contain only these forms (anything else raises PvraftError
+naming the declaration):
+  - `PVRAFT_API <ret> pvraft_x(<params>);`  with <ret> one of int, int64_t, const char*, and `(void)` for no parameters;
+  - `typedef struct pvraft_x { <fields> } pvraft_x;`  one or more `<type> <declarator>, ...;` per field line, a
+    declarator optionally a fixed array (`const float* in[3];`);
+  - `typedef enum pvraft_x { ... } pvraft_x;`  (not bound: the Python side names the values it uses);
+  - the `extern "C" {` ... `}` wrapper.
+Types: int, int64_t, float, double as scalars; pointers (const or not) to float, double, int32_t, int8_t, uint8_t,
+uint16_t, int, void or one of the header's structs, all passed as c_void_p.  Each pointer's pointee is recorded
+(FUNCTIONS, STRUCT_FIELDS) so that ops can check the tensor behind it.
+
+The shared library is mandatory: importing the package never falls back to PyTorch ops or to the CPU oracle -- a
+missing/unbuildable `libpvraft_b200.so` raises at first use.
 """
 import ctypes as C
+import keyword
 import os
+import re
 import threading
+from typing import NamedTuple
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libpvraft_b200.so')
-
-c_float_p = C.POINTER(C.c_float)
-c_double_p = C.POINTER(C.c_double)
-c_int32_p = C.POINTER(C.c_int32)
-c_int8_p = C.POINTER(C.c_int8)
-VP = C.c_void_p   # device pointers travel as plain addresses
+HEADER_PATH = os.path.join(_HERE, '..', 'include', 'pvraft_b200.h')
 
 IN_PLAIN, IN_GN, IN_GN_MINMAX = 0, 1, 2
 ACT_NONE, ACT_RELU, ACT_LRELU = 0, 1, 2
@@ -22,171 +33,97 @@ KNN = 32
 MOMENTS = 16
 
 
-class LinearArgs(C.Structure):
-    _fields_ = [('in_', VP), ('in_min', VP), ('in_stats', VP), ('in_gamma', VP), ('in_beta', VP),
-                ('in_count', C.c_double), ('in_mode', C.c_int), ('in_act', C.c_int), ('in_slope', C.c_float),
-                ('weight', VP), ('w_ld', C.c_int), ('w_cin', C.c_int), ('bias', VP), ('residual', VP), ('out_act', C.c_int),
-                ('out', VP), ('out_stats', VP), ('B', C.c_int), ('N', C.c_int), ('cin', C.c_int), ('cout', C.c_int)]
+class PvraftError(RuntimeError):
+    pass
 
 
-class TcLinearArgs(C.Structure):
-    _fields_ = [('in_', VP * 3), ('in_channels', C.c_int * 3), ('in_min', VP), ('in_stats', VP), ('in_gamma', VP),
-                ('in_beta', VP), ('in_count', C.c_double), ('in_act', C.c_int), ('in_slope', C.c_float), ('w_hi', VP),
-                ('w_lo', VP), ('n_pad', C.c_int), ('cout', C.c_int), ('bias', VP), ('bias2', VP), ('out_act', C.c_int),
-                ('residual', VP), ('out', VP), ('out2', VP), ('h', VP), ('z', VP), ('out_stats', VP), ('epilogue', C.c_int),
-                ('B', C.c_int), ('N', C.c_int), ('tail', VP), ('w3', VP), ('b3', VP), ('coords1', VP), ('coords2', VP),
-                ('coords2_out', VP), ('flow_out', VP), ('params_settled', C.c_int), ('w_bf16', VP)]
+class Decl(NamedTuple):
+    """One parameter or struct field of the C ABI."""
+    name: str          # as Python spells it (a keyword gets a trailing '_': `in` -> `in_`)
+    ctype: object      # its ctypes type (an array type for a fixed array field)
+    pointee: object    # the C type a pointer points to ('float', 'pvraft_linear_args', ...); None for a scalar
+    length: int        # elements of a fixed array field; 1 otherwise
 
 
-class UpdateChainArgs(C.Structure):
-    _fields_ = [('y1', VP), ('y1_stats', VP), ('gn_gamma', VP), ('gn_beta', VP), ('gn_count', C.c_double),
-                ('gn_slope', C.c_float), ('kfeat', VP), ('cflow', VP), ('flow', VP), ('net', VP), ('inp', VP),
-                ('w_hi', VP * 5), ('w_lo', VP * 5), ('b_cc', VP), ('b_m', VP), ('b_z', VP), ('b_r', VP), ('b_q', VP),
-                ('net_out', VP), ('p_out', VP), ('B', C.c_int), ('N', C.c_int), ('hidden', C.c_int), ('context', C.c_int),
-                ('y1_channels', C.c_int), ('w_bf16', VP * 5)]
+_SCALARS = {'int': C.c_int, 'int64_t': C.c_int64, 'float': C.c_float, 'double': C.c_double}
+_POINTEES = {'float', 'double', 'int32_t', 'int8_t', 'uint8_t', 'uint16_t', 'int', 'void'}
+_RETURNS = {'int': C.c_int, 'int64_t': C.c_int64, 'const char*': C.c_char_p}
+
+_FORM = re.compile(r'''\s*(?:
+    (?P<extern>extern\s+"C"\s*\{) | (?P<close>\}) |
+    typedef\s+enum\s+(?P<enum>\w+)\s*\{[^{}]*\}\s*(?P=enum)\s*; |
+    typedef\s+struct\s+(?P<struct>\w+)\s*\{(?P<fields>[^{}]*)\}\s*(?P=struct)\s*; |
+    PVRAFT_API\s+(?P<ret>[\w\s*]*?)\s*\b(?P<fn>pvraft_\w+)\s*\((?P<params>[^()]*)\)\s*;
+)''', re.X)
+_TYPE = re.compile(r'\s*(?:const\s+)?(\w+)\s*(.*)', re.S)
+_DECLARATOR = re.compile(r'\s*(\*?)\s*(\w+)\s*(?:\[(\d+)\])?\s*')
 
 
-class KnnBranchArgs(C.Structure):
-    _fields_ = [('knn_sel', VP), ('moments', VP), ('w_knn', VP), ('b_knn', VP), ('gnk_gamma', VP), ('gnk_beta', VP),
-                ('preluk', VP), ('preluk_host', C.c_float), ('kfeat', VP), ('flow', VP), ('w_cf', VP), ('b_cf', VP),
-                ('cflow', VP), ('B', C.c_int), ('N', C.c_int)]
+def _decls(text, structs, what, arrays):
+    """`<type> <declarator>[, <declarator> ...]` -> [Decl]; `what` names the declaration in errors."""
+    m = _TYPE.fullmatch(text)
+    if not m:
+        raise PvraftError(f'{HEADER_PATH}: cannot read `{text.strip()}` in {what}')
+    base, out = m.group(1), []
+    for d in m.group(2).split(','):
+        dm = _DECLARATOR.fullmatch(d)
+        if not dm or (dm.group(3) and not arrays):
+            raise PvraftError(f'{HEADER_PATH}: cannot read `{text.strip()}` in {what}')
+        star, name, length = dm.group(1), dm.group(2), int(dm.group(3) or 1)
+        if star:
+            if base not in _POINTEES and base not in structs:
+                raise PvraftError(f'{HEADER_PATH}: pointer to unknown type `{base}` in {what}')
+            ctype, pointee = C.c_void_p, base
+        else:
+            if base not in _SCALARS:
+                raise PvraftError(f'{HEADER_PATH}: unknown type `{base}` in {what}')
+            ctype, pointee = _SCALARS[base], None
+        name = name + '_' if keyword.iskeyword(name) else name
+        out.append(Decl(name, ctype * length if length > 1 else ctype, pointee, length))
+    return out
 
 
-class CorrFeatArgs(C.Structure):
-    _fields_ = [('y1', VP), ('y1_stats', VP), ('gn1_gamma', VP), ('gn1_beta', VP), ('prelu1', VP), ('w_out', VP),
-                ('b_out', VP), ('knn_sel', VP), ('moments', VP), ('w_knn', VP), ('b_knn', VP), ('gnk_gamma', VP),
-                ('gnk_beta', VP), ('preluk', VP), ('w_kout', VP), ('b_kout', VP), ('corr_feat', VP), ('corr_in', VP),
-                ('flow', VP), ('w_cc', VP), ('b_cc', VP), ('w_cf', VP), ('b_cf', VP), ('w_cm', VP), ('b_cm', VP),
-                ('motion', VP), ('B', C.c_int), ('N', C.c_int)]
+def parse_header(text):
+    """Header text -> (functions {name: (restype, [Decl])}, structs {name: [Decl]}), in declaration order."""
+    text = re.sub(r'/\*.*?\*/', ' ', text, flags=re.S)      # a comment ends at its first */
+    text = re.sub(r'^[ \t]*#.*$', ' ', text, flags=re.M)
+    functions, structs = {}, {}
+    pos = 0
+    while text[pos:].strip():
+        m = _FORM.match(text, pos)
+        if not m:
+            raise PvraftError(f'{HEADER_PATH}: unsupported declaration `{text[pos:].strip().splitlines()[0]}`')
+        pos = m.end()
+        if m.group('struct'):
+            what = f'struct {m.group("struct")}'
+            structs[m.group('struct')] = [d for line in m.group('fields').split(';') if line.strip()
+                                          for d in _decls(line, structs, what, arrays=True)]
+        elif m.group('fn'):
+            name, ret, params = m.group('fn'), re.sub(r'\s*\*', '*', m.group('ret').strip()), m.group('params').strip()
+            if ret not in _RETURNS:
+                raise PvraftError(f'{HEADER_PATH}: unsupported return type `{ret}` of {name}')
+            functions[name] = (_RETURNS[ret], [] if params == 'void' else
+                               [d for p in params.split(',') for d in _decls(p, structs, name, arrays=False)])
+    return functions, structs
 
 
-class GruArgs(C.Structure):
-    _fields_ = [('net', VP), ('inp', VP), ('motion', VP), ('w_z', VP), ('b_z', VP), ('w_r', VP), ('b_r', VP),
-                ('w_q', VP), ('b_q', VP), ('net_out', VP), ('B', C.c_int), ('N', C.c_int)]
+def _class_name(struct):
+    """pvraft_tc_linear_args -> TcLinearArgs; pvraft_corrfeat_args -> CorrFeatArgs, pvraft_flowout_args -> FlowOutArgs."""
+    stem = struct[len('pvraft_'):-len('_args')]
+    return {'corrfeat': 'CorrFeat', 'flowout': 'FlowOut'}.get(stem, stem.title().replace('_', '')) + 'Args'
 
 
-class FlowOutArgs(C.Structure):
-    _fields_ = [('z3', VP), ('z3_stats', VP), ('gn3_gamma', VP), ('gn3_beta', VP), ('net', VP), ('w_c1', VP),
-                ('b_c1', VP), ('w_o0', VP), ('b_o0', VP), ('w_o2', VP), ('b_o2', VP), ('coords1', VP),
-                ('coords2', VP), ('delta', VP), ('coords2_out', VP), ('flow_out', VP), ('B', C.c_int), ('N', C.c_int)]
-
-
-_SIGNATURES = {
-    'pvraft_version': (C.c_int, []),
-    'pvraft_last_error_string': (C.c_char_p, []),
-    'pvraft_device_info': (C.c_int, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
-    'pvraft_corr_matmul_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
-    'pvraft_corr_matmul_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_tf32_split_fwd': (C.c_int, [VP, C.c_int64, VP, VP, VP]),
-    'pvraft_corr_matmul_window_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                                C.c_int, VP, C.c_int64, VP]),
-    'pvraft_corr_topk_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_corr_topk_window_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, VP, VP, VP, C.c_int64, VP]),
-    'pvraft_corr_reorder': (C.c_int, [VP, VP, C.c_int64, C.c_int, VP, VP, VP]),
-    'pvraft_xyz_pad_fwd': (C.c_int, [VP, C.c_int64, VP, VP]),
-    'pvraft_corr_lookup_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                         VP, C.c_int, VP, VP, VP, VP, VP, VP]),
-    'pvraft_corr_lookup_bf16_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                              VP, C.c_int, VP, VP, VP, VP, VP, VP]),
-    'pvraft_corr_lookup_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_corr_lookup_table_in_smem': (C.c_int, [C.c_int, C.c_int]),
-    'pvraft_corr_state_pack_bf16': (C.c_int, [VP, VP, C.c_int64, VP, VP, VP]),
-    'pvraft_linear_fwd': (C.c_int, [C.POINTER(LinearArgs), VP, VP]),
-    'pvraft_linear_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_tc_linear_fwd': (C.c_int, [C.POINTER(TcLinearArgs), VP, VP]),
-    'pvraft_tc_linear_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_update_chain_fwd': (C.c_int, [C.POINTER(UpdateChainArgs), VP]),
-    'pvraft_tc_weight_split':(C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_tc_weight_bf16': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP]),
-    'pvraft_gn_act_fwd': (C.c_int, [VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int,
-                                    C.c_int, VP, VP, VP]),
-    'pvraft_corr_feature_fwd': (C.c_int, [C.POINTER(CorrFeatArgs), VP]),
-    'pvraft_knn_branch_fwd': (C.c_int, [C.POINTER(KnnBranchArgs), VP]),
-    'pvraft_point_order_fwd': (C.c_int, [VP, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_gru_fwd': (C.c_int, [C.POINTER(GruArgs), VP]),
-    'pvraft_setconv_edge_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP, VP]),
-    'pvraft_setconv_edge_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_edge_plan_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, VP, VP]),
-    'pvraft_edge_plan_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_flow_out_fwd': (C.c_int, [C.POINTER(FlowOutArgs), VP]),
-    'pvraft_knn_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_knn_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
-    'pvraft_linear_wgrad': (C.c_int, [VP, VP, C.c_int64, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP]),
-    'pvraft_linear_wgrad_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_tc_wgrad_bf16': (C.c_int, [VP, VP, C.c_int64, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP]),
-    'pvraft_tc_wgrad_bf16_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_gn_act_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int64, C.c_int, VP, VP, VP, VP,
-                                    VP, VP, VP, VP, VP]),
-    'pvraft_gn_act_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_linear_bwd_small': (C.c_int, [VP, VP, VP, C.c_int64, C.c_int, C.c_int, C.c_int, VP, C.c_int, VP, VP, VP, VP]),
-    'pvraft_linear_bwd_small_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_gn_act_maxk_fwd': (C.c_int, [VP, VP, VP, VP, C.c_double, C.c_int, C.c_float, C.c_int, C.c_int64, C.c_int, VP, VP, VP, VP]),
-    'pvraft_edge_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_edge_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_edge_bwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_edge_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
-    'pvraft_maxk_fwd': (C.c_int, [VP, C.c_int64, C.c_int, VP, VP, VP]),
-    'pvraft_maxk_bwd': (C.c_int, [VP, VP, C.c_int64, C.c_int, VP, VP]),
-    'pvraft_corr_lookup_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_int, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                         VP, VP]),
-    'pvraft_corr_lookup_xyz_bwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_corr_lookup_xyz_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_corr_init_bwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
-    'pvraft_corr_init_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
-    'pvraft_flow_metrics_fwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, VP]),
-    'pvraft_flow_metrics_det_workspace_bytes': (C.c_int64, []),
-    'pvraft_flow_l1_bwd': (C.c_int, [VP, VP, VP, C.c_int64, VP, VP, C.c_float, VP, VP]),
-    'pvraft_chamfer_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP]),
-    'pvraft_chamfer_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_chamfer_bwd': (C.c_int, [VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
-    'pvraft_chamfer_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
-    'pvraft_flow_smooth_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_flow_smooth_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_flow_smooth_bwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_flow_smooth_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_cloud_laplacian_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP]),
-    'pvraft_cloud_laplacian_bwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_cloud_laplacian_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_laplacian_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP]),
-    'pvraft_laplacian_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_laplacian_bwd': (C.c_int, [VP, VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP,
-                                       VP]),
-    'pvraft_laplacian_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
-    'pvraft_flow_propagate_fwd':(C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_flow_propagate_grid_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP]),
-    'pvraft_grid_index_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_grid_index_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, VP, VP]),
-    'pvraft_chamfer_grid_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
-    'pvraft_chamfer_grid_fwd': (C.c_int, [VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP, VP]),
-    'pvraft_laplacian_grid_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP,
-                                            VP]),
-    'pvraft_flow_consistency_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, VP, VP,
-                                              VP, VP, VP, VP]),
-    'pvraft_flow_consistency_fwd_det_workspace_bytes': (C.c_int64, [C.c_int]),
-    'pvraft_flow_consistency_grid_fwd': (C.c_int, [VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, VP,
-                                                   VP, VP, VP, VP, VP, VP]),
-    'pvraft_flow_consistency_bwd': (C.c_int, [VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP, VP,
-                                              VP]),
-    'pvraft_flow_consistency_bwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
-    'pvraft_euclidean_clusters_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int, VP, VP, VP, VP,
-                                                VP]),
-    'pvraft_euclidean_clusters_workspace_bytes': (C.c_int64, [C.c_int, C.c_int]),
-    'pvraft_rigid_objects_fwd': (C.c_int, [VP, VP, VP, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int, VP, VP, VP, VP,
-                                           VP, VP, VP, VP, VP, VP, VP]),
-    'pvraft_rigid_objects_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
-    'pvraft_rigid_objects_fwd_det_workspace_bytes': (C.c_int64, [C.c_int, C.c_int, C.c_int]),
-    'pvraft_rigid_objects_bwd': (C.c_int, [VP, VP, VP, VP, VP, VP, VP, C.c_int, C.c_int, C.c_int, VP, VP, VP]),
-    'pvraft_sizeof': (C.c_int, [C.c_int]),
-    'pvraft_transpose_fwd': (C.c_int, [VP, C.c_int, C.c_int, C.c_int, VP, VP]),
-}
+with open(HEADER_PATH) as _f:
+    FUNCTIONS, STRUCT_FIELDS = parse_header(_f.read())
+# the argument structs as ctypes classes, by their C name and under their Python names (LinearArgs, TcLinearArgs, ...)
+STRUCTS = {s: type(_class_name(s), (C.Structure,), {'_fields_': [(d.name, d.ctype) for d in fields]})
+           for s, fields in STRUCT_FIELDS.items()}
+globals().update({cls.__name__: cls for cls in STRUCTS.values()})
+_SIGNATURES = {name: (res, [d.ctype for d in params]) for name, (res, params) in FUNCTIONS.items()}
 EXPORTS = tuple(_SIGNATURES)
 
 _lib = None
 _lock = threading.Lock()
-
-
-class PvraftError(RuntimeError):
-    pass
 
 
 def lib():

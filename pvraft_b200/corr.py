@@ -13,7 +13,7 @@ properties for API parity.
 import torch
 import torch.nn as nn
 
-from . import _lib, ops
+from . import ops
 from .ops import ACT_LRELU, ACT_NONE, ACT_RELU
 
 
@@ -141,26 +141,13 @@ class CorrBlock(nn.Module):
         return ops.corr_lookup(self.corr_val, self.corr_idx, self._xyz2p, coords.detach().contiguous().float(),
                                self.num_levels, self.base_scale, **kw)
 
-    def feature_args(self, lk, y1, y1_stats, b, n):
-        oc, kc = self.out_conv, self.knn_conv
-        a = _lib.CorrFeatArgs()
-        a.y1, a.y1_stats = ops._p(y1), ops._p(y1_stats, torch.float64)
-        a.gn1_gamma, a.gn1_beta, a.prelu1 = ops._p(_w(oc[1].weight)), ops._p(_w(oc[1].bias)), ops._p(_w(oc[2].weight))
-        a.w_out, a.b_out = ops._p(_w(oc[3].weight)), ops._p(_w(oc[3].bias))
-        a.knn_sel, a.moments = ops._p(lk['knn_sel']), ops._p(lk['moments'], torch.float64)
-        a.w_knn, a.b_knn = ops._p(_w(kc[0].weight)), ops._p(_w(kc[0].bias))
-        a.gnk_gamma, a.gnk_beta, a.preluk = ops._p(_w(kc[1].weight)), ops._p(_w(kc[1].bias)), ops._p(_w(kc[2].weight))
-        a.w_kout, a.b_kout = ops._p(_w(self.knn_out.weight)), ops._p(_w(self.knn_out.bias))
-        a.B, a.N = b, n
-        return a
-
     def feature_point_major(self, coords, motion_args=None):
         """coords [B,N,3] -> correlation feature [B,N,64] (point-major).  `motion_args` lets
         UpdateBlock fuse its MotionEncoder into the same launch (see update.py)."""
         b, n, _ = coords.shape
         nvox = self.num_levels * 27
         stats = ops.new_stats(b, coords.device, 1)
-        oc = self.out_conv
+        oc, kc = self.out_conv, self.knn_conv
         kpad = (nvox + 31) // 32 * 32
         if ops.tc_supported(n) and kpad - nvox <= 32:
             # out_conv[0] on wgmma: the lookup pads the voxel rows to a multiple of 32 channels (zeros)
@@ -170,9 +157,12 @@ class CorrBlock(nn.Module):
         else:
             lk = self.lookup(coords)
             y1 = ops.linear(lk['vox'], _w(oc[0].weight), _w(oc[0].bias), w_cin=nvox, out_stats=stats[0], out_act=ACT_NONE)
-        a = self.feature_args(lk, y1, stats[0], b, n)
         corr = torch.empty(b, n, 64, dtype=torch.float32, device=coords.device)
-        a.corr_feat = ops._p(corr)
+        a = ops.pack.CorrFeatArgs(y1=y1, y1_stats=stats[0], gn1_gamma=_w(oc[1].weight), gn1_beta=_w(oc[1].bias),
+                                  prelu1=_w(oc[2].weight), w_out=_w(oc[3].weight), b_out=_w(oc[3].bias), knn_sel=lk['knn_sel'],
+                                  moments=lk['moments'], w_knn=_w(kc[0].weight), b_knn=_w(kc[0].bias), gnk_gamma=_w(kc[1].weight),
+                                  gnk_beta=_w(kc[1].bias), preluk=_w(kc[2].weight), w_kout=_w(self.knn_out.weight),
+                                  b_kout=_w(self.knn_out.bias), corr_feat=corr, B=b, N=n)
         keep = [lk, y1, stats, corr]
         if motion_args is not None:
             motion_args(a, keep)
@@ -217,17 +207,13 @@ class CorrBlock(nn.Module):
         lk = self.lookup(coords, vox_ld=kpad)
         y1 = ops.tc_linear([lk['vox']], ops.tc_weights(oc[0].weight, cols=nvox, k_pad=kpad), _w(oc[0].bias), out_stats=stats[0])
         # kNN branch (ALU) + flow embedding
-        a = _lib.KnnBranchArgs()
-        a.knn_sel, a.moments = ops._p(lk['knn_sel']), ops._p(lk['moments'], torch.float64)
-        a.w_knn, a.b_knn = ops._p(_w(kc[0].weight)), ops._p(_w(kc[0].bias))
-        a.gnk_gamma, a.gnk_beta, a.preluk = ops._p(_w(kc[1].weight)), ops._p(_w(kc[1].bias)), ops._p(_w(kc[2].weight))
-        a.preluk_host = ops.derived((kc[2].weight,), 'slope', lambda w: float(w.detach().reshape(-1)[0]))
+        preluk_host = ops.derived((kc[2].weight,), 'slope', lambda w: float(w.detach().reshape(-1)[0]))
         kfeat = torch.empty(b, n, 64, dtype=torch.float32, device=dev)
         cflow = torch.empty(b, n, 64, dtype=torch.float32, device=dev)
-        a.kfeat, a.flow, a.cflow = ops._p(kfeat), ops._p(flow), ops._p(cflow)
-        a.w_cf, a.b_cf = ops._p(_w(me.conv_flow.weight)), ops._p(_w(me.conv_flow.bias))
-        a.B, a.N = b, n
-        ops.knn_branch(a)
+        ops.knn_branch(ops.pack.KnnBranchArgs(knn_sel=lk['knn_sel'], moments=lk['moments'], w_knn=_w(kc[0].weight),
+                                              b_knn=_w(kc[0].bias), gnk_gamma=_w(kc[1].weight), gnk_beta=_w(kc[1].bias),
+                                              preluk=_w(kc[2].weight), preluk_host=preluk_host, kfeat=kfeat, flow=flow,
+                                              cflow=cflow, w_cf=_w(me.conv_flow.weight), b_cf=_w(me.conv_flow.bias), B=b, N=n))
         gn = dict(in_stats=stats[0], in_gamma=_w(oc[1].weight), in_beta=_w(oc[1].bias), in_count=float(n) * 16.0, in_act=ACT_LRELU,
                   in_slope=ops.derived((oc[2].weight,), 'slope', lambda w: float(w.detach().reshape(-1)[0])))
         return y1, kfeat, cflow, gn

@@ -7,20 +7,14 @@ from typing import NamedTuple
 import torch
 
 from . import ops
-from ._lib import lib
+
+
+_metrics = ops.flow_metrics   # acc [8] f64 of pvraft_flow_metrics_fwd: the sums behind the masked L1 loss and the EPE metrics
 
 
 def _gt(batch):
     mask, flow = batch['ground_truth'][0], batch['ground_truth'][1]
     return mask[..., 0].contiguous().float(), flow.contiguous().float()
-
-
-def _metrics(est, gt, mask):
-    acc = torch.zeros(8, dtype=torch.float64, device=est.device)
-    ws = ops._det_workspace(lib().pvraft_flow_metrics_det_workspace_bytes, device=est.device)
-    ops._count(lib().pvraft_flow_metrics_fwd(ops._p(est), ops._p(gt), ops._p(mask), est.numel() // 3, acc.data_ptr(), ops._p(ws, torch.uint8),
-                                             ops._stream()), 'flow_metrics')
-    return acc
 
 
 class MaskedL1Fn(torch.autograd.Function):
@@ -37,10 +31,7 @@ class MaskedL1Fn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         est, gt, mask, acc = ctx.saved_tensors
-        d = torch.empty_like(est)
-        ops._count(lib().pvraft_flow_l1_bwd(ops._p(est), ops._p(gt), ops._p(mask), est.numel() // 3, acc.data_ptr(),
-                                            ops._p(g.contiguous().float().reshape(1)), ctx.weight, ops._p(d), ops._stream()), 'flow_l1_bwd')
-        return d, None, None, None
+        return ops.flow_l1_bwd(est, gt, mask, acc, g.contiguous().float().reshape(1), ctx.weight), None, None, None
 
 
 def compute_loss(est_flow, batch):

@@ -3,9 +3,14 @@
 PyTorch is plumbing here: it owns device memory and the CUDA stream; every arithmetic step of the
 hot path happens inside libpvraft_b200.so.  All wrappers require contiguous CUDA tensors and raise
 on anything else -- there is deliberately no CPU / eager fallback.
+
+Every call into the library goes through `abi` (one callable per entry point, `abi.knn_fwd` for pvraft_knn_fwd) and
+every argument struct is filled by `pack`: both check each tensor against the pointee type the header declares for its
+parameter or field, so the wrappers pass tensors and never restate a dtype.
 """
 import ctypes as C
 import threading
+import types
 import weakref
 from typing import NamedTuple
 
@@ -25,26 +30,101 @@ def _stream():
 
 
 def _p(t, dtype=torch.float32):
-    if t is None:
-        return None
-    if not torch.is_tensor(t):
-        raise TypeError(f'expected a tensor, got {type(t)}')
+    """The device address of tensor t, checked: a contiguous CUDA tensor on the current device of dtype `dtype` (or of one
+    of them, for a tuple).  None (NULL) and anything that is not a tensor (a ctypes byref object, a plain address) pass
+    as they are."""
+    if t is None or not isinstance(t, torch.Tensor):
+        return t
     if not t.is_cuda:
         raise _lib.PvraftError('pvraft_b200 kernels need CUDA tensors (no CPU fallback exists)')
     if t.device.index != torch.cuda.current_device():
         raise _lib.PvraftError(f'tensor on {t.device} but the current CUDA device is {torch.cuda.current_device()}: the kernels '
                                'launch on the current device -- wrap the call in `with torch.cuda.device(t.device):`')
-    if t.dtype != dtype:
+    if t.dtype != dtype and not (isinstance(dtype, tuple) and t.dtype in dtype):
         raise TypeError(f'expected {dtype}, got {t.dtype}')
     if not t.is_contiguous():
         raise ValueError('expected a contiguous tensor')
     return t.data_ptr()
 
 
+# The tensor dtype a pointer of the header points to: the bf16 state and bf16 weights travel as uint16_t, and so do the
+# uint16 candidate ids (held in an int16 tensor); void* is byte scratch (workspaces, the edge plan).
+_DTYPES = {'float': torch.float32, 'double': torch.float64, 'int32_t': torch.int32, 'int': torch.int32, 'uint8_t': torch.uint8,
+           'int8_t': torch.int8, 'uint16_t': (torch.bfloat16, torch.int16), 'void': torch.uint8}
+
+
 def _count(rc, what):
     global launch_count
     check(rc, what)
     launch_count += 1
+
+
+def _convert(i, d, value, namespace):
+    """The expression that converts `value` for parameter or field i, declared as d: a scalar as it is (ctypes converts
+    it), a struct of the C ABI by reference, any other pointer through _p with its pointee's dtype (namespace collects
+    the constants the expression names)."""
+    if d.pointee is None:
+        return value
+    if d.pointee in _lib.STRUCTS:
+        namespace[f'_t{i}'] = _lib.STRUCTS[d.pointee]
+        return f'_byref({value}) if isinstance({value}, _t{i}) else {value}'
+    namespace[f'_d{i}'] = _DTYPES[d.pointee]
+    return f'_p({value}, _d{i})'
+
+
+def _compile(src, name, namespace):
+    """The function `name` defined by the source text src, its defaults taken from namespace and its globals this module's
+    (so that it reads lib, _p, _stream and launch_count at call time, as a hand-written wrapper does)."""
+    namespace['_byref'] = C.byref
+    signature = ', '.join(f'{k}={k}' for k in namespace)
+    exec(src.replace('@DEFAULTS@', signature), globals(), namespace)
+    return namespace[name]
+
+
+# The weight conversions behind tc_weights run once per parameter version and have never been part of launch_count.
+_UNCOUNTED = ('pvraft_tc_weight_split', 'pvraft_tc_weight_bf16')
+
+
+def _entry(name, params):
+    """The Python form of the entry point `name`: a function of its parameters (less `void* stream`), positional, that
+    converts each argument (_convert) and calls the library.  An entry point whose last parameter is `void* stream`
+    launches: the call appends the current stream, raises on a non-zero return code and counts the launch; any other
+    returns what the library returns.  It is generated once, from the header's declaration, so that a call costs what a
+    hand-written call costs."""
+    launches = bool(params) and params[-1].name == 'stream' and params[-1].pointee == 'void'
+    params = params[:-1] if launches else params
+    namespace = {}
+    args = [f'a{i}' for i in range(len(params))]
+    call = ', '.join(_convert(i, d, f'a{i}', namespace) for i, d in enumerate(params))
+    if launches:
+        body = f"{'check' if name in _UNCOUNTED else '_count'}(lib().{name}({call}{', ' if params else ''}_stream()), {name!r})"
+    else:
+        body = f'return lib().{name}({call})'
+    return _compile(f"def {name}({', '.join(args + ['*'])}, @DEFAULTS@):\n    {body}\n", name, namespace)
+
+
+def _packer(struct, fields):
+    """The function that fills an argument struct -- the one given, or a new one -- from keyword arguments named as its
+    fields, each converted as _entry converts a parameter of the same type; an array field takes a sequence that fills its
+    first entries.  A field not given, or given as None, is left as it is (0 / NULL in a new struct); an unknown one
+    raises TypeError.  Generated once per struct, as _entry is."""
+    namespace = {'_S': struct}
+    lines = ['if _s is None:\n        _s = _S()']
+    for i, d in enumerate(fields):
+        if d.length > 1:
+            lines.append(f'if {d.name} is not None:\n        for _i, _v in enumerate({d.name}):\n'
+                         f'            _s.{d.name}[_i] = {_convert(i, d, "_v", namespace)}')
+        else:
+            lines.append(f'if {d.name} is not None:\n        _s.{d.name} = {_convert(i, d, d.name, namespace)}')
+    lines.append('return _s')
+    names = ', '.join(f'{d.name}=None' for d in fields)
+    return _compile(f'def {struct.__name__}(_s=None, /, *, {names}, @DEFAULTS@):\n    ' + '\n    '.join(lines) + '\n',
+                    struct.__name__, namespace)
+
+
+# abi.<name>(...) calls pvraft_<name>; pack.<StructName>([struct], field=...) fills an argument struct (pack.TcLinearArgs).
+abi = types.SimpleNamespace(**{name[len('pvraft_'):]: _entry(name, params) for name, (_, params) in _lib.FUNCTIONS.items()})
+pack = types.SimpleNamespace(**{cls.__name__: _packer(cls, _lib.STRUCT_FIELDS[s]) for s, cls in _lib.STRUCTS.items()})
 
 
 def deterministic():
@@ -122,8 +202,7 @@ def corr_reorder(val, idx):
     """Bank-aware permutation of every row of the truncated state (val [B,N,K] f32, idx [B,N,K] int32)."""
     b, n, k = val.shape
     val_out, idx_out = torch.empty_like(val), torch.empty_like(idx)
-    _count(lib().pvraft_corr_reorder(_p(val), _p(idx, torch.int32), b * n, k, _p(val_out), _p(idx_out, torch.int32), _stream()),
-           'corr_reorder')
+    abi.corr_reorder(val, idx, b * n, k, val_out, idx_out)
     return val_out, idx_out
 
 
@@ -136,8 +215,7 @@ def corr_state_pack_bf16(val, idx, m=None):
         raise ValueError(f'uint16 candidate ids need a second cloud of at most 65536 points (N2 <= 65536), got {m}')
     v16 = torch.empty(val.shape, dtype=torch.bfloat16, device=val.device)
     i16 = torch.empty(idx.shape, dtype=torch.int16, device=idx.device)
-    _count(lib().pvraft_corr_state_pack_bf16(_p(val), _p(idx, torch.int32), val.numel(), _p(v16, torch.bfloat16), _p(i16, torch.int16),
-                                             _stream()), 'corr_state_pack_bf16')
+    abi.corr_state_pack_bf16(val, idx, val.numel(), v16, i16)
     return v16, i16
 
 
@@ -148,9 +226,8 @@ def corr_matmul(fmap1_pm, fmap2_pm):
     if fmap2_pm.shape != (b, m, c):
         raise ValueError(f'corr_matmul: feature maps {tuple(fmap1_pm.shape)} and {tuple(fmap2_pm.shape)}')
     corr = torch.empty(b, n, m, dtype=torch.float32, device=fmap1_pm.device)
-    ws = torch.empty(int(lib().pvraft_corr_matmul_workspace_bytes(b, n, m, c)), dtype=torch.uint8, device=fmap1_pm.device)
-    _count(lib().pvraft_corr_matmul_fwd(_p(fmap1_pm), _p(fmap2_pm), b, n, m, c, _p(corr), _p(ws, torch.uint8), _stream()),
-           'corr_matmul')
+    ws = _workspace(abi.corr_matmul_workspace_bytes(b, n, m, c), fmap1_pm.device)
+    abi.corr_matmul_fwd(fmap1_pm, fmap2_pm, b, n, m, c, corr, ws)
     return corr
 
 
@@ -159,7 +236,7 @@ def corr_topk(corr, k):
     b, n, m = corr.shape
     val = torch.empty(b, n, k, dtype=torch.float32, device=corr.device)
     idx = torch.empty(b, n, k, dtype=torch.int32, device=corr.device)
-    _count(lib().pvraft_corr_topk_fwd(_p(corr), b, n, m, k, _p(val), _p(idx, torch.int32), _stream()), 'corr_topk')
+    abi.corr_topk_fwd(corr, b, n, m, k, val, idx)
     return val, idx
 
 
@@ -250,7 +327,7 @@ def corr_build(fmap1_pm, fmap2_pm, k, plan=None):
     ws_b = torch.empty(2, b, mpad, c, dtype=torch.float32, device=dev)
     for ws, f, rows_f in ((ws_a, fmap1_pm, n), (ws_b, fmap2_pm, m)):
         for s in range(b):
-            _count(lib().pvraft_tf32_split_fwd(_p(f[s]), rows_f * c, _p(ws[0, s]), _p(ws[1, s]), _stream()), 'tf32_split')
+            abi.tf32_split_fwd(f[s], rows_f * c, ws[0, s], ws[1, s])
     nw = len(plan.windows)
     wk = nw * k
     rows = max(r for _, r in plan.row_blocks)
@@ -260,15 +337,13 @@ def corr_build(fmap1_pm, fmap2_pm, k, plan=None):
     val = torch.empty(b, n, k, dtype=torch.float32, device=dev)
     idx = torch.empty(b, n, k, dtype=torch.int32, device=dev)
     for s in range(b):
-        split = [_p(ws_a[0, s]), _p(ws_a[1, s]), _p(ws_b[0, s]), _p(ws_b[1, s])]
+        split = (ws_a[0, s], ws_a[1, s], ws_b[0, s], ws_b[1, s])
         for r0, nr in plan.row_blocks:
             for j, (c0, nc) in enumerate(plan.windows):
-                _count(lib().pvraft_corr_matmul_window_fwd(*split, 1, npad, mpad, c, r0, nr, c0, nc, _p(slab), plan.ld, _stream()),
-                       'corr_matmul_window')
-                _count(lib().pvraft_corr_topk_window_fwd(_p(slab), nr, nc, plan.ld, k, c0, None, _p(cand_val) + 4 * j * k,
-                                                         _p(cand_idx, torch.int32) + 4 * j * k, wk, _stream()), 'corr_topk_window')
-            _count(lib().pvraft_corr_topk_window_fwd(_p(cand_val), nr, wk, wk, k, 0, _p(cand_idx, torch.int32), _p(val[s, r0:r0 + nr]),
-                                                     _p(idx[s, r0:r0 + nr], torch.int32), k, _stream()), 'corr_topk_merge')
+                abi.corr_matmul_window_fwd(*split, 1, npad, mpad, c, r0, nr, c0, nc, slab, plan.ld)
+                # window j's candidates: columns j*K.. of every row (row stride W*K), addressed from the flat buffers
+                abi.corr_topk_window_fwd(slab, nr, nc, plan.ld, k, c0, None, cand_val.view(-1)[j * k:], cand_idx.view(-1)[j * k:], wk)
+            abi.corr_topk_window_fwd(cand_val, nr, wk, wk, k, 0, cand_idx, val[s, r0:r0 + nr], idx[s, r0:r0 + nr], k)
     return val, idx
 
 
@@ -298,7 +373,7 @@ def xyz_pad(xyz):
     """[B,N,3] -> [B,N,4] = (x,y,z,0): the lookup kernel's gather table (one 128-bit load per candidate), built once per forward."""
     b, n, _ = xyz.shape
     out = torch.empty(b, n, 4, dtype=torch.float32, device=xyz.device)
-    _count(lib().pvraft_xyz_pad_fwd(_p(xyz), b * n, _p(out), _stream()), 'xyz_pad')
+    abi.xyz_pad_fwd(xyz, b * n, out)
     return out
 
 
@@ -320,12 +395,10 @@ def corr_lookup(corr_val, corr_idx, xyz2_pad, coords, levels, base_scale, vox=No
         moments = new_stats(b, dev, 1).view(b, MOMENTS) if MOMENTS == 16 else torch.zeros(b, MOMENTS, dtype=torch.float64, device=dev)
     slots = torch.empty(b, n, KNN, dtype=torch.int32, device=dev) if want_slots else None
     cube = torch.empty(b, n, k, levels, dtype=torch.int8, device=dev) if want_cube else None
-    half = corr_val.dtype == torch.bfloat16   # reduced-precision state: bf16 values + uint16 ids (stored as int16)
-    state = (_p(corr_val, torch.bfloat16), _p(corr_idx, torch.int16)) if half else (_p(corr_val), _p(corr_idx, torch.int32))
-    fn = lib().pvraft_corr_lookup_bf16_fwd if half else lib().pvraft_corr_lookup_fwd
-    ws = _det_workspace(lib().pvraft_corr_lookup_det_workspace_bytes, b, device=dev)
-    _count(fn(*state, _p(xyz2_pad), _p(coords), b, n, m, k, levels, float(base_scale), _p(vox), vox.shape[-1], _p(knn_sel),
-              _p(slots, torch.int32), _p(moments, torch.float64), _p(cube, torch.int8), _p(ws, torch.uint8), _stream()), 'corr_lookup')
+    # reduced-precision state: bf16 values + uint16 ids (stored as int16)
+    fn = abi.corr_lookup_bf16_fwd if corr_val.dtype == torch.bfloat16 else abi.corr_lookup_fwd
+    ws = _det_workspace(abi.corr_lookup_det_workspace_bytes, b, device=dev)
+    fn(corr_val, corr_idx, xyz2_pad, coords, b, n, m, k, levels, float(base_scale), vox, vox.shape[-1], knn_sel, slots, moments, cube, ws)
     return dict(vox=vox, knn_sel=knn_sel, moments=moments, knn_slot=slots, cube=cube)
 
 
@@ -338,11 +411,11 @@ def linear(x, weight, bias=None, *, cin=None, w_ld=0, w_cin=0, in_mode=IN_PLAIN,
     cout = weight.shape[0] if cout is None else cout
     if out is None:
         out = torch.empty(b, n, cout, dtype=torch.float32, device=x.device)
-    a = _lib.LinearArgs(_p(x), _p(in_min), _p(in_stats, torch.float64), _p(in_gamma), _p(in_beta), float(in_count),
-                        in_mode, in_act, float(in_slope), _p(weight), int(w_ld), int(w_cin), _p(bias), _p(residual), out_act,
-                        _p(out), _p(out_stats, torch.float64), b, n, cin, cout)
-    ws = _det_workspace(lib().pvraft_linear_det_workspace_bytes, b, device=x.device) if out_stats is not None else None
-    _count(lib().pvraft_linear_fwd(C.byref(a), _p(ws, torch.uint8), _stream()), 'linear')
+    a = pack.LinearArgs(in_=x, in_min=in_min, in_stats=in_stats, in_gamma=in_gamma, in_beta=in_beta, in_count=float(in_count),
+                        in_mode=in_mode, in_act=in_act, in_slope=float(in_slope), weight=weight, w_ld=int(w_ld), w_cin=int(w_cin),
+                        bias=bias, residual=residual, out_act=out_act, out=out, out_stats=out_stats, B=b, N=n, cin=cin, cout=cout)
+    ws = _det_workspace(abi.linear_det_workspace_bytes, b, device=x.device) if out_stats is not None else None
+    abi.linear_fwd(a, ws)
     return out
 
 
@@ -388,11 +461,9 @@ def tc_weights(weights, col0=0, cols=None, k_pad=None, kcat=False, transposed=No
     r0 = 0
     for m in mats:
         if bf16:
-            check(lib().pvraft_tc_weight_bf16(_p(m.contiguous()), m.shape[0], ncols, ld, col0, m.shape[0], kp, hi[r0:].data_ptr(),
-                                              _stream()), 'tc_weight_bf16')
+            abi.tc_weight_bf16(m.contiguous(), m.shape[0], ncols, ld, col0, m.shape[0], kp, hi[r0:])
         else:
-            check(lib().pvraft_tc_weight_split(_p(m.contiguous()), m.shape[0], ncols, ld, col0, m.shape[0], kp,
-                                               hi[r0:].data_ptr(), lo[r0:].data_ptr(), _stream()), 'tc_weight_split')
+            abi.tc_weight_split(m.contiguous(), m.shape[0], ncols, ld, col0, m.shape[0], kp, hi[r0:], lo[r0:])
         r0 += m.shape[0]
     if len(_TC_WEIGHTS) > 512:
         _TC_WEIGHTS.clear()
@@ -430,12 +501,12 @@ def point_order(points):
     """[B,N,3] -> [B,N] int32: Morton order over the cells of the kNN grid, from the library's in-shared-memory sort
     (one launch; the torch formulation below costs ~40 launches)."""
     b, n, _ = points.shape
-    ws_bytes = int(lib().pvraft_knn_workspace_bytes(b, n))
+    ws_bytes = int(abi.knn_workspace_bytes(b, n))
     if ws_bytes <= 0 or n < 64 or n > KNN_SORT_MAX_N:
         return morton_order(points).to(torch.int32).contiguous()
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=points.device)
+    ws = _workspace(ws_bytes, points.device)
     perm = torch.empty(b, n, dtype=torch.int32, device=points.device)
-    _count(lib().pvraft_point_order_fwd(_p(points), b, n, _p(perm, torch.int32), _p(ws, torch.uint8), _stream()), 'point_order')
+    abi.point_order_fwd(points, b, n, perm, ws)
     return perm
 
 
@@ -472,31 +543,21 @@ def tc_linear(sources, w, bias=None, *, in_min=None, in_stats=None, in_gamma=Non
     cout = rows if cout is None else cout
     if out is None:
         out = torch.empty(b, n, cout + (3 if tail is not None else 0), dtype=torch.float32, device=sources[0].device)
-    a = _lib.TcLinearArgs()
-    for i, src in enumerate(sources):
-        a.in_[i] = _p(src)
-        a.in_channels[i] = src.shape[-1]
-    a.in_min, a.in_stats, a.in_gamma, a.in_beta = _p(in_min), _p(in_stats, torch.float64), _p(in_gamma), _p(in_beta)
-    a.in_count, a.in_act, a.in_slope = float(in_count), in_act, float(in_slope)
-    if lo is None:
-        a.w_bf16 = _p(hi, torch.bfloat16)
-    else:
-        a.w_hi, a.w_lo = _p(hi), _p(lo)
-    a.n_pad, a.cout = n_pad, cout
-    a.bias, a.bias2, a.out_act, a.residual = _p(bias), _p(bias2), out_act, _p(residual)
-    a.out, a.out2, a.h, a.z = _p(out), _p(out2), _p(h), _p(z)
-    a.out_stats, a.epilogue, a.B, a.N = _p(out_stats, torch.float64), epilogue, b, n
-    a.tail = _p(tail)
-    a.w3, a.b3, a.coords1, a.coords2 = _p(w3), _p(b3), _p(coords1), _p(coords2)
-    a.coords2_out, a.flow_out = _p(coords2_out), _p(flow_out)
+    # the bf16 form (lo None) sets w_bf16 in place of w_hi / w_lo
+    a = pack.TcLinearArgs(in_=sources, in_channels=[src.shape[-1] for src in sources], in_min=in_min, in_stats=in_stats,
+                          in_gamma=in_gamma, in_beta=in_beta, in_count=float(in_count), in_act=in_act, in_slope=float(in_slope),
+                          w_hi=None if lo is None else hi, w_lo=lo, w_bf16=hi if lo is None else None, n_pad=n_pad, cout=cout,
+                          bias=bias, bias2=bias2, out_act=out_act, residual=residual, out=out, out2=out2, h=h, z=z,
+                          out_stats=out_stats, epilogue=epilogue, B=b, N=n, tail=tail, w3=w3, b3=b3, coords1=coords1,
+                          coords2=coords2, coords2_out=coords2_out, flow_out=flow_out)
     # The kernel may fetch its parameters while the previous kernel drains (PDL) once they are settled: not during the
     # three tensor-core launches that follow a weight split or a re-derived folded parameter on this thread.
     pending = getattr(_TLS, 'unsettled', 0)
     a.params_settled = 1 if pending == 0 else 0
     if pending:
         _TLS.unsettled = pending - 1
-    ws = _det_workspace(lib().pvraft_tc_linear_det_workspace_bytes, b, device=out.device) if out_stats is not None else None
-    _count(lib().pvraft_tc_linear_fwd(C.byref(a), _p(ws, torch.uint8), _stream()), 'tc_linear')
+    ws = _det_workspace(abi.tc_linear_det_workspace_bytes, b, device=out.device) if out_stats is not None else None
+    abi.tc_linear_fwd(a, ws)
     return out
 
 
@@ -511,19 +572,15 @@ def update_chain(y1, gn, kfeat, cflow, flow, net, inp, weights, biases):
     Returns (net' [B,N,64], P [B,N,64])."""
     b, n, _ = net.shape
     net_out, p_out = torch.empty_like(net), torch.empty_like(net)
-    a = _lib.UpdateChainArgs()
-    a.y1, a.y1_stats = _p(y1), _p(gn['in_stats'], torch.float64)
-    a.gn_gamma, a.gn_beta, a.gn_count, a.gn_slope = _p(gn['in_gamma']), _p(gn['in_beta']), float(gn['in_count']), float(gn['in_slope'])
-    a.kfeat, a.cflow, a.flow, a.net, a.inp = _p(kfeat), _p(cflow), _p(flow), _p(net), _p(inp)
-    for i, (hi, lo, _, _) in enumerate(weights):
-        if lo is None:
-            a.w_bf16[i] = _p(hi, torch.bfloat16)
-        else:
-            a.w_hi[i], a.w_lo[i] = _p(hi), _p(lo)
-    a.b_cc, a.b_m, a.b_z, a.b_r, a.b_q = (_p(x) for x in biases)
-    a.net_out, a.p_out = _p(net_out), _p(p_out)
-    a.B, a.N, a.hidden, a.context, a.y1_channels = b, n, net.shape[-1], inp.shape[-1], y1.shape[-1]
-    _count(lib().pvraft_update_chain_fwd(C.byref(a), _stream()), 'update_chain')
+    b_cc, b_m, b_z, b_r, b_q = biases
+    abi.update_chain_fwd(pack.UpdateChainArgs(y1=y1, y1_stats=gn['in_stats'], gn_gamma=gn['in_gamma'], gn_beta=gn['in_beta'],
+                                              gn_count=float(gn['in_count']), gn_slope=float(gn['in_slope']), kfeat=kfeat,
+                                              cflow=cflow, flow=flow, net=net, inp=inp,
+                                              w_hi=[None if lo is None else hi for hi, lo, _, _ in weights],
+                                              w_lo=[lo for _, lo, _, _ in weights],
+                                              w_bf16=[hi if lo is None else None for hi, lo, _, _ in weights], b_cc=b_cc, b_m=b_m,
+                                              b_z=b_z, b_r=b_r, b_q=b_q, net_out=net_out, p_out=p_out, B=b, N=n,
+                                              hidden=net.shape[-1], context=inp.shape[-1], y1_channels=y1.shape[-1]))
     return net_out, p_out
 
 
@@ -531,8 +588,7 @@ def gn_act(x, stats, gamma, beta, count, act=ACT_LRELU, slope=0.1, transpose_out
     """slope_dev: optional one-element device tensor (a PReLU weight) the kernel reads instead of the scalar `slope`."""
     b, n, c = x.shape
     out = torch.empty((b, c, n) if transpose_out else (b, n, c), dtype=torch.float32, device=x.device)
-    _count(lib().pvraft_gn_act_fwd(_p(x), _p(stats, torch.float64), _p(gamma), _p(beta), float(count), act, float(slope),
-                                   b, n, c, int(transpose_out), _p(out), _p(slope_dev), _stream()), 'gn_act')
+    abi.gn_act_fwd(x, stats, gamma, beta, float(count), act, float(slope), b, n, c, int(transpose_out), out, slope_dev)
     return out
 
 
@@ -540,35 +596,38 @@ def transpose(x):
     """[B,R,C] -> [B,C,R] contiguous."""
     b, r, c = x.shape
     out = torch.empty(b, c, r, dtype=torch.float32, device=x.device)
-    _count(lib().pvraft_transpose_fwd(_p(x), b, r, c, _p(out), _stream()), 'transpose')
+    abi.transpose_fwd(x, b, r, c, out)
     return out
 
 
 def corr_feature(args):
-    _count(lib().pvraft_corr_feature_fwd(C.byref(args), _stream()), 'corr_feature')
+    """pvraft_corr_feature_fwd on an argument struct, pack.CorrFeatArgs(...)."""
+    abi.corr_feature_fwd(args)
 
 
 def knn_branch(args):
-    _count(lib().pvraft_knn_branch_fwd(C.byref(args), _stream()), 'knn_branch')
+    """pvraft_knn_branch_fwd on an argument struct, pack.KnnBranchArgs(...)."""
+    abi.knn_branch_fwd(args)
 
 
 def gru(args):
-    _count(lib().pvraft_gru_fwd(C.byref(args), _stream()), 'gru')
+    """pvraft_gru_fwd on an argument struct, pack.GruArgs(...)."""
+    abi.gru_fwd(args)
 
 
 def flow_out(args):
-    _count(lib().pvraft_flow_out_fwd(C.byref(args), _stream()), 'flow_out')
+    """pvraft_flow_out_fwd on an argument struct, pack.FlowOutArgs(...)."""
+    abi.flow_out_fwd(args)
 
 
 def edge_plan(nbr, order=None):
     """The SetConv edge kernel's gather plan of the kNN graph nbr [B,N,32] processed in `order` ([B,N] or None):
     uint8 [B, tiles per sample, record bytes], sample-major, so plan[:b] is the plan of nbr[:b] (csrc/edge_plan.cuh)."""
     b, n, _ = nbr.shape
-    rec = int(lib().pvraft_edge_plan_bytes(1, 1))
-    tiles = int(lib().pvraft_edge_plan_bytes(1, n)) // rec
+    rec = int(abi.edge_plan_bytes(1, 1))
+    tiles = int(abi.edge_plan_bytes(1, n)) // rec
     plan = torch.empty(b, tiles, rec, dtype=torch.uint8, device=nbr.device)
-    _count(lib().pvraft_edge_plan_fwd(_p(nbr, torch.int32), _p(order, torch.int32), b, n, _p(plan, torch.uint8), _stream()),
-           'edge_plan')
+    abi.edge_plan_fwd(nbr, order, b, n, plan)
     return plan
 
 
@@ -581,12 +640,10 @@ def setconv_edge(fc1p, nbr, edge_feats, w_fc1, cin, stats, ymax=None, ymin=None,
         ymin = torch.empty_like(fc1p)
     if plan is None:
         plan = edge_plan(nbr, order)
-    elif plan.shape[0] != b or plan.numel() != int(lib().pvraft_edge_plan_bytes(b, n)):
+    elif plan.shape[0] != b or plan.numel() != int(abi.edge_plan_bytes(b, n)):
         raise ValueError(f'edge plan of shape {tuple(plan.shape)} does not belong to a graph of {b} x {n} points')
-    ws = _det_workspace(lib().pvraft_setconv_edge_det_workspace_bytes, b, device=fc1p.device)
-    _count(lib().pvraft_setconv_edge_fwd(_p(fc1p), _p(nbr, torch.int32), _p(edge_feats), _p(w_fc1), cin, b, n, c, _p(ymax), _p(ymin),
-                                         _p(stats, torch.float64), _p(order, torch.int32), _p(plan, torch.uint8), _p(ws, torch.uint8),
-                                         _stream()), 'setconv_edge')
+    ws = _det_workspace(abi.setconv_edge_det_workspace_bytes, b, device=fc1p.device)
+    abi.setconv_edge_fwd(fc1p, nbr, edge_feats, w_fc1, cin, b, n, c, ymax, ymin, stats, order, plan, ws)
     return ymax, ymin
 
 
@@ -597,10 +654,9 @@ def knn(xyz, query, k, mode=0, want_rel=False, use_sweep=True):
     s = query.shape[1]
     out = torch.empty(b, s, k, dtype=torch.int32, device=xyz.device)
     rel = torch.empty(b, s, k, 3, dtype=torch.float32, device=xyz.device) if want_rel else None
-    ws_bytes = int(lib().pvraft_knn_workspace_bytes(b, n)) if use_sweep else 0
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=xyz.device) if ws_bytes > 0 else None
-    _count(lib().pvraft_knn_fwd(_p(xyz), _p(query), b, n, s, k, mode, _p(out, torch.int32), _p(rel),
-                                _p(ws, torch.uint8), _stream()), 'knn')
+    ws_bytes = int(abi.knn_workspace_bytes(b, n)) if use_sweep else 0
+    ws = _workspace(ws_bytes, xyz.device) if ws_bytes > 0 else None
+    abi.knn_fwd(xyz, query, b, n, s, k, mode, out, rel, ws)
     return (out, rel) if want_rel else out
 
 
@@ -608,9 +664,8 @@ def knn(xyz, query, k, mode=0, want_rel=False, use_sweep=True):
 def linear_wgrad(x, dy, dw, db=None):
     """dw [cout,cin] += dy^T x, db [cout] += column sums of dy (both zeroed by the caller); x [B,R,cin], dy [B,R,cout]."""
     rows = x.shape[0] * x.shape[1]
-    ws = _det_workspace(lib().pvraft_linear_wgrad_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
-    _count(lib().pvraft_linear_wgrad(_p(x), _p(dy), rows, x.shape[-1], dy.shape[-1], _p(dw), dw.shape[-1], _p(db), _p(ws, torch.uint8),
-                                     _stream()), 'linear_wgrad')
+    ws = _det_workspace(abi.linear_wgrad_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
+    abi.linear_wgrad(x, dy, rows, x.shape[-1], dy.shape[-1], dw, dw.shape[-1], db, ws)
 
 
 def tc_wgrad_bf16(x, dy, dw, db=None):
@@ -618,18 +673,16 @@ def tc_wgrad_bf16(x, dy, dw, db=None):
     bf16(dy)^T bf16(x), db [cout] += column sums of the unrounded dy; x [B,R,cin], dy [B,R,cout], cin in {32..192} and
     cout in {32..128} multiples of 32."""
     rows = x.shape[0] * x.shape[1]
-    ws = _det_workspace(lib().pvraft_tc_wgrad_bf16_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
-    _count(lib().pvraft_tc_wgrad_bf16(_p(x), _p(dy), rows, x.shape[-1], dy.shape[-1], _p(dw), dw.shape[-1], _p(db), _p(ws, torch.uint8),
-                                      _stream()), 'tc_wgrad_bf16')
+    ws = _det_workspace(abi.tc_wgrad_bf16_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
+    abi.tc_wgrad_bf16(x, dy, rows, x.shape[-1], dy.shape[-1], dw, dw.shape[-1], db, ws)
 
 
 def linear_bwd_small(x, dy, w, dw, db=None, want_dx=False):
     """cin <= 4, cout in {16,32,48,64,96,128}: dw += dy^T x, db += column sums, and dx = dy w (returned, or None) in one pass over dy."""
     rows = x.shape[0] * x.shape[1]
     dx = torch.empty_like(x) if want_dx else None
-    ws = _det_workspace(lib().pvraft_linear_bwd_small_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
-    _count(lib().pvraft_linear_bwd_small(_p(x), _p(dy), _p(w), rows, x.shape[-1], dy.shape[-1], w.shape[-1], _p(dw), dw.shape[-1], _p(db),
-                                         _p(dx), _p(ws, torch.uint8), _stream()), 'linear_bwd_small')
+    ws = _det_workspace(abi.linear_bwd_small_det_workspace_bytes, x.shape[-1], dy.shape[-1], device=x.device)
+    abi.linear_bwd_small(x, dy, w, rows, x.shape[-1], dy.shape[-1], w.shape[-1], dw, dw.shape[-1], db, dx, ws)
     return dx
 
 
@@ -638,8 +691,7 @@ def gn_act_maxk(x, stats, gamma, beta, count, act, slope, slope_dev=None):
     b, rows, c = x.shape
     y = torch.empty(b, rows // 32, c, dtype=torch.float32, device=x.device)
     arg = torch.empty(b, rows // 32, c, dtype=torch.uint8, device=x.device)
-    _count(lib().pvraft_gn_act_maxk_fwd(_p(x), _p(stats, torch.float64), _p(gamma), _p(beta), float(count), act, float(slope), b,
-                                        rows // 32, c, _p(y), _p(arg, torch.uint8), _p(slope_dev), _stream()), 'gn_act_maxk')
+    abi.gn_act_maxk_fwd(x, stats, gamma, beta, float(count), act, float(slope), b, rows // 32, c, y, arg, slope_dev)
     return y, arg
 
 
@@ -650,39 +702,37 @@ def gn_act_bwd(x, dy, stats, gamma, beta, count, act, slope, want_dslope=False, 
     scratch = torch.zeros(b * 16 + 2 * c + 1, dtype=torch.float64, device=dev)   # gsum | dgamma | dbeta | dslope
     gsum, dgamma, dbeta, dslope = scratch[:b * 16], scratch[b * 16:b * 16 + c], scratch[b * 16 + c:b * 16 + 2 * c], scratch[-1:]
     dx = torch.empty_like(x)
-    ws = _det_workspace(lib().pvraft_gn_act_bwd_det_workspace_bytes, b, c, device=dev)
-    _count(lib().pvraft_gn_act_bwd(_p(x), _p(dy), _p(stats, torch.float64), _p(gamma), _p(beta), float(count), act, float(slope), b, rows, c,
-                                   gsum.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), dslope.data_ptr() if want_dslope else None, _p(dx),
-                                   _p(slope_dev), _p(arg, torch.uint8), _p(ws, torch.uint8), _stream()), 'gn_act_bwd')
+    ws = _det_workspace(abi.gn_act_bwd_det_workspace_bytes, b, c, device=dev)
+    abi.gn_act_bwd(x, dy, stats, gamma, beta, float(count), act, float(slope), b, rows, c, gsum, dgamma, dbeta,
+                   dslope if want_dslope else None, dx, slope_dev, arg, ws)
     return dx, dgamma.float(), dbeta.float(), (dslope.float() if want_dslope else None)
 
 
 def edge_fwd(p, nbr, e, stats=None):
     """e [B,N*32,C] <- p[nbr] - p[centre] + e in place; stats [B,8,2] f64 accumulated."""
     b, n, c = p.shape
-    ws = _det_workspace(lib().pvraft_edge_fwd_det_workspace_bytes, b, device=p.device) if stats is not None else None
-    _count(lib().pvraft_edge_fwd(_p(p), _p(nbr, torch.int32), _p(e), b, n, c, _p(stats, torch.float64), _p(ws, torch.uint8), _stream()),
-           'edge_fwd')
+    ws = _det_workspace(abi.edge_fwd_det_workspace_bytes, b, device=p.device) if stats is not None else None
+    abi.edge_fwd(p, nbr, e, b, n, c, stats, ws)
     return e
 
 
 def edge_bwd(dt, nbr, dp):
     b, n, c = dp.shape
-    ws = _det_workspace(lib().pvraft_edge_bwd_det_workspace_bytes, b, n, c, device=dp.device)
-    _count(lib().pvraft_edge_bwd(_p(dt), _p(nbr, torch.int32), b, n, c, _p(dp), _p(ws, torch.uint8), _stream()), 'edge_bwd')
+    ws = _det_workspace(abi.edge_bwd_det_workspace_bytes, b, n, c, device=dp.device)
+    abi.edge_bwd(dt, nbr, b, n, c, dp, ws)
     return dp
 
 
 def maxk_fwd(x, pts, c):
     y = torch.empty(pts, c, dtype=torch.float32, device=x.device)
     arg = torch.empty(pts, c, dtype=torch.uint8, device=x.device)
-    _count(lib().pvraft_maxk_fwd(_p(x), pts, c, _p(y), _p(arg, torch.uint8), _stream()), 'maxk_fwd')
+    abi.maxk_fwd(x, pts, c, y, arg)
     return y, arg
 
 
 def maxk_bwd(dy, arg, pts, c):
     dx = torch.empty(pts, KNN, c, dtype=torch.float32, device=dy.device)
-    _count(lib().pvraft_maxk_bwd(_p(dy), _p(arg, torch.uint8), pts, c, _p(dx), _stream()), 'maxk_bwd')
+    abi.maxk_bwd(dy, arg, pts, c, dx)
     return dx
 
 
@@ -690,7 +740,7 @@ def lookup_table_in_smem(m, k):
     """True when corr_lookup stages the gather table of a second cloud of m points in shared memory at truncate_k = k (the
     faster path).  At K = 512 a table of 8 192 points fits and one of 12 000 does not: the kernel then gathers from global
     memory."""
-    return bool(lib().pvraft_corr_lookup_table_in_smem(int(m), int(k)))
+    return bool(abi.corr_lookup_table_in_smem(int(m), int(k)))
 
 
 def corr_lookup_bwd(corr_idx, xyz2_pad, coords, slots, g_vox, g_sel, levels, base_scale):
@@ -698,9 +748,7 @@ def corr_lookup_bwd(corr_idx, xyz2_pad, coords, slots, g_vox, g_sel, levels, bas
     b, n, k = corr_idx.shape
     m = _table_rows(xyz2_pad, b)
     d_corr = torch.empty(b, n, k, dtype=torch.float32, device=corr_idx.device)
-    _count(lib().pvraft_corr_lookup_bwd(_p(corr_idx, torch.int32), _p(xyz2_pad), _p(coords), _p(slots, torch.int32), _p(g_vox),
-                                        g_vox.shape[-1], _p(g_sel), b, n, m, k, levels, float(base_scale), _p(d_corr), _stream()),
-           'corr_lookup_bwd')
+    abi.corr_lookup_bwd(corr_idx, xyz2_pad, coords, slots, g_vox, g_vox.shape[-1], g_sel, b, n, m, k, levels, float(base_scale), d_corr)
     return d_corr
 
 
@@ -709,9 +757,8 @@ def corr_lookup_xyz_bwd(corr_idx, slots, g_sel, d_xyz2):
     rows, through the state's ids corr_idx [B,N,K] and the forward's slots [B,N,32]."""
     b, n, k = corr_idx.shape
     m = d_xyz2.shape[1]
-    ws = _det_workspace(lib().pvraft_corr_lookup_xyz_bwd_det_workspace_bytes, b, m, device=d_xyz2.device)
-    _count(lib().pvraft_corr_lookup_xyz_bwd(_p(corr_idx, torch.int32), _p(slots, torch.int32), _p(g_sel), b, n, m, k, _p(d_xyz2),
-                                            _p(ws, torch.uint8), _stream()), 'corr_lookup_xyz_bwd')
+    ws = _det_workspace(abi.corr_lookup_xyz_bwd_det_workspace_bytes, b, m, device=d_xyz2.device)
+    abi.corr_lookup_xyz_bwd(corr_idx, slots, g_sel, b, n, m, k, d_xyz2, ws)
     return d_xyz2
 
 
@@ -723,10 +770,25 @@ def corr_init_bwd(g, idx, fmap1, fmap2):
         raise ValueError(f'corr_init_bwd: feature maps {tuple(fmap1.shape)} and {tuple(fmap2.shape)}')
     d1 = torch.empty_like(fmap1)
     d2 = torch.zeros_like(fmap2)
-    ws = _det_workspace(lib().pvraft_corr_init_bwd_det_workspace_bytes, b, m, c, device=fmap1.device)
-    _count(lib().pvraft_corr_init_bwd(_p(g), _p(idx, torch.int32), _p(fmap1), _p(fmap2), b, n, m, c, g.shape[-1], _p(d1), _p(d2),
-                                      _p(ws, torch.uint8), _stream()), 'corr_init_bwd')
+    ws = _det_workspace(abi.corr_init_bwd_det_workspace_bytes, b, m, c, device=fmap1.device)
+    abi.corr_init_bwd(g, idx, fmap1, fmap2, b, n, m, c, g.shape[-1], d1, d2, ws)
     return d1, d2
+
+
+def flow_metrics(est, gt, mask):
+    """est, gt [..., 3], mask [...] f32 (> 0 = valid) -> acc [8] f64: [0..5] the sums of pvraft_flow_metrics_fwd, [6..7] unused."""
+    acc = torch.zeros(8, dtype=torch.float64, device=est.device)
+    ws = _det_workspace(abi.flow_metrics_det_workspace_bytes, device=est.device)
+    abi.flow_metrics_fwd(est, gt, mask, est.numel() // 3, acc, ws)
+    return acc
+
+
+def flow_l1_bwd(est, gt, mask, acc, g, weight):
+    """Gradient of weight * acc[0] / (3 acc[1]) (flow_metrics' masked L1 loss) for the upstream gradient g [1] (on the
+    device) -> d_est."""
+    d = torch.empty_like(est)
+    abi.flow_l1_bwd(est, gt, mask, est.numel() // 3, acc, g, float(weight), d)
+    return d
 
 
 def _loss_batch(what, x, b_rows, m=None):
@@ -774,14 +836,12 @@ def chamfer(a, b, use_grid=None):
     acc = torch.zeros(s, 2, dtype=torch.float64, device=a.device)
     nn_ab = torch.empty(s, n, dtype=torch.int32, device=a.device)
     nn_ba = torch.empty(s, m, dtype=torch.int32, device=a.device)
-    ws = _det_workspace(lib().pvraft_chamfer_fwd_det_workspace_bytes, s, device=a.device)
+    ws = _det_workspace(abi.chamfer_fwd_det_workspace_bytes, s, device=a.device)
     if use_grid_search('chamfer', max(n, m), use_grid):
-        gw = _workspace(lib().pvraft_chamfer_grid_workspace_bytes(s, bb, n, m), a.device)
-        _count(lib().pvraft_chamfer_grid_fwd(_p(a), _p(b), s, bb, n, m, _p(nn_ab, torch.int32), _p(nn_ba, torch.int32), _p(acc, torch.float64),
-                                             _p(gw, torch.uint8), _p(ws, torch.uint8), _stream()), 'chamfer_grid_fwd')
+        gw = _workspace(abi.chamfer_grid_workspace_bytes(s, bb, n, m), a.device)
+        abi.chamfer_grid_fwd(a, b, s, bb, n, m, nn_ab, nn_ba, acc, gw, ws)
         return acc, nn_ab, nn_ba
-    _count(lib().pvraft_chamfer_fwd(_p(a), _p(b), s, bb, n, m, _p(nn_ab, torch.int32), _p(nn_ba, torch.int32), _p(acc, torch.float64),
-                                    _p(ws, torch.uint8), _stream()), 'chamfer_fwd')
+    abi.chamfer_fwd(a, b, s, bb, n, m, nn_ab, nn_ba, acc, ws)
     return acc, nn_ab, nn_ba
 
 
@@ -795,9 +855,8 @@ def chamfer_bwd(a, b, nn_ab, nn_ba, g, want_db=True):
         raise ValueError(f'chamfer_bwd: expected g [{s}], got {tuple(g.shape)}')
     d_a = torch.zeros_like(a)
     d_b = torch.zeros_like(b) if want_db else None
-    ws = _det_workspace(lib().pvraft_chamfer_bwd_det_workspace_bytes, s, bb, n, m, device=a.device)
-    _count(lib().pvraft_chamfer_bwd(_p(a), _p(b), _p(nn_ab, torch.int32), _p(nn_ba, torch.int32), _p(g), s, bb, n, m, _p(d_a), _p(d_b),
-                                    _p(ws, torch.uint8), _stream()), 'chamfer_bwd')
+    ws = _det_workspace(abi.chamfer_bwd_det_workspace_bytes, s, bb, n, m, device=a.device)
+    abi.chamfer_bwd(a, b, nn_ab, nn_ba, g, s, bb, n, m, d_a, d_b, ws)
     return d_a, d_b
 
 
@@ -812,9 +871,8 @@ def flow_smooth(f, nbr):
     """f [S,N,3], nbr [B,N,k] int32 (sample s uses nbr[s % B]) -> acc [S] f64: sum over the edges of ||f_j - f_i||."""
     s, bb, n, k = _smooth_args('flow_smooth', f, nbr)
     acc = torch.zeros(s, dtype=torch.float64, device=f.device)
-    ws = _det_workspace(lib().pvraft_flow_smooth_fwd_det_workspace_bytes, s, device=f.device)
-    _count(lib().pvraft_flow_smooth_fwd(_p(f), _p(nbr, torch.int32), s, bb, n, k, _p(acc, torch.float64), _p(ws, torch.uint8), _stream()),
-           'flow_smooth_fwd')
+    ws = _det_workspace(abi.flow_smooth_fwd_det_workspace_bytes, s, device=f.device)
+    abi.flow_smooth_fwd(f, nbr, s, bb, n, k, acc, ws)
     return acc
 
 
@@ -824,9 +882,8 @@ def flow_smooth_bwd(f, nbr, g):
     if g.shape != (s,):
         raise ValueError(f'flow_smooth_bwd: expected g [{s}], got {tuple(g.shape)}')
     d_f = torch.zeros_like(f)
-    ws = _det_workspace(lib().pvraft_flow_smooth_bwd_det_workspace_bytes, s, n, device=f.device)
-    _count(lib().pvraft_flow_smooth_bwd(_p(f), _p(nbr, torch.int32), _p(g), s, bb, n, k, _p(d_f), _p(ws, torch.uint8), _stream()),
-           'flow_smooth_bwd')
+    ws = _det_workspace(abi.flow_smooth_bwd_det_workspace_bytes, s, n, device=f.device)
+    abi.flow_smooth_bwd(f, nbr, g, s, bb, n, k, d_f, ws)
     return d_f
 
 
@@ -847,7 +904,7 @@ def cloud_laplacian(x, nbr):
     L(x)_i = sum_e (x[nbr[i,e]] - x_i) / (k - 1)."""
     b, n, k = _graph_args('cloud_laplacian', x, nbr)
     out = torch.empty_like(x)
-    _count(lib().pvraft_cloud_laplacian_fwd(_p(x), _p(nbr, torch.int32), b, n, k, _p(out), _stream()), 'cloud_laplacian_fwd')
+    abi.cloud_laplacian_fwd(x, nbr, b, n, k, out)
     return out
 
 
@@ -856,9 +913,8 @@ def cloud_laplacian_bwd(g_l, nbr, d_x):
     b, n, k = _graph_args('cloud_laplacian_bwd', g_l, nbr)
     if d_x.shape != g_l.shape:
         raise ValueError(f'cloud_laplacian_bwd: d_x {tuple(d_x.shape)} does not match g_l {tuple(g_l.shape)}')
-    ws = _det_workspace(lib().pvraft_cloud_laplacian_bwd_det_workspace_bytes, b, n, device=g_l.device)
-    _count(lib().pvraft_cloud_laplacian_bwd(_p(g_l), _p(nbr, torch.int32), b, n, k, _p(d_x), _p(ws, torch.uint8), _stream()),
-           'cloud_laplacian_bwd')
+    ws = _det_workspace(abi.cloud_laplacian_bwd_det_workspace_bytes, b, n, device=g_l.device)
+    abi.cloud_laplacian_bwd(g_l, nbr, b, n, k, d_x, ws)
     return d_x
 
 
@@ -885,15 +941,12 @@ def laplacian(w, p2, l2, g1, k_int, use_grid=None):
     acc = torch.zeros(s, dtype=torch.float64, device=w.device)
     nn_idx = torch.empty(s, n, k_int, dtype=torch.int32, device=w.device)
     res = torch.empty_like(w)
-    ws = _det_workspace(lib().pvraft_laplacian_fwd_det_workspace_bytes, s, device=w.device)
+    ws = _det_workspace(abi.laplacian_fwd_det_workspace_bytes, s, device=w.device)
     if use_grid_search('laplacian', m, use_grid):
-        gw = _workspace(lib().pvraft_grid_index_workspace_bytes(bb, m), w.device)
-        _count(lib().pvraft_laplacian_grid_fwd(_p(w), _p(p2), _p(l2), _p(g1, torch.int32), s, bb, n, m, kl, k_int, _p(nn_idx, torch.int32),
-                                               _p(res), _p(acc, torch.float64), _p(gw, torch.uint8), _p(ws, torch.uint8), _stream()),
-               'laplacian_grid_fwd')
+        gw = _workspace(abi.grid_index_workspace_bytes(bb, m), w.device)
+        abi.laplacian_grid_fwd(w, p2, l2, g1, s, bb, n, m, kl, k_int, nn_idx, res, acc, gw, ws)
         return acc, nn_idx, res
-    _count(lib().pvraft_laplacian_fwd(_p(w), _p(p2), _p(l2), _p(g1, torch.int32), s, bb, n, m, kl, k_int, _p(nn_idx, torch.int32), _p(res),
-                                      _p(acc, torch.float64), _p(ws, torch.uint8), _stream()), 'laplacian_fwd')
+    abi.laplacian_fwd(w, p2, l2, g1, s, bb, n, m, kl, k_int, nn_idx, res, acc, ws)
     return acc, nn_idx, res
 
 
@@ -909,9 +962,8 @@ def laplacian_bwd(w, p2, l2, g1, nn_idx, res, g, want_dp2=True):
     d_w = torch.zeros_like(w)
     d_p2 = torch.zeros_like(p2) if want_dp2 else None
     d_l2 = torch.zeros_like(p2) if want_dp2 else None
-    ws = _det_workspace(lib().pvraft_laplacian_bwd_det_workspace_bytes, s, bb, n, m, device=w.device)
-    _count(lib().pvraft_laplacian_bwd(_p(w), _p(p2), _p(l2), _p(g1, torch.int32), _p(nn_idx, torch.int32), _p(res), _p(g), s, bb, n, m, kl,
-                                      int(nn_idx.shape[-1]), _p(d_w), _p(d_p2), _p(d_l2), _p(ws, torch.uint8), _stream()), 'laplacian_bwd')
+    ws = _det_workspace(abi.laplacian_bwd_det_workspace_bytes, s, bb, n, m, device=w.device)
+    abi.laplacian_bwd(w, p2, l2, g1, nn_idx, res, g, s, bb, n, m, kl, int(nn_idx.shape[-1]), d_w, d_p2, d_l2, ws)
     return d_w, d_p2, d_l2
 
 
@@ -946,14 +998,12 @@ def flow_consistency(w, f12, p2, f21, k, alpha, beta, use_grid=None):
     nn_idx = torch.empty(s, n, k, dtype=torch.int32, device=w.device)
     res = torch.empty_like(w)
     ok = torch.empty(s, n, dtype=torch.uint8, device=w.device)
-    ws = _det_workspace(lib().pvraft_flow_consistency_fwd_det_workspace_bytes, s, device=w.device)
-    args = (_p(w), _p(f12), _p(p2), _p(f21), s, bb, n, m, k, float(alpha), float(beta), _p(nn_idx, torch.int32), _p(res),
-            _p(ok, torch.uint8), _p(acc, torch.float64))
+    ws = _det_workspace(abi.flow_consistency_fwd_det_workspace_bytes, s, device=w.device)
+    args = (w, f12, p2, f21, s, bb, n, m, k, float(alpha), float(beta), nn_idx, res, ok, acc)
     if use_grid_search('laplacian', m, use_grid):
-        gw = _workspace(lib().pvraft_grid_index_workspace_bytes(bb, m), w.device)
-        _count(lib().pvraft_flow_consistency_grid_fwd(*args, _p(gw, torch.uint8), _p(ws, torch.uint8), _stream()), 'flow_consistency_grid_fwd')
+        abi.flow_consistency_grid_fwd(*args, _workspace(abi.grid_index_workspace_bytes(bb, m), w.device), ws)
     else:
-        _count(lib().pvraft_flow_consistency_fwd(*args, _p(ws, torch.uint8), _stream()), 'flow_consistency_fwd')
+        abi.flow_consistency_fwd(*args, ws)
     return acc, nn_idx, res, ok
 
 
@@ -970,9 +1020,8 @@ def flow_consistency_bwd(w, p2, f21, nn_idx, res, g, want_dp2=True):
     d_f12 = torch.empty_like(w)
     d_p2 = torch.zeros_like(p2) if want_dp2 else None
     d_f21 = torch.zeros_like(f21)
-    ws = _det_workspace(lib().pvraft_flow_consistency_bwd_det_workspace_bytes, s, bb, m, device=w.device)
-    _count(lib().pvraft_flow_consistency_bwd(_p(w), _p(p2), _p(f21), _p(nn_idx, torch.int32), _p(res), _p(g), s, bb, n, m, k, _p(d_w),
-                                             _p(d_f12), _p(d_p2), _p(d_f21), _p(ws, torch.uint8), _stream()), 'flow_consistency_bwd')
+    ws = _det_workspace(abi.flow_consistency_bwd_det_workspace_bytes, s, bb, m, device=w.device)
+    abi.flow_consistency_bwd(w, p2, f21, nn_idx, res, g, s, bb, n, m, k, d_w, d_f12, d_p2, d_f21, ws)
     return d_w, d_f12, d_p2, d_f21
 
 
@@ -1006,12 +1055,10 @@ def flow_propagate(xyz_prev, flow_prev, xyz, k=3, want_idx=False, use_grid=None)
     out = torch.empty(b, n, 3, dtype=torch.float32, device=xyz.device)
     idx = torch.empty(b, n, k, dtype=torch.int32, device=xyz.device) if want_idx else None
     if use_grid_search('flow_propagate', m, use_grid):
-        gw = _workspace(lib().pvraft_grid_index_workspace_bytes(b, m), xyz.device)
-        _count(lib().pvraft_flow_propagate_grid_fwd(_p(xyz_prev), _p(flow_prev), _p(xyz), b, m, n, k, _p(out), _p(idx, torch.int32),
-                                                    _p(gw, torch.uint8), _stream()), 'flow_propagate_grid_fwd')
+        gw = _workspace(abi.grid_index_workspace_bytes(b, m), xyz.device)
+        abi.flow_propagate_grid_fwd(xyz_prev, flow_prev, xyz, b, m, n, k, out, idx, gw)
         return (out, idx) if want_idx else out
-    _count(lib().pvraft_flow_propagate_fwd(_p(xyz_prev), _p(flow_prev), _p(xyz), b, m, n, k, _p(out), _p(idx, torch.int32), _stream()),
-           'flow_propagate_fwd')
+    abi.flow_propagate_fwd(xyz_prev, flow_prev, xyz, b, m, n, k, out, idx)
     return (out, idx) if want_idx else out
 
 
@@ -1029,11 +1076,9 @@ def euclidean_clusters(x, f, mask, radius, flow_radius, min_points, max_objects)
     labels = torch.empty(b, n, dtype=torch.int32, device=dev)
     num = torch.empty(b, dtype=torch.int32, device=dev)
     sizes = torch.empty(b, max_objects, dtype=torch.int32, device=dev)
-    ws = _workspace(lib().pvraft_euclidean_clusters_workspace_bytes(b, n), dev)
-    _count(lib().pvraft_euclidean_clusters_fwd(_p(x), _p(f), _p(mask, torch.uint8), b, n, float(radius),
-                                               float(flow_radius) if f is not None else 0.0, min_points, max_objects,
-                                               _p(labels, torch.int32), _p(num, torch.int32), _p(sizes, torch.int32),
-                                               _p(ws, torch.uint8), _stream()), 'euclidean_clusters_fwd')
+    ws = _workspace(abi.euclidean_clusters_workspace_bytes(b, n), dev)
+    abi.euclidean_clusters_fwd(x, f, mask, b, n, float(radius), float(flow_radius) if f is not None else 0.0, min_points, max_objects,
+                               labels, num, sizes, ws)
     return labels, num, sizes
 
 
@@ -1054,12 +1099,10 @@ def rigid_objects(x, f, labels, objects, threshold, hypotheses, rounds, seed, wa
     state = torch.empty(b, o, 32, dtype=torch.float64, device=dev)
     triples = torch.empty(b * o, hypotheses, 3, dtype=torch.int32, device=dev) if want_samples else None
     hcount = torch.empty(b * o, hypotheses, dtype=torch.int32, device=dev) if want_samples else None
-    ws = _workspace(lib().pvraft_rigid_objects_workspace_bytes(b, n, o, hypotheses, rounds), dev)
-    det = _det_workspace(lib().pvraft_rigid_objects_fwd_det_workspace_bytes, b, o, rounds, device=dev)
-    _count(lib().pvraft_rigid_objects_fwd(_p(x), _p(f), _p(labels, torch.int32), b, n, o, float(threshold), hypotheses, rounds, seed,
-                                          _p(R), _p(t), _p(inl, torch.uint8), _p(count, torch.int32), _p(degen, torch.uint8),
-                                          _p(state, torch.float64), _p(triples, torch.int32), _p(hcount, torch.int32),
-                                          _p(ws, torch.uint8), _p(det, torch.uint8), _stream()), 'rigid_objects_fwd')
+    ws = _workspace(abi.rigid_objects_workspace_bytes(b, n, o, hypotheses, rounds), dev)
+    det = _det_workspace(abi.rigid_objects_fwd_det_workspace_bytes, b, o, rounds, device=dev)
+    abi.rigid_objects_fwd(x, f, labels, b, n, o, float(threshold), hypotheses, rounds, seed, R, t, inl, count, degen, state, triples,
+                          hcount, ws, det)
     out = (R, t, inl, count, degen, state)
     return out + (triples, hcount) if want_samples else out
 
@@ -1074,12 +1117,11 @@ def rigid_objects_bwd(x, f, labels, inliers, state, dR, dt):
                          f'{None if labels is None else tuple(labels.shape)}, inliers {tuple(inliers.shape)}, state '
                          f'{tuple(state.shape)}, dR {tuple(dR.shape)}, dt {tuple(dt.shape)} do not agree')
     d_x, d_f = torch.empty_like(x), torch.empty_like(x)
-    _count(lib().pvraft_rigid_objects_bwd(_p(x), _p(f), _p(labels, torch.int32), _p(inliers, torch.uint8), _p(state, torch.float64),
-                                          _p(dR), _p(dt), b, n, o, _p(d_x), _p(d_f), _stream()), 'rigid_objects_bwd')
+    abi.rigid_objects_bwd(x, f, labels, inliers, state, dR, dt, b, n, o, d_x, d_f)
     return d_x, d_f
 
 
 def device_info():
     sm, smem = C.c_int(0), C.c_int(0)
-    check(lib().pvraft_device_info(C.byref(sm), C.byref(smem)), 'device_info')
+    check(abi.device_info(C.byref(sm), C.byref(smem)), 'device_info')
     return sm.value, smem.value

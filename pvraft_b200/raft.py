@@ -296,13 +296,7 @@ class _RaftBase(nn.Module):
                 _, motion = self.corr_block.feature_motion_tc(coords2, flow, me, need_corr=False)          # :42 + update.py:83
             else:
                 motion = torch.empty(b, n, 64, dtype=torch.float32, device=xyz1.device)
-
-                def attach(a, keep, flow=flow, motion=motion):
-                    me.fill(a, flow)
-                    a.motion = ops._p(motion)
-                    keep.append(motion)
-
-                _, keep = self.corr_block.feature_point_major(coords2, motion_args=attach)   # :42 + update.py:83
+                self.corr_block.feature_point_major(coords2, motion_args=lambda a, keep: me.fill(a, flow, motion))   # :42 + :83
             new_flow = torch.empty_like(xyz1)
             net, _ = self.update_block.forward_pm(net, inp, motion, graph_context, coords1=xyz1, coords2=coords2,
                                                   coords2_out=coords2, flow_out=new_flow)   # :44-46

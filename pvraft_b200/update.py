@@ -8,7 +8,7 @@ RAFT loop uses (no transposes inside the loop).
 import torch
 import torch.nn as nn
 
-from . import _lib, ops
+from . import ops
 from .gconv import SetConv
 
 
@@ -32,21 +32,17 @@ class MotionEncoder(nn.Module):
         self.conv_flow = nn.Conv1d(3, 64, 1)
         self.conv = nn.Conv1d(64 + 64, 64 - 3, 1)
 
-    def fill(self, a, flow):
-        """Attach the motion stage to a CorrFeatArgs (pvraft_corr_feature_fwd)."""
-        a.flow = ops._p(flow)
-        a.w_cc, a.b_cc = ops._p(_w(self.conv_corr.weight)), ops._p(_w(self.conv_corr.bias))
-        a.w_cf, a.b_cf = ops._p(_w(self.conv_flow.weight)), ops._p(_w(self.conv_flow.bias))
-        a.w_cm, a.b_cm = ops._p(_w(self.conv.weight)), ops._p(_w(self.conv.bias))
+    def fill(self, a, flow, motion=None):
+        """Attach the motion stage to a CorrFeatArgs (pvraft_corr_feature_fwd), with its output `motion` when given."""
+        ops.pack.CorrFeatArgs(a, flow=flow, w_cc=_w(self.conv_corr.weight), b_cc=_w(self.conv_corr.bias),
+                              w_cf=_w(self.conv_flow.weight), b_cf=_w(self.conv_flow.bias), w_cm=_w(self.conv.weight),
+                              b_cm=_w(self.conv.bias), motion=motion)
 
     def forward_pm(self, flow, corr_pm):
         b, n, _ = flow.shape
-        a = _lib.CorrFeatArgs()
-        a.corr_in = ops._p(corr_pm)
-        self.fill(a, flow)
         motion = torch.empty(b, n, 64, dtype=torch.float32, device=flow.device)
-        a.motion = ops._p(motion)
-        a.B, a.N = b, n
+        a = ops.pack.CorrFeatArgs(corr_in=corr_pm, B=b, N=n)
+        self.fill(a, flow, motion)
         ops.corr_feature(a)
         return motion
 
@@ -76,10 +72,9 @@ class ConvGRU(nn.Module):
             ops.tc_linear([rh, inp, motion], ops.tc_weights(self.convq.weight), _w(self.convq.bias), epilogue=ops.TC_GRU_Q,
                           out=out, h=net, z=z, cout=64)
             return out
-        a = _lib.GruArgs(ops._p(net), ops._p(inp), ops._p(motion), ops._p(_w(self.convz.weight)), ops._p(_w(self.convz.bias)),
-                         ops._p(_w(self.convr.weight)), ops._p(_w(self.convr.bias)), ops._p(_w(self.convq.weight)),
-                         ops._p(_w(self.convq.bias)), ops._p(out), b, n)
-        ops.gru(a)
+        ops.gru(ops.pack.GruArgs(net=net, inp=inp, motion=motion, w_z=_w(self.convz.weight), b_z=_w(self.convz.bias),
+                                 w_r=_w(self.convr.weight), b_r=_w(self.convr.bias), w_q=_w(self.convq.weight),
+                                 b_q=_w(self.convq.bias), net_out=out, B=b, N=n))
         return out
 
     def forward(self, h, x):
@@ -133,11 +128,10 @@ class FlowHead(nn.Module):
                           w3=_w(oc[2].weight), b3=_w(oc[2].bias), coords1=coords1, coords2=coords2, coords2_out=coords2_out,
                           flow_out=flow_out)
             return delta
-        a = _lib.FlowOutArgs(ops._p(d.z), ops._p(d.stats, torch.float64), ops._p(d.gamma), ops._p(d.beta), ops._p(net),
-                             ops._p(_w(self.conv1.weight)), ops._p(_w(self.conv1.bias)), ops._p(_w(oc[0].weight)),
-                             ops._p(_w(oc[0].bias)), ops._p(_w(oc[2].weight)), ops._p(_w(oc[2].bias)), ops._p(coords1),
-                             ops._p(coords2), ops._p(delta), ops._p(coords2_out), ops._p(flow_out), b, n)
-        ops.flow_out(a)
+        ops.flow_out(ops.pack.FlowOutArgs(z3=d.z, z3_stats=d.stats, gn3_gamma=d.gamma, gn3_beta=d.beta, net=net,
+                                          w_c1=_w(self.conv1.weight), b_c1=_w(self.conv1.bias), w_o0=_w(oc[0].weight),
+                                          b_o0=_w(oc[0].bias), w_o2=_w(oc[2].weight), b_o2=_w(oc[2].bias), coords1=coords1,
+                                          coords2=coords2, delta=delta, coords2_out=coords2_out, flow_out=flow_out, B=b, N=n))
         return delta
 
     def forward(self, x, graph):

@@ -50,20 +50,14 @@ def test_bf16_compute_scope_nests_and_restores():
 
 def test_one_weight_format_per_launch():
     """w_bf16 together with w_hi / w_lo, or a chain whose layers mix the formats, is rejected before any launch."""
-    from pvraft_b200 import _lib
+    from pvraft_b200 import _lib, ops
     lib = _lib.lib()
-    a = _lib.TcLinearArgs()
-    a.in_[0], a.in_channels[0], a.out, a.n_pad, a.cout, a.B, a.N = 16, 32, 16, 16, 16, 1, 128
-    a.w_hi, a.w_lo, a.w_bf16 = 16, 16, 16
+    a = ops.pack.TcLinearArgs(in_=[16], in_channels=[32], out=16, n_pad=16, cout=16, B=1, N=128, w_hi=16, w_lo=16, w_bf16=16)
     assert lib.pvraft_tc_linear_fwd(ctypes.byref(a), None, None) == -1
     assert b'w_bf16' in lib.pvraft_last_error_string()
-    c = _lib.UpdateChainArgs()
-    for f in ('y1', 'y1_stats', 'gn_gamma', 'gn_beta', 'kfeat', 'cflow', 'flow', 'net', 'inp', 'b_cc', 'b_m', 'b_z', 'b_r', 'b_q',
-              'p_out'):
-        setattr(c, f, 16)
-    c.net_out, c.B, c.N, c.hidden, c.context, c.y1_channels = 32, 1, 128, 64, 64, 128
-    for i in range(5):
-        c.w_bf16[i] = 16
+    c = ops.pack.UpdateChainArgs(**{f: 16 for f in ('y1', 'y1_stats', 'gn_gamma', 'gn_beta', 'kfeat', 'cflow', 'flow', 'net', 'inp',
+                                                        'b_cc', 'b_m', 'b_z', 'b_r', 'b_q', 'p_out')},
+                 net_out=32, B=1, N=128, hidden=64, context=64, y1_channels=128, w_bf16=[16] * 5)
     c.w_hi[3], c.w_lo[3] = 16, 16
     assert lib.pvraft_update_chain_fwd(ctypes.byref(c), None) == -1
     assert b'layer 3' in lib.pvraft_last_error_string()
