@@ -829,6 +829,46 @@ PVRAFT_API int pvraft_rigid_objects_bwd(const float* xyz1, const float* flow, co
                                         const double* state, const float* dR, const float* dt, int B, int N, int O, float* d_xyz1,
                                         float* d_flow, void* stream);
 
+/* Multi-object tracking from scene flow (no counterpart in the reference): one step of pvraft_b200.track.ObjectTracker.  A
+ * sequence gives scans P_0, P_1, ...; for the pair (P_{t-1}, P_t) the caller has the flow F on P_{t-1} and the objects
+ * found on P_{t-1} (pvraft_euclidean_clusters_fwd labels and num_objects, O slots).  A step associates them with the O_prev
+ * object slots of the previous step, which were found on X = xyz_prev = P_{t-2} (labels_prev [B,M]).  flow_prev [B,M,3] is
+ * G, the previous step's rigid flow (pvraft_b200.rigid_flow of X, its flow and fits); R_prev [B,O_prev,3,3] and t_prev
+ * [B,O_prev,3] are the previous step's per-object fits (X -> P_{t-1}); track_prev, age_prev [B,O_prev] and pose_prev
+ * [B,O_prev,12] are the previous step's outputs.
+ *   Moved previous points: W_i = X_i + G_i, one fp32 add per coordinate (the add of pvraft_flow_propagate_fwd).
+ *   Nearest moved point: nn [B,N] int32 is, for every point j of xyz = P_{t-1}, the nearest W_i on (diff_sq, i), -1 for an
+ *       unfilled slot: exactly idx_out of pvraft_flow_propagate_fwd (or its grid form) with k = 1.  No search runs here.
+ *   Votes: point j of sample b takes part when 0 <= c = labels[b,j] < min(num_objects[b], O); it adds 1 to members[b,c],
+ *       and 1 to overlap[b,c,a] when 0 <= i = nn[b,j] < M, 0 <= a = labels_prev[b,i] < O_prev, track_prev[b,a] >= 0 (a
+ *       previous slot holds an object) and diff_sq(P_j, W_i) <= fl(gate * gate), diff_sq the fp32 difference form of the
+ *       searches ((dx dx + dy dy) + dz dz, every operation rounded to nearest, none contracted) on the same W_i, so the same
+ *       bits the search ranked on.  Integer counts: the result does not depend on the order of any atomic operation.
+ *   Eligible pairs: (c, a) with overlap[b,c,a] >= 1 and overlap[b,c,a] >= min_overlap * members[b,c], the product in
+ *       double.  A slot's votes for different previous objects are disjoint, so it has at most 16 eligible pairs.
+ *   Greedy matching: the eligible pairs by larger overlap, then lower c, then lower a; a pair is accepted when neither its
+ *       c nor its a has been accepted before.  (Not Hungarian.)
+ *   Slots c < min(num_objects[b], O): matched to a, track[b,c] = track_prev[b,a], match[b,c] = a, age[b,c] = age_prev[b,a]
+ *       + 1 and pose = (R_a R_p, R_a t_p + t_a) with (R_a, t_a) the fit of a and (R_p, t_p) = pose_prev[b,a], in double,
+ *       each entry summed k = 0, 1, 2 as (x0 y0 + x1 y1) + x2 y2 (the translation then + t_a), every operation rounded to
+ *       nearest, none contracted; unmatched, a new track: ids next_id[b], next_id[b] + 1, ... in ascending c, match -1, age
+ *       0, identity pose, and next_id[b] advances by their number.  Other slots: track = match = age = -1, identity pose.
+ *       A pose [12] is R row-major, then t: it maps the object's points in the scan it was born on to its points in xyz.
+ *   First step: M = 0 and O_prev = 0, the previous pointers and nn NULL: every object is born.
+ *   pvraft_track_objects_fwd: -> next_id [B] int32 (in/out), overlap [B,O,O_prev] int32 (NULL allowed with O_prev = 0),
+ *       members [B,O] int32 (both cleared on the stream here), match, track, age [B,O] int32, pose [B,O,12] double.  Every
+ *       output element is written.  No det_workspace: integer decisions and a fixed-order double composition, bitwise
+ *       reproducible as they are.  No host synchronisation.
+ * Null required pointers (xyz_prev, flow_prev, labels_prev and nn with M > 0; track_prev, age_prev, pose_prev, R_prev,
+ * t_prev and overlap with O_prev > 0), B < 1, N < 1, M < 0, O outside 1..256, O_prev outside 0..256, M = 0 with O_prev !=
+ * 0, a gate that is not finite and > 0 or whose square overflows fp32, and min_overlap outside [1/16, 1] return
+ * PVRAFT_ERR_BAD_ARG before any launch; B > 65535 PVRAFT_ERR_UNSUPPORTED. */
+PVRAFT_API int pvraft_track_objects_fwd(const float* xyz_prev, const float* flow_prev, const int32_t* labels_prev, const int32_t* track_prev,
+                                        const int32_t* age_prev, const double* pose_prev, const float* R_prev, const float* t_prev,
+                                        const float* xyz, const int32_t* labels, const int32_t* num_objects, const int32_t* nn, int B, int M,
+                                        int N, int O_prev, int O, float gate, double min_overlap, int32_t* next_id, int32_t* overlap,
+                                        int32_t* members, int32_t* match, int32_t* track, int32_t* age, double* pose, void* stream);
+
 /* sizeof() of the argument structs as compiled into the library (0 = linear, 1 = corrfeat, 2 = gru, 3 = flowout,
  * 4 = tc_linear, 5 = knn_branch, 6 = update_chain; -1 otherwise): lets a foreign-language binding verify its struct layout
  * at load time. */

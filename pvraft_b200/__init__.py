@@ -10,8 +10,10 @@ from .raft import RSF, RSF_refine
 from .refine import FlotRefine
 from .rigid import RigidMotion, RigidObjects, rigid_flow, rigid_motion, rigid_objects
 from .stream import SceneFlowStream
+from .track import ObjectTracker, ObjectTracks
 from .update import ConvGRU, ConvRNN, FlowHead, MotionEncoder, UpdateBlock
 
 __all__ = ['RSF', 'RSF_refine', 'CorrBlock', 'UpdateBlock', 'MotionEncoder', 'ConvGRU', 'ConvRNN', 'FlowHead',
            'FlotEncoder', 'FlotRefine', 'SetConv', 'Graph', 'knn_point', 'square_distance', 'SceneFlowStream',
-           'flow_consistency', 'rigid_motion', 'RigidMotion', 'rigid_objects', 'RigidObjects', 'rigid_flow']
+           'flow_consistency', 'rigid_motion', 'RigidMotion', 'rigid_objects', 'RigidObjects', 'rigid_flow', 'ObjectTracker',
+           'ObjectTracks']

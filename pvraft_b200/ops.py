@@ -1121,6 +1121,32 @@ def rigid_objects_bwd(x, f, labels, inliers, state, dR, dt):
     return d_x, d_f
 
 
+TRACK_MIN_OVERLAP = 1 / 16   # pvraft_track_objects_fwd's least min_overlap: a slot then has at most 16 eligible pairs
+
+
+def track_objects(prev, xyz, labels, num_objects, objects, nn, gate, min_overlap, next_id):
+    """One step of the object association (include/pvraft_b200.h, pvraft_track_objects_fwd): prev is None on the first step,
+    else (xyz_prev [B,M,3] f32, flow_prev [B,M,3] f32 (the previous rigid flow), labels_prev [B,M] int32, track_prev,
+    age_prev [B,O_prev] int32, pose_prev [B,O_prev,12] f64, R_prev [B,O_prev,3,3] f32, t_prev [B,O_prev,3] f32); xyz
+    [B,N,3] f32, labels [B,N] int32 and num_objects [B] int32 of the current objects, O = objects slots; nn [B,N] int32
+    (the propagation search's neighbour of every point, k = 1; None with prev None); next_id [B] int32, advanced in place ->
+    (overlap [B,O,O_prev], members [B,O], match, track, age [B,O] int32, pose [B,O,12] f64).  The arguments are checked by
+    pvraft_b200.track.ObjectTracker."""
+    b, n, o = int(xyz.shape[0]), int(xyz.shape[1]), int(objects)
+    dev = xyz.device
+    if prev is None:
+        prev, m, o_prev = (None,) * 8, 0, 0
+    else:
+        m, o_prev = int(prev[0].shape[1]), int(prev[3].shape[1])
+    overlap = torch.empty(b, o, o_prev, dtype=torch.int32, device=dev)
+    members = torch.empty(b, o, dtype=torch.int32, device=dev)
+    match, track, age = (torch.empty(b, o, dtype=torch.int32, device=dev) for _ in range(3))
+    pose = torch.empty(b, o, 12, dtype=torch.float64, device=dev)
+    abi.track_objects_fwd(*prev, xyz, labels, num_objects, nn, b, m, n, o_prev, o, float(gate), float(min_overlap), next_id,
+                          overlap if o_prev else None, members, match, track, age, pose)
+    return overlap, members, match, track, age, pose
+
+
 def device_info():
     sm, smem = C.c_int(0), C.c_int(0)
     check(abi.device_info(C.byref(sm), C.byref(smem)), 'device_info')
