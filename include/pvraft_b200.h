@@ -829,6 +829,57 @@ PVRAFT_API int pvraft_rigid_objects_bwd(const float* xyz1, const float* flow, co
                                         const double* state, const float* dR, const float* dt, int B, int N, int O, float* d_xyz1,
                                         float* d_flow, void* stream);
 
+/* Point-to-plane ICP of rigid fits against the second scan (no counterpart in the reference): pvraft_b200.rigid_refine.
+ * The segments are those of pvraft_rigid_objects_fwd (labels [B,N], value o: segment (b, o); NULL only with O = 1: every
+ * point) and the same grouping: each segment's members are an ascending list.  A source point takes part when it is a
+ * member and its three coordinates are finite.  No host synchronisation; every required output element is written.
+ *   Targets: point j of xyz2 [B,M,3] is a target when target_mask[b,j] != 0 (every point with target_mask NULL) and its
+ *       three coordinates are finite.  diff_sq below is the fp32 difference form of the searches ((dx dx + dy dy) + dz dz,
+ *       every operation rounded to nearest, none contracted).
+ *   Normals: target j's neighbours are its k_normal nearest targets, itself included, ranked on (diff_sq, id).  With
+ *       d_r = neighbour - target in double (exact), the covariance C = sum (d_r - mean)(d_r - mean)^T, mean = sum d_r /
+ *       k_normal, in double; its eigen-decomposition by cyclic Jacobi (at most 12 sweeps) in double; lambda0 <= lambda1 <=
+ *       lambda2.  The normal is the unit eigenvector of lambda0 (any sign), VALID when lambda0 < kappa lambda1, kappa = 1/4,
+ *       and when k_normal targets exist; stored in fp32.  Only targets with a valid normal can be matched.
+ *   State of segment (b, o): (R, c_x, c_y) in double.  c_x = the centroid of the taking-part members (sums over windows of
+ *       256 point ids, the windows' partial sums added); rho = sqrt(sum |x - c_x|^2 / n) over them (1 if 0).  Initially R =
+ *       R_in and c_y = R c_x + t_in (each entry (R_k0 c_0 + R_k1 c_1) + R_k2 c_2, then + t_k, rounded, none contracted).
+ *   Iteration (at most `iterations`), per live segment (one with a member that has not converged):
+ *     Move: R, c_x, c_y rounded to fp32 once; p = R (x - c_x) + c_y in fp32: d = x - c_x, p_k = ((R_k0 d_0 + R_k1 d_1) + R_k2
+ *       d_2) + c_y_k, each operation rounded to nearest, none contracted (the order of the fit's residual).
+ *     Match: the target q with a valid normal n that minimises (diff_sq(p, q), id) among those with diff_sq(p, q) <=
+ *       fl(max_distance * max_distance); none when there is no such target or p is not finite.  The search is exact.
+ *     Sums: r = n . (p - q), J = [((p - c_y) x n)^T, n^T] in double from the fp32 values; upper J^T J (21 values), J^T r (6),
+ *       the count and sum r^2, per window of 256 point ids (warp butterfly, then the warps in order), the windows added
+ *       (det_workspace: in fixed point, so a segment's sums are the bits of its own B = 1, O = 1 call).
+ *     Solve: with count < 6 no update (rank 0).  Otherwise the system scaled to unknowns (rho omega, dt) is decomposed by
+ *       cyclic Jacobi (at most 12 sweeps) in double and solved along the eigen-directions with lambda > 1e-4 lambda_max
+ *       only (the degeneracy-aware solution; rank = their number): z = -sum (v . g) / lambda v; then R <- exp([omega]x) R
+ *       (Rodrigues, double) and c_y <- c_y + dt.  The segment stops after the first update with rho |omega| + |dt| <= 1e-6.
+ *   pvraft_rigid_refine_fwd: xyz1 [B,N,3], xyz2 [B,M,3], labels, target_mask [B,M] uint8 or NULL, the fit R_in [B,O,3,3],
+ *       t_in [B,O,3], degenerate_in [B,O] uint8 -> R [B,O,3,3], t [B,O,3] fp32 (t = c_y - R c_x in double, rounded; a segment
+ *       that took no update keeps R_in and t_in bit for bit), degenerate [B,O] uint8 (degenerate_in AND last rank < 6),
+ *       matched [B,O] int32, rmse [B,O] f32 (sqrt(sum r^2 / matched), 0 with none), rank [B,O] int32 of the last iteration
+ *       the segment ran, steps [B,O] int32 (updates taken).  Optional (NULL to skip): history [B,O,iterations+1,12] double,
+ *       the state (R row-major, c_y) before the first and after every iteration; corr [B,N] int32, the last iteration's
+ *       matched target id of each member (-1 for none and off the members); normals [B,M,4] f32 (n, 1) or (0, 0, 0, 0) for
+ *       a target without a valid normal or a point that is no target; neighbours [B,M,k_normal] int32, each target's
+ *       neighbour ids nearest first (-1 for a slot no target filled, and for a point that is no target).  workspace:
+ *       pvraft_rigid_refine_workspace_bytes(B, N,
+ *       M, O, iterations) bytes, 16-byte aligned, no initialisation needed; det_workspace:
+ *       pvraft_rigid_refine_det_workspace_bytes(B, O, iterations) bytes or NULL ("Deterministic mode").  The correspondences
+ *       are exact fp32 decisions; only the sums depend on the mode.
+ * Null required pointers, labels NULL with O != 1, B < 1, N < 1, M < 1, O outside 1..256, B O > 65535, B N or B M >= 2^31,
+ * iterations outside 1..64, a max_distance that is not finite and > 0 or whose square overflows fp32, and k_normal outside
+ * 3..min(32, M) return PVRAFT_ERR_BAD_ARG before any launch. */
+PVRAFT_API int pvraft_rigid_refine_fwd(const float* xyz1, const float* xyz2, const int32_t* labels, const uint8_t* target_mask,
+                                       const float* R_in, const float* t_in, const uint8_t* degenerate_in, int B, int N, int M, int O,
+                                       int iterations, float max_distance, int k_normal, float* R, float* t, uint8_t* degenerate,
+                                       int32_t* matched, float* rmse, int32_t* rank, int32_t* steps, double* history, int32_t* corr,
+                                       float* normals, int32_t* neighbours, void* workspace, void* det_workspace, void* stream);
+PVRAFT_API int64_t pvraft_rigid_refine_workspace_bytes(int B, int N, int M, int O, int iterations);
+PVRAFT_API int64_t pvraft_rigid_refine_det_workspace_bytes(int B, int O, int iterations);
+
 /* Multi-object tracking from scene flow (no counterpart in the reference): one step of pvraft_b200.track.ObjectTracker.  A
  * sequence gives scans P_0, P_1, ...; for the pair (P_{t-1}, P_t) the caller has the flow F on P_{t-1} and the objects
  * found on P_{t-1} (pvraft_euclidean_clusters_fwd labels and num_objects, O slots).  A step associates them with the O_prev

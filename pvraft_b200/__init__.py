@@ -8,12 +8,13 @@ from .loss import flow_consistency
 from .pointconv import knn_point, square_distance
 from .raft import RSF, RSF_refine
 from .refine import FlotRefine
-from .rigid import RigidMotion, RigidObjects, rigid_flow, rigid_motion, rigid_objects
+from .rigid import RigidMotion, RigidObjects, RigidRefinement, rigid_flow, rigid_motion, rigid_objects, rigid_refine
 from .stream import SceneFlowStream
 from .track import ObjectTracker, ObjectTracks
 from .update import ConvGRU, ConvRNN, FlowHead, MotionEncoder, UpdateBlock
 
 __all__ = ['RSF', 'RSF_refine', 'CorrBlock', 'UpdateBlock', 'MotionEncoder', 'ConvGRU', 'ConvRNN', 'FlowHead',
            'FlotEncoder', 'FlotRefine', 'SetConv', 'Graph', 'knn_point', 'square_distance', 'SceneFlowStream',
-           'flow_consistency', 'rigid_motion', 'RigidMotion', 'rigid_objects', 'RigidObjects', 'rigid_flow', 'ObjectTracker',
+           'flow_consistency', 'rigid_motion', 'RigidMotion', 'rigid_objects', 'RigidObjects', 'rigid_flow', 'rigid_refine',
+           'RigidRefinement', 'ObjectTracker',
            'ObjectTracks']

@@ -26,7 +26,7 @@
 // double state the forward saves (eigenvectors, eigenvalues, centroids, count):
 //   dt -> d y-bar += dt, d x-bar -= R^T dt, dR -= dt x-bar^T;  dR -> dq through R(q);  dq -> dN = sym(sum_{j>=1} v_j v_j^T dq
 //   v_0^T / (lambda0 - lambda_j));  dN -> dS;  dx_i = dS (y_i - y-bar) + d x-bar / n, dy_i = dS^T (x_i - x-bar) + d y-bar / n.
-#include "fixed_point.cuh"
+#include "rigid_segments.cuh"
 
 namespace pvraft {
 
@@ -37,7 +37,6 @@ constexpr int kRmMaxH = 4096;
 constexpr int kRmMaxRounds = 8;
 constexpr double kCollinearTol = 1e-6;
 constexpr double kGapTol = 1e-5;
-constexpr int kJacobiSweeps = 12;
 
 __host__ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long z) {
     z += 0x9e3779b97f4a7c15ull;
@@ -63,40 +62,7 @@ __device__ __forceinline__ void horn_matrix(const double (&S)[9], double (&a)[4]
 }
 
 // Cyclic Jacobi on a symmetric 4x4 matrix: a becomes diagonal (the eigenvalues), column j of v the eigenvector of a[j][j].
-__device__ __forceinline__ void jacobi4(double (&a)[4][4], double (&v)[4][4]) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) v[i][j] = i == j ? 1.0 : 0.0;
-    for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
-        const double off = fabs(a[0][1]) + fabs(a[0][2]) + fabs(a[0][3]) + fabs(a[1][2]) + fabs(a[1][3]) + fabs(a[2][3]);
-        if (off == 0.0) break;
-#pragma unroll
-        for (int p = 0; p < 3; ++p)
-#pragma unroll
-            for (int q = p + 1; q < 4; ++q) {
-                const double apq = a[p][q];
-                if (apq == 0.0) continue;
-                const double theta = (a[q][q] - a[p][p]) / (2.0 * apq);
-                const double t = fabs(theta) > 1e150 ? 0.5 / theta : copysign(1.0, theta) / (fabs(theta) + sqrt(theta * theta + 1.0));
-                const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-                a[p][p] -= t * apq;
-                a[q][q] += t * apq;
-                a[p][q] = a[q][p] = 0.0;
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    if (k != p && k != q) {
-                        const double akp = a[k][p], akq = a[k][q];
-                        a[k][p] = a[p][k] = c * akp - s * akq;
-                        a[k][q] = a[q][k] = s * akp + c * akq;
-                    }
-                    const double vkp = v[k][p], vkq = v[k][q];
-                    v[k][p] = c * vkp - s * vkq;
-                    v[k][q] = s * vkp + c * vkq;
-                }
-            }
-    }
-}
+__device__ __forceinline__ void jacobi4(double (&a)[4][4], double (&v)[4][4]) { jacobi_sym<4>(a, v); }
 
 __device__ __forceinline__ void quat_rot(const double (&q)[4], double (&R)[9]) {
     const double w = q[0], x = q[1], y = q[2], z = q[3];
@@ -216,19 +182,6 @@ __global__ void __launch_bounds__(kRmScan) k_rigid_allowed(const int32_t* __rest
     __syncthreads();
     if (threadIdx.x == 0) nmem[s] = base_sh;
 }
-
-// The segments of one fit: segment g is a subset of sample g / per, and its members, ascending, are list[first(g), first(g) +
-// count(g)), first(g) = start[g] (g N with start NULL: k_rigid_allowed) -- or, with list NULL (no labels), all N points of
-// the sample.
-struct RmSegs {
-    const int32_t* list;    // [B,N] member ids, or NULL
-    const int32_t* start;   // [G] offset of each segment's members in list, or NULL
-    const int32_t* n;       // [G] member counts (read with list only)
-    int N, per;
-    __device__ __forceinline__ int count(int g) const { return list ? n[g] : N; }
-    __device__ __forceinline__ long long first(int g) const { return start ? (long long)start[g] : (long long)g * N; }
-    __device__ __forceinline__ int member(int g, long long j) const { return list ? __ldg(list + first(g) + j) : (int)j; }
-};
 
 // One thread per (segment, hypothesis): draw, test and fit the triple -> hyp [G,H,kRmModel] (flag 1: accepted, 0: rejected),
 // hcnt [G,H] zeroed, triples [G,H,3] (or NULL: the drawn point indices, -1 with no member)
@@ -406,7 +359,6 @@ __global__ void __launch_bounds__(kSelThreads) k_rigid_select(const float* __res
 // membership labels == o): grid (any, B), each CTA taking items x, x + gridDim.x, ...; inliers written for members only.
 // A window's partial sum is the same value either way, so in the DET form a segment's moments are those of the one-segment
 // launch with labels = where(labels == o, 0, -1).
-constexpr int kMomThreads = 256;
 template <bool DET>
 __global__ void __launch_bounds__(kMomThreads) k_rigid_moments(const float* __restrict__ x, const float* __restrict__ f,
                                                                const int32_t* __restrict__ labels, const int32_t* __restrict__ items,
@@ -634,9 +586,6 @@ __global__ void __launch_bounds__(256) k_rigid_bwd(const float* __restrict__ x, 
 //                       holding a member of o, and the score items (j << 8) | o of every kScPoints members of o
 //   k_ro_group_scatter  per window, each point's rank among the window's points of its object (warp match, then the warps
 //                       before it): list[pre + rank] = i, so each object's members are ascending
-constexpr int kRoChunk = 256;
-constexpr int kRoMaxObjects = 256;
-static_assert(kRoChunk == kMomThreads, "the moment items are the grouping's windows");
 
 __global__ void __launch_bounds__(kRoChunk) k_ro_group_count(const int32_t* __restrict__ labels, int N, int O, int C,
                                                              int32_t* __restrict__ cnt) {
@@ -728,16 +677,47 @@ __global__ void __launch_bounds__(kRoChunk) k_ro_group_scatter(const int32_t* __
     list[(long long)s * N + __ldg(pre + ((long long)s * C + c) * O + l) + before] = i;
 }
 
-// the forward's workspace: list [B,N] | start [G] | n [G] | cnt [B,C,O] | pre [B,C,O] | moment items [B,N] | nm [B] |
-// score items [B,S] | ns [B] | hyp [G,H,16] f32 | hcnt [G,H] | model [G,16] f32 | mom [rounds,G,16] f64, each range 16-byte
-// aligned (O = 1 uses list and n only of the grouping's ranges)
+RmGroupWs rm_group_carve(char* base, int64_t& off, int B, int N, int O) {
+    auto take = [&](int64_t bytes) {
+        char* p = base ? base + off : nullptr;
+        off += (bytes + 15) / 16 * 16;
+        return reinterpret_cast<int32_t*>(p);
+    };
+    RmGroupWs L;
+    const long long G = (long long)B * O;
+    L.C = (N + kRoChunk - 1) / kRoChunk;
+    L.S = (N + kScPoints - 1) / kScPoints + O;
+    L.list = take(4ll * B * N);
+    L.start = take(4 * G);
+    L.n = take(4 * G);
+    L.cnt = take(4ll * B * L.C * O);
+    L.pre = take(4ll * B * L.C * O);
+    L.mitems = take(4ll * B * N);
+    L.nm = take(4ll * B);
+    L.sitems = take(4ll * B * L.S);
+    L.ns = take(4ll * B);
+    return L;
+}
+
+int rm_group(const int32_t* labels, int B, int N, int O, const RmGroupWs& L, cudaStream_t st) {
+    if (O == 1) {
+        if (labels) k_rigid_allowed<<<B, kRmScan, 0, st>>>(labels, N, L.list, L.n);
+    } else {
+        k_ro_group_count<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.cnt);
+        k_ro_group_scan<<<B, kRoMaxObjects, 0, st>>>(L.cnt, N, O, L.C, L.S, L.pre, L.start, L.n, L.mitems, L.nm, L.sitems, L.ns);
+        k_ro_group_scatter<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.pre, L.list);
+    }
+    return check_launch("rigid segment grouping");
+}
+
+// the forward's workspace: the grouping's ranges (RmGroupWs) | hyp [G,H,16] f32 | hcnt [G,H] | model [G,16] f32 | mom
+// [rounds,G,16] f64, each range 16-byte aligned
 struct FitWs {
-    int32_t *list, *start, *n, *cnt, *pre, *mitems, *nm, *sitems, *ns;
+    RmGroupWs grp;
     float* hyp;
     int32_t* hcnt;
     float* model;
     double* mom;
-    int C, S;
     int64_t bytes;
 };
 static FitWs fit_ws(void* ws, int B, int N, int O, int H, int rounds) {
@@ -750,17 +730,7 @@ static FitWs fit_ws(void* ws, int B, int N, int O, int H, int rounds) {
     };
     FitWs L;
     const long long G = (long long)B * O;
-    L.C = (N + kRoChunk - 1) / kRoChunk;
-    L.S = (N + kScPoints - 1) / kScPoints + O;
-    L.list = reinterpret_cast<int32_t*>(take(4ll * B * N));
-    L.start = reinterpret_cast<int32_t*>(take(4 * G));
-    L.n = reinterpret_cast<int32_t*>(take(4 * G));
-    L.cnt = reinterpret_cast<int32_t*>(take(4ll * B * L.C * O));
-    L.pre = reinterpret_cast<int32_t*>(take(4ll * B * L.C * O));
-    L.mitems = reinterpret_cast<int32_t*>(take(4ll * B * N));
-    L.nm = reinterpret_cast<int32_t*>(take(4ll * B));
-    L.sitems = reinterpret_cast<int32_t*>(take(4ll * B * L.S));
-    L.ns = reinterpret_cast<int32_t*>(take(4ll * B));
+    L.grp = rm_group_carve(base, off, B, N, O);
     L.hyp = reinterpret_cast<float*>(take(4 * G * H * kRmModel));
     L.hcnt = reinterpret_cast<int32_t*>(take(4 * G * H));
     L.model = reinterpret_cast<float*>(take(4 * G * kRmModel));
@@ -800,25 +770,22 @@ extern "C" int pvraft_rigid_objects_fwd(const float* xyz1, const float* flow, co
     const float thr2 = threshold * threshold;
     // O = 1: the member list in one launch (none without labels), and the score and moment kernels' one-segment grids;
     // O > 1: the stable grouping, and work items that cover each segment's members
+    const RmGroupWs& Lg = L.grp;
     const int32_t *sitems = nullptr, *nsitems = nullptr, *mitems = nullptr, *nmitems = nullptr;
-    unsigned score_x = (unsigned)((N + kScPoints - 1) / kScPoints), mom_x = (unsigned)L.C;
-    if (O == 1) {
-        if (labels) k_rigid_allowed<<<B, kRmScan, 0, st>>>(labels, N, L.list, L.n);
-    } else {
+    unsigned score_x = (unsigned)((N + kScPoints - 1) / kScPoints), mom_x = (unsigned)Lg.C;
+    if (O > 1) {
         cudaError_t e = cudaMemsetAsync(inliers, 0, (size_t)B * N, st);   // the moments write the members' inliers only
         if (e != cudaSuccess) return fail((int)e, "rigid_objects_fwd: memset failed: %s", cudaGetErrorString(e));
-        k_ro_group_count<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.cnt);
-        k_ro_group_scan<<<B, kRoMaxObjects, 0, st>>>(L.cnt, N, O, L.C, L.S, L.pre, L.start, L.n, L.mitems, L.nm, L.sitems, L.ns);
-        k_ro_group_scatter<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.pre, L.list);
-        sitems = L.sitems, nsitems = L.ns, mitems = L.mitems, nmitems = L.nm;
-        score_x = (unsigned)L.S;
+        sitems = Lg.sitems, nsitems = Lg.ns, mitems = Lg.mitems, nmitems = Lg.nm;
+        score_x = (unsigned)Lg.S;
         mom_x += (unsigned)O;
     }
-    const RmSegs sg{labels ? L.list : nullptr, O > 1 ? L.start : nullptr, L.n, N, O};
+    if (int rc = rm_group(labels, B, N, O, Lg, st)) return rc;
+    const RmSegs sg = rm_segs(labels, N, O, Lg);
     k_rigid_hypotheses<<<dim3((unsigned)((H + 127) / 128), (unsigned)G), 128, 0, st>>>(xyz1, flow, sg, H, (unsigned long long)seed,
                                                                                       threshold, L.hyp, L.hcnt, triples);
     k_rigid_score<<<dim3(score_x, (unsigned)((H + kScHyp - 1) / kScHyp), (unsigned)B), kScThreads, 0, st>>>(
-        xyz1, flow, sg, sitems, nsitems, L.S, H, thr2, L.hyp, L.hcnt);
+        xyz1, flow, sg, sitems, nsitems, Lg.S, H, thr2, L.hyp, L.hcnt);
     k_rigid_select<<<G, kSelThreads, 0, st>>>(xyz1, flow, sg, H, G, rounds, L.hyp, L.hcnt, L.model, L.mom, hyp_count);
     const unsigned sblocks = (unsigned)((G + 63) / 64);
     for (int r = 0; r < rounds; ++r) {

@@ -1121,6 +1121,35 @@ def rigid_objects_bwd(x, f, labels, inliers, state, dR, dt):
     return d_x, d_f
 
 
+RIGID_REFINE_MAX_ITERATIONS = 64   # pvraft_rigid_refine_fwd runs at most this many ICP iterations
+RIGID_REFINE_K_NORMAL = (3, 32)    # the normals' neighbour counts it accepts
+
+
+def rigid_refine(x1, x2, labels, target_mask, R, t, degenerate, iterations, max_distance, k_normal, want_trace=False):
+    """x1 [B,N,3] f32, x2 [B,M,3] f32, labels [B,N] int32 (segment o of sample b: labels[b] == o), target_mask [B,M] uint8 or
+    None, the fit R [B,O,3,3], t [B,O,3] f32, degenerate [B,O] uint8 -> (R, t, degenerate, matched [B,O] int32, rmse [B,O]
+    f32, rank, steps [B,O] int32), plus (history [B,O,iterations+1,12] f64, corr [B,N] int32, normals [B,M,4] f32,
+    neighbours [B,M,k_normal] int32) with want_trace.  Point-to-plane ICP of every segment against x2 (include/pvraft_b200.h, pvraft_rigid_refine_fwd); the
+    arguments are checked by pvraft_b200.rigid_refine."""
+    b, n, m, o = int(x1.shape[0]), int(x1.shape[1]), int(x2.shape[1]), int(R.shape[1])
+    dev = x1.device
+    R_out = torch.empty(b, o, 3, 3, dtype=torch.float32, device=dev)
+    t_out = torch.empty(b, o, 3, dtype=torch.float32, device=dev)
+    degen = torch.empty(b, o, dtype=torch.uint8, device=dev)
+    matched, rank, steps = (torch.empty(b, o, dtype=torch.int32, device=dev) for _ in range(3))
+    rmse = torch.empty(b, o, dtype=torch.float32, device=dev)
+    hist = torch.empty(b, o, iterations + 1, 12, dtype=torch.float64, device=dev) if want_trace else None
+    corr = torch.empty(b, n, dtype=torch.int32, device=dev) if want_trace else None
+    normals = torch.empty(b, m, 4, dtype=torch.float32, device=dev) if want_trace else None
+    nbr = torch.empty(b, m, k_normal, dtype=torch.int32, device=dev) if want_trace else None
+    ws = _workspace(abi.rigid_refine_workspace_bytes(b, n, m, o, iterations), dev)
+    det = _det_workspace(abi.rigid_refine_det_workspace_bytes, b, o, iterations, device=dev)
+    abi.rigid_refine_fwd(x1, x2, labels, target_mask, R, t, degenerate, b, n, m, o, iterations, float(max_distance), k_normal, R_out,
+                         t_out, degen, matched, rmse, rank, steps, hist, corr, normals, nbr, ws, det)
+    out = (R_out, t_out, degen, matched, rmse, rank, steps)
+    return out + (hist, corr, normals, nbr) if want_trace else out
+
+
 TRACK_MIN_OVERLAP = 1 / 16   # pvraft_track_objects_fwd's least min_overlap: a slot then has at most 16 eligible pairs
 
 

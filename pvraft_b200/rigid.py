@@ -173,3 +173,91 @@ def rigid_flow(xyz1, flow, objects, ego=None):
     moved = torch.einsum('bnjk,bnk->bnj', R, xyz1) + t - xyz1
     use = objects.inliers & (lab >= 0) & ~torch.gather(objects.degenerate, 1, idx)
     return torch.where(use[..., None], moved, out)
+
+
+class RigidRefinement(NamedTuple):
+    fit: object                 # the input's type (RigidMotion or RigidObjects) with rotation and translation refined
+    matched: torch.Tensor       # [B,O] int32: correspondences of the last iteration (O = 1 for a RigidMotion)
+    rmse: torch.Tensor          # [B,O] f32: their point-to-plane RMS residual (metres)
+    rank: torch.Tensor          # [B,O] int32: the directions of (rotation, translation) the last iteration could observe
+    steps: torch.Tensor         # [B,O] int32: the updates each fit took
+
+
+def _check_cloud(name, arg, v):
+    if not torch.is_tensor(v) or v.dim() != 3 or v.shape[-1] != 3 or not v.is_floating_point():
+        raise ValueError(f'{name}: expected {arg} [B,N,3] floating point, got {tuple(v.shape) if torch.is_tensor(v) else type(v)}')
+
+
+def rigid_refine(xyz1, xyz2, fit, target_mask=None, iterations=10, max_distance=0.3, k_normal=16):
+    """Refine rigid fits of xyz1 [B,N,3] against the second scan xyz2 [B,M,3] by point-to-plane ICP on the device: `fit` is
+    a RigidMotion (one segment per sample: its inliers) or a RigidObjects (segment o: the inliers labelled o), and each
+    segment's points, moved by its fit, are matched to the nearest point of xyz2 within `max_distance` (metres) that has a
+    valid normal (from its `k_normal` nearest neighbours), for at most `iterations` Gauss-Newton steps.  Directions the
+    matched surfaces leave unobservable (a flat ground, a single wall) keep the input fit's value.  target_mask (bool
+    [B,M]) leaves points of xyz2 out of the targets, e.g. the ground or known movers.  -> RigidRefinement whose `fit` has
+    the input's type, labels, inliers and counts, so rigid_flow and ObjectTracker.step take it as they take the input; a
+    degenerate input fit becomes proper only when all six directions were observed.  The outputs carry no gradient
+    (rigid_motion is the differentiable path).  Nothing synchronises with the host, so the call can be captured in a CUDA
+    graph; under torch.use_deterministic_algorithms(True) the result is bitwise reproducible, a batched call equals
+    per-sample calls, and object o's result equals that of the object refined alone.  max_distance = 0.3 m, k_normal = 16
+    and the solver's thresholds have not been checked against real scans."""
+    name = 'rigid_refine'
+    _check_cloud(name, 'xyz1', xyz1)
+    _check_cloud(name, 'xyz2', xyz2)
+    b, n, m = int(xyz1.shape[0]), int(xyz1.shape[1]), int(xyz2.shape[1])
+    if b < 1 or n < 1 or m < 1 or int(xyz2.shape[0]) != b:
+        raise ValueError(f'rigid_refine: xyz1 {tuple(xyz1.shape)} and xyz2 {tuple(xyz2.shape)} need the same B >= 1 and N, M >= 1')
+    if b * n >= 2 ** 31 or b * m >= 2 ** 31:
+        raise ValueError(f'rigid_refine: B N = {b * n}, B M = {b * m} points (at most 2^31 - 1 each)')
+    if isinstance(fit, RigidMotion):
+        o = 1
+        shapes = ((fit.rotation, (b, 3, 3)), (fit.translation, (b, 3)), (fit.inliers, (b, n)), (fit.degenerate, (b,)))
+    elif isinstance(fit, RigidObjects):
+        o = int(fit.rotation.shape[1]) if torch.is_tensor(fit.rotation) and fit.rotation.dim() == 4 else -1
+        shapes = ((fit.rotation, (b, o, 3, 3)), (fit.translation, (b, o, 3)), (fit.inliers, (b, n)), (fit.labels, (b, n)),
+                  (fit.degenerate, (b, o)))
+    else:
+        raise ValueError(f'rigid_refine: fit must be a RigidMotion or a RigidObjects, got {type(fit)}')
+    for v, want in shapes:
+        if not torch.is_tensor(v) or tuple(v.shape) != want:
+            raise ValueError(f'rigid_refine: the fit\'s tensors do not match xyz1 {tuple(xyz1.shape)}: expected {want}, got '
+                             f'{tuple(v.shape) if torch.is_tensor(v) else type(v)}')
+    kinds = [(fit.rotation, 'rotation', 'floating point', lambda v: v.is_floating_point()),
+             (fit.translation, 'translation', 'floating point', lambda v: v.is_floating_point()),
+             (fit.inliers, 'inliers', 'bool', lambda v: v.dtype == torch.bool),
+             (fit.degenerate, 'degenerate', 'bool', lambda v: v.dtype == torch.bool)]
+    if isinstance(fit, RigidObjects):
+        kinds.append((fit.labels, 'labels', 'int32', lambda v: v.dtype == torch.int32))
+    for v, arg, kind, ok in kinds:
+        if not ok(v):
+            raise ValueError(f'rigid_refine: the fit\'s {arg} must be {kind}, got {v.dtype}')
+    if not 1 <= o <= ops.RIGID_MAX_OBJECTS or b * o > 65535:
+        raise ValueError(f'rigid_refine: {o} objects per sample at B = {b} (1..{ops.RIGID_MAX_OBJECTS}, B O at most 65535)')
+    if target_mask is not None and (not torch.is_tensor(target_mask) or target_mask.dtype != torch.bool or
+                                    tuple(target_mask.shape) != (b, m)):
+        raise ValueError(f'rigid_refine: target_mask must be bool [{b},{m}], got '
+                         f'{(tuple(target_mask.shape), target_mask.dtype) if torch.is_tensor(target_mask) else type(target_mask)}')
+    if not _is_int(iterations) or not 1 <= iterations <= ops.RIGID_REFINE_MAX_ITERATIONS:
+        raise ValueError(f'rigid_refine: iterations={iterations!r} must be an integer in 1..{ops.RIGID_REFINE_MAX_ITERATIONS}')
+    _positive(name, 'max_distance', max_distance)
+    lo, hi = ops.RIGID_REFINE_K_NORMAL
+    if not _is_int(k_normal) or not lo <= k_normal <= min(hi, m):
+        raise ValueError(f'rigid_refine: k_normal={k_normal!r} must be an integer in {lo}..min({hi}, M = {m})')
+    _need_cuda(xyz1, xyz2, target_mask, *(v for v, *_ in kinds))
+    with torch.no_grad():
+        x1, x2 = xyz1.float().contiguous(), xyz2.float().contiguous()
+        if o == 1:   # where(inliers, 0, -1), one elementwise launch
+            labels = torch.empty(b, n, dtype=torch.int32, device=x1.device)
+            torch.add(fit.inliers, -1, out=labels)
+        else:
+            labels = torch.where(fit.inliers, fit.labels, -1).contiguous()
+        tm = None if target_mask is None else target_mask.contiguous().view(torch.uint8)
+        R, t, degen, matched, rmse, rank, steps = ops.rigid_refine(
+            x1, x2, labels, tm, fit.rotation.detach().float().reshape(b, o, 3, 3).contiguous(),
+            fit.translation.detach().float().reshape(b, o, 3).contiguous(), fit.degenerate.reshape(b, o).contiguous().view(torch.uint8),
+            iterations, float(max_distance), k_normal)
+    if o == 1 and isinstance(fit, RigidMotion):
+        out = fit._replace(rotation=R.view(b, 3, 3), translation=t.view(b, 3), degenerate=degen.view(b).bool())
+    else:
+        out = fit._replace(rotation=R, translation=t, degenerate=degen.bool())
+    return RigidRefinement(out, matched, rmse, rank, steps)
