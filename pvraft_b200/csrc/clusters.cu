@@ -2,8 +2,8 @@
 // the objects of pvraft_b200.rigid_objects.  Every decision is an integer one, so the labels are the same bits in any mode
 // and from run to run (the rule is stated in include/pvraft_b200.h, pvraft_euclidean_clusters_fwd):
 //
-//   k_cc_stage    a point takes part when allowed (mask) and finite: its coordinates are staged as they are, any other point's
-//                 as NaN, so the index's bounds ignore it and no distance to it compares <= r2; parent[i] = i
+//   k_cc_stage    a point takes part when allowed (mask) and finite (takes_part): its coordinates are staged as they are,
+//                 any other point's as NaN, so the index's bounds ignore it and no distance to it compares <= r2; parent[i] = i
 //   (index)       grid_index_build on the staged cloud
 //   k_cc_edges    one warp per query: grid_radius_visit (grid_index.cuh, exact for the fp32 predicate); every edge (i, j) with
 //                 j < i is united: the two roots are found (path halving) and the larger is hooked under the smaller with an
@@ -15,13 +15,13 @@
 //                 largest key by an 8-bit radix select, then each kept key's rank among the kept (a count) is its object
 //   k_cc_label    labels[i] = the object of i's root, or -1
 #include "grid_index.cuh"
+#include "rigid_segments.cuh"
 
 namespace pvraft {
 
 constexpr int kCcThreads = 256;
 constexpr int kCcWarps = kCcThreads / kWarp;
 constexpr int kCcRankThreads = 1024;
-constexpr int kCcMaxObjects = 256;
 
 __global__ void __launch_bounds__(kCcThreads) k_cc_stage(const float* __restrict__ xyz, const uint8_t* __restrict__ mask, int N,
                                                          long long points, float* __restrict__ staged, int32_t* __restrict__ parent,
@@ -29,7 +29,7 @@ __global__ void __launch_bounds__(kCcThreads) k_cc_stage(const float* __restrict
     const long long p = (long long)blockIdx.x * kCcThreads + threadIdx.x;
     if (p >= points) return;
     const float x = xyz[3 * p], y = xyz[3 * p + 1], z = xyz[3 * p + 2];
-    const bool on = (!mask || mask[p] != 0) && isfinite(x) && isfinite(y) && isfinite(z);
+    const bool on = takes_part(mask, p, x, y, z);
     staged[3 * p] = on ? x : NAN;
     staged[3 * p + 1] = on ? y : NAN;
     staged[3 * p + 2] = on ? z : NAN;
@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(kCcRankThreads) k_cc_rank(const int32_t* __res
                                                             unsigned long long* __restrict__ cand, int32_t* __restrict__ objmap,
                                                             int32_t* __restrict__ counts, int32_t* __restrict__ num_objects) {
     __shared__ int n_sh, nsel_sh, hist[256];
-    __shared__ unsigned long long sel[kCcMaxObjects];
+    __shared__ unsigned long long sel[kMaxObjects];
     __shared__ unsigned long long prefix_sh;
     const int s = blockIdx.x;
     const int32_t* sz = size + (long long)s * N;
@@ -196,22 +196,16 @@ struct ClusterWs {
     int64_t bytes;
 };
 static ClusterWs cluster_ws(void* ws, int B, int N) {
-    char* base = static_cast<char*>(ws);
-    int64_t off = 0;
-    auto take = [&](int64_t bytes) {
-        char* p = base ? base + off : nullptr;
-        off += (bytes + 15) / 16 * 16;
-        return p;
-    };
+    ByteCarve w(ws);
     const long long pts = (long long)B * N;
     ClusterWs L;
-    L.index = take(grid_index_bytes(B, N));
-    L.staged = reinterpret_cast<float*>(take(12 * pts));
-    L.parent = reinterpret_cast<int32_t*>(take(4 * pts));
-    L.size = reinterpret_cast<int32_t*>(take(4 * pts));
-    L.objmap = reinterpret_cast<int32_t*>(take(4 * pts));
-    L.cand = reinterpret_cast<unsigned long long*>(take(8 * pts));
-    L.bytes = off;
+    L.index = w.take<void>(grid_index_bytes(B, N));
+    L.staged = w.take<float>(12 * pts);
+    L.parent = w.take<int32_t>(4 * pts);
+    L.size = w.take<int32_t>(4 * pts);
+    L.objmap = w.take<int32_t>(4 * pts);
+    L.cand = w.take<unsigned long long>(8 * pts);
+    L.bytes = w.bytes;
     return L;
 }
 
@@ -229,7 +223,7 @@ extern "C" int pvraft_euclidean_clusters_fwd(const float* xyz, const float* flow
                                              float flow_radius, int min_points, int max_objects, int32_t* labels,
                                              int32_t* num_objects, int32_t* counts, void* workspace, void* stream) {
     if (!xyz || !labels || !num_objects || !counts || !workspace || B < 1 || N < 1 || (long long)B * N > 0x7fffffffll ||
-        bad_radius(radius) || (flow && bad_radius(flow_radius)) || min_points < 1 || max_objects < 1 || max_objects > kCcMaxObjects)
+        bad_radius(radius) || (flow && bad_radius(flow_radius)) || min_points < 1 || max_objects < 1 || max_objects > kMaxObjects)
         return fail(PVRAFT_ERR_BAD_ARG, "euclidean_clusters_fwd: bad argument");
     if (B > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "euclidean_clusters_fwd: B = %d samples (at most 65535)", B);
     if (reinterpret_cast<uintptr_t>(workspace) & 15) return fail(PVRAFT_ERR_BAD_ARG, "euclidean_clusters_fwd: workspace not 16-byte aligned");

@@ -152,6 +152,20 @@ struct FxCarve {
     int64_t bytes() const { return fx_bytes(slots); }
 };
 
+// Host: a workspace carved into consecutive byte ranges, each starting 16-byte aligned, in the order of the take() calls;
+// a null base only counts (bytes: the size so far)
+struct ByteCarve {
+    char* base;
+    int64_t bytes = 0;
+    explicit ByteCarve(void* ws) : base(static_cast<char*>(ws)) {}
+    template <typename T>
+    T* take(int64_t n) {
+        T* r = reinterpret_cast<T*>(base ? base + bytes : nullptr);
+        bytes += (n + 15) / 16 * 16;
+        return r;
+    }
+};
+
 // The [B,16] GroupNorm statistics (slot b * 16 + 2 * group + moment) of k_linear, k_tc_linear, k_setconv_edge_pairs and
 // k_edge_fwd
 inline int64_t gn_stats_ws_bytes(int B) { return fx_bytes(16ll * B); }

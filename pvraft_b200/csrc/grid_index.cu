@@ -10,6 +10,7 @@
 // The ranks come from atomics, so the order of the points WITHIN a cell can differ from run to run.  That is allowed only
 // because every search on the index ranks candidates on (distance, original id) and visits a cell's points as a set: the
 // result does not depend on the order inside a cell, and is bitwise the same from run to run.
+#include "fixed_point.cuh"
 #include "grid_index.cuh"
 
 namespace pvraft {
@@ -166,8 +167,6 @@ __global__ void __launch_bounds__(kGiThreads) k_gi_scatter(const float* __restri
     ids[dst] = i;
 }
 
-static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
-
 int grid_index_cells(int N) {
     const long long c = (long long)kGridCellsPerPoint * N;
     return (int)(c < kGridMinCells ? kGridMinCells : (c > (1 << 28) ? (1 << 28) : c));
@@ -175,60 +174,58 @@ int grid_index_cells(int N) {
 
 // workspace: float4 pts[S*N] | int32 ids[S*N] | int32 key[S*N] | int32 rank[S*N] | int32 cell_start[S*(cells+1)] |
 //            GridParams[S] | unsigned lo[S*4] | unsigned hi[S*4], every block 16-byte aligned
-static size_t part_bytes(int S, int N, size_t out[8]) {
-    const size_t sn = (size_t)S * N;
-    const size_t cs = (size_t)S * (grid_index_cells(N) + 1);
-    const size_t sizes[8] = {sn * sizeof(float4), sn * 4, sn * 4, sn * 4, cs * 4, (size_t)S * sizeof(GridParams), (size_t)S * 16, (size_t)S * 16};
-    size_t off = 0;
-    for (int i = 0; i < 8; ++i) {
-        out[i] = off;
-        off += align16(sizes[i]);
-    }
-    return off;
+struct GiWs {
+    float4* pts;
+    int32_t *ids, *key, *rank, *cell_start;
+    GridParams* params;
+    unsigned *lo, *hi;
+    int64_t bytes;
+};
+static GiWs gi_ws(void* ws, int S, int N) {
+    ByteCarve w(ws);
+    const long long sn = (long long)S * N;
+    GiWs L;
+    L.pts = w.take<float4>(sn * (long long)sizeof(float4));
+    L.ids = w.take<int32_t>(4 * sn);
+    L.key = w.take<int32_t>(4 * sn);
+    L.rank = w.take<int32_t>(4 * sn);
+    L.cell_start = w.take<int32_t>(4ll * S * (grid_index_cells(N) + 1));
+    L.params = w.take<GridParams>((long long)S * (long long)sizeof(GridParams));
+    L.lo = w.take<unsigned>(16ll * S);
+    L.hi = w.take<unsigned>(16ll * S);
+    L.bytes = w.bytes;
+    return L;
 }
 
-int64_t grid_index_bytes(int S, int N) {
-    if (S < 1 || N < 1) return 0;
-    size_t off[8];
-    return (int64_t)part_bytes(S, N, off);
-}
+int64_t grid_index_bytes(int S, int N) { return S < 1 || N < 1 ? 0 : gi_ws(nullptr, S, N).bytes; }
 
 GridIndex grid_index_carve(void* workspace, int S, int N) {
-    size_t off[8];
-    part_bytes(S, N, off);
-    char* w = static_cast<char*>(workspace);
-    return GridIndex{reinterpret_cast<float4*>(w + off[0]), reinterpret_cast<int32_t*>(w + off[1]), reinterpret_cast<int32_t*>(w + off[4]),
-                     reinterpret_cast<GridParams*>(w + off[5]), grid_index_cells(N)};
+    const GiWs L = gi_ws(workspace, S, N);
+    return GridIndex{L.pts, L.ids, L.cell_start, L.params, grid_index_cells(N)};
 }
 
 int grid_index_build(const float* xyz, const float* offset, int S, int N, void* workspace, cudaStream_t st, GridIndex* ix) {
     if (!xyz || !workspace || S < 1 || N < 1) return fail(PVRAFT_ERR_BAD_ARG, "grid_index: bad argument");
     if (S > 65535) return fail(PVRAFT_ERR_UNSUPPORTED, "grid_index: S = %d samples (at most 65535)", S);
     if (reinterpret_cast<uintptr_t>(workspace) & 15) return fail(PVRAFT_ERR_BAD_ARG, "grid_index: workspace not 16-byte aligned");
-    size_t off[8];
-    part_bytes(S, N, off);
-    char* w = static_cast<char*>(workspace);
+    const GiWs L = gi_ws(workspace, S, N);
     *ix = grid_index_carve(workspace, S, N);
-    int32_t* key = reinterpret_cast<int32_t*>(w + off[2]);
-    int32_t* rank = reinterpret_cast<int32_t*>(w + off[3]);
-    unsigned* lo = reinterpret_cast<unsigned*>(w + off[6]);
-    unsigned* hi = reinterpret_cast<unsigned*>(w + off[7]);
     const int cells = ix->cells;
-    cudaError_t e = cudaMemsetAsync(lo, 0xff, (size_t)S * 16, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(hi, 0, (size_t)S * 16, st);
+    cudaError_t e = cudaMemsetAsync(L.lo, 0xff, (size_t)S * 16, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(L.hi, 0, (size_t)S * 16, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ix->cell_start, 0, (size_t)S * (cells + 1) * 4, st);
     if (e != cudaSuccess) return fail((int)e, "grid_index: memset failed: %s", cudaGetErrorString(e));
     const int per_sample = (N + kGiThreads - 1) / kGiThreads;
     int rc;
-    k_gi_bounds<<<dim3(min(per_sample, kGiBoundCtas), S), kGiThreads, 0, st>>>(xyz, offset, N, lo, hi);
+    k_gi_bounds<<<dim3(min(per_sample, kGiBoundCtas), S), kGiThreads, 0, st>>>(xyz, offset, N, L.lo, L.hi);
     if ((rc = check_launch("grid_index bounds"))) return rc;
-    k_gi_params<<<(S + 31) / 32, 32, 0, st>>>(lo, hi, S, N, cells, ix->params);
+    k_gi_params<<<(S + 31) / 32, 32, 0, st>>>(L.lo, L.hi, S, N, cells, ix->params);
     if ((rc = check_launch("grid_index params"))) return rc;
-    k_gi_count<<<dim3(per_sample, S), kGiThreads, 0, st>>>(xyz, offset, N, cells, ix->params, ix->cell_start, key, rank);
+    k_gi_count<<<dim3(per_sample, S), kGiThreads, 0, st>>>(xyz, offset, N, cells, ix->params, ix->cell_start, L.key, L.rank);
     if ((rc = check_launch("grid_index count"))) return rc;
     k_gi_scan<<<S, kGiScanThreads, 0, st>>>(ix->cell_start, cells);
     if ((rc = check_launch("grid_index scan"))) return rc;
-    k_gi_scatter<<<dim3(per_sample, S), kGiThreads, 0, st>>>(xyz, offset, N, cells, ix->cell_start, key, rank, ix->pts, ix->ids);
+    k_gi_scatter<<<dim3(per_sample, S), kGiThreads, 0, st>>>(xyz, offset, N, cells, ix->cell_start, L.key, L.rank, ix->pts, ix->ids);
     return check_launch("grid_index scatter");
 }
 

@@ -19,8 +19,8 @@
 //
 // A fit is O SEGMENTS per sample: segment (b, o) is the points with labels[b, i] == o, or, with labels NULL (O = 1), every
 // point of the sample.  rigid_motion is O = 1 (labels = where(mask, 0, -1), or NULL without a mask), rigid_objects one
-// segment per object.  The grouping (k_rigid_allowed for O = 1, k_ro_group_* otherwise) gives both the same RmSegs, and
-// every kernel after it has one form.
+// segment per object.  The grouping (k_ro_group_*, whenever labels are given) gives both the same RmSegs, and every kernel
+// after it has one form.
 //
 // Backward (k_rigid_bwd, one thread per point, each gradient written once): the inlier set held fixed, from the per-segment
 // double state the forward saves (eigenvectors, eigenvalues, centroids, count):
@@ -31,7 +31,6 @@
 namespace pvraft {
 
 constexpr int kRmState = 32;          // doubles per segment in the saved state
-constexpr int kRmModel = 16;          // floats per model: R (9, row-major), c_x (3), c_y (3), flag
 constexpr int kRmMoments = 16;        // n, sum dx (3), sum dy (3), sum dx dy^T (9, row-major)
 constexpr int kRmMaxH = 4096;
 constexpr int kRmMaxRounds = 8;
@@ -61,9 +60,6 @@ __device__ __forceinline__ void horn_matrix(const double (&S)[9], double (&a)[4]
     a[2][3] = a[3][2] = yz + zy;
 }
 
-// Cyclic Jacobi on a symmetric 4x4 matrix: a becomes diagonal (the eigenvalues), column j of v the eigenvector of a[j][j].
-__device__ __forceinline__ void jacobi4(double (&a)[4][4], double (&v)[4][4]) { jacobi_sym<4>(a, v); }
-
 __device__ __forceinline__ void quat_rot(const double (&q)[4], double (&R)[9]) {
     const double w = q[0], x = q[1], y = q[2], z = q[3];
     R[0] = w * w + x * x - y * y - z * z;
@@ -82,7 +78,7 @@ __device__ __forceinline__ void quat_rot(const double (&q)[4], double (&R)[9]) {
 __device__ __forceinline__ bool horn_fit(const double (&S)[9], double (&V)[4][4], double (&lam)[4], double (&R)[9]) {
     double a[4][4];
     horn_matrix(S, a);
-    jacobi4(a, V);
+    jacobi_sym<4>(a, V);
     double l[4] = {a[0][0], a[1][1], a[2][2], a[3][3]};
     int top = 0;
     double lmax = l[0];
@@ -113,19 +109,14 @@ __device__ __forceinline__ bool horn_fit(const double (&S)[9], double (&V)[4][4]
     return l[0] - second > kGapTol * l[0];
 }
 
-// ||R (x - c_x) - (y - c_y)||^2 in fp32: d = x - c_x, e = y - c_y; r_k = ((R_k0 d_0 + R_k1 d_1) + R_k2 d_2) - e_k;
-// (r_0^2 + r_1^2) + r_2^2; every operation rounded to nearest, none contracted
+// ||R (x - c_x) - (y - c_y)||^2 in fp32: r_k = (R (x - c_x))_k - (y_k - c_y_k) (model_rotate); (r_0^2 + r_1^2) + r_2^2;
+// every operation rounded to nearest, none contracted
 __device__ __forceinline__ float residual2(const float* m, float x0, float x1, float x2, float y0, float y1, float y2) {
-    const float d0 = __fsub_rn(x0, m[9]), d1 = __fsub_rn(x1, m[10]), d2 = __fsub_rn(x2, m[11]);
-    const float e0 = __fsub_rn(y0, m[12]), e1 = __fsub_rn(y1, m[13]), e2 = __fsub_rn(y2, m[14]);
-    const float r0 = __fsub_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[0], d0), __fmul_rn(m[1], d1)), __fmul_rn(m[2], d2)), e0);
-    const float r1 = __fsub_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[3], d0), __fmul_rn(m[4], d1)), __fmul_rn(m[5], d2)), e1);
-    const float r2 = __fsub_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[6], d0), __fmul_rn(m[7], d1)), __fmul_rn(m[8], d2)), e2);
+    const float e0 = __fsub_rn(y0, m[kModelCy]), e1 = __fsub_rn(y1, m[kModelCy + 1]), e2 = __fsub_rn(y2, m[kModelCy + 2]);
+    float q[3];
+    model_rotate(m, x0, x1, x2, q);
+    const float r0 = __fsub_rn(q[0], e0), r1 = __fsub_rn(q[1], e1), r2 = __fsub_rn(q[2], e2);
     return __fadd_rn(__fadd_rn(__fmul_rn(r0, r0), __fmul_rn(r1, r1)), __fmul_rn(r2, r2));
-}
-
-__device__ __forceinline__ double dot3(double a0, double a1, double a2, double b0, double b1, double b2) {
-    return __dadd_rn(__dadd_rn(__dmul_rn(a0, b0), __dmul_rn(a1, b1)), __dmul_rn(a2, b2));
 }
 
 // The rejection tests of a triple with distinct indices (x, y [3][3] as doubles of the fp32 values): near-collinear unless
@@ -151,39 +142,7 @@ __device__ __forceinline__ bool triple_rejected(const double (&x)[3][3], const d
     return false;
 }
 
-// The O = 1 grouping: the members (labels == 0) of each sample in ascending order -> list [B,N] (the first n[s] entries of
-// row s), one CTA of kRmScan threads per sample
-constexpr int kRmScan = 1024;
-__global__ void __launch_bounds__(kRmScan) k_rigid_allowed(const int32_t* __restrict__ labels, int N, int32_t* __restrict__ list,
-                                                           int32_t* __restrict__ nmem) {
-    __shared__ int warp_tot[kRmScan / kWarp];
-    __shared__ int base_sh;
-    const int s = blockIdx.x, lane = lane_id(), wid = warp_id();
-    const int32_t* l = labels + (long long)s * N;
-    int32_t* out = list + (long long)s * N;
-    if (threadIdx.x == 0) base_sh = 0;
-    for (int c0 = 0; c0 < N; c0 += kRmScan) {
-        const int i = c0 + threadIdx.x;
-        const bool on = i < N && l[i] == 0;
-        const unsigned bal = __ballot_sync(kFull, on);
-        __syncthreads();   // base_sh of the previous chunk is final; warp_tot free
-        if (lane == 0) warp_tot[wid] = __popc(bal);
-        __syncthreads();
-        int before = base_sh;
-        for (int w = 0; w < wid; ++w) before += warp_tot[w];
-        if (on) out[before + __popc(bal & ((1u << lane) - 1u))] = i;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            int tot = 0;
-            for (int w = 0; w < kRmScan / kWarp; ++w) tot += warp_tot[w];
-            base_sh += tot;
-        }
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) nmem[s] = base_sh;
-}
-
-// One thread per (segment, hypothesis): draw, test and fit the triple -> hyp [G,H,kRmModel] (flag 1: accepted, 0: rejected),
+// One thread per (segment, hypothesis): draw, test and fit the triple -> hyp [G,H,kModel] (flag 1: accepted, 0: rejected),
 // hcnt [G,H] zeroed, triples [G,H,3] (or NULL: the drawn point indices, -1 with no member)
 __global__ void __launch_bounds__(128) k_rigid_hypotheses(const float* __restrict__ x, const float* __restrict__ f, RmSegs sg, int H,
                                                           unsigned long long seed, float thr, float* __restrict__ hyp,
@@ -202,7 +161,7 @@ __global__ void __launch_bounds__(128) k_rigid_hypotheses(const float* __restric
         if (triples) triples[hs * 3 + r] = idx[r];
     }
     hcnt[hs] = 0;
-    float* m = hyp + hs * kRmModel;
+    float* m = hyp + hs * kModel;
     bool rejected = n_al <= 0 || j[0] == j[1] || j[0] == j[2] || j[1] == j[2];
     double xd[3][3], yd[3][3];
     if (!rejected) {
@@ -218,7 +177,7 @@ __global__ void __launch_bounds__(128) k_rigid_hypotheses(const float* __restric
         rejected = triple_rejected(xd, yd, (double)thr);
     }
     if (rejected) {
-        m[15] = 0.f;
+        m[kModelFlag] = 0.f;
         return;
     }
     double cx[3], cy[3], S[9];
@@ -242,10 +201,10 @@ __global__ void __launch_bounds__(128) k_rigid_hypotheses(const float* __restric
     for (int k = 0; k < 9; ++k) m[k] = (float)R[k];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-        m[9 + c] = (float)cx[c];
-        m[12 + c] = (float)cy[c];
+        m[kModelCx + c] = (float)cx[c];
+        m[kModelCy + c] = (float)cy[c];
     }
-    m[15] = 1.f;
+    m[kModelFlag] = 1.f;
 }
 
 // Inlier counts of every (hypothesis, member) pair.  A CTA holds kScHyp hypotheses in shared memory (read as broadcasts) and
@@ -259,21 +218,17 @@ __global__ void __launch_bounds__(kScThreads) k_rigid_score(const float* __restr
                                                             const int32_t* __restrict__ items, const int32_t* __restrict__ nitems,
                                                             int stride, int H, float thr2, const float* __restrict__ hyp,
                                                             int32_t* __restrict__ hcnt) {
-    __shared__ float sh[kScHyp][kRmModel];
+    __shared__ float sh[kScHyp][kModel];
     __shared__ int cnt[kScHyp];
     const int s = blockIdx.z, h0 = blockIdx.y * kScHyp, lane = lane_id(), N = sg.N;
-    int g = s, base = blockIdx.x * kScPoints;
-    if (items) {
-        if ((int)blockIdx.x >= nitems[s]) return;   // uniform over the CTA
-        const int w = items[(long long)s * stride + blockIdx.x];
-        g = s * sg.per + (w & 255);
-        base = (w >> 8) * kScPoints;
-    }
+    if (items && (int)blockIdx.x >= nitems[s]) return;   // uniform over the CTA
+    const SegItem w = seg_item(items, s, sg.per, stride, blockIdx.x);
+    const int g = w.g, base = w.c * kScPoints;
     const int n_g = sg.count(g);
     if (base >= n_g) return;   // no member left: uniform over the CTA
-    for (int i = threadIdx.x; i < kScHyp * kRmModel; i += kScThreads) {
-        const int hh = h0 + i / kRmModel;
-        sh[i / kRmModel][i % kRmModel] = hh < H ? __ldg(hyp + ((long long)g * H + h0) * kRmModel + i) : 0.f;
+    for (int i = threadIdx.x; i < kScHyp * kModel; i += kScThreads) {
+        const int hh = h0 + i / kModel;
+        sh[i / kModel][i % kModel] = hh < H ? __ldg(hyp + ((long long)g * H + h0) * kModel + i) : 0.f;
     }
     if (threadIdx.x < kScHyp) cnt[threadIdx.x] = 0;
     float px[kScPer][3], py[kScPer][3];
@@ -294,7 +249,7 @@ __global__ void __launch_bounds__(kScThreads) k_rigid_score(const float* __restr
     int mine = 0;
     for (int j = 0; j < kScHyp; ++j) {
         const float* m = sh[j];
-        if (m[15] == 0.f) continue;   // rejected or past H: uniform over the CTA
+        if (m[kModelFlag] == 0.f) continue;   // rejected or past H: uniform over the CTA
         int c = 0;
 #pragma unroll
         for (int k = 0; k < kScPer; ++k)
@@ -306,7 +261,7 @@ __global__ void __launch_bounds__(kScThreads) k_rigid_score(const float* __restr
     if (threadIdx.x < kScHyp && h0 + threadIdx.x < H && cnt[threadIdx.x]) atomicAdd(hcnt + (long long)g * H + h0 + threadIdx.x, cnt[threadIdx.x]);
 }
 
-// One CTA per segment: the accepted hypothesis with the most inliers (lowest h on ties) -> model [G,kRmModel] (flag 1), or,
+// One CTA per segment: the accepted hypothesis with the most inliers (lowest h on ties) -> model [G,kModel] (flag 1), or,
 // with none accepted, R = I about the first member (flag 0: every member an inlier); hyp_count [G,H] (or NULL: the counts,
 // -1 for a rejected hypothesis); the segment's moment accumulators of every round zeroed
 constexpr int kSelThreads = 256;
@@ -319,7 +274,7 @@ __global__ void __launch_bounds__(kSelThreads) k_rigid_select(const float* __res
     long long best = -1;   // (count << 32) | (H - 1 - h): the largest wins
     for (int h = threadIdx.x; h < H; h += kSelThreads) {
         const long long hs = (long long)s * H + h;
-        const bool acc = hyp[hs * kRmModel + 15] != 0.f;
+        const bool acc = hyp[hs * kModel + kModelFlag] != 0.f;
         const int c = hcnt[hs];
         if (hyp_count) hyp_count[hs] = acc ? c : -1;
         if (acc) best = max(best, ((long long)c << 32) | (long long)(H - 1 - h));
@@ -332,11 +287,11 @@ __global__ void __launch_bounds__(kSelThreads) k_rigid_select(const float* __res
     __syncthreads();
     if (threadIdx.x != 0) return;
     for (int w = 0; w < kSelThreads / kWarp; ++w) best = max(best, best_w[w]);
-    float* m = model + (long long)s * kRmModel;
+    float* m = model + (long long)s * kModel;
     if (best >= 0) {
         const int h = H - 1 - (int)(best & 0xffffffffll);
-        const float* src = hyp + ((long long)s * H + h) * kRmModel;
-        for (int k = 0; k < kRmModel; ++k) m[k] = src[k];
+        const float* src = hyp + ((long long)s * H + h) * kModel;
+        for (int k = 0; k < kModel; ++k) m[k] = src[k];
         return;
     }
     const int n_al = sg.count(s);
@@ -344,21 +299,19 @@ __global__ void __launch_bounds__(kSelThreads) k_rigid_select(const float* __res
     for (int k = 0; k < 9; ++k) m[k] = k % 4 == 0 ? 1.f : 0.f;
     for (int c = 0; c < 3; ++c) {
         const float xv = i0 < 0 ? 0.f : x[((long long)smp * N + i0) * 3 + c];
-        m[9 + c] = xv;
-        m[12 + c] = i0 < 0 ? 0.f : __fadd_rn(xv, f[((long long)smp * N + i0) * 3 + c]);
+        m[kModelCx + c] = xv;
+        m[kModelCy + c] = i0 < 0 ? 0.f : __fadd_rn(xv, f[((long long)smp * N + i0) * 3 + c]);
     }
-    m[15] = 0.f;
+    m[kModelFlag] = 0.f;
 }
 
 // One refit round's moments over windows of kMomThreads consecutive point ids: point i of sample s is an inlier of segment g
 // when it is a member and (flag 0, or residual2 under g's model <= thr2); (1, dx, dy, dx dy^T) with dx = x - c_x, dy = y - c_y
-// in double summed per warp (xor butterfly), then over the CTA's warps in order, and added once per (window, segment) into
-// acc [G,kRmMoments] (DET: fixed-point slots).  Without `items` (one segment per sample): grid (ceil(N / kMomThreads), B),
-// membership labels == 0 (every point with labels NULL), inliers [B,N] written for every point.  With items [B,N] (nitems
-// [B] per sample; item (c << 8) | o: the window c of point ids [c kMomThreads, (c + 1) kMomThreads), of segment (sample, o),
-// membership labels == o): grid (any, B), each CTA taking items x, x + gridDim.x, ...; inliers written for members only.
-// A window's partial sum is the same value either way, so in the DET form a segment's moments are those of the one-segment
-// launch with labels = where(labels == o, 0, -1).
+// in double summed by window_add into acc [G,kRmMoments] (DET: fixed-point slots), over the segments' window walk
+// (rigid_segments.cuh).  Without `items` (one segment per sample): grid (ceil(N / kMomThreads), B), membership labels == 0
+// (every point with labels NULL), inliers [B,N] written for every point.  With items: grid (any, B), membership labels ==
+// o, inliers written for members only.  A window's partial sum is the same value either way, so in the DET form a
+// segment's moments are those of the one-segment launch with labels = where(labels == o, 0, -1).
 template <bool DET>
 __global__ void __launch_bounds__(kMomThreads) k_rigid_moments(const float* __restrict__ x, const float* __restrict__ f,
                                                                const int32_t* __restrict__ labels, const int32_t* __restrict__ items,
@@ -369,28 +322,24 @@ __global__ void __launch_bounds__(kMomThreads) k_rigid_moments(const float* __re
     const int s = blockIdx.y;
     const int n_items = items ? nitems[s] : 1;
     for (int it = items ? (int)blockIdx.x : 0; it < n_items; it += gridDim.x) {
-        int g = s, o = 0, c = blockIdx.x;
-        if (items) {
-            const int w = items[(long long)s * N + it];
-            o = w & 255;
-            g = s * per + o;
-            c = w >> 8;
-        }
-        const int i = c * kMomThreads + threadIdx.x;
-        const float* m = model + (long long)g * kRmModel;
+        const SegItem w = seg_item(items, s, per, N, items ? it : (int)blockIdx.x);
+        const int i = w.c * kMomThreads + threadIdx.x;
+        const float* m = model + (long long)w.g * kModel;
         double v[kRmMoments];
 #pragma unroll
         for (int k = 0; k < kRmMoments; ++k) v[k] = 0.0;
         if (i < N) {
             const long long p = (long long)s * N + i;
-            const bool member = !labels || labels[p] == o;
+            const bool member = !labels || labels[p] == w.o;
             const float x0 = __ldg(x + 3 * p), x1 = __ldg(x + 3 * p + 1), x2 = __ldg(x + 3 * p + 2);
             const float y0 = __fadd_rn(x0, __ldg(f + 3 * p)), y1 = __fadd_rn(x1, __ldg(f + 3 * p + 1)), y2 = __fadd_rn(x2, __ldg(f + 3 * p + 2));
-            const bool in = member && (m[15] == 0.f || residual2(m, x0, x1, x2, y0, y1, y2) <= thr2);
+            const bool in = member && (m[kModelFlag] == 0.f || residual2(m, x0, x1, x2, y0, y1, y2) <= thr2);
             if (!items || member) inliers[p] = in;
             if (in) {
-                const double d[3] = {(double)x0 - (double)m[9], (double)x1 - (double)m[10], (double)x2 - (double)m[11]};
-                const double e[3] = {(double)y0 - (double)m[12], (double)y1 - (double)m[13], (double)y2 - (double)m[14]};
+                const float* cx = m + kModelCx;
+                const float* cy = m + kModelCy;
+                const double d[3] = {(double)x0 - (double)cx[0], (double)x1 - (double)cx[1], (double)x2 - (double)cx[2]};
+                const double e[3] = {(double)y0 - (double)cy[0], (double)y1 - (double)cy[1], (double)y2 - (double)cy[2]};
                 v[0] = 1.0;
 #pragma unroll
                 for (int k = 0; k < 3; ++k) {
@@ -403,18 +352,7 @@ __global__ void __launch_bounds__(kMomThreads) k_rigid_moments(const float* __re
                     for (int l = 0; l < 3; ++l) v[7 + 3 * k + l] = d[k] * e[l];
             }
         }
-#pragma unroll
-        for (int k = 0; k < kRmMoments; ++k) v[k] = warp_sum(v[k]);
-        if (lane_id() == 0)
-#pragma unroll
-            for (int k = 0; k < kRmMoments; ++k) part[warp_id()][k] = v[k];
-        __syncthreads();
-        if (threadIdx.x < kRmMoments) {
-            double t = 0.0;
-            for (int w = 0; w < kMomThreads / kWarp; ++w) t += part[w][threadIdx.x];
-            if (t != 0.0) add(acc, (long long)g * kRmMoments + threadIdx.x, t);
-        }
-        __syncthreads();   // part is reused by the next item
+        window_add<kRmMoments>(v, part, acc, w.g);
     }
 }
 
@@ -428,20 +366,17 @@ __global__ void __launch_bounds__(64) k_rigid_solve(const double* __restrict__ m
     if (s >= B) return;
     double mo[kRmMoments];
 #pragma unroll
-    for (int k = 0; k < kRmMoments; ++k) {
-        const long long i = (long long)s * kRmMoments + k;
-        mo[k] = DET ? fx_value(slots.base + i * kFxWords) : mom[i];
-    }
-    float* m = model + (long long)s * kRmModel;
-    const bool sampled = m[15] != 0.f;
+    for (int k = 0; k < kRmMoments; ++k) mo[k] = acc_read<DET>(mom, slots, (long long)s * kRmMoments + k);
+    float* m = model + (long long)s * kModel;
+    const bool sampled = m[kModelFlag] != 0.f;
     const double n = mo[0];
     double xb[3], yb[3], mdx[3], mdy[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
         mdx[c] = n > 0.0 ? mo[1 + c] / n : 0.0;
         mdy[c] = n > 0.0 ? mo[4 + c] / n : 0.0;
-        xb[c] = n > 0.0 ? (double)m[9 + c] + mdx[c] : 0.0;
-        yb[c] = n > 0.0 ? (double)m[12 + c] + mdy[c] : 0.0;
+        xb[c] = n > 0.0 ? (double)m[kModelCx + c] + mdx[c] : 0.0;
+        yb[c] = n > 0.0 ? (double)m[kModelCy + c] + mdy[c] : 0.0;
     }
     double S[9];
 #pragma unroll
@@ -480,8 +415,8 @@ __global__ void __launch_bounds__(64) k_rigid_solve(const double* __restrict__ m
     }
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-        m[9 + c] = (float)xb[c];
-        m[12 + c] = (float)yb[c];
+        m[kModelCx + c] = (float)xb[c];
+        m[kModelCy + c] = (float)yb[c];
     }
     count[s] = (int32_t)n;
     degenerate[s] = !proper;
@@ -577,19 +512,19 @@ __global__ void __launch_bounds__(256) k_rigid_bwd(const float* __restrict__ x, 
     }
 }
 
-// ---- the grouping for O > 1 ------------------------------------------------------------------------------------------------
+// ---- the grouping ---------------------------------------------------------------------------------------------------------
 // The points of each sample grouped stably by label (labels [B,N], -1 or out of [0, O): no segment) in windows of kRoChunk
 // point ids, with integer counts only:
 //   k_ro_group_count    per window, the number of points of each object -> cnt [B,C,O] (C = ceil(N / kRoChunk))
 //   k_ro_group_scan     one CTA per sample, thread o per object: n[g] and start[g] = s N + (members of the objects before
-//                       o); pre [B,C,O] = where window c's members of o go in the sample's list; the moment items (c << 8) | o of every window
-//                       holding a member of o, and the score items (j << 8) | o of every kScPoints members of o
+//                       o); pre [B,C,O] = where window c's members of o go in the sample's list; the moment items (c, o) of
+//                       every window c holding a member of o, and the score items (j, o) of every kScPoints members of o
 //   k_ro_group_scatter  per window, each point's rank among the window's points of its object (warp match, then the warps
 //                       before it): list[pre + rank] = i, so each object's members are ascending
 
 __global__ void __launch_bounds__(kRoChunk) k_ro_group_count(const int32_t* __restrict__ labels, int N, int O, int C,
                                                              int32_t* __restrict__ cnt) {
-    __shared__ int c_sh[kRoMaxObjects];
+    __shared__ int c_sh[kMaxObjects];
     const int s = blockIdx.y, c = blockIdx.x, i = c * kRoChunk + threadIdx.x;
     if (threadIdx.x < O) c_sh[threadIdx.x] = 0;
     __syncthreads();
@@ -599,31 +534,11 @@ __global__ void __launch_bounds__(kRoChunk) k_ro_group_count(const int32_t* __re
     if (threadIdx.x < O) cnt[((long long)s * C + c) * O + threadIdx.x] = c_sh[threadIdx.x];
 }
 
-__device__ __forceinline__ int cta_exclusive_scan(int v, int* sh, int& total) {
-    sh[threadIdx.x] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int run = 0;
-        for (int k = 0; k < (int)blockDim.x; ++k) {
-            const int u = sh[k];
-            sh[k] = run;
-            run += u;
-        }
-        sh[blockDim.x] = run;
-    }
-    __syncthreads();
-    const int r = sh[threadIdx.x];
-    total = sh[blockDim.x];
-    __syncthreads();
-    return r;
-}
-
-__global__ void __launch_bounds__(kRoMaxObjects) k_ro_group_scan(const int32_t* __restrict__ cnt, int N, int O, int C, int sstride,
+__global__ void __launch_bounds__(kMaxObjects) k_ro_group_scan(const int32_t* __restrict__ cnt, int N, int O, int C, int sstride,
                                                                  int32_t* __restrict__ pre, int32_t* __restrict__ start,
                                                                  int32_t* __restrict__ nseg, int32_t* __restrict__ mitems,
                                                                  int32_t* __restrict__ nmitems, int32_t* __restrict__ sitems,
                                                                  int32_t* __restrict__ nsitems) {
-    __shared__ int sh[kRoMaxObjects + 1];
     const int s = blockIdx.x, o = threadIdx.x;
     const bool on = o < O;
     const int32_t* cs = cnt + (long long)s * C * O;
@@ -636,9 +551,9 @@ __global__ void __launch_bounds__(kRoMaxObjects) k_ro_group_scan(const int32_t* 
         }
     const int ns = (n + kScPoints - 1) / kScPoints;
     int tn, tw, ts;
-    const int bn = cta_exclusive_scan(n, sh, tn);
-    int bw = cta_exclusive_scan(nw, sh, tw);
-    const int bs = cta_exclusive_scan(ns, sh, ts);
+    const int bn = block_exclusive_scan<kMaxObjects>(n, tn);
+    int bw = block_exclusive_scan<kMaxObjects>(nw, tw);
+    const int bs = block_exclusive_scan<kMaxObjects>(ns, ts);
     if (on) {
         const long long g = (long long)s * O + o;
         start[g] = (int32_t)((long long)s * N + bn);
@@ -648,10 +563,10 @@ __global__ void __launch_bounds__(kRoMaxObjects) k_ro_group_scan(const int32_t* 
         for (int c = 0; c < C; ++c) {
             const int v = __ldg(cs + (long long)c * O + o);
             ps[(long long)c * O + o] = run;
-            if (v) mitems[(long long)s * N + bw++] = (c << 8) | o;
+            if (v) mitems[(long long)s * N + bw++] = seg_item_code(c, o);
             run += v;
         }
-        for (int j = 0; j < ns; ++j) sitems[(long long)s * sstride + bs + j] = (j << 8) | o;
+        for (int j = 0; j < ns; ++j) sitems[(long long)s * sstride + bs + j] = seg_item_code(j, o);
     }
     if (threadIdx.x == 0) {
         nmitems[s] = tw;
@@ -661,9 +576,9 @@ __global__ void __launch_bounds__(kRoMaxObjects) k_ro_group_scan(const int32_t* 
 
 __global__ void __launch_bounds__(kRoChunk) k_ro_group_scatter(const int32_t* __restrict__ labels, int N, int O, int C,
                                                                const int32_t* __restrict__ pre, int32_t* __restrict__ list) {
-    __shared__ int wc[kRoChunk / kWarp][kRoMaxObjects];
+    __shared__ int wc[kRoChunk / kWarp][kMaxObjects];
     const int s = blockIdx.y, c = blockIdx.x, i = c * kRoChunk + threadIdx.x, lane = lane_id(), warp = warp_id();
-    for (int k = threadIdx.x; k < (kRoChunk / kWarp) * kRoMaxObjects; k += kRoChunk) (&wc[0][0])[k] = 0;
+    for (int k = threadIdx.x; k < (kRoChunk / kWarp) * kMaxObjects; k += kRoChunk) (&wc[0][0])[k] = 0;
     __syncthreads();
     int l = i < N ? labels[(long long)s * N + i] : -1;
     if (l < 0 || l >= O) l = -1;
@@ -677,36 +592,28 @@ __global__ void __launch_bounds__(kRoChunk) k_ro_group_scatter(const int32_t* __
     list[(long long)s * N + __ldg(pre + ((long long)s * C + c) * O + l) + before] = i;
 }
 
-RmGroupWs rm_group_carve(char* base, int64_t& off, int B, int N, int O) {
-    auto take = [&](int64_t bytes) {
-        char* p = base ? base + off : nullptr;
-        off += (bytes + 15) / 16 * 16;
-        return reinterpret_cast<int32_t*>(p);
-    };
+RmGroupWs rm_group_carve(ByteCarve& w, int B, int N, int O) {
     RmGroupWs L;
     const long long G = (long long)B * O;
     L.C = (N + kRoChunk - 1) / kRoChunk;
     L.S = (N + kScPoints - 1) / kScPoints + O;
-    L.list = take(4ll * B * N);
-    L.start = take(4 * G);
-    L.n = take(4 * G);
-    L.cnt = take(4ll * B * L.C * O);
-    L.pre = take(4ll * B * L.C * O);
-    L.mitems = take(4ll * B * N);
-    L.nm = take(4ll * B);
-    L.sitems = take(4ll * B * L.S);
-    L.ns = take(4ll * B);
+    L.list = w.take<int32_t>(4ll * B * N);
+    L.start = w.take<int32_t>(4 * G);
+    L.n = w.take<int32_t>(4 * G);
+    L.cnt = w.take<int32_t>(4ll * B * L.C * O);
+    L.pre = w.take<int32_t>(4ll * B * L.C * O);
+    L.mitems = w.take<int32_t>(4ll * B * N);
+    L.nm = w.take<int32_t>(4ll * B);
+    L.sitems = w.take<int32_t>(4ll * B * L.S);
+    L.ns = w.take<int32_t>(4ll * B);
     return L;
 }
 
 int rm_group(const int32_t* labels, int B, int N, int O, const RmGroupWs& L, cudaStream_t st) {
-    if (O == 1) {
-        if (labels) k_rigid_allowed<<<B, kRmScan, 0, st>>>(labels, N, L.list, L.n);
-    } else {
-        k_ro_group_count<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.cnt);
-        k_ro_group_scan<<<B, kRoMaxObjects, 0, st>>>(L.cnt, N, O, L.C, L.S, L.pre, L.start, L.n, L.mitems, L.nm, L.sitems, L.ns);
-        k_ro_group_scatter<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.pre, L.list);
-    }
+    if (!labels) return 0;
+    k_ro_group_count<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.cnt);
+    k_ro_group_scan<<<B, kMaxObjects, 0, st>>>(L.cnt, N, O, L.C, L.S, L.pre, L.start, L.n, L.mitems, L.nm, L.sitems, L.ns);
+    k_ro_group_scatter<<<dim3((unsigned)L.C, (unsigned)B), kRoChunk, 0, st>>>(labels, N, O, L.C, L.pre, L.list);
     return check_launch("rigid segment grouping");
 }
 
@@ -721,26 +628,20 @@ struct FitWs {
     int64_t bytes;
 };
 static FitWs fit_ws(void* ws, int B, int N, int O, int H, int rounds) {
-    char* base = static_cast<char*>(ws);
-    int64_t off = 0;
-    auto take = [&](int64_t bytes) {
-        char* p = base ? base + off : nullptr;
-        off += (bytes + 15) / 16 * 16;
-        return p;
-    };
+    ByteCarve w(ws);
     FitWs L;
     const long long G = (long long)B * O;
-    L.grp = rm_group_carve(base, off, B, N, O);
-    L.hyp = reinterpret_cast<float*>(take(4 * G * H * kRmModel));
-    L.hcnt = reinterpret_cast<int32_t*>(take(4 * G * H));
-    L.model = reinterpret_cast<float*>(take(4 * G * kRmModel));
-    L.mom = reinterpret_cast<double*>(take(8 * rounds * G * kRmMoments));
-    L.bytes = off;
+    L.grp = rm_group_carve(w, B, N, O);
+    L.hyp = w.take<float>(4 * G * H * kModel);
+    L.hcnt = w.take<int32_t>(4 * G * H);
+    L.model = w.take<float>(4 * G * kModel);
+    L.mom = w.take<double>(8 * rounds * G * kRmMoments);
+    L.bytes = w.bytes;
     return L;
 }
 
 static bool bad_sizes(int B, int N, int O, int H, int rounds) {
-    return B < 1 || N < 1 || O < 1 || O > kRoMaxObjects || H < 1 || H > kRmMaxH || rounds < 1 || rounds > kRmMaxRounds ||
+    return B < 1 || N < 1 || O < 1 || O > kMaxObjects || H < 1 || H > kRmMaxH || rounds < 1 || rounds > kRmMaxRounds ||
            (long long)B * N > 0x7fffffffll;
 }
 
@@ -753,7 +654,7 @@ extern "C" int64_t pvraft_rigid_objects_workspace_bytes(int B, int N, int O, int
 }
 
 extern "C" int64_t pvraft_rigid_objects_fwd_det_workspace_bytes(int B, int O, int rounds) {
-    return B < 1 || O < 1 || O > kRoMaxObjects || rounds < 1 || rounds > kRmMaxRounds ? 0 : fx_bytes((long long)rounds * B * O * kRmMoments);
+    return B < 1 || O < 1 || O > kMaxObjects || rounds < 1 || rounds > kRmMaxRounds ? 0 : fx_bytes((long long)rounds * B * O * kRmMoments);
 }
 
 extern "C" int pvraft_rigid_objects_fwd(const float* xyz1, const float* flow, const int32_t* labels, int B, int N, int O, float threshold,
@@ -768,8 +669,8 @@ extern "C" int pvraft_rigid_objects_fwd(const float* xyz1, const float* flow, co
     const FitWs L = fit_ws(workspace, B, N, O, H, rounds);
     const int G = B * O;
     const float thr2 = threshold * threshold;
-    // O = 1: the member list in one launch (none without labels), and the score and moment kernels' one-segment grids;
-    // O > 1: the stable grouping, and work items that cover each segment's members
+    // the member lists whenever labels are given; O = 1: the score and moment kernels' one-segment grids, O > 1: work items
+    // that cover each segment's members
     const RmGroupWs& Lg = L.grp;
     const int32_t *sitems = nullptr, *nsitems = nullptr, *mitems = nullptr, *nmitems = nullptr;
     unsigned score_x = (unsigned)((N + kScPoints - 1) / kScPoints), mom_x = (unsigned)Lg.C;
@@ -808,7 +709,7 @@ extern "C" int pvraft_rigid_objects_bwd(const float* xyz1, const float* flow, co
                                         const double* state, const float* dR, const float* dt, int B, int N, int O, float* d_xyz1,
                                         float* d_flow, void* stream) {
     if (!xyz1 || !flow || (!labels && O != 1) || !inliers || !state || !dR || !dt || !d_xyz1 || !d_flow || B < 1 || N < 1 || O < 1 ||
-        O > kRoMaxObjects || (long long)B * N > 0x7fffffffll)
+        O > kMaxObjects || (long long)B * N > 0x7fffffffll)
         return fail(PVRAFT_ERR_BAD_ARG, "rigid_objects_bwd: bad argument");
     const long long points = (long long)B * N;
     const unsigned blocks = (unsigned)scatter_blocks(points, false);

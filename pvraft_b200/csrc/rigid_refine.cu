@@ -1,8 +1,8 @@
 // Point-to-plane ICP of rigid fits against the second scan, every segment of every sample in one launch sequence, with no
 // host synchronisation (the rule is stated in include/pvraft_b200.h, pvraft_rigid_refine_fwd):
 //
-//   k_rf_stage     a target takes part when target_mask allows it and its coordinates are finite: staged as it is, any
-//                  other point as NaN, so the index's bounds ignore it and no distance to it compares <= r2
+//   k_rf_stage     a target takes part when target_mask allows it and its coordinates are finite (takes_part): staged as
+//                  it is, any other point as NaN, so the index's bounds ignore it and no distance to it compares <= r2
 //   (index)        grid_index_build on the staged targets
 //   k_rf_normals   one warp per target: its k_normal nearest targets (grid_knn_diff, on (diff_sq, id)), their covariance
 //                  about their mean in double, the eigenvector of its smallest eigenvalue (cyclic Jacobi); a target whose
@@ -29,17 +29,14 @@ constexpr int kRfMom = 29;              // per segment and iteration: upper JtJ 
 constexpr int kRfMemb = 5;              // per segment: n, sum x (3), sum |x - c_x|^2
 constexpr int kRfState = 21;            // doubles per segment: R (9), c_y (3), c_x (3), rho, steps, done, rank, matched, sse
 constexpr int kRfHist = 12;             // R (9), c_y (3)
-constexpr int kRfModel = 16;            // floats per model: R (9), c_x (3), c_y (3), flag
 constexpr int kRfNormalWarps = 8;
-
-__device__ __forceinline__ bool finite3(float x, float y, float z) { return isfinite(x) && isfinite(y) && isfinite(z); }
 
 __global__ void __launch_bounds__(256) k_rf_stage(const float* __restrict__ xyz2, const uint8_t* __restrict__ mask, long long points,
                                                   float* __restrict__ staged) {
     const long long p = (long long)blockIdx.x * 256 + threadIdx.x;
     if (p >= points) return;
     const float x = xyz2[3 * p], y = xyz2[3 * p + 1], z = xyz2[3 * p + 2];
-    const bool on = (!mask || mask[p] != 0) && finite3(x, y, z);
+    const bool on = takes_part(mask, p, x, y, z);
     staged[3 * p] = on ? x : NAN;
     staged[3 * p + 1] = on ? y : NAN;
     staged[3 * p + 2] = on ? z : NAN;
@@ -106,35 +103,6 @@ __global__ void __launch_bounds__(kRfNormalWarps * kWarp) k_rf_normals(const flo
     if (!valid) staged[3 * q] = staged[3 * q + 1] = staged[3 * q + 2] = NAN;
 }
 
-// The item loop of the windowed kernels (k_rigid_moments' form): with items (O > 1), CTA x takes items x, x + gridDim.x, ...
-// of its sample, item (c << 8) | o being window c of segment (sample, o); without, CTA x is window x of segment (sample, 0).
-struct RfItem {
-    int g, o, c;
-};
-__device__ __forceinline__ RfItem rf_item(const int32_t* items, int s, int per, int N, int it) {
-    if (!items) return RfItem{s, 0, it};
-    const int w = items[(long long)s * N + it];
-    return RfItem{s * per + (w & 255), w & 255, w >> 8};
-}
-
-// Sum v[0..K) over the CTA's warps in order (warp xor butterfly, then warp 0, 1, ...) and add it once into acc slot
-// g * K + k.  part: [kMomThreads / kWarp][K] shared.
-template <int K, class A>
-__device__ __forceinline__ void rf_window_add(double (&v)[K], double (*part)[K], A acc, long long g) {
-#pragma unroll
-    for (int k = 0; k < K; ++k) v[k] = warp_sum(v[k]);
-    if (lane_id() == 0)
-#pragma unroll
-        for (int k = 0; k < K; ++k) part[warp_id()][k] = v[k];
-    __syncthreads();
-    if (threadIdx.x < K) {
-        double t = 0.0;
-        for (int w = 0; w < kMomThreads / kWarp; ++w) t += part[w][threadIdx.x];
-        if (t != 0.0) add(acc, g * K + threadIdx.x, t);
-    }
-    __syncthreads();   // part is reused by the next item
-}
-
 // A source point takes part in segment (s, o) when labels[s, i] == o (every point with labels NULL) and its coordinates are
 // finite.  pass 0: (1, x) into acc slots 0..3; pass 1: |x - c_x|^2 into slot 4, c_x from the state.
 template <bool DET>
@@ -146,7 +114,7 @@ __global__ void __launch_bounds__(kMomThreads) k_rf_members(const float* __restr
     const int s = blockIdx.y;
     const int n_items = items ? nitems[s] : 1;
     for (int it = items ? (int)blockIdx.x : 0; it < n_items; it += gridDim.x) {
-        const RfItem w = rf_item(items, s, per, N, items ? it : (int)blockIdx.x);
+        const SegItem w = seg_item(items, s, per, N, items ? it : (int)blockIdx.x);
         const int i = w.c * kMomThreads + threadIdx.x;
         double v[kRfMemb] = {0.0, 0.0, 0.0, 0.0, 0.0};
         if (i < N) {
@@ -165,13 +133,8 @@ __global__ void __launch_bounds__(kMomThreads) k_rf_members(const float* __restr
                 }
             }
         }
-        rf_window_add<kRfMemb>(v, part, acc, w.g);
+        window_add<kRfMemb>(v, part, acc, w.g);
     }
-}
-
-template <bool DET>
-__device__ __forceinline__ double rf_read(const double* mom, FxSlots slots, long long i) {
-    return DET ? fx_value(slots.base + i * kFxWords) : mom[i];
 }
 
 // the fp32 model of the step kernel from the double state: R, c_x, c_y rounded once; flag 1 while the segment iterates
@@ -180,10 +143,10 @@ __device__ __forceinline__ void rf_model(const double* st, bool live, float* m) 
     for (int k = 0; k < 9; ++k) m[k] = (float)st[k];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-        m[9 + c] = (float)st[12 + c];
-        m[12 + c] = (float)st[9 + c];
+        m[kModelCx + c] = (float)st[12 + c];
+        m[kModelCy + c] = (float)st[9 + c];
     }
-    m[15] = live ? 1.f : 0.f;
+    m[kModelFlag] = live ? 1.f : 0.f;
 }
 
 __device__ __forceinline__ void rf_history(double* hist, int g, int iterations, int k, const double* st) {
@@ -200,13 +163,13 @@ __global__ void __launch_bounds__(64) k_rf_setup(const double* __restrict__ memb
                                                  float* __restrict__ model, double* __restrict__ hist) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= G) return;
-    const double n = rf_read<DET>(memb, slots, (long long)g * kRfMemb);
+    const double n = acc_read<DET>(memb, slots, (long long)g * kRfMemb);
     double* st = state + (long long)g * kRfState;
 #pragma unroll
     for (int k = 0; k < kRfState; ++k) st[k] = 0.0;
     double cx[3];
 #pragma unroll
-    for (int c = 0; c < 3; ++c) cx[c] = n > 0.0 ? rf_read<DET>(memb, slots, (long long)g * kRfMemb + 1 + c) / n : 0.0;
+    for (int c = 0; c < 3; ++c) cx[c] = n > 0.0 ? acc_read<DET>(memb, slots, (long long)g * kRfMemb + 1 + c) / n : 0.0;
 #pragma unroll
     for (int k = 0; k < 9; ++k) st[k] = (double)R_in[9ll * g + k];
 #pragma unroll
@@ -216,16 +179,16 @@ __global__ void __launch_bounds__(64) k_rf_setup(const double* __restrict__ memb
         st[12 + r] = cx[r];
     }
     rf_history(hist, g, iterations, 0, st);
-    rf_model(st, n > 0.0, model + (long long)g * kRfModel);
+    rf_model(st, n > 0.0, model + (long long)g * kModel);
 }
 
 // The hot path, one iteration over the windows of every live segment.  Per member i with finite x:
-//   move    p = R (x - c_x) + c_y in fp32 (d = x - c_x; p_k = ((R_k0 d_0 + R_k1 d_1) + R_k2 d_2) + c_y_k, each operation
-//           rounded, none contracted), R, c_x, c_y the model's fp32 values;
+//   move    p = R (x - c_x) + c_y in fp32 (p_k = (R (x - c_x))_k + c_y_k, model_rotate, each operation rounded, none
+//           contracted), R, c_x, c_y the model's fp32 values;
 //   match   the nearest target q of the second index on (diff_sq(p, q), id) with diff_sq <= r2, found by
 //           grid_radius_visit (exact for the fp32 predicate; a non-finite p matches nothing) -> corr (id or -1);
 //   sum     r = n . (p - q), J = [(p - c_y) x n, n] in double from the fp32 values: upper J J^T (21), J r (6), 1, r^2,
-//           per warp, then over the CTA's warps in order, added once per (window, segment) into acc [G,kRfMom].
+//           summed by window_add into acc [G,kRfMom].
 template <bool DET>
 __global__ void __launch_bounds__(kMomThreads) k_icp_step(const float* __restrict__ x, const int32_t* __restrict__ labels,
                                                           const int32_t* __restrict__ items, const int32_t* __restrict__ nitems,
@@ -240,9 +203,9 @@ __global__ void __launch_bounds__(kMomThreads) k_icp_step(const float* __restric
     const int32_t* I = ix.ids + tbase;
     const int32_t* CS = ix.cell_start + (long long)s * (ix.cells + 1);
     for (int it = items ? (int)blockIdx.x : 0; it < n_items; it += gridDim.x) {
-        const RfItem w = rf_item(items, s, per, N, items ? it : (int)blockIdx.x);
-        const float* m = model + (long long)w.g * kRfModel;
-        if (m[15] == 0.f) continue;   // converged or empty: uniform over the CTA
+        const SegItem w = seg_item(items, s, per, N, items ? it : (int)blockIdx.x);
+        const float* m = model + (long long)w.g * kModel;
+        if (m[kModelFlag] == 0.f) continue;   // converged or empty: uniform over the CTA
         const int i = w.c * kMomThreads + threadIdx.x;
         double v[kRfMom];
 #pragma unroll
@@ -257,10 +220,9 @@ __global__ void __launch_bounds__(kMomThreads) k_icp_step(const float* __restric
         if (member) {
             int best = -1;
             if (finite3(x0, x1, x2)) {
-                const float d0 = __fsub_rn(x0, m[9]), d1 = __fsub_rn(x1, m[10]), d2 = __fsub_rn(x2, m[11]);
-                const float p0 = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[0], d0), __fmul_rn(m[1], d1)), __fmul_rn(m[2], d2)), m[12]);
-                const float p1 = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[3], d0), __fmul_rn(m[4], d1)), __fmul_rn(m[5], d2)), m[13]);
-                const float p2 = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[6], d0), __fmul_rn(m[7], d1)), __fmul_rn(m[8], d2)), m[14]);
+                float q[3];
+                model_rotate(m, x0, x1, x2, q);
+                const float p0 = __fadd_rn(q[0], m[kModelCy]), p1 = __fadd_rn(q[1], m[kModelCy + 1]), p2 = __fadd_rn(q[2], m[kModelCy + 2]);
                 if (finite3(p0, p1, p2)) {
                     float bd = INFINITY;
                     int bk = -1;
@@ -281,7 +243,8 @@ __global__ void __launch_bounds__(kMomThreads) k_icp_step(const float* __restric
                         const float4 nq = __ldg(normals + tbase + best);
                         const double n[3] = {nq.x, nq.y, nq.z};
                         const double e[3] = {(double)p0 - (double)q.x, (double)p1 - (double)q.y, (double)p2 - (double)q.z};
-                        const double a[3] = {(double)p0 - (double)m[12], (double)p1 - (double)m[13], (double)p2 - (double)m[14]};
+                        const double a[3] = {(double)p0 - (double)m[kModelCy], (double)p1 - (double)m[kModelCy + 1],
+                                             (double)p2 - (double)m[kModelCy + 2]};
                         const double r = n[0] * e[0] + n[1] * e[1] + n[2] * e[2];
                         const double J[6] = {a[1] * n[2] - a[2] * n[1], a[2] * n[0] - a[0] * n[2], a[0] * n[1] - a[1] * n[0], n[0], n[1], n[2]};
                         int u = 0;
@@ -298,7 +261,7 @@ __global__ void __launch_bounds__(kMomThreads) k_icp_step(const float* __restric
             }
             if (corr) corr[p] = best;
         }
-        rf_window_add<kRfMom>(v, part, acc, w.g);
+        window_add<kRfMom>(v, part, acc, w.g);
     }
 }
 
@@ -336,16 +299,16 @@ __global__ void __launch_bounds__(64) k_icp_solve(const double* __restrict__ mom
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= G) return;
     double* st = state + (long long)g * kRfState;
-    float* m = model + (long long)g * kRfModel;
-    if (m[15] != 0.f) {
+    float* m = model + (long long)g * kModel;
+    if (m[kModelFlag] != 0.f) {
         const long long b0 = (long long)g * kRfMom;
-        const double cnt = rf_read<DET>(mom, slots, b0 + 27);
+        const double cnt = acc_read<DET>(mom, slots, b0 + 27);
         st[19] = cnt;
-        st[20] = rf_read<DET>(mom, slots, b0 + 28);
+        st[20] = acc_read<DET>(mom, slots, b0 + 28);
         st[18] = 0.0;
         if (cnt >= (double)kRfMinMatches) {
-            const double n = rf_read<DET>(memb, mslots, (long long)g * kRfMemb);
-            double rho = sqrt(rf_read<DET>(memb, mslots, (long long)g * kRfMemb + 4) / n);
+            const double n = acc_read<DET>(memb, mslots, (long long)g * kRfMemb);
+            double rho = sqrt(acc_read<DET>(memb, mslots, (long long)g * kRfMemb + 4) / n);
             if (!(rho > 0.0)) rho = 1.0;
             st[15] = rho;
             double A[6][6], V[6][6], y[6];
@@ -356,9 +319,9 @@ __global__ void __launch_bounds__(64) k_icp_solve(const double* __restrict__ mom
 #pragma unroll
                 for (int l = j; l < 6; ++l) {
                     const double sl = l < 3 ? 1.0 / rho : 1.0;
-                    A[j][l] = A[l][j] = rf_read<DET>(mom, slots, b0 + u++) * sj * sl;
+                    A[j][l] = A[l][j] = acc_read<DET>(mom, slots, b0 + u++) * sj * sl;
                 }
-                y[j] = rf_read<DET>(mom, slots, b0 + 21 + j) * sj;
+                y[j] = acc_read<DET>(mom, slots, b0 + 21 + j) * sj;
             }
             jacobi_sym<6>(A, V);
             double lmax = A[0][0];
@@ -429,29 +392,23 @@ struct RefineWs {
     int64_t bytes;
 };
 static RefineWs refine_ws(void* ws, int B, int N, int M, int O, int iterations) {
-    char* base = static_cast<char*>(ws);
-    int64_t off = 0;
-    auto take = [&](int64_t bytes) {
-        char* p = base ? base + off : nullptr;
-        off += (bytes + 15) / 16 * 16;
-        return p;
-    };
+    ByteCarve w(ws);
     const long long G = (long long)B * O, tm = (long long)B * M;
     RefineWs L;
-    L.index = take(grid_index_bytes(B, M));
-    L.staged = reinterpret_cast<float*>(take(12 * tm));
-    L.normals = reinterpret_cast<float4*>(take(16 * tm));
-    L.grp = O > 1 ? rm_group_carve(base, off, B, N, O) : RmGroupWs{};
-    L.model = reinterpret_cast<float*>(take(4 * G * kRfModel));
-    L.state = reinterpret_cast<double*>(take(8 * G * kRfState));
-    L.memb = reinterpret_cast<double*>(take(8 * G * kRfMemb));
-    L.mom = reinterpret_cast<double*>(take(8 * iterations * G * kRfMom));
-    L.bytes = off;
+    L.index = w.take<void>(grid_index_bytes(B, M));
+    L.staged = w.take<float>(12 * tm);
+    L.normals = w.take<float4>(16 * tm);
+    L.grp = O > 1 ? rm_group_carve(w, B, N, O) : RmGroupWs{};
+    L.model = w.take<float>(4 * G * kModel);
+    L.state = w.take<double>(8 * G * kRfState);
+    L.memb = w.take<double>(8 * G * kRfMemb);
+    L.mom = w.take<double>(8 * iterations * G * kRfMom);
+    L.bytes = w.bytes;
     return L;
 }
 
 static bool bad_sizes(int B, int N, int M, int O, int iterations) {
-    return B < 1 || N < 1 || M < 1 || O < 1 || O > kRoMaxObjects || iterations < 1 || iterations > kRfMaxIterations ||
+    return B < 1 || N < 1 || M < 1 || O < 1 || O > kMaxObjects || iterations < 1 || iterations > kRfMaxIterations ||
            (long long)B * N > 0x7fffffffll || (long long)B * M > 0x7fffffffll || (long long)B * O > 65535;
 }
 
@@ -464,7 +421,7 @@ extern "C" int64_t pvraft_rigid_refine_workspace_bytes(int B, int N, int M, int 
 }
 
 extern "C" int64_t pvraft_rigid_refine_det_workspace_bytes(int B, int O, int iterations) {
-    return B < 1 || O < 1 || O > kRoMaxObjects || iterations < 1 || iterations > kRfMaxIterations || (long long)B * O > 65535
+    return B < 1 || O < 1 || O > kMaxObjects || iterations < 1 || iterations > kRfMaxIterations || (long long)B * O > 65535
                ? 0
                : fx_bytes((long long)B * O * (kRfMemb + (long long)iterations * kRfMom));
 }
@@ -501,7 +458,6 @@ extern "C" int pvraft_rigid_refine_fwd(const float* xyz1, const float* xyz2, con
         xyz2, M, tpts, k_normal, ix, L.staged, L.normals, reinterpret_cast<float4*>(normals), neighbours);
     if ((rc = check_launch("rigid_refine_fwd normals"))) return rc;
     if ((rc = grid_index_build(L.staged, nullptr, B, M, L.index, st, &ix))) return rc;
-    // the segments
     // the segments: with O = 1 window c of sample s is item c and membership is read from labels, so only O > 1 groups
     if (O > 1 && (rc = rm_group(labels, B, N, O, L.grp, st))) return rc;
     const int32_t* items = O > 1 ? L.grp.mitems : nullptr;

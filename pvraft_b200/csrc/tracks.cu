@@ -13,14 +13,14 @@
 //                   greedy pass, a block scan that numbers the new tracks, and one thread per slot for its track, match, age
 //                   and pose (composed in double)
 #include "nn_search.cuh"
+#include "rigid_segments.cuh"
 
 namespace pvraft {
 
 constexpr int kTvThreads = 256;
 constexpr int kTaThreads = 256;
-constexpr int kTrMaxObjects = 256;
-constexpr int kTaMaxPairs = 16 * kTrMaxObjects;   // min_overlap >= 1/16: at most 16 eligible previous objects per slot
-static_assert(kTaThreads == kTrMaxObjects, "one assigning thread per slot");
+constexpr int kTaMaxPairs = 16 * kMaxObjects;   // min_overlap >= 1/16: at most 16 eligible previous objects per slot
+static_assert(kTaThreads == kMaxObjects, "one assigning thread per slot");
 
 // members[b,c] and overlap[b,c,a] (both zeroed on the stream first); grid (ceil(N / kTvThreads), B)
 __global__ void __launch_bounds__(kTvThreads) k_track_votes(const float* __restrict__ xyz_prev, const float* __restrict__ flow_prev,
@@ -57,35 +57,7 @@ __global__ void __launch_bounds__(kTvThreads) k_track_votes(const float* __restr
     if (key >= 0 && !(pa & below)) atomicAdd(overlap + (long long)b * O * O_prev + key, __popc(pa));
 }
 
-// an exclusive scan of v over the CTA's kTaThreads threads (warp shuffles, then the warp totals); total: the sum
-__device__ __forceinline__ int block_exclusive_scan(int v, int& total) {
-    __shared__ int warp_sum[kTaThreads / kWarp];
-    const int lane = lane_id(), warp = warp_id();
-    int x = v;
-#pragma unroll
-    for (int o = 1; o < kWarp; o <<= 1) {
-        const int y = __shfl_up_sync(kFull, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == kWarp - 1) warp_sum[warp] = x;
-    __syncthreads();
-    int before = 0;
-    total = 0;
-#pragma unroll
-    for (int w = 0; w < kTaThreads / kWarp; ++w) {
-        const int s = warp_sum[w];
-        before += w < warp ? s : 0;
-        total += s;
-    }
-    return before + x - v;
-}
-
-// R = Ra Rp, t = Ra tp + ta in double, each entry (x0 y0 + x1 y1) + x2 y2, every operation rounded to nearest, none contracted
-__device__ __forceinline__ double dot3(double x0, double x1, double x2, double y0, double y1, double y2) {
-    return __dadd_rn(__dadd_rn(__dmul_rn(x0, y0), __dmul_rn(x1, y1)), __dmul_rn(x2, y2));
-}
-
-// one CTA per sample
+// one CTA per sample; a matched slot's pose is R = Ra Rp, t = Ra tp + ta in double, each entry a dot3
 __global__ void __launch_bounds__(kTaThreads) k_track_assign(const int32_t* __restrict__ overlap, const int32_t* __restrict__ members,
                                                              const int32_t* __restrict__ num_objects, const int32_t* __restrict__ track_prev,
                                                              const int32_t* __restrict__ age_prev, const double* __restrict__ pose_prev,
@@ -94,9 +66,9 @@ __global__ void __launch_bounds__(kTaThreads) k_track_assign(const int32_t* __re
                                                              int32_t* __restrict__ match, int32_t* __restrict__ track,
                                                              int32_t* __restrict__ age, double* __restrict__ pose) {
     __shared__ unsigned long long keys[kTaMaxPairs];
-    __shared__ int mem_sh[kTrMaxObjects];
-    __shared__ int match_sh[kTrMaxObjects];
-    __shared__ unsigned char taken_sh[kTrMaxObjects];
+    __shared__ int mem_sh[kMaxObjects];
+    __shared__ int match_sh[kMaxObjects];
+    __shared__ unsigned char taken_sh[kMaxObjects];
     __shared__ int count_sh;
     const int b = blockIdx.x, c = threadIdx.x;
     const int nb = max(0, min(num_objects[b], O));
@@ -154,7 +126,7 @@ __global__ void __launch_bounds__(kTaThreads) k_track_assign(const int32_t* __re
     const bool live = c < nb;
     const int a = live ? match_sh[c] : -1;
     int born_total;
-    const int rank = block_exclusive_scan(live && a < 0 ? 1 : 0, born_total);
+    const int rank = block_exclusive_scan<kTaThreads>(live && a < 0 ? 1 : 0, born_total);
     if (threadIdx.x == 0) next_id[b] = base_id + born_total;
     if (c >= O) return;
     const long long r = (long long)b * O + c;
@@ -197,7 +169,7 @@ extern "C" int pvraft_track_objects_fwd(const float* xyz_prev, const float* flow
                                         int N, int O_prev, int O, float gate, double min_overlap, int32_t* next_id, int32_t* overlap,
                                         int32_t* members, int32_t* match, int32_t* track, int32_t* age, double* pose, void* stream) {
     if (!xyz || !labels || !num_objects || !next_id || !members || !match || !track || !age || !pose || B < 1 || N < 1 || M < 0 ||
-        O < 1 || O > kTrMaxObjects || O_prev < 0 || O_prev > kTrMaxObjects || (M == 0 && O_prev != 0) ||
+        O < 1 || O > kMaxObjects || O_prev < 0 || O_prev > kMaxObjects || (M == 0 && O_prev != 0) ||
         (M > 0 && (!xyz_prev || !flow_prev || !labels_prev || !nn)) ||
         (O_prev > 0 && (!track_prev || !age_prev || !pose_prev || !R_prev || !t_prev || !overlap)) || bad_gate(gate) ||
         !(min_overlap >= 1.0 / 16.0 && min_overlap <= 1.0))
