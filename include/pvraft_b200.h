@@ -880,6 +880,45 @@ PVRAFT_API int pvraft_rigid_refine_fwd(const float* xyz1, const float* xyz2, con
 PVRAFT_API int64_t pvraft_rigid_refine_workspace_bytes(int B, int N, int M, int O, int iterations);
 PVRAFT_API int64_t pvraft_rigid_refine_det_workspace_bytes(int B, int O, int iterations);
 
+/* An oriented box for every segment of a clustering (no counterpart in the reference): pvraft_b200.object_boxes.  Axis up
+ * (0, 1 or 2) is vertical; the box plane is spanned by p = (up + 1) % 3 and q = (up + 2) % 3 (e_p x e_q = e_up), and an
+ * angle in it is measured from e_p towards e_q.  No host synchronisation; every output element is written.
+ *   Members: segment (b, o) is the points with labels[b,i] == o whose three coordinates are finite -- every labelled point,
+ *       not only a fit's inliers.  P = x_p, Q = x_q, H = x_up as stored.
+ *   Directions: for a = 0 .. A - 1, (c_a, s_a) are the fp32 roundings of the double cos and sin of a pi / (2 A) (sincospi
+ *       of a / (2.0 A)).
+ *   Extents: per member u_a = fl(fl(c_a P) + fl(s_a Q)), v_a = fl(fl(c_a Q) - fl(s_a P)), every operation rounded to nearest,
+ *       none contracted; per segment and angle umin, umax, vmin, vmax, and per segment hmin, hmax of H.  Exact fp32 minima
+ *       and maxima: no result depends on the order of any atomic operation, so there is no det_workspace and a batched
+ *       call equals per-sample calls bit for bit.
+ *   Choice: area_a = (umax - umin)(vmax - vmin) in double (each difference exact, the product rounded once; a NaN area
+ *       counts as +inf); a* is the lowest a of the least area -- the minimum-area rectangle over the candidate directions.
+ *   Box: du, dv the two differences at a*; the length axis is at phi = pi (a* / (2.0 A)) when du >= dv, else at phi + pi / 2
+ *       (double); size = (max(du, dv), min(du, dv), hmax - hmin) rounded to fp32.  Centre in double from the fp32 (c, s):
+ *       mid_u = (umin + umax) / 2, mid_v = (vmin + vmax) / 2, P_c = c mid_u - s mid_v, Q_c = s mid_u + c mid_v, H_c = (hmin +
+ *       hmax) / 2, each rounded to fp32.
+ *   Displacement of the fp32 centre c over the pair, in double from the fp32 fits, each row (R_k0 c_0 + R_k1 c_1) + R_k2 c_2
+ *       then + t_k, every operation rounded to nearest, none contracted: y = R_o c + t_o; without an ego fit, or with a
+ *       degenerate one, d = y - c (relative to the sensor); otherwise d = R_e^T (y - t_e) - c (relative to the static scene).
+ *       d is rounded to fp32.
+ *   Heading: if d_p cos(phi) + d_q sin(phi) < 0 (double d), phi += pi; then phi > pi becomes phi - 2 pi, so yaw = phi in
+ *       (-pi, pi] (rounded to fp32): the box faces the way it moves, and one that does not move keeps phi in [0, pi).
+ *       rotation's columns are cos(phi) e_p + sin(phi) e_q, -sin(phi) e_p + cos(phi) e_q and e_up, in double, rounded.
+ *   Empty segment (count 0): centre, size, yaw and displacement 0, rotation the basis (e_p, e_q, e_up).
+ *   pvraft_object_boxes_fwd: xyz [B,N,3], labels [B,N] int32, the segments' fits R_o [B,O,3,3], t_o [B,O,3] f32, and the
+ *       ego fit R_e [B,3,3], t_e [B,3] f32, ego_degenerate [B] uint8 (all three, or all NULL for none) -> center, size
+ *       (length, width, height), displacement [B,O,3] f32, yaw [B,O] f32, rotation [B,O,3,3] f32 (row-major), count [B,O]
+ *       int32 (the members).  Optional (NULL to skip): extents [B,O,A,4] f32 (umin, umax, vmin, vmax; +inf, -inf, +inf,
+ *       -inf for an empty segment), dirs [A,2] f32 (c_a, s_a).  workspace: pvraft_object_boxes_workspace_bytes(B, N, O, A)
+ *       bytes, 16-byte aligned, no initialisation needed.
+ * Null required pointers (or only some of R_e, t_e, ego_degenerate), B < 1, N < 1, B N >= 2^31, O outside 1..256, up outside
+ * 0..2 and A outside 1..256 return PVRAFT_ERR_BAD_ARG before any launch; B O > 65535 PVRAFT_ERR_UNSUPPORTED. */
+PVRAFT_API int pvraft_object_boxes_fwd(const float* xyz, const int32_t* labels, const float* R_o, const float* t_o, const float* R_e,
+                                       const float* t_e, const uint8_t* ego_degenerate, int B, int N, int O, int up, int A, float* center,
+                                       float* size, float* yaw, float* rotation, float* displacement, int32_t* count, float* extents,
+                                       float* dirs, void* workspace, void* stream);
+PVRAFT_API int64_t pvraft_object_boxes_workspace_bytes(int B, int N, int O, int A);
+
 /* Multi-object tracking from scene flow (no counterpart in the reference): one step of pvraft_b200.track.ObjectTracker.  A
  * sequence gives scans P_0, P_1, ...; for the pair (P_{t-1}, P_t) the caller has the flow F on P_{t-1} and the objects
  * found on P_{t-1} (pvraft_euclidean_clusters_fwd labels and num_objects, O slots).  A step associates them with the O_prev

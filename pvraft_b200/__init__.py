@@ -8,7 +8,8 @@ from .loss import flow_consistency
 from .pointconv import knn_point, square_distance
 from .raft import RSF, RSF_refine
 from .refine import FlotRefine
-from .rigid import RigidMotion, RigidObjects, RigidRefinement, rigid_flow, rigid_motion, rigid_objects, rigid_refine
+from .rigid import (ObjectBoxes, RigidMotion, RigidObjects, RigidRefinement, object_boxes, rigid_flow, rigid_motion, rigid_objects,
+                    rigid_refine)
 from .stream import SceneFlowStream
 from .track import ObjectTracker, ObjectTracks
 from .update import ConvGRU, ConvRNN, FlowHead, MotionEncoder, UpdateBlock
@@ -16,5 +17,4 @@ from .update import ConvGRU, ConvRNN, FlowHead, MotionEncoder, UpdateBlock
 __all__ = ['RSF', 'RSF_refine', 'CorrBlock', 'UpdateBlock', 'MotionEncoder', 'ConvGRU', 'ConvRNN', 'FlowHead',
            'FlotEncoder', 'FlotRefine', 'SetConv', 'Graph', 'knn_point', 'square_distance', 'SceneFlowStream',
            'flow_consistency', 'rigid_motion', 'RigidMotion', 'rigid_objects', 'RigidObjects', 'rigid_flow', 'rigid_refine',
-           'RigidRefinement', 'ObjectTracker',
-           'ObjectTracks']
+           'RigidRefinement', 'object_boxes', 'ObjectBoxes', 'ObjectTracker', 'ObjectTracks']

@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libpvraft_b200.so')
-SOURCES = ['capi.cu', 'clusters.cu', 'flow_metrics.cu', 'corr_gemm.cu', 'corr_lookup.cu', 'fixed_point.cu', 'corr_topk.cu', 'edge_plan.cu', 'flow_consistency.cu', 'flow_propagate.cu', 'grid_index.cu', 'knn.cu', 'knn_branch.cu', 'laplacian.cu', 'pointmlp.cu', 'rigid_motion.cu', 'rigid_refine.cu', 'self_supervised.cu', 'setconv_edge.cu', 'tc_linear.cu', 'tc_wgrad.cu', 'tracks.cu', 'train.cu', 'update_chain.cu']
+SOURCES = ['capi.cu', 'clusters.cu', 'flow_metrics.cu', 'corr_gemm.cu', 'corr_lookup.cu', 'fixed_point.cu', 'corr_topk.cu', 'edge_plan.cu', 'flow_consistency.cu', 'flow_propagate.cu', 'grid_index.cu', 'knn.cu', 'knn_branch.cu', 'laplacian.cu', 'pointmlp.cu', 'rigid_motion.cu', 'object_boxes.cu', 'rigid_refine.cu', 'self_supervised.cu', 'setconv_edge.cu', 'tc_linear.cu', 'tc_wgrad.cu', 'tracks.cu', 'train.cu', 'update_chain.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '--expt-relaxed-constexpr']
 

@@ -52,6 +52,14 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
+// float -> uint key with the same order, for atomicMin / atomicMax and radix selects on floats: negatives get every bit
+// flipped, the rest the sign bit set (-0 orders below +0; a NaN with the sign bit clear above +inf); ord_float inverts it
+__device__ __forceinline__ unsigned ord_key(float f) {
+    const unsigned u = __float_as_uint(f);
+    return u ^ ((unsigned)((int)u >> 31) | 0x80000000u);
+}
+__device__ __forceinline__ float ord_float(unsigned k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+
 // streaming (read-once) 128-bit loads that do not pollute L1
 __device__ __forceinline__ float4 ld_stream_f4(const float4* p) {
     float4 r;

@@ -16,13 +16,6 @@ namespace pvraft {
 
 constexpr int kTopkThreads = 256;
 
-__device__ __forceinline__ unsigned f2key(float f) {
-    const unsigned u = __float_as_uint(f);
-    return u ^ ((unsigned)((int)u >> 31) | 0x80000000u);   // negatives: all bits flipped, others: sign bit set -> larger float, larger key
-}
-__device__ __forceinline__ float key2f(unsigned k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
 __device__ __forceinline__ int padded(int i) { return i + (i >> 5); }
 
 // Both kernels read M columns of row r at corr + r * ld and write its K survivors to val / idx + r * ld_out; the id of column j
@@ -38,7 +31,7 @@ __global__ void __launch_bounds__(kTopkThreads) k_corr_topk(const float* __restr
     const size_t row = blockIdx.x;
     const float* src = corr + row * (size_t)ld;
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-    for (int i = tid; i < M; i += kTopkThreads) s_key[padded(i)] = f2key(__ldg(src + i));
+    for (int i = tid; i < M; i += kTopkThreads) s_key[padded(i)] = ord_key(__ldg(src + i));
     if (tid == 0) { s_prefix = 0u; s_need = (unsigned)K; }
     // ---- radix select: after pass p the top 8*(p+1) bits of the K-th largest key are known --------------
     for (int pass = 0; pass < 4; ++pass) {
@@ -110,7 +103,7 @@ __global__ void __launch_bounds__(kTopkThreads) k_corr_topk(const float* __restr
         bool keep = k > T;
         if (k == T) { keep = eq_seen < need_eq; ++eq_seen; }
         if (keep) {
-            val[row * ld_out + pos] = key2f(k);
+            val[row * ld_out + pos] = ord_float(k);
             idx[row * ld_out + pos] = ids ? __ldg(ids + row * ld + i) : col_base + i;
             ++pos;
         }
@@ -144,7 +137,7 @@ __global__ void __launch_bounds__(kTopkThreads) k_corr_topk_vec(const float* __r
         uint4 kk = make_uint4(0u, 0u, 0u, 0u);   // padding: below every real key, never selected (K <= M)
         if (c4 * 4 < M) {
             const float4 v = __ldg(src + c4);
-            kk = make_uint4(f2key(v.x), f2key(v.y), f2key(v.z), f2key(v.w));
+            kk = make_uint4(ord_key(v.x), ord_key(v.y), ord_key(v.z), ord_key(v.w));
         }
         s_key[c4] = kk;
     }
@@ -343,7 +336,7 @@ __global__ void __launch_bounds__(kTopkThreads) k_corr_topk_vec(const float* __r
     int32_t* irow = idx + row * (size_t)ld_out;
     const int32_t* idrow = ids ? ids + row * (size_t)ld : nullptr;
     for (int i = tid; i < K; i += kTopkThreads) {
-        vrow[i] = key2f(s_oval[i]);
+        vrow[i] = ord_float(s_oval[i]);
         irow[i] = idrow ? __ldg(idrow + s_oidx[i]) : col_base + s_oidx[i];
     }
 }

@@ -19,13 +19,6 @@ constexpr int kGiThreads = 256;
 constexpr int kGiScanThreads = 1024;
 constexpr int kGiBoundCtas = 64;   // CTAs per sample of the bounds reduction
 
-// float -> unsigned key with the same order (for atomicMin / atomicMax)
-__device__ __forceinline__ unsigned ord_key(float f) {
-    const unsigned u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float ord_float(unsigned k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
-
 __device__ __forceinline__ void load_point(const float* __restrict__ xyz, const float* __restrict__ off, long long p, float& x, float& y,
                                            float& z) {
     x = __ldg(xyz + 3 * p);

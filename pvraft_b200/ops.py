@@ -1150,6 +1150,30 @@ def rigid_refine(x1, x2, labels, target_mask, R, t, degenerate, iterations, max_
     return out + (hist, corr, normals, nbr) if want_trace else out
 
 
+OBJECT_BOXES_MAX_ANGLES = 256   # pvraft_object_boxes_fwd tries at most this many box directions per quarter turn
+
+
+def object_boxes(x, labels, R, t, ego, up, angles, want_trace=False):
+    """x [B,N,3] f32, labels [B,N] int32 (segment o of sample b: labels[b] == o), the fits R [B,O,3,3], t [B,O,3] f32, ego
+    None or (R_e [B,3,3], t_e [B,3] f32, degenerate [B] uint8), up in 0..2, angles in 1..256 -> (center [B,O,3], size
+    [B,O,3], yaw [B,O], rotation [B,O,3,3], displacement [B,O,3] f32, count [B,O] int32), plus (extents [B,O,A,4], dirs
+    [A,2] f32) with want_trace.  The box of every segment (include/pvraft_b200.h, pvraft_object_boxes_fwd); the arguments
+    are checked by pvraft_b200.object_boxes."""
+    b, n, o = int(x.shape[0]), int(x.shape[1]), int(R.shape[1])
+    dev = x.device
+    center, size, disp = (torch.empty(b, o, 3, dtype=torch.float32, device=dev) for _ in range(3))
+    yaw = torch.empty(b, o, dtype=torch.float32, device=dev)
+    rot = torch.empty(b, o, 3, 3, dtype=torch.float32, device=dev)
+    count = torch.empty(b, o, dtype=torch.int32, device=dev)
+    extents = torch.empty(b, o, angles, 4, dtype=torch.float32, device=dev) if want_trace else None
+    dirs = torch.empty(angles, 2, dtype=torch.float32, device=dev) if want_trace else None
+    ws = _workspace(abi.object_boxes_workspace_bytes(b, n, o, angles), dev)
+    abi.object_boxes_fwd(x, labels, R, t, *(ego if ego is not None else (None,) * 3), b, n, o, up, angles, center, size, yaw, rot,
+                         disp, count, extents, dirs, ws)
+    out = (center, size, yaw, rot, disp, count)
+    return out + (extents, dirs) if want_trace else out
+
+
 TRACK_MIN_OVERLAP = 1 / 16   # pvraft_track_objects_fwd's least min_overlap: a slot then has at most 16 eligible pairs
 
 

@@ -2,7 +2,8 @@
 that carries them, fitted on the device without a host synchronisation (csrc/rigid_motion.cu; the algorithm is stated in
 include/pvraft_b200.h, pvraft_rigid_objects_fwd); the rigidly moving objects among the other points, by Euclidean clustering
 (csrc/clusters.cu) and one such fit per object; and the flow those fits imply.  Both fits are one operation: O segments per
-sample, given by labels, and the ego-motion is the case O = 1."""
+sample, given by labels, and the ego-motion is the case O = 1.  Each object also gets an oriented box -- extent, heading
+and displacement over the pair (csrc/object_boxes.cu)."""
 import math
 from typing import NamedTuple
 
@@ -261,3 +262,65 @@ def rigid_refine(xyz1, xyz2, fit, target_mask=None, iterations=10, max_distance=
     else:
         out = fit._replace(rotation=R, translation=t, degenerate=degen.bool())
     return RigidRefinement(out, matched, rmse, rank, steps)
+
+
+class ObjectBoxes(NamedTuple):
+    center: torch.Tensor        # [B,O,3] f32: the box centre in xyz1
+    size: torch.Tensor          # [B,O,3] f32: length, width, height
+    yaw: torch.Tensor           # [B,O] f32: the length axis' angle about `up`, from e_p towards e_q, in (-pi, pi]
+    rotation: torch.Tensor      # [B,O,3,3] f32: columns the length axis, the width axis, e_up
+    displacement: torch.Tensor  # [B,O,3] f32: the centre's motion over the pair (relative to the static scene with `ego`)
+    count: torch.Tensor         # [B,O] int32: the points in the box (0 for an empty slot)
+
+
+def object_boxes(xyz1, objects, up=None, ego=None, angles=90):
+    """An oriented box for every object slot of `objects` (a RigidObjects: rigid_objects(xyz1, ...), or the fit of a
+    rigid_refine of it) over every point of xyz1 [B,N,3] labelled with the object: the least-area rectangle among `angles`
+    directions a pi / (2 angles), a = 0 .. angles - 1, in the plane across axis `up` (0, 1 or 2; required, because LiDAR
+    frames are z-up (up=2) while many preprocessed datasets are y-up (up=1)), with the height along `up`.  The length axis
+    is turned to face the way the box centre moves under the object's fit: relative to the sensor, or with `ego` (a
+    RigidMotion, e.g. rigid_motion's ego-motion; ignored where degenerate) relative to the static scene, which is what the
+    displacement then reports.  Box slot o is object slot o, so ObjectTracker.step's track_id[b, o] names box (b, o).  ->
+    ObjectBoxes; an empty slot has count 0, zeros and the identity frame (e_p, e_q, e_up).  The outputs carry no gradient
+    and are bitwise reproducible in every mode; a batched call equals per-sample calls.  Nothing synchronises with the
+    host, so the call can be captured in a CUDA graph.  The rule is stated in include/pvraft_b200.h,
+    pvraft_object_boxes_fwd."""
+    name = 'object_boxes'
+    _check_cloud(name, 'xyz1', xyz1)
+    b, n = int(xyz1.shape[0]), int(xyz1.shape[1])
+    if b < 1 or n < 1:
+        raise ValueError(f'object_boxes: need B >= 1 and N >= 1, got {tuple(xyz1.shape)}')
+    if b * n >= 2 ** 31:
+        raise ValueError(f'object_boxes: B N = {b * n} points (at most 2^31 - 1)')
+    if not _is_int(up) or not 0 <= up <= 2:
+        raise ValueError(f'object_boxes: up={up!r} must be the vertical axis, 0, 1 or 2 (z-up LiDAR frames: 2)')
+    if not _is_int(angles) or not 1 <= angles <= ops.OBJECT_BOXES_MAX_ANGLES:
+        raise ValueError(f'object_boxes: angles={angles!r} must be an integer in 1..{ops.OBJECT_BOXES_MAX_ANGLES}')
+    if not isinstance(objects, RigidObjects):
+        raise ValueError(f'object_boxes: objects must be a RigidObjects, got {type(objects)}')
+    if ego is not None and not isinstance(ego, RigidMotion):
+        raise ValueError(f'object_boxes: ego must be a RigidMotion or None, got {type(ego)}')
+    o = int(objects.rotation.shape[1]) if torch.is_tensor(objects.rotation) and objects.rotation.dim() == 4 else -1
+    shapes = [(objects.labels, (b, n), 'int32', lambda v: v.dtype == torch.int32),
+              (objects.rotation, (b, o, 3, 3), 'floating point', lambda v: v.is_floating_point()),
+              (objects.translation, (b, o, 3), 'floating point', lambda v: v.is_floating_point())]
+    if ego is not None:
+        shapes += [(ego.rotation, (b, 3, 3), 'floating point', lambda v: v.is_floating_point()),
+                   (ego.translation, (b, 3), 'floating point', lambda v: v.is_floating_point()),
+                   (ego.degenerate, (b,), 'bool', lambda v: v.dtype == torch.bool)]
+    for v, want, kind, ok in shapes:
+        if not torch.is_tensor(v) or tuple(v.shape) != want or not ok(v):
+            raise ValueError(f'object_boxes: the fits do not match xyz1 {tuple(xyz1.shape)}: expected {kind} {want}, got '
+                             f'{(tuple(v.shape), v.dtype) if torch.is_tensor(v) else type(v)}')
+    if not 1 <= o <= ops.RIGID_MAX_OBJECTS or b * o > 65535:
+        raise ValueError(f'object_boxes: {o} objects per sample at B = {b} (1..{ops.RIGID_MAX_OBJECTS}, B O at most 65535)')
+    _need_cuda(xyz1, *(v for v, *_ in shapes))
+    with torch.no_grad():
+        e = None
+        if ego is not None:
+            e = (ego.rotation.detach().float().contiguous(), ego.translation.detach().float().contiguous(),
+                 ego.degenerate.contiguous().view(torch.uint8))
+        out = ops.object_boxes(xyz1.detach().float().contiguous(), objects.labels.contiguous(),
+                               objects.rotation.detach().float().contiguous(), objects.translation.detach().float().contiguous(), e,
+                               up, angles)
+    return ObjectBoxes(*out)
