@@ -18,12 +18,23 @@ is left between the two gradients is the arithmetic.
   (construct_graph, corr_init, voxel_cube_index, knn_select, neighbour_max, leaky_relu, prelu, relu): 'record' keeps
   what the oracle decides, 'replay' takes the decisions from `d`.
 
-Records are keyed by what they decide and where, never by call order: ('graph', cloud), ('topk',), ('slots', it),
-('cells', it, level), (GroupNorm name, phase) for an arg-max, ('act', GroupNorm name, phase) and ('relu', layer, it),
-with phase = the cloud for an encoder, the iteration in the loop and 'refine' in the refiner (it = -1 before the loop).
-Masks and args are kept in the oracle's layout.  The library encodes both clouds in one 2B pass and reuses pc1's graph for the context encoder,
-while the oracle calls these separately; `Decisions.get` asserts that every oracle call finds its one record, and
-`Decisions.unused` lists records no call asked for.
+Records are keyed by what they decide and where, never by call order: ('graph', cloud), ('topk', dir), ('slots', it, dir),
+('cells', it, level, dir), (GroupNorm name, *phase) for an arg-max, ('act', GroupNorm name, *phase) and
+('relu', layer, it, dir), with phase = (cloud,) for an encoder, (it, dir) in the loop (it = -1 before it) and
+('refine', dir) in the refiner.  dir is the direction a loop or refiner runs in: '12' for xyz1 -> xyz2, '21' for a
+bidirectional forward's reverse pass.  The library runs an equal-size bidirectional forward as one 2B stack; each of its
+records is split into the first B samples ('12') and the last B ('21').  Clouds of different sizes run one loop per
+direction.  The oracle runs O.rsf_forward(P, x1, x2) and O.rsf_forward(P, x2, x1), each under its direction.
+Masks and args are kept in the oracle's layout.  The library encodes both clouds in one 2B pass and reuses pc1's graph for
+the context encoder, while the oracle calls these separately; `Decisions.get` asserts that every oracle call finds its one
+record, and `Decisions.unused` lists records no call asked for.
+
+The self-supervised loss (pvraft_b200/loss.py) decides too, and record_library keeps those decisions from the `ops` calls
+the loss makes: ('knn', cloud, k), the smoothness and Laplacian graphs of ops.knn(p, p, k, mode=0), recorded once however
+many directions build them; ('nn_ab', dir) / ('nn_ba', dir), Chamfer's nearest points; ('lap', dir), the Laplacian's
+interpolation neighbours; ('cons', dir), the consistency term's.  Each of the last three is the [n*B, ...] tensor of its one
+launch.  `self_supervised64` restates the loss in float64 on those records (tests/losses64.py).  A rigid fit's inlier set
+is recorded by the caller as ('inliers',).
 """
 import contextlib
 import functools
@@ -34,6 +45,7 @@ import os
 import numpy as np
 import torch
 
+import losses64 as L
 from oracle import pvraft_oracle as O
 from ties_restated import fma32
 
@@ -45,6 +57,13 @@ class Decisions:
     def put(self, key, value):
         assert key not in self.rec, f'two records for {key}'
         self.rec[key] = value
+
+    def put_same(self, key, value):
+        """A decision that several calls take (a graph two directions share): recorded once, and equal every time."""
+        if key in self.rec:
+            assert torch.equal(self.rec[key], value), f'two different records for {key}'
+        else:
+            self.rec[key] = value
 
     def get(self, key):
         assert key in self.rec, f'no record for {key}'
@@ -101,14 +120,16 @@ def _edge_layout(mask, axis):
 
 @contextlib.contextmanager
 def record_library(model, xyz1, xyz2):
-    """Records the decisions of the library's training-path forward(s) run inside the scope -> Decisions.  Also keeps
-    the refiner's input flow under ('refine_input',) (not a decision: the replay of a refine step starts from it)."""
+    """Records the decisions of the library's training-path forward(s), and of the self-supervised loss, run inside the
+    scope -> Decisions.  Also keeps each refiner's input flow under ('refine_input', dir) (not a decision: the replay of a
+    refine step starts from it)."""
     from pvraft_b200 import graph as G, ops, train as T
     d = Decisions()
     names = {id(m): n for n, m in model.named_modules()}
     x1, x2 = xyz1.detach().float(), xyz2.detach().float()
     b = x1.shape[0]
-    st = dict(phase=None, it=-1, arg=None, lin=None, ctx=None)
+    # dirs: [(direction, batch slice)] of the loop running now, None outside one
+    st = dict(phase=None, it=-1, arg=None, lin=None, ctx=None, dirs=None)
     pnames = {id(prm): n for n, prm in model.named_parameters()}
 
     def clouds_of(pc):
@@ -120,6 +141,15 @@ def record_library(model, xyz1, xyz2):
                 return [(name, slice(None))]
         raise AssertionError('a cloud that is neither input')
 
+    def directions(pc):
+        """The loop or refiner that starts on pc -> [(direction, slice)]: the 2B stack is both directions."""
+        return [('12' if cloud == 'pc1' else '21', sl) for cloud, sl in clouds_of(pc)]
+
+    def direction_of(target):
+        """The direction of a loss launch, from the cloud it searches (pc2 for '12')."""
+        (cloud, _), = clouds_of(target)
+        return '12' if cloud == 'pc2' else '21'
+
     p = _Patches()
     construct = G.Graph.__dict__['construct_graph'].__func__
 
@@ -130,7 +160,7 @@ def record_library(model, xyz1, xyz2):
         return g
 
     def flot_encoder(m, pc, graph, _orig=T.flot_encoder):
-        st['phase'] = clouds_of(pc)
+        st['phase'] = [((cloud,), sl) for cloud, sl in clouds_of(pc)]
         try:
             out = _orig(m, pc, graph)
         finally:
@@ -140,14 +170,14 @@ def record_library(model, xyz1, xyz2):
         return out
 
     def phases():
-        return st['phase'] if st['phase'] is not None else [(st['it'], slice(None))]
+        return st['phase'] if st['phase'] is not None else [((st['it'], dr), sl) for dr, sl in st['dirs']]
 
     def put_branch(name, x, stats, gn, act, edge_axis=None):
         if act != ops.ACT_LRELU:
             return
         mask = gn_branch(x.detach(), stats, gn.weight.detach(), gn.bias.detach())
         for ph, sl in phases():
-            d.put(('act', name, ph), _edge_layout(mask[sl], edge_axis) if edge_axis else mask[sl].transpose(1, 2))
+            d.put(('act', name, *ph), _edge_layout(mask[sl], edge_axis) if edge_axis else mask[sl].transpose(1, 2))
 
     def gn_act(x, stats, gn, act=ops.ACT_LRELU, *a, _orig=T.gn_act, **k):
         put_branch(names[id(gn)], x, stats, gn, act)
@@ -166,12 +196,18 @@ def record_library(model, xyz1, xyz2):
             layer = 'context_extractor'
         else:
             return y
-        d.put(('relu', layer, st['it']), (y > 0).transpose(1, 2))
+        for dr, sl in st['dirs']:
+            d.put(('relu', layer, st['it'], dr), (y[sl] > 0).transpose(1, 2))
         return y
 
     def flot_refine(m, flow, graph, _orig=T.flot_refine):
-        d.put(('refine_input',), flow.detach().clone())
-        st['phase'] = [('refine', slice(None))]
+        if flow.shape[0] == 2 * b and x1.shape == x2.shape:         # the 2B stack of a bidirectional forward
+            dirs = [('12', slice(0, b)), ('21', slice(b, 2 * b))]
+        else:
+            dirs = [('12' if flow.shape[1] == x1.shape[1] else '21', slice(None))]
+        for dr, sl in dirs:
+            d.put(('refine_input', dr), flow[sl].detach().clone())
+        st['phase'] = [(('refine', dr), sl) for dr, sl in dirs]
         try:
             return _orig(m, flow, graph)
         finally:
@@ -187,12 +223,21 @@ def record_library(model, xyz1, xyz2):
         st['arg'] = None
         y = _orig(x, stats, gn, act, *a, **k)
         for ph, sl in phases():
-            d.put((name, ph), st['arg'][sl].long())
+            d.put((name, *ph), st['arg'][sl].long())
         return y
+
+    def rsf_loop(model_, xyz1_, *a, _orig=T._rsf_loop, **k):
+        st['dirs'], st['it'] = directions(xyz1_), -1                  # the iteration count restarts per direction
+        try:
+            return _orig(model_, xyz1_, *a, **k)
+        finally:
+            st['dirs'] = None
 
     def corr_reorder(val, idx, _orig=ops.corr_reorder):
         val, idx = _orig(val, idx)
-        d.put(('topk',), idx.long())
+        if st['dirs'] is not None:                                      # (not the inference path's correlation)
+            for dr, sl in st['dirs']:
+                d.put(('topk', dr), idx[sl].long())
         return val, idx
 
     def corr_lookup(*a, _orig=ops.corr_lookup, **k):
@@ -201,9 +246,35 @@ def record_library(model, xyz1, xyz2):
         st['it'] += 1
         k['want_cube'] = True
         out = _orig(*a, **k)
-        d.put(('slots', st['it']), out['knn_slot'].long())
-        for lvl in range(out['cube'].shape[-1]):
-            d.put(('cells', st['it'], lvl), out['cube'][..., lvl].long())
+        for dr, sl in st['dirs']:
+            d.put(('slots', st['it'], dr), out['knn_slot'][sl].long())
+            for lvl in range(out['cube'].shape[-1]):
+                d.put(('cells', st['it'], lvl, dr), out['cube'][sl][..., lvl].long())
+        return out
+
+    # the self-supervised loss's own searches
+    def knn(xyz, query, k, *a, _orig=ops.knn, **kw):
+        out = _orig(xyz, query, k, *a, **kw)
+        if not a and kw.get('mode', 0) == 0 and not kw.get('want_rel', False) and torch.equal(xyz, query):
+            (cloud, _), = clouds_of(xyz)
+            d.put_same(('knn', cloud, k), out.long())
+        return out
+
+    def chamfer(w, target, *a, _orig=ops.chamfer, **kw):
+        out = _orig(w, target, *a, **kw)
+        dr = direction_of(target)
+        d.put(('nn_ab', dr), out[1].long())
+        d.put(('nn_ba', dr), out[2].long())
+        return out
+
+    def laplacian(w, target, *a, _orig=ops.laplacian, **kw):
+        out = _orig(w, target, *a, **kw)
+        d.put(('lap', direction_of(target)), out[1].long())
+        return out
+
+    def flow_consistency(w, f12, target, *a, _orig=ops.flow_consistency, **kw):
+        out = _orig(w, f12, target, *a, **kw)
+        d.put(('cons', direction_of(target)), out[1].long())
         return out
 
     p.set(G.Graph, 'construct_graph', construct_graph, static=True)
@@ -216,6 +287,11 @@ def record_library(model, xyz1, xyz2):
     p.set(ops, 'gn_act_maxk', gn_act_maxk)
     p.set(ops, 'corr_reorder', corr_reorder)
     p.set(ops, 'corr_lookup', corr_lookup)
+    p.set(T, '_rsf_loop', rsf_loop)
+    p.set(ops, 'knn', knn)
+    p.set(ops, 'chamfer', chamfer)
+    p.set(ops, 'laplacian', laplacian)
+    p.set(ops, 'flow_consistency', flow_consistency)
     try:
         yield d
     finally:
@@ -246,14 +322,16 @@ PRELU_SLOPE = {'corr_block.out_conv.1': 'corr_block.out_conv.2.weight', 'corr_bl
 
 
 @contextlib.contextmanager
-def oracle_decisions(d, xyz1, xyz2, base_scale, mode, slope_terms=None):
+def oracle_decisions(d, xyz1, xyz2, base_scale, mode, slope_terms=None, direction='12'):
     """Inside the scope the oracle's deciding functions record into (mode 'record') or replay from (mode 'replay') the
-    Decisions d.  xyz1 / xyz2 are the very tensors the oracle is given (an encoder's cloud is recognised by identity).
-    slope_terms: a dict that every later backward through a PReLU adds sum |dy * t| over its t < 0 to, under the slope's
-    parameter name."""
-    assert mode in ('record', 'replay')
+    Decisions d.  xyz1 / xyz2 are the very tensors the oracle is given (an encoder's cloud is recognised by identity);
+    direction: '12' for a forward on (xyz1, xyz2), '21' for one on (xyz2, xyz1).  slope_terms: a dict that every later
+    backward through a PReLU adds sum |dy * t| over its t < 0 to, under the slope's parameter name.  In 'record' mode a
+    decision that is taken again (an encoder that both directions run) must equal its record."""
+    assert mode in ('record', 'replay') and direction in ('12', '21')
     rec = mode == 'record'
     st = dict(phase=None, it=-1)
+    put = d.put_same
     orig = {n: getattr(O, n) for n in ('construct_graph', 'flot_encoder', 'flot_refine', 'corr_init', 'corr_lookup',
                                        'voxel_cube_index', 'knn_select', 'neighbour_max', 'leaky_relu', 'prelu', 'relu')}
 
@@ -268,23 +346,20 @@ def oracle_decisions(d, xyz1, xyz2, base_scale, mode, slope_terms=None):
         if rec:
             g = orig['construct_graph'](pc, k)
             b, n, _ = pc.shape
-            nbr = g.edges.reshape(b, n, k) - (torch.arange(b, device=pc.device) * n).view(b, 1, 1)
-            if key in d.rec:                  # pc1's graph again, for the context encoder: the same decision
-                assert torch.equal(d.rec[key], nbr), key
-            else:
-                d.put(key, nbr)
-            return g
+            put(key, g.edges.reshape(b, n, k) - (torch.arange(b, device=pc.device) * n).view(b, 1, 1))   # (again for the context encoder)
+            # the replay's arithmetic on the decision: a float64 record and its replay give the same bits
+            return graph_from(pc, d.rec[key])
         return graph_from(pc, d.get(key))
 
     def flot_encoder(P, prefix, pc, graph=None):
-        st['phase'] = cloud_of(pc)
+        st['phase'] = (cloud_of(pc),)
         try:
             return orig['flot_encoder'](P, prefix, pc, graph)
         finally:
             st['phase'] = None
 
     def flot_refine(P, prefix, flow, graph):
-        st['phase'] = 'refine'
+        st['phase'] = ('refine', direction)
         try:
             return orig['flot_refine'](P, prefix, flow, graph)
         finally:
@@ -293,19 +368,19 @@ def oracle_decisions(d, xyz1, xyz2, base_scale, mode, slope_terms=None):
     def corr_init(fmap1, fmap2, xyz2_, truncate_k):
         if rec:
             s = orig['corr_init'](fmap1, fmap2, xyz2_, truncate_k)
-            d.put(('topk',), s.indices)
-            return s
-        return _corr_state(fmap1, fmap2, xyz2_, d.get(('topk',)))
+            put(('topk', direction), s.indices)
+            return _corr_state(fmap1, fmap2, xyz2_, s.indices)
+        return _corr_state(fmap1, fmap2, xyz2_, d.get(('topk', direction)))
 
     def corr_lookup(*a, **k):
         st['it'] += 1
         return orig['corr_lookup'](*a, **k)
 
     def voxel_cube_index(state, coords, r):
-        key = ('cells', st['it'], int(round(math.log2(r / base_scale))))
+        key = ('cells', st['it'], int(round(math.log2(r / base_scale))), direction)
         if rec:
             cube, valid = orig['voxel_cube_index'](state, coords, r)
-            d.put(key, torch.where(valid, cube, -1))
+            put(key, torch.where(valid, cube, -1))
             return cube, valid
         cell = d.get(key)
         return cell.clamp_min(0), cell >= 0
@@ -313,34 +388,34 @@ def oracle_decisions(d, xyz1, xyz2, base_scale, mode, slope_terms=None):
     def knn_select(state, coords, knn=O.KNN):
         if rec:
             s = orig['knn_select'](state, coords, knn)
-            d.put(('slots', st['it']), s)
+            put(('slots', st['it'], direction), s)
             return s
-        return d.get(('slots', st['it']))
+        return d.get(('slots', st['it'], direction))
 
     def neighbour_max(x, dim, layer):
         # x [B,C,32,N] (dim 2) or [B,C,N,32] (dim 3); the arg is kept as the library keeps it, [B,N,C]
-        key = (layer, st['phase'] if st['phase'] is not None else st['it'])
+        key = (layer, *phase())
         if rec:
             v, i = x.max(dim=dim)
-            d.put(key, i.transpose(1, 2))
+            put(key, i.transpose(1, 2))
             return v
         idx = d.get(key).transpose(1, 2).unsqueeze(dim)
         return x.gather(dim, idx).squeeze(dim)
 
     def phase():
-        return st['phase'] if st['phase'] is not None else st['it']
+        return st['phase'] if st['phase'] is not None else (st['it'], direction)
 
     def branch(key, x):
         if rec:
-            d.put(key, x >= 0)
+            put(key, x >= 0)
             return x >= 0
         return d.get(key)
 
     def leaky_relu(x, slope=0.1, layer=None):
-        return torch.where(branch(('act', layer, phase()), x), x, slope * x)
+        return torch.where(branch(('act', layer, *phase()), x), x, slope * x)
 
     def prelu(x, a, layer=None):
-        mask = branch(('act', layer, phase()), x)
+        mask = branch(('act', layer, *phase()), x)
         y = torch.where(mask, x, a.view(-1)[0] * x)
         if slope_terms is not None and y.requires_grad:
             def terms(g, x=x.detach(), neg=~mask, name=PRELU_SLOPE[layer]):
@@ -349,9 +424,9 @@ def oracle_decisions(d, xyz1, xyz2, base_scale, mode, slope_terms=None):
         return y
 
     def relu(x, layer=None):
-        key = ('relu', layer, st['it'])
+        key = ('relu', layer, st['it'], direction)
         if rec:
-            d.put(key, x > 0)
+            put(key, x > 0)
             return torch.relu(x)
         return torch.where(d.get(key), x, torch.zeros_like(x))
 
@@ -386,43 +461,98 @@ def sequence_loss(flows, gt, signs=None, gamma=0.8):
     return sum(gamma ** (n - i - 1) * (signs[i].to(gt.dtype) * (flows[i] - gt)).sum(-1).mean() for i in range(n))
 
 
-def replay_rsf(W, pc1, pc2, d, iters, levels, base_scale, truncate_k, losses, device):
+def self_supervised64(d, flows, x1, x2, gamma=0.8, k=9, wc=1.0, ws=1.0, wl=0.0, k_lap=10, k_int=5, wcons=0.0):
+    """sequence_self_supervised_loss in float64 with every neighbour set taken from d's loss records.  flows: a list of
+    [B,N1,3] (one direction), or the pair (list [B,N1,3], list [B,N2,3]) of a bidirectional forward.  A refiner's loss,
+    self_supervised_loss of one flow or of a pair, is the same with one-element lists."""
+    pair = isinstance(flows, tuple)
+    n = len(flows[0]) if pair else len(flows)
+    recs = []
+    for dr, a, b in (('12', 'pc1', 'pc2'), ('21', 'pc2', 'pc1'))[:2 if pair else 1]:
+        def split(key):                                # the [n*B, ...] tensor of one launch -> n tensors [B, ...]
+            t = d.get((key, dr))
+            return list(t.unflatten(0, (n, t.shape[0] // n)))
+        graphs = (d.get(('knn', a, k)),) + ((d.get(('knn', a, k_lap)), d.get(('knn', b, k_lap))) if wl != 0 else (None, None))
+        recs.append(dict(nbrs=graphs, chamfer=list(zip(split('nn_ab'), split('nn_ba'))),
+                         lap=split('lap') if wl != 0 else None, cons=split('cons') if pair and wcons != 0 else None))
+    if not pair:
+        r = recs[0]
+        nbr, g1, g2 = r['nbrs']
+        return L.loss64(flows, x1, x2, nbr, g1, g2, gamma=gamma, wc=wc, ws=ws, wl=wl, k_int=k_int, lap_idx=r['lap'],
+                        chamfer_idx=r['chamfer'])
+    return L.pair_loss64(flows[0], flows[1], x1, x2, gamma=gamma, wc=wc, ws=ws, wl=wl, wcons=wcons, k_int=k_int,
+                         nbrs=[r['nbrs'] for r in recs], chamfer_idx=[r['chamfer'] for r in recs],
+                         lap_idx=[r['lap'] for r in recs], cons_idx=[r['cons'] for r in recs] if wcons != 0 else None)
+
+
+def rsf_flows(P, x1, x2, iters, levels, base_scale, truncate_k, flow_init=None):
+    """O.rsf_forward, with the loop started at xyz1 + flow_init when it is given (a constant: no gradient reaches it;
+    RSF.forward's warm start)."""
+    li = O.prepare(P, x1, x2, truncate_k)
+    if flow_init is None:
+        return O.raft_loop(P, li, x1, iters, levels, base_scale)
+    coords2, net, flows = x1 + flow_init.detach(), li.net, []
+    for _ in range(iters):
+        coords2 = coords2.detach()
+        corr = O.corr_lookup(P, li.state, coords2, levels, base_scale)
+        net, delta = O.update_block(P, net, li.inp, corr, coords2 - x1, li.graph)
+        coords2 = coords2 + delta
+        flows.append(coords2 - x1)
+    return flows
+
+
+def detached(out):
+    return tuple(detached(o) for o in out) if isinstance(out, tuple) else [f.detach() for f in out] if isinstance(out, list) else out.detach()
+
+
+def replay_rsf(W, pc1, pc2, d, iters, levels, base_scale, truncate_k, losses, device, flow_init=None, bidirectional=False):
     """The oracle's RSF forward in float64 on `device` with d's decisions; -> (flows, [grads of each loss], [the PReLU
     slopes' sum |dy * t| of each loss]) where a grads dict holds every parameter and 'xyz1' / 'xyz2'.  losses: functions
-    of the flows."""
+    (flows, xyz1, xyz2) -> scalar, the clouds being the replay's float64 leaves.  flow_init: the warm start.
+    bidirectional: flows is the pair (O.rsf_forward(P, x1, x2) under '12', O.rsf_forward(P, x2, x1) under '21')."""
     P = {k: v.detach().to(device, torch.float64).requires_grad_(True) for k, v in W.items()}
     x1 = pc1.detach().to(device, torch.float64).requires_grad_(True)
     x2 = pc2.detach().to(device, torch.float64).requires_grad_(True)
+    init = None if flow_init is None else flow_init.detach().to(device, torch.float64)
     terms = {}
     with oracle_decisions(d, x1, x2, base_scale, 'replay', terms):
-        flows = O.rsf_forward(P, x1, x2, iters, levels, base_scale, truncate_k)
+        flows = rsf_flows(P, x1, x2, iters, levels, base_scale, truncate_k, init)
+    if bidirectional:
+        with oracle_decisions(d, x1, x2, base_scale, 'replay', terms, direction='21'):
+            flows = (flows, rsf_flows(P, x2, x1, iters, levels, base_scale, truncate_k))
     grads, scales = [], []
     for i, fn in enumerate(losses):
         terms.clear()
         grads += _grads([fn], flows, P, x1, x2, retain=i + 1 < len(losses))
         scales.append(dict(terms))
-    return [f.detach() for f in flows], grads, scales
+    return detached(flows), grads, scales
 
 
-def replay_refine(W, pc1, flow, nbr, d, losses, device):
+def replay_refine(W, pc1, pc2, d, losses, device, bidirectional=False):
     """The refine step (RSF_refine's refiner on the loop's last flow, RAFTSceneFlowRefine.py:46) in float64 with d's
-    arg-max decisions.  flow: the refiner's input (the other run's loop output, no gradient); nbr: pc1's adjacency.
-    -> (refined, [grads of each loss]): the refine_block parameters and 'xyz1' (= - d flow)."""
+    arg-max decisions, starting from the recorded ('refine_input', dir) (the other run's loop output, no gradient) on the
+    recorded graph of the cloud it starts on.  bidirectional: both directions, the refined flows as a pair.  losses:
+    functions (refined, xyz1, xyz2) -> scalar.  -> (refined, [grads of each loss]): the refine_block parameters and 'xyz1'
+    (= - d flow), and 'xyz2' for a pair."""
     P = {k: v.detach().to(device, torch.float64).requires_grad_(k.startswith('refine_block.')) for k, v in W.items()}
     x1 = pc1.detach().to(device, torch.float64).requires_grad_(True)
-    f = flow.detach().to(device, torch.float64) + (x1.detach() - x1)
-    graph = graph_from(x1.detach(), nbr.to(device))
-    with oracle_decisions(d, x1, None, 1.0, 'replay'):
-        refined = O.flot_refine(P, 'refine_block', f, graph)
+    x2 = pc2.detach().to(device, torch.float64).requires_grad_(bidirectional)
+    out = []
+    for dr, x, cloud in (('12', x1, 'pc1'), ('21', x2, 'pc2'))[:2 if bidirectional else 1]:
+        f = d.get(('refine_input', dr)).to(device, torch.float64) + (x.detach() - x)
+        graph = graph_from(x.detach(), d.get(('graph', cloud)).to(device))
+        with oracle_decisions(d, x1, x2, 1.0, 'replay', direction=dr):
+            out.append(O.flot_refine(P, 'refine_block', f, graph))
+    refined = tuple(out) if bidirectional else out[0]
     P = {k: v for k, v in P.items() if v.requires_grad}
-    return refined.detach(), _grads(losses, refined, P, x1, None)
+    return detached(refined), _grads(losses, refined, P, x1, x2 if bidirectional else None)
 
 
 def _grads(losses, out, P, x1, x2, retain=False):
     leaves = dict(P, xyz1=x1, **({} if x2 is None else {'xyz2': x2}))
     res = []
     for i, fn in enumerate(losses):
-        g = torch.autograd.grad(fn(out), list(leaves.values()), retain_graph=retain or i + 1 < len(losses), allow_unused=True)
+        g = torch.autograd.grad(fn(out, x1, x2), list(leaves.values()), retain_graph=retain or i + 1 < len(losses), allow_unused=True)
         res.append({k: (torch.zeros_like(v) if gv is None else gv) for (k, v), gv in zip(leaves.items(), g)})
     return res
 

@@ -8,8 +8,8 @@ import torch
 
 from conftest import default_weights, rel_err
 import unequal_oracle as U
-from test_gpu_flow_consistency import consistency64
-from test_gpu_laplacian import graphs, leaf, loss64, nn64_knearest, same_bits
+from losses64 import graphs, pair_loss64
+from test_gpu_laplacian import leaf, same_bits
 from train_helpers import compare_grads, oracle_adjacency
 
 pytestmark = pytest.mark.gpu
@@ -189,29 +189,6 @@ def test_adam_lowers_the_four_term_loss(dev):
 
 
 # ---- against the oracle and float64 ----------------------------------------------------------------------------------------
-def pair_loss64(f12s, f21s, p1, p2, dev, gamma=0.8, wc=1.0, ws=1.0, wl=0.3, wcons=0.3, k_int=5, k_cons=3, lap_idx=None,
-                cons_idx=None):
-    """sequence_self_supervised_loss of the pair (f12s [B,N1,3] list, f21s [B,N2,3] list) in float64: the three-term loss of
-    each direction (the reverse one with P1 and P2 swapped) plus wcons times its consistency term, the two averaged.  The
-    neighbour searches run in float64 unless lap_idx / cons_idx ((forward list, backward list) of [B,N,k] per prediction)
-    give them."""
-    from pvraft_b200 import ops
-    n, total = len(f12s), 0
-    dirs = ((f12s, f21s, p1, p2), (f21s, f12s, p2, p1))
-    for d, (fs, fo, pa, pb) in enumerate(dirs):
-        pad, pbd = pa.detach().float().to(dev).contiguous(), pb.detach().float().to(dev).contiguous()
-        nbr = ops.knn(pad, pad, 9, mode=0).long().cpu()
-        g1, g2 = (t.long().cpu() for t in graphs(pad, pbd, 10))
-        total = total + loss64(fs, pa, pb, nbr, g1, g2, gamma=gamma, wc=wc, ws=ws, wl=wl, k_int=k_int,
-                               lap_idx=None if lap_idx is None else lap_idx[d]) / 2
-        for i in range(n):
-            f, r = fs[i].double(), fo[i].double()
-            w = pa.double() + f
-            idx = nn64_knearest(w.detach(), pb.double().detach(), k_cons) if cons_idx is None else cons_idx[d][i]
-            total = total + gamma ** (n - i - 1) * wcons * consistency64(w, f, pb.double(), r, idx)[0].mean() / 2
-    return total
-
-
 @pytest.mark.parametrize('n1,n2', [(1024, 1024), (1024, 1280)])
 def test_rsf_gradients_match_oracle(dev, n1, n2):
     """A 3-iteration stage-1 step with a bidirectional forward and the four-term pair loss (w_laplacian = w_consistency =

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 import torch
 
+from losses64 import consistency64
 from test_gpu_laplacian import knearest_host, same_bits
 
 pytestmark = pytest.mark.gpu
@@ -27,21 +28,6 @@ def det():
         yield
     finally:
         torch.use_deterministic_algorithms(was, warn_only=warn)
-
-
-def consistency64(w, f12, p2, f21, nn_idx):
-    """[S] F_s, r [S,N,3] and bhat [S,N,3] in float64 with the neighbours nn_idx [S,N,k] held fixed."""
-    out, res, bh = [], [], []
-    for s in range(w.shape[0]):
-        b, idx = s % p2.shape[0], nn_idx[s].long()
-        d = ((w[s][:, None, :] - p2[b][idx]) ** 2).sum(-1)
-        wt = 1.0 / (d + 1e-8)
-        bhat = (wt[..., None] * f21[s][idx]).sum(1) / wt.sum(1, keepdim=True)
-        r = f12[s] + bhat
-        out.append((r ** 2).sum(-1).mean())
-        res.append(r)
-        bh.append(bhat)
-    return torch.stack(out), torch.stack(res), torch.stack(bh)
 
 
 def case(s, b, n, m, seed, shift=0.0, scale=4.0, dup=False):

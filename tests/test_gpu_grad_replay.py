@@ -132,7 +132,7 @@ def test_stage1_gradients_match_float64_replay(dev, case, det):
     del m
     torch.cuda.empty_cache()
     ref_flows, want, scales = R.replay_rsf(W, pc1, pc2, d, c['iters'], 3, 0.25, c['k'],
-                                           [lambda f: R.linear_loss(f, G), lambda f: R.sequence_loss(f, gt, signs)], dev)
+                                           [lambda f, *_: R.linear_loss(f, G), lambda f, *_: R.sequence_loss(f, gt, signs)], dev)
     assert not d.unused(), d.unused()
     e_f = max(float((f.double() - r).norm() / r.norm()) for f, r in zip(flows, ref_flows))
     worst = worst_slope = 0.0
@@ -165,8 +165,7 @@ def test_refine_gradients_match_float64_replay(dev, det):
                                     lambda m, x1, x2: m([x1, x2], iters))
     assert len(got[0]) == 29 + 1
     signs = torch.sign(refined - gt)
-    ref, want = R.replay_refine(W, pc1, d.rec[('refine_input',)], d.rec[('graph', 'pc1')], d,
-                                [lambda r: (r * G).sum(), lambda r: (signs * (r - gt)).sum(-1).mean()], dev)
+    ref, want = R.replay_refine(W, pc1, pc2, d, [lambda r, *_: (r * G).sum(), lambda r, *_: (signs * (r - gt)).sum(-1).mean()], dev)
     e_f = float((refined.double() - ref).norm() / ref.norm())
     worst = 0.0
     for loss, gg, ww in zip(('linear', 'l1'), got, want):
@@ -190,7 +189,7 @@ def test_stage1_gradients_match_the_reference(dev):
                                  lambda m, x1, x2: m([x1, x2], num_iters=3))
     for cloud, key in (('pc1', 'nbr1'), ('pc2', 'nbr2')):
         assert torch.equal(d.rec[('graph', cloud)].sort(-1).values.cpu(), z[key].long().sort(-1).values)
-    assert torch.equal(d.rec[('topk',)].sort(-1).values.cpu(), z['topk'].long().sort(-1).values)
+    assert torch.equal(d.rec[('topk', '12')].sort(-1).values.cpu(), z['topk'].long().sort(-1).values)
     errs = R.sketched_rel_l2(got, want)          # (estimates within 1 +- 0.2 for tensors of more than 128 elements)
     slope = 'corr_block.knn_conv.2.weight'
     worst = report('library vs reference float64', {k: v for k, v in errs.items() if k != slope})

@@ -15,8 +15,8 @@ import pytest
 import torch
 
 from conftest import default_weights, rel_err
+from losses64 import graphs, lap64, laplacian64, loss64, term64
 from oracle import pvraft_oracle as O
-from test_gpu_self_supervised import chamfer64, nn64_indices, smooth64
 from train_helpers import compare_grads, oracle_adjacency
 
 pytestmark = pytest.mark.gpu
@@ -66,59 +66,6 @@ def knearest_host(q, c, k):
         part.sort(axis=1)
         out[r0:r0 + rows] = part[:, :k] & 0xffffffff
     return out
-
-
-def lap64(x, nbr):
-    """L(x) [N,3] over the graph nbr [N,k]."""
-    return (x[nbr] - x[:, None, :]).sum(1) / (nbr.shape[1] - 1)
-
-
-def term64(w, p2, l2, g1, nn_idx):
-    """[S] R_s in float64 with the interpolation neighbours nn_idx [S,N,k_int] held fixed; l2 [B,M,3] given."""
-    out = []
-    for s in range(w.shape[0]):
-        b = s % p2.shape[0]
-        idx = nn_idx[s]
-        d = ((w[s][:, None, :] - p2[b][idx]) ** 2).sum(-1)
-        wt = 1.0 / (d + 1e-8)
-        lhat = (wt[..., None] * l2[b][idx]).sum(1) / wt.sum(1, keepdim=True)
-        out.append(((lhat - lap64(w[s], g1[b])) ** 2).sum(-1).mean())
-    return torch.stack(out)
-
-
-def laplacian64(w, p2, g1, g2, nn_idx):
-    l2 = torch.stack([lap64(p2[b], g2[b]) for b in range(p2.shape[0])])
-    return term64(w, p2, l2, g1, nn_idx)
-
-
-def nn64_knearest(w, p2, k):
-    """Float64 k nearest of every W_i in P2[s % B] -> [S,N,k]."""
-    out = []
-    for s in range(w.shape[0]):
-        d = ((w[s][:, None, :] - p2[s % p2.shape[0]][None, :, :]) ** 2).sum(-1)
-        out.append(d.topk(k, 1, largest=False).indices)
-    return torch.stack(out)
-
-
-def graphs(p1, p2, k_lap):
-    from pvraft_b200 import ops
-    p1, p2 = p1.detach().contiguous(), p2.detach().contiguous()
-    return ops.knn(p1, p1, k_lap, mode=0), ops.knn(p2, p2, k_lap, mode=0)
-
-
-def loss64(flows, p1, p2, nbr, g1, g2, gamma=0.8, wc=1.0, ws=1.0, wl=0.3, k_int=5, lap_idx=None):
-    """The three-term sequence loss in float64 for a list of [B,N,3] flows; every search in float64 unless lap_idx (one
-    [S,N,k_int] per flow) gives the interpolation neighbours."""
-    n, total = len(flows), 0
-    for i, f in enumerate(flows):
-        f = f.double()
-        w = p1.double() + f
-        nn_ab, nn_ba = nn64_indices(w.detach(), p2.double())
-        idx = nn64_knearest(w.detach(), p2.double(), k_int) if lap_idx is None else lap_idx[i]
-        per = (wc * chamfer64(w, p2.double(), nn_ab, nn_ba) + ws * smooth64(f, nbr)
-               + wl * laplacian64(w, p2.double(), g1, g2, idx))
-        total = total + gamma ** (n - i - 1) * per.mean()
-    return total
 
 
 # ---- search ----------------------------------------------------------------------------------------------------------------

@@ -14,6 +14,7 @@ import pytest
 import torch
 
 from conftest import default_weights, rel_err
+from losses64 import chamfer64, loss64, smooth64
 from oracle import pvraft_oracle as O
 from train_helpers import compare_grads, oracle_adjacency
 
@@ -62,52 +63,6 @@ def nn_host(q, c, dtype):
 def dist64(q, c, idx):
     d = q.astype(np.float64) - c.astype(np.float64)[idx]
     return (d * d).sum(-1)
-
-
-def chamfer64(w, p2, nn_ab=None, nn_ba=None):
-    """[S] in float64.  With indices: the loss with the pairs held fixed (the function the kernels differentiate)."""
-    out = []
-    for s in range(w.shape[0]):
-        b = p2[s % p2.shape[0]]
-        if nn_ab is None:
-            d = ((w[s][:, None, :] - b[None, :, :]) ** 2).sum(-1)
-            out.append(d.min(1).values.mean() + d.min(0).values.mean())
-        else:
-            out.append(((w[s] - b[nn_ab[s]]) ** 2).sum(-1).mean() + ((w[s][nn_ba[s]] - b) ** 2).sum(-1).mean())
-    return torch.stack(out)
-
-
-def smooth64(f, nbr):
-    """[S] in float64; the gradient of the length at 0 is 0."""
-    out = []
-    for s in range(f.shape[0]):
-        d = f[s][nbr[s % nbr.shape[0]]] - f[s][:, None, :]
-        n2 = (d * d).sum(-1)
-        pos = n2 > 0
-        out.append((torch.where(pos, n2, torch.ones_like(n2)).sqrt() * pos).mean())
-    return torch.stack(out)
-
-
-def nn64_indices(w, p2):
-    """Float64 argmin of both directions for every sample: the pairs of the float64 loss."""
-    ab, ba = [], []
-    for s in range(w.shape[0]):
-        d = ((w[s][:, None, :] - p2[s % p2.shape[0]][None, :, :]) ** 2).sum(-1)
-        ab.append(d.argmin(1))
-        ba.append(d.argmin(0))
-    return torch.stack(ab), torch.stack(ba)
-
-
-def loss64(flows, p1, p2, nbr, gamma=0.8, wc=1.0, ws=1.0):
-    """sequence_self_supervised_loss in float64 for a list of [B,N,3] flows, the pairs from the float64 search."""
-    n, total = len(flows), 0
-    for i, f in enumerate(flows):
-        f = f.double()
-        w = p1.double() + f
-        nn_ab, nn_ba = nn64_indices(w.detach(), p2.double())
-        per = wc * chamfer64(w, p2.double(), nn_ab, nn_ba) + ws * smooth64(f, nbr)
-        total = total + gamma ** (n - i - 1) * per.mean()
-    return total
 
 
 # ---- search ----------------------------------------------------------------------------------------------------------------

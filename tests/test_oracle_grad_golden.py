@@ -66,7 +66,7 @@ def test_reference_decisions_equal_the_fp32_oracle(fixture1):
     oracle_rsf_step(W, pc1, pc2, torch.float32, 'record', d)
     for cloud, key in (('pc1', 'nbr1'), ('pc2', 'nbr2')):
         assert torch.equal(d.rec[('graph', cloud)].sort(-1).values, g[key].long().sort(-1).values), cloud
-    assert torch.equal(d.rec[('topk',)].sort(-1).values, g['topk'].long().sort(-1).values)
+    assert torch.equal(d.rec[('topk', '12')].sort(-1).values, g['topk'].long().sort(-1).values)
 
 
 def test_fp32_oracle_gradients_match_the_reference(fixture1):
